@@ -66,6 +66,11 @@ def test_struct_layouts_match_header_sizes():
         out = subprocess.run([os.path.join(d, "t")], check=True, capture_output=True, text=True).stdout.split()
     assert [int(x) for x in out] == [C.sizeof(_abi.FleetC), C.sizeof(_abi.AllocsC), C.sizeof(_abi.GridC),
                                      C.sizeof(_abi.SummaryC)]
+    # the column tables name the mirrors' array fields in order, with their element types
+    import numpy as np
+    for struct, table in ((_abi.FleetC, _abi.FLEET_COLUMNS), (_abi.AllocsC, _abi.ALLOC_COLUMNS)):
+        arrays = [(n, t._type_) for n, t in struct._fields_ if issubclass(t, C._Pointer)]
+        assert arrays == [(col[0], _abi._CT[np.dtype(col[1])]) for col in table]
 
 
 def test_create_without_gpu_fails_loudly(lib):

@@ -129,6 +129,38 @@ def ptr(a: np.ndarray):
     return a.ctypes.data_as(C.POINTER(_CT[a.dtype]))
 
 
+# The array columns of wva_fleet: (name, dtype, length).  The length is "A" (accelerators), "T" (accelerator
+# types), "MA" (models x accelerators, a row-major [M, A] table) or "S" (servers).
+FLEET_COLUMNS = (
+    ("acc_cost", np.float32, "A"),
+    ("acc_multiplicity", np.int32, "A"),
+    ("acc_type", np.int32, "A"),
+    ("type_capacity", np.int32, "T"),
+    ("perf_present", np.uint8, "MA"),
+    ("perf_alpha", np.float32, "MA"),
+    ("perf_beta", np.float32, "MA"),
+    ("perf_gamma", np.float32, "MA"),
+    ("perf_delta", np.float32, "MA"),
+    ("perf_acc_count", np.int32, "MA"),
+    ("perf_max_batch", np.int32, "MA"),
+    ("perf_at_tokens", np.int32, "MA"),
+    ("srv_model", np.int32, "S"),
+    ("srv_priority", np.int32, "S"),
+    ("srv_has_target", np.uint8, "S"),
+    ("srv_slo_itl", np.float32, "S"),
+    ("srv_slo_ttft", np.float32, "S"),
+    ("srv_slo_tps", np.float32, "S"),
+    ("srv_keep_acc", np.uint8, "S"),
+    ("srv_min_replicas", np.int32, "S"),
+    ("srv_max_batch", np.int32, "S"),
+    ("srv_arrival_rpm", np.float32, "S"),
+    ("srv_in_tokens", np.int32, "S"),
+    ("srv_out_tokens", np.int32, "S"),
+    ("srv_cur_acc", np.int32, "S"),
+    ("srv_cur_replicas", np.int32, "S"),
+    ("srv_cur_cost", np.float32, "S"),
+)
+
 ALLOC_COLUMNS = (
     ("feasible", np.uint8),
     ("acc", np.int32),

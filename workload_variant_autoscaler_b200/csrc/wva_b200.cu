@@ -66,22 +66,52 @@ struct PinBuf {
 
 inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
+// Columns packed into one buffer, each starting on an `align`-byte boundary (an empty column still gets an
+// address of its own).  The offsets take() returns hand out the device pointers, and take() records where a
+// column with a host destination lies, so the layout and the copy-back cannot disagree.
+struct Cols {
+    struct Col {
+        size_t off, bytes;
+        void* dst;
+    };
+    size_t align, bytes = 0;
+    std::vector<Col> out;  // the columns that have a host destination
+    explicit Cols(size_t a) : align(a) {}
+    size_t take(size_t n, void* dst = nullptr) {
+        const size_t at = bytes;
+        if (dst) out.push_back({at, n, dst});
+        bytes = align_up(at + std::max<size_t>(n, 1), align);
+        return at;
+    }
+    // device buffer `dev` -> the destinations, enqueued on `st`
+    cudaError_t copy_back(const void* dev, cudaStream_t st) const {
+        for (const Col& c : out)
+            if (c.bytes) {
+                const cudaError_t e = cudaMemcpyAsync(c.dst, (const char*)dev + c.off, c.bytes, cudaMemcpyDeviceToHost, st);
+                if (e != cudaSuccess) return e;
+            }
+        return cudaSuccess;
+    }
+    // host image of the buffer -> the destinations
+    void scatter(const void* host) const {
+        for (const Col& c : out)
+            if (c.bytes) memcpy(c.dst, (const char*)host + c.off, c.bytes);
+    }
+};
+
+// One allocation record on the host (the limited-mode solve works on these).
+struct HostCand {
+#define HOST_FIELD(name, type, required) type name;
+    WVA_ALLOC_COLUMNS(HOST_FIELD)
+#undef HOST_FIELD
+};
+
 // Host copy of the fleet columns (the caller's pointers are never retained).
 struct HostFleet {
     int A = 0, T = 0, M = 0, S = 0;
-    std::vector<float> acc_cost;
-    std::vector<int32_t> acc_mult, acc_type, type_capacity;
-    std::vector<uint8_t> perf_present;
-    std::vector<float> perf_alpha, perf_beta, perf_gamma, perf_delta;
-    std::vector<int32_t> perf_acc_count, perf_max_batch, perf_at_tokens;
-    std::vector<int32_t> srv_model, srv_priority;
-    std::vector<uint8_t> srv_has_target;
-    std::vector<float> srv_slo_itl, srv_slo_ttft, srv_slo_tps;
-    std::vector<uint8_t> srv_keep_acc;
-    std::vector<int32_t> srv_min_replicas, srv_max_batch;
-    std::vector<float> srv_arrival_rpm;
-    std::vector<int32_t> srv_in_tokens, srv_out_tokens, srv_cur_acc, srv_cur_replicas;
-    std::vector<float> srv_cur_cost;
+#define HOST_COLUMN(abi, name, type, len) std::vector<type> name;
+    WVA_FLEET_COLUMNS(HOST_COLUMN)
+#undef HOST_COLUMN
     bool unlimited = true, delayed_best_effort = false;
     int saturation_policy = 0;
     wva_tunables tun{10, 0.1f};
@@ -103,6 +133,12 @@ struct HostFleet {
         const size_t k = (size_t)srv_model[s] * A + a;
         const long long t = (long long)perf_max_batch[k] * (long long)perf_at_tokens[k] / srv_out_tokens[s];
         return (int)std::max<long long>(t, 1);
+    }
+    // limited mode charges every allocation to its accelerator's type: each accelerator needs one
+    bool every_acc_typed() const {
+        for (int a = 0; a < A; ++a)
+            if (T <= 0 || acc_type[a] < 0 || acc_type[a] >= T) return false;
+        return true;
     }
 };
 
@@ -158,9 +194,7 @@ struct wva_handle {
     } xchg;
     // the most recent solution (for wva_summarize): 0 none, 1 winner block on the device, 2 host copy (greedy)
     int last_kind = 0;
-    std::vector<int32_t> last_acc, last_replicas;
-    std::vector<float> last_cost;
-    std::vector<uint8_t> last_feasible;
+    std::vector<HostCand> last_win;
     DevBuf d_summary;
     bool dbg_cycles = false;
     const unsigned* dbg_plan = nullptr;
@@ -189,65 +223,46 @@ namespace {
 // control block on the device: a handful of ints
 enum { CTRL_COUNTER = 0, CTRL_FB_COUNT = 1, CTRL_FB_STATUS = 2, CTRL_INTS = 8 };
 
-// ---- SoA result blocks -------------------------------------------------------
+// ---- SoA result blocks: the wva_allocs columns of n records, 16-byte aligned ----------------
 struct Block {
-    size_t off_feasible, off_acc, off_replicas, off_batch, off_cost, off_value, off_itl, off_ttft, off_rho, off_rate;
+    struct {
+#define BLOCK_OFFSET(name, type, required) size_t name;
+        WVA_ALLOC_COLUMNS(BLOCK_OFFSET)
+#undef BLOCK_OFFSET
+    } off;
     size_t bytes;
     size_t n;
 };
 Block block_layout(size_t n) {
     Block b;
-    size_t o = 0;
+    Cols c(16);
+#define BLOCK_PLACE(name, type, required) b.off.name = c.take(sizeof(type) * n);
+    WVA_ALLOC_COLUMNS(BLOCK_PLACE)
+#undef BLOCK_PLACE
+    b.bytes = c.bytes;
     b.n = n;
-    b.off_feasible = o; o = align_up(o + n, 16);
-    b.off_acc = o; o = align_up(o + 4 * n, 16);
-    b.off_replicas = o; o = align_up(o + 4 * n, 16);
-    b.off_batch = o; o = align_up(o + 4 * n, 16);
-    b.off_cost = o; o = align_up(o + 4 * n, 16);
-    b.off_value = o; o = align_up(o + 4 * n, 16);
-    b.off_itl = o; o = align_up(o + 4 * n, 16);
-    b.off_ttft = o; o = align_up(o + 4 * n, 16);
-    b.off_rho = o; o = align_up(o + 4 * n, 16);
-    b.off_rate = o; o = align_up(o + 4 * n, 16);
-    b.bytes = o;
     return b;
 }
 AllocCols block_cols(void* base, const Block& b) {
-    char* p = (char*)base;
     AllocCols c;
-    c.feasible = (uint8_t*)(p + b.off_feasible);
-    c.acc = (int*)(p + b.off_acc);
-    c.replicas = (int*)(p + b.off_replicas);
-    c.batch = (int*)(p + b.off_batch);
-    c.cost = (float*)(p + b.off_cost);
-    c.value = (float*)(p + b.off_value);
-    c.itl = (float*)(p + b.off_itl);
-    c.ttft = (float*)(p + b.off_ttft);
-    c.rho = (float*)(p + b.off_rho);
-    c.max_rate = (float*)(p + b.off_rate);
+#define BLOCK_COL(name, type, required) c.name = (type*)((char*)base + b.off.name);
+    WVA_ALLOC_COLUMNS(BLOCK_COL)
+#undef BLOCK_COL
     return c;
 }
 void scatter_block(const void* host_block, const Block& b, const wva_allocs* out) {
     if (!out) return;
-    const char* p = (const char*)host_block;
-    const size_t n = b.n;
-    if (out->feasible) memcpy(out->feasible, p + b.off_feasible, n);
-    if (out->acc) memcpy(out->acc, p + b.off_acc, 4 * n);
-    if (out->replicas) memcpy(out->replicas, p + b.off_replicas, 4 * n);
-    if (out->batch) memcpy(out->batch, p + b.off_batch, 4 * n);
-    if (out->cost) memcpy(out->cost, p + b.off_cost, 4 * n);
-    if (out->value) memcpy(out->value, p + b.off_value, 4 * n);
-    if (out->itl) memcpy(out->itl, p + b.off_itl, 4 * n);
-    if (out->ttft) memcpy(out->ttft, p + b.off_ttft, 4 * n);
-    if (out->rho) memcpy(out->rho, p + b.off_rho, 4 * n);
-    if (out->max_rate) memcpy(out->max_rate, p + b.off_rate, 4 * n);
+#define BLOCK_SCATTER(name, type, required) \
+    if (out->name) memcpy(out->name, (const char*)host_block + b.off.name, sizeof(type) * b.n);
+    WVA_ALLOC_COLUMNS(BLOCK_SCATTER)
+#undef BLOCK_SCATTER
 }
 AllocCols cols_from_abi(const wva_allocs* a) {
     AllocCols c{};
     if (!a) return c;
-    c.feasible = a->feasible; c.acc = a->acc; c.replicas = a->replicas; c.batch = a->batch;
-    c.cost = a->cost; c.value = a->value; c.itl = a->itl; c.ttft = a->ttft; c.rho = a->rho;
-    c.max_rate = a->max_rate;
+#define ABI_COL(name, type, required) c.name = a->name;
+    WVA_ALLOC_COLUMNS(ABI_COL)
+#undef ABI_COL
     return c;
 }
 
@@ -256,72 +271,30 @@ AllocCols cols_from_abi(const wva_allocs* a) {
 const char* fleet_problem(const wva_fleet* f) {
     if (!f) return "fleet is NULL";
     if (f->n_acc < 0 || f->n_types < 0 || f->n_models < 0 || f->n_servers < 0) return "negative size in fleet";
-    const bool need_a = f->n_acc > 0, need_t = f->n_types > 0, need_ma = f->n_models > 0 && f->n_acc > 0,
-               need_s = f->n_servers > 0;
-    if (need_a && (!f->acc_cost || !f->acc_multiplicity || !f->acc_type)) return "NULL accelerator column";
-    if (need_t && !f->type_capacity) return "NULL capacity column";
-    if (need_ma && (!f->perf_present || !f->perf_alpha || !f->perf_beta || !f->perf_gamma || !f->perf_delta ||
-                    !f->perf_acc_count || !f->perf_max_batch || !f->perf_at_tokens))
-        return "NULL perf column";
-    if (need_s && (!f->srv_model || !f->srv_priority || !f->srv_has_target || !f->srv_slo_itl || !f->srv_slo_ttft ||
-                   !f->srv_slo_tps || !f->srv_keep_acc || !f->srv_min_replicas || !f->srv_max_batch ||
-                   !f->srv_arrival_rpm || !f->srv_in_tokens || !f->srv_out_tokens || !f->srv_cur_acc ||
-                   !f->srv_cur_replicas || !f->srv_cur_cost))
-        return "NULL server column";
+    // a column of positive length must be there; the message names the column's group
+    struct Len {
+        long long n;
+        const char* null_column;
+    };
+    const Len A{f->n_acc, "NULL accelerator column"}, T{f->n_types, "NULL capacity column"},
+        MA{(long long)f->n_models * f->n_acc, "NULL perf column"}, S{f->n_servers, "NULL server column"};
+#define NULL_CHECK(abi, name, type, len) \
+    if (len.n > 0 && !f->abi) return len.null_column;
+    WVA_FLEET_COLUMNS(NULL_CHECK)
+#undef NULL_CHECK
     for (int a = 0; a < f->n_acc; ++a)
         if (f->n_types > 0 && (f->acc_type[a] < 0 || f->acc_type[a] >= f->n_types)) return "accelerator type id out of range";
     if (f->tun.max_queue_to_batch_ratio < 0) return "negative queue ratio";
     return nullptr;
 }
-int validate_fleet(wva_handle* h, const wva_fleet* f) {
-    if (const char* what = fleet_problem(f)) return h->fail(WVA_ERR_BAD_ARG, what);
-    return WVA_OK;
-}
-
-template <class T>
-void copy_col(std::vector<T>& dst, const T* src, size_t n) {
-    dst.assign(src, src + n);
-}
-
-template <class T>
-Column place(std::vector<std::pair<Column, const void*>>& plan, size_t& off, const std::vector<T>& v) {
-    Column c{off, v.size() * sizeof(T)};
-    plan.push_back({c, v.data()});
-    off = align_up(off + std::max<size_t>(c.bytes, 1));
-    return c;
-}
 
 // Host copy of every column (the caller's pointers are never retained).
 void fill_host_fleet(HostFleet& hf, const wva_fleet* f) {
-    const size_t A = f->n_acc, T = f->n_types, M = f->n_models, S = f->n_servers;
+    const size_t A = f->n_acc, T = f->n_types, M = f->n_models, S = f->n_servers, MA = M * A;
     hf.A = (int)A; hf.T = (int)T; hf.M = (int)M; hf.S = (int)S;
-    copy_col(hf.acc_cost, f->acc_cost, A);
-    copy_col(hf.acc_mult, f->acc_multiplicity, A);
-    copy_col(hf.acc_type, f->acc_type, A);
-    copy_col(hf.type_capacity, f->type_capacity, T);
-    copy_col(hf.perf_present, f->perf_present, M * A);
-    copy_col(hf.perf_alpha, f->perf_alpha, M * A);
-    copy_col(hf.perf_beta, f->perf_beta, M * A);
-    copy_col(hf.perf_gamma, f->perf_gamma, M * A);
-    copy_col(hf.perf_delta, f->perf_delta, M * A);
-    copy_col(hf.perf_acc_count, f->perf_acc_count, M * A);
-    copy_col(hf.perf_max_batch, f->perf_max_batch, M * A);
-    copy_col(hf.perf_at_tokens, f->perf_at_tokens, M * A);
-    copy_col(hf.srv_model, f->srv_model, S);
-    copy_col(hf.srv_priority, f->srv_priority, S);
-    copy_col(hf.srv_has_target, f->srv_has_target, S);
-    copy_col(hf.srv_slo_itl, f->srv_slo_itl, S);
-    copy_col(hf.srv_slo_ttft, f->srv_slo_ttft, S);
-    copy_col(hf.srv_slo_tps, f->srv_slo_tps, S);
-    copy_col(hf.srv_keep_acc, f->srv_keep_acc, S);
-    copy_col(hf.srv_min_replicas, f->srv_min_replicas, S);
-    copy_col(hf.srv_max_batch, f->srv_max_batch, S);
-    copy_col(hf.srv_arrival_rpm, f->srv_arrival_rpm, S);
-    copy_col(hf.srv_in_tokens, f->srv_in_tokens, S);
-    copy_col(hf.srv_out_tokens, f->srv_out_tokens, S);
-    copy_col(hf.srv_cur_acc, f->srv_cur_acc, S);
-    copy_col(hf.srv_cur_replicas, f->srv_cur_replicas, S);
-    copy_col(hf.srv_cur_cost, f->srv_cur_cost, S);
+#define FILL(abi, name, type, len) hf.name.assign(f->abi, f->abi + len);
+    WVA_FLEET_COLUMNS(FILL)
+#undef FILL
     hf.unlimited = f->unlimited != 0;
     hf.delayed_best_effort = f->delayed_best_effort != 0;
     hf.saturation_policy = f->saturation_policy;
@@ -329,83 +302,33 @@ void fill_host_fleet(HostFleet& hf, const wva_fleet* f) {
 }
 
 int upload_fleet(wva_handle* h, const wva_fleet* f) {
-    int rc = validate_fleet(h, f);
-    if (rc) return rc;
+    if (const char* what = fleet_problem(f)) return h->fail(WVA_ERR_BAD_ARG, what);
     CK(cudaStreamSynchronize(h->stream));  // the pinned stage may still feed an earlier async copy
     HostFleet& hf = h->hf;
     fill_host_fleet(hf, f);
 
-    // one arena, one H2D copy; the three load columns are adjacent so that
-    // wva_update_load moves a single contiguous range
-    std::vector<std::pair<Column, const void*>> plan;
-    size_t off = 0;
-    Column c_rate = place(plan, off, hf.srv_arrival_rpm);
-    Column c_in = place(plan, off, hf.srv_in_tokens);
-    Column c_out = place(plan, off, hf.srv_out_tokens);
-    Column c_acc_cost = place(plan, off, hf.acc_cost);
-    Column c_acc_mult = place(plan, off, hf.acc_mult);
-    Column c_acc_type = place(plan, off, hf.acc_type);
-    Column c_cap = place(plan, off, hf.type_capacity);
-    Column c_pp = place(plan, off, hf.perf_present);
-    Column c_pa = place(plan, off, hf.perf_alpha);
-    Column c_pb = place(plan, off, hf.perf_beta);
-    Column c_pg = place(plan, off, hf.perf_gamma);
-    Column c_pd = place(plan, off, hf.perf_delta);
-    Column c_pc = place(plan, off, hf.perf_acc_count);
-    Column c_pm = place(plan, off, hf.perf_max_batch);
-    Column c_pt = place(plan, off, hf.perf_at_tokens);
-    Column c_sm = place(plan, off, hf.srv_model);
-    Column c_sp = place(plan, off, hf.srv_priority);
-    Column c_st = place(plan, off, hf.srv_has_target);
-    Column c_si = place(plan, off, hf.srv_slo_itl);
-    Column c_sf = place(plan, off, hf.srv_slo_ttft);
-    Column c_ss = place(plan, off, hf.srv_slo_tps);
-    Column c_sk = place(plan, off, hf.srv_keep_acc);
-    Column c_sn = place(plan, off, hf.srv_min_replicas);
-    Column c_sb = place(plan, off, hf.srv_max_batch);
-    Column c_ca = place(plan, off, hf.srv_cur_acc);
-    Column c_cr = place(plan, off, hf.srv_cur_replicas);
-    Column c_cc = place(plan, off, hf.srv_cur_cost);
-    const size_t total = off;
-    CK(h->arena.ensure(total));
-    CK(h->stage.ensure(total));
-    for (auto& pr : plan)
-        if (pr.first.bytes) memcpy((char*)h->stage.p + pr.first.off, pr.second, pr.first.bytes);
-    CK(cudaMemcpyAsync(h->arena.p, h->stage.p, total, cudaMemcpyHostToDevice, h->stream));
-
-    char* d = (char*)h->arena.p;
+    // one arena in list order, one H2D copy
+    Cols arena(256);
+#define ARENA_PLACE(abi, name, type, len)                   \
+    const size_t bytes_##name = sizeof(type) * hf.name.size(); \
+    const Column c_##name{arena.take(bytes_##name), bytes_##name};
+    WVA_FLEET_COLUMNS(ARENA_PLACE)
+#undef ARENA_PLACE
+    CK(h->arena.ensure(arena.bytes));
+    CK(h->stage.ensure(arena.bytes));
+    char* st = (char*)h->stage.p;
+    const char* d = (const char*)h->arena.p;
     DevFleet& df = h->df;
+#define ARENA_FILL(abi, name, type, len)                                         \
+    if (c_##name.bytes) memcpy(st + c_##name.off, hf.name.data(), c_##name.bytes); \
+    df.name = (const type*)(d + c_##name.off);
+    WVA_FLEET_COLUMNS(ARENA_FILL)
+#undef ARENA_FILL
+    CK(cudaMemcpyAsync(h->arena.p, h->stage.p, arena.bytes, cudaMemcpyHostToDevice, h->stream));
     df.A = hf.A; df.T = hf.T; df.M = hf.M; df.S = hf.S;
-    df.acc_cost = (const float*)(d + c_acc_cost.off);
-    df.acc_mult = (const int*)(d + c_acc_mult.off);
-    df.acc_type = (const int*)(d + c_acc_type.off);
-    df.type_capacity = (const int*)(d + c_cap.off);
-    df.perf_present = (const uint8_t*)(d + c_pp.off);
-    df.perf_alpha = (const float*)(d + c_pa.off);
-    df.perf_beta = (const float*)(d + c_pb.off);
-    df.perf_gamma = (const float*)(d + c_pg.off);
-    df.perf_delta = (const float*)(d + c_pd.off);
-    df.perf_acc_count = (const int*)(d + c_pc.off);
-    df.perf_max_batch = (const int*)(d + c_pm.off);
-    df.perf_at_tokens = (const int*)(d + c_pt.off);
-    df.srv_model = (const int*)(d + c_sm.off);
-    df.srv_priority = (const int*)(d + c_sp.off);
-    df.srv_has_target = (const uint8_t*)(d + c_st.off);
-    df.srv_slo_itl = (const float*)(d + c_si.off);
-    df.srv_slo_ttft = (const float*)(d + c_sf.off);
-    df.srv_slo_tps = (const float*)(d + c_ss.off);
-    df.srv_keep_acc = (const uint8_t*)(d + c_sk.off);
-    df.srv_min_replicas = (const int*)(d + c_sn.off);
-    df.srv_max_batch = (const int*)(d + c_sb.off);
-    df.srv_arrival_rpm = (const float*)(d + c_rate.off);
-    df.srv_in_tokens = (const int*)(d + c_in.off);
-    df.srv_out_tokens = (const int*)(d + c_out.off);
-    df.srv_cur_acc = (const int*)(d + c_ca.off);
-    df.srv_cur_replicas = (const int*)(d + c_cr.off);
-    df.srv_cur_cost = (const float*)(d + c_cc.off);
     df.ratio = hf.tun.max_queue_to_batch_ratio;
     df.penalty = hf.tun.accel_penalty_factor;
-    h->col_rate = c_rate; h->col_in = c_in; h->col_out = c_out;
+    h->col_rate = c_srv_arrival_rpm; h->col_in = c_srv_in_tokens; h->col_out = c_srv_out_tokens;
     h->resident = true;
     h->epoch_tokens++;
     h->last_kind = 0;
@@ -427,26 +350,36 @@ int ensure_scratch(wva_handle* h, int Nmax, int ratio, size_t* slot_doubles, int
     return WVA_OK;
 }
 
+// The (server, accelerator) pairs that keep(s, a) accepts, as ids s * A + a with their batch sizes N, sorted
+// by descending N (stable: equal N keep the pair order).
+template <class Keep>
+int sorted_pairs(wva_handle* h, Keep keep, std::vector<int>& pairs, std::vector<int>& N) {
+    const HostFleet& hf = h->hf;
+    const int A = hf.A, S = hf.S;
+    std::vector<int> Ns((size_t)S * A, 0);
+    pairs.clear();
+    for (int s = 0; s < S; ++s)
+        for (int a = 0; a < A; ++a)
+            if (keep(s, a)) {
+                const int n = hf.pair_batch(s, a);
+                if (n > (1 << 20)) return h->fail(WVA_ERR_UNSUPPORTED, "batch size above 2^20");
+                Ns[(size_t)s * A + a] = n;
+                pairs.push_back(s * A + a);
+            }
+    std::stable_sort(pairs.begin(), pairs.end(), [&](int x, int y) { return Ns[x] > Ns[y]; });
+    N.resize(pairs.size());
+    for (size_t j = 0; j < pairs.size(); ++j) N[j] = Ns[pairs[j]];
+    return WVA_OK;
+}
+
 // ---- size path (K1) ---------------------------------------------------------
 int prepare_size(wva_handle* h) {
     if (h->size_epoch == h->epoch_tokens) return WVA_OK;
     const HostFleet& hf = h->hf;
-    const int A = hf.A, S = hf.S;
-    std::vector<int> pairs;
-    std::vector<int> Ns((size_t)S * A, 0);
-    for (int s = 0; s < S; ++s)
-        for (int a = 0; a < A; ++a)
-            if (hf.pair_class(s, a, true) == PAIR_LOAD) {
-                const int N = hf.pair_batch(s, a);
-                if (N > (1 << 20)) return h->fail(WVA_ERR_UNSUPPORTED, "batch size above 2^20");
-                Ns[(size_t)s * A + a] = N;
-                pairs.push_back(s * A + a);
-            }
-    std::stable_sort(pairs.begin(), pairs.end(), [&](int x, int y) { return Ns[x] > Ns[y]; });
-    const int n = (int)pairs.size();
-    h->cand_pair = pairs;
-    h->cand_N.resize(n);
-    for (int j = 0; j < n; ++j) h->cand_N[j] = Ns[pairs[j]];
+    int rc = sorted_pairs(h, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, h->cand_pair,
+                          h->cand_N);
+    if (rc) return rc;
+    const int n = (int)h->cand_pair.size();
     h->size_Nmax = n ? h->cand_N[0] : 1;
     if (n) {
         CK(h->d_cand_pair.ensure(sizeof(int) * n));
@@ -499,28 +432,28 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     const size_t cap = per_cand * (size_t)n;                 // requests per round, worst case
     const size_t n2 = 2 * (size_t)n;
     // state block
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t at = o; o = align_up(o + bytes, 16); return at; };
-    const size_t o_xmin = take(4 * n2), o_xmax = take(4 * n2), o_xs = take(4 * n2);
-    const size_t o_sst = take(n2), o_inc = take(n2), o_iter = take(n2), o_ind = take(n2), o_slot = take(4 * n2);
-    const size_t o_phase = take(n), o_rmax = take(4 * (size_t)n), o_l2s0 = take(4 * (size_t)n), o_l2sN = take(4 * (size_t)n),
-                 o_lsN = take(4 * (size_t)n), o_rstar = take(4 * (size_t)n), o_cost = take(4 * (size_t)n),
-                 o_nrep = take(8 * (size_t)n), o_aslot = take(4 * (size_t)n);
-    CK(h->d_sz_state.ensure(o));
+    Cols st(16);
+    const size_t o_xmin = st.take(4 * n2), o_xmax = st.take(4 * n2), o_xs = st.take(4 * n2);
+    const size_t o_sst = st.take(n2), o_inc = st.take(n2), o_iter = st.take(n2), o_ind = st.take(n2),
+                 o_slot = st.take(4 * n2);
+    const size_t o_phase = st.take(n), o_rmax = st.take(4 * (size_t)n), o_l2s0 = st.take(4 * (size_t)n),
+                 o_l2sN = st.take(4 * (size_t)n), o_lsN = st.take(4 * (size_t)n), o_rstar = st.take(4 * (size_t)n),
+                 o_cost = st.take(4 * (size_t)n), o_nrep = st.take(8 * (size_t)n), o_aslot = st.take(4 * (size_t)n);
+    CK(h->d_sz_state.ensure(st.bytes));
     char* sp = (char*)h->d_sz_state.p;
     // request block
-    o = 0;
-    const size_t r_id = take(4 * cap), r_lam = take(4 * cap), r_key = take(cap), r_out = take(16 * cap), r_bail = take(cap),
-                 r_cnt = take(16);
-    CK(h->d_sz_req.ensure(o));
+    Cols rq(16);
+    const size_t r_id = rq.take(4 * cap), r_lam = rq.take(4 * cap), r_key = rq.take(cap), r_out = rq.take(16 * cap),
+                 r_bail = rq.take(cap), r_cnt = rq.take(16);
+    CK(h->d_sz_req.ensure(rq.bytes));
     char* rp = (char*)h->d_sz_req.p;
     // sort workspace
     const size_t chunks = (cap + kSortChunk - 1) / kSortChunk;
     const size_t max_items = (cap + 31) / 32 + chunks;
-    o = 0;
-    const size_t w_order = take(4 * cap), w_items = take(8 * max_items), w_sorted = take(8 * max_items),
-                 w_cnt = take(4 * (2 * kClasses + 8));
-    CK(h->d_sz_sort.ensure(o));
+    Cols ws(16);
+    const size_t w_order = ws.take(4 * cap), w_items = ws.take(8 * max_items), w_sorted = ws.take(8 * max_items),
+                 w_cnt = ws.take(4 * (2 * kClasses + 8));
+    CK(h->d_sz_sort.ensure(ws.bytes));
     char* wp = (char*)h->d_sz_sort.p;
     CK(h->sz_pin.ensure(64));
 
@@ -647,10 +580,56 @@ int finish_timing(wva_handle* h) {
     return WVA_OK;
 }
 
-int check_fallback_status(wva_handle* h, const int* ctrl_host, long long cap) {
-    if (ctrl_host[CTRL_FB_STATUS] != 0)
+// What a call with host results places on the device and copies back.  Every call has a winner block [S];
+// the size path also writes a candidate block [S*A].
+struct HostCall {
+    bool cand;                      // the work writes a candidate block
+    bool copy_cand, copy_win;       // which blocks come back to the host
+    const Cols* extra = nullptr;    // further device columns copied straight to their destinations ...
+    const void* extra_dev = nullptr;  // ... from this buffer
+    // set by run_host: the block layouts and their host copies in out_stage (NULL when not copied)
+    Block bc{}, bw{};
+    const char *cand_host = nullptr, *win_host = nullptr;
+};
+
+// The shared end of every call with host results, in stream order: place the blocks on the device, record
+// ev_d0, enqueue the work, copy the wanted blocks and the control ints into out_stage and then c.extra,
+// synchronise once and check the fallback status.  enqueue(dc, dw, fb_cap) enqueues the kernels into the
+// device blocks and sets the largest fallback count that is not an error.
+template <class Enqueue>
+int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
+    const HostFleet& hf = h->hf;
+    c.bc = block_layout(c.cand ? (size_t)hf.S * hf.A : 0);
+    c.bw = block_layout(hf.S);
+    if (c.cand) CK(h->d_cand_block.ensure(c.bc.bytes + 16));
+    CK(h->d_win_block.ensure(c.bw.bytes + 16));
+    const AllocCols dc = c.cand ? block_cols(h->d_cand_block.p, c.bc) : AllocCols{};
+    const AllocCols dw = block_cols(h->d_win_block.p, c.bw);
+    CK(cudaEventRecord(h->ev_d0, h->stream));
+    long long fb_cap = 0;
+    int rc = enqueue(dc, dw, fb_cap);
+    if (rc) return rc;
+    Cols stage(256);
+    const size_t o_cand = stage.take(c.copy_cand ? c.bc.bytes : 0), o_win = stage.take(c.copy_win ? c.bw.bytes : 0),
+                 o_ctrl = stage.take(CTRL_INTS * sizeof(int));
+    CK(h->out_stage.ensure(stage.bytes));
+    char* hs = (char*)h->out_stage.p;
+    if (c.copy_cand) {
+        CK(cudaMemcpyAsync(hs + o_cand, h->d_cand_block.p, c.bc.bytes, cudaMemcpyDeviceToHost, h->stream));
+        c.cand_host = hs + o_cand;
+    }
+    if (c.copy_win) {
+        CK(cudaMemcpyAsync(hs + o_win, h->d_win_block.p, c.bw.bytes, cudaMemcpyDeviceToHost, h->stream));
+        c.win_host = hs + o_win;
+    }
+    const int* ctrl = (const int*)(hs + o_ctrl);
+    CK(cudaMemcpyAsync(hs + o_ctrl, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    if (c.extra) CK(c.extra->copy_back(c.extra_dev, h->stream));
+    rc = finish_timing(h);
+    if (rc) return rc;
+    if (ctrl[CTRL_FB_STATUS] != 0)
         return h->fail(WVA_ERR_UNSUPPORTED, "input outside the supported numeric domain (rescale loop does not terminate)");
-    if ((long long)ctrl_host[CTRL_FB_COUNT] > cap)
+    if ((long long)ctrl[CTRL_FB_COUNT] > fb_cap)
         return h->fail(WVA_ERR_UNSUPPORTED, "too many cells need the stored-vector fallback");
     return WVA_OK;
 }
@@ -658,29 +637,15 @@ int check_fallback_status(wva_handle* h, const int* ctrl_host, long long cap) {
 // resident analyze/solve with host outputs
 int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     if (!h->resident) return h->fail(WVA_ERR_STATE, "no resident fleet (call wva_upload first)");
-    const HostFleet& hf = h->hf;
-    const size_t n_pairs = (size_t)hf.S * hf.A;
-    const Block bc = block_layout(n_pairs), bw = block_layout(hf.S);
-    CK(h->d_cand_block.ensure(bc.bytes + 16));
-    CK(h->d_win_block.ensure(bw.bytes + 16));
-    const AllocCols dc = block_cols(h->d_cand_block.p, bc), dw = block_cols(h->d_win_block.p, bw);
-    CK(cudaEventRecord(h->ev_d0, h->stream));
-    int rc = enqueue_size(h, dc, winners ? &dw : nullptr);
+    HostCall c{true, candidates != nullptr, winners != nullptr};
+    const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
+        const int rc = enqueue_size(h, dc, winners ? &dw : nullptr);
+        fb_cap = (long long)h->cand_pair.size() + 1;
+        return rc;
+    });
     if (rc) return rc;
-    const size_t stage_bytes = align_up(bc.bytes) + align_up(bw.bytes) + 256;
-    CK(h->out_stage.ensure(stage_bytes));
-    char* hs = (char*)h->out_stage.p;
-    if (candidates && bc.bytes) CK(cudaMemcpyAsync(hs, h->d_cand_block.p, bc.bytes, cudaMemcpyDeviceToHost, h->stream));
-    if (winners && bw.bytes)
-        CK(cudaMemcpyAsync(hs + align_up(bc.bytes), h->d_win_block.p, bw.bytes, cudaMemcpyDeviceToHost, h->stream));
-    int* ctrl_host = (int*)(hs + align_up(bc.bytes) + align_up(bw.bytes));
-    CK(cudaMemcpyAsync(ctrl_host, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    rc = finish_timing(h);
-    if (rc) return rc;
-    rc = check_fallback_status(h, ctrl_host, (long long)h->cand_pair.size() + 1);
-    if (rc) return rc;
-    scatter_block(hs, bc, candidates);
-    scatter_block(hs + align_up(bc.bytes), bw, winners);
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
     return WVA_OK;
 }
 
@@ -702,21 +667,26 @@ struct GridPlan {
     size_t n_cells;
     int n_blocks;
     int Bmax;
+    Cols cells{256};  // layout of d_cells; the copy-back goes to the caller's cell table
 };
 
 // Per-cell columns kept on the device for every grid solve: flags + ttft/itl/rho (+ throughput
-// when the caller asked for the cell table).
-int ensure_cells(wva_handle* h, GridPlan& plan, bool want_cells, bool want_throughput) {
-    const size_t nc = std::max<size_t>(plan.n_cells, 1);
-    const size_t bytes = align_up(nc) + 4 * align_up(4 * nc);
-    CK(h->d_cells.ensure(bytes));
+// when the caller asked for it).  They travel to the host only when `cells` names a column.
+int ensure_cells(wva_handle* h, GridPlan& plan, const wva_cells* cells) {
+    const bool want = cells && (cells->flags || cells->ttft || cells->itl || cells->rho || cells->throughput);
+    const wva_cells dst = want ? *cells : wva_cells{};
+    const size_t nc = plan.n_cells;
+    Cols& c = plan.cells;
+    const size_t o_flags = c.take(nc, dst.flags), o_ttft = c.take(4 * nc, dst.ttft), o_itl = c.take(4 * nc, dst.itl),
+                 o_rho = c.take(4 * nc, dst.rho), o_thr = c.take(4 * nc, dst.throughput);
+    CK(h->d_cells.ensure(c.bytes));
     char* p = (char*)h->d_cells.p;
-    plan.args.cells.flags = (uint8_t*)p;
-    plan.args.cells.ttft = (float*)(p + align_up(nc));
-    plan.args.cells.itl = (float*)(p + align_up(nc) + align_up(4 * nc));
-    plan.args.cells.rho = (float*)(p + align_up(nc) + 2 * align_up(4 * nc));
-    plan.args.cells.throughput = want_throughput ? (float*)(p + align_up(nc) + 3 * align_up(4 * nc)) : nullptr;
-    plan.args.want_cells = want_cells ? 1 : 0;
+    plan.args.cells.flags = (uint8_t*)(p + o_flags);
+    plan.args.cells.ttft = (float*)(p + o_ttft);
+    plan.args.cells.itl = (float*)(p + o_itl);
+    plan.args.cells.rho = (float*)(p + o_rho);
+    plan.args.cells.throughput = dst.throughput ? (float*)(p + o_thr) : nullptr;
+    plan.args.want_cells = want ? 1 : 0;
     return WVA_OK;
 }
 
@@ -820,28 +790,32 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     plan->n_cells = (size_t)n_cells;
     plan->n_blocks = (int)((n_cells + kSortChunk - 1) / kSortChunk);
     const size_t nc = std::max<size_t>(plan->n_cells, 1);
-    // sort workspace: order u32 [n_cells] | items u64 | items_sorted u64 | item counter
+    // sort workspace: order u32 [n_cells] | items u64 | items_sorted u64 | item counter |
+    // per-cell records in global item order (32 x 16 bytes per item)
     const size_t max_items = (nc + 31) / 32 + (size_t)std::max(plan->n_blocks, 1);
-    // ... | per-cell records in global item order (32 x 16 bytes per item)
-    const size_t ws = align_up(4 * nc) + 2 * align_up(8 * max_items) + align_up(4 * (2 * kClasses + 32)) +
-                      align_up(512 * max_items);
-    CK(h->d_sort.ensure(ws));
+    Cols ws(256);
+    const size_t o_order = ws.take(4 * nc), o_items = ws.take(8 * max_items), o_sorted = ws.take(8 * max_items),
+                 o_count = ws.take(4 * (2 * kClasses + 32)), o_recs = ws.take(512 * max_items);
+    CK(h->d_sort.ensure(ws.bytes));
     char* w = (char*)h->d_sort.p;
-    g.order = (unsigned*)w;
-    g.items = (unsigned long long*)(w + align_up(4 * nc));
-    g.items_sorted = (unsigned long long*)(w + align_up(4 * nc) + align_up(8 * max_items));
-    g.item_count = (unsigned*)(w + align_up(4 * nc) + 2 * align_up(8 * max_items));
-    g.recs = (uint4*)(w + align_up(4 * nc) + 2 * align_up(8 * max_items) + align_up(4 * (2 * kClasses + 32)));
+    g.order = (unsigned*)(w + o_order);
+    g.items = (unsigned long long*)(w + o_items);
+    g.items_sorted = (unsigned long long*)(w + o_sorted);
+    g.item_count = (unsigned*)(w + o_count);
+    g.recs = (uint4*)(w + o_recs);
     h->dbg_plan = g.item_count + 2 * kClasses + 1;
     const size_t n_best = std::max<size_t>((size_t)S * A * R, 1);
     CK(h->d_best.ensure(sizeof(int) * n_best));
     g.best_rank = (int*)h->d_best.p;
     const size_t n_pairs_alloc = std::max<size_t>((size_t)S * A, 1);
-    CK(h->d_rows.ensure(align_up((2 * sizeof(double) + sizeof(int)) * n_best + 64) + 48 * n_pairs_alloc));
-    g.row_acc = (double*)h->d_rows.p;
+    Cols rows(256);
+    const size_t o_rows = rows.take((2 * sizeof(double) + sizeof(int)) * n_best + 64),  // row_acc | row_sump | row_j
+        o_pair_rec = rows.take(48 * n_pairs_alloc);
+    CK(h->d_rows.ensure(rows.bytes));
+    g.row_acc = (double*)((char*)h->d_rows.p + o_rows);
     g.row_sump = g.row_acc + n_best;
     g.row_j = (int*)(g.row_sump + n_best);
-    g.pair_rec = (float4*)((char*)h->d_rows.p + align_up((2 * sizeof(double) + sizeof(int)) * n_best + 64));
+    g.pair_rec = (float4*)((char*)h->d_rows.p + o_pair_rec);
     g.Bmax = h->grid_Bmax;
     g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
     g.fb_cap = (int)std::min<size_t>(nc, (size_t)1 << 22);
@@ -877,7 +851,6 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
     int Kmax;
     int rc = ensure_scratch(h, plan.Bmax, hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
     if (rc) return rc;
-    const size_t n_best = (size_t)hf.S * hf.A * g.R;
     if (plan.n_cells == 0) CK(cudaEventRecord(h->ev_k0, h->stream));
     if (plan.n_cells > 0) {
         CK(cudaMemsetAsync(g.item_count, 0, sizeof(unsigned) * (2 * kClasses + 32), h->stream));
@@ -888,9 +861,6 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
         }
         h->launches++;
         grid_sort_local<<<plan.n_blocks, kSortThreads, 0, h->stream>>>(g);
-        // one warp per item; the item count lives on the device, so launch for the worst case
-        const size_t max_items = (plan.n_cells + 31) / 32 + (size_t)plan.n_blocks;
-        (void)max_items;
         grid_items_scatter<<<(unsigned)(16 * h->sm_count), 256, 0, h->stream>>>(g);  // warp per item (grid-stride)
         h->launches++;
         CK(cudaEventRecord(h->ev_k0, h->stream));  // wva_last_kernel_ms = the dominant kernel alone
@@ -918,12 +888,6 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
 // device; the greedy pass is inherently sequential over a shared capacity map (SURVEY.md
 // §8e), so it stays on the host.  Sorts are stable (the reference's pdqsort is not): ties
 // resolve by server id / accelerator id.
-struct HostCand {
-    uint8_t feasible;
-    int acc, replicas, batch;
-    float cost, value, itl, ttft, rho, max_rate;
-};
-
 struct GreedyEntry {  // greedy.go:16-22
     int server, priority, cur = 0;
     std::vector<int> accs;  // candidate accelerator ids ordered by value
@@ -1116,94 +1080,55 @@ class GreedySolver {
 };
 
 void block_to_cands(const void* host_block, const Block& b, std::vector<HostCand>& out) {
-    const char* p = (const char*)host_block;
     out.resize(b.n);
-    for (size_t i = 0; i < b.n; ++i) {
-        HostCand& c = out[i];
-        c.feasible = ((const uint8_t*)(p + b.off_feasible))[i];
-        c.acc = ((const int*)(p + b.off_acc))[i];
-        c.replicas = ((const int*)(p + b.off_replicas))[i];
-        c.batch = ((const int*)(p + b.off_batch))[i];
-        c.cost = ((const float*)(p + b.off_cost))[i];
-        c.value = ((const float*)(p + b.off_value))[i];
-        c.itl = ((const float*)(p + b.off_itl))[i];
-        c.ttft = ((const float*)(p + b.off_ttft))[i];
-        c.rho = ((const float*)(p + b.off_rho))[i];
-        c.max_rate = ((const float*)(p + b.off_rate))[i];
-    }
+#define BLOCK_LOAD(name, type, required) \
+    for (size_t i = 0; i < b.n; ++i) out[i].name = ((const type*)((const char*)host_block + b.off.name))[i];
+    WVA_ALLOC_COLUMNS(BLOCK_LOAD)
+#undef BLOCK_LOAD
 }
 void cands_to_abi(const std::vector<HostCand>& v, wva_allocs* out) {
     if (!out) return;
-    for (size_t i = 0; i < v.size(); ++i) {
-        const HostCand& c = v[i];
-        if (out->feasible) out->feasible[i] = c.feasible;
-        if (out->acc) out->acc[i] = c.acc;
-        if (out->replicas) out->replicas[i] = c.replicas;
-        if (out->batch) out->batch[i] = c.batch;
-        if (out->cost) out->cost[i] = c.cost;
-        if (out->value) out->value[i] = c.value;
-        if (out->itl) out->itl[i] = c.itl;
-        if (out->ttft) out->ttft[i] = c.ttft;
-        if (out->rho) out->rho[i] = c.rho;
-        if (out->max_rate) out->max_rate[i] = c.max_rate;
-    }
+#define ABI_STORE(name, type, required) \
+    if (out->name)                      \
+        for (size_t i = 0; i < v.size(); ++i) out->name[i] = v[i].name;
+    WVA_ALLOC_COLUMNS(ABI_STORE)
+#undef ABI_STORE
 }
 
+// The required columns must be there; the others read as 0 when NULL.
 bool abi_to_cands(const wva_allocs* in, size_t n, std::vector<HostCand>& out) {
-    if (!in || (n && (!in->feasible || !in->acc || !in->replicas || !in->cost || !in->value))) return false;
-    out.resize(n);
-    for (size_t i = 0; i < n; ++i) {
-        HostCand& c = out[i];
-        c.feasible = in->feasible[i];
-        c.acc = in->acc[i];
-        c.replicas = in->replicas[i];
-        c.batch = in->batch ? in->batch[i] : 0;
-        c.cost = in->cost[i];
-        c.value = in->value[i];
-        c.itl = in->itl ? in->itl[i] : 0.0f;
-        c.ttft = in->ttft ? in->ttft[i] : 0.0f;
-        c.rho = in->rho ? in->rho[i] : 0.0f;
-        c.max_rate = in->max_rate ? in->max_rate[i] : 0.0f;
-    }
+    if (!in) return false;
+#define ABI_REQUIRED(name, type, required) \
+    if (required && n && !in->name) return false;
+    WVA_ALLOC_COLUMNS(ABI_REQUIRED)
+#undef ABI_REQUIRED
+    out.assign(n, HostCand{});
+#define ABI_LOAD(name, type, required) \
+    if (in->name)                      \
+        for (size_t i = 0; i < n; ++i) out[i].name = in->name[i];
+    WVA_ALLOC_COLUMNS(ABI_LOAD)
+#undef ABI_LOAD
     return true;
 }
 
 // resident analyze + greedy solve with host outputs
 int run_greedy_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     const HostFleet& hf = h->hf;
-    for (int a = 0; a < hf.A; ++a)
-        if (hf.T <= 0 || hf.acc_type[a] < 0 || hf.acc_type[a] >= hf.T)
-            return h->fail(WVA_ERR_BAD_ARG, "limited mode needs a type id and a capacity for every accelerator");
-    const size_t n_pairs = (size_t)hf.S * hf.A;
-    const Block bc = block_layout(n_pairs), bw = block_layout(hf.S);
-    CK(h->d_cand_block.ensure(bc.bytes + 16));
-    CK(h->d_win_block.ensure(bw.bytes + 16));
-    const AllocCols dc = block_cols(h->d_cand_block.p, bc), dw = block_cols(h->d_win_block.p, bw);
-    CK(cudaEventRecord(h->ev_d0, h->stream));
-    int rc = enqueue_size(h, dc, &dw);  // the unlimited kernel also assigns value = transition penalty
-    if (rc) return rc;
-    const size_t stage_bytes = align_up(bc.bytes) + 256;
-    CK(h->out_stage.ensure(stage_bytes));
-    char* hs = (char*)h->out_stage.p;
-    if (bc.bytes) CK(cudaMemcpyAsync(hs, h->d_cand_block.p, bc.bytes, cudaMemcpyDeviceToHost, h->stream));
-    int* ctrl_host = (int*)(hs + align_up(bc.bytes));
-    CK(cudaMemcpyAsync(ctrl_host, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    rc = finish_timing(h);
-    if (rc) return rc;
-    rc = check_fallback_status(h, ctrl_host, (long long)h->cand_pair.size() + 1);
+    if (!hf.every_acc_typed())
+        return h->fail(WVA_ERR_BAD_ARG, "limited mode needs a type id and a capacity for every accelerator");
+    HostCall c{true, true, false};
+    const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
+        const int rc = enqueue_size(h, dc, &dw);  // the unlimited kernel also assigns value = transition penalty
+        fb_cap = (long long)h->cand_pair.size() + 1;
+        return rc;
+    });
     if (rc) return rc;
     std::vector<HostCand> cand, win((size_t)hf.S);
-    block_to_cands(hs, bc, cand);
+    block_to_cands(c.cand_host, c.bc, cand);
     GreedySolver(hf, cand, win).run();
     cands_to_abi(cand, candidates);
     cands_to_abi(win, winners);
-    h->last_feasible.resize(hf.S); h->last_acc.resize(hf.S); h->last_replicas.resize(hf.S); h->last_cost.resize(hf.S);
-    for (int s = 0; s < hf.S; ++s) {
-        h->last_feasible[s] = win[s].feasible;
-        h->last_acc[s] = win[s].acc;
-        h->last_replicas[s] = win[s].replicas;
-        h->last_cost[s] = win[s].cost;
-    }
+    h->last_win = std::move(win);
     h->last_kind = 2;
     return WVA_OK;
 }
@@ -1472,8 +1397,7 @@ int wva_solve_greedy(const wva_fleet* fleet, wva_allocs* candidates, wva_allocs*
     if (fleet_problem(fleet) || !winners) return WVA_ERR_BAD_ARG;
     HostFleet hf;
     fill_host_fleet(hf, fleet);
-    for (int a = 0; a < hf.A; ++a)
-        if (hf.T <= 0 || hf.acc_type[a] < 0 || hf.acc_type[a] >= hf.T) return WVA_ERR_BAD_ARG;
+    if (!hf.every_acc_typed()) return WVA_ERR_BAD_ARG;
     std::vector<HostCand> cand, win((size_t)hf.S);
     if (!abi_to_cands(candidates, (size_t)hf.S * hf.A, cand)) return WVA_ERR_BAD_ARG;
     GreedySolver(hf, cand, win).run();
@@ -1528,7 +1452,7 @@ int wva_grid_solve_device(wva_handle* h, const wva_grid* grid, wva_allocs* winne
     GridPlan plan;
     rc = prepare_grid(h, grid, &plan);
     if (rc) return rc;
-    rc = ensure_cells(h, plan, false, false);
+    rc = ensure_cells(h, plan, nullptr);
     if (rc) return rc;
     CK(cudaEventRecord(h->ev_d0, h->stream));
     rc = enqueue_grid(h, plan, cols_from_abi(winners_dev));
@@ -1549,43 +1473,17 @@ int wva_grid_solve(wva_handle* h, const wva_fleet* fleet, const wva_grid* grid, 
     GridPlan plan;
     rc = prepare_grid(h, grid, &plan);
     if (rc) return rc;
-    const HostFleet& hf = h->hf;
-    const Block bw = block_layout(hf.S);
-    CK(h->d_win_block.ensure(bw.bytes + 16));
-    const AllocCols dw = block_cols(h->d_win_block.p, bw);
-    // per-cell columns live on the device for every solve; they travel to the host only on request
-    const size_t nc = plan.n_cells;
-    const bool want_cells = cells && (cells->flags || cells->ttft || cells->itl || cells->rho || cells->throughput);
-    rc = ensure_cells(h, plan, want_cells, want_cells && cells->throughput);
+    rc = ensure_cells(h, plan, cells);
     if (rc) return rc;
-    if (want_cells && nc)  // cells that are never analysed must read back as 0
-        CK(cudaMemsetAsync(h->d_cells.p, 0, align_up(nc) + 4 * align_up(4 * nc), h->stream));
-    CK(cudaEventRecord(h->ev_d0, h->stream));
-    rc = enqueue_grid(h, plan, dw);
+    if (plan.args.want_cells && plan.n_cells)  // cells that are never analysed must read back as 0
+        CK(cudaMemsetAsync(h->d_cells.p, 0, plan.cells.bytes, h->stream));
+    HostCall c{false, false, true, &plan.cells, h->d_cells.p};
+    rc = run_host(h, c, [&](const AllocCols&, const AllocCols& dw, long long& fb_cap) {
+        fb_cap = plan.args.fb_cap;
+        return enqueue_grid(h, plan, dw);
+    });
     if (rc) return rc;
-    const size_t stage_bytes = align_up(bw.bytes) + 256;
-    CK(h->out_stage.ensure(stage_bytes));
-    char* hs = (char*)h->out_stage.p;
-    if (bw.bytes) CK(cudaMemcpyAsync(hs, h->d_win_block.p, bw.bytes, cudaMemcpyDeviceToHost, h->stream));
-    int* ctrl_host = (int*)(hs + align_up(bw.bytes));
-    CK(cudaMemcpyAsync(ctrl_host, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    if (want_cells && nc) {
-        const char* p = (const char*)h->d_cells.p;
-        if (cells->flags) CK(cudaMemcpyAsync(cells->flags, p, nc, cudaMemcpyDeviceToHost, h->stream));
-        if (cells->ttft) CK(cudaMemcpyAsync(cells->ttft, p + align_up(nc), 4 * nc, cudaMemcpyDeviceToHost, h->stream));
-        if (cells->itl)
-            CK(cudaMemcpyAsync(cells->itl, p + align_up(nc) + align_up(4 * nc), 4 * nc, cudaMemcpyDeviceToHost, h->stream));
-        if (cells->rho)
-            CK(cudaMemcpyAsync(cells->rho, p + align_up(nc) + 2 * align_up(4 * nc), 4 * nc, cudaMemcpyDeviceToHost, h->stream));
-        if (cells->throughput)
-            CK(cudaMemcpyAsync(cells->throughput, p + align_up(nc) + 3 * align_up(4 * nc), 4 * nc, cudaMemcpyDeviceToHost,
-                               h->stream));
-    }
-    rc = finish_timing(h);
-    if (rc) return rc;
-    rc = check_fallback_status(h, ctrl_host, plan.args.fb_cap);
-    if (rc) return rc;
-    scatter_block(hs, bw, winners);
+    scatter_block(c.win_host, c.bw, winners);
     h->last_kind = 1;
     return WVA_OK;
 }
@@ -1607,8 +1505,9 @@ int wva_summarize(wva_handle* h, wva_summary* out) {
         std::vector<float> cost(T, 0.0f);
         std::vector<int64_t> cnt(T, 0);
         for (size_t s = 0; s < S; ++s) {
-            const int feas = h->last_feasible[s], acc = h->last_acc[s], rep = h->last_replicas[s];
-            const float c = h->last_cost[s];
+            const HostCand& w = h->last_win[s];
+            const int feas = w.feasible, acc = w.acc, rep = w.replicas;
+            const float c = w.cost;
             const int m = hf.srv_model[s];
             if (feas && acc >= 0 && acc < hf.A && m >= 0 && m < hf.M) {
                 const int t = hf.acc_type[acc];
@@ -1639,12 +1538,14 @@ int wva_summarize(wva_handle* h, wva_summary* out) {
     // device winner block of the last solve
     const Block bw = block_layout(S);
     const AllocCols dw = block_cols(h->d_win_block.p, bw);
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t at = o; o = align_up(o + std::max<size_t>(bytes, 1), 16); return at; };
-    const size_t o_cnt = take(8 * T), o_pres = take(T), o_lim = take(4 * T), o_cost = take(4 * T);
-    const size_t o_oa = take(4 * S), o_na = take(4 * S), o_or = take(4 * S), o_nr = take(4 * S), o_dc = take(4 * S);
-    CK(h->d_summary.ensure(o));
-    CK(h->out_stage.ensure(o));
+    Cols sc(16);
+    const size_t o_cnt = sc.take(8 * T, out->type_count), o_pres = sc.take(T, out->type_present),
+                 o_lim = sc.take(4 * T, out->type_limit), o_cost = sc.take(4 * T, out->type_cost);
+    const size_t o_oa = sc.take(4 * S, out->diff_old_acc), o_na = sc.take(4 * S, out->diff_new_acc),
+                 o_or = sc.take(4 * S, out->diff_old_replicas), o_nr = sc.take(4 * S, out->diff_new_replicas),
+                 o_dc = sc.take(4 * S, out->diff_cost);
+    CK(h->d_summary.ensure(sc.bytes));
+    CK(h->out_stage.ensure(sc.bytes));
     char* d = (char*)h->d_summary.p;
     SummaryOut so;
     so.type_count = (long long*)(d + o_cnt);
@@ -1660,17 +1561,9 @@ int wva_summarize(wva_handle* h, wva_summary* out) {
     h->launches++;
     CK(cudaGetLastError());
     char* hs = (char*)h->out_stage.p;
-    CK(cudaMemcpyAsync(hs, d, o, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(hs, d, sc.bytes, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    if (out->type_count) memcpy(out->type_count, hs + o_cnt, 8 * T);
-    if (out->type_present) memcpy(out->type_present, hs + o_pres, T);
-    if (out->type_limit) memcpy(out->type_limit, hs + o_lim, 4 * T);
-    if (out->type_cost) memcpy(out->type_cost, hs + o_cost, 4 * T);
-    if (out->diff_old_acc) memcpy(out->diff_old_acc, hs + o_oa, 4 * S);
-    if (out->diff_new_acc) memcpy(out->diff_new_acc, hs + o_na, 4 * S);
-    if (out->diff_old_replicas) memcpy(out->diff_old_replicas, hs + o_or, 4 * S);
-    if (out->diff_new_replicas) memcpy(out->diff_new_replicas, hs + o_nr, 4 * S);
-    if (out->diff_cost) memcpy(out->diff_cost, hs + o_dc, 4 * S);
+    sc.scatter(hs);
     return WVA_OK;
 }
 
@@ -1684,14 +1577,15 @@ int wva_mm1k_solve(wva_handle* h, int32_t n, const int32_t* K, const float* lamb
         if (K[i] > (1 << 20)) return h->fail(WVA_ERR_UNSUPPORTED, "MM1K: K above 2^20");
     CK(cudaSetDevice(h->device));
     const size_t N = (size_t)n;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t at = o; o = align_up(o + bytes, 16); return at; };
-    const size_t i_K = take(4 * N), i_lam = take(4 * N), i_mu = take(4 * N);
-    const size_t in_bytes = o;
-    const size_t o_sum = take(8 * N), o_valid = take(N), o_rho = take(4 * N), o_nsys = take(4 * N), o_thr = take(4 * N),
-                 o_resp = take(4 * N), o_serv = take(4 * N), o_wait = take(4 * N), o_qlen = take(4 * N);
-    CK(h->d_summary.ensure(o));
-    CK(h->out_stage.ensure(o));
+    Cols mc(16);
+    const size_t i_K = mc.take(4 * N), i_lam = mc.take(4 * N), i_mu = mc.take(4 * N);
+    const size_t in_bytes = mc.bytes;
+    const size_t o_sum = mc.take(8 * N, out->sum_p), o_valid = mc.take(N, out->is_valid), o_rho = mc.take(4 * N, out->rho),
+                 o_nsys = mc.take(4 * N, out->avg_num_in_system), o_thr = mc.take(4 * N, out->throughput),
+                 o_resp = mc.take(4 * N, out->avg_resp_time), o_serv = mc.take(4 * N, out->avg_serv_time),
+                 o_wait = mc.take(4 * N, out->avg_wait_time), o_qlen = mc.take(4 * N, out->avg_queue_length);
+    CK(h->d_summary.ensure(mc.bytes));
+    CK(h->out_stage.ensure(mc.bytes));
     char* d = (char*)h->d_summary.p;
     char* hs = (char*)h->out_stage.p;
     memcpy(hs + i_K, K, 4 * N);
@@ -1715,17 +1609,9 @@ int wva_mm1k_solve(wva_handle* h, int32_t n, const int32_t* K, const float* lamb
     mm1k_kernel<<<(unsigned)((N + 127) / 128), 128, 0, h->stream>>>(g);
     h->launches++;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(hs + in_bytes, d + in_bytes, o - in_bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(hs + in_bytes, d + in_bytes, mc.bytes - in_bytes, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    if (out->sum_p) memcpy(out->sum_p, hs + o_sum, 8 * N);
-    if (out->is_valid) memcpy(out->is_valid, hs + o_valid, N);
-    if (out->rho) memcpy(out->rho, hs + o_rho, 4 * N);
-    if (out->avg_num_in_system) memcpy(out->avg_num_in_system, hs + o_nsys, 4 * N);
-    if (out->throughput) memcpy(out->throughput, hs + o_thr, 4 * N);
-    if (out->avg_resp_time) memcpy(out->avg_resp_time, hs + o_resp, 4 * N);
-    if (out->avg_serv_time) memcpy(out->avg_serv_time, hs + o_serv, 4 * N);
-    if (out->avg_wait_time) memcpy(out->avg_wait_time, hs + o_wait, 4 * N);
-    if (out->avg_queue_length) memcpy(out->avg_queue_length, hs + o_qlen, 4 * N);
+    mc.scatter(hs);
     return WVA_OK;
 }
 
@@ -1740,34 +1626,31 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
     if (rc) return rc;
     const HostFleet& hf = h->hf;
     const int A = hf.A, S = hf.S;
-    // every (server, acc) with a profile, ignoring keepAccelerator; sorted by descending N
-    std::vector<int> pairs, Ns((size_t)S * A, 0);
-    for (int s = 0; s < S; ++s)
-        for (int a = 0; a < A; ++a) {
-            const int m = hf.srv_model[s];
-            if (hf.srv_in_tokens[s] < 0 || hf.srv_out_tokens[s] < 1 || m < 0 || m >= hf.M ||
-                !hf.perf_present[(size_t)m * A + a])
-                continue;
-            const int N = hf.pair_batch(s, a);
-            if (N > (1 << 20)) return h->fail(WVA_ERR_UNSUPPORTED, "batch size above 2^20");
-            Ns[(size_t)s * A + a] = N;
-            pairs.push_back(s * A + a);
-        }
-    std::stable_sort(pairs.begin(), pairs.end(), [&](int x, int y) { return Ns[x] > Ns[y]; });
+    // every (server, acc) with a profile, ignoring keepAccelerator
+    std::vector<int> pairs, lens;
+    rc = sorted_pairs(h,
+                      [&](int s, int a) {
+                          const int m = hf.srv_model[s];
+                          return hf.srv_in_tokens[s] >= 0 && hf.srv_out_tokens[s] >= 1 && m >= 0 && m < hf.M &&
+                                 hf.perf_present[(size_t)m * A + a];
+                      },
+                      pairs, lens);
+    if (rc) return rc;
     const int n = (int)pairs.size();
-    std::vector<int> lens(n);
     std::vector<long long> offs(n);
     long long off = 0;
     for (int e = 0; e < n; ++e) {
-        lens[e] = Ns[pairs[e]];
         offs[e] = off;
         off += lens[e];
     }
     const size_t n_out = (size_t)S * A * n_rates;
-    const size_t out_bytes = align_up(n_out) + 5 * align_up(4 * n_out);
-    CK(h->d_sweep.ensure(std::max<size_t>(out_bytes, 256)));
+    Cols sw(256);
+    const size_t o_valid = sw.take(n_out, out->valid), o_rate = sw.take(4 * n_out, out->rate),
+                 o_ttft = sw.take(4 * n_out, out->ttft), o_itl = sw.take(4 * n_out, out->itl),
+                 o_thr = sw.take(4 * n_out, out->throughput), o_rho = sw.take(4 * n_out, out->rho);
+    CK(h->d_sweep.ensure(sw.bytes));
     char* p = (char*)h->d_sweep.p;
-    CK(cudaMemsetAsync(p, 0, std::max<size_t>(out_bytes, 256), h->stream));
+    CK(cudaMemsetAsync(p, 0, sw.bytes, h->stream));
     CK(cudaEventRecord(h->ev_d0, h->stream));
     CK(cudaEventRecord(h->ev_k0, h->stream));
     if (n) {
@@ -1793,12 +1676,12 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         g.n_rates = n_rates;
         g.n_chunks = (n_rates + 31) / 32;
         g.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
-        g.valid = (uint8_t*)p;
-        g.rate = (float*)(p + align_up(n_out));
-        g.ttft = (float*)(p + align_up(n_out) + align_up(4 * n_out));
-        g.itl = (float*)(p + align_up(n_out) + 2 * align_up(4 * n_out));
-        g.throughput = (float*)(p + align_up(n_out) + 3 * align_up(4 * n_out));
-        g.rho = (float*)(p + align_up(n_out) + 4 * align_up(4 * n_out));
+        g.valid = (uint8_t*)(p + o_valid);
+        g.rate = (float*)(p + o_rate);
+        g.ttft = (float*)(p + o_ttft);
+        g.itl = (float*)(p + o_itl);
+        g.throughput = (float*)(p + o_thr);
+        g.rho = (float*)(p + o_rho);
         g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
         int per_sm = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sweep_kernel, 256, 0));
@@ -1814,17 +1697,7 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
     CK(h->out_stage.ensure(256));
     int* ctrl_host = (int*)h->out_stage.p;
     CK(cudaMemcpyAsync(ctrl_host, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    if (n_out) {
-        CK(cudaMemcpyAsync(out->valid, p, n_out, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaMemcpyAsync(out->rate, p + align_up(n_out), 4 * n_out, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaMemcpyAsync(out->ttft, p + align_up(n_out) + align_up(4 * n_out), 4 * n_out, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaMemcpyAsync(out->itl, p + align_up(n_out) + 2 * align_up(4 * n_out), 4 * n_out, cudaMemcpyDeviceToHost,
-                           h->stream));
-        CK(cudaMemcpyAsync(out->throughput, p + align_up(n_out) + 3 * align_up(4 * n_out), 4 * n_out,
-                           cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaMemcpyAsync(out->rho, p + align_up(n_out) + 4 * align_up(4 * n_out), 4 * n_out, cudaMemcpyDeviceToHost,
-                           h->stream));
-    }
+    CK(sw.copy_back(p, h->stream));
     rc = finish_timing(h);
     if (rc) return rc;
     if (ctrl_host[CTRL_FB_COUNT] != 0)

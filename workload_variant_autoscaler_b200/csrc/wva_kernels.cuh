@@ -16,25 +16,46 @@
 
 namespace wva {
 
+// The columns of wva_fleet in declaration order: X(wva_fleet member, DevFleet / HostFleet member, element type,
+// length).  The length is A (accelerators), T (accelerator types), MA (models x accelerators) or S (servers).
+// DevFleet and the host engine's copy, upload and NULL checks are generated from this list.  The host arena
+// follows this order, and wva_update_load copies srv_arrival_rpm, srv_in_tokens and srv_out_tokens as one
+// range: those three must stay adjacent.
+#define WVA_FLEET_COLUMNS(X)                          \
+    X(acc_cost, acc_cost, float, A)                   \
+    X(acc_multiplicity, acc_mult, int32_t, A)         \
+    X(acc_type, acc_type, int32_t, A)                 \
+    X(type_capacity, type_capacity, int32_t, T)       \
+    X(perf_present, perf_present, uint8_t, MA)        \
+    X(perf_alpha, perf_alpha, float, MA)              \
+    X(perf_beta, perf_beta, float, MA)                \
+    X(perf_gamma, perf_gamma, float, MA)              \
+    X(perf_delta, perf_delta, float, MA)              \
+    X(perf_acc_count, perf_acc_count, int32_t, MA)    \
+    X(perf_max_batch, perf_max_batch, int32_t, MA)    \
+    X(perf_at_tokens, perf_at_tokens, int32_t, MA)    \
+    X(srv_model, srv_model, int32_t, S)               \
+    X(srv_priority, srv_priority, int32_t, S)         \
+    X(srv_has_target, srv_has_target, uint8_t, S)     \
+    X(srv_slo_itl, srv_slo_itl, float, S)             \
+    X(srv_slo_ttft, srv_slo_ttft, float, S)           \
+    X(srv_slo_tps, srv_slo_tps, float, S)             \
+    X(srv_keep_acc, srv_keep_acc, uint8_t, S)         \
+    X(srv_min_replicas, srv_min_replicas, int32_t, S) \
+    X(srv_max_batch, srv_max_batch, int32_t, S)       \
+    X(srv_arrival_rpm, srv_arrival_rpm, float, S)     \
+    X(srv_in_tokens, srv_in_tokens, int32_t, S)       \
+    X(srv_out_tokens, srv_out_tokens, int32_t, S)     \
+    X(srv_cur_acc, srv_cur_acc, int32_t, S)           \
+    X(srv_cur_replicas, srv_cur_replicas, int32_t, S) \
+    X(srv_cur_cost, srv_cur_cost, float, S)
+
 // Device image of wva_fleet (all pointers are device pointers).
 struct DevFleet {
     int A, T, M, S;
-    const float* acc_cost;
-    const int* acc_mult;
-    const int* acc_type;
-    const int* type_capacity;
-    const uint8_t* perf_present;
-    const float *perf_alpha, *perf_beta, *perf_gamma, *perf_delta;
-    const int *perf_acc_count, *perf_max_batch, *perf_at_tokens;
-    const int *srv_model, *srv_priority;
-    const uint8_t* srv_has_target;
-    const float *srv_slo_itl, *srv_slo_ttft, *srv_slo_tps;
-    const uint8_t* srv_keep_acc;
-    const int *srv_min_replicas, *srv_max_batch;
-    const float* srv_arrival_rpm;
-    const int *srv_in_tokens, *srv_out_tokens;
-    const int *srv_cur_acc, *srv_cur_replicas;
-    const float* srv_cur_cost;
+#define WVA_DEV_COLUMN(abi, name, type, len) const type* name;
+    WVA_FLEET_COLUMNS(WVA_DEV_COLUMN)
+#undef WVA_DEV_COLUMN
     int ratio;      // config.MaxQueueToBatchRatio
     float penalty;  // config.AccelPenaltyFactor
 };
@@ -85,29 +106,37 @@ __device__ __forceinline__ Cand cand_warp_min(Cand c) {
     return c;
 }
 
+// The columns of wva_allocs in declaration order, each also a member of Cand: X(member, element type,
+// required): wva_solve_greedy needs the required columns on input and reads a NULL column of the others as 0.
+#define WVA_ALLOC_COLUMNS(X) \
+    X(feasible, uint8_t, 1)  \
+    X(acc, int32_t, 1)       \
+    X(replicas, int32_t, 1)  \
+    X(batch, int32_t, 0)     \
+    X(cost, float, 1)        \
+    X(value, float, 1)       \
+    X(itl, float, 0)         \
+    X(ttft, float, 0)        \
+    X(rho, float, 0)         \
+    X(max_rate, float, 0)
+
 // SoA columns of wva_allocs on the device.
 struct AllocCols {
-    uint8_t* feasible;
-    int *acc, *replicas, *batch;
-    float *cost, *value, *itl, *ttft, *rho, *max_rate;
+#define WVA_ALLOC_COLUMN(name, type, required) type* name;
+    WVA_ALLOC_COLUMNS(WVA_ALLOC_COLUMN)
+#undef WVA_ALLOC_COLUMN
 };
 __device__ __forceinline__ void store_cand(const AllocCols& o, size_t i, const Cand& c) {
-    if (o.feasible) o.feasible[i] = (uint8_t)c.feasible;
-    if (o.acc) o.acc[i] = c.acc;
-    if (o.replicas) o.replicas[i] = c.replicas;
-    if (o.batch) o.batch[i] = c.batch;
-    if (o.cost) o.cost[i] = c.cost;
-    if (o.value) o.value[i] = c.value;
-    if (o.itl) o.itl[i] = c.itl;
-    if (o.ttft) o.ttft[i] = c.ttft;
-    if (o.rho) o.rho[i] = c.rho;
-    if (o.max_rate) o.max_rate[i] = c.max_rate;
+#define WVA_STORE_COLUMN(name, type, required) \
+    if (o.name) o.name[i] = (type)c.name;
+    WVA_ALLOC_COLUMNS(WVA_STORE_COLUMN)
+#undef WVA_STORE_COLUMN
 }
 __device__ __forceinline__ Cand load_cand(const AllocCols& o, size_t i) {
     Cand c;
-    c.feasible = o.feasible[i]; c.acc = o.acc[i]; c.replicas = o.replicas[i]; c.batch = o.batch[i];
-    c.cost = o.cost[i]; c.value = o.value[i]; c.itl = o.itl[i]; c.ttft = o.ttft[i]; c.rho = o.rho[i];
-    c.max_rate = o.max_rate[i];
+#define WVA_LOAD_COLUMN(name, type, required) c.name = o.name[i];
+    WVA_ALLOC_COLUMNS(WVA_LOAD_COLUMN)
+#undef WVA_LOAD_COLUMN
     return c;
 }
 

@@ -20,16 +20,8 @@ DEFAULT_LOW_PRIORITY = 100           # defaults.go:27
 DEFAULT_HIGH_PRIORITY = 1            # defaults.go:30
 
 
-def _f32(x):
-    return np.ascontiguousarray(x, dtype=np.float32)
-
-
 def _i32(x):
     return np.ascontiguousarray(x, dtype=np.int32)
-
-
-def _u8(x):
-    return np.ascontiguousarray(x, dtype=np.uint8)
 
 
 @dataclass
@@ -77,26 +69,18 @@ class Fleet:
     server_names: list = field(default_factory=list)
     type_names: list = field(default_factory=list)
 
-    _F32 = ("acc_cost", "perf_alpha", "perf_beta", "perf_gamma", "perf_delta", "srv_slo_itl", "srv_slo_ttft",
-            "srv_slo_tps", "srv_arrival_rpm", "srv_cur_cost")
-    _I32 = ("acc_multiplicity", "acc_type", "type_capacity", "perf_acc_count", "perf_max_batch", "perf_at_tokens",
-            "srv_model", "srv_priority", "srv_min_replicas", "srv_max_batch", "srv_in_tokens", "srv_out_tokens",
-            "srv_cur_acc", "srv_cur_replicas")
-    _U8 = ("perf_present", "srv_has_target", "srv_keep_acc")
+    # the array columns by element type (bench.py counts the fleet's bytes over these)
+    _F32, _I32, _U8 = (tuple(n for n, dt, _ in _abi.FLEET_COLUMNS if dt is t) for t in (np.float32, np.int32, np.uint8))
 
     def __post_init__(self):
-        for n in self._F32:
-            setattr(self, n, _f32(getattr(self, n)))
-        for n in self._I32:
-            setattr(self, n, _i32(getattr(self, n)))
-        for n in self._U8:
-            setattr(self, n, _u8(getattr(self, n)))
+        for n, dt, _ in _abi.FLEET_COLUMNS:
+            setattr(self, n, np.ascontiguousarray(getattr(self, n), dtype=dt))
         A = self.n_acc
-        for n in ("perf_present", "perf_alpha", "perf_beta", "perf_gamma", "perf_delta", "perf_acc_count",
-                  "perf_max_batch", "perf_at_tokens"):
-            a = getattr(self, n)
-            assert a.size % max(A, 1) == 0, n
-            setattr(self, n, a.reshape(-1, A) if A else a.reshape(0, 0))
+        for n, _, length in _abi.FLEET_COLUMNS:
+            if length == "MA":
+                a = getattr(self, n)
+                assert a.size % max(A, 1) == 0, n
+                setattr(self, n, a.reshape(-1, A) if A else a.reshape(0, 0))
 
     @property
     def n_acc(self) -> int:
@@ -118,7 +102,7 @@ class Fleet:
         """ctypes ``wva_fleet`` viewing this object's arrays (keep ``self`` alive)."""
         # building ~45 ctypes pointers costs more than the rest of a small solve's host path: the struct is
         # cached and reused while the very same array objects are still attached (in-place edits keep it valid)
-        names = self._F32 + self._I32 + self._U8
+        names = [n for n, _, _ in _abi.FLEET_COLUMNS]
         arrs = [getattr(self, n) for n in names]
         cache = self.__dict__.get("_c_cache")
         if cache is not None and all(a is b for a, b in zip(cache[0], arrs)):
