@@ -872,7 +872,13 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
     if (plan.n_cells > 0) {
         grid_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
                                                                (int*)h->d_ctrl.p + CTRL_FB_STATUS);
-        h->launches++;
+        // the shared-chain cells: 32 rows per warp; with a cell table, one warp per 32 rows and slice of ranks
+        const size_t n_warps = ((size_t)hf.S * hf.A * g.R + 31) / 32 *
+                               (g.want_cells ? (size_t)(g.B + kSharedSlice - 1) / kSharedSlice : 1);
+        const unsigned ctas = (unsigned)((n_warps + kSharedThreads / 32 - 1) / (kSharedThreads / 32));
+        if (g.want_cells) grid_shared<1><<<ctas, kSharedThreads, 0, h->stream>>>(g);
+        else grid_shared<32><<<ctas, kSharedThreads, 0, h->stream>>>(g);
+        h->launches += 2;  // grid_fallback, grid_shared
     }
     if (hf.S > 0) {
         grid_finalize<<<hf.S, 256, 0, h->stream>>>(g, winners);

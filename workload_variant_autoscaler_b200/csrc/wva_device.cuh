@@ -807,7 +807,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 // same head-type exit test at the same state, never reaches its tail, and every state it
 // accumulates lies below N = b.  Those cells therefore share pass 1 and pass 2 outright (same
 // operations in the same order, hence the same bits) and differ only in the N-dependent float
-// tail, which grid_sort_local evaluates per cell.  Anything off the plain fast path (tiny p that
+// tail, which grid_shared evaluates per cell.  Anything off the plain fast path (tiny p that
 // needs IEEE division, a chain that reaches the table end, window violations) just reports
 // "no sharing" and the cells go through grid_kernel as usual.
 // ---------------------------------------------------------------------------

@@ -318,7 +318,7 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 //   grid_rows        per (pair, replica level): the chain every large-enough batch size shares
 //                    (solve_row); also the (server, replica) rate block and the batch-rank reset
 //   grid_sort_local  per chunk of 8192 cells: gates + Analyze's rate checks; cells that share their
-//                    row's chain are finished inline; the others get a log-domain length estimate,
+//                    row's chain are left to grid_shared; the others get a log-domain length estimate,
 //                    an 8-bit class and a local counting sort -> warp items; the last CTA plans
 //                    grid_kernel's queues (grid_items_plan)
 //   grid_items_scatter  items ordered globally, longest class first
@@ -327,6 +327,8 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 //                    per-cell columns, atomicMin of the smallest feasible batch rank per
 //                    (server, accelerator, replica)
 //   grid_fallback   stored-vector re-run of the rare cells the streaming solve bails on
+//   grid_shared     per (pair, replica level): the cells that share the row's chain, in ascending batch
+//                   order up to the row's first feasible one (all of them when the cell table is stored)
 //   grid_finalize   per-server argmin (warp shuffle -> shared memory -> winner record)
 //
 // For a fixed (server, accelerator, replica level) the transition penalty and the cost do
@@ -370,7 +372,8 @@ struct GridArgs {
                              // {min_replicas, tps flag (int bits), 0, 0} -- one 48-byte record instead of ten scattered loads
     uint4* recs;             // [items][32] per sorted cell: {cell, lambda bits, table entry offset, batch size | class << 23 | pad << 31}
     int want_cells;          // 0: the caller did not ask for the cell table -> cells that share their row's chain store
-                             // nothing (grid_finalize recomputes the few winners among them); 1: every cell is stored
+                             // nothing and are evaluated only up to the row's first feasible one (grid_finalize
+                             // recomputes the few winners among them); 1: every cell is stored
     int* fb_count;           // cells that need the stored-vector fallback
     long long* fb_cells;
     int fb_cap;
@@ -467,7 +470,7 @@ __device__ __forceinline__ void store_cell(const GridArgs& g, long long cell, in
     if (g.cells.throughput) g.cells.throughput[cell] = m.throughput;
 }
 
-// A cell that shares its row's chain (grid_sort_local): stats_from_row + metrics_from with everything that does
+// A cell that shares its row's chain (grid_shared): stats_from_row + metrics_from with everything that does
 // not depend on the batch size hoisted — per pair (PairConst: the operands of EffectiveConcurrency, PrefillTime,
 // DecodeTime), per (pair, replica level) (resp = avgNumInSystem / throughput, 1 - sumP).  Same operations in the
 // same order on the same operands as the unhoisted functions, hence the same bits.
@@ -678,51 +681,22 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
         const unsigned R = (unsigned)g.R, B = (unsigned)g.B, A = (unsigned)f.A;
         const unsigned row0 = (unsigned)(base / R), row1 = (unsigned)((base + n_here - 1) / R);
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        // feasible shared cells lower best_rank[(pair, replica level)]: a lane meets the same replica
-        // levels row after row, so it keeps the running minimum of its first two levels in registers
-        // and issues one atomic per pair instead of one per cell
-        unsigned cur_sa = 0xffffffffu;
-        int best0 = INT_MAX, best1 = INT_MAX;
-        auto flush_best = [&]() {
-            if (best0 != INT_MAX) atomicMin(&g.best_rank[(size_t)cur_sa * R + lane], best0);
-            if (best1 != INT_MAX) atomicMin(&g.best_rank[(size_t)cur_sa * R + lane + 32], best1);
-            best0 = best1 = INT_MAX;
-        };
         // pair-level constants are re-read only when the walk crosses into the next pair; so are the
         // lane's own row constants (its first two replica levels: rate, lambda, the row's shared chain)
         struct LaneRow {
             float4 rt;
-            // shared-chain results of the row.  inv == false: a = sum(i p[i]), b = 1 - sumP, r = resp (avgNumInSystem /
-            // throughput).  inv == true (row_invariant holds): the three floats of RowInv ride in the same registers
-            // (a = {f0, w0}, r = effu), so the hot loop carries no more state than before.
-            double a, b;
-            float r;
-            int jl, rep;
-            bool inv;
+            int jl;
         };
+        unsigned cur_sa = 0xffffffffu;
         LaneRow c0{}, c1{};
         unsigned sa = (row0 + warp) / B;
         int bi = (int)(row0 + warp - sa * B);
         int s = 0, t = 0;
         long long toff = -1;
-        PairConst pc{};
-        FeasRow fr{};
         auto load_lane = [&](unsigned ri, LaneRow& c) {
             if (ri >= R || toff < 0) return;
-            const size_t rowid = (size_t)sa * R + ri;
             c.rt = g.rt[(unsigned)s * R + ri];
-            c.jl = g.row_j[rowid];
-            c.a = g.row_acc[rowid];
-            c.b = __dsub_rn(1.0, g.row_sump[rowid]);
-            c.r = row_resp_time(c.a, c.rt.y);
-            c.rep = g.replicas[ri];
-            c.inv = false;
-            RowInv inv;
-            if (c.jl != INT_MAX && row_invariant(pc, c.a, c.b, c.r, c.rt.y, g.Bmax, inv)) {
-                c.inv = true;
-                c.a = __hiloint2double(__float_as_int(inv.w0), __float_as_int(inv.f0));
-                c.r = inv.effu;
-            }
+            c.jl = g.row_j[(size_t)sa * R + ri];
         };
         for (unsigned row = row0 + warp; row <= row1; row += kSortThreads / 32, bi += kSortThreads / 32) {
             while (bi >= (int)B) {
@@ -730,15 +704,10 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
                 ++sa;
             }
             if (sa != cur_sa) {
-                flush_best();
                 cur_sa = sa;
                 s = (int)(sa / A);
                 toff = g.pair_tab_off[sa];
-                if (toff >= 0) {
-                    t = g.pair_tab_idx[sa];
-                    pc = pair_const(qparams_of(f, s, (int)(sa - (unsigned)s * A)));
-                }
-                fr = feas_row(f, s, 0.0f);
+                if (toff >= 0) t = g.pair_tab_idx[sa];
                 load_lane(lane, c0);
                 load_lane(lane + 32, c1);
             }
@@ -746,53 +715,29 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
             const int K = b + b * f.ratio;
             float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
             if (toff >= 0) pb = g.pb[(size_t)t * g.B + bi];
-            if (fr.tps) fr.lim = feas_lim(pb.x);
-            const int rank = g.batch_rank[bi];
             // one cell: (row, ri) with the lane's cached row constants
-            auto do_cell = [&](unsigned ri, const LaneRow& c, int slot) {
+            auto do_cell = [&](unsigned ri, const LaneRow& c) {
                 const long long cell = (long long)row * R + ri;
                 if (cell < base || cell >= base + n_here) return;
                 int key = 255;
-                bool done_here = false;
                 if (toff >= 0 && !(c.rt.x <= 0.0f) && !(c.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
-                    if (c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23)) {
-                        done_here = true;
-                        // the whole solve is shared with the row: only the N-dependent tail is per cell
-                        Metrics m;
-                        if (c.inv) {
-                            RowInv inv;
-                            inv.f0 = __int_as_float(__double2loint(c.a));
-                            inv.w0 = __int_as_float(__double2hiint(c.a));
-                            inv.effu = c.r;
-                            m = shared_cell_metrics_inv(pc, inv, c.rt.y, b, g.want_cells != 0);
-                        } else {
-                            m = shared_cell_metrics(pc, c.a, c.b, c.r, c.rt.y, b);
-                        }
-                        const bool feas = cell_feasible(fr, c.rep, c.rt.y, m);
-                        if (g.want_cells) store_cell(g, cell, 1, feas ? 1 : 0, m);
-                        if (feas) {
-                            if (slot == 0) best0 = min(best0, rank);
-                            else if (slot == 1) best1 = min(best1, rank);
-                            else atomicMin(&g.best_rank[(size_t)sa * R + ri], rank);
-                        }
-                    } else {
+                    // a cell that shares its row's chain stays at class 255: grid_shared evaluates it after grid_kernel
+                    if (!(c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23)))
                         key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, c.rt.y, c.rt.z, pb.w, pb.y, pb.z));
-                    }
                 }
                 keys[cell - base] = (uint8_t)key;
-                if (key != 255) seg_inc(hist, key);  // class 255 (finished here / not analysable) needs no slot
+                if (key != 255) seg_inc(hist, key);  // class 255 (shared / not analysable) needs no slot
                 // (the cell table, when requested, is cleared by the host before the launch: cells that are never
                 // analysed read back as 0 without a store per cell here)
             };
-            if ((unsigned)lane < R) do_cell(lane, c0, 0);
-            if ((unsigned)lane + 32 < R) do_cell(lane + 32, c1, 1);
+            if ((unsigned)lane < R) do_cell(lane, c0);
+            if ((unsigned)lane + 32 < R) do_cell(lane + 32, c1);
             for (unsigned ri = lane + 64; ri < R; ri += 32) {
                 LaneRow c;
                 load_lane(ri, c);
-                do_cell(ri, c, 2);
+                do_cell(ri, c);
             }
         }
-        flush_best();
     }
     __syncthreads();
     if (threadIdx.x < 32) {  // exclusive scan of the 256 class counts by one warp
@@ -1148,12 +1093,123 @@ __global__ void grid_fallback(GridArgs g, double* scratch, size_t slot_doubles, 
     }
 }
 
+// The cells that share their row's chain (analysable, b >= jl + 2, K < 2^23), after grid_kernel and grid_fallback.
+// Ranks ascend in batch size, so a row's shared cells are one run of ranks; its cells with K >= 2^23 (grid_kernel's)
+// follow that run and end it.  Without a cell table only the row's smallest feasible rank counts: a row whose
+// best_rank already lies below its first shared rank is decided, and otherwise its walk up the ranks stops at the
+// first feasible shared cell or at best_rank, whichever comes first.  With a cell table every shared cell is
+// evaluated and stored.
+//
+// A warp owns 32 rows (a lane each) and finds which of them need a walk and between which ranks; the rows to walk
+// are then taken 32 / G at a time, G lanes per row and G ranks per step.  Without a cell table (G = 32) most rows are
+// decided, so a warp's rows are spread over the grid (the undecided ones cluster by pair) and each of the few
+// others gets the whole warp.  With a cell table (G = 1) every shared cell is work: a warp owns 32 consecutive
+// replica levels (coalesced stores) and one slice of kSharedSlice ranks, and each lane walks its own row.
+struct SharedRow {
+    float4 rt;
+    double acc, one_m_sump;
+    float resp;
+    PairConst pc;
+    FeasRow fr;
+    RowInv inv;
+    int t, rep, lo, end;
+    bool is_inv;
+};
+constexpr int kSharedThreads = 64, kSharedSlice = 32;
+template <int G>
+__global__ void __launch_bounds__(kSharedThreads) grid_shared(GridArgs g) {
+    __shared__ SharedRow rows[kSharedThreads / 32][32];
+    const DevFleet& f = g.f;
+    const int R = g.R, B = g.B;
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5, grp = lane / G, sub = lane % G;
+    const unsigned gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (grp * G);
+    const unsigned wg = blockIdx.x * (kSharedThreads / 32) + warp, n_warps = gridDim.x * (kSharedThreads / 32);
+    size_t my_row;
+    int r_beg = 0, r_end = B;
+    if (G == 32) {
+        my_row = (size_t)lane * n_warps + wg;
+    } else {
+        const unsigned n_slices = (unsigned)(B + kSharedSlice - 1) / kSharedSlice;
+        my_row = (size_t)(wg / n_slices) * 32 + lane;
+        r_beg = (int)(wg % n_slices) * kSharedSlice;
+        r_end = min(B, r_beg + kSharedSlice);
+    }
+    bool todo = false;
+    if (my_row < (size_t)f.S * f.A * R) {
+        const size_t row = my_row;
+        const int jl = g.row_j[row];  // a shared chain implies a table and a positive rate (grid_rows)
+        SharedRow& x = rows[warp][lane];
+        x.lo = 0;
+        x.end = g.want_cells ? r_end : min(B, g.best_rank[row]);
+        if (jl != INT_MAX) {
+            int hi = x.end;  // first shared rank: the first rank whose batch size is >= jl + 2
+            while (x.lo < hi) {
+                const int mid = (x.lo + hi) >> 1;
+                if (g.batch[g.rank_to_bi[mid]] < jl + 2) x.lo = mid + 1; else hi = mid;
+            }
+            x.lo = max(x.lo, r_beg);
+            todo = x.lo < x.end;
+        }
+        if (todo) {
+            const unsigned sa = (unsigned)(row / R);
+            const int ri = (int)(row - (size_t)sa * R), s = (int)(sa / f.A);
+            x.t = g.pair_tab_idx[sa];
+            x.rt = g.rt[s * R + ri];
+            x.rep = g.replicas[ri];
+            x.acc = g.row_acc[row];
+            x.one_m_sump = __dsub_rn(1.0, g.row_sump[row]);
+            x.resp = row_resp_time(x.acc, x.rt.y);
+            x.pc = pair_const(qparams_of(f, s, (int)(sa - (unsigned)s * f.A)));
+            x.fr = feas_row(f, s, 0.0f);
+            x.is_inv = row_invariant(x.pc, x.acc, x.one_m_sump, x.resp, x.rt.y, g.Bmax, x.inv);
+        }
+    }
+    __syncwarp();
+    for (unsigned left = __ballot_sync(0xffffffffu, todo); left;) {
+        const unsigned own = __fns(left, 0, (int)grp + 1);  // this group's row (>= 32: none left for it)
+        for (int k = 0; k < 32 / G && left; ++k) left &= left - 1;
+        bool active = own < 32;
+        SharedRow x = rows[warp][active ? own : 0];
+        const size_t row = __shfl_sync(0xffffffffu, my_row, active ? own : 0);
+        const unsigned sa = (unsigned)(row / R);
+        const int ri = (int)(row - (size_t)sa * R);
+        bool found = false;  // this row's best_rank has been lowered
+        for (int r0 = x.lo; __any_sync(0xffffffffu, active); r0 += G) {
+            const int r = r0 + (int)sub;
+            bool feas = false, past = false;
+            if (active && r < x.end) {
+                const int bi = g.rank_to_bi[r];
+                const int b = g.batch[bi];
+                const int K = b + b * f.ratio;
+                if (K >= (1 << 23)) {
+                    past = true;
+                } else {
+                    const float4 pb = g.pb[(size_t)x.t * B + bi];
+                    if (!(x.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
+                        // the whole solve is shared with the row: only the N-dependent tail is per cell
+                        const Metrics m = x.is_inv ? shared_cell_metrics_inv(x.pc, x.inv, x.rt.y, b, g.want_cells != 0)
+                                                   : shared_cell_metrics(x.pc, x.acc, x.one_m_sump, x.resp, x.rt.y, b);
+                        if (x.fr.tps) x.fr.lim = feas_lim(pb.x);
+                        feas = cell_feasible(x.fr, x.rep, x.rt.y, m);
+                        if (g.want_cells) store_cell(g, ((long long)sa * B + bi) * R + ri, 1, feas ? 1 : 0, m);
+                    }
+                }
+            }
+            const unsigned fm = __ballot_sync(0xffffffffu, feas) & gmask;
+            const bool stop = (__ballot_sync(0xffffffffu, past) & gmask) != 0;
+            if (fm && !found && lane == (unsigned)(__ffs(fm) - 1)) atomicMin(&g.best_rank[row], r);
+            found = found || fm != 0;
+            if (stop || r0 + G >= x.end || (found && !g.want_cells)) active = false;
+        }
+    }
+}
+
 // K3: per-server argmin.  One CTA per server: one candidate per (accelerator, replica
 // level) = its smallest feasible batch size; warp-shuffle reduction, cross-warp reduction
 // staged through shared memory.  The order (value, cost, replicas, batch, accelerator) does not involve the
 // latency metrics, so only the keys are reduced; the winner's itl / ttft / rho are fetched once at the end:
 // from the cell columns, or — for a cell that shares its row's chain and was not stored (want_cells == 0) —
-// by the same stats_from_row + metrics_from evaluation grid_sort_local ran for it.
+// by the same stats_from_row + metrics_from evaluation grid_shared ran for it.
 struct GridKey {
     float value, cost;
     int replicas, batch, acc, bi, ri, feasible;  // bi < 0: zero-load allocation of accelerator ri
@@ -1254,7 +1310,7 @@ __global__ void __launch_bounds__(256) grid_finalize(GridArgs g, AllocCols winne
                 const int jl = g.row_j[row];
                 const int K = b + b * f.ratio;
                 if (!g.want_cells && jl != INT_MAX && b >= jl + 2 && K < (1 << 23)) {
-                    // the cell shares its row's chain and was not stored: grid_sort_local's evaluation again
+                    // the cell shares its row's chain and was not stored: grid_shared's evaluation again
                     const float lambda = g.rt[s * g.R + ri].y;
                     ModelStats st;
                     stats_from_row(g.row_acc[row], g.row_sump[row], b, lambda, st);
