@@ -810,12 +810,18 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     const size_t n_pairs_alloc = std::max<size_t>((size_t)S * A, 1);
     Cols rows(256);
     const size_t o_rows = rows.take((2 * sizeof(double) + sizeof(int)) * n_best + 64),  // row_acc | row_sump | row_j
-        o_pair_rec = rows.take(48 * n_pairs_alloc);
+        o_pair_rec = rows.take(48 * n_pairs_alloc), o_grp = rows.take(sizeof(unsigned) * n_best),
+                 o_bound = rows.take(sizeof(unsigned long long) * std::max(S, 1));
     CK(h->d_rows.ensure(rows.bytes));
     g.row_acc = (double*)((char*)h->d_rows.p + o_rows);
     g.row_sump = g.row_acc + n_best;
     g.row_j = (int*)(g.row_sump + n_best);
     g.pair_rec = (float4*)((char*)h->d_rows.p + o_pair_rec);
+    g.row_grp = (unsigned*)((char*)h->d_rows.p + o_grp);
+    g.bound = (unsigned long long*)((char*)h->d_rows.p + o_bound);
+    // grid_order ranks a server's rows in shared memory, and a cell's key holds the accelerator in 8 bits and the batch
+    // size in 24; outside those limits every cell is evaluated (grid_order still walks the shared runs)
+    g.prune = A <= 256 && Bmax < (1 << 24) && (long long)A * R <= kOrderMaxRows;
     g.Bmax = h->grid_Bmax;
     g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
     g.fb_cap = (int)std::min<size_t>(nc, (size_t)1 << 22);
@@ -860,6 +866,13 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
             grid_rows<<<(unsigned)(hf.S * hf.A), rows_threads, rows_smem, h->stream>>>(g);
         }
         h->launches++;
+        if (g.want_cells) {
+            g.prune = 0;  // every cell is evaluated and stored
+        } else {
+            // the shared-chain cells and each server's bound, before grid_sort_local skips the cells above it
+            grid_order<<<(unsigned)hf.S, kOrderThreads, 0, h->stream>>>(g);
+            h->launches++;
+        }
         grid_sort_local<<<plan.n_blocks, kSortThreads, 0, h->stream>>>(g);
         grid_items_scatter<<<(unsigned)(16 * h->sm_count), 256, 0, h->stream>>>(g);  // warp per item (grid-stride)
         h->launches++;
@@ -872,13 +885,13 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
     if (plan.n_cells > 0) {
         grid_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
                                                                (int*)h->d_ctrl.p + CTRL_FB_STATUS);
-        // the shared-chain cells: 32 rows per warp; with a cell table, one warp per 32 rows and slice of ranks
-        const size_t n_warps = ((size_t)hf.S * hf.A * g.R + 31) / 32 *
-                               (g.want_cells ? (size_t)(g.B + kSharedSlice - 1) / kSharedSlice : 1);
-        const unsigned ctas = (unsigned)((n_warps + kSharedThreads / 32 - 1) / (kSharedThreads / 32));
-        if (g.want_cells) grid_shared<1><<<ctas, kSharedThreads, 0, h->stream>>>(g);
-        else grid_shared<32><<<ctas, kSharedThreads, 0, h->stream>>>(g);
-        h->launches += 2;  // grid_fallback, grid_shared
+        h->launches++;
+        if (g.want_cells) {  // the shared-chain cells with a cell table: one warp per 32 rows and slice of ranks
+            const size_t n_warps = ((size_t)hf.S * hf.A * g.R + 31) / 32 * ((size_t)(g.B + kSharedSlice - 1) / kSharedSlice);
+            const unsigned ctas = (unsigned)((n_warps + kSharedThreads / 32 - 1) / (kSharedThreads / 32));
+            grid_shared<<<ctas, kSharedThreads, 0, h->stream>>>(g);
+            h->launches++;
+        }
     }
     if (hf.S > 0) {
         grid_finalize<<<hf.S, 256, 0, h->stream>>>(g, winners);

@@ -317,18 +317,22 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 //
 //   grid_rows        per (pair, replica level): the chain every large-enough batch size shares
 //                    (solve_row); also the (server, replica) rate block and the batch-rank reset
+//   grid_order       without a cell table, per server: the rows' order under grid_finalize's key, the cells
+//                    that share their row's chain up to the row's first feasible one, and the server's bound
+//                    (the smallest key of a feasible cell found)
 //   grid_sort_local  per chunk of 8192 cells: gates + Analyze's rate checks; cells that share their
-//                    row's chain are left to grid_shared; the others get a log-domain length estimate,
-//                    an 8-bit class and a local counting sort -> warp items; the last CTA plans
-//                    grid_kernel's queues (grid_items_plan)
+//                    row's chain are left to grid_order / grid_shared, and without a cell table cells
+//                    that cannot be feasible or lie above the bound are dropped; the others get a
+//                    log-domain length estimate, an 8-bit class and a local counting sort -> warp items;
+//                    the last CTA plans grid_kernel's queues (grid_items_plan)
 //   grid_items_scatter  items ordered globally, longest class first
 //   grid_kernel      persistent CTA per SM; warps pull items (32 cells of nearly equal chain length)
 //                    from a long and a short queue: streaming solve, metrics, SLO feasibility,
 //                    per-cell columns, atomicMin of the smallest feasible batch rank per
-//                    (server, accelerator, replica)
+//                    (server, accelerator, replica) and of the server's bound; an item whose cells
+//                    are all above the bound by then is skipped
 //   grid_fallback   stored-vector re-run of the rare cells the streaming solve bails on
-//   grid_shared     per (pair, replica level): the cells that share the row's chain, in ascending batch
-//                   order up to the row's first feasible one (all of them when the cell table is stored)
+//   grid_shared     with a cell table, per (pair, replica level): every cell that shares the row's chain
 //   grid_finalize   per-server argmin (warp shuffle -> shared memory -> winner record)
 //
 // For a fixed (server, accelerator, replica level) the transition penalty and the cost do
@@ -373,7 +377,11 @@ struct GridArgs {
     uint4* recs;             // [items][32] per sorted cell: {cell, lambda bits, table entry offset, batch size | class << 23 | pad << 31}
     int want_cells;          // 0: the caller did not ask for the cell table -> cells that share their row's chain store
                              // nothing and are evaluated only up to the row's first feasible one (grid_finalize
-                             // recomputes the few winners among them); 1: every cell is stored
+                             // recomputes the few winners among them), and cells that cannot be a server's winner
+                             // are skipped (grid_order); 1: every cell is evaluated and stored
+    int prune;               // grid_order ranks the rows (A <= 256, Bmax < 2^24, A*R <= kOrderMaxRows; want_cells == 0)
+    unsigned* row_grp;       // [S*A*R] group rank of the row: rows of the server strictly below it in (value, cost, replicas)
+    unsigned long long* bound;  // [S] smallest key of a feasible cell found so far (kBoundOff: no pruning)
     int* fb_count;           // cells that need the stored-vector fallback
     long long* fb_cells;
     int fb_cap;
@@ -385,6 +393,15 @@ struct GridArgs {
     unsigned* dbg_cycles;    // diagnostics: per order index, SM cycles spent in grid_kernel (or NULL)
     size_t dbg_n;            // cells; dbg_cycles[dbg_n + idx] holds the warp timeline (start ns, SM, end ns)
 };
+
+// A cell's place in grid_finalize's order (value, cost, replicas, batch, accelerator) among the cells of its server:
+// the row's group rank, then the batch SIZE (repeated sizes stay tied), then the accelerator.  A cell whose key is
+// strictly above the key of some feasible cell of the same server cannot be the server's winner.
+constexpr unsigned long long kBoundOff = ~0ull;       // the server is not pruned (no order, or a NaN value / cost)
+constexpr unsigned long long kBoundNone = ~0ull - 1;  // no feasible cell found yet (above every key)
+__device__ __forceinline__ unsigned long long cell_key(unsigned grp, int b, int a) {
+    return ((unsigned long long)grp << 32) | ((unsigned long long)(unsigned)b << 8) | (unsigned)a;
+}
 
 __device__ __forceinline__ void decode_cell(const GridArgs& g, long long cell, int& s, int& a, int& bi, int& ri) {
     unsigned t = (unsigned)cell;  // n_cells < 2^32 (checked on the host): 32-bit divisions
@@ -638,6 +655,172 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
     }
 }
 
+// Without a cell table, between grid_rows and grid_sort_local: one CTA per server.
+//  1. Group ranks (g.prune): every (accelerator, replica level) row gets the number of rows of the server strictly
+//     below it in (value, cost, replicas), with value and cost computed as grid_finalize computes them.  A counting
+//     rank, Q threads per row.  It keeps key_better's order, ties included (-0 == +0); rows without a table take part
+//     with a fixed key, which does not change the order of the others.  A NaN value or cost would make the order
+//     depend on the reduction, so it turns pruning off for the server (bound = kBoundOff).
+//  2. The shared runs (b >= jl + 2, K < 2^23): each row is walked from its first shared rank up to its first feasible
+//     cell, which lowers best_rank; the smallest key among those cells is the server's bound.  Rows are taken in group
+//     order, kOrderG lanes per row, and a row's walk also stops at the first cell whose key is above the bound so far
+//     (keys grow along a row), so once a group has a feasible shared cell the rows of later groups stop at once.
+//     A walk step is a chain of dependent loads, and a row without a feasible shared cell walks its whole run, so
+//     the batch sizes in rank order and the pairs' RateRange.Max per rank are staged in shared memory first (in the
+//     space the ranking used).
+//
+// No pass over the shared cells is needed after grid_kernel.  Every cell that is never evaluated — a shared cell
+// after the stop of its row's walk, or a non-shared cell that grid_sort_local or grid_kernel skips — either cannot be
+// feasible (the exact gates of grid_sort_local) or has a key strictly above a feasible cell of its server.  So the
+// winner W (the smallest key among the feasible cells) is evaluated, and so is every feasible cell of W's row below W,
+// which has a smaller or equal key: best_rank of W's row is W's rank.  Any other best_rank is a feasible cell, whose
+// key is >= W's.  grid_finalize picks W exactly as when every cell is evaluated.
+constexpr int kOrderThreads = 1024, kOrderG = 4, kOrderMaxRows = 2048;
+__global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
+    __shared__ float s_vc[2 * kOrderMaxRows];  // ranking: values | costs; walk: RateRange.Max per (accelerator, rank)
+    __shared__ int s_rep[kOrderMaxRows];        // ranking: replicas; walk: batch size per rank
+    float* s_val = s_vc;
+    float* s_cost = s_vc + kOrderMaxRows;
+    __shared__ unsigned s_grp[kOrderMaxRows];
+    __shared__ unsigned short s_at[kOrderMaxRows];  // the row at each position of the group order
+    __shared__ unsigned long long s_bound;
+    const DevFleet& f = g.f;
+    const int s = blockIdx.x, A = f.A, R = g.R, B = g.B, n = A * R;
+    const size_t row0 = (size_t)s * n;
+    const unsigned tid = threadIdx.x, lane = tid & 31;
+    if (tid == 0) s_bound = kBoundNone;
+    int nan = 0;
+    if (g.prune) {
+        for (int k = tid; k < n; k += blockDim.x) {
+            const int a = k / R, ri = k - a * R;
+            float v = INFINITY, c = INFINITY;
+            int r = INT_MAX;
+            if (g.pair_tab_off[s * A + a] >= 0) {  // grid_finalize: cost, then value = penalty_of
+                Cand x = cand_nil();
+                x.acc = a;
+                x.replicas = r = g.replicas[ri];
+                x.cost = c = __fmul_rn(f.acc_cost[a], (float)((long long)num_instances(f, f.srv_model[s], a) * (long long)r));
+                v = penalty_of(f, s, x);
+                nan |= v != v || c != c;
+            }
+            s_val[k] = v;
+            s_cost[k] = c;
+            s_rep[k] = r;
+        }
+    }
+    const bool prune = g.prune && !__syncthreads_or(nan);
+    if (prune) {
+        int q = 1;  // threads per row: a power of two <= 32, so that they are lanes of one warp
+        while (q < 32 && 2 * q * n <= (int)blockDim.x) q *= 2;
+        const int per = (int)blockDim.x / q;
+        for (int base = 0; base < n; base += per) {
+            const int i = base + (int)tid / q;
+            unsigned lt = 0, eq = 0;  // rows strictly below row i; equal rows before it (its place among its ties)
+            if (i < n) {
+                const float vi = s_val[i], ci = s_cost[i];
+                const int ri = s_rep[i];
+                for (int j = (int)tid % q; j < n; j += q) {
+                    const float vj = s_val[j], cj = s_cost[j];
+                    const int rj = s_rep[j];
+                    lt += vj < vi || (vj == vi && (cj < ci || (cj == ci && rj < ri)));
+                    eq += vj == vi && cj == ci && rj == ri && j < i;
+                }
+            }
+            for (int d = 1; d < q; d <<= 1) {
+                lt += __shfl_xor_sync(0xffffffffu, lt, d);
+                eq += __shfl_xor_sync(0xffffffffu, eq, d);
+            }
+            if (i < n && (int)tid % q == 0) {
+                s_grp[i] = lt;
+                s_at[lt + eq] = (unsigned short)i;
+                g.row_grp[row0 + i] = lt;
+            }
+        }
+    } else if (g.prune) {
+        for (int k = tid; k < n; k += blockDim.x) g.row_grp[row0 + k] = 0;
+    }
+    __syncthreads();
+    const bool stage_b = B <= kOrderMaxRows, stage_rmax = A * B <= 2 * kOrderMaxRows;
+    if (stage_b)
+        for (int r = tid; r < B; r += blockDim.x) s_rep[r] = g.batch[g.rank_to_bi[r]];
+    if (stage_rmax)
+        for (int k = tid; k < A * B; k += blockDim.x) {
+            const int a = k / B, r = k - a * B;
+            const long long toff = g.pair_tab_off[s * A + a];
+            s_vc[k] = toff >= 0 ? g.pb[(size_t)g.pair_tab_idx[s * A + a] * B + g.rank_to_bi[r]].x : 0.0f;
+        }
+    __syncthreads();
+    auto batch_at = [&](int r) { return stage_b ? s_rep[r] : g.batch[g.rank_to_bi[r]]; };
+    const unsigned sub = lane % kOrderG, gmask = ((1u << kOrderG) - 1u) << (lane - sub);
+    for (int base = 0; base < n; base += (int)blockDim.x / kOrderG) {
+        const int p = base + (int)tid / kOrderG;
+        const int k = p < n ? (prune ? s_at[p] : p) : 0;
+        const int a = k / R, ri = k - a * R;
+        const size_t row = row0 + k;
+        const unsigned grp = prune ? s_grp[k] : 0u;
+        const int jl = p < n ? g.row_j[row] : INT_MAX;  // a shared chain implies a table and a positive rate (grid_rows)
+        int lo = 0;
+        bool active = false;
+        float4 rt;
+        double acc, one_m_sump;
+        float resp;
+        PairConst pc;
+        FeasRow fr;
+        RowInv inv;
+        int t, rep;
+        bool is_inv;
+        if (jl != INT_MAX) {
+            int hi = B;  // first shared rank: the first rank whose batch size is >= jl + 2
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (batch_at(mid) < jl + 2) lo = mid + 1; else hi = mid;
+            }
+            active = lo < B;
+        }
+        if (active) {
+            t = g.pair_tab_idx[s * A + a];
+            rt = g.rt[s * R + ri];
+            rep = g.replicas[ri];
+            acc = g.row_acc[row];
+            one_m_sump = __dsub_rn(1.0, g.row_sump[row]);
+            resp = row_resp_time(acc, rt.y);
+            pc = pair_const(qparams_of(f, s, a));
+            fr = feas_row(f, s, 0.0f);
+            is_inv = row_invariant(pc, acc, one_m_sump, resp, rt.y, g.Bmax, inv);
+        }
+        for (int r0 = lo; __any_sync(0xffffffffu, active); r0 += kOrderG) {
+            const int r = r0 + (int)sub;
+            bool feas = false, stop = false;
+            unsigned long long key = 0;
+            if (active && r < B) {
+                const int b = batch_at(r);
+                const int K = b + b * f.ratio;
+                key = cell_key(grp, b, a);
+                if (K >= (1 << 23) || (prune && key > *(volatile unsigned long long*)&s_bound)) {
+                    stop = true;  // grid_kernel's cells from here on, or no cell from here on can win
+                } else {
+                    const float rmax = stage_rmax ? s_vc[a * B + r] : g.pb[(size_t)t * B + g.rank_to_bi[r]].x;
+                    if (!(rt.x > rmax) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
+                        const Metrics m = is_inv ? shared_cell_metrics_inv(pc, inv, rt.y, b, false)
+                                                 : shared_cell_metrics(pc, acc, one_m_sump, resp, rt.y, b);
+                        if (fr.tps) fr.lim = feas_lim(rmax);
+                        feas = cell_feasible(fr, rep, rt.y, m);
+                    }
+                }
+            }
+            const unsigned fm = __ballot_sync(0xffffffffu, feas) & gmask;
+            const bool stopped = (__ballot_sync(0xffffffffu, stop) & gmask) != 0;
+            if (fm && lane == (unsigned)(__ffs(fm) - 1)) {
+                atomicMin(&g.best_rank[row], r);
+                if (prune) atomicMin(&s_bound, key);
+            }
+            if (fm || stopped || r0 + kOrderG >= B) active = false;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) g.bound[s] = prune ? s_bound : kBoundOff;
+}
+
 // Counter increment for lanes whose equal keys sit in CONTIGUOUS lane ranges (along a row the
 // length class is monotone in the replica level, so equal classes are adjacent): one atomic per
 // run instead of one per lane, found with a shuffle and a ballot.  Returns the lane's slot.
@@ -686,6 +869,7 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
         struct LaneRow {
             float4 rt;
             int jl;
+            unsigned grp;
         };
         unsigned cur_sa = 0xffffffffu;
         LaneRow c0{}, c1{};
@@ -693,10 +877,16 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
         int bi = (int)(row0 + warp - sa * B);
         int s = 0, t = 0;
         long long toff = -1;
+        // without a cell table, cells that cannot be feasible or cannot be the server's winner are not evaluated:
+        // TPS servers above the stability limit, ITL = alpha + beta * eff >= alpha > slo_itl (eff >= 0, beta >= 0),
+        // and keys above the server's bound from grid_order
+        unsigned long long bound = kBoundOff;
+        bool tps = false, itl_out = false;
         auto load_lane = [&](unsigned ri, LaneRow& c) {
             if (ri >= R || toff < 0) return;
             c.rt = g.rt[(unsigned)s * R + ri];
             c.jl = g.row_j[(size_t)sa * R + ri];
+            if (g.prune) c.grp = g.row_grp[(size_t)sa * R + ri];
         };
         for (unsigned row = row0 + warp; row <= row1; row += kSortThreads / 32, bi += kSortThreads / 32) {
             while (bi >= (int)B) {
@@ -708,6 +898,13 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
                 s = (int)(sa / A);
                 toff = g.pair_tab_off[sa];
                 if (toff >= 0) t = g.pair_tab_idx[sa];
+                if (toff >= 0 && !g.want_cells) {  // a table implies a valid model index (pair_class == PAIR_LOAD)
+                    const int k = f.srv_model[s] * (int)A + (int)(sa - (unsigned)s * A);
+                    const float slo_itl = f.srv_slo_itl[s];
+                    bound = g.bound[s];
+                    tps = f.srv_slo_tps[s] > 0.0f;
+                    itl_out = slo_itl != 0.0f && f.perf_beta[k] >= 0.0f && f.perf_alpha[k] > slo_itl;
+                }
                 load_lane(lane, c0);
                 load_lane(lane + 32, c1);
             }
@@ -721,8 +918,12 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
                 if (cell < base || cell >= base + n_here) return;
                 int key = 255;
                 if (toff >= 0 && !(c.rt.x <= 0.0f) && !(c.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
-                    // a cell that shares its row's chain stays at class 255: grid_shared evaluates it after grid_kernel
-                    if (!(c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23)))
+                    // a cell that shares its row's chain stays at class 255: grid_order (without a cell table) or
+                    // grid_shared (with one) evaluates it
+                    const bool shared = c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23);
+                    const bool skip = itl_out || (tps && !(c.rt.y <= feas_lim(pb.x))) ||
+                                      (bound != kBoundOff && cell_key(c.grp, b, (int)(sa - (unsigned)s * A)) > bound);
+                    if (!shared && !skip)
                         key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, c.rt.y, c.rt.z, pb.w, pb.y, pb.z));
                 }
                 keys[cell - base] = (uint8_t)key;
@@ -966,6 +1167,15 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
     const bool valid = (rec.w >> 31) == 0;
     const int K = N + N * f.ratio;
     const unsigned pair = cell / ((unsigned)g.B * (unsigned)g.R);
+    if (g.prune) {
+        // the bound may have dropped since grid_sort_local (feasible cells found by earlier items): an item none of
+        // whose cells can still be its server's winner is not solved
+        const unsigned s = pair / (unsigned)f.A;
+        const unsigned long long bound = __ldcg(g.bound + s);
+        const unsigned grp = g.row_grp[(size_t)pair * g.R + cell % (unsigned)g.R];
+        const bool live = valid && cell_key(grp, N, (int)(pair - s * (unsigned)f.A)) <= bound;
+        if (!__any_sync(0xffffffffu, live)) return;
+    }
     // one pair per item is the rule (an item is cut from one sort chunk); then lanes 0..2 fetch its record
     const bool one_pair = __all_sync(0xffffffffu, pair == __shfl_sync(0xffffffffu, pair, 0));
     __syncwarp();  // the previous item's readers of pair_buf are done
@@ -999,7 +1209,11 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
             const Metrics m = metrics_from(q, N, st);
             const bool feas = cell_feasible(fr, g.replicas[ri], lambda, m);
             store_cell(g, (long long)cell, 1, feas ? 1 : 0, m);
-            if (feas) atomicMin(&g.best_rank[(size_t)pair * g.R + ri], g.batch_rank[bi]);
+            if (feas) {
+                atomicMin(&g.best_rank[(size_t)pair * g.R + ri], g.batch_rank[bi]);
+                if (g.prune && __ldcg(g.bound + s) != kBoundOff)
+                    atomicMin(g.bound + s, cell_key(g.row_grp[(size_t)pair * g.R + ri], N, a));
+            }
             if (g.dbg_cycles) {
                 g.dbg_cycles[idx] = (unsigned)(clock64() - t_start);
                 if (lane < 3) {  // timeline: [0] start ns, [1] SM id, [2] end ns (low 32 bits of %globaltimer)
@@ -1093,18 +1307,13 @@ __global__ void grid_fallback(GridArgs g, double* scratch, size_t slot_doubles, 
     }
 }
 
-// The cells that share their row's chain (analysable, b >= jl + 2, K < 2^23), after grid_kernel and grid_fallback.
-// Ranks ascend in batch size, so a row's shared cells are one run of ranks; its cells with K >= 2^23 (grid_kernel's)
-// follow that run and end it.  Without a cell table only the row's smallest feasible rank counts: a row whose
-// best_rank already lies below its first shared rank is decided, and otherwise its walk up the ranks stops at the
-// first feasible shared cell or at best_rank, whichever comes first.  With a cell table every shared cell is
-// evaluated and stored.
+// With a cell table, the cells that share their row's chain (analysable, b >= jl + 2, K < 2^23), after grid_kernel
+// and grid_fallback: every one is evaluated and stored.  Ranks ascend in batch size, so a row's shared cells are one
+// run of ranks; its cells with K >= 2^23 (grid_kernel's) follow that run and end it.  (Without a cell table grid_order
+// walks the shared runs before grid_kernel, up to each row's first feasible cell.)
 //
-// A warp owns 32 rows (a lane each) and finds which of them need a walk and between which ranks; the rows to walk
-// are then taken 32 / G at a time, G lanes per row and G ranks per step.  Without a cell table (G = 32) most rows are
-// decided, so a warp's rows are spread over the grid (the undecided ones cluster by pair) and each of the few
-// others gets the whole warp.  With a cell table (G = 1) every shared cell is work: a warp owns 32 consecutive
-// replica levels (coalesced stores) and one slice of kSharedSlice ranks, and each lane walks its own row.
+// A warp owns 32 consecutive replica levels (coalesced stores) and one slice of kSharedSlice ranks; it finds which
+// of its rows have shared cells in the slice, and each lane then walks one of those rows.
 struct SharedRow {
     float4 rt;
     double acc, one_m_sump;
@@ -1116,31 +1325,22 @@ struct SharedRow {
     bool is_inv;
 };
 constexpr int kSharedThreads = 64, kSharedSlice = 32;
-template <int G>
 __global__ void __launch_bounds__(kSharedThreads) grid_shared(GridArgs g) {
     __shared__ SharedRow rows[kSharedThreads / 32][32];
     const DevFleet& f = g.f;
     const int R = g.R, B = g.B;
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5, grp = lane / G, sub = lane % G;
-    const unsigned gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (grp * G);
-    const unsigned wg = blockIdx.x * (kSharedThreads / 32) + warp, n_warps = gridDim.x * (kSharedThreads / 32);
-    size_t my_row;
-    int r_beg = 0, r_end = B;
-    if (G == 32) {
-        my_row = (size_t)lane * n_warps + wg;
-    } else {
-        const unsigned n_slices = (unsigned)(B + kSharedSlice - 1) / kSharedSlice;
-        my_row = (size_t)(wg / n_slices) * 32 + lane;
-        r_beg = (int)(wg % n_slices) * kSharedSlice;
-        r_end = min(B, r_beg + kSharedSlice);
-    }
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned wg = blockIdx.x * (kSharedThreads / 32) + warp;
+    const unsigned n_slices = (unsigned)(B + kSharedSlice - 1) / kSharedSlice;
+    const size_t my_row = (size_t)(wg / n_slices) * 32 + lane;
+    const int r_beg = (int)(wg % n_slices) * kSharedSlice, r_end = min(B, r_beg + kSharedSlice);
     bool todo = false;
     if (my_row < (size_t)f.S * f.A * R) {
         const size_t row = my_row;
         const int jl = g.row_j[row];  // a shared chain implies a table and a positive rate (grid_rows)
         SharedRow& x = rows[warp][lane];
         x.lo = 0;
-        x.end = g.want_cells ? r_end : min(B, g.best_rank[row]);
+        x.end = r_end;
         if (jl != INT_MAX) {
             int hi = x.end;  // first shared rank: the first rank whose batch size is >= jl + 2
             while (x.lo < hi) {
@@ -1165,42 +1365,30 @@ __global__ void __launch_bounds__(kSharedThreads) grid_shared(GridArgs g) {
         }
     }
     __syncwarp();
-    for (unsigned left = __ballot_sync(0xffffffffu, todo); left;) {
-        const unsigned own = __fns(left, 0, (int)grp + 1);  // this group's row (>= 32: none left for it)
-        for (int k = 0; k < 32 / G && left; ++k) left &= left - 1;
-        bool active = own < 32;
-        SharedRow x = rows[warp][active ? own : 0];
-        const size_t row = __shfl_sync(0xffffffffu, my_row, active ? own : 0);
-        const unsigned sa = (unsigned)(row / R);
-        const int ri = (int)(row - (size_t)sa * R);
-        bool found = false;  // this row's best_rank has been lowered
-        for (int r0 = x.lo; __any_sync(0xffffffffu, active); r0 += G) {
-            const int r = r0 + (int)sub;
-            bool feas = false, past = false;
-            if (active && r < x.end) {
-                const int bi = g.rank_to_bi[r];
-                const int b = g.batch[bi];
-                const int K = b + b * f.ratio;
-                if (K >= (1 << 23)) {
-                    past = true;
-                } else {
-                    const float4 pb = g.pb[(size_t)x.t * B + bi];
-                    if (!(x.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
-                        // the whole solve is shared with the row: only the N-dependent tail is per cell
-                        const Metrics m = x.is_inv ? shared_cell_metrics_inv(x.pc, x.inv, x.rt.y, b, g.want_cells != 0)
-                                                   : shared_cell_metrics(x.pc, x.acc, x.one_m_sump, x.resp, x.rt.y, b);
-                        if (x.fr.tps) x.fr.lim = feas_lim(pb.x);
-                        feas = cell_feasible(x.fr, x.rep, x.rt.y, m);
-                        if (g.want_cells) store_cell(g, ((long long)sa * B + bi) * R + ri, 1, feas ? 1 : 0, m);
-                    }
-                }
-            }
-            const unsigned fm = __ballot_sync(0xffffffffu, feas) & gmask;
-            const bool stop = (__ballot_sync(0xffffffffu, past) & gmask) != 0;
-            if (fm && !found && lane == (unsigned)(__ffs(fm) - 1)) atomicMin(&g.best_rank[row], r);
-            found = found || fm != 0;
-            if (stop || r0 + G >= x.end || (found && !g.want_cells)) active = false;
+    const unsigned own = __fns(__ballot_sync(0xffffffffu, todo), 0, (int)lane + 1);  // this lane's row (>= 32: none)
+    bool active = own < 32;
+    SharedRow x = rows[warp][active ? own : 0];
+    const size_t row = __shfl_sync(0xffffffffu, my_row, active ? own : 0);
+    const unsigned sa = (unsigned)(row / R);
+    const int ri = (int)(row - (size_t)sa * R);
+    bool found = false;  // this row's best_rank has been lowered
+    for (int r = x.lo; active; ++r) {
+        const int bi = g.rank_to_bi[r];
+        const int b = g.batch[bi];
+        const int K = b + b * f.ratio;
+        if (K >= (1 << 23)) break;
+        const float4 pb = g.pb[(size_t)x.t * B + bi];
+        if (!(x.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
+            // the whole solve is shared with the row: only the N-dependent tail is per cell
+            const Metrics m = x.is_inv ? shared_cell_metrics_inv(x.pc, x.inv, x.rt.y, b, true)
+                                       : shared_cell_metrics(x.pc, x.acc, x.one_m_sump, x.resp, x.rt.y, b);
+            if (x.fr.tps) x.fr.lim = feas_lim(pb.x);
+            const bool feas = cell_feasible(x.fr, x.rep, x.rt.y, m);
+            store_cell(g, ((long long)sa * B + bi) * R + ri, 1, feas ? 1 : 0, m);
+            if (feas && !found) atomicMin(&g.best_rank[row], r);
+            found = found || feas;
         }
+        if (r + 1 >= x.end) active = false;
     }
 }
 
@@ -1209,7 +1397,7 @@ __global__ void __launch_bounds__(kSharedThreads) grid_shared(GridArgs g) {
 // staged through shared memory.  The order (value, cost, replicas, batch, accelerator) does not involve the
 // latency metrics, so only the keys are reduced; the winner's itl / ttft / rho are fetched once at the end:
 // from the cell columns, or — for a cell that shares its row's chain and was not stored (want_cells == 0) —
-// by the same stats_from_row + metrics_from evaluation grid_shared ran for it.
+// by the same stats_from_row + metrics_from evaluation grid_order ran for it.
 struct GridKey {
     float value, cost;
     int replicas, batch, acc, bi, ri, feasible;  // bi < 0: zero-load allocation of accelerator ri
@@ -1310,7 +1498,7 @@ __global__ void __launch_bounds__(256) grid_finalize(GridArgs g, AllocCols winne
                 const int jl = g.row_j[row];
                 const int K = b + b * f.ratio;
                 if (!g.want_cells && jl != INT_MAX && b >= jl + 2 && K < (1 << 23)) {
-                    // the cell shares its row's chain and was not stored: grid_shared's evaluation again
+                    // the cell shares its row's chain and was not stored: grid_order's evaluation again
                     const float lambda = g.rt[s * g.R + ri].y;
                     ModelStats st;
                     stats_from_row(g.row_acc[row], g.row_sump[row], b, lambda, st);
