@@ -412,22 +412,6 @@ int size_depth_for(int n) {
 }
 int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     const int D = size_depth_for(n);
-    int size_rev = 1;  // solver returns to the block vote after a per-step excursion (0 = stays on the per-step path)
-    if (const char* e = getenv("WVA_SIZE_REV")) size_rev = atoi(e);
-    // blocks of sz2_solve per SM (register limit: 4).  Fewer co-resident warps = a larger share of the sub-partition's
-    // FP64 pipe for each, i.e. a shorter critical path for the rounds that are as long as their longest chains;
-    // unused dynamic shared memory is what limits the residency.
-    int solve_bpsm = 4;
-    if (const char* e = getenv("WVA_SIZE_BLOCKS_PER_SM")) solve_bpsm = std::min(std::max(atoi(e), 1), 4);
-    size_t solve_pad = 0;
-    if (solve_bpsm < 4) {
-        solve_pad = (size_t)(227 * 1024) / (size_t)solve_bpsm - 2048;
-        solve_pad = solve_pad / 1024 * 1024;
-        CK(cudaFuncSetAttribute(sz2_solve<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_pad));
-        CK(cudaFuncSetAttribute(sz2_solve<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_pad));
-    }
-    int dbg_round = -1;  // diagnostics: record per-request SM cycles of this round's sz2_solve (wva_dbg_read_size)
-    if (const char* e = getenv("WVA_SIZE_DBG_ROUND")) dbg_round = atoi(e);
     const size_t per_cand = 2 * ((size_t)(1 << D) - 1 + 2);  // two searches: a tree each, plus the two end points
     const size_t cap = per_cand * (size_t)n;                 // requests per round, worst case
     const size_t n2 = 2 * (size_t)n;
@@ -500,15 +484,7 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
             sz2_sort_local<<<cks, kSortThreads, 0, h->stream>>>(g);
             ws_items_scan<<<1, 256, 0, h->stream>>>(g.ws);
             ws_items_scatter<<<items_blocks, 256, 0, h->stream>>>(g.ws);
-            g.dbg = nullptr;
-            if (dbg_round == round + r) {
-                CK(h->d_dbg.ensure(16 * cap));
-                CK(cudaMemsetAsync(h->d_dbg.p, 0, 16 * cap, h->stream));
-                g.dbg = (unsigned*)h->d_dbg.p;
-                h->dbg_n = cap;
-            }
-            if (size_rev) sz2_solve<1><<<solve_blocks, 256, solve_pad, h->stream>>>(g);
-            else sz2_solve<0><<<solve_blocks, 256, solve_pad, h->stream>>>(g);
+            sz2_solve<<<solve_blocks, 256, 0, h->stream>>>(g);
             h->launches += 6;
         }
         // candidates still unfinished after the group's last advance decide whether another group is needed
@@ -829,12 +805,10 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     g.fb_cells = (long long*)h->d_fb_list.p;
     {
         // grid_kernel's long queue: items of at least ~min_len states, at most long_per_sm per SM
-        int long_per_sm = kGkLong, min_len = 1024;
+        const int min_len = 1024;
+        int long_per_sm = kGkLong;
         if (const char* e = getenv("WVA_GRID_LONG")) long_per_sm = std::min(std::max(atoi(e), -1), kGkWarps / 4);
-        if (const char* e = getenv("WVA_GRID_LONG_MINLEN")) min_len = std::max(atoi(e), 2);
         g.long_per_sm = long_per_sm;
-        g.long_share = 0;
-        if (const char* e = getenv("WVA_GRID_SHARE")) g.long_share = std::max(atoi(e), 0);
         g.long_cls = 254 - std::min(std::max((int)(log2f((float)min_len) * 12.0f), 0), 254);
         g.long_cap = (unsigned)(std::max(long_per_sm, 0) * h->sm_count);
         g.n_ctas = h->sm_count;
@@ -1809,12 +1783,6 @@ long long wva_dbg_div_selfcheck(wva_handle* h, unsigned long long seed, int bloc
     return (long long)out;
 }
 
-#ifdef WVA_PROF
-int wva_dbg_prof(long long* out, int reset) {
-    if (reset) { long long z[16] = {0}; return (int)cudaMemcpyToSymbol(wva::wva_prof, z, sizeof(z)); }
-    return (int)cudaMemcpyFromSymbol(out, wva::wva_prof, sizeof(long long) * 16);
-}
-#endif
 int wva_dbg_read_plan(wva_handle* h, unsigned* out32) {  // grid_items_plan's queue plan: item_count[2*kClasses+1 ..+31]
     if (!h || !h->d_sort.p || !h->dbg_plan) return -1;
     return (int)cudaMemcpy(out32, h->dbg_plan, sizeof(unsigned) * 31, cudaMemcpyDeviceToHost);
@@ -1823,21 +1791,6 @@ int wva_dbg_enable_cycles(wva_handle* h, int on) {
     if (!h) return WVA_ERR_BAD_ARG;
     h->dbg_cycles = on != 0;
     return WVA_OK;
-}
-int wva_dbg_szcnt(unsigned long long* out24, int reset) {
-#ifdef WVA_SZCNT
-    if (reset) { unsigned long long z[24] = {0}; return (int)cudaMemcpyToSymbol(wva::wva_szcnt, z, sizeof(z)); }
-    return (int)cudaMemcpyFromSymbol(out24, wva::wva_szcnt, sizeof(unsigned long long) * 24);
-#else
-    (void)out24; (void)reset;
-    return -1;
-#endif
-}
-long long wva_dbg_read_size(wva_handle* h, unsigned* out4, long long cap) {  // rows of {cycles, N | kind << 16, lambda bits, warp}
-    if (!h || !h->d_dbg.p) return 0;
-    const long long n = std::min<long long>((long long)h->dbg_n, cap);
-    cudaMemcpy(out4, h->d_dbg.p, 16 * n, cudaMemcpyDeviceToHost);
-    return n;
 }
 long long wva_dbg_read_cycles(wva_handle* h, unsigned* cycles, unsigned* cells, long long cap) {
     if (!h || !h->d_dbg.p) return 0;

@@ -259,23 +259,6 @@ __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefe
 // state j, one 8-byte column per lane) and pass 2 reads them back instead of re-running the
 // recurrence for those states — most grid chains are shorter than that.
 //
-#ifdef WVA_SZCNT  // diagnostics build (tools/size_dbg.py): which loop the full-length N = 256 chains spend their steps in
-__device__ unsigned long long wva_szcnt[24];
-#define WVA_CNT(k) ++cnt_[k]
-#define WVA_CNT_ADD(k, v) cnt_[k] += (v)
-#else
-#define WVA_CNT(k)
-#define WVA_CNT_ADD(k, v)
-#endif
-#ifdef WVA_PROF  // diagnostics build (tools/prof_chain.py): phase clocks and counters of the last solve
-__device__ long long wva_prof[16];
-#define WVA_PROF_T(k) wva_prof[k] = clock64()
-#define WVA_PROF_C(k) ++wva_prof[k]
-#else
-#define WVA_PROF_T(k)
-#define WVA_PROF_C(k)
-#endif
-//
 // STAGED (grid_kernel): when the 32 lanes of a full warp read the SAME pair table (they usually do: an
 // item is cut from one pair's cells) the head of both passes runs from a 32-entry window of the table
 // that the warp stages in shared memory (`tbuf`, 1 KB per warp) with one coalesced load per 32 steps,
@@ -286,7 +269,6 @@ __device__ long long wva_prof[16];
 // constants in one batch at the top of the solve, so a short item (most of them: batch sizes below 64) makes ONE
 // trip to L2 for everything it reads; pass 2 re-uses that window when the whole head fits in it (hmax <= 64).
 // Later windows are 32 entries, prefetched in registers as before.  `tbuf` holds kStagedSlots entries.
-// REV: pairs of checked steps a lane set takes on the per-step path before it returns to the block vote (0 = never returns)
 __device__ __forceinline__ void dev_cp_async16(void* smem_dst, const void* gmem_src) {
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
@@ -297,7 +279,7 @@ constexpr int kStagedTbufD = kStagedSlots * 4 + 128;  // doubles per warp: the w
 // WIDE: the windows of the comment above kHiPLo.  grid_kernel's instantiation (STAGED) keeps the round-1 windows
 // (2^600 / 2^620, fixed pass-2 bound): its batch sizes stay below what needs more, and the extra pass-2 set-up
 // perturbs its register allocation; everything else (size path, sweep, row solve callers) is WIDE.
-template <int STASH, int PF = 10, bool STAGED = false, int REV = 1, bool WIDE = !STAGED>
+template <int STASH, int PF = 10, bool STAGED = false, bool WIDE = !STAGED>
 __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N, int K, float lambda, ModelStats& st,
                                            double* __restrict__ stash, double* __restrict__ tbuf = nullptr) {
     constexpr unsigned kHiPHi = WIDE ? wva::kHiPHi : kHiPHiNarrow;   // shadow the namespace constants
@@ -306,9 +288,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     const unsigned warp_mask = __activemask();
     const double lam = (double)lambda;
     const int nh = N - 1;
-#ifdef WVA_SZCNT
-    unsigned cnt_[16] = {0};
-#endif
     Recip A, B;  // reciprocal triples of two consecutive steps (software-pipelined table loads)
     // staged head: full warp, one table.  Everything the solve reads from the table is requested here in one
     // batch: the first 64-entry window, the lane's tail entry (T stays in registers for the whole solve) and
@@ -404,7 +383,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     }
 
     // ---- pass 1 -----------------------------------------------------------------
-    WVA_PROF_T(0);
     double sum = __dadd_rn(1.0, p);
     int j_end = K + 1;
     if (STASH > 0) stash[0] = p;
@@ -445,7 +423,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             if (kStagedFirst + 1 < hmax) nxt = tab4[min(kStagedFirst + 1 + lane, hmax)];
             if (STASH > 0) { WVA_SP1(true, kStagedFirst) } else { WVA_SP1(false, kStagedFirst) }
             for (int n0 = kStagedFirst + 1; ok && n0 < hmax; n0 += 32) {
-                WVA_PROF_C(4);
                 __syncwarp();
                 tb[lane] = nxt;
                 __syncwarp();
@@ -455,10 +432,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 #undef WVA_SP1_GROUP
 #undef WVA_SP1
         }
-        WVA_PROF_T(12);
-#ifdef WVA_PROF
-        wva_prof[5] = n;
-#endif
         // invariant at the top of the loop: A = triple of step n, B = triple of step n+1 (the tail entry is
         // already in registers: a warp that is past its heads issues no load here)
         WVA_LOAD_TAIL(A)
@@ -479,12 +452,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             //    chains spend 10/11 of their steps;
             //  * generic 4-step blocks otherwise.
             for (;;) {
-                WVA_CNT(8); WVA_CNT_ADD(9, __popc(__activemask()));
-                if (!(n > nh + 1)) WVA_CNT(4);
-                if (!(n + 16 <= n_stop)) WVA_CNT(5);
-                if (!WVA_FASTWIN(p, blk16_lo, blk16_span)) WVA_CNT(6);
                 if (__all_sync(__activemask(), n > nh + 1 && n >= STASH && n + 16 <= n_stop && WVA_FASTWIN(p, blk16_lo, blk16_span))) {
-                    WVA_CNT(0);
                     const double cA = __dmul_rn(lam, A.yl);
 #pragma unroll
                     for (int u = 0; u < 16; ++u) {
@@ -496,7 +464,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                 }
                 if (__all_sync(__activemask(), n + 4 <= n_stop && WVA_FASTWIN(p, blk_lo, blk_span))) {
                     if (n < nh) prefetch_l1(tab + 4 * (n + PF));
-                    WVA_CNT(1);
                     WVA_P1_STEP(A)
                     WVA_P1_STEP(B)
                     WVA_P1_STEP(A)
@@ -508,20 +475,16 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             // Per-step phase: at most two checked steps, then back to the vote — the lane that failed the
             // block vote (near its end, or p about to leave the window) is usually gone by then and the
             // others must not stay on this slower path for the rest of their chain.
-            for (int rv = 0; REV == 0 || rv < REV; ++rv) {
-                if (n >= n_stop || !WVA_FASTWIN(p, lo_eff, span_eff)) goto p1_slow;
-                if (n < nh) prefetch_l1(tab + 4 * (n + PF));
-                WVA_CNT(2);
-                WVA_P1_STEP(A)
-                if (n >= n_stop || !WVA_FASTWIN(p, lo_eff, span_eff)) goto p1_slow;
-                WVA_P1_STEP(B)
-            }
+            if (n >= n_stop || !WVA_FASTWIN(p, lo_eff, span_eff)) goto p1_slow;
+            if (n < nh) prefetch_l1(tab + 4 * (n + PF));
+            WVA_P1_STEP(A)
+            if (n >= n_stop || !WVA_FASTWIN(p, lo_eff, span_eff)) goto p1_slow;
+            WVA_P1_STEP(B)
             continue;
 #undef WVA_P1_STEP
         p1_slow:
             if (n >= n_stop) break;
             // p[n] is outside the fast window
-            WVA_CNT(3);
             const unsigned hp = (unsigned)__double2hiint(p);
             if (hp < thr_hi && (n >= nh ? tail_mono : rate_below(lambda, tab_suffix_min(tab, n)))) {
                 j_end = n + 1;  // negligible and past the mode: states > n contribute nothing
@@ -543,7 +506,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
         }
     }
     __syncwarp(warp_mask);
-    WVA_PROF_T(1);
     if (!in_window(sum, kHiSumLo, kHiSumHi)) bail = true;
     if (bail) { sum = 1.0; j_end = 1; }
 
@@ -635,7 +597,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                                                                  : __ddiv_rn(__dmul_rn(pprev, lam), A.b);
             }
         }
-        WVA_PROF_T(2);
         if (STAGED && staged && __all_sync(0xffffffffu, i == __shfl_sync(0xffffffffu, i, 0))) {
             // staged head of pass 2 (see pass 1): states i < nh take their step's entry from the window
             const double4* tab4 = reinterpret_cast<const double4*>(tab);
@@ -677,7 +638,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             double4 nxt;
             if (!reuse && i < hmax) nxt = tab4[min(i + lane, hmax)];
             for (int i0 = i; ok && i0 < hmax; i0 += 32) {
-                WVA_PROF_C(7);
                 if (reuse) {
                     tbp = tb + (i0 - 1);  // slots up to (hmax - 1) + 31 < kStagedSlots may be touched (values unused)
                 } else {
@@ -691,10 +651,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 #undef WVA_SP2_GROUP
 #undef WVA_SP2
         }
-        WVA_PROF_T(13);
-#ifdef WVA_PROF
-        wva_prof[8] = i;
-#endif
         // invariant at the top of the loop: A = triple of the step out of state i, B = of state i+1
         WVA_LOAD_TAIL(A)
         B = A;
@@ -716,10 +672,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
         ++i;                                                                \
     }
             for (;;) {  // block phase, as in pass 1; pure-tail also needs i > N (sumP complete)
-                if (!(i + 16 <= j_end)) WVA_CNT(14);
-                if (!WVA_FASTWIN(p, blk16b_lo, blk16b_span)) WVA_CNT(15);
                 if (__all_sync(__activemask(), i > nh + 1 && i > N && i + 16 <= j_end && WVA_FASTWIN(p, blk16b_lo, blk16b_span))) {
-                    WVA_CNT(10);
                     const double cA = __dmul_rn(lam, A.yl);
 #pragma unroll
                     for (int u = 0; u < 16; ++u) {
@@ -733,7 +686,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                 }
                 if (__all_sync(__activemask(), i + 4 <= j_end && WVA_FASTWIN(p, blk2_lo, blk2_span))) {
                     if (i < nh) prefetch_l1(tab + 4 * (i + PF));
-                    WVA_CNT(11);
                     WVA_P2_STEP(A)
                     WVA_P2_STEP(B)
                     WVA_P2_STEP(A)
@@ -742,14 +694,12 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                 }
                 break;
             }
-            for (int rv = 0; REV == 0 || rv < REV; ++rv) {  // per-step phase (see pass 1)
-                if (i >= j_end || !WVA_FASTWIN(p, lo2, span2)) goto p2_slow;
-                if (i < nh) prefetch_l1(tab + 4 * (i + PF));
-                WVA_CNT(12);
-                WVA_P2_STEP(A)
-                if (i >= j_end || !WVA_FASTWIN(p, lo2, span2)) goto p2_slow;
-                WVA_P2_STEP(B)
-            }
+            // per-step phase (see pass 1)
+            if (i >= j_end || !WVA_FASTWIN(p, lo2, span2)) goto p2_slow;
+            if (i < nh) prefetch_l1(tab + 4 * (i + PF));
+            WVA_P2_STEP(A)
+            if (i >= j_end || !WVA_FASTWIN(p, lo2, span2)) goto p2_slow;
+            WVA_P2_STEP(B)
             continue;
 #undef WVA_P2_STEP
         p2_slow:
@@ -774,7 +724,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
         }
     }
     __syncwarp(warp_mask);
-    WVA_PROF_T(3);
     // acc_at_N tracked acc while i <= N: it holds acc at state min(N, last state)
     const double in_serv = __dadd_rn(acc_at_N, __dmul_rn(__dsub_rn(1.0, sum_p), (double)N));
     const double pnK = (j_end == K + 1) ? pn : 0.0;
@@ -788,14 +737,6 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     if (w < 0.0f) w = 0.0f;
     st.avg_wait_time = w;
 #undef WVA_LOAD_TAIL
-#ifdef WVA_SZCNT
-    if (N == 256 && j_end > K - 16) {  // full-length chains of the largest batch size only
-        for (int k = 0; k < 16; ++k) if (cnt_[k]) atomicAdd(&wva_szcnt[k], (unsigned long long)cnt_[k]);
-        atomicAdd(&wva_szcnt[16], 1ull);
-        atomicAdd(&wva_szcnt[17], (unsigned long long)(blk16_span != 0));
-        atomicAdd(&wva_szcnt[18], (unsigned long long)nh);
-    }
-#endif
     return bail ? kSolveBail : kSolveOk;
 }
 
@@ -928,9 +869,8 @@ __device__ __forceinline__ int solve_shared(const double* __restrict__ tab, int 
     return solve_shared_t<0>(tab, N, K, lambda, st, nullptr);
 }
 // Per-lane private tables (size path): every lane streams its own table, so prefetch much further ahead.
-template <int REV>
 __device__ __forceinline__ int solve_private(const double* __restrict__ tab, int N, int K, float lambda, ModelStats& st) {
-    return solve_shared_t<0, 48, false, REV>(tab, N, K, lambda, st, nullptr);
+    return solve_shared_t<0, 48>(tab, N, K, lambda, st, nullptr);
 }
 
 // Stored-vector fallback: a literal restatement of computeProbabilities /

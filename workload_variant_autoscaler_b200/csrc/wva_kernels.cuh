@@ -387,7 +387,6 @@ struct GridArgs {
     int fb_cap;
     int long_per_sm;         // grid_kernel: long items per sub-partition 0 (< 0: chosen per launch by grid_items_plan)
     int n_ctas;              // CTAs of grid_kernel (= SMs)
-    int long_share;          // ... and how many other warps of that sub-partition may pull short items meanwhile
     int long_cls;            // items of class <= long_cls are "long" ...
     unsigned long_cap;       // ... up to this many (long_per_sm x CTAs)
     unsigned* dbg_cycles;    // diagnostics: per order index, SM cycles spent in grid_kernel (or NULL)
@@ -1182,9 +1181,7 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
     if (one_pair && lane < 3) cp_async16(pair_buf + lane, g.pair_rec + 3 * (size_t)pair + lane);
     cp_async_commit();
     ModelStats st;
-    WVA_PROF_T(10);
     const int rc = solve_shared_t<kGridStash, 10, true>(tab, N, K, lambda, st, stash_warp + lane, tbuf_warp);
-    WVA_PROF_T(11);
     cp_async_wait<0>();
     __syncwarp();
     if (valid) {
@@ -1227,7 +1224,6 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
         }
     }
     __syncwarp();
-    WVA_PROF_T(14);
 }
 
 __global__ void __launch_bounds__(kGkThreads, 1) grid_kernel(GridArgs g) {
@@ -1242,10 +1238,9 @@ __global__ void __launch_bounds__(kGkThreads, 1) grid_kernel(GridArgs g) {
     const int long_ctas = per > 0 ? (int)((n_long + per - 1) / per) : 0;
     const int my_long = (int)blockIdx.x < long_ctas ? per : 0;
     const bool long_warp = sub0 && (int)(warp >> 2) < my_long;
-    // sub-partition 0: long_per_sm warps pull the long queue, long_share more may pull short items next
-    // to them, the rest wait on named barrier 1 (blocked in hardware: no issue slots) until the long warps
-    // of this CTA have drained the long queue
-    const int n_parked = my_long > 0 ? kGkWarps / 4 - my_long - g.long_share : 0;
+    // sub-partition 0: long_per_sm warps pull the long queue, the rest wait on named barrier 1 (blocked in
+    // hardware: no issue slots) until the long warps of this CTA have drained the long queue
+    const int n_parked = my_long > 0 ? kGkWarps / 4 - my_long : 0;
     const int bar_threads = 32 * (my_long + (n_parked > 0 ? n_parked : 0));
     if (long_warp && n_long) {
         for (;;) {
@@ -1257,7 +1252,7 @@ __global__ void __launch_bounds__(kGkThreads, 1) grid_kernel(GridArgs g) {
             item_run(g, w, rec, lane, warp_smem);
         }
         if (n_parked > 0) asm volatile("bar.arrive 1, %0;" ::"r"(bar_threads) : "memory");
-    } else if (sub0 && my_long > 0 && !long_warp && (int)(warp >> 2) >= my_long + g.long_share) {
+    } else if (sub0 && my_long > 0 && !long_warp) {
         asm volatile("bar.sync 1, %0;" ::"r"(bar_threads) : "memory");
     }
     // short queue: the list is longest-first and every warp takes the next item when it is free (LPT).  Reserving

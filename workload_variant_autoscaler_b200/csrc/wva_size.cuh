@@ -60,7 +60,6 @@ struct Sz2Args {
     int* fb_count;
     int* fb_list;
     int fb_cap;
-    unsigned* dbg;         // diagnostics (WVA_SIZE_DBG_ROUND): per slot {SM cycles, N, lambda bits, warp}, or NULL
 };
 
 __device__ __forceinline__ float sz_mid(float lo, float hi) { return __fmul_rn(0.5f, __fadd_rn(lo, hi)); }  // utils.go:55
@@ -358,7 +357,6 @@ __global__ void __launch_bounds__(kSortThreads) sz2_sort_local(Sz2Args g) {
 }
 
 // One request per lane, 32 requests of similar chain length per warp.
-template <int REV>
 __global__ void __launch_bounds__(256, 4) sz2_solve(Sz2Args g) {
     const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned w = idx >> 5, lane = idx & 31;
@@ -373,14 +371,7 @@ __global__ void __launch_bounds__(256, 4) sz2_solve(Sz2Args g) {
     const int N = g.cand_N[j], K = N + N * f.ratio;
     const float lambda = g.req_lam[slot];
     ModelStats st;
-    const long long t0 = g.dbg ? clock64() : 0;
-    const int rc = solve_private<REV>(g.tab + 4 * g.tab_off[j], N, K, lambda, st);
-    if (g.dbg) {
-        g.dbg[4 * slot] = (unsigned)(clock64() - t0);
-        g.dbg[4 * slot + 1] = (unsigned)N | ((unsigned)kind << 16);
-        g.dbg[4 * slot + 2] = __float_as_uint(lambda);
-        g.dbg[4 * slot + 3] = w;
-    }
+    const int rc = solve_private(g.tab + 4 * g.tab_off[j], N, K, lambda, st);
     g.req_bail[slot] = rc != kSolveOk;
     if (rc != kSolveOk) return;
     const QParams q = qparams_of(f, pair / f.A, pair % f.A);
