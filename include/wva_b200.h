@@ -238,7 +238,11 @@ int wva_grid_solve(wva_handle *h, const wva_fleet *fleet, const wva_grid *grid,
  */
 int wva_solve_greedy(const wva_fleet *fleet, wva_allocs *candidates, wva_allocs *winners);
 
-/* Latency sweep of QueueAnalyzer.Analyze over n_rates rates per (server, acc). */
+/*
+ * Latency sweep of QueueAnalyzer.Analyze over n_rates rates per (server, acc).  A point whose chain leaves
+ * the streaming solve's exponent windows is re-run on the stored p[0..K] vector with the reference's rescale
+ * loops, like a grid cell; WVA_ERR_UNSUPPORTED only when that rescale loop would not terminate (NaN rates).
+ */
 int wva_sweep(wva_handle *h, const wva_fleet *fleet, int32_t n_rates, wva_sweep_out *out);
 
 /*

@@ -1646,6 +1646,7 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
     CK(cudaMemsetAsync(p, 0, sw.bytes, h->stream));
     CK(cudaEventRecord(h->ev_d0, h->stream));
     CK(cudaEventRecord(h->ev_k0, h->stream));
+    int fb_cap = 0;
     if (n) {
         CK(h->d_tab_pair.ensure(sizeof(int) * n));
         CK(h->d_tab_off.ensure(sizeof(long long) * n));
@@ -1676,6 +1677,10 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         g.throughput = (float*)(p + o_thr);
         g.rho = (float*)(p + o_rho);
         g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
+        fb_cap = (int)std::min<size_t>((size_t)n * n_rates, (size_t)1 << 22);
+        CK(h->d_fb_list.ensure(sizeof(int2) * fb_cap));
+        g.fb_points = (int2*)h->d_fb_list.p;
+        g.fb_cap = fb_cap;
         int per_sm = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sweep_kernel, 256, 0));
         per_sm = std::max(1, std::min(per_sm, 8));
@@ -1684,17 +1689,29 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         CK(cudaEventRecord(h->ev_k0, h->stream));
         sweep_kernel<<<blocks, 256, 0, h->stream>>>(g);
         h->launches++;
+        CK(cudaEventRecord(h->ev_k1, h->stream));
+        // the points whose chain left the streaming solve's window: stored vector, as the reference
+        size_t slot_doubles;
+        int Kmax;
+        rc = ensure_scratch(h, lens[0], hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
+        if (rc) return rc;
+        sweep_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
+                                                                (int*)h->d_ctrl.p + CTRL_FB_STATUS);
+        h->launches++;
         CK(cudaGetLastError());
+    } else {
+        CK(cudaEventRecord(h->ev_k1, h->stream));
     }
-    CK(cudaEventRecord(h->ev_k1, h->stream));
     CK(h->out_stage.ensure(256));
     int* ctrl_host = (int*)h->out_stage.p;
     CK(cudaMemcpyAsync(ctrl_host, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     CK(sw.copy_back(p, h->stream));
     rc = finish_timing(h);
     if (rc) return rc;
-    if (ctrl_host[CTRL_FB_COUNT] != 0)
-        return h->fail(WVA_ERR_UNSUPPORTED, "sweep point outside the streaming solve's numeric window");
+    if (ctrl_host[CTRL_FB_STATUS] != 0)
+        return h->fail(WVA_ERR_UNSUPPORTED, "input outside the supported numeric domain (rescale loop does not terminate)");
+    if ((long long)ctrl_host[CTRL_FB_COUNT] > fb_cap)
+        return h->fail(WVA_ERR_UNSUPPORTED, "too many sweep points need the stored-vector fallback");
     return WVA_OK;
 }
 

@@ -1893,7 +1893,17 @@ struct SweepArgs {
     uint8_t* valid;
     float *rate, *ttft, *itl, *throughput, *rho;
     int* fb_count;
+    int2* fb_points;       // points that bailed: {entry of pair_list, rate index}
+    int fb_cap;
 };
+
+// The sweep's rate i of a pair (same float32 expressions as the oracle's sweep).
+__device__ __forceinline__ float sweep_rate(float rmin, float rmax, int i, int n_rates) {
+    const float hi = __fmul_rn(rmax, 0.999f);
+    const float span = __fsub_rn(hi, rmin);
+    const float frac = n_rates > 1 ? __fdiv_rn((float)i, (float)(n_rates - 1)) : 0.0f;
+    return __fadd_rn(rmin, __fmul_rn(span, frac));
+}
 
 __global__ void __launch_bounds__(256) sweep_kernel(SweepArgs g) {
     const DevFleet& f = g.f;
@@ -1916,10 +1926,7 @@ __global__ void __launch_bounds__(256) sweep_kernel(SweepArgs g) {
         const float rmin = rate_min_of((float)tab[0]), rmax = rate_max_of((float)tail.b);
         const int i = chunk * 32 + lane;
         if (i < g.n_rates) {
-        const float hi = __fmul_rn(rmax, 0.999f);
-        const float span = __fsub_rn(hi, rmin);
-        const float frac = g.n_rates > 1 ? __fdiv_rn((float)i, (float)(g.n_rates - 1)) : 0.0f;
-        const float rate = __fadd_rn(rmin, __fmul_rn(span, frac));
+        const float rate = sweep_rate(rmin, rmax, i, g.n_rates);
         const size_t o = (size_t)pair * g.n_rates + i;
         g.rate[o] = rate;
         uint8_t ok = 0;
@@ -1932,7 +1939,8 @@ __global__ void __launch_bounds__(256) sweep_kernel(SweepArgs g) {
                 m = metrics_from(q, N, st);
                 ok = 1;
             } else {
-                atomicAdd(g.fb_count, 1);
+                const int k = atomicAdd(g.fb_count, 1);
+                if (k < g.fb_cap) g.fb_points[k] = make_int2(e, i);
             }
         }
         g.valid[o] = ok;
@@ -1941,6 +1949,40 @@ __global__ void __launch_bounds__(256) sweep_kernel(SweepArgs g) {
         g.throughput[o] = m.throughput;
         g.rho[o] = m.rho;
         }
+    }
+}
+
+// Stored-vector re-run of the sweep points sweep_kernel bailed on (slot k handles list entries k, k + n_slots, ..);
+// scratch per slot as in grid_fallback.
+__global__ void sweep_fallback(SweepArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+    const DevFleet& f = g.f;
+    const int n_slots = gridDim.x * blockDim.x;
+    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+    int n = *g.fb_count;
+    if (n > g.fb_cap) n = g.fb_cap;
+    double* p = scratch + (size_t)slot * slot_doubles;
+    float* sr = (float*)(p + Kmax + 1);
+    for (int k = slot; k < n; k += n_slots) {
+        const int e = g.fb_points[k].x, i = g.fb_points[k].y;
+        const int pair = g.pair_list[e];
+        const int s = pair / f.A, a = pair % f.A;
+        const int N = g.pair_N[e], K = N + N * f.ratio;
+        const double* tab = g.tab + 4 * g.tab_off[e];
+        for (int u = 0; u < N; ++u) sr[u] = (float)tab[4 * u];
+        const float rate = sweep_rate(rate_min_of(sr[0]), rate_max_of(sr[N - 1]), i, g.n_rates);
+        ModelStats st;
+        const int rc = solve_stored(p, sr, N, K, __fdiv_rn(rate, 1000.0f), st);
+        if (rc != 0) {
+            atomicExch(fb_status, rc);
+            continue;
+        }
+        const Metrics m = metrics_from(qparams_of(f, s, a), N, st);
+        const size_t o = (size_t)pair * g.n_rates + i;
+        g.valid[o] = 1;
+        g.ttft[o] = m.ttft;
+        g.itl[o] = m.avg_token_time;
+        g.throughput[o] = m.throughput;
+        g.rho[o] = m.rho;
     }
 }
 
