@@ -276,6 +276,27 @@ def long_queue_fleet():
     return _fleet(1.0, 0.0, np.ones(len(rows)), [r[0] for r in rows], tps=tps, ratio=LONG_RATIO)
 
 
+def overflow_search_fleet(slo_itl, slo_ttft):
+    """The N = 1024 overflow fleet of the grid's stored-vector test with ITL (and TTFT) targets: the ITL bisection's
+    end point lambda_max overflows float64, so the streaming solve bails in the search's first round and the
+    stored-vector fallback bisects across overflowing midpoints."""
+    fleet = synth_fleet(2, 1, seed=29, max_batch_choices=(1024,))
+    fleet.perf_alpha[:] = 7.47
+    fleet.perf_beta[:] = 0.0001
+    fleet.perf_gamma[:] = 1.0
+    fleet.perf_delta[:] = 0.00001
+    fleet.srv_in_tokens[:] = 64
+    fleet.srv_out_tokens[:] = 64
+    fleet.srv_slo_tps[:] = 0
+    fleet.srv_slo_itl[:] = slo_itl
+    fleet.srv_slo_ttft[:] = slo_ttft
+    fleet.srv_arrival_rpm[:] = [60.0 * 2100, 60.0 * 1900]
+    return fleet
+
+
+OVERFLOW_SEARCHES = [(7.55, 0.0, 1.6744), (7.56, 200.0, 1.8813)]  # slo_itl, slo_ttft, the candidates' max_rate
+
+
 def sweep_fleet():
     """Sweep pairs: N = 1024 (x up to ~1022: 680, 880, 900, pass 2, overflow), N = 4096 (steep crossings of 2^880),
     and the rate edges at N = 16."""
@@ -488,6 +509,29 @@ def test_long_queue_cases_reach_the_pass2_ieee_path(oracle_mod):
     assert ieee.sum() >= 3, P["esum"]
 
 
+def test_overflow_search_cases_bail_inside_the_search(oracle_mod):
+    """The ITL bisection of overflow_search_fleet iterates (EvalITL crosses the targets between lambda_min and
+    lambda_max), its end point lambda_max and 0.9 lambda_max overflow float64 while lambda_max / 2 does not, and the
+    candidates are feasible."""
+    import oracle
+    f = overflow_search_fleet(7.55, 0.0)
+    ratio = f.max_queue_to_batch_ratio
+    qa = oracle.Analyzer(1024, 1024 * ratio, float(f.perf_alpha[0, 0]), float(f.perf_beta[0, 0]),
+                         float(f.perf_gamma[0, 0]), float(f.perf_delta[0, 0]), int(f.srv_in_tokens[0]),
+                         int(f.srv_out_tokens[0]))
+    lo, hi = qa.rate_range()
+    lmin, lmax = _lam_of_rate(lo), _lam_of_rate(hi)
+    (e0, y0), (e1, y1) = qa.eval_itl(float(lmin)), qa.eval_itl(float(lmax))
+    assert e0 == 0 and e1 == 0
+    assert y0 < min(t for t, _, _ in OVERFLOW_SEARCHES) and y1 > max(t for t, _, _ in OVERFLOW_SEARCHES)
+    P = chain_profile(qa.serv_rate(), qa.K, [lmax, f32(f32(0.9) * lmax), f32(lmax / f32(2))])
+    assert P["over"].tolist() == [True, True, False]
+    for slo_itl, slo_ttft, max_rate in OVERFLOW_SEARCHES:
+        cand, _ = oracle_mod.solve(overflow_search_fleet(slo_itl, slo_ttft))
+        assert (cand["feasible"] == 1).all() and (cand["replicas"] == 2).all()
+        assert np.allclose(cand["max_rate"], max_rate, rtol=1e-4)
+
+
 def test_sweep_cases_reach_their_bands(oracle_mod):
     fleet = sweep_fleet()
     o = oracle_mod.sweep(fleet, SWEEP_RATES)
@@ -557,6 +601,22 @@ def test_size_long_queue_at_window_edges(engine, oracle_mod, monkeypatch, small_
     cand_g, win_g = engine.solve(fleet)
     assert_allocs_equal(cand_g, cand_o, f"long-queue size candidates (small max {small_max})")
     assert_allocs_equal(win_g, win_o, f"long-queue winners (small max {small_max})")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("small_max,depth", [("1024", "5"), ("0", "1"), ("0", "5")])
+@pytest.mark.parametrize("case", range(len(OVERFLOW_SEARCHES)))
+def test_size_search_bails_to_stored_vector(engine, oracle_mod, monkeypatch, small_max, depth, case):
+    """A bisection whose streaming solves overflow float64 (the warp kernel and the rounds at depths 1 and 5): the
+    candidate is re-run on the stored vector, whose search crosses overflowing midpoints."""
+    monkeypatch.setenv("WVA_SIZE_SMALL_MAX", small_max)
+    monkeypatch.setenv("WVA_SIZE_DEPTH", depth)
+    slo_itl, slo_ttft, _ = OVERFLOW_SEARCHES[case]
+    fleet = overflow_search_fleet(slo_itl, slo_ttft)
+    cand_o, win_o = oracle_mod.solve(fleet)
+    cand_g, win_g = engine.solve(fleet)
+    assert_allocs_equal(cand_g, cand_o, f"size candidates (overflowing search, small max {small_max}, D = {depth})")
+    assert_allocs_equal(win_g, win_o, f"winners (overflowing search, small max {small_max}, D = {depth})")
 
 
 def _sweep_equal(g, o, what):

@@ -447,8 +447,8 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     g.cand_N = sa.cand_N;
     g.n_cand = n;
     g.depth = D;
-    g.tab = (const double*)h->d_sz_tab.p;
-    g.tab_off = (const long long*)h->d_sz_off.p;
+    g.tab = sa.tab;
+    g.tab_off = sa.tab_off;
     g.ls = (const float*)h->d_sz_ls.p;
     g.xmin = (float*)(sp + o_xmin); g.xmax = (float*)(sp + o_xmax); g.xs = (float*)(sp + o_xs);
     g.sst = (uint8_t*)(sp + o_sst); g.inc = (uint8_t*)(sp + o_inc); g.iter = (uint8_t*)(sp + o_iter);
@@ -514,6 +514,8 @@ int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners)
     g.cand_pair = (const int*)h->d_cand_pair.p;
     g.cand_N = (const int*)h->d_cand_N.p;
     g.n_cand = n;
+    g.tab = (const double*)h->d_sz_tab.p;
+    g.tab_off = (const long long*)h->d_sz_off.p;
     g.cand = cand;
     g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
     CK(h->d_fb_list.ensure(sizeof(int) * std::max(n, 1)));
@@ -523,8 +525,7 @@ int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners)
     int small_max = 1024;  // up to here a warp per candidate beats rounds (the GPU is mostly empty either way)
     if (const char* e = getenv("WVA_SIZE_SMALL_MAX")) small_max = atoi(e);
     if (n > 0 && n <= small_max) {
-        size_warp_kernel<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g, (const double*)h->d_sz_tab.p,
-                                                                          (const long long*)h->d_sz_off.p);
+        size_warp_kernel<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
         h->launches++;
     } else if (n > 0) {
         rc = run_size_rounds(h, g, n);

@@ -5,12 +5,12 @@
 //                       sort, persistent warps pulling 32-cell items, fused feasibility + batch-rank minimum
 //   grid_fallback       stored-vector re-run of the rare cells the streaming solve bails on
 //   grid_finalize  K3   per-server argmin over partials (warp shuffle -> smem -> record)
-//   sz2_* kernels  K1   (wva_size.cuh) CreateAllocation per (server, acc) candidate as rounds of sorted solve
-//                       batches with speculative bisection trees
-//   size_fallback       stored-vector re-run of candidates that bailed
 //   trivial_kernel      nil / zero-load candidates
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
+//
+// K1, CreateAllocation per (server, accelerator) candidate (the rounds, the warp-per-candidate kernel and the
+// stored-vector fallback), is in wva_size.cuh.
 #pragma once
 #include "wva_device.cuh"
 
@@ -1512,202 +1512,6 @@ __global__ void __launch_bounds__(256) grid_finalize(GridArgs g, AllocCols winne
         }
     }
 }
-
-// ---------------------------------------------------------------------------
-// K1: size candidates (CreateAllocation).
-// ---------------------------------------------------------------------------
-
-// Solver policies: a solver evaluates Model.Solve(lambda, 1) and reports bail-outs.
-struct StoredSolver {  // stored-vector fallback
-    double* p;
-    const float* sr;
-    int N, K;
-    int bail;
-    __device__ __forceinline__ int solve(float lambda, ModelStats& st) {
-        const int rc = solve_stored(p, sr, N, K, lambda, st);
-        if (rc != 0) bail = rc;
-        return rc;
-    }
-};
-
-// EvalTTFT / EvalITL (queueanalyzer.go:270-290) + BinarySearch (utils.go:26-70).
-// which = 0: TTFT, 1: ITL.  Returns 0 ok (xstar, ind), 2 eval error / bail.
-template <class Solver>
-__device__ int eval_target(Solver& sv, const QParams& q, int which, float x, float& y) {
-    ModelStats st;
-    if (sv.solve(x, st) != 0) return 2;
-    const float eff = effective_concurrency(q, st.avg_serv_time, sv.N);
-    if (which == 0)
-        y = __fadd_rn(st.avg_wait_time, prefill_time(q, eff));
-    else
-        y = decode_time(q, eff);
-    return 0;
-}
-template <class Solver>
-__device__ int binary_search(Solver& sv, const QParams& q, int which, float xmin, float xmax, float ytarget,
-                             float& xstar, int& ind) {
-    xstar = 0.0f;
-    ind = 0;
-    if (xmin > xmax) return 1;
-    float y0, y1;
-    if (eval_target(sv, q, which, xmin, y0)) return 2;
-    if (within_tolerance(y0, ytarget, 1e-6f)) { xstar = xmin; return 0; }
-    if (eval_target(sv, q, which, xmax, y1)) return 2;
-    if (within_tolerance(y1, ytarget, 1e-6f)) { xstar = xmax; return 0; }
-    const bool increasing = y0 < y1;
-    if ((increasing && ytarget < y0) || (!increasing && ytarget > y0)) { xstar = xmin; ind = -1; return 0; }
-    if ((increasing && ytarget > y1) || (!increasing && ytarget < y1)) { xstar = xmax; ind = 1; return 0; }
-    float xs = 0.0f, ys = 0.0f;
-    for (int it = 0; it < 100; ++it) {
-        xs = __fmul_rn(0.5f, __fadd_rn(xmin, xmax));
-        if (eval_target(sv, q, which, xs, ys)) return 2;
-        if (within_tolerance(ys, ytarget, 1e-6f)) break;
-        const float pmin = xmin, pmax = xmax;
-        if ((increasing && ytarget < ys) || (!increasing && ytarget > ys))
-            xmax = xs;
-        else
-            xmin = xs;
-        // Fixed point: the iteration is a deterministic function of (xmin, xmax), so once an
-        // iteration leaves both bounds unchanged (the float32 interval has collapsed) the
-        // reference's remaining iterations repeat the same solve and return the same xStar.
-        if (xmin == pmin && xmax == pmax) break;
-    }
-    xstar = xs;
-    return 0;
-}
-
-// Analyze (queueanalyzer.go:134-174) -> 0 ok.
-template <class Solver>
-__device__ int analyze(Solver& sv, const QParams& q, float rmax, float rate, Metrics& m) {
-    if (rate <= 0.0f) return 1;
-    if (rate > rmax) return 2;
-    ModelStats st;
-    if (sv.solve(__fdiv_rn(rate, 1000.0f), st) != 0) return 3;
-    m = metrics_from(q, sv.N, st);
-    return 0;
-}
-
-// CreateAllocation under load (allocation.go:77-163); value = cost.
-// s1 / sN = servRate[0] / servRate[N-1] (float32).
-template <class Solver>
-__device__ Cand create_allocation(const DevFleet& f, int s, int a, Solver& sv, float s1, float sN) {
-    Cand out = cand_nil();
-    if (sv.K < 2) return out;  // a model with K <= 1 is never valid (queuemodel.go:31, stale rho = 1)
-    const QParams q = qparams_of(f, s, a);
-    const float rmin = rate_min_of(s1), rmax = rate_max_of(sN);
-    const float slo_ttft = f.srv_slo_ttft[s], slo_itl = f.srv_slo_itl[s], slo_tps = f.srv_slo_tps[s];
-    if (slo_itl < 0.0f || slo_ttft < 0.0f || slo_tps < 0.0f) return out;  // TargetPerf.check :322-329
-    const float lambda_min = __fdiv_rn(rmin, 1000.0f), lambda_max = __fdiv_rn(rmax, 1000.0f);
-    int ind = 0;
-    float l_ttft = lambda_max, l_itl = lambda_max, l_tps = lambda_max;
-    if (slo_ttft > 0.0f) {  // queueanalyzer.go:205-215
-        const int err = binary_search(sv, q, 0, lambda_min, lambda_max, slo_ttft, l_ttft, ind);
-        if (ind < 0 || err != 0) return out;
-    }
-    if (slo_itl > 0.0f) {  // :218-228
-        const int err = binary_search(sv, q, 1, lambda_min, lambda_max, slo_itl, l_itl, ind);
-        if (ind < 0 || err != 0) return out;
-    }
-    if (slo_tps > 0.0f) l_tps = __fmul_rn(lambda_max, __fsub_rn(1.0f, 0.1f));  // :231-234
-    const float lambda = go_minf(go_minf(l_ttft, l_itl), l_tps);
-    Metrics m;
-    if (analyze(sv, q, rmax, __fmul_rn(lambda, 1000.0f), m) != 0) return out;  // :237-241
-    const float rate_star = m.throughput;
-
-    const float total_rate = total_rate_of(f, s);  // allocation.go:134-141
-    long long nrep = go_f64_to_int(ceil(__ddiv_rn((double)total_rate, (double)rate_star)));
-    const long long min_rep = f.srv_min_replicas[s];
-    if (nrep < min_rep) nrep = min_rep;
-    const long long total = (long long)num_instances(f, f.srv_model[s], a) * nrep;  // :144-145
-    const float cost = __fmul_rn(f.acc_cost[a], (float)total);
-    const float rate = __fdiv_rn(total_rate, (float)nrep);  // :148-153
-    if (analyze(sv, q, rmax, rate, m) != 0) return out;
-    out.feasible = 1;
-    out.acc = a;
-    out.replicas = (int)nrep;
-    out.batch = sv.N;
-    out.cost = cost;
-    out.value = cost;
-    out.itl = m.avg_token_time;
-    out.ttft = m.ttft;
-    out.rho = m.rho;
-    out.max_rate = __fdiv_rn(rate_star, 1000.0f);
-    return out;
-}
-
-struct SizeArgs {
-    DevFleet f;
-    const int* cand_pair;  // [n_cand] pair ids sorted by descending N
-    const int* cand_N;     // [n_cand]
-    int n_cand;
-    AllocCols cand;        // [S*A]
-    int* fb_count;
-    int* fb_list;          // candidate indices that bailed
-    int fb_cap;
-};
-
-// Stored-vector re-run of bailed candidates (slot k handles list entries k, k+n_slots, ..).
-__global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
-    const DevFleet& f = g.f;
-    const int n_slots = gridDim.x * blockDim.x;
-    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
-    int n = *g.fb_count;
-    if (n > g.fb_cap) n = g.fb_cap;
-    double* p = scratch + (size_t)slot * slot_doubles;
-    float* sr = (float*)(p + Kmax + 1);
-    for (int k = slot; k < n; k += n_slots) {
-        const int j = g.fb_list[k];
-        const int pair = g.cand_pair[j];
-        const int s = pair / f.A, a = pair % f.A;
-        StoredSolver sv;
-        sv.N = g.cand_N[j];
-        sv.K = sv.N + sv.N * f.ratio;
-        sv.p = p;
-        sv.sr = sr;
-        sv.bail = 0;
-        const QParams q = qparams_of(f, s, a);
-        for (int i = 0; i < sv.N; ++i) sr[i] = serv_rate(q, i + 1);
-        for (int i = 0; i <= sv.K; ++i) p[i] = 0.0;
-        Cand c = create_allocation(f, s, a, sv, sr[0], sr[sv.N - 1]);
-        if (sv.bail) {
-            atomicExch(fb_status, sv.bail);
-            c = cand_nil();
-        }
-        store_cand(g.cand, pair, c);
-    }
-}
-
-// ---------------------------------------------------------------------------
-// K1 (size candidates as rounds of sorted solve batches) lives in wva_size.cuh; the sort workspace and the
-// item ordering kernels it shares with nothing else stay here next to the grid's.
-// ---------------------------------------------------------------------------
-struct SortWs {
-    unsigned* order;
-    unsigned long long* items;
-    unsigned long long* items_sorted;
-    unsigned* item_count;  // [0] items, [1..256] per class, [257..512] cursors
-};
-enum { PH_SEARCH = 0, PH_WAIT_STAR = 1, PH_WAIT_FINAL = 2, PH_DONE = 3, PH_NIL = 4, PH_BAIL = 5 };
-__global__ void __launch_bounds__(256) ws_items_scan(SortWs ws) {
-    __shared__ unsigned tot[kClasses];
-    tot[threadIdx.x] = ws.item_count[1 + threadIdx.x];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned acc = 0;
-        for (int c = 0; c < kClasses; ++c) {
-            ws.item_count[1 + kClasses + c] = acc;
-            acc += tot[c];
-        }
-    }
-}
-__global__ void __launch_bounds__(256) ws_items_scatter(SortWs ws) {
-    const unsigned n = *ws.item_count;
-    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const unsigned long long it = ws.items[i];
-    ws.items_sorted[agg_inc(ws.item_count + 1 + kClasses, (int)((it >> 40) & 0xff))] = it;
-}
-
 
 // nil and zero-load candidates (everything the size kernel does not own).
 __global__ void trivial_kernel(DevFleet f, AllocCols cand) {

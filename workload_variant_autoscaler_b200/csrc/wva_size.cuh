@@ -1,5 +1,8 @@
 // wva_size.cuh — K1, the reference's decision path: CreateAllocation (pkg/core/allocation.go:27-163) for every
-// (server, accelerator) candidate as ROUNDS of sorted solve batches with SPECULATIVE bisection.
+// (server, accelerator) candidate.  The decisions (the start, the bisections' end-point test and walk, lambda*, the
+// replica count, the feasible candidate) are written once below and driven two ways: large fleets run ROUNDS of
+// sorted solve batches with SPECULATIVE bisection (sz2_*); small fleets and the stored-vector fallback run
+// create_allocation straight through (size_warp_kernel, size_fallback).
 //
 // The reference runs, per candidate, two sequential bisections (pkg/analyzer/utils.go:26-70) of <= 102 model
 // solves each, then two Analyze calls.  The solves of one bisection depend on each other only through ONE
@@ -25,6 +28,49 @@
 namespace wva {
 
 constexpr int kSzMaxDepth = 5;  // midpoint tree depth: at most 31 evaluations per search per round
+
+struct SizeArgs {
+    DevFleet f;
+    const int* cand_pair;      // [n_cand] pair ids sorted by descending N
+    const int* cand_N;         // [n_cand]
+    int n_cand;
+    const double* tab;         // shared-format tables, one per candidate
+    const long long* tab_off;  // [n_cand]
+    AllocCols cand;            // [S*A]
+    int* fb_count;
+    int* fb_list;              // candidate indices that bailed
+    int fb_cap;
+};
+
+// The rounds' sort workspace and its item ordering kernels.
+struct SortWs {
+    unsigned* order;
+    unsigned long long* items;
+    unsigned long long* items_sorted;
+    unsigned* item_count;  // [0] items, [1..256] per class, [257..512] cursors
+};
+__global__ void __launch_bounds__(256) ws_items_scan(SortWs ws) {
+    __shared__ unsigned tot[kClasses];
+    tot[threadIdx.x] = ws.item_count[1 + threadIdx.x];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned acc = 0;
+        for (int c = 0; c < kClasses; ++c) {
+            ws.item_count[1 + kClasses + c] = acc;
+            acc += tot[c];
+        }
+    }
+}
+__global__ void __launch_bounds__(256) ws_items_scatter(SortWs ws) {
+    const unsigned n = *ws.item_count;
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long it = ws.items[i];
+    ws.items_sorted[agg_inc(ws.item_count + 1 + kClasses, (int)((it >> 40) & 0xff))] = it;
+}
+
+// candidate phase (rounds)
+enum { PH_SEARCH = 0, PH_WAIT_STAR = 1, PH_WAIT_FINAL = 2, PH_DONE = 3, PH_NIL = 4, PH_BAIL = 5 };
 
 enum { SZ2_START = 0, SZ2_WAIT_FIRST = 1, SZ2_WAIT_ITER = 2, SZ2_DONE = 3, SZ2_OFF = 4 };
 
@@ -62,6 +108,16 @@ struct Sz2Args {
     int fb_cap;
 };
 
+// ---------------------------------------------------------------------------
+// The decision pieces of CreateAllocation, shared by every driver.  They do not know where an evaluation ran: a
+// driver hands them {y, bail} per evaluated point, and a bail-out of a point they never consult is ignored.
+// ---------------------------------------------------------------------------
+struct SzPt {
+    float y;
+    bool bail;
+};
+enum { SZ_MORE = 0, SZ_DONE = 1, SZ_BAIL = 2 };
+
 __device__ __forceinline__ float sz_mid(float lo, float hi) { return __fmul_rn(0.5f, __fadd_rn(lo, hi)); }  // utils.go:55
 
 // Midpoint of heap node v (1-based) of the tree over (lo, hi): follow v's path bits below its leading one.
@@ -74,6 +130,127 @@ __device__ __forceinline__ float sz_node_value(int v, float lo, float hi) {
     return sz_mid(lo, hi);
 }
 
+// EvalTTFT (which = 0) / EvalITL (which = 1) from the solved model: queueanalyzer.go:270-290.
+__device__ __forceinline__ float target_value(const QParams& q, int which, int N, const ModelStats& st) {
+    const float eff = effective_concurrency(q, st.avg_serv_time, N);
+    return which == 0 ? __fadd_rn(st.avg_wait_time, prefill_time(q, eff)) : decode_time(q, eff);
+}
+
+// The start of CreateAllocation: RateRange and the bisection bounds.  nil: a model with K <= 1 is never valid
+// (queuemodel.go:31), negative targets fail TargetPerf.check (:322-329), and a bisection with lambda_min >
+// lambda_max returns an error before it evaluates anything (utils.go:29-31).
+struct SzStart {
+    float rmax, lmin, lmax;
+    bool nil;
+};
+__device__ __forceinline__ SzStart sz_start(const DevFleet& f, int s, int K, float s1, float sN) {
+    SzStart b;
+    b.rmax = rate_max_of(sN);
+    b.lmin = __fdiv_rn(rate_min_of(s1), 1000.0f);
+    b.lmax = __fdiv_rn(b.rmax, 1000.0f);
+    const float slo_ttft = f.srv_slo_ttft[s], slo_itl = f.srv_slo_itl[s], slo_tps = f.srv_slo_tps[s];
+    b.nil = K < 2 || slo_itl < 0.0f || slo_ttft < 0.0f || slo_tps < 0.0f ||
+            (b.lmin > b.lmax && (slo_ttft > 0.0f || slo_itl > 0.0f));
+    return b;
+}
+
+// One BinarySearch (utils.go:26-70).  xs = lambdaStar so far; ind < 0: "target is below the bounded region".
+struct SzSearch {
+    float lo, hi, xs;
+    int it, ind;
+    bool inc;
+};
+
+// The two boundary evaluations (utils.go:36-51); end(0) / end(1) = the points at lo / hi.  A bail-out at hi
+// counts only when the point at lo was not within tolerance.
+template <class End>
+__device__ __forceinline__ int sz_ends(SzSearch& S, float target, End&& end) {
+    const SzPt p0 = end(0);
+    if (p0.bail) return SZ_BAIL;
+    if (within_tolerance(p0.y, target, 1e-6f)) { S.xs = S.lo; return SZ_DONE; }
+    const SzPt p1 = end(1);
+    if (p1.bail) return SZ_BAIL;
+    if (within_tolerance(p1.y, target, 1e-6f)) { S.xs = S.hi; return SZ_DONE; }
+    const float y0 = p0.y, y1 = p1.y;
+    S.inc = y0 < y1;
+    if ((S.inc && target < y0) || (!S.inc && target > y0)) { S.xs = S.lo; S.ind = -1; return SZ_DONE; }
+    if ((S.inc && target > y1) || (!S.inc && target < y1)) { S.xs = S.hi; S.ind = 1; return SZ_DONE; }
+    return SZ_MORE;
+}
+
+// Up to D iterations of the bisection (utils.go:54-68) over a tree of evaluated midpoints: node(v) is the point
+// of heap node v over the current (lo, hi) (sz_node_value).
+template <class Node>
+__device__ __forceinline__ int sz_walk(SzSearch& S, float target, int D, Node&& node) {
+    int v = 1;
+    for (int level = 0; level < D; ++level) {
+        const SzPt p = node(v);
+        if (p.bail) return SZ_BAIL;
+        S.xs = sz_mid(S.lo, S.hi);
+        if (within_tolerance(p.y, target, 1e-6f)) return SZ_DONE;
+        const float pmin = S.lo, pmax = S.hi;
+        if ((S.inc && target < p.y) || (!S.inc && target > p.y)) { S.hi = S.xs; v = 2 * v; }
+        else { S.lo = S.xs; v = 2 * v + 1; }
+        ++S.it;
+        // fixed point of the float32 interval: the remaining iterations repeat this solve
+        if ((S.lo == pmin && S.hi == pmax) || S.it >= 100) return SZ_DONE;
+    }
+    return SZ_MORE;
+}
+
+// Analyze's rate check (queueanalyzer.go:135-143): false when it rejects the rate, else the lambda it solves at.
+__device__ __forceinline__ bool sz_gate(float rate, float rmax, float& lam) {
+    if (rate <= 0.0f || rate > rmax) return false;
+    lam = __fdiv_rn(rate, 1000.0f);
+    return true;
+}
+
+// queueanalyzer.go:231-241: lambda = min(lambdaStarTTFT, lambdaStarITL, lambdaStarTPS), then Analyze's check.
+__device__ __forceinline__ bool sz_lambda(const DevFleet& f, int s, float rmax, float xs_ttft, float xs_itl,
+                                          float& lam) {
+    const float lmax = __fdiv_rn(rmax, 1000.0f);
+    float l_tps = lmax;
+    if (f.srv_slo_tps[s] > 0.0f) l_tps = __fmul_rn(lmax, __fsub_rn(1.0f, 0.1f));
+    return sz_gate(__fmul_rn(go_minf(go_minf(xs_ttft, xs_itl), l_tps), 1000.0f), rmax, lam);
+}
+
+// allocation.go:134-153: replicas and cost for the throughput rate_star, then Analyze's check of the final rate.
+struct SzReplicas {
+    long long nrep;
+    float cost;
+};
+__device__ __forceinline__ bool sz_replicas(const DevFleet& f, int s, int a, float rmax, float rate_star,
+                                            SzReplicas& r, float& lam) {
+    const float total_rate = total_rate_of(f, s);
+    r.nrep = go_f64_to_int(ceil(__ddiv_rn((double)total_rate, (double)rate_star)));
+    const long long min_rep = f.srv_min_replicas[s];
+    if (r.nrep < min_rep) r.nrep = min_rep;
+    const long long total = (long long)num_instances(f, f.srv_model[s], a) * r.nrep;
+    r.cost = __fmul_rn(f.acc_cost[a], (float)total);
+    return sz_gate(__fdiv_rn(total_rate, (float)r.nrep), rmax, lam);
+}
+
+// The feasible allocation (allocation.go:155-163); value = cost.
+__device__ __forceinline__ Cand sz_cand(int a, int N, const SzReplicas& r, float rate_star, float ttft, float itl,
+                                        float rho) {
+    Cand c = cand_nil();
+    c.feasible = 1;
+    c.acc = a;
+    c.replicas = (int)r.nrep;
+    c.batch = N;
+    c.cost = r.cost;
+    c.value = r.cost;
+    c.itl = itl;
+    c.ttft = ttft;
+    c.rho = rho;
+    c.max_rate = __fdiv_rn(rate_star, 1000.0f);
+    return c;
+}
+
+// ---------------------------------------------------------------------------
+// The rounds (more than WVA_SIZE_SMALL_MAX candidates): one thread per candidate keeps the search state in global
+// columns between rounds; both searches of a candidate emit their trees in the same round.
+// ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= g.n_cand) return;
@@ -82,29 +259,25 @@ __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
     const int N = g.cand_N[j], K = N + N * f.ratio;
     const double* tab = g.tab + 4 * g.tab_off[j];
     const float s1 = (float)tab[0], sN = (float)tab[4 * (N - 1)];
-    const float rmin = rate_min_of(s1), rmax = rate_max_of(sN);
-    g.rmax[j] = rmax;
+    const SzStart b = sz_start(f, s, K, s1, sN);
+    g.rmax[j] = b.rmax;
     g.l2s0[j] = log2f(s1);
     g.l2sN[j] = log2f(sN);
     g.lsN[j] = (g.ls + g.tab_off[j] + j)[N - 1];
-    const float slo_ttft = f.srv_slo_ttft[s], slo_itl = f.srv_slo_itl[s], slo_tps = f.srv_slo_tps[s];
-    uint8_t ph = PH_SEARCH;
-    // K <= 1: the model is never valid (queuemodel.go:31); negative targets: TargetPerf.check :322-329
-    if (K < 2 || slo_itl < 0.0f || slo_ttft < 0.0f || slo_tps < 0.0f) ph = PH_NIL;
-    g.phase[j] = ph;
-    const float lmin = __fdiv_rn(rmin, 1000.0f), lmax = __fdiv_rn(rmax, 1000.0f);
+    g.phase[j] = b.nil ? PH_NIL : PH_SEARCH;
     for (int w = 0; w < 2; ++w) {
-        const float target = w == 0 ? slo_ttft : slo_itl;
-        g.xmin[2 * j + w] = lmin;
-        g.xmax[2 * j + w] = lmax;
-        g.xs[2 * j + w] = lmax;  // lambdaStar when the target is disabled (queueanalyzer.go:205,218)
+        const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+        g.xmin[2 * j + w] = b.lmin;
+        g.xmax[2 * j + w] = b.lmax;
+        g.xs[2 * j + w] = b.lmax;  // lambdaStar when the target is disabled (queueanalyzer.go:205,218)
         g.sst[2 * j + w] = target > 0.0f ? SZ2_START : SZ2_OFF;
         g.ind[2 * j + w] = 0;
+        g.inc[2 * j + w] = 0;
         g.iter[2 * j + w] = 0;
         g.slot[2 * j + w] = -1;
     }
     g.aslot[j] = -1;
-    if (ph == PH_NIL) store_cand(g.cand, pair, cand_nil());
+    if (b.nil) store_cand(g.cand, pair, cand_nil());
 }
 
 // Advance every candidate: consume last round's results (walking the midpoint trees with the reference's
@@ -134,65 +307,35 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
     if (live_in) {
         if (ph == PH_SEARCH) {
             bool all_done = true, nil = false, bail = false;
-            for (int w = 0; w < 2 && !bail && !nil; ++w) {
+            for (int w = 0; w < 2; ++w) {
                 const int k = 2 * j + w;
                 int st = g.sst[k];
                 if (st == SZ2_DONE || st == SZ2_OFF) continue;
                 const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
                 float lo = g.xmin[k], hi = g.xmax[k];
-                bool searching = true;
-                if (st == SZ2_START) {  // utils.go:29-31
-                    if (lo > hi) { nil = true; break; }
+                if (st == SZ2_START) {
                     emit_ends[w] = true;
                     st = SZ2_WAIT_FIRST;
-                } else {
-                    int base = g.slot[k];
-                    bool inc = g.inc[k] != 0;
-                    if (st == SZ2_WAIT_FIRST) {  // utils.go:36-51: the two boundary evaluations
-                        if (g.req_bail[base]) { bail = true; break; }
-                        const float y0 = g.req_out[base].x;
-                        if (within_tolerance(y0, target, 1e-6f)) { g.xs[k] = lo; searching = false; }
-                        else {
-                            if (g.req_bail[base + 1]) { bail = true; break; }
-                            const float y1 = g.req_out[base + 1].x;
-                            if (within_tolerance(y1, target, 1e-6f)) { g.xs[k] = hi; searching = false; }
-                            else {
-                                inc = y0 < y1;
-                                g.inc[k] = inc;
-                                if ((inc && target < y0) || (!inc && target > y0)) { g.xs[k] = lo; g.ind[k] = -1; searching = false; }
-                                else if ((inc && target > y1) || (!inc && target < y1)) { g.xs[k] = hi; g.ind[k] = 1; searching = false; }
-                            }
-                        }
-                        base += 2;
-                        st = SZ2_WAIT_ITER;
-                    }
-                    if (searching) {  // utils.go:54-68, D iterations: walk the tree of midpoints evaluated last round
-                        int it = g.iter[k];
-                        int v = 1;
-                        for (int level = 0; level < D; ++level) {
-                            const float xs = sz_mid(lo, hi);
-                            if (g.req_bail[base + v - 1]) { bail = true; break; }
-                            const float y = g.req_out[base + v - 1].x;
-                            g.xs[k] = xs;
-                            if (within_tolerance(y, target, 1e-6f)) { searching = false; break; }
-                            const float pmin = lo, pmax = hi;
-                            if ((inc && target < y) || (!inc && target > y)) { hi = xs; v = 2 * v; }
-                            else { lo = xs; v = 2 * v + 1; }
-                            ++it;
-                            // fixed point of the float32 interval: the remaining iterations repeat this solve
-                            if ((lo == pmin && hi == pmax) || it >= 100) { searching = false; break; }
-                        }
-                        if (bail) break;
-                        g.iter[k] = (uint8_t)it;
-                        g.xmin[k] = lo;
-                        g.xmax[k] = hi;
-                    }
-                    if (!searching) st = SZ2_DONE;
+                } else {  // last round's points: the two end points (first round only), then the tree
+                    SzSearch S{lo, hi, g.xs[k], g.iter[k], g.ind[k], g.inc[k] != 0};
+                    const int base = g.slot[k];
+                    auto at = [&](int i) { return SzPt{g.req_out[base + i].x, g.req_bail[base + i] != 0}; };
+                    int r = SZ_MORE;
+                    const int nodes = st == SZ2_WAIT_FIRST ? 2 : 0;
+                    if (st == SZ2_WAIT_FIRST) r = sz_ends(S, target, at);
+                    if (r == SZ_MORE) r = sz_walk(S, target, D, [&](int v) { return at(nodes + v - 1); });
+                    if (r == SZ_BAIL) { bail = true; break; }
+                    if (r == SZ_DONE && S.ind < 0) { nil = true; break; }  // "target is below the bounded region"
+                    g.xmin[k] = lo = S.lo;
+                    g.xmax[k] = hi = S.hi;
+                    g.xs[k] = S.xs;
+                    g.iter[k] = (uint8_t)S.it;
+                    g.ind[k] = (int8_t)S.ind;
+                    g.inc[k] = S.inc;
+                    st = r == SZ_DONE ? SZ2_DONE : SZ2_WAIT_ITER;
                 }
                 g.sst[k] = (uint8_t)st;
-                if (st == SZ2_DONE) {
-                    if (g.ind[k] < 0) { nil = true; break; }  // "target is below the bounded region"
-                } else {
+                if (st != SZ2_DONE) {
                     emit_n[w] = M + (emit_ends[w] ? 2 : 0);
                     emit_lo[w] = lo;
                     emit_hi[w] = hi;
@@ -202,14 +345,8 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
             if (bail) ph = PH_BAIL;
             else if (nil) ph = PH_NIL;
             else if (all_done) {
-                // queueanalyzer.go:231-241: lambda = min(lambdaStarTTFT, lambdaStarITL, lambdaStarTPS)
-                const float lmax = __fdiv_rn(rmax, 1000.0f);
-                float l_tps = lmax;
-                if (f.srv_slo_tps[s] > 0.0f) l_tps = __fmul_rn(lmax, __fsub_rn(1.0f, 0.1f));
-                const float lambda = go_minf(go_minf(g.xs[2 * j], g.xs[2 * j + 1]), l_tps);
-                const float rate = __fmul_rn(lambda, 1000.0f);
-                if (rate <= 0.0f || rate > rmax) ph = PH_NIL;  // Analyze: :135-143
-                else { an_kind = 2; an_lambda = __fdiv_rn(rate, 1000.0f); ph = PH_WAIT_STAR; }
+                if (!sz_lambda(f, s, rmax, g.xs[2 * j], g.xs[2 * j + 1], an_lambda)) ph = PH_NIL;
+                else { an_kind = 2; ph = PH_WAIT_STAR; }
             }
             if (ph != PH_SEARCH) emit_n[0] = emit_n[1] = 0;
         } else if (ph == PH_WAIT_STAR) {
@@ -217,35 +354,21 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
             if (g.req_bail[slot]) ph = PH_BAIL;
             else {
                 const float rate_star = g.req_out[slot].x;  // metrics.Throughput
-                const float total_rate = total_rate_of(f, s);  // allocation.go:134-141
-                long long nrep = go_f64_to_int(ceil(__ddiv_rn((double)total_rate, (double)rate_star)));
-                const long long min_rep = f.srv_min_replicas[s];
-                if (nrep < min_rep) nrep = min_rep;
-                const long long total = (long long)num_instances(f, f.srv_model[s], a) * nrep;
+                SzReplicas r;
+                const bool ok = sz_replicas(f, s, a, rmax, rate_star, r, an_lambda);
                 g.rate_star[j] = rate_star;
-                g.nrep[j] = nrep;
-                g.cost[j] = __fmul_rn(f.acc_cost[a], (float)total);
-                const float rate = __fdiv_rn(total_rate, (float)nrep);  // :148-153
-                if (rate <= 0.0f || rate > rmax) ph = PH_NIL;
-                else { an_kind = 3; an_lambda = __fdiv_rn(rate, 1000.0f); ph = PH_WAIT_FINAL; }
+                g.nrep[j] = r.nrep;
+                g.cost[j] = r.cost;
+                if (!ok) ph = PH_NIL;
+                else { an_kind = 3; ph = PH_WAIT_FINAL; }
             }
         } else {  // PH_WAIT_FINAL
             const int slot = g.aslot[j];
             if (g.req_bail[slot]) ph = PH_BAIL;
             else {
                 const float4 m = g.req_out[slot];
-                Cand c = cand_nil();
-                c.feasible = 1;
-                c.acc = a;
-                c.replicas = (int)g.nrep[j];
-                c.batch = g.cand_N[j];
-                c.cost = g.cost[j];
-                c.value = c.cost;
-                c.itl = m.z;
-                c.ttft = m.y;
-                c.rho = m.w;
-                c.max_rate = __fdiv_rn(g.rate_star[j], 1000.0f);
-                store_cand(g.cand, pair, c);
+                const SzReplicas r{g.nrep[j], g.cost[j]};
+                store_cand(g.cand, pair, sz_cand(a, g.cand_N[j], r, g.rate_star[j], m.y, m.z, m.w));
                 ph = PH_DONE;
             }
         }
@@ -376,147 +499,14 @@ __global__ void __launch_bounds__(256, 4) sz2_solve(Sz2Args g) {
     if (rc != kSolveOk) return;
     const QParams q = qparams_of(f, pair / f.A, pair % f.A);
     float4 out;
-    if (kind <= 1) {  // EvalTTFT / EvalITL: queueanalyzer.go:270-290
-        const float eff = effective_concurrency(q, st.avg_serv_time, N);
-        out.x = kind == 0 ? __fadd_rn(st.avg_wait_time, prefill_time(q, eff)) : decode_time(q, eff);
+    if (kind <= 1) {  // EvalTTFT / EvalITL
+        out.x = target_value(q, kind, N, st);
         out.y = out.z = out.w = 0.0f;
     } else {  // Analyze: :152-172
         const Metrics m = metrics_from(q, N, st);
         out = make_float4(m.throughput, m.ttft, m.avg_token_time, m.rho);
     }
     g.req_out[slot] = out;
-}
-
-// ---------------------------------------------------------------------------
-// Small fleets (BASELINE configs[0]: one VariantAutoscaling = one candidate): ONE warp per candidate runs the whole
-// CreateAllocation in one launch — the same speculative midpoint trees, but evaluated by the warp's lanes (round one:
-// the two end points + 15 midpoints = 4 iterations; later rounds: 31 midpoints = 5 iterations) and walked in
-// registers with warp shuffles.  No rounds, no sort, no host round trip: a reconcile of a handful of variants is
-// three launches (trivial, this, unlimited argmin) instead of sixty.  Same lambdas, same solves, same comparisons
-// as the round-based path and the reference.
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ float sz_eval(const QParams& q, int which, const double* tab, int N, int K, float x, int& bail) {
-    ModelStats st;
-    if (solve_shared(tab, N, K, x, st) != kSolveOk) { bail = 1; return 0.0f; }
-    const float eff = effective_concurrency(q, st.avg_serv_time, N);  // queueanalyzer.go:270-290
-    return which == 0 ? __fadd_rn(st.avg_wait_time, prefill_time(q, eff)) : decode_time(q, eff);
-}
-__global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g, const double* __restrict__ tabs,
-                                                        const long long* __restrict__ tab_off) {
-    const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
-    const int lane = threadIdx.x & 31;
-    if (j >= g.n_cand) return;
-    const DevFleet& f = g.f;
-    const int pair = g.cand_pair[j], s = pair / f.A, a = pair % f.A;
-    const int N = g.cand_N[j], K = N + N * f.ratio;
-    const double* tab = tabs + 4 * tab_off[j];
-    const QParams q = qparams_of(f, s, a);
-    const float rmin = rate_min_of((float)tab[0]), rmax = rate_max_of((float)tab[4 * (N - 1)]);
-    const float slo_ttft = f.srv_slo_ttft[s], slo_itl = f.srv_slo_itl[s], slo_tps = f.srv_slo_tps[s];
-    bool nil = K < 2 || slo_itl < 0.0f || slo_ttft < 0.0f || slo_tps < 0.0f;  // queuemodel.go:31, TargetPerf.check
-    bool bail = false;
-    const float lmin = __fdiv_rn(rmin, 1000.0f), lmax = __fdiv_rn(rmax, 1000.0f);
-    float xstar[2] = {lmax, lmax};  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
-    for (int w = 0; w < 2 && !nil && !bail; ++w) {
-        const float target = w == 0 ? slo_ttft : slo_itl;
-        if (!(target > 0.0f)) continue;
-        float lo = lmin, hi = lmax;
-        if (lo > hi) { nil = true; break; }  // utils.go:29-31
-        bool first = true, searching = true, inc = false;
-        int it = 0, ind = 0;
-        float xs = 0.0f;
-        while (searching && !bail) {
-            // this lane's evaluation point: round one = {xmin, xmax, nodes 1..15}, later rounds = nodes 1..31
-            const int D = first ? 4 : 5;
-            const int v_mine = first ? lane - 1 : lane + 1;
-            const bool has = first ? lane < 17 : lane < 31;
-            float x = lo;
-            if (first && lane == 1) x = hi;
-            if (has && !(first && lane < 2)) x = sz_node_value(v_mine, lo, hi);
-            float y = 0.0f;
-            int b = 0;
-            if (has) y = sz_eval(q, w, tab, N, K, x, b);
-            __syncwarp();
-            if (first) {  // utils.go:36-51: the two boundary evaluations
-                const float y0 = __shfl_sync(0xffffffffu, y, 0), y1 = __shfl_sync(0xffffffffu, y, 1);
-                const int b0 = __shfl_sync(0xffffffffu, b, 0), b1 = __shfl_sync(0xffffffffu, b, 1);
-                if (b0) { bail = true; break; }
-                if (within_tolerance(y0, target, 1e-6f)) { xs = lo; searching = false; }
-                else {
-                    if (b1) { bail = true; break; }
-                    if (within_tolerance(y1, target, 1e-6f)) { xs = hi; searching = false; }
-                    else {
-                        inc = y0 < y1;
-                        if ((inc && target < y0) || (!inc && target > y0)) { xs = lo; ind = -1; searching = false; }
-                        else if ((inc && target > y1) || (!inc && target < y1)) { xs = hi; ind = 1; searching = false; }
-                    }
-                }
-            }
-            if (searching) {  // utils.go:54-68, D iterations over the evaluated tree
-                int v = 1;
-                for (int level = 0; level < D; ++level) {
-                    const int src = first ? v + 1 : v - 1;  // the lane that evaluated node v
-                    const float yv = __shfl_sync(0xffffffffu, y, src);
-                    const int bv = __shfl_sync(0xffffffffu, b, src);
-                    xs = sz_mid(lo, hi);
-                    if (bv) { bail = true; break; }
-                    if (within_tolerance(yv, target, 1e-6f)) { searching = false; break; }
-                    const float pmin = lo, pmax = hi;
-                    if ((inc && target < yv) || (!inc && target > yv)) { hi = xs; v = 2 * v; }
-                    else { lo = xs; v = 2 * v + 1; }
-                    ++it;
-                    if ((lo == pmin && hi == pmax) || it >= 100) { searching = false; break; }
-                }
-            }
-            first = false;
-        }
-        xstar[w] = xs;
-        if (ind < 0) nil = true;  // "target is below the bounded region"
-    }
-    Cand out = cand_nil();
-    if (!nil && !bail) {
-        // queueanalyzer.go:231-241, allocation.go:134-163 — every lane computes the same values
-        float l_tps = lmax;
-        if (slo_tps > 0.0f) l_tps = __fmul_rn(lmax, __fsub_rn(1.0f, 0.1f));
-        const float lambda = go_minf(go_minf(xstar[0], xstar[1]), l_tps);
-        const float rate0 = __fmul_rn(lambda, 1000.0f);
-        ModelStats st;
-        if (rate0 <= 0.0f || rate0 > rmax) nil = true;
-        else if (solve_shared(tab, N, K, __fdiv_rn(rate0, 1000.0f), st) != kSolveOk) bail = true;
-        else {
-            const float rate_star = metrics_from(q, N, st).throughput;
-            const float total_rate = total_rate_of(f, s);
-            long long nrep = go_f64_to_int(ceil(__ddiv_rn((double)total_rate, (double)rate_star)));
-            const long long min_rep = f.srv_min_replicas[s];
-            if (nrep < min_rep) nrep = min_rep;
-            const long long total = (long long)num_instances(f, f.srv_model[s], a) * nrep;
-            const float cost = __fmul_rn(f.acc_cost[a], (float)total);
-            const float rate = __fdiv_rn(total_rate, (float)nrep);
-            if (rate <= 0.0f || rate > rmax) nil = true;
-            else if (solve_shared(tab, N, K, __fdiv_rn(rate, 1000.0f), st) != kSolveOk) bail = true;
-            else {
-                const Metrics m = metrics_from(q, N, st);
-                out.feasible = 1;
-                out.acc = a;
-                out.replicas = (int)nrep;
-                out.batch = N;
-                out.cost = cost;
-                out.value = cost;
-                out.itl = m.avg_token_time;
-                out.ttft = m.ttft;
-                out.rho = m.rho;
-                out.max_rate = __fdiv_rn(rate_star, 1000.0f);
-            }
-        }
-    }
-    if (lane == 0) {
-        if (bail) {
-            const int k = atomicAdd(g.fb_count, 1);
-            if (k < g.fb_cap) g.fb_list[k] = j;
-            out = cand_nil();
-        }
-        store_cand(g.cand, pair, out);
-    }
 }
 
 // Per-round reset of the device counters (one tiny kernel instead of two memsets; part of the captured round).
@@ -527,6 +517,168 @@ __global__ void sz2_round_reset(Sz2Args g) {
         *g.n_live = 0;
     }
     if (i < 2 * kClasses + 1) g.ws.item_count[i] = 0;
+}
+
+// ---------------------------------------------------------------------------
+// CreateAllocation (allocation.go:77-163) straight through, for one candidate.  Eval evaluates the points:
+//   round(which, lo, hi, first)  the points of one round of the search `which` over (lo, hi): the two end points
+//                                (first round only) and the midpoint tree of depth depth()
+//   end(i), node(v)              {y, bail} of end point i / tree node v of the last round
+//   solve(lambda, st)            Model.Solve for Analyze; false when it bailed
+// Returns false when a consulted solve bailed (out is then nil).
+// ---------------------------------------------------------------------------
+template <class Eval>
+__device__ __forceinline__ bool create_allocation(const DevFleet& f, int s, int a, int N, int K, float s1, float sN,
+                                                  Eval& ev, Cand& out) {
+    out = cand_nil();
+    const SzStart b = sz_start(f, s, K, s1, sN);
+    if (b.nil) return true;
+    float xs_ttft = b.lmax, xs_itl = b.lmax;  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
+    for (int w = 0; w < 2; ++w) {
+        const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+        if (!(target > 0.0f)) continue;
+        SzSearch S{b.lmin, b.lmax, 0.0f, 0, 0, false};
+        ev.round(w, S.lo, S.hi, true);
+        int r = sz_ends(S, target, [&](int i) { return ev.end(i); });
+        while (r == SZ_MORE) {
+            r = sz_walk(S, target, ev.depth(), [&](int v) { return ev.node(v); });
+            if (r == SZ_MORE) ev.round(w, S.lo, S.hi, false);
+        }
+        if (r == SZ_BAIL) return false;
+        if (S.ind < 0) return true;
+        (w == 0 ? xs_ttft : xs_itl) = S.xs;
+    }
+    float lam;
+    ModelStats st;
+    if (!sz_lambda(f, s, b.rmax, xs_ttft, xs_itl, lam)) return true;
+    if (!ev.solve(lam, st)) return false;
+    const float rate_star = metrics_from(ev.q, N, st).throughput;
+    SzReplicas r;
+    if (!sz_replicas(f, s, a, b.rmax, rate_star, r, lam)) return true;
+    if (!ev.solve(lam, st)) return false;
+    const Metrics m = metrics_from(ev.q, N, st);
+    out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
+    return true;
+}
+
+// ---------------------------------------------------------------------------
+// Small fleets (BASELINE configs[0]: one VariantAutoscaling = one candidate): ONE warp per candidate runs
+// create_allocation in one launch — the same speculative midpoint trees as the rounds, but evaluated by the warp's
+// lanes (round one: the two end points + 15 midpoints = 4 iterations; later rounds: 31 midpoints = 5 iterations)
+// and read with warp shuffles.  No rounds, no sort, no host round trip: a reconcile of a handful of variants is
+// three launches (trivial, this, unlimited argmin) instead of sixty.  Every lane computes the same decisions.
+// ---------------------------------------------------------------------------
+struct WarpEval {
+    const double* tab;
+    QParams q;
+    int N, K, lane;
+    bool first;
+    float y;  // this lane's point
+    int bail;
+    __device__ __forceinline__ int depth() const { return first ? 4 : 5; }
+    __device__ __forceinline__ void round(int which, float lo, float hi, bool first_round) {
+        first = first_round;
+        // this lane's point: round one = {lo, hi, nodes 1..15}, later rounds = nodes 1..31
+        const bool has = first ? lane < 17 : lane < 31;
+        float x = first && lane == 1 ? hi : lo;
+        if (has && !(first && lane < 2)) x = sz_node_value(first ? lane - 1 : lane + 1, lo, hi);
+        y = 0.0f;
+        bail = 0;
+        ModelStats st;
+        if (has && !solve(x, st)) bail = 1;
+        else if (has) y = target_value(q, which, N, st);
+        __syncwarp();
+    }
+    __device__ __forceinline__ SzPt at(int src) const {
+        return SzPt{__shfl_sync(0xffffffffu, y, src), __shfl_sync(0xffffffffu, bail, src) != 0};
+    }
+    __device__ __forceinline__ SzPt end(int i) const { return at(i); }
+    __device__ __forceinline__ SzPt node(int v) const { return at(first ? v + 1 : v - 1); }
+    __device__ __forceinline__ bool solve(float lambda, ModelStats& st) const {
+        return solve_shared(tab, N, K, lambda, st) == kSolveOk;
+    }
+};
+
+__global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) {
+    const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (j >= g.n_cand) return;
+    const DevFleet& f = g.f;
+    const int pair = g.cand_pair[j], s = pair / f.A, a = pair % f.A;
+    const int N = g.cand_N[j], K = N + N * f.ratio;
+    WarpEval ev;
+    ev.tab = g.tab + 4 * g.tab_off[j];
+    ev.q = qparams_of(f, s, a);
+    ev.N = N;
+    ev.K = K;
+    ev.lane = lane;
+    Cand c;
+    const bool ok = create_allocation(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
+    if (lane == 0) {
+        if (!ok) {
+            const int k = atomicAdd(g.fb_count, 1);
+            if (k < g.fb_cap) g.fb_list[k] = j;
+        }
+        store_cand(g.cand, pair, c);
+    }
+}
+
+// ---------------------------------------------------------------------------
+// Stored-vector re-run of the candidates that bailed (slot k handles list entries k, k + n_slots, ..): one thread
+// per candidate evaluates exactly the reference's points, one at a time, with the literal restatement solve_stored
+// on its scratch slot (p[0..Kmax], then servRate[0..N-1] as float32).
+// ---------------------------------------------------------------------------
+struct StoredEval {
+    double* p;
+    const float* sr;
+    QParams q;
+    int N, K;
+    int rc;  // solve_stored's code of the last solve
+    int which;
+    float lo, hi;
+    __device__ __forceinline__ int depth() const { return 1; }
+    __device__ __forceinline__ void round(int w, float l, float h, bool) {
+        which = w;
+        lo = l;
+        hi = h;
+    }
+    __device__ __forceinline__ SzPt at(float x) {
+        ModelStats st;
+        if (!solve(x, st)) return SzPt{0.0f, true};
+        return SzPt{target_value(q, which, N, st), false};
+    }
+    __device__ __forceinline__ SzPt end(int i) { return at(i ? hi : lo); }
+    __device__ __forceinline__ SzPt node(int) { return at(sz_mid(lo, hi)); }
+    __device__ __forceinline__ bool solve(float lambda, ModelStats& st) {
+        rc = solve_stored(p, sr, N, K, lambda, st);
+        return rc == 0;
+    }
+};
+
+__global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+    const DevFleet& f = g.f;
+    const int n_slots = gridDim.x * blockDim.x;
+    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+    int n = *g.fb_count;
+    if (n > g.fb_cap) n = g.fb_cap;
+    StoredEval ev;
+    ev.p = scratch + (size_t)slot * slot_doubles;
+    float* sr = (float*)(ev.p + Kmax + 1);
+    ev.sr = sr;
+    for (int k = slot; k < n; k += n_slots) {
+        const int j = g.fb_list[k];
+        const int pair = g.cand_pair[j];
+        const int s = pair / f.A, a = pair % f.A;
+        const int N = g.cand_N[j];
+        const double* tab = g.tab + 4 * g.tab_off[j];
+        for (int i = 0; i < N; ++i) sr[i] = (float)tab[4 * i];
+        ev.q = qparams_of(f, s, a);
+        ev.N = N;
+        ev.K = N + N * f.ratio;
+        Cand c;
+        if (!create_allocation(f, s, a, N, ev.K, sr[0], sr[N - 1], ev, c)) atomicExch(fb_status, ev.rc);
+        store_cand(g.cand, pair, c);
+    }
 }
 
 }  // namespace wva
