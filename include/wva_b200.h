@@ -229,6 +229,30 @@ int wva_grid_solve(wva_handle *h, const wva_fleet *fleet, const wva_grid *grid,
                    wva_cells *cells, wva_allocs *winners);
 
 /*
+ * Size grid: Server.Calculate (the reference's CreateAllocation rule, as in wva_analyze) once per listed
+ * batch size, and the min-value (accelerator, batch size) per server.
+ *
+ * Candidate (s, a, bi), index (s*A + a)*n_batch + bi, is exactly what wva_analyze returns for (s, a) on the
+ * same fleet with every server's srv_max_batch set to batch[bi]: N = batch[bi], the queue size is
+ * max_queue_to_batch_ratio * N, and a zero-load candidate uses N in zeroLoadAllocation.  perf_max_batch,
+ * perf_at_tokens and srv_max_batch are not read.  The candidate rule (keepAccelerator), the gates and
+ * value = TransitionPenalty(current, candidate) are those of wva_analyze.
+ *
+ * winners[s] is the feasible candidate of server s with the smallest value under SolveUnlimited's rule
+ * (strict '<' starting from MaxFloat32: a NaN value, or one not below MaxFloat32, never wins); ties go to
+ * the smaller batch size, then the lower accelerator id.  With one batch size this is wva_solve's winner.
+ * Repeated batch sizes give identical records.  Like wva_grid_solve, the minimum does not read
+ * fleet->unlimited or the capacities.  The winners stay resident for wva_summarize.
+ *
+ * `candidates` (S*A*n_batch entries) may be NULL; `winners` has S entries.  n_batch == 0 is valid (every
+ * winner is nil).  WVA_ERR_BAD_ARG: n_batch < 0, batch NULL with n_batch > 0, or a batch size outside
+ * [1, 2^20].  WVA_ERR_UNSUPPORTED: S*A*n_batch >= 2^31, or, as for wva_solve, too many candidates need the
+ * stored-vector fallback or its rescale loop would not terminate.
+ */
+int wva_size_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_batch, const int32_t *batch,
+                  wva_allocs *candidates, wva_allocs *winners);
+
+/*
  * Solver.SolveGreedy + the best-effort saturation policies (pkg/solver/greedy.go:35-341) over a candidate
  * table the caller already holds: `candidates` (S*A, value = transition penalty as wva_analyze returns it) is
  * read, and modified where the reference scales best-effort allocations; `winners` (S) is written.  Host only
@@ -274,7 +298,7 @@ typedef struct wva_summary {
     float *diff_cost;
 } wva_summary;
 
-/* Summary of the most recent wva_solve / wva_resolve / wva_grid_solve on this handle (the winners
+/* Summary of the most recent wva_solve / wva_resolve / wva_grid_solve / wva_size_grid on this handle (the winners
  * stay resident until the next call).  WVA_ERR_STATE when there is none. */
 int wva_summarize(wva_handle *h, wva_summary *out);
 

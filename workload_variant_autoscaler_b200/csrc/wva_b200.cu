@@ -174,6 +174,15 @@ struct wva_handle {
     DevBuf d_sz_tab, d_sz_ls, d_sz_off, d_sz_state, d_sz_req, d_sz_sort;
     PinBuf sz_pin;
 
+    // size-grid caches: buffers of their own, so that wva_solve's size cache above stays valid
+    uint64_t sg_epoch = ~0ull;
+    std::vector<int> sg_batch;
+    int sg_n = 0, sg_Bmax = 1;
+    // byte offsets in d_sg_lists of the candidate columns (pair, N, record, table index, table offset) and the
+    // batch list
+    size_t sg_pair = 0, sg_N = 0, sg_rec = 0, sg_idx = 0, sg_off = 0, sg_bl = 0;
+    DevBuf d_sg_lists, d_sg_tab, d_sg_ls;
+
     // grid path caches
     uint64_t grid_epoch = ~0ull;
     std::vector<int> grid_batch, grid_replicas;
@@ -414,6 +423,7 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     const int D = size_depth_for(n);
     const size_t per_cand = 2 * ((size_t)(1 << D) - 1 + 2);  // two searches: a tree each, plus the two end points
     const size_t cap = per_cand * (size_t)n;                 // requests per round, worst case
+    if (cap >= 0xffffffffull) return h->fail(WVA_ERR_UNSUPPORTED, "too many size candidates for one call (request slots are 32-bit)");
     const size_t n2 = 2 * (size_t)n;
     // state block
     Cols st(16);
@@ -449,7 +459,8 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     g.depth = D;
     g.tab = sa.tab;
     g.tab_off = sa.tab_off;
-    g.ls = (const float*)h->d_sz_ls.p;
+    g.ls = sa.ls;
+    g.place = sa.place;
     g.xmin = (float*)(sp + o_xmin); g.xmax = (float*)(sp + o_xmax); g.xs = (float*)(sp + o_xs);
     g.sst = (uint8_t*)(sp + o_sst); g.inc = (uint8_t*)(sp + o_inc); g.iter = (uint8_t*)(sp + o_iter);
     g.ind = (int8_t*)(sp + o_ind); g.slot = (int*)(sp + o_slot);
@@ -496,27 +507,10 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     return WVA_OK;
 }
 
-// Enqueue analyze (+ unlimited solve). cand/winner columns are device pointers.
-int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners) {
-    int rc = prepare_size(h);
-    if (rc) return rc;
-    rc = ensure_ctrl(h);
-    if (rc) return rc;
-    const HostFleet& hf = h->hf;
-    const int n_pairs = hf.S * hf.A;
-    const int n = (int)h->cand_pair.size();
-    if (n_pairs > 0) {
-        trivial_kernel<<<(n_pairs + 255) / 256, 256, 0, h->stream>>>(h->df, cand);
-        h->launches++;
-    }
-    SizeArgs g{};
-    g.f = h->df;
-    g.cand_pair = (const int*)h->d_cand_pair.p;
-    g.cand_N = (const int*)h->d_cand_N.p;
-    g.n_cand = n;
-    g.tab = (const double*)h->d_sz_tab.p;
-    g.tab_off = (const long long*)h->d_sz_off.p;
-    g.cand = cand;
+// CreateAllocation for the load candidates g lists (g.cand_pair .. g.place set, batch sizes at most Nmax): the
+// warp-per-candidate kernel or the rounds, timed as the call's kernel, then the stored-vector fallback.
+int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax) {
+    const int n = g.n_cand;
     g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
     CK(h->d_fb_list.ensure(sizeof(int) * std::max(n, 1)));
     g.fb_list = (int*)h->d_fb_list.p;
@@ -528,19 +522,47 @@ int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners)
         size_warp_kernel<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
         h->launches++;
     } else if (n > 0) {
-        rc = run_size_rounds(h, g, n);
+        const int rc = run_size_rounds(h, g, n);
         if (rc) return rc;
     }
     CK(cudaEventRecord(h->ev_k1, h->stream));
     if (n > 0) {
         size_t slot_doubles;
         int Kmax;
-        rc = ensure_scratch(h, h->size_Nmax, hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
+        const int rc = ensure_scratch(h, Nmax, h->hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
         if (rc) return rc;
         size_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
                                                                (int*)h->d_ctrl.p + CTRL_FB_STATUS);
         h->launches++;
     }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// Enqueue analyze (+ unlimited solve). cand/winner columns are device pointers.
+int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners) {
+    int rc = prepare_size(h);
+    if (rc) return rc;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const HostFleet& hf = h->hf;
+    const int n_pairs = hf.S * hf.A;
+    if (n_pairs > 0) {
+        trivial_kernel<<<(n_pairs + 255) / 256, 256, 0, h->stream>>>(h->df, cand, nullptr, 1);
+        h->launches++;
+    }
+    SizeArgs g{};
+    g.f = h->df;
+    g.cand_pair = (const int*)h->d_cand_pair.p;
+    g.cand_N = (const int*)h->d_cand_N.p;
+    g.n_cand = (int)h->cand_pair.size();
+    g.tab = (const double*)h->d_sz_tab.p;
+    g.tab_off = (const long long*)h->d_sz_off.p;
+    g.ls = (const float*)h->d_sz_ls.p;
+    g.place = CandPlace{nullptr, nullptr};
+    g.cand = cand;
+    rc = enqueue_candidates(h, g, h->size_Nmax);
+    if (rc) return rc;
     if (winners && hf.S > 0) {
         unlimited_kernel<<<(hf.S + 127) / 128, 128, 0, h->stream>>>(h->df, cand, *winners);
         h->launches++;
@@ -558,9 +580,9 @@ int finish_timing(wva_handle* h) {
 }
 
 // What a call with host results places on the device and copies back.  Every call has a winner block [S];
-// the size path also writes a candidate block [S*A].
+// the size path also writes a candidate block ([S*A], [S*A*B] for the size grid).
 struct HostCall {
-    bool cand;                      // the work writes a candidate block
+    size_t n_cand;                  // records of the candidate block the work writes (0: none)
     bool copy_cand, copy_win;       // which blocks come back to the host
     const Cols* extra = nullptr;    // further device columns copied straight to their destinations ...
     const void* extra_dev = nullptr;  // ... from this buffer
@@ -576,11 +598,11 @@ struct HostCall {
 template <class Enqueue>
 int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
     const HostFleet& hf = h->hf;
-    c.bc = block_layout(c.cand ? (size_t)hf.S * hf.A : 0);
+    c.bc = block_layout(c.n_cand);
     c.bw = block_layout(hf.S);
-    if (c.cand) CK(h->d_cand_block.ensure(c.bc.bytes + 16));
+    if (c.n_cand) CK(h->d_cand_block.ensure(c.bc.bytes + 16));
     CK(h->d_win_block.ensure(c.bw.bytes + 16));
-    const AllocCols dc = c.cand ? block_cols(h->d_cand_block.p, c.bc) : AllocCols{};
+    const AllocCols dc = c.n_cand ? block_cols(h->d_cand_block.p, c.bc) : AllocCols{};
     const AllocCols dw = block_cols(h->d_win_block.p, c.bw);
     CK(cudaEventRecord(h->ev_d0, h->stream));
     long long fb_cap = 0;
@@ -614,7 +636,7 @@ int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
 // resident analyze/solve with host outputs
 int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     if (!h->resident) return h->fail(WVA_ERR_STATE, "no resident fleet (call wva_upload first)");
-    HostCall c{true, candidates != nullptr, winners != nullptr};
+    HostCall c{(size_t)h->hf.S * h->hf.A, candidates != nullptr, winners != nullptr};
     const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
         const int rc = enqueue_size(h, dc, winners ? &dw : nullptr);
         fb_cap = (long long)h->cand_pair.size() + 1;
@@ -623,6 +645,104 @@ int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     if (rc) return rc;
     scatter_block(c.cand_host, c.bc, candidates);
     scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
+// ---- size grid: CreateAllocation at every listed batch size --------------------------------------
+// The load pairs x the batch list, sorted by descending N (stable: pair order, then list order), with one
+// Bmax-long table per pair that the pair's candidates share.  Cached until the token statistics, the fleet or
+// the batch list change.
+int prepare_size_grid(wva_handle* h, int B, const int32_t* batch) {
+    if (h->sg_epoch == h->epoch_tokens && (int)h->sg_batch.size() == B &&
+        std::equal(h->sg_batch.begin(), h->sg_batch.end(), batch))
+        return WVA_OK;
+    h->sg_epoch = ~0ull;
+    const HostFleet& hf = h->hf;
+    int Bmax = 1;
+    for (int i = 0; i < B; ++i) Bmax = std::max(Bmax, batch[i]);
+    std::vector<int> tab_pair;
+    for (int s = 0; s < hf.S; ++s)
+        for (int a = 0; a < hf.A; ++a)
+            if (hf.pair_class(s, a, true) == PAIR_LOAD) tab_pair.push_back(s * hf.A + a);
+    const int n_tab = (int)tab_pair.size();
+    if ((long long)n_tab * Bmax > 0xffffffffll) return h->fail(WVA_ERR_UNSUPPORTED, "size-grid tables above 2^32 entries");
+    const int n = n_tab * B;  // <= S * A * B < 2^31 (checked by the caller)
+    std::vector<int> order(n);  // candidate t * B + bi of table t
+    std::iota(order.begin(), order.end(), 0);
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return batch[x % B] > batch[y % B]; });
+    Cols c(16);
+    const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_rec = c.take(4 * (size_t)n),
+                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_bl = c.take(4 * (size_t)B),
+                 o_tpair = c.take(4 * (size_t)n_tab), o_toff = c.take(8 * (size_t)n_tab), o_tlen = c.take(4 * (size_t)n_tab);
+    std::vector<char> host(c.bytes);
+    char* p = host.data();
+    for (int j = 0; j < n; ++j) {
+        const int t = order[j] / B, bi = order[j] % B;
+        ((int*)(p + o_pair))[j] = tab_pair[t];
+        ((int*)(p + o_N))[j] = batch[bi];
+        ((int*)(p + o_rec))[j] = tab_pair[t] * B + bi;
+        ((int*)(p + o_idx))[j] = t;
+        ((long long*)(p + o_off))[j] = (long long)t * Bmax;
+    }
+    if (B) memcpy(p + o_bl, batch, 4 * (size_t)B);
+    for (int t = 0; t < n_tab; ++t) {
+        ((int*)(p + o_tpair))[t] = tab_pair[t];
+        ((long long*)(p + o_toff))[t] = (long long)t * Bmax;
+        ((int*)(p + o_tlen))[t] = Bmax;
+    }
+    CK(h->d_sg_lists.ensure(c.bytes));
+    // pageable source: cudaMemcpyAsync has consumed it by the time it returns
+    CK(cudaMemcpyAsync(h->d_sg_lists.p, p, c.bytes, cudaMemcpyHostToDevice, h->stream));
+    if (n_tab) {
+        CK(h->d_sg_tab.ensure(sizeof(double) * 4 * (size_t)n_tab * Bmax));
+        CK(h->d_sg_ls.ensure(sizeof(float) * ((size_t)n_tab * Bmax + n_tab)));
+        const char* d = (const char*)h->d_sg_lists.p;
+        build_pair_tables<<<n_tab, 128, 0, h->stream>>>(h->df, (const int*)(d + o_tpair), (const long long*)(d + o_toff),
+                                                        (const int*)(d + o_tlen), n_tab, (double*)h->d_sg_tab.p,
+                                                        (float*)h->d_sg_ls.p, nullptr, 0, nullptr);
+        h->launches++;
+        CK(cudaGetLastError());
+    }
+    h->sg_pair = o_pair; h->sg_N = o_N; h->sg_rec = o_rec; h->sg_idx = o_idx; h->sg_off = o_off; h->sg_bl = o_bl;
+    h->sg_n = n;
+    h->sg_Bmax = Bmax;
+    h->sg_batch.assign(batch, batch + B);
+    h->sg_epoch = h->epoch_tokens;
+    return WVA_OK;
+}
+
+// Enqueue the size grid: nil / zero-load candidates, CreateAllocation for the load candidates, then values and the
+// per-server winners.  cand ([S*A*B]) and winners ([S]) are device columns.
+int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCols& cand, const AllocCols& winners) {
+    int rc = prepare_size_grid(h, B, batch);
+    if (rc) return rc;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const HostFleet& hf = h->hf;
+    const int n_rec = hf.S * hf.A * B;
+    const char* d = (const char*)h->d_sg_lists.p;
+    const int* d_batch = (const int*)(d + h->sg_bl);
+    if (n_rec > 0) {
+        trivial_kernel<<<(n_rec + 255) / 256, 256, 0, h->stream>>>(h->df, cand, d_batch, B);
+        h->launches++;
+    }
+    SizeArgs g{};
+    g.f = h->df;
+    g.cand_pair = (const int*)(d + h->sg_pair);
+    g.cand_N = (const int*)(d + h->sg_N);
+    g.n_cand = h->sg_n;
+    g.tab = (const double*)h->d_sg_tab.p;
+    g.tab_off = (const long long*)(d + h->sg_off);
+    g.ls = (const float*)h->d_sg_ls.p;
+    g.place = CandPlace{(const int*)(d + h->sg_idx), (const int*)(d + h->sg_rec)};
+    g.cand = cand;
+    rc = enqueue_candidates(h, g, h->sg_Bmax);
+    if (rc) return rc;
+    if (hf.S > 0) {
+        size_grid_finalize<<<(unsigned)((hf.S + 3) / 4), 128, 0, h->stream>>>(h->df, cand, d_batch, B, winners);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
     return WVA_OK;
 }
 
@@ -1110,7 +1230,7 @@ int run_greedy_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) 
     const HostFleet& hf = h->hf;
     if (!hf.every_acc_typed())
         return h->fail(WVA_ERR_BAD_ARG, "limited mode needs a type id and a capacity for every accelerator");
-    HostCall c{true, true, false};
+    HostCall c{(size_t)hf.S * hf.A, true, false};
     const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
         const int rc = enqueue_size(h, dc, &dw);  // the unlimited kernel also assigns value = transition penalty
         fb_cap = (long long)h->cand_pair.size() + 1;
@@ -1184,7 +1304,8 @@ void wva_destroy(wva_handle* h) {
     if (!h) return;
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    DevBuf* bufs[] = {&h->arena, &h->d_cand_pair, &h->d_cand_N, &h->d_sz_tab, &h->d_sz_ls, &h->d_sz_off, &h->d_sz_state, &h->d_sz_req, &h->d_sz_sort, &h->d_grid_lists,
+    DevBuf* bufs[] = {&h->arena, &h->d_cand_pair, &h->d_cand_N, &h->d_sz_tab, &h->d_sz_ls, &h->d_sz_off, &h->d_sz_state, &h->d_sz_req, &h->d_sz_sort,
+                      &h->d_sg_lists, &h->d_sg_tab, &h->d_sg_ls, &h->d_grid_lists,
                       &h->d_pair_tab, &h->d_tab_pair, &h->d_tab_off, &h->d_tab_len, &h->d_tab, &h->d_ls, &h->d_sort, &h->d_best, &h->d_pb, &h->d_rows,
                       &h->d_cand_block, &h->d_win_block, &h->d_ctrl, &h->d_fb_list, &h->d_scratch,
                       &h->d_cells, &h->d_sweep, &h->d_summary, &h->d_dbg};
@@ -1471,12 +1592,37 @@ int wva_grid_solve(wva_handle* h, const wva_fleet* fleet, const wva_grid* grid, 
     if (rc) return rc;
     if (plan.args.want_cells && plan.n_cells)  // cells that are never analysed must read back as 0
         CK(cudaMemsetAsync(h->d_cells.p, 0, plan.cells.bytes, h->stream));
-    HostCall c{false, false, true, &plan.cells, h->d_cells.p};
+    HostCall c{0, false, true, &plan.cells, h->d_cells.p};
     rc = run_host(h, c, [&](const AllocCols&, const AllocCols& dw, long long& fb_cap) {
         fb_cap = plan.args.fb_cap;
         return enqueue_grid(h, plan, dw);
     });
     if (rc) return rc;
+    scatter_block(c.win_host, c.bw, winners);
+    h->last_kind = 1;
+    return WVA_OK;
+}
+
+int wva_size_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_batch, const int32_t* batch, wva_allocs* candidates,
+                  wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_batch < 0 || (n_batch > 0 && !batch)) return h->fail(WVA_ERR_BAD_ARG, "negative batch count or NULL batch list");
+    for (int i = 0; i < n_batch; ++i)
+        if (batch[i] < 1 || batch[i] > (1 << 20)) return h->fail(WVA_ERR_BAD_ARG, "batch size out of range");
+    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
+    if ((long long)fleet->n_servers * fleet->n_acc * n_batch >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "size grid too large for one call (>= 2^31 candidates)");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_batch, candidates != nullptr, true};
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
+        const int rc = enqueue_size_grid(h, n_batch, batch, dc, dw);
+        fb_cap = (long long)h->sg_n + 1;
+        return rc;
+    });
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
     scatter_block(c.win_host, c.bw, winners);
     h->last_kind = 1;
     return WVA_OK;

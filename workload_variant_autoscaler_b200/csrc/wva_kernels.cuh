@@ -7,6 +7,7 @@
 //   grid_finalize  K3   per-server argmin over partials (warp shuffle -> smem -> record)
 //   trivial_kernel      nil / zero-load candidates
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server
+//   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
 //
 // K1, CreateAllocation per (server, accelerator) candidate (the rounds, the warp-per-candidate kernel and the
@@ -175,15 +176,13 @@ __device__ __forceinline__ float penalty_of(const DevFleet& f, int s, const Cand
     return transition_penalty(f.penalty, f.srv_cur_acc[s], f.srv_cur_replicas[s], f.srv_cur_cost[s], c.acc,
                               c.replicas, c.cost);
 }
-// zeroLoadAllocation: allocation.go:259-288 (value = cost; caller applies the penalty)
-__device__ __forceinline__ Cand zero_load_alloc(const DevFleet& f, int s, int a) {
+// zeroLoadAllocation: allocation.go:259-288 at batch size max_batch (value = cost; caller applies the penalty)
+__device__ __forceinline__ Cand zero_load_alloc(const DevFleet& f, int s, int a, int max_batch) {
     Cand c = cand_nil();
     c.feasible = 1;
     const long long nrep = f.srv_min_replicas[s];
     if (nrep == 0) return c;  // accelerator "", all zero
     const int m = f.srv_model[s], k = m * f.A + a;
-    int max_batch = f.perf_max_batch[k];
-    if (f.srv_max_batch[s] > 0) max_batch = f.srv_max_batch[s];
     const long long total = (long long)num_instances(f, m, a) * nrep;
     c.acc = a;
     c.replicas = (int)nrep;
@@ -195,6 +194,11 @@ __device__ __forceinline__ Cand zero_load_alloc(const DevFleet& f, int s, int a)
     c.ttft = __fadd_rn(f.perf_gamma[k], f.perf_delta[k]);
     c.max_rate = __fdiv_rn((float)max_batch, __fadd_rn(c.ttft, max_decode));
     return c;
+}
+// ... at the batch size the server or the perf data fixes
+__device__ __forceinline__ Cand zero_load_alloc(const DevFleet& f, int s, int a) {
+    const int k = f.srv_model[s] * f.A + a;
+    return zero_load_alloc(f, s, a, f.srv_max_batch[s] > 0 ? f.srv_max_batch[s] : f.perf_max_batch[k]);
 }
 
 // ---------------------------------------------------------------------------
@@ -1513,16 +1517,19 @@ __global__ void __launch_bounds__(256) grid_finalize(GridArgs g, AllocCols winne
     }
 }
 
-// nil and zero-load candidates (everything the size kernel does not own).
-__global__ void trivial_kernel(DevFleet f, AllocCols cand) {
-    const int pair = blockIdx.x * blockDim.x + threadIdx.x;
-    if (pair >= f.S * f.A) return;
+// nil and zero-load candidates (everything the size kernel does not own).  batch == NULL: one candidate per pair
+// at the pair's own batch size; else B candidates per pair, record pair * B + bi at batch size batch[bi]
+// (S * A * B < 2^31, checked on the host).
+__global__ void trivial_kernel(DevFleet f, AllocCols cand, const int* batch, int B) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= f.S * f.A * B) return;
+    const int pair = i / B, bi = i - pair * B;
     const int s = pair / f.A, a = pair % f.A;
     const int cls = pair_class(f, s, a, true);
     if (cls == PAIR_LOAD) return;
     Cand c = cand_nil();
-    if (cls == PAIR_ZERO) c = zero_load_alloc(f, s, a);
-    store_cand(cand, pair, c);
+    if (cls == PAIR_ZERO) c = batch ? zero_load_alloc(f, s, a, batch[bi]) : zero_load_alloc(f, s, a);
+    store_cand(cand, i, c);
 }
 
 // Server.Calculate's value (server.go:60-63) + SolveUnlimited (solver.go:63-79):
@@ -1544,6 +1551,58 @@ __global__ void unlimited_kernel(DevFleet f, AllocCols cand, AllocCols winners) 
         }
     }
     store_cand(winners, s, best);
+}
+
+// wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record
+// (s * A + a) * B + bi), strided, so any A * B fits.  Every feasible candidate gets value = TransitionPenalty as in
+// unlimited_kernel.  The winner is SolveUnlimited's (strict '<' from MaxFloat32: a NaN value or one not below
+// MaxFloat32 never wins), ties to the smaller batch size, then the lower accelerator id, then the lower bi
+// (repeated batch sizes give identical records).
+struct SgKey {
+    float value;
+    int batch, a, bi;  // bi < 0: none
+};
+__device__ __forceinline__ bool sg_better(const SgKey& x, const SgKey& y) {
+    if (x.bi < 0) return false;
+    if (y.bi < 0) return true;
+    if (x.value != y.value) return x.value < y.value;
+    if (x.batch != y.batch) return x.batch < y.batch;
+    if (x.a != y.a) return x.a < y.a;
+    return x.bi < y.bi;
+}
+__global__ void __launch_bounds__(128) size_grid_finalize(DevFleet f, AllocCols cand, const int* batch, int B,
+                                                          AllocCols winners) {
+    const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (s >= f.S) return;
+    const int n = f.A * B;
+    const size_t base = (size_t)s * n;
+    SgKey best{0.0f, 0, 0, -1};
+    for (int k = lane; k < n; k += 32) {
+        if (!cand.feasible[base + k]) continue;
+        const float v = penalty_of(f, s, load_cand(cand, base + k));
+        cand.value[base + k] = v;
+        const int a = k / B, bi = k - a * B;
+        const SgKey key{v, batch[bi], a, bi};
+        if (v < 3.40282346638528859811704183484516925440e+38f && sg_better(key, best)) best = key;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        SgKey o;
+        o.value = __shfl_down_sync(0xffffffffu, best.value, d);
+        o.batch = __shfl_down_sync(0xffffffffu, best.batch, d);
+        o.a = __shfl_down_sync(0xffffffffu, best.a, d);
+        o.bi = __shfl_down_sync(0xffffffffu, best.bi, d);
+        if (sg_better(o, best)) best = o;
+    }
+    if (lane == 0) {
+        Cand c = cand_nil();
+        if (best.bi >= 0) {
+            c = load_cand(cand, base + (size_t)best.a * B + best.bi);
+            c.value = best.value;
+        }
+        store_cand(winners, s, c);
+    }
 }
 
 // ---------------------------------------------------------------------------

@@ -29,14 +29,32 @@ namespace wva {
 
 constexpr int kSzMaxDepth = 5;  // midpoint tree depth: at most 31 evaluations per search per round
 
+// Where a candidate's table and record are.  wva_solve: one table per candidate (N entries, table index j) and
+// record = pair id.  wva_size_grid: the candidates of one pair at its batch sizes share the pair's table of Bmax
+// >= N entries and write record pair * B + bi.  A longer table changes no result: the solves read entries 0..N-1,
+// and column 4's suffix minimum at n is then min(servRate[n..Bmax-1]), a lower bound of the minimum over the
+// rates the chain reads (servRate[n..N-1]), so the early exit (rate_below) fires only where it would have fired on
+// an N-long table, and the exponent bound from entry 0's suffix minimum only narrows the block windows
+// (grid_kernel's cells rely on the same).
+struct CandPlace {
+    const int* tab_idx;   // [n_cand] table index, for the ls column (NULL: j)
+    const int* rec;       // [n_cand] output record (NULL: the pair id)
+    __device__ __forceinline__ int record(int j, int pair) const { return rec ? rec[j] : pair; }
+    __device__ __forceinline__ const float* ls_of(const float* ls, const long long* tab_off, int j) const {
+        return ls + tab_off[j] + (tab_idx ? tab_idx[j] : j);  // a table of len entries has len + 1 ls entries
+    }
+};
+
 struct SizeArgs {
     DevFleet f;
     const int* cand_pair;      // [n_cand] pair ids sorted by descending N
     const int* cand_N;         // [n_cand]
     int n_cand;
-    const double* tab;         // shared-format tables, one per candidate
-    const long long* tab_off;  // [n_cand]
-    AllocCols cand;            // [S*A]
+    const double* tab;         // shared-format tables
+    const long long* tab_off;  // [n_cand] entry offset of the candidate's table
+    const float* ls;           // prefix log2 sums of the tables (scheduling estimate only)
+    CandPlace place;
+    AllocCols cand;
     int* fb_count;
     int* fb_list;              // candidate indices that bailed
     int fb_cap;
@@ -80,9 +98,10 @@ struct Sz2Args {
     const int* cand_N;     // [n]
     int n_cand;
     int depth;             // D
-    const double* tab;     // shared-format tables, one per candidate
+    const double* tab;     // shared-format tables
     const long long* tab_off;  // [n]
     const float* ls;
+    CandPlace place;
     // search state, index 2*j + which (0: TTFT, 1: ITL)
     float *xmin, *xmax, *xs;
     uint8_t *sst, *inc, *iter;
@@ -263,7 +282,7 @@ __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
     g.rmax[j] = b.rmax;
     g.l2s0[j] = log2f(s1);
     g.l2sN[j] = log2f(sN);
-    g.lsN[j] = (g.ls + g.tab_off[j] + j)[N - 1];
+    g.lsN[j] = g.place.ls_of(g.ls, g.tab_off, j)[N - 1];
     g.phase[j] = b.nil ? PH_NIL : PH_SEARCH;
     for (int w = 0; w < 2; ++w) {
         const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
@@ -277,7 +296,7 @@ __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
         g.slot[2 * j + w] = -1;
     }
     g.aslot[j] = -1;
-    if (b.nil) store_cand(g.cand, pair, cand_nil());
+    if (b.nil) store_cand(g.cand, g.place.record(j, pair), cand_nil());
 }
 
 // Advance every candidate: consume last round's results (walking the midpoint trees with the reference's
@@ -368,15 +387,15 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
             else {
                 const float4 m = g.req_out[slot];
                 const SzReplicas r{g.nrep[j], g.cost[j]};
-                store_cand(g.cand, pair, sz_cand(a, g.cand_N[j], r, g.rate_star[j], m.y, m.z, m.w));
+                store_cand(g.cand, g.place.record(j, pair), sz_cand(a, g.cand_N[j], r, g.rate_star[j], m.y, m.z, m.w));
                 ph = PH_DONE;
             }
         }
-        if (ph == PH_NIL) store_cand(g.cand, pair, cand_nil());
+        if (ph == PH_NIL) store_cand(g.cand, g.place.record(j, pair), cand_nil());
         if (ph == PH_BAIL) {
             const int k = atomicAdd(g.fb_count, 1);
             if (k < g.fb_cap) g.fb_list[k] = j;
-            store_cand(g.cand, pair, cand_nil());
+            store_cand(g.cand, g.place.record(j, pair), cand_nil());
         }
         g.phase[j] = (uint8_t)ph;
     }
@@ -398,11 +417,12 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
     unsigned slot = warp_base + (unsigned)(incl - mine);
     const int N = g.cand_N[j], K = N + N * f.ratio;
     const long long off = g.tab_off[j];
+    const float* ls = g.place.ls_of(g.ls, g.tab_off, j);
     const float l2s0 = g.l2s0[j], l2sN = g.l2sN[j], lsN = g.lsN[j];
     auto put = [&](int kind, float lambda) {
         g.req_id[slot] = (unsigned)j * 4u + (unsigned)kind;
         g.req_lam[slot] = lambda;
-        g.req_key[slot] = (uint8_t)length_class(estimate_len(g.tab + 4 * off, g.ls + off + j, N, K, lambda, log2f(lambda),
+        g.req_key[slot] = (uint8_t)length_class(estimate_len(g.tab + 4 * off, ls, N, K, lambda, log2f(lambda),
                                                              l2s0, l2sN, lsN));
         ++slot;
     };
@@ -619,7 +639,7 @@ __global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) {
             const int k = atomicAdd(g.fb_count, 1);
             if (k < g.fb_cap) g.fb_list[k] = j;
         }
-        store_cand(g.cand, pair, c);
+        store_cand(g.cand, g.place.record(j, pair), c);
     }
 }
 
@@ -677,7 +697,7 @@ __global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, 
         ev.K = N + N * f.ratio;
         Cand c;
         if (!create_allocation(f, s, a, N, ev.K, sr[0], sr[N - 1], ev, c)) atomicExch(fb_status, ev.rc);
-        store_cand(g.cand, pair, c);
+        store_cand(g.cand, g.place.record(j, pair), c);
     }
 }
 

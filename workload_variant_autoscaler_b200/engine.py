@@ -108,6 +108,26 @@ class Engine:
                                            C.byref(wc)))
         return cells, win
 
+    def size_grid(self, fleet: Fleet, batches, want_candidates: bool = False, out: Allocs | None = None):
+        """The reference's ``Server.Calculate`` at every listed batch size -> (candidates [S*A*B] | None,
+        winners [S]).
+
+        Candidate ``(s*A + a)*B + bi`` is what ``analyze`` returns for ``(s, a)`` with every server's
+        ``srv_max_batch`` set to ``batches[bi]``; ``winners[s]`` is the min-value candidate (ties: smaller batch
+        size, then lower accelerator id; see ``wva_size_grid`` in include/wva_b200.h).  ``out``: an ``Allocs``
+        of ``fleet.n_servers`` records to write the winners into."""
+        b = np.ascontiguousarray(batches, np.int32).reshape(-1)
+        if out is not None and out.n != fleet.n_servers:
+            raise ValueError("out must hold fleet.n_servers records")
+        win = out if out is not None else Allocs(fleet.n_servers)
+        cand = Allocs(fleet.n_servers * fleet.n_acc * int(b.size)) if want_candidates else None
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_size_grid(self._h, C.byref(fc), int(b.size), _abi.ptr(b),
+                                          C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
+
     def sweep(self, fleet: Fleet, n_rates: int) -> dict:
         n = fleet.n_servers * fleet.n_acc * n_rates
         out = {"valid": np.zeros(n, np.uint8)}
