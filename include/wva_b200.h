@@ -253,6 +253,32 @@ int wva_size_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_batch, const 
                   wva_allocs *candidates, wva_allocs *winners);
 
 /*
+ * Load grid: Server.Calculate (as in wva_analyze) and SolveUnlimited's winner at each of n_levels caller-given
+ * arrival-rate rows, e.g. a load forecast or a peak scenario.
+ *
+ * Let f_l be the fleet with srv_arrival_rpm replaced by row l of arrival_rpm ([n_levels * S], index l*S + s,
+ * req/min).  Candidate block l (records (l*S + s)*A + a) is byte for byte what wva_analyze returns for f_l,
+ * value = TransitionPenalty included.  Winner block l (records l*S + s) is wva_solve's winner block for f_l with
+ * unlimited = 1: strict '<' from MaxFloat32, ties to the lower accelerator id.  Per level a pair is nil at a
+ * negative rate, zeroLoadAllocation at rate 0 (or out_tokens 0), and sized under load otherwise, NaN and +Inf
+ * included.  fleet->srv_arrival_rpm, fleet->unlimited and the capacities are not read; every other column
+ * (tokens, targets, current allocations) comes from `fleet`.  Each candidate block is a valid input for
+ * wva_solve_greedy, which serves limited mode.
+ *
+ * The sizing part of CreateAllocation (QueueAnalyzer.Size and rateStar) does not read the load, so it runs once
+ * per (server, accelerator); only the replica count, the cost and one Analyze run per level.
+ *
+ * The fleet becomes resident, as with every call that takes one; there is no single solution afterwards, so
+ * wva_summarize returns WVA_ERR_STATE.  `candidates` (n_levels*S*A entries) may be NULL; `winners` has
+ * n_levels*S entries.  n_levels == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG: n_levels < 0,
+ * arrival_rpm NULL with n_levels > 0, or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_levels >= 2^31 (refused
+ * before the fleet is read), or a level on which wva_analyze of f_l fails the same way (a NaN rate whose
+ * rescale loop would not terminate, too many stored-vector fallbacks).
+ */
+int wva_load_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
+                  wva_allocs *candidates, wva_allocs *winners);
+
+/*
  * Solver.SolveGreedy + the best-effort saturation policies (pkg/solver/greedy.go:35-341) over a candidate
  * table the caller already holds: `candidates` (S*A, value = transition penalty as wva_analyze returns it) is
  * read, and modified where the reference scales best-effort allocations; `winners` (S) is written.  Host only
@@ -299,7 +325,7 @@ typedef struct wva_summary {
 } wva_summary;
 
 /* Summary of the most recent wva_solve / wva_resolve / wva_grid_solve / wva_size_grid on this handle (the winners
- * stay resident until the next call).  WVA_ERR_STATE when there is none. */
+ * stay resident until the next call).  WVA_ERR_STATE when there is none, e.g. after wva_load_grid. */
 int wva_summarize(wva_handle *h, wva_summary *out);
 
 /* ---- MM1KModel (closed form) --------------------------------------------- */

@@ -117,14 +117,16 @@ struct HostFleet {
     wva_tunables tun{10, 0.1f};
 
     // gates of CreateAllocation + candidate rule (mirrors pair_class on the device)
-    int pair_class(int s, int a, bool honour_keep) const {
+    int pair_class(int s, int a, bool honour_keep) const { return pair_class(s, a, honour_keep, srv_arrival_rpm[s]); }
+    // ... at the arrival rate rpm
+    int pair_class(int s, int a, bool honour_keep, float rpm) const {
         if (honour_keep && srv_keep_acc[s] && srv_cur_acc[s] != WVA_ACC_NONE && srv_cur_acc[s] != a) return 0;
-        if (srv_arrival_rpm[s] < 0.0f || srv_in_tokens[s] < 0 || srv_out_tokens[s] < 0) return 0;
+        if (rpm < 0.0f || srv_in_tokens[s] < 0 || srv_out_tokens[s] < 0) return 0;
         const int m = srv_model[s];
         if (m < 0 || m >= M) return 0;
         if (!perf_present[(size_t)m * A + a]) return 0;
         if (!srv_has_target[s]) return 0;
-        if (srv_arrival_rpm[s] == 0.0f || srv_out_tokens[s] == 0) return PAIR_ZERO;
+        if (rpm == 0.0f || srv_out_tokens[s] == 0) return PAIR_ZERO;
         return PAIR_LOAD;
     }
     // batch size of a candidate: pkg/core/allocation.go:77-87
@@ -183,6 +185,10 @@ struct wva_handle {
     size_t sg_pair = 0, sg_N = 0, sg_rec = 0, sg_idx = 0, sg_off = 0, sg_bl = 0;
     DevBuf d_sg_lists, d_sg_tab, d_sg_ls;
 
+    // load-grid buffers, also apart from wva_solve's size cache: the candidate lists (pair, N, table offset) and
+    // the level rates, one N-entry table per candidate, and the rateStar column
+    DevBuf d_lg_lists, d_lg_tab, d_lg_ls, d_lg_star;
+
     // grid path caches
     uint64_t grid_epoch = ~0ull;
     std::vector<int> grid_batch, grid_replicas;
@@ -230,7 +236,8 @@ namespace {
 
 
 // control block on the device: a handful of ints
-enum { CTRL_COUNTER = 0, CTRL_FB_COUNT = 1, CTRL_FB_STATUS = 2, CTRL_INTS = 8 };
+// CTRL_FB2_COUNT: a second fallback list of the same call (the load grid's tail items)
+enum { CTRL_COUNTER = 0, CTRL_FB_COUNT = 1, CTRL_FB_STATUS = 2, CTRL_FB2_COUNT = 3, CTRL_INTS = 8 };
 
 // ---- SoA result blocks: the wva_allocs columns of n records, 16-byte aligned ----------------
 struct Block {
@@ -419,7 +426,7 @@ int size_depth_for(int n) {
     if (const char* e = getenv("WVA_SIZE_DEPTH")) d = atoi(e);
     return std::min(std::max(d, 1), kSzMaxDepth);
 }
-int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
+int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
     const int D = size_depth_for(n);
     const size_t per_cand = 2 * ((size_t)(1 << D) - 1 + 2);  // two searches: a tree each, plus the two end points
     const size_t cap = per_cand * (size_t)n;                 // requests per round, worst case
@@ -491,7 +498,8 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     for (int round = 0; round < max_rounds; round += group) {
         for (int r = 0; r < group; ++r) {
             sz2_round_reset<<<3, 256, 0, h->stream>>>(g);
-            sz2_advance<<<nb, 256, 0, h->stream>>>(g);
+            if (star) sz2_advance_star<<<nb, 256, 0, h->stream>>>(g);
+            else sz2_advance<<<nb, 256, 0, h->stream>>>(g);
             sz2_sort_local<<<cks, kSortThreads, 0, h->stream>>>(g);
             ws_items_scan<<<1, 256, 0, h->stream>>>(g.ws);
             ws_items_scatter<<<items_blocks, 256, 0, h->stream>>>(g.ws);
@@ -507,9 +515,10 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n) {
     return WVA_OK;
 }
 
-// CreateAllocation for the load candidates g lists (g.cand_pair .. g.place set, batch sizes at most Nmax): the
-// warp-per-candidate kernel or the rounds, timed as the call's kernel, then the stored-vector fallback.
-int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax) {
+// CreateAllocation for the load candidates g lists (g.cand_pair .. g.place set, batch sizes at most Nmax), or up to
+// rateStar when star is set (create_allocation's rateStar mode): the warp-per-candidate kernel or the rounds, timed
+// as the call's kernel, then the stored-vector fallback.
+int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, bool star = false) {
     const int n = g.n_cand;
     g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
     CK(h->d_fb_list.ensure(sizeof(int) * std::max(n, 1)));
@@ -519,10 +528,11 @@ int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax) {
     int small_max = 1024;  // up to here a warp per candidate beats rounds (the GPU is mostly empty either way)
     if (const char* e = getenv("WVA_SIZE_SMALL_MAX")) small_max = atoi(e);
     if (n > 0 && n <= small_max) {
-        size_warp_kernel<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
+        if (star) size_warp_star<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
+        else size_warp_kernel<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
         h->launches++;
     } else if (n > 0) {
-        const int rc = run_size_rounds(h, g, n);
+        const int rc = run_size_rounds(h, g, n, star);
         if (rc) return rc;
     }
     CK(cudaEventRecord(h->ev_k1, h->stream));
@@ -531,8 +541,9 @@ int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax) {
         int Kmax;
         const int rc = ensure_scratch(h, Nmax, h->hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
         if (rc) return rc;
-        size_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
-                                                               (int*)h->d_ctrl.p + CTRL_FB_STATUS);
+        auto* fallback = star ? size_fallback_star : size_fallback;
+        fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
+                                                          (int*)h->d_ctrl.p + CTRL_FB_STATUS);
         h->launches++;
     }
     CK(cudaGetLastError());
@@ -548,7 +559,7 @@ int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners)
     const HostFleet& hf = h->hf;
     const int n_pairs = hf.S * hf.A;
     if (n_pairs > 0) {
-        trivial_kernel<<<(n_pairs + 255) / 256, 256, 0, h->stream>>>(h->df, cand, nullptr, 1);
+        trivial_kernel<<<(n_pairs + 255) / 256, 256, 0, h->stream>>>(h->df, cand, (const int*)nullptr, 1);
         h->launches++;
     }
     SizeArgs g{};
@@ -579,13 +590,16 @@ int finish_timing(wva_handle* h) {
     return WVA_OK;
 }
 
-// What a call with host results places on the device and copies back.  Every call has a winner block [S];
-// the size path also writes a candidate block ([S*A], [S*A*B] for the size grid).
+// What a call with host results places on the device and copies back.  Every call has a winner block ([S], [L*S]
+// for the load grid); the size path also writes a candidate block ([S*A], [S*A*B] for the size grid, [L*S*A] for
+// the load grid).
 struct HostCall {
     size_t n_cand;                  // records of the candidate block the work writes (0: none)
     bool copy_cand, copy_win;       // which blocks come back to the host
     const Cols* extra = nullptr;    // further device columns copied straight to their destinations ...
     const void* extra_dev = nullptr;  // ... from this buffer
+    size_t win_blocks = 1;          // winner blocks of S records
+    long long fb2_cap = 0;          // largest count of the second fallback list that is not an error
     // set by run_host: the block layouts and their host copies in out_stage (NULL when not copied)
     Block bc{}, bw{};
     const char *cand_host = nullptr, *win_host = nullptr;
@@ -599,7 +613,7 @@ template <class Enqueue>
 int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
     const HostFleet& hf = h->hf;
     c.bc = block_layout(c.n_cand);
-    c.bw = block_layout(hf.S);
+    c.bw = block_layout((size_t)hf.S * c.win_blocks);
     if (c.n_cand) CK(h->d_cand_block.ensure(c.bc.bytes + 16));
     CK(h->d_win_block.ensure(c.bw.bytes + 16));
     const AllocCols dc = c.n_cand ? block_cols(h->d_cand_block.p, c.bc) : AllocCols{};
@@ -628,7 +642,7 @@ int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
     if (rc) return rc;
     if (ctrl[CTRL_FB_STATUS] != 0)
         return h->fail(WVA_ERR_UNSUPPORTED, "input outside the supported numeric domain (rescale loop does not terminate)");
-    if ((long long)ctrl[CTRL_FB_COUNT] > fb_cap)
+    if ((long long)ctrl[CTRL_FB_COUNT] > fb_cap || (long long)ctrl[CTRL_FB2_COUNT] > c.fb2_cap)
         return h->fail(WVA_ERR_UNSUPPORTED, "too many cells need the stored-vector fallback");
     return WVA_OK;
 }
@@ -740,6 +754,123 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
     if (rc) return rc;
     if (hf.S > 0) {
         size_grid_finalize<<<(unsigned)((hf.S + 3) / 4), 128, 0, h->stream>>>(h->df, cand, d_batch, B, winners);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- load grid: CreateAllocation and the unlimited winner at every listed load level -------------------------
+// Phase 1 sizes each candidate once: the pairs that pass the gates and are a load at some level, sorted by
+// descending N with one N-entry table each, run through the size drivers in rateStar mode.  Phase 2 (load_kernel,
+// load_fallback) is the tail per (candidate, level).  rpm [L*S] is the caller's level list; cand ([L*S*A]) and
+// winners ([L*S]) are device columns.  Sets the largest counts of the two phases' fallback lists that are not an
+// error.
+int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& cand, const AllocCols& winners,
+                      long long& fb_cap, long long& fb2_cap) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A;
+    std::vector<char> loaded(S, 0);  // server s is a load at some level (NaN and +Inf included)
+    for (int l = 0; l < L; ++l)
+        for (int s = 0; s < S; ++s) loaded[s] |= !(rpm[(size_t)l * S + s] < 0.0f) && rpm[(size_t)l * S + s] != 0.0f;
+    std::vector<int> pairs, Ns;
+    int rc = sorted_pairs(h, [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, true, 1.0f) == PAIR_LOAD; },
+                          pairs, Ns);
+    if (rc) return rc;
+    const int n = (int)pairs.size();
+    const long long n_items = (long long)n * L;
+    Cols c(16);
+    const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n),
+                 o_rpm = c.take(4 * (size_t)L * S);
+    std::vector<char> host(c.bytes);
+    char* p = host.data();
+    long long off = 0;
+    for (int j = 0; j < n; ++j) {
+        ((int*)(p + o_pair))[j] = pairs[j];
+        ((int*)(p + o_N))[j] = Ns[j];
+        ((long long*)(p + o_off))[j] = off;
+        off += Ns[j];
+    }
+    if ((size_t)L * S) memcpy(p + o_rpm, rpm, 4 * (size_t)L * S);
+    CK(h->d_lg_lists.ensure(c.bytes));
+    // pageable source: cudaMemcpyAsync has consumed it by the time it returns
+    CK(cudaMemcpyAsync(h->d_lg_lists.p, p, c.bytes, cudaMemcpyHostToDevice, h->stream));
+    const char* d = (const char*)h->d_lg_lists.p;
+    const float* d_rpm = (const float*)(d + o_rpm);
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
+    if (n_rec > 0) {
+        trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(h->df, cand, d_rpm, L);
+        h->launches++;
+    }
+    // rateStar mode's records by pair id: feasible and max_rate = rateStar
+    const size_t n_pairs = (size_t)S * A;
+    CK(h->d_lg_star.ensure(5 * n_pairs + 16));
+    AllocCols star{};
+    star.max_rate = (float*)h->d_lg_star.p;
+    star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
+    if (n > 0) {
+        CK(h->d_lg_tab.ensure(sizeof(double) * 4 * (size_t)off));
+        CK(h->d_lg_ls.ensure(sizeof(float) * ((size_t)off + n)));
+        build_pair_tables<<<n, 128, 0, h->stream>>>(h->df, (const int*)(d + o_pair), (const long long*)(d + o_off),
+                                                    (const int*)(d + o_N), n, (double*)h->d_lg_tab.p,
+                                                    (float*)h->d_lg_ls.p, nullptr, 0, nullptr);
+        h->launches++;
+    }
+    // the fallback lists of both phases share d_fb_list (phase 1's is consumed before load_kernel starts)
+    const int fb2_list = (int)std::min<long long>(n_items, 1 << 22);
+    fb_cap = (long long)n + 1;
+    fb2_cap = fb2_list;
+    CK(h->d_fb_list.ensure(std::max(sizeof(int) * std::max(n, 1), sizeof(int2) * std::max(fb2_list, 1))));
+    SizeArgs g{};
+    g.f = h->df;
+    g.cand_pair = (const int*)(d + o_pair);
+    g.cand_N = (const int*)(d + o_N);
+    g.n_cand = n;
+    g.tab = (const double*)h->d_lg_tab.p;
+    g.tab_off = (const long long*)(d + o_off);
+    g.ls = (const float*)h->d_lg_ls.p;
+    g.place = CandPlace{nullptr, nullptr};
+    g.cand = star;
+    rc = enqueue_candidates(h, g, n ? Ns[0] : 1, true);
+    if (rc) return rc;
+    if (n > 0 && L > 0) {
+        LoadArgs la{};
+        la.f = h->df;
+        la.cand_pair = g.cand_pair;
+        la.cand_N = g.cand_N;
+        la.tab_off = g.tab_off;
+        la.tab = g.tab;
+        la.star_ok = star.feasible;
+        la.rate_star = star.max_rate;
+        la.level_rpm = d_rpm;
+        la.n_cand = n;
+        la.L = L;
+        la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+        la.cand = cand;
+        la.fb_count = (int*)h->d_ctrl.p + CTRL_FB2_COUNT;
+        la.fb_points = (int2*)h->d_fb_list.p;
+        la.fb_cap = fb2_list;
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, load_kernel, 256, 0));
+        per_sm = std::max(1, std::min(per_sm, 8));
+        const long long warps = (n_items + 31) / 32;
+        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
+        load_kernel<<<blocks, 256, 0, h->stream>>>(la);
+        h->launches++;
+        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
+        size_t slot_doubles;
+        int Kmax;
+        rc = ensure_scratch(h, Ns[0], hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
+        if (rc) return rc;
+        load_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(la, (double*)h->d_scratch.p, slot_doubles, Kmax,
+                                                               (int*)h->d_ctrl.p + CTRL_FB_STATUS);
+        h->launches++;
+    }
+    if (S > 0 && L > 0) {
+        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
+            h->df, cand, winners, L);
         h->launches++;
     }
     CK(cudaGetLastError());
@@ -1305,7 +1436,8 @@ void wva_destroy(wva_handle* h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     DevBuf* bufs[] = {&h->arena, &h->d_cand_pair, &h->d_cand_N, &h->d_sz_tab, &h->d_sz_ls, &h->d_sz_off, &h->d_sz_state, &h->d_sz_req, &h->d_sz_sort,
-                      &h->d_sg_lists, &h->d_sg_tab, &h->d_sg_ls, &h->d_grid_lists,
+                      &h->d_sg_lists, &h->d_sg_tab, &h->d_sg_ls, &h->d_lg_lists, &h->d_lg_tab, &h->d_lg_ls, &h->d_lg_star,
+                      &h->d_grid_lists,
                       &h->d_pair_tab, &h->d_tab_pair, &h->d_tab_off, &h->d_tab_len, &h->d_tab, &h->d_ls, &h->d_sort, &h->d_best, &h->d_pb, &h->d_rows,
                       &h->d_cand_block, &h->d_win_block, &h->d_ctrl, &h->d_fb_list, &h->d_scratch,
                       &h->d_cells, &h->d_sweep, &h->d_summary, &h->d_dbg};
@@ -1625,6 +1757,29 @@ int wva_size_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_batch, const 
     scatter_block(c.cand_host, c.bc, candidates);
     scatter_block(c.win_host, c.bw, winners);
     h->last_kind = 1;
+    return WVA_OK;
+}
+
+int wva_load_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                  wva_allocs* candidates, wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_levels < 0 || (n_levels > 0 && !arrival_rpm))
+        return h->fail(WVA_ERR_BAD_ARG, "negative level count or NULL level list");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "load grid too large for one call (>= 2^31 candidates)");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
+    c.win_blocks = (size_t)n_levels;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
+        return enqueue_load_grid(h, n_levels, arrival_rpm, dc, dw, fb_cap, c.fb2_cap);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
     return WVA_OK;
 }
 

@@ -5,8 +5,8 @@
 //                       sort, persistent warps pulling 32-cell items, fused feasibility + batch-rank minimum
 //   grid_fallback       stored-vector re-run of the rare cells the streaming solve bails on
 //   grid_finalize  K3   per-server argmin over partials (warp shuffle -> smem -> record)
-//   trivial_kernel      nil / zero-load candidates
-//   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server
+//   trivial_kernel      nil / zero-load candidates (overload: per load level of wva_load_grid)
+//   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
 //   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
 //
@@ -171,6 +171,12 @@ __device__ __forceinline__ QParams qparams_of(const DevFleet& f, int s, int a) {
 __device__ __forceinline__ float total_rate_of(const DevFleet& f, int s) {  // allocation.go:134-139
     if (f.srv_slo_tps[s] == 0.0f) return __fdiv_rn(f.srv_arrival_rpm[s], 60.0f);
     return __fdiv_rn(f.srv_slo_tps[s], (float)f.srv_out_tokens[s]);
+}
+// The fleet as the load grid sees it at level l: the arrival rates are row l of the level list.
+__device__ __forceinline__ DevFleet at_level(const DevFleet& f, const float* level_rpm, int l) {
+    DevFleet fl = f;
+    fl.srv_arrival_rpm = level_rpm + (size_t)l * f.S;
+    return fl;
 }
 __device__ __forceinline__ float penalty_of(const DevFleet& f, int s, const Cand& c) {
     return transition_penalty(f.penalty, f.srv_cur_acc[s], f.srv_cur_replicas[s], f.srv_cur_cost[s], c.acc,
@@ -1531,12 +1537,33 @@ __global__ void trivial_kernel(DevFleet f, AllocCols cand, const int* batch, int
     if (cls == PAIR_ZERO) c = batch ? zero_load_alloc(f, s, a, batch[bi]) : zero_load_alloc(f, s, a);
     store_cand(cand, i, c);
 }
+// ... of the load grid: L level blocks of S * A records (record l * S * A + pair), each pair classed at its
+// level's rate level_rpm[l * S + s]; a zero-load candidate at the pair's own batch size (S * A * L < 2^31, checked
+// on the host).
+__global__ void trivial_kernel(DevFleet f, AllocCols cand, const float* level_rpm, int L) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n_pairs = f.S * f.A;
+    if (i >= n_pairs * L) return;
+    const int l = i / n_pairs, pair = i - l * n_pairs;
+    const int s = pair / f.A, a = pair % f.A;
+    const int cls = pair_class(at_level(f, level_rpm, l), s, a, true);
+    if (cls == PAIR_LOAD) return;
+    store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
+}
+
+// The columns of c from record i on.
+__device__ __forceinline__ AllocCols cols_at(const AllocCols& c, size_t i) {
+    AllocCols o;
+#define WVA_OFFSET_COLUMN(name, type, required) o.name = c.name ? c.name + i : nullptr;
+    WVA_ALLOC_COLUMNS(WVA_OFFSET_COLUMN)
+#undef WVA_OFFSET_COLUMN
+    return o;
+}
 
 // Server.Calculate's value (server.go:60-63) + SolveUnlimited (solver.go:63-79):
 // one thread per server; strict '<' from MaxFloat32, lowest accelerator id wins ties.
-__global__ void unlimited_kernel(DevFleet f, AllocCols cand, AllocCols winners) {
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= f.S) return;
+__device__ __forceinline__ void unlimited_server(const DevFleet& f, const AllocCols& cand, const AllocCols& winners,
+                                                 int s) {
     float min_val = 3.40282346638528859811704183484516925440e+38f;
     Cand best = cand_nil();
     for (int a = 0; a < f.A; ++a) {
@@ -1551,6 +1578,18 @@ __global__ void unlimited_kernel(DevFleet f, AllocCols cand, AllocCols winners) 
         }
     }
     store_cand(winners, s, best);
+}
+__global__ void unlimited_kernel(DevFleet f, AllocCols cand, AllocCols winners) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= f.S) return;
+    unlimited_server(f, cand, winners, s);
+}
+// ... over the load grid's L level blocks (candidates l * S * A .., winners l * S ..); grid.y strides the levels.
+__global__ void unlimited_kernel(DevFleet f, AllocCols cand, AllocCols winners, int L) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= f.S) return;
+    for (int l = blockIdx.y; l < L; l += gridDim.y)
+        unlimited_server(f, cols_at(cand, (size_t)l * f.S * f.A), cols_at(winners, (size_t)l * f.S), s);
 }
 
 // wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record

@@ -2,7 +2,8 @@
 // (server, accelerator) candidate.  The decisions (the start, the bisections' end-point test and walk, lambda*, the
 // replica count, the feasible candidate) are written once below and driven two ways: large fleets run ROUNDS of
 // sorted solve batches with SPECULATIVE bisection (sz2_*); small fleets and the stored-vector fallback run
-// create_allocation straight through (size_warp_kernel, size_fallback).
+// create_allocation straight through (size_warp_kernel, size_fallback).  The load grid runs the same drivers up to
+// rateStar (the part that does not read the load), then its tail per load level (load_kernel, load_fallback).
 //
 // The reference runs, per candidate, two sequential bisections (pkg/analyzer/utils.go:26-70) of <= 102 model
 // solves each, then two Analyze calls.  The solves of one bisection depend on each other only through ONE
@@ -233,14 +234,14 @@ __device__ __forceinline__ bool sz_lambda(const DevFleet& f, int s, float rmax, 
     return sz_gate(__fmul_rn(go_minf(go_minf(xs_ttft, xs_itl), l_tps), 1000.0f), rmax, lam);
 }
 
-// allocation.go:134-153: replicas and cost for the throughput rate_star, then Analyze's check of the final rate.
+// allocation.go:140-153: replicas and cost for the throughput rate_star at totalRate (:134-139, total_rate_of),
+// then Analyze's check of the final rate.
 struct SzReplicas {
     long long nrep;
     float cost;
 };
 __device__ __forceinline__ bool sz_replicas(const DevFleet& f, int s, int a, float rmax, float rate_star,
-                                            SzReplicas& r, float& lam) {
-    const float total_rate = total_rate_of(f, s);
+                                            float total_rate, SzReplicas& r, float& lam) {
     r.nrep = go_f64_to_int(ceil(__ddiv_rn((double)total_rate, (double)rate_star)));
     const long long min_rep = f.srv_min_replicas[s];
     if (r.nrep < min_rep) r.nrep = min_rep;
@@ -263,6 +264,15 @@ __device__ __forceinline__ Cand sz_cand(int a, int N, const SzReplicas& r, float
     c.ttft = ttft;
     c.rho = rho;
     c.max_rate = __fdiv_rn(rate_star, 1000.0f);
+    return c;
+}
+
+// rateStar mode's record of a candidate whose sizing succeeded: feasible, max_rate = rateStar (req/s, not yet
+// divided by 1000).  The caller passes only the feasible and max_rate columns.
+__device__ __forceinline__ Cand star_cand(float rate_star) {
+    Cand c = cand_nil();
+    c.feasible = 1;
+    c.max_rate = rate_star;
     return c;
 }
 
@@ -300,8 +310,9 @@ __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
 }
 
 // Advance every candidate: consume last round's results (walking the midpoint trees with the reference's
-// comparisons), then emit this round's requests into consecutive slots.
-__global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
+// comparisons), then emit this round's requests into consecutive slots.  kStar: rateStar mode (create_allocation).
+template <bool kStar>
+__device__ __forceinline__ void sz2_advance_body(const Sz2Args& g) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     const DevFleet& f = g.f;
     const int D = g.depth, M = (1 << D) - 1;
@@ -373,13 +384,18 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
             if (g.req_bail[slot]) ph = PH_BAIL;
             else {
                 const float rate_star = g.req_out[slot].x;  // metrics.Throughput
-                SzReplicas r;
-                const bool ok = sz_replicas(f, s, a, rmax, rate_star, r, an_lambda);
-                g.rate_star[j] = rate_star;
-                g.nrep[j] = r.nrep;
-                g.cost[j] = r.cost;
-                if (!ok) ph = PH_NIL;
-                else { an_kind = 3; ph = PH_WAIT_FINAL; }
+                if constexpr (kStar) {
+                    store_cand(g.cand, g.place.record(j, pair), star_cand(rate_star));
+                    ph = PH_DONE;
+                } else {
+                    SzReplicas r;
+                    const bool ok = sz_replicas(f, s, a, rmax, rate_star, total_rate_of(f, s), r, an_lambda);
+                    g.rate_star[j] = rate_star;
+                    g.nrep[j] = r.nrep;
+                    g.cost[j] = r.cost;
+                    if (!ok) ph = PH_NIL;
+                    else { an_kind = 3; ph = PH_WAIT_FINAL; }
+                }
             }
         } else {  // PH_WAIT_FINAL
             const int slot = g.aslot[j];
@@ -440,6 +456,8 @@ __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) {
         put(an_kind, an_lambda);
     }
 }
+__global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) { sz2_advance_body<false>(g); }
+__global__ void __launch_bounds__(256) sz2_advance_star(Sz2Args g) { sz2_advance_body<true>(g); }
 
 // Local counting sort of this round's requests by length class (keys precomputed by sz2_advance); stable inside a
 // warp's 32 requests, so the requests of one candidate (consecutive slots) stay adjacent within their class.
@@ -546,8 +564,12 @@ __global__ void sz2_round_reset(Sz2Args g) {
 //   end(i), node(v)              {y, bail} of end point i / tree node v of the last round
 //   solve(lambda, st)            Model.Solve for Analyze; false when it bailed
 // Returns false when a consulted solve bailed (out is then nil).
+//
+// kStar: rateStar mode (the load grid) stops where the tail that reads the load starts (allocation.go:134), with
+// out = nil or star_cand(rateStar).  Everything before that point (N from the tokens and srv_max_batch, the
+// bisections, lambda*, rateStar = Analyze(lambda*).Throughput) does not read the load.
 // ---------------------------------------------------------------------------
-template <class Eval>
+template <bool kStar, class Eval>
 __device__ __forceinline__ bool create_allocation(const DevFleet& f, int s, int a, int N, int K, float s1, float sN,
                                                   Eval& ev, Cand& out) {
     out = cand_nil();
@@ -573,8 +595,12 @@ __device__ __forceinline__ bool create_allocation(const DevFleet& f, int s, int 
     if (!sz_lambda(f, s, b.rmax, xs_ttft, xs_itl, lam)) return true;
     if (!ev.solve(lam, st)) return false;
     const float rate_star = metrics_from(ev.q, N, st).throughput;
+    if constexpr (kStar) {
+        out = star_cand(rate_star);
+        return true;
+    }
     SzReplicas r;
-    if (!sz_replicas(f, s, a, b.rmax, rate_star, r, lam)) return true;
+    if (!sz_replicas(f, s, a, b.rmax, rate_star, total_rate_of(f, s), r, lam)) return true;
     if (!ev.solve(lam, st)) return false;
     const Metrics m = metrics_from(ev.q, N, st);
     out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
@@ -619,7 +645,8 @@ struct WarpEval {
     }
 };
 
-__global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) {
+template <bool kStar>
+__device__ __forceinline__ void size_warp(const SizeArgs& g) {
     const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
     if (j >= g.n_cand) return;
@@ -633,7 +660,7 @@ __global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) {
     ev.K = K;
     ev.lane = lane;
     Cand c;
-    const bool ok = create_allocation(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
+    const bool ok = create_allocation<kStar>(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
     if (lane == 0) {
         if (!ok) {
             const int k = atomicAdd(g.fb_count, 1);
@@ -642,6 +669,8 @@ __global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) {
         store_cand(g.cand, g.place.record(j, pair), c);
     }
 }
+__global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) { size_warp<false>(g); }
+__global__ void __launch_bounds__(128) size_warp_star(SizeArgs g) { size_warp<true>(g); }
 
 // ---------------------------------------------------------------------------
 // Stored-vector re-run of the candidates that bailed (slot k handles list entries k, k + n_slots, ..): one thread
@@ -675,7 +704,9 @@ struct StoredEval {
     }
 };
 
-__global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+template <bool kStar>
+__device__ __forceinline__ void size_fallback_body(const SizeArgs& g, double* scratch, size_t slot_doubles, int Kmax,
+                                                   int* fb_status) {
     const DevFleet& f = g.f;
     const int n_slots = gridDim.x * blockDim.x;
     const int slot = blockIdx.x * blockDim.x + threadIdx.x;
@@ -696,8 +727,121 @@ __global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, 
         ev.N = N;
         ev.K = N + N * f.ratio;
         Cand c;
-        if (!create_allocation(f, s, a, N, ev.K, sr[0], sr[N - 1], ev, c)) atomicExch(fb_status, ev.rc);
+        if (!create_allocation<kStar>(f, s, a, N, ev.K, sr[0], sr[N - 1], ev, c)) atomicExch(fb_status, ev.rc);
         store_cand(g.cand, g.place.record(j, pair), c);
+    }
+}
+__global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+    size_fallback_body<false>(g, scratch, slot_doubles, Kmax, fb_status);
+}
+__global__ void size_fallback_star(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+    size_fallback_body<true>(g, scratch, slot_doubles, Kmax, fb_status);
+}
+
+// ---------------------------------------------------------------------------
+// The load grid's tail (allocation.go:134-163) at every level of a caller-given load list: one lane per (candidate,
+// level) item whose level rate is a load (not negative, not zero; NaN and +Inf included).  The candidates are the
+// load pairs in descending N with their rateStar from the rateStar mode above, which does not read the load.  Items
+// are candidate-major (item e * L + l), so a warp reads the tables of one or a few pairs; a work counter hands out
+// warps, as in sweep_kernel.  The final per-replica rate totalRate / replicas is at most rateStar, so a pair's
+// chains are bounded by its lambda* chain.  Record (l * S + s) * A + a of the candidate block.
+// ---------------------------------------------------------------------------
+struct LoadArgs {
+    DevFleet f;
+    const int* cand_pair;       // [n_cand] pair ids sorted by descending N
+    const int* cand_N;          // [n_cand]
+    const long long* tab_off;   // [n_cand] entry offset of the candidate's table (N entries)
+    const double* tab;
+    const uint8_t* star_ok;     // [S * A] by pair: rateStar mode's records (0: nil at every load level) ...
+    const float* rate_star;     // ... and their rateStar
+    const float* level_rpm;     // [L * S] arrival rate of server s at level l (req/min)
+    int n_cand, L;
+    unsigned* counter;
+    AllocCols cand;             // [L * S * A]
+    int* fb_count;
+    int2* fb_points;            // items that bailed: {candidate, level}
+    int fb_cap;
+};
+
+// Candidate e's record at level l (nil, or the feasible allocation); solve(lambda, st) is Model.Solve for the
+// final Analyze.  Returns false when that solve bailed (out is then nil).
+template <class Solve>
+__device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, int l, float sN, Solve&& solve, Cand& out) {
+    const DevFleet& f = g.f;
+    const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A, N = g.cand_N[e];
+    out = cand_nil();
+    if (!g.star_ok[pair]) return true;
+    const float rate_star = g.rate_star[pair];
+    SzReplicas r;
+    float lam;
+    if (!sz_replicas(f, s, a, rate_max_of(sN), rate_star, total_rate_of(at_level(f, g.level_rpm, l), s), r, lam))
+        return true;
+    ModelStats st;
+    if (!solve(lam, st)) return false;
+    const Metrics m = metrics_from(qparams_of(f, s, a), N, st);
+    out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
+    return true;
+}
+
+__device__ __forceinline__ size_t load_record(const LoadArgs& g, int e, int l) {
+    return (size_t)l * g.f.S * g.f.A + g.cand_pair[e];
+}
+
+__global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
+    const DevFleet& f = g.f;
+    const int lane = threadIdx.x & 31;
+    const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
+    for (;;) {
+        unsigned w = 0;
+        if (lane == 0) w = atomicAdd(g.counter, 1u);
+        w = __shfl_sync(0xffffffffu, w, 0);
+        if ((unsigned long long)w * 32 >= n_items) break;
+        const unsigned i = w * 32 + lane;
+        if (i < n_items) {
+            const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
+            const float rpm = g.level_rpm[(size_t)l * f.S + g.cand_pair[e] / f.A];
+            if (!(rpm < 0.0f) && rpm != 0.0f) {  // else trivial_kernel's nil / zero-load record
+                const int N = g.cand_N[e], K = N + N * f.ratio;
+                const double* tab = g.tab + 4 * g.tab_off[e];
+                Cand c;
+                const bool ok = load_tail(g, e, l, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
+                    return solve_shared(tab, N, K, lam, st) == kSolveOk;
+                }, c);
+                if (!ok) {
+                    const int k = atomicAdd(g.fb_count, 1);
+                    if (k < g.fb_cap) g.fb_points[k] = make_int2(e, l);
+                }
+                store_cand(g.cand, load_record(g, e, l), c);
+            }
+        }
+    }
+}
+
+// Stored-vector re-run of the items load_kernel bailed on (slot k handles list entries k, k + n_slots, ..); scratch
+// per slot as in size_fallback.
+__global__ void load_fallback(LoadArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+    const DevFleet& f = g.f;
+    const int n_slots = gridDim.x * blockDim.x;
+    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+    int n = *g.fb_count;
+    if (n > g.fb_cap) n = g.fb_cap;
+    double* p = scratch + (size_t)slot * slot_doubles;
+    float* sr = (float*)(p + Kmax + 1);
+    for (int k = slot; k < n; k += n_slots) {
+        const int e = g.fb_points[k].x, l = g.fb_points[k].y;
+        const int N = g.cand_N[e], K = N + N * f.ratio;
+        const double* tab = g.tab + 4 * g.tab_off[e];
+        for (int u = 0; u < N; ++u) sr[u] = (float)tab[4 * u];
+        int rc = 0;
+        Cand c;
+        if (!load_tail(g, e, l, sr[N - 1], [&](float lam, ModelStats& st) {
+                rc = solve_stored(p, sr, N, K, lam, st);
+                return rc == 0;
+            }, c)) {
+            atomicExch(fb_status, rc);
+            continue;
+        }
+        store_cand(g.cand, load_record(g, e, l), c);
     }
 }
 

@@ -128,6 +128,29 @@ class Engine:
                                           C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
+    def load_grid(self, fleet: Fleet, arrival_rpm, want_candidates: bool = False, out: Allocs | None = None):
+        """The reference's ``Server.Calculate`` and ``SolveUnlimited`` winner at each row of ``arrival_rpm``
+        (shape (L, S), req/min) -> (candidates [L*S*A] | None, winners [L*S]), both level-major.
+
+        Candidate block ``l`` is what ``analyze`` returns for the fleet with ``srv_arrival_rpm`` = row ``l``, and
+        winner block ``l`` is ``solve``'s winners for it in unlimited mode (see ``wva_load_grid`` in
+        include/wva_b200.h); ``fleet.srv_arrival_rpm`` is not read.  ``out``: an ``Allocs`` of ``L * S`` records
+        to write the winners into."""
+        rpm = np.ascontiguousarray(arrival_rpm, np.float32)
+        if rpm.ndim != 2 or rpm.shape[1] != fleet.n_servers:
+            raise ValueError(f"arrival_rpm must have shape (L, {fleet.n_servers}), got {rpm.shape}")
+        L = rpm.shape[0]
+        if out is not None and out.n != L * fleet.n_servers:
+            raise ValueError("out must hold L * fleet.n_servers records")
+        win = out if out is not None else Allocs(L * fleet.n_servers)
+        cand = Allocs(L * fleet.n_servers * fleet.n_acc) if want_candidates else None
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_load_grid(self._h, C.byref(fc), L, _abi.ptr(rpm.reshape(-1)),
+                                          C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
+
     def sweep(self, fleet: Fleet, n_rates: int) -> dict:
         n = fleet.n_servers * fleet.n_acc * n_rates
         out = {"valid": np.zeros(n, np.uint8)}
