@@ -25,9 +25,16 @@ using namespace wva;
 
 namespace {
 
+// Growable buffers that own their memory: freed when the handle that holds them is deleted.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() {
+        if (p) cudaFree(p);
+    }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -38,15 +45,16 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
 };
 struct PinBuf {
     void* p = nullptr;
     size_t cap = 0;
+    PinBuf() = default;
+    PinBuf(const PinBuf&) = delete;
+    PinBuf& operator=(const PinBuf&) = delete;
+    ~PinBuf() {
+        if (p) cudaFreeHost(p);
+    }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFreeHost(p);
@@ -56,11 +64,6 @@ struct PinBuf {
         cudaError_t e = cudaMallocHost(&p, want);
         if (e == cudaSuccess) cap = want;
         return e;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
     }
 };
 
@@ -148,6 +151,24 @@ struct Column {
     size_t off, bytes;
 };
 
+constexpr uint64_t kUncached = ~0ull;  // an epoch no fleet reaches
+
+// One set of shared service-rate tables (build_pair_tables) and the device image of the lists that describe them:
+// upload_tables() fills it, build_tables() builds the tables, and the caching rules are at upload_tables().
+struct PairTables {
+    DevBuf lists, tab, ls;  // the lists image; 4 doubles per entry; entries + n floats of prefix log2 sums
+    // what the lists were uploaded for: epoch_tokens and the path's other inputs (kUncached: nothing to reuse)
+    uint64_t epoch = kUncached;
+    std::vector<int> key;
+    int n = 0, len_max = 1;                   // tables, the longest one (1 when there are none)
+    bool with_ls = false;                     // ls is built (the sweep needs none)
+    size_t o_pair = 0, o_off = 0, o_len = 0;  // byte offsets in `lists` of the pair ids, entry offsets and lengths
+    bool holds(uint64_t e, const std::vector<int>& k = {}) const { return epoch == e && key == k; }
+    const int* pair() const { return (const int*)((const char*)lists.p + o_pair); }
+    const long long* off() const { return (const long long*)((const char*)lists.p + o_off); }
+    const int* len() const { return (const int*)((const char*)lists.p + o_len); }
+};
+
 }  // namespace
 
 struct wva_handle {
@@ -168,32 +189,17 @@ struct wva_handle {
     Column col_rate{}, col_in{}, col_out{};
     uint64_t epoch_tokens = 0;  // bumped when service-rate tables become stale
 
-    // size path caches
-    uint64_t size_epoch = ~0ull;
-    std::vector<int> cand_pair, cand_N;
-    int size_Nmax = 0;
-    DevBuf d_cand_pair, d_cand_N;
-    DevBuf d_sz_tab, d_sz_ls, d_sz_off, d_sz_state, d_sz_req, d_sz_sort;
+    // service-rate tables: one set per path, so that a size grid or a load grid never evicts wva_solve's; the
+    // sweep builds into the grid's
+    PairTables size_tabs, sg_tabs, lg_tabs, grid_tabs;
+
+    // size path
+    DevBuf d_sz_state, d_sz_req, d_sz_sort;
     PinBuf sz_pin;
+    DevBuf d_lg_star;  // the load grid's rateStar records
 
-    // size-grid caches: buffers of their own, so that wva_solve's size cache above stays valid
-    uint64_t sg_epoch = ~0ull;
-    std::vector<int> sg_batch;
-    int sg_n = 0, sg_Bmax = 1;
-    // byte offsets in d_sg_lists of the candidate columns (pair, N, record, table index, table offset) and the
-    // batch list
-    size_t sg_pair = 0, sg_N = 0, sg_rec = 0, sg_idx = 0, sg_off = 0, sg_bl = 0;
-    DevBuf d_sg_lists, d_sg_tab, d_sg_ls;
-
-    // load-grid buffers, also apart from wva_solve's size cache: the candidate lists (pair, N, table offset) and
-    // the level rates, one N-entry table per candidate, and the rateStar column
-    DevBuf d_lg_lists, d_lg_tab, d_lg_ls, d_lg_star;
-
-    // grid path caches
-    uint64_t grid_epoch = ~0ull;
-    std::vector<int> grid_batch, grid_replicas;
-    int grid_Bmax = 0, grid_n_tab = 0;
-    DevBuf d_grid_lists, d_pair_tab, d_tab_pair, d_tab_off, d_tab_len, d_tab, d_ls, d_sort, d_best, d_pb, d_rows;
+    // grid path
+    DevBuf d_sort, d_best, d_pb, d_rows;
     // shared
     DevBuf d_cand_block, d_win_block, d_ctrl, d_fb_list, d_scratch, d_cells, d_sweep, d_dbg;
     // peer exchange of the winner block (multi-GPU, one process per GPU on one node)
@@ -388,35 +394,82 @@ int sorted_pairs(wva_handle* h, Keep keep, std::vector<int>& pairs, std::vector<
     return WVA_OK;
 }
 
-// ---- size path (K1) ---------------------------------------------------------
-int prepare_size(wva_handle* h) {
-    if (h->size_epoch == h->epoch_tokens) return WVA_OK;
-    const HostFleet& hf = h->hf;
-    int rc = sorted_pairs(h, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, h->cand_pair,
-                          h->cand_N);
-    if (rc) return rc;
-    const int n = (int)h->cand_pair.size();
-    h->size_Nmax = n ? h->cand_N[0] : 1;
-    if (n) {
-        CK(h->d_cand_pair.ensure(sizeof(int) * n));
-        CK(h->d_cand_N.ensure(sizeof(int) * n));
-        CK(cudaMemcpyAsync(h->d_cand_pair.p, h->cand_pair.data(), sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->d_cand_N.p, h->cand_N.data(), sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-        // one shared-format service-rate table per candidate (N entries), cached until the token
-        // statistics or the fleet change
-        std::vector<long long> off(n + 1, 0);
-        for (int j = 0; j < n; ++j) off[j + 1] = off[j] + h->cand_N[j];
-        CK(h->d_sz_off.ensure(sizeof(long long) * (n + 1)));
-        CK(h->d_sz_tab.ensure(sizeof(double) * 4 * (size_t)off[n] + 1024));
-        CK(h->d_sz_ls.ensure(sizeof(float) * ((size_t)off[n] + n + 1)));
-        CK(cudaMemcpyAsync(h->d_sz_off.p, off.data(), sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, h->stream));
-        build_pair_tables<<<n, 128, 0, h->stream>>>(h->df, (const int*)h->d_cand_pair.p, (const long long*)h->d_sz_off.p,
-                                                    (const int*)h->d_cand_N.p, n, (double*)h->d_sz_tab.p,
-                                                    (float*)h->d_sz_ls.p, nullptr, 0, nullptr);
-        h->launches++;
-        CK(cudaGetLastError());
+// ---- shared service-rate tables ---------------------------------------------
+// Upload the lists of one set of tables: table t is pair[t]'s first len[t] service rates, in the caller's order,
+// at entry offset len[0] + .. + len[t-1].  The columns the caller laid out in `c` come first in the same image and
+// fill(host image) writes them; the table lists follow.  One H2D copy, then tab (and ls when with_ls) are sized.
+// The instance is left keyed kUncached; a path that caches sets the key once its tables are built.
+//
+// Every entry point that takes a fleet calls upload_fleet, which bumps epoch_tokens, so only the resident calls can
+// reuse lists.  Each path's rule:
+// - solve path (size_tabs): lists and tables are rebuilt only when epoch_tokens changes.  A wva_update_load +
+//   wva_resolve (or wva_resolve_device) tick with unchanged tokens and pair classes uploads nothing and launches
+//   no build_pair_tables.
+// - size grid (sg_tabs) and load grid (lg_tabs): rebuilt on every call.
+// - grid (grid_tabs): the lists are uploaded only when epoch_tokens, the batch list or the replica list changed,
+//   which leaves wva_grid_solve_device as the only call that can find them unchanged.  build_pair_tables (with the
+//   per-(table, batch) constants) runs on every call: the tables are part of the evaluation.
+// - sweep: builds into grid_tabs on every call; the upload leaves them keyed kUncached, so the grid's next call
+//   uploads its own lists again.
+template <class Fill>
+int upload_tables(wva_handle* h, PairTables& pt, const std::vector<int>& pair, const std::vector<int>& len,
+                  bool with_ls, Cols& c, Fill&& fill) {
+    const int n = (int)pair.size();
+    pt.epoch = kUncached;
+    pt.key.clear();
+    pt.o_pair = c.take(4 * (size_t)n);
+    pt.o_off = c.take(8 * (size_t)n);
+    pt.o_len = c.take(4 * (size_t)n);
+    std::vector<char> host(c.bytes);
+    char* p = host.data();
+    long long entries = 0;
+    pt.len_max = 1;
+    for (int t = 0; t < n; ++t) {
+        ((int*)(p + pt.o_pair))[t] = pair[t];
+        ((long long*)(p + pt.o_off))[t] = entries;
+        ((int*)(p + pt.o_len))[t] = len[t];
+        entries += len[t];
+        pt.len_max = std::max(pt.len_max, len[t]);
     }
-    h->size_epoch = h->epoch_tokens;
+    fill(p);
+    CK(pt.lists.ensure(c.bytes));
+    // pageable source: cudaMemcpyAsync has consumed it by the time it returns
+    CK(cudaMemcpyAsync(pt.lists.p, p, c.bytes, cudaMemcpyHostToDevice, h->stream));
+    if (n) {
+        CK(pt.tab.ensure(sizeof(double) * 4 * (size_t)entries));
+        if (with_ls) CK(pt.ls.ensure(sizeof(float) * ((size_t)entries + n)));
+    }
+    pt.n = n;
+    pt.with_ls = with_ls;
+    return WVA_OK;
+}
+
+// build_pair_tables over the uploaded lists; the grid passes its batch list and gets the per-(table, batch)
+// constants in pb
+int build_tables(wva_handle* h, const PairTables& pt, const int* batch = nullptr, int B = 0, float4* pb = nullptr) {
+    if (pt.n == 0) return WVA_OK;
+    build_pair_tables<<<pt.n, 128, 0, h->stream>>>(h->df, pt.pair(), pt.off(), pt.len(), pt.n, (double*)pt.tab.p,
+                                                   pt.with_ls ? (float*)pt.ls.p : nullptr, batch, B, pb);
+    h->launches++;
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- size path (K1) ---------------------------------------------------------
+// one table per load pair (N entries), sorted by descending N
+int prepare_size(wva_handle* h) {
+    PairTables& pt = h->size_tabs;
+    if (pt.holds(h->epoch_tokens)) return WVA_OK;
+    const HostFleet& hf = h->hf;
+    std::vector<int> pairs, Ns;
+    int rc = sorted_pairs(h, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
+    if (rc) return rc;
+    Cols c(16);
+    rc = upload_tables(h, pt, pairs, Ns, true, c, [](char*) {});
+    if (rc) return rc;
+    rc = build_tables(h, pt);
+    if (rc) return rc;
+    pt.epoch = h->epoch_tokens;
     return WVA_OK;
 }
 
@@ -562,17 +615,18 @@ int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners)
         trivial_kernel<<<(n_pairs + 255) / 256, 256, 0, h->stream>>>(h->df, cand, (const int*)nullptr, 1);
         h->launches++;
     }
+    const PairTables& pt = h->size_tabs;
     SizeArgs g{};
     g.f = h->df;
-    g.cand_pair = (const int*)h->d_cand_pair.p;
-    g.cand_N = (const int*)h->d_cand_N.p;
-    g.n_cand = (int)h->cand_pair.size();
-    g.tab = (const double*)h->d_sz_tab.p;
-    g.tab_off = (const long long*)h->d_sz_off.p;
-    g.ls = (const float*)h->d_sz_ls.p;
+    g.cand_pair = pt.pair();
+    g.cand_N = pt.len();
+    g.n_cand = pt.n;
+    g.tab = (const double*)pt.tab.p;
+    g.tab_off = pt.off();
+    g.ls = (const float*)pt.ls.p;
     g.place = CandPlace{nullptr, nullptr};
     g.cand = cand;
-    rc = enqueue_candidates(h, g, h->size_Nmax);
+    rc = enqueue_candidates(h, g, pt.len_max);
     if (rc) return rc;
     if (winners && hf.S > 0) {
         unlimited_kernel<<<(hf.S + 127) / 128, 128, 0, h->stream>>>(h->df, cand, *winners);
@@ -653,7 +707,7 @@ int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     HostCall c{(size_t)h->hf.S * h->hf.A, candidates != nullptr, winners != nullptr};
     const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
         const int rc = enqueue_size(h, dc, winners ? &dw : nullptr);
-        fb_cap = (long long)h->cand_pair.size() + 1;
+        fb_cap = (long long)h->size_tabs.n + 1;
         return rc;
     });
     if (rc) return rc;
@@ -664,14 +718,12 @@ int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
 
 // ---- size grid: CreateAllocation at every listed batch size --------------------------------------
 // The load pairs x the batch list, sorted by descending N (stable: pair order, then list order), with one
-// Bmax-long table per pair that the pair's candidates share.  Cached until the token statistics, the fleet or
-// the batch list change.
-int prepare_size_grid(wva_handle* h, int B, const int32_t* batch) {
-    if (h->sg_epoch == h->epoch_tokens && (int)h->sg_batch.size() == B &&
-        std::equal(h->sg_batch.begin(), h->sg_batch.end(), batch))
-        return WVA_OK;
-    h->sg_epoch = ~0ull;
+// Bmax-long table per pair that the pair's candidates share.  Enqueues the nil / zero-load candidates,
+// CreateAllocation for the load candidates, then values and the per-server winners.  cand ([S*A*B]) and winners
+// ([S]) are device columns.
+int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
+    PairTables& pt = h->sg_tabs;
     int Bmax = 1;
     for (int i = 0; i < B; ++i) Bmax = std::max(Bmax, batch[i]);
     std::vector<int> tab_pair;
@@ -686,71 +738,41 @@ int prepare_size_grid(wva_handle* h, int B, const int32_t* batch) {
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return batch[x % B] > batch[y % B]; });
     Cols c(16);
     const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_rec = c.take(4 * (size_t)n),
-                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_bl = c.take(4 * (size_t)B),
-                 o_tpair = c.take(4 * (size_t)n_tab), o_toff = c.take(8 * (size_t)n_tab), o_tlen = c.take(4 * (size_t)n_tab);
-    std::vector<char> host(c.bytes);
-    char* p = host.data();
-    for (int j = 0; j < n; ++j) {
-        const int t = order[j] / B, bi = order[j] % B;
-        ((int*)(p + o_pair))[j] = tab_pair[t];
-        ((int*)(p + o_N))[j] = batch[bi];
-        ((int*)(p + o_rec))[j] = tab_pair[t] * B + bi;
-        ((int*)(p + o_idx))[j] = t;
-        ((long long*)(p + o_off))[j] = (long long)t * Bmax;
-    }
-    if (B) memcpy(p + o_bl, batch, 4 * (size_t)B);
-    for (int t = 0; t < n_tab; ++t) {
-        ((int*)(p + o_tpair))[t] = tab_pair[t];
-        ((long long*)(p + o_toff))[t] = (long long)t * Bmax;
-        ((int*)(p + o_tlen))[t] = Bmax;
-    }
-    CK(h->d_sg_lists.ensure(c.bytes));
-    // pageable source: cudaMemcpyAsync has consumed it by the time it returns
-    CK(cudaMemcpyAsync(h->d_sg_lists.p, p, c.bytes, cudaMemcpyHostToDevice, h->stream));
-    if (n_tab) {
-        CK(h->d_sg_tab.ensure(sizeof(double) * 4 * (size_t)n_tab * Bmax));
-        CK(h->d_sg_ls.ensure(sizeof(float) * ((size_t)n_tab * Bmax + n_tab)));
-        const char* d = (const char*)h->d_sg_lists.p;
-        build_pair_tables<<<n_tab, 128, 0, h->stream>>>(h->df, (const int*)(d + o_tpair), (const long long*)(d + o_toff),
-                                                        (const int*)(d + o_tlen), n_tab, (double*)h->d_sg_tab.p,
-                                                        (float*)h->d_sg_ls.p, nullptr, 0, nullptr);
-        h->launches++;
-        CK(cudaGetLastError());
-    }
-    h->sg_pair = o_pair; h->sg_N = o_N; h->sg_rec = o_rec; h->sg_idx = o_idx; h->sg_off = o_off; h->sg_bl = o_bl;
-    h->sg_n = n;
-    h->sg_Bmax = Bmax;
-    h->sg_batch.assign(batch, batch + B);
-    h->sg_epoch = h->epoch_tokens;
-    return WVA_OK;
-}
-
-// Enqueue the size grid: nil / zero-load candidates, CreateAllocation for the load candidates, then values and the
-// per-server winners.  cand ([S*A*B]) and winners ([S]) are device columns.
-int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCols& cand, const AllocCols& winners) {
-    int rc = prepare_size_grid(h, B, batch);
+                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_bl = c.take(4 * (size_t)B);
+    int rc = upload_tables(h, pt, tab_pair, std::vector<int>(n_tab, Bmax), true, c, [&](char* p) {
+        for (int j = 0; j < n; ++j) {
+            const int t = order[j] / B, bi = order[j] % B;
+            ((int*)(p + o_pair))[j] = tab_pair[t];
+            ((int*)(p + o_N))[j] = batch[bi];
+            ((int*)(p + o_rec))[j] = tab_pair[t] * B + bi;
+            ((int*)(p + o_idx))[j] = t;
+            ((long long*)(p + o_off))[j] = (long long)t * Bmax;
+        }
+        if (B) memcpy(p + o_bl, batch, 4 * (size_t)B);
+    });
+    if (rc) return rc;
+    rc = build_tables(h, pt);
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
-    const HostFleet& hf = h->hf;
     const int n_rec = hf.S * hf.A * B;
-    const char* d = (const char*)h->d_sg_lists.p;
-    const int* d_batch = (const int*)(d + h->sg_bl);
+    const char* d = (const char*)pt.lists.p;
+    const int* d_batch = (const int*)(d + o_bl);
     if (n_rec > 0) {
         trivial_kernel<<<(n_rec + 255) / 256, 256, 0, h->stream>>>(h->df, cand, d_batch, B);
         h->launches++;
     }
     SizeArgs g{};
     g.f = h->df;
-    g.cand_pair = (const int*)(d + h->sg_pair);
-    g.cand_N = (const int*)(d + h->sg_N);
-    g.n_cand = h->sg_n;
-    g.tab = (const double*)h->d_sg_tab.p;
-    g.tab_off = (const long long*)(d + h->sg_off);
-    g.ls = (const float*)h->d_sg_ls.p;
-    g.place = CandPlace{(const int*)(d + h->sg_idx), (const int*)(d + h->sg_rec)};
+    g.cand_pair = (const int*)(d + o_pair);
+    g.cand_N = (const int*)(d + o_N);
+    g.n_cand = n;
+    g.tab = (const double*)pt.tab.p;
+    g.tab_off = (const long long*)(d + o_off);
+    g.ls = (const float*)pt.ls.p;
+    g.place = CandPlace{(const int*)(d + o_idx), (const int*)(d + o_rec)};
     g.cand = cand;
-    rc = enqueue_candidates(h, g, h->sg_Bmax);
+    rc = enqueue_candidates(h, g, Bmax);
     if (rc) return rc;
     if (hf.S > 0) {
         size_grid_finalize<<<(unsigned)((hf.S + 3) / 4), 128, 0, h->stream>>>(h->df, cand, d_batch, B, winners);
@@ -779,24 +801,14 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     if (rc) return rc;
     const int n = (int)pairs.size();
     const long long n_items = (long long)n * L;
+    PairTables& pt = h->lg_tabs;
     Cols c(16);
-    const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n),
-                 o_rpm = c.take(4 * (size_t)L * S);
-    std::vector<char> host(c.bytes);
-    char* p = host.data();
-    long long off = 0;
-    for (int j = 0; j < n; ++j) {
-        ((int*)(p + o_pair))[j] = pairs[j];
-        ((int*)(p + o_N))[j] = Ns[j];
-        ((long long*)(p + o_off))[j] = off;
-        off += Ns[j];
-    }
-    if ((size_t)L * S) memcpy(p + o_rpm, rpm, 4 * (size_t)L * S);
-    CK(h->d_lg_lists.ensure(c.bytes));
-    // pageable source: cudaMemcpyAsync has consumed it by the time it returns
-    CK(cudaMemcpyAsync(h->d_lg_lists.p, p, c.bytes, cudaMemcpyHostToDevice, h->stream));
-    const char* d = (const char*)h->d_lg_lists.p;
-    const float* d_rpm = (const float*)(d + o_rpm);
+    const size_t o_rpm = c.take(4 * (size_t)L * S);
+    rc = upload_tables(h, pt, pairs, Ns, true, c, [&](char* p) {
+        if ((size_t)L * S) memcpy(p + o_rpm, rpm, 4 * (size_t)L * S);
+    });
+    if (rc) return rc;
+    const float* d_rpm = (const float*)((const char*)pt.lists.p + o_rpm);
     rc = ensure_ctrl(h);
     if (rc) return rc;
     const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
@@ -810,14 +822,8 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     AllocCols star{};
     star.max_rate = (float*)h->d_lg_star.p;
     star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
-    if (n > 0) {
-        CK(h->d_lg_tab.ensure(sizeof(double) * 4 * (size_t)off));
-        CK(h->d_lg_ls.ensure(sizeof(float) * ((size_t)off + n)));
-        build_pair_tables<<<n, 128, 0, h->stream>>>(h->df, (const int*)(d + o_pair), (const long long*)(d + o_off),
-                                                    (const int*)(d + o_N), n, (double*)h->d_lg_tab.p,
-                                                    (float*)h->d_lg_ls.p, nullptr, 0, nullptr);
-        h->launches++;
-    }
+    rc = build_tables(h, pt);
+    if (rc) return rc;
     // the fallback lists of both phases share d_fb_list (phase 1's is consumed before load_kernel starts)
     const int fb2_list = (int)std::min<long long>(n_items, 1 << 22);
     fb_cap = (long long)n + 1;
@@ -825,15 +831,15 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     CK(h->d_fb_list.ensure(std::max(sizeof(int) * std::max(n, 1), sizeof(int2) * std::max(fb2_list, 1))));
     SizeArgs g{};
     g.f = h->df;
-    g.cand_pair = (const int*)(d + o_pair);
-    g.cand_N = (const int*)(d + o_N);
+    g.cand_pair = pt.pair();
+    g.cand_N = pt.len();
     g.n_cand = n;
-    g.tab = (const double*)h->d_lg_tab.p;
-    g.tab_off = (const long long*)(d + o_off);
-    g.ls = (const float*)h->d_lg_ls.p;
+    g.tab = (const double*)pt.tab.p;
+    g.tab_off = pt.off();
+    g.ls = (const float*)pt.ls.p;
     g.place = CandPlace{nullptr, nullptr};
     g.cand = star;
-    rc = enqueue_candidates(h, g, n ? Ns[0] : 1, true);
+    rc = enqueue_candidates(h, g, pt.len_max, true);
     if (rc) return rc;
     if (n > 0 && L > 0) {
         LoadArgs la{};
@@ -862,7 +868,7 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
         CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
         size_t slot_doubles;
         int Kmax;
-        rc = ensure_scratch(h, Ns[0], hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
+        rc = ensure_scratch(h, pt.len_max, hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
         if (rc) return rc;
         load_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(la, (double*)h->d_scratch.p, slot_doubles, Kmax,
                                                                (int*)h->d_ctrl.p + CTRL_FB_STATUS);
@@ -921,97 +927,70 @@ int ensure_cells(wva_handle* h, GridPlan& plan, const wva_cells* cells) {
 int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     const HostFleet& hf = h->hf;
     const int A = hf.A, S = hf.S, B = grid->n_batch, R = grid->n_replicas;
-    const bool same_grid = h->grid_epoch == h->epoch_tokens && (int)h->grid_batch.size() == B &&
-                           (int)h->grid_replicas.size() == R &&
-                           std::equal(h->grid_batch.begin(), h->grid_batch.end(), grid->batch) &&
-                           std::equal(h->grid_replicas.begin(), h->grid_replicas.end(), grid->replicas);
-    const int n_pairs = S * A;
+    const size_t n_pairs = std::max(S * A, 1);
     int Bmax = 1;
     for (int i = 0; i < B; ++i) Bmax = std::max(Bmax, grid->batch[i]);
-    // device lists: batch[B], batch_rank[B], rank_to_bi[B], replicas[R]
-    CK(h->d_grid_lists.ensure(sizeof(int) * (size_t)(3 * B + R + 1)));
-    CK(h->d_pair_tab.ensure((sizeof(long long) + sizeof(int)) * std::max(n_pairs, 1)));
-    long long* d_pair_off = (long long*)h->d_pair_tab.p;
-    int* d_pair_idx = (int*)(d_pair_off + std::max(n_pairs, 1));
-    if (!same_grid) {
-        // pageable sources: cudaMemcpyAsync has consumed them by the time it returns
-        std::vector<int> lists(3 * B + R + 1), tab_pair, tab_len, pair_idx(std::max(n_pairs, 1), -1);
-        std::vector<long long> pair_tab(std::max(n_pairs, 1), -1), tab_off;
-        h->grid_batch.assign(grid->batch, grid->batch + B);
-        h->grid_replicas.assign(grid->replicas, grid->replicas + R);
-        std::vector<int> order(B);
-        std::iota(order.begin(), order.end(), 0);
-        std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return grid->batch[x] < grid->batch[y]; });
-        for (int i = 0; i < B; ++i) {
-            lists[i] = grid->batch[i];
-            lists[B + order[i]] = i;      // batch_rank[bi]
-            lists[2 * B + i] = order[i];  // rank_to_bi[rank]
-        }
-        for (int i = 0; i < R; ++i) lists[3 * B + i] = grid->replicas[i];
-        if (3 * B + R > 0)
-            CK(cudaMemcpyAsync(h->d_grid_lists.p, lists.data(), sizeof(int) * (size_t)(3 * B + R), cudaMemcpyHostToDevice,
-                               h->stream));
+    // the grid's columns in the lists image: batch[B], batch_rank[B], rank_to_bi[B], replicas[R], then each pair's
+    // table offset and index (-1 without a table)
+    PairTables& pt = h->grid_tabs;
+    Cols c(16);
+    const size_t o_lists = c.take(sizeof(int) * (size_t)(3 * B + R)), o_poff = c.take(sizeof(long long) * n_pairs),
+                 o_pidx = c.take(sizeof(int) * n_pairs);
+    std::vector<int> key(grid->batch, grid->batch + B);
+    key.insert(key.end(), grid->replicas, grid->replicas + R);
+    key.push_back(B);
+    if (!pt.holds(h->epoch_tokens, key)) {
         // shared service-rate tables for every pair that carries load
-        long long off = 0;
+        std::vector<int> tab_pair;
         for (int s = 0; s < S; ++s)
             for (int a = 0; a < A; ++a)
-                if (hf.pair_class(s, a, true) == PAIR_LOAD && hf.srv_out_tokens[s] >= 1) {
-                    pair_tab[(size_t)s * A + a] = off;
-                    pair_idx[(size_t)s * A + a] = (int)tab_pair.size();
-                    tab_pair.push_back(s * A + a);
-                    tab_off.push_back(off);
-                    tab_len.push_back(Bmax);
-                    off += Bmax;
-                }
-        if (off > 0xffffffffll) return h->fail(WVA_ERR_UNSUPPORTED, "grid tables above 2^32 entries");
+                if (hf.pair_class(s, a, true) == PAIR_LOAD && hf.srv_out_tokens[s] >= 1) tab_pair.push_back(s * A + a);
         const int n_tab = (int)tab_pair.size();
-        CK(cudaMemcpyAsync(d_pair_off, pair_tab.data(), sizeof(long long) * std::max(n_pairs, 1), cudaMemcpyHostToDevice,
-                           h->stream));
-        CK(cudaMemcpyAsync(d_pair_idx, pair_idx.data(), sizeof(int) * std::max(n_pairs, 1), cudaMemcpyHostToDevice,
-                           h->stream));
-        if (n_tab) {
-            CK(h->d_tab_pair.ensure(sizeof(int) * n_tab));
-            CK(h->d_tab_off.ensure(sizeof(long long) * n_tab));
-            CK(h->d_tab_len.ensure(sizeof(int) * n_tab));
-            CK(h->d_tab.ensure(sizeof(double) * 4 * (size_t)off));
-            CK(h->d_ls.ensure(sizeof(float) * ((size_t)off + n_tab)));
-            CK(cudaMemcpyAsync(h->d_tab_pair.p, tab_pair.data(), sizeof(int) * n_tab, cudaMemcpyHostToDevice, h->stream));
-            CK(cudaMemcpyAsync(h->d_tab_off.p, tab_off.data(), sizeof(long long) * n_tab, cudaMemcpyHostToDevice, h->stream));
-            CK(cudaMemcpyAsync(h->d_tab_len.p, tab_len.data(), sizeof(int) * n_tab, cudaMemcpyHostToDevice, h->stream));
-        }
-        h->grid_n_tab = n_tab;
-        h->grid_Bmax = Bmax;
-        h->grid_epoch = h->epoch_tokens;
+        if ((long long)n_tab * Bmax > 0xffffffffll) return h->fail(WVA_ERR_UNSUPPORTED, "grid tables above 2^32 entries");
+        int rc = upload_tables(h, pt, tab_pair, std::vector<int>(n_tab, Bmax), true, c, [&](char* p) {
+            int* lists = (int*)(p + o_lists);
+            std::vector<int> order(B);
+            std::iota(order.begin(), order.end(), 0);
+            std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return grid->batch[x] < grid->batch[y]; });
+            for (int i = 0; i < B; ++i) {
+                lists[i] = grid->batch[i];
+                lists[B + order[i]] = i;      // batch_rank[bi]
+                lists[2 * B + i] = order[i];  // rank_to_bi[rank]
+            }
+            for (int i = 0; i < R; ++i) lists[3 * B + i] = grid->replicas[i];
+            long long* pair_off = (long long*)(p + o_poff);
+            int* pair_idx = (int*)(p + o_pidx);
+            std::fill(pair_off, pair_off + n_pairs, -1ll);
+            std::fill(pair_idx, pair_idx + n_pairs, -1);
+            for (int t = 0; t < n_tab; ++t) {
+                pair_off[tab_pair[t]] = (long long)t * Bmax;
+                pair_idx[tab_pair[t]] = t;
+            }
+        });
+        if (rc) return rc;
+        pt.epoch = h->epoch_tokens;
+        pt.key = std::move(key);
     }
-    // the tables are rebuilt on every call (only the host-side work lists are cached):
-    // they are part of the evaluation, not an input
     // [tables x batch] constants, then the [server x replica] rate block grid_rows fills (always allocated)
-    CK(h->d_pb.ensure(sizeof(float4) * ((size_t)h->grid_n_tab * std::max(B, 1) + (size_t)S * std::max(R, 1) + 1)));
-    if (h->grid_n_tab) {
-        float4* d_pb = (float4*)h->d_pb.p;
-        build_pair_tables<<<h->grid_n_tab, 128, 0, h->stream>>>(h->df, (const int*)h->d_tab_pair.p,
-                                                                (const long long*)h->d_tab_off.p,
-                                                                (const int*)h->d_tab_len.p, h->grid_n_tab,
-                                                                (double*)h->d_tab.p, (float*)h->d_ls.p,
-                                                                (const int*)h->d_grid_lists.p, B, d_pb);
-        h->launches += 1;
-        CK(cudaGetLastError());
-    }
+    CK(h->d_pb.ensure(sizeof(float4) * ((size_t)pt.n * std::max(B, 1) + (size_t)S * std::max(R, 1) + 1)));
+    const char* d = (const char*)pt.lists.p;
     GridArgs& g = plan->args;
     g = GridArgs{};
     g.f = h->df;
-    g.batch = (const int*)h->d_grid_lists.p;
+    g.batch = (const int*)(d + o_lists);
     g.batch_rank = g.batch + B;
     g.rank_to_bi = g.batch + 2 * B;
     g.replicas = g.batch + 3 * B;
+    int rc = build_tables(h, pt, g.batch, B, (float4*)h->d_pb.p);
+    if (rc) return rc;
     g.B = B;
     g.R = R;
-    g.tab = (const double*)h->d_tab.p;
-    g.ls = (const float*)h->d_ls.p;
-    g.pair_tab_off = d_pair_off;
-    g.pair_tab_idx = d_pair_idx;
+    g.tab = (const double*)pt.tab.p;
+    g.ls = (const float*)pt.ls.p;
+    g.pair_tab_off = (const long long*)(d + o_poff);
+    g.pair_tab_idx = (const int*)(d + o_pidx);
     g.pb = (const float4*)h->d_pb.p;
-    g.rt = (float4*)h->d_pb.p + (size_t)h->grid_n_tab * std::max(B, 1);
+    g.rt = (float4*)h->d_pb.p + (size_t)pt.n * std::max(B, 1);
     const unsigned long long n_cells = (unsigned long long)S * A * B * R;
     if (n_cells > 0xfffffff0ull) return h->fail(WVA_ERR_UNSUPPORTED, "grid too large for one call (>= 2^32 cells)");
     g.n_cells = (long long)n_cells;
@@ -1050,7 +1029,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     // grid_order ranks a server's rows in shared memory, and a cell's key holds the accelerator in 8 bits and the batch
     // size in 24; outside those limits every cell is evaluated (grid_order still walks the shared runs)
     g.prune = A <= 256 && Bmax < (1 << 24) && (long long)A * R <= kOrderMaxRows;
-    g.Bmax = h->grid_Bmax;
+    g.Bmax = Bmax;
     g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
     g.fb_cap = (int)std::min<size_t>(nc, (size_t)1 << 22);
     CK(h->d_fb_list.ensure(sizeof(long long) * g.fb_cap));
@@ -1364,7 +1343,7 @@ int run_greedy_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) 
     HostCall c{(size_t)hf.S * hf.A, true, false};
     const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
         const int rc = enqueue_size(h, dc, &dw);  // the unlimited kernel also assigns value = transition penalty
-        fb_cap = (long long)h->cand_pair.size() + 1;
+        fb_cap = (long long)h->size_tabs.n + 1;
         return rc;
     });
     if (rc) return rc;
@@ -1435,16 +1414,6 @@ void wva_destroy(wva_handle* h) {
     if (!h) return;
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    DevBuf* bufs[] = {&h->arena, &h->d_cand_pair, &h->d_cand_N, &h->d_sz_tab, &h->d_sz_ls, &h->d_sz_off, &h->d_sz_state, &h->d_sz_req, &h->d_sz_sort,
-                      &h->d_sg_lists, &h->d_sg_tab, &h->d_sg_ls, &h->d_lg_lists, &h->d_lg_tab, &h->d_lg_ls, &h->d_lg_star,
-                      &h->d_grid_lists,
-                      &h->d_pair_tab, &h->d_tab_pair, &h->d_tab_off, &h->d_tab_len, &h->d_tab, &h->d_ls, &h->d_sort, &h->d_best, &h->d_pb, &h->d_rows,
-                      &h->d_cand_block, &h->d_win_block, &h->d_ctrl, &h->d_fb_list, &h->d_scratch,
-                      &h->d_cells, &h->d_sweep, &h->d_summary, &h->d_dbg};
-    for (DevBuf* b : bufs) b->release();
-    h->stage.release();
-    h->out_stage.release();
-    h->sz_pin.release();
     if (h->ev_k0) cudaEventDestroy(h->ev_k0);
     if (h->ev_k1) cudaEventDestroy(h->ev_k1);
     if (h->ev_d0) cudaEventDestroy(h->ev_d0);
@@ -1750,7 +1719,7 @@ int wva_size_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_batch, const 
     HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_batch, candidates != nullptr, true};
     rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
         const int rc = enqueue_size_grid(h, n_batch, batch, dc, dw);
-        fb_cap = (long long)h->sg_n + 1;
+        fb_cap = (long long)h->sg_tabs.n * n_batch + 1;
         return rc;
     });
     if (rc) return rc;
@@ -1932,12 +1901,6 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
                       pairs, lens);
     if (rc) return rc;
     const int n = (int)pairs.size();
-    std::vector<long long> offs(n);
-    long long off = 0;
-    for (int e = 0; e < n; ++e) {
-        offs[e] = off;
-        off += lens[e];
-    }
     const size_t n_out = (size_t)S * A * n_rates;
     Cols sw(256);
     const size_t o_valid = sw.take(n_out, out->valid), o_rate = sw.take(4 * n_out, out->rate),
@@ -1950,24 +1913,19 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
     CK(cudaEventRecord(h->ev_k0, h->stream));
     int fb_cap = 0;
     if (n) {
-        CK(h->d_tab_pair.ensure(sizeof(int) * n));
-        CK(h->d_tab_off.ensure(sizeof(long long) * n));
-        CK(h->d_tab_len.ensure(sizeof(int) * n));
-        CK(h->d_tab.ensure(sizeof(double) * 4 * (size_t)off));
-        CK(cudaMemcpyAsync(h->d_tab_pair.p, pairs.data(), sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->d_tab_off.p, offs.data(), sizeof(long long) * n, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->d_tab_len.p, lens.data(), sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-        h->grid_epoch = ~0ull;  // the shared-table buffers now hold sweep tables
-        build_pair_tables<<<n, 128, 0, h->stream>>>(h->df, (const int*)h->d_tab_pair.p, (const long long*)h->d_tab_off.p,
-                                                    (const int*)h->d_tab_len.p, n, (double*)h->d_tab.p, nullptr,
-                                                    nullptr, 0, nullptr);
-        h->launches++;
+        // the grid's tables, without the ls column: a sweep holds no device memory of its own for them
+        PairTables& pt = h->grid_tabs;
+        Cols c(16);
+        rc = upload_tables(h, pt, pairs, lens, false, c, [](char*) {});
+        if (rc) return rc;
+        rc = build_tables(h, pt);
+        if (rc) return rc;
         SweepArgs g{};
         g.f = h->df;
-        g.pair_list = (const int*)h->d_tab_pair.p;
-        g.pair_N = (const int*)h->d_tab_len.p;
-        g.tab_off = (const long long*)h->d_tab_off.p;
-        g.tab = (const double*)h->d_tab.p;
+        g.pair_list = pt.pair();
+        g.pair_N = pt.len();
+        g.tab_off = pt.off();
+        g.tab = (const double*)pt.tab.p;
         g.n_pairs = n;
         g.n_rates = n_rates;
         g.n_chunks = (n_rates + 31) / 32;
