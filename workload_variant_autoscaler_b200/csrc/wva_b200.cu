@@ -201,7 +201,7 @@ struct wva_handle {
     // grid path
     DevBuf d_sort, d_best, d_pb, d_rows;
     // shared
-    DevBuf d_cand_block, d_win_block, d_ctrl, d_fb_list, d_scratch, d_cells, d_sweep, d_dbg;
+    DevBuf d_cand_block, d_win_block, d_ctrl, d_fb_list[2], d_scratch, d_cells, d_sweep, d_dbg;
     // peer exchange of the winner block (multi-GPU, one process per GPU on one node)
     struct Xchg {
         int world = 0, rank = 0;
@@ -243,7 +243,9 @@ namespace {
 
 // control block on the device: a handful of ints
 // CTRL_FB2_COUNT: a second fallback list of the same call (the load grid's tail items)
-enum { CTRL_COUNTER = 0, CTRL_FB_COUNT = 1, CTRL_FB_STATUS = 2, CTRL_FB2_COUNT = 3, CTRL_INTS = 8 };
+enum {
+    CTRL_COUNTER = 0, CTRL_FB_COUNT = 1, CTRL_FB_STATUS = 2, CTRL_FB2_COUNT = 3, CTRL_FB_OVERFLOW = 4, CTRL_INTS = 8
+};
 
 // ---- SoA result blocks: the wva_allocs columns of n records, 16-byte aligned ----------------
 struct Block {
@@ -363,13 +365,31 @@ int ensure_ctrl(wva_handle* h) {
     return WVA_OK;
 }
 
-// Scratch for the stored-vector fallback kernels: a fixed number of slots.
+// The stored-vector fallback (DESIGN.md §3.2): a call has up to two lists (the load grid's two phases), each with
+// its own count and buffer, re-run by a fixed number of threads with one scratch slot each.
 constexpr int kFbBlocks = 2, kFbThreads = 64, kFbSlots = kFbBlocks * kFbThreads;
-int ensure_scratch(wva_handle* h, int Nmax, int ratio, size_t* slot_doubles, int* Kmax) {
-    *Kmax = Nmax + Nmax * ratio;
-    *slot_doubles = (size_t)*Kmax + 1 + ((size_t)Nmax + 1) / 2 + 1;
-    CK(h->d_scratch.ensure(*slot_doubles * sizeof(double) * kFbSlots));
+constexpr int kFbCount[2] = {CTRL_FB_COUNT, CTRL_FB2_COUNT};
+
+// List `list` (0 or 1) of up to cap entries, and the scratch for chains of batch size up to Nmax.  Called before the
+// kernels that use them are enqueued: a DevBuf that grows frees its old memory, and cudaFree synchronises.
+int prepare_fallback(wva_handle* h, int list, int cap, int Nmax, FbRun& r) {
+    CK(h->d_fb_list[list].ensure(sizeof(unsigned long long) * std::max(cap, 1)));
+    const int Kmax = Nmax + Nmax * h->hf.tun.max_queue_to_batch_ratio;
+    CK(h->d_scratch.ensure(sizeof(double) * ((size_t)Kmax + 1) * kFbSlots));
+    int* ctrl = (int*)h->d_ctrl.p;
+    r.list = FbList{ctrl + kFbCount[list], (unsigned long long*)h->d_fb_list[list].p, cap};
+    r.scratch = (double*)h->d_scratch.p;
+    r.Kmax = Kmax;
+    r.status = ctrl + CTRL_FB_STATUS;
+    r.overflow = ctrl + CTRL_FB_OVERFLOW;
     return WVA_OK;
+}
+
+// Enqueues a re-run kernel (grid_fallback, size_fallback, ...) over r's list.
+template <class Args>
+void launch_fallback(wva_handle* h, void (*kernel)(Args, FbRun), const Args& g, const FbRun& r) {
+    kernel<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, r);
+    h->launches++;
 }
 
 // The (server, accelerator) pairs that keep(s, a) accepts, as ids s * A + a with their batch sizes N, sorted
@@ -535,7 +555,7 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
     g.ws.order = (unsigned*)(wp + w_order); g.ws.items = (unsigned long long*)(wp + w_items);
     g.ws.items_sorted = (unsigned long long*)(wp + w_sorted); g.ws.item_count = (unsigned*)(wp + w_cnt);
     g.cand = sa.cand;
-    g.fb_count = sa.fb_count; g.fb_list = sa.fb_list; g.fb_cap = sa.fb_cap;
+    g.fb = sa.fb;
 
     const unsigned nb = (unsigned)((n + 255) / 256);
     const unsigned cks = (unsigned)chunks, items_blocks = (unsigned)((max_items + 255) / 256),
@@ -573,10 +593,10 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
 // as the call's kernel, then the stored-vector fallback.
 int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, bool star = false) {
     const int n = g.n_cand;
-    g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
-    CK(h->d_fb_list.ensure(sizeof(int) * std::max(n, 1)));
-    g.fb_list = (int*)h->d_fb_list.p;
-    g.fb_cap = std::max(n, 1);
+    FbRun fb;
+    const int rc = prepare_fallback(h, 0, n, Nmax, fb);
+    if (rc) return rc;
+    g.fb = fb.list;
     CK(cudaEventRecord(h->ev_k0, h->stream));
     int small_max = 1024;  // up to here a warp per candidate beats rounds (the GPU is mostly empty either way)
     if (const char* e = getenv("WVA_SIZE_SMALL_MAX")) small_max = atoi(e);
@@ -589,16 +609,7 @@ int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, bool star = false) 
         if (rc) return rc;
     }
     CK(cudaEventRecord(h->ev_k1, h->stream));
-    if (n > 0) {
-        size_t slot_doubles;
-        int Kmax;
-        const int rc = ensure_scratch(h, Nmax, h->hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
-        if (rc) return rc;
-        auto* fallback = star ? size_fallback_star : size_fallback;
-        fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
-                                                          (int*)h->d_ctrl.p + CTRL_FB_STATUS);
-        h->launches++;
-    }
+    if (n > 0) launch_fallback(h, star ? size_fallback_star : size_fallback, g, fb);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -653,7 +664,6 @@ struct HostCall {
     const Cols* extra = nullptr;    // further device columns copied straight to their destinations ...
     const void* extra_dev = nullptr;  // ... from this buffer
     size_t win_blocks = 1;          // winner blocks of S records
-    long long fb2_cap = 0;          // largest count of the second fallback list that is not an error
     // set by run_host: the block layouts and their host copies in out_stage (NULL when not copied)
     Block bc{}, bw{};
     const char *cand_host = nullptr, *win_host = nullptr;
@@ -661,8 +671,8 @@ struct HostCall {
 
 // The shared end of every call with host results, in stream order: place the blocks on the device, record
 // ev_d0, enqueue the work, copy the wanted blocks and the control ints into out_stage and then c.extra,
-// synchronise once and check the fallback status.  enqueue(dc, dw, fb_cap) enqueues the kernels into the
-// device blocks and sets the largest fallback count that is not an error.
+// synchronise once and check the fallback's status words.  enqueue(dc, dw) enqueues the kernels into the device
+// blocks.
 template <class Enqueue>
 int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
     const HostFleet& hf = h->hf;
@@ -673,8 +683,7 @@ int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
     const AllocCols dc = c.n_cand ? block_cols(h->d_cand_block.p, c.bc) : AllocCols{};
     const AllocCols dw = block_cols(h->d_win_block.p, c.bw);
     CK(cudaEventRecord(h->ev_d0, h->stream));
-    long long fb_cap = 0;
-    int rc = enqueue(dc, dw, fb_cap);
+    int rc = enqueue(dc, dw);
     if (rc) return rc;
     Cols stage(256);
     const size_t o_cand = stage.take(c.copy_cand ? c.bc.bytes : 0), o_win = stage.take(c.copy_win ? c.bw.bytes : 0),
@@ -696,8 +705,8 @@ int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
     if (rc) return rc;
     if (ctrl[CTRL_FB_STATUS] != 0)
         return h->fail(WVA_ERR_UNSUPPORTED, "input outside the supported numeric domain (rescale loop does not terminate)");
-    if ((long long)ctrl[CTRL_FB_COUNT] > fb_cap || (long long)ctrl[CTRL_FB2_COUNT] > c.fb2_cap)
-        return h->fail(WVA_ERR_UNSUPPORTED, "too many cells need the stored-vector fallback");
+    if (ctrl[CTRL_FB_OVERFLOW] != 0)
+        return h->fail(WVA_ERR_UNSUPPORTED, "too many entries need the stored-vector fallback");
     return WVA_OK;
 }
 
@@ -705,10 +714,8 @@ int run_host(wva_handle* h, HostCall& c, Enqueue&& enqueue) {
 int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     if (!h->resident) return h->fail(WVA_ERR_STATE, "no resident fleet (call wva_upload first)");
     HostCall c{(size_t)h->hf.S * h->hf.A, candidates != nullptr, winners != nullptr};
-    const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
-        const int rc = enqueue_size(h, dc, winners ? &dw : nullptr);
-        fb_cap = (long long)h->size_tabs.n + 1;
-        return rc;
+    const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_size(h, dc, winners ? &dw : nullptr);
     });
     if (rc) return rc;
     scatter_block(c.cand_host, c.bc, candidates);
@@ -786,10 +793,8 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
 // Phase 1 sizes each candidate once: the pairs that pass the gates and are a load at some level, sorted by
 // descending N with one N-entry table each, run through the size drivers in rateStar mode.  Phase 2 (load_kernel,
 // load_fallback) is the tail per (candidate, level).  rpm [L*S] is the caller's level list; cand ([L*S*A]) and
-// winners ([L*S]) are device columns.  Sets the largest counts of the two phases' fallback lists that are not an
-// error.
-int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& cand, const AllocCols& winners,
-                      long long& fb_cap, long long& fb2_cap) {
+// winners ([L*S]) are device columns.
+int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     std::vector<char> loaded(S, 0);  // server s is a load at some level (NaN and +Inf included)
@@ -824,11 +829,10 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
     rc = build_tables(h, pt);
     if (rc) return rc;
-    // the fallback lists of both phases share d_fb_list (phase 1's is consumed before load_kernel starts)
-    const int fb2_list = (int)std::min<long long>(n_items, 1 << 22);
-    fb_cap = (long long)n + 1;
-    fb2_cap = fb2_list;
-    CK(h->d_fb_list.ensure(std::max(sizeof(int) * std::max(n, 1), sizeof(int2) * std::max(fb2_list, 1))));
+    // phase 2's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
+    FbRun fb2;
+    rc = prepare_fallback(h, 1, (int)std::min<long long>(n_items, 1 << 22), pt.len_max, fb2);
+    if (rc) return rc;
     SizeArgs g{};
     g.f = h->df;
     g.cand_pair = pt.pair();
@@ -855,9 +859,7 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
         la.cand = cand;
-        la.fb_count = (int*)h->d_ctrl.p + CTRL_FB2_COUNT;
-        la.fb_points = (int2*)h->d_fb_list.p;
-        la.fb_cap = fb2_list;
+        la.fb = fb2.list;
         int per_sm = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, load_kernel, 256, 0));
         per_sm = std::max(1, std::min(per_sm, 8));
@@ -866,13 +868,7 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
         load_kernel<<<blocks, 256, 0, h->stream>>>(la);
         h->launches++;
         CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
-        size_t slot_doubles;
-        int Kmax;
-        rc = ensure_scratch(h, pt.len_max, hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
-        if (rc) return rc;
-        load_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(la, (double*)h->d_scratch.p, slot_doubles, Kmax,
-                                                               (int*)h->d_ctrl.p + CTRL_FB_STATUS);
-        h->launches++;
+        launch_fallback(h, load_fallback, la, fb2);
     }
     if (S > 0 && L > 0) {
         unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
@@ -898,6 +894,7 @@ int validate_grid(wva_handle* h, const wva_grid* g) {
 
 struct GridPlan {
     GridArgs args;
+    FbRun fb;
     size_t n_cells;
     int n_blocks;
     int Bmax;
@@ -1030,10 +1027,11 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     // size in 24; outside those limits every cell is evaluated (grid_order still walks the shared runs)
     g.prune = A <= 256 && Bmax < (1 << 24) && (long long)A * R <= kOrderMaxRows;
     g.Bmax = Bmax;
-    g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
-    g.fb_cap = (int)std::min<size_t>(nc, (size_t)1 << 22);
-    CK(h->d_fb_list.ensure(sizeof(long long) * g.fb_cap));
-    g.fb_cells = (long long*)h->d_fb_list.p;
+    rc = prepare_fallback(h, 0, (int)std::min<size_t>(nc, (size_t)1 << 22), Bmax, plan->fb);
+    if (rc) return rc;
+    g.fb_count = plan->fb.list.count;
+    g.fb_cells = plan->fb.list.item;
+    g.fb_cap = plan->fb.list.cap;
     {
         // grid_kernel's long queue: items of at least ~min_len states, at most long_per_sm per SM
         const int min_len = 1024;
@@ -1058,10 +1056,6 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
 int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
     GridArgs& g = plan.args;
     const HostFleet& hf = h->hf;
-    size_t slot_doubles;
-    int Kmax;
-    int rc = ensure_scratch(h, plan.Bmax, hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
-    if (rc) return rc;
     if (plan.n_cells == 0) CK(cudaEventRecord(h->ev_k0, h->stream));
     if (plan.n_cells > 0) {
         CK(cudaMemsetAsync(g.item_count, 0, sizeof(unsigned) * (2 * kClasses + 32), h->stream));
@@ -1088,9 +1082,7 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
     }
     CK(cudaEventRecord(h->ev_k1, h->stream));
     if (plan.n_cells > 0) {
-        grid_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
-                                                               (int*)h->d_ctrl.p + CTRL_FB_STATUS);
-        h->launches++;
+        launch_fallback(h, grid_fallback, g, plan.fb);
         if (g.want_cells) {  // the shared-chain cells with a cell table: one warp per 32 rows and slice of ranks
             const size_t n_warps = ((size_t)hf.S * hf.A * g.R + 31) / 32 * ((size_t)(g.B + kSharedSlice - 1) / kSharedSlice);
             const unsigned ctas = (unsigned)((n_warps + kSharedThreads / 32 - 1) / (kSharedThreads / 32));
@@ -1341,10 +1333,8 @@ int run_greedy_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) 
     if (!hf.every_acc_typed())
         return h->fail(WVA_ERR_BAD_ARG, "limited mode needs a type id and a capacity for every accelerator");
     HostCall c{(size_t)hf.S * hf.A, true, false};
-    const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
-        const int rc = enqueue_size(h, dc, &dw);  // the unlimited kernel also assigns value = transition penalty
-        fb_cap = (long long)h->size_tabs.n + 1;
-        return rc;
+    const int rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_size(h, dc, &dw);  // the unlimited kernel also assigns value = transition penalty
     });
     if (rc) return rc;
     std::vector<HostCand> cand, win((size_t)hf.S);
@@ -1694,10 +1684,7 @@ int wva_grid_solve(wva_handle* h, const wva_fleet* fleet, const wva_grid* grid, 
     if (plan.args.want_cells && plan.n_cells)  // cells that are never analysed must read back as 0
         CK(cudaMemsetAsync(h->d_cells.p, 0, plan.cells.bytes, h->stream));
     HostCall c{0, false, true, &plan.cells, h->d_cells.p};
-    rc = run_host(h, c, [&](const AllocCols&, const AllocCols& dw, long long& fb_cap) {
-        fb_cap = plan.args.fb_cap;
-        return enqueue_grid(h, plan, dw);
-    });
+    rc = run_host(h, c, [&](const AllocCols&, const AllocCols& dw) { return enqueue_grid(h, plan, dw); });
     if (rc) return rc;
     scatter_block(c.win_host, c.bw, winners);
     h->last_kind = 1;
@@ -1717,10 +1704,8 @@ int wva_size_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_batch, const 
     int rc = upload_fleet(h, fleet);
     if (rc) return rc;
     HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_batch, candidates != nullptr, true};
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
-        const int rc = enqueue_size_grid(h, n_batch, batch, dc, dw);
-        fb_cap = (long long)h->sg_tabs.n * n_batch + 1;
-        return rc;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_size_grid(h, n_batch, batch, dc, dw);
     });
     if (rc) return rc;
     scatter_block(c.cand_host, c.bc, candidates);
@@ -1742,8 +1727,8 @@ int wva_load_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const
     if (rc) return rc;
     HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
     c.win_blocks = (size_t)n_levels;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw, long long& fb_cap) {
-        return enqueue_load_grid(h, n_levels, arrival_rpm, dc, dw, fb_cap, c.fb2_cap);
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_load_grid(h, n_levels, arrival_rpm, dc, dw);
     });
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;
@@ -1909,16 +1894,23 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
     CK(h->d_sweep.ensure(sw.bytes));
     char* p = (char*)h->d_sweep.p;
     CK(cudaMemsetAsync(p, 0, sw.bytes, h->stream));
-    CK(cudaEventRecord(h->ev_d0, h->stream));
-    CK(cudaEventRecord(h->ev_k0, h->stream));
-    int fb_cap = 0;
-    if (n) {
+    HostCall call{0, false, false, &sw, p};
+    call.win_blocks = 0;
+    return run_host(h, call, [&](const AllocCols&, const AllocCols&) {
+        if (!n) {
+            CK(cudaEventRecord(h->ev_k0, h->stream));
+            CK(cudaEventRecord(h->ev_k1, h->stream));
+            return WVA_OK;
+        }
         // the grid's tables, without the ls column: a sweep holds no device memory of its own for them
         PairTables& pt = h->grid_tabs;
         Cols c(16);
-        rc = upload_tables(h, pt, pairs, lens, false, c, [](char*) {});
+        int rc = upload_tables(h, pt, pairs, lens, false, c, [](char*) {});
         if (rc) return rc;
         rc = build_tables(h, pt);
+        if (rc) return rc;
+        FbRun fb;
+        rc = prepare_fallback(h, 0, (int)std::min<size_t>((size_t)n * n_rates, (size_t)1 << 22), lens[0], fb);
         if (rc) return rc;
         SweepArgs g{};
         g.f = h->df;
@@ -1936,11 +1928,7 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         g.itl = (float*)(p + o_itl);
         g.throughput = (float*)(p + o_thr);
         g.rho = (float*)(p + o_rho);
-        g.fb_count = (int*)h->d_ctrl.p + CTRL_FB_COUNT;
-        fb_cap = (int)std::min<size_t>((size_t)n * n_rates, (size_t)1 << 22);
-        CK(h->d_fb_list.ensure(sizeof(int2) * fb_cap));
-        g.fb_points = (int2*)h->d_fb_list.p;
-        g.fb_cap = fb_cap;
+        g.fb = fb.list;
         int per_sm = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sweep_kernel, 256, 0));
         per_sm = std::max(1, std::min(per_sm, 8));
@@ -1951,28 +1939,10 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         h->launches++;
         CK(cudaEventRecord(h->ev_k1, h->stream));
         // the points whose chain left the streaming solve's window: stored vector, as the reference
-        size_t slot_doubles;
-        int Kmax;
-        rc = ensure_scratch(h, lens[0], hf.tun.max_queue_to_batch_ratio, &slot_doubles, &Kmax);
-        if (rc) return rc;
-        sweep_fallback<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, (double*)h->d_scratch.p, slot_doubles, Kmax,
-                                                                (int*)h->d_ctrl.p + CTRL_FB_STATUS);
-        h->launches++;
+        launch_fallback(h, sweep_fallback, g, fb);
         CK(cudaGetLastError());
-    } else {
-        CK(cudaEventRecord(h->ev_k1, h->stream));
-    }
-    CK(h->out_stage.ensure(256));
-    int* ctrl_host = (int*)h->out_stage.p;
-    CK(cudaMemcpyAsync(ctrl_host, h->d_ctrl.p, CTRL_INTS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(sw.copy_back(p, h->stream));
-    rc = finish_timing(h);
-    if (rc) return rc;
-    if (ctrl_host[CTRL_FB_STATUS] != 0)
-        return h->fail(WVA_ERR_UNSUPPORTED, "input outside the supported numeric domain (rescale loop does not terminate)");
-    if ((long long)ctrl_host[CTRL_FB_COUNT] > fb_cap)
-        return h->fail(WVA_ERR_UNSUPPORTED, "too many sweep points need the stored-vector fallback");
-    return WVA_OK;
+        return WVA_OK;
+    });
 }
 
 // ---- self-check of the exact-division primitive (not part of the public ABI) ------------------

@@ -875,14 +875,15 @@ __device__ __forceinline__ int solve_private(const double* __restrict__ tab, int
 
 // Stored-vector fallback: a literal restatement of computeProbabilities /
 // computeStatistics on a scratch p[0..K] in global memory, including the overflow
-// rescale loops.  Used only for cells the streaming solve bailed out of.
+// rescale loops.  Used only for cells the streaming solve bailed out of.  tab is the
+// entry's service-rate table; column 0 is float32 servRate widened to double.
 // Returns 0 ok, 2 = the reference's rescale loop would not terminate (unsupported input).
-__device__ __noinline__ int solve_stored(double* p, const float* serv_rate, int N, int K, float lambda, ModelStats& st) {
+__device__ __noinline__ int solve_stored(double* p, const double* tab, int N, int K, float lambda, ModelStats& st) {
     const double lam = (double)lambda;
     p[0] = 1.0;
     const double scale = __ddiv_rn(1.7976931348623157e308, (double)K);
     for (int n = 0; n < K; ++n) {
-        const double s_rate = (double)serv_rate[n < N ? n : N - 1];
+        const double s_rate = tab[4 * (n < N ? n : N - 1)];
         double v = __ddiv_rn(__dmul_rn(p[n], lam), s_rate);
         int guard = 0;
         while (v < 0.0 || isinf(v) || isnan(v)) {
@@ -919,6 +920,49 @@ __device__ __noinline__ int solve_stored(double* p, const float* serv_rate, int 
     if (w < 0.0f) w = 0.0f;
     st.avg_wait_time = w;
     return 0;
+}
+
+// The entries a streaming kernel bailed on, for the stored-vector re-run.  Each path packs its entry into 64 bits
+// (fb_pack for two ints).  An append past cap is counted but not stored; fb_rerun reports it.
+struct FbList {
+    int* count;
+    unsigned long long* item;
+    int cap;
+};
+__device__ __forceinline__ void fb_push(const FbList& l, unsigned long long item) {
+    const int k = atomicAdd(l.count, 1);
+    if (k < l.cap) l.item[k] = item;
+}
+__device__ __forceinline__ unsigned long long fb_pack(int hi, int lo) {
+    return (unsigned long long)(unsigned)hi << 32 | (unsigned)lo;
+}
+
+// What a re-run kernel needs besides its path's arguments: the list, one scratch slot of Kmax + 1 doubles per
+// thread (p[0..K] of solve_stored) and the two status words the host checks after the call.
+struct FbRun {
+    FbList list;
+    double* scratch;
+    int Kmax;
+    int* status;    // solve_stored's code of a solve that failed
+    int* overflow;  // 1: the list had more entries than its cap
+};
+
+// The re-run loop: thread `slot` takes list entries slot, slot + n_slots, ...; body(item, p) re-runs one entry on
+// scratch p and returns solve_stored's code (0: ok).
+template <class Body>
+__device__ __forceinline__ void fb_rerun(const FbRun& r, Body&& body) {
+    const int n_slots = gridDim.x * blockDim.x;
+    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+    int n = *r.list.count;
+    if (n > r.list.cap) {
+        if (slot == 0) *r.overflow = 1;
+        n = r.list.cap;
+    }
+    double* p = r.scratch + (size_t)slot * ((size_t)r.Kmax + 1);
+    for (int k = slot; k < n; k += n_slots) {
+        const int rc = body(r.list.item[k], p);
+        if (rc != 0) atomicExch(r.status, rc);
+    }
 }
 
 // ---------------------------------------------------------------------------

@@ -392,8 +392,10 @@ struct GridArgs {
     int prune;               // grid_order ranks the rows (A <= 256, Bmax < 2^24, A*R <= kOrderMaxRows; want_cells == 0)
     unsigned* row_grp;       // [S*A*R] group rank of the row: rows of the server strictly below it in (value, cost, replicas)
     unsigned long long* bound;  // [S] smallest key of a feasible cell found so far (kBoundOff: no pruning)
-    int* fb_count;           // cells that need the stored-vector fallback
-    long long* fb_cells;
+    // cells that need the stored-vector fallback: an FbList's fields, kept flat so that the ints below keep their
+    // parameter offsets (a nested FbList pads to 24 bytes)
+    int* fb_count;
+    unsigned long long* fb_cells;
     int fb_cap;
     int long_per_sm;         // grid_kernel: long items per sub-partition 0 (< 0: chosen per launch by grid_items_plan)
     int n_ctas;              // CTAs of grid_kernel (= SMs)
@@ -1196,8 +1198,7 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
     __syncwarp();
     if (valid) {
         if (rc != kSolveOk) {
-            const int k = atomicAdd(g.fb_count, 1);
-            if (k < g.fb_cap) g.fb_cells[k] = (long long)cell;
+            fb_push(FbList{g.fb_count, g.fb_cells, g.fb_cap}, cell);
         } else {
             const float4 r0 = one_pair ? pair_buf[0] : g.pair_rec[3 * (size_t)pair + 0];
             const float4 r1 = one_pair ? pair_buf[1] : g.pair_rec[3 * (size_t)pair + 1];
@@ -1279,37 +1280,25 @@ __global__ void __launch_bounds__(kGkThreads, 1) grid_kernel(GridArgs g) {
     }
 }
 
-// Stored-vector re-run of bailed cells. One thread per slot; slot k handles cells
-// k, k + n_slots, ...  scratch per slot: (Kmax + 1) doubles then Nmax floats.
-__global__ void grid_fallback(GridArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+// Stored-vector re-run of the cells grid_kernel bailed on (r.list holds cell ids).
+__global__ void grid_fallback(GridArgs g, FbRun r) {
     const DevFleet& f = g.f;
-    const int n_slots = gridDim.x * blockDim.x;
-    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
-    int n = *g.fb_count;
-    if (n > g.fb_cap) n = g.fb_cap;
-    double* p = scratch + (size_t)slot * slot_doubles;
-    float* sr = (float*)(p + Kmax + 1);  // servRate copy lives behind the p[0..Kmax] vector
-    for (int k = slot; k < n; k += n_slots) {
-        const long long cell = g.fb_cells[k];
+    fb_rerun(r, [&](unsigned long long cell, double* p) {
         int s, a, bi, ri;
-        decode_cell(g, cell, s, a, bi, ri);
-        const int b = g.batch[bi], r = g.replicas[ri];
+        decode_cell(g, (long long)cell, s, a, bi, ri);
+        const int b = g.batch[bi], rep = g.replicas[ri];
         const double* tab = g.tab + 4 * g.pair_tab_off[s * f.A + a];
-        for (int i = 0; i < b; ++i) sr[i] = (float)tab[4 * i];
-        const float rmax = rate_max_of(sr[b - 1]);
-        const float rate = __fdiv_rn(total_rate_of(f, s), (float)r);
+        const float rate = __fdiv_rn(total_rate_of(f, s), (float)rep);
         ModelStats st;
-        const int rc = solve_stored(p, sr, b, b + b * f.ratio, __fdiv_rn(rate, 1000.0f), st);
-        if (rc != 0) {
-            atomicExch(fb_status, rc);
-            continue;
-        }
-        const QParams q = qparams_of(f, s, a);
-        const Metrics m = metrics_from(q, b, st);
-        const bool feas = cell_feasible(feas_row(f, s, rmax), r, __fdiv_rn(rate, 1000.0f), m);
-        store_cell(g, cell, 1, feas ? 1 : 0, m);
+        const int rc = solve_stored(p, tab, b, b + b * f.ratio, __fdiv_rn(rate, 1000.0f), st);
+        if (rc != 0) return rc;
+        const Metrics m = metrics_from(qparams_of(f, s, a), b, st);
+        const float rmax = rate_max_of((float)tab[4 * (b - 1)]);
+        const bool feas = cell_feasible(feas_row(f, s, rmax), rep, __fdiv_rn(rate, 1000.0f), m);
+        store_cell(g, (long long)cell, 1, feas ? 1 : 0, m);
         if (feas) atomicMin(&g.best_rank[((size_t)s * f.A + a) * g.R + ri], g.batch_rank[bi]);
-    }
+        return 0;
+    });
 }
 
 // With a cell table, the cells that share their row's chain (analysable, b >= jl + 2, K < 2^23), after grid_kernel
@@ -1794,9 +1783,7 @@ struct SweepArgs {
     unsigned* counter;
     uint8_t* valid;
     float *rate, *ttft, *itl, *throughput, *rho;
-    int* fb_count;
-    int2* fb_points;       // points that bailed: {entry of pair_list, rate index}
-    int fb_cap;
+    FbList fb;             // points that bailed: fb_pack(entry of pair_list, rate index)
 };
 
 // The sweep's rate i of a pair (same float32 expressions as the oracle's sweep).
@@ -1841,8 +1828,7 @@ __global__ void __launch_bounds__(256) sweep_kernel(SweepArgs g) {
                 m = metrics_from(q, N, st);
                 ok = 1;
             } else {
-                const int k = atomicAdd(g.fb_count, 1);
-                if (k < g.fb_cap) g.fb_points[k] = make_int2(e, i);
+                fb_push(g.fb, fb_pack(e, i));
             }
         }
         g.valid[o] = ok;
@@ -1854,30 +1840,19 @@ __global__ void __launch_bounds__(256) sweep_kernel(SweepArgs g) {
     }
 }
 
-// Stored-vector re-run of the sweep points sweep_kernel bailed on (slot k handles list entries k, k + n_slots, ..);
-// scratch per slot as in grid_fallback.
-__global__ void sweep_fallback(SweepArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+// Stored-vector re-run of the sweep points sweep_kernel bailed on.
+__global__ void sweep_fallback(SweepArgs g, FbRun r) {
     const DevFleet& f = g.f;
-    const int n_slots = gridDim.x * blockDim.x;
-    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
-    int n = *g.fb_count;
-    if (n > g.fb_cap) n = g.fb_cap;
-    double* p = scratch + (size_t)slot * slot_doubles;
-    float* sr = (float*)(p + Kmax + 1);
-    for (int k = slot; k < n; k += n_slots) {
-        const int e = g.fb_points[k].x, i = g.fb_points[k].y;
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        const int e = (int)(item >> 32), i = (int)(unsigned)item;
         const int pair = g.pair_list[e];
         const int s = pair / f.A, a = pair % f.A;
         const int N = g.pair_N[e], K = N + N * f.ratio;
         const double* tab = g.tab + 4 * g.tab_off[e];
-        for (int u = 0; u < N; ++u) sr[u] = (float)tab[4 * u];
-        const float rate = sweep_rate(rate_min_of(sr[0]), rate_max_of(sr[N - 1]), i, g.n_rates);
+        const float rate = sweep_rate(rate_min_of((float)tab[0]), rate_max_of((float)tab[4 * (N - 1)]), i, g.n_rates);
         ModelStats st;
-        const int rc = solve_stored(p, sr, N, K, __fdiv_rn(rate, 1000.0f), st);
-        if (rc != 0) {
-            atomicExch(fb_status, rc);
-            continue;
-        }
+        const int rc = solve_stored(p, tab, N, K, __fdiv_rn(rate, 1000.0f), st);
+        if (rc != 0) return rc;
         const Metrics m = metrics_from(qparams_of(f, s, a), N, st);
         const size_t o = (size_t)pair * g.n_rates + i;
         g.valid[o] = 1;
@@ -1885,7 +1860,8 @@ __global__ void sweep_fallback(SweepArgs g, double* scratch, size_t slot_doubles
         g.itl[o] = m.avg_token_time;
         g.throughput[o] = m.throughput;
         g.rho[o] = m.rho;
-    }
+        return 0;
+    });
 }
 
 }  // namespace wva

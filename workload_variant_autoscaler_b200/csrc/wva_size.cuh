@@ -56,9 +56,7 @@ struct SizeArgs {
     const float* ls;           // prefix log2 sums of the tables (scheduling estimate only)
     CandPlace place;
     AllocCols cand;
-    int* fb_count;
-    int* fb_list;              // candidate indices that bailed
-    int fb_cap;
+    FbList fb;                 // candidate indices that bailed
 };
 
 // The rounds' sort workspace and its item ordering kernels.
@@ -123,9 +121,7 @@ struct Sz2Args {
     unsigned* n_live;      // device counter: candidates that are not finished yet (host stop test)
     SortWs ws;
     AllocCols cand;
-    int* fb_count;
-    int* fb_list;
-    int fb_cap;
+    FbList fb;
 };
 
 // ---------------------------------------------------------------------------
@@ -409,8 +405,7 @@ __device__ __forceinline__ void sz2_advance_body(const Sz2Args& g) {
         }
         if (ph == PH_NIL) store_cand(g.cand, g.place.record(j, pair), cand_nil());
         if (ph == PH_BAIL) {
-            const int k = atomicAdd(g.fb_count, 1);
-            if (k < g.fb_cap) g.fb_list[k] = j;
+            fb_push(g.fb, (unsigned)j);
             store_cand(g.cand, g.place.record(j, pair), cand_nil());
         }
         g.phase[j] = (uint8_t)ph;
@@ -662,10 +657,7 @@ __device__ __forceinline__ void size_warp(const SizeArgs& g) {
     Cand c;
     const bool ok = create_allocation<kStar>(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
     if (lane == 0) {
-        if (!ok) {
-            const int k = atomicAdd(g.fb_count, 1);
-            if (k < g.fb_cap) g.fb_list[k] = j;
-        }
+        if (!ok) fb_push(g.fb, (unsigned)j);
         store_cand(g.cand, g.place.record(j, pair), c);
     }
 }
@@ -673,13 +665,12 @@ __global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) { size_warp<
 __global__ void __launch_bounds__(128) size_warp_star(SizeArgs g) { size_warp<true>(g); }
 
 // ---------------------------------------------------------------------------
-// Stored-vector re-run of the candidates that bailed (slot k handles list entries k, k + n_slots, ..): one thread
-// per candidate evaluates exactly the reference's points, one at a time, with the literal restatement solve_stored
-// on its scratch slot (p[0..Kmax], then servRate[0..N-1] as float32).
+// Stored-vector re-run of the candidates that bailed: one thread per candidate evaluates exactly the reference's
+// points, one at a time, with the literal restatement solve_stored on its scratch slot.
 // ---------------------------------------------------------------------------
 struct StoredEval {
     double* p;
-    const float* sr;
+    const double* tab;
     QParams q;
     int N, K;
     int rc;  // solve_stored's code of the last solve
@@ -699,44 +690,34 @@ struct StoredEval {
     __device__ __forceinline__ SzPt end(int i) { return at(i ? hi : lo); }
     __device__ __forceinline__ SzPt node(int) { return at(sz_mid(lo, hi)); }
     __device__ __forceinline__ bool solve(float lambda, ModelStats& st) {
-        rc = solve_stored(p, sr, N, K, lambda, st);
+        rc = solve_stored(p, tab, N, K, lambda, st);
         return rc == 0;
     }
 };
 
+// A candidate whose re-run fails is stored nil, as the drivers store a candidate that bailed.
 template <bool kStar>
-__device__ __forceinline__ void size_fallback_body(const SizeArgs& g, double* scratch, size_t slot_doubles, int Kmax,
-                                                   int* fb_status) {
+__device__ __forceinline__ void size_fallback_body(const SizeArgs& g, const FbRun& r) {
     const DevFleet& f = g.f;
-    const int n_slots = gridDim.x * blockDim.x;
-    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
-    int n = *g.fb_count;
-    if (n > g.fb_cap) n = g.fb_cap;
-    StoredEval ev;
-    ev.p = scratch + (size_t)slot * slot_doubles;
-    float* sr = (float*)(ev.p + Kmax + 1);
-    ev.sr = sr;
-    for (int k = slot; k < n; k += n_slots) {
-        const int j = g.fb_list[k];
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        const int j = (int)item;
         const int pair = g.cand_pair[j];
         const int s = pair / f.A, a = pair % f.A;
         const int N = g.cand_N[j];
-        const double* tab = g.tab + 4 * g.tab_off[j];
-        for (int i = 0; i < N; ++i) sr[i] = (float)tab[4 * i];
+        StoredEval ev;
+        ev.p = p;
+        ev.tab = g.tab + 4 * g.tab_off[j];
         ev.q = qparams_of(f, s, a);
         ev.N = N;
         ev.K = N + N * f.ratio;
         Cand c;
-        if (!create_allocation<kStar>(f, s, a, N, ev.K, sr[0], sr[N - 1], ev, c)) atomicExch(fb_status, ev.rc);
+        const bool ok = create_allocation<kStar>(f, s, a, N, ev.K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
         store_cand(g.cand, g.place.record(j, pair), c);
-    }
+        return ok ? 0 : ev.rc;
+    });
 }
-__global__ void size_fallback(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
-    size_fallback_body<false>(g, scratch, slot_doubles, Kmax, fb_status);
-}
-__global__ void size_fallback_star(SizeArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
-    size_fallback_body<true>(g, scratch, slot_doubles, Kmax, fb_status);
-}
+__global__ void size_fallback(SizeArgs g, FbRun r) { size_fallback_body<false>(g, r); }
+__global__ void size_fallback_star(SizeArgs g, FbRun r) { size_fallback_body<true>(g, r); }
 
 // ---------------------------------------------------------------------------
 // The load grid's tail (allocation.go:134-163) at every level of a caller-given load list: one lane per (candidate,
@@ -758,9 +739,7 @@ struct LoadArgs {
     int n_cand, L;
     unsigned* counter;
     AllocCols cand;             // [L * S * A]
-    int* fb_count;
-    int2* fb_points;            // items that bailed: {candidate, level}
-    int fb_cap;
+    FbList fb;                  // items that bailed: fb_pack(candidate, level)
 };
 
 // Candidate e's record at level l (nil, or the feasible allocation); solve(lambda, st) is Model.Solve for the
@@ -807,42 +786,30 @@ __global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
                 const bool ok = load_tail(g, e, l, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
                     return solve_shared(tab, N, K, lam, st) == kSolveOk;
                 }, c);
-                if (!ok) {
-                    const int k = atomicAdd(g.fb_count, 1);
-                    if (k < g.fb_cap) g.fb_points[k] = make_int2(e, l);
-                }
+                if (!ok) fb_push(g.fb, fb_pack(e, l));
                 store_cand(g.cand, load_record(g, e, l), c);
             }
         }
     }
 }
 
-// Stored-vector re-run of the items load_kernel bailed on (slot k handles list entries k, k + n_slots, ..); scratch
-// per slot as in size_fallback.
-__global__ void load_fallback(LoadArgs g, double* scratch, size_t slot_doubles, int Kmax, int* fb_status) {
+// Stored-vector re-run of the items load_kernel bailed on.
+__global__ void load_fallback(LoadArgs g, FbRun r) {
     const DevFleet& f = g.f;
-    const int n_slots = gridDim.x * blockDim.x;
-    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
-    int n = *g.fb_count;
-    if (n > g.fb_cap) n = g.fb_cap;
-    double* p = scratch + (size_t)slot * slot_doubles;
-    float* sr = (float*)(p + Kmax + 1);
-    for (int k = slot; k < n; k += n_slots) {
-        const int e = g.fb_points[k].x, l = g.fb_points[k].y;
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        const int e = (int)(item >> 32), l = (int)(unsigned)item;
         const int N = g.cand_N[e], K = N + N * f.ratio;
         const double* tab = g.tab + 4 * g.tab_off[e];
-        for (int u = 0; u < N; ++u) sr[u] = (float)tab[4 * u];
         int rc = 0;
         Cand c;
-        if (!load_tail(g, e, l, sr[N - 1], [&](float lam, ModelStats& st) {
-                rc = solve_stored(p, sr, N, K, lam, st);
+        if (!load_tail(g, e, l, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
+                rc = solve_stored(p, tab, N, K, lam, st);
                 return rc == 0;
-            }, c)) {
-            atomicExch(fb_status, rc);
-            continue;
-        }
+            }, c))
+            return rc;
         store_cand(g.cand, load_record(g, e, l), c);
-    }
+        return 0;
+    });
 }
 
 }  // namespace wva
