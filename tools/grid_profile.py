@@ -4,8 +4,11 @@ torch.profiler with CUDA activities records every kernel and memset of K steps a
 L2 flush that bench.py runs followed by one wva_grid_solve_device.  Prints, per launch, the median device time
 over the steps, then the median step span (first launch start to last launch end) and the idle time inside it.
 With --cells, also the median wall time of engine.grid_solve(..., want_cells=True) (cell table copied back).
+With --nan, every server gets an infinite current cost on accelerator 0, which makes the value of its other
+accelerators NaN and turns pruning off: every non-shared cell of a loaded row is a candidate (the worst case of
+grid_sort_cands).  Also prints the candidates and chunks grid_order listed.
 
-    python tools/grid_profile.py [--steps 50] [--trace DIR] [--cells]
+    python tools/grid_profile.py [--steps 50] [--trace DIR] [--cells] [--nan]
 """
 import argparse
 import ctypes as C
@@ -40,10 +43,15 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--trace", default=None, help="also write the chrome trace into this directory")
     ap.add_argument("--cells", action="store_true", help="also time grid_solve(want_cells=True)")
+    ap.add_argument("--nan", action="store_true", help="NaN values on every server: nothing pruned")
     args = ap.parse_args()
 
     eng = Engine(0)
     fleet, grid = synth_fleet(100, 4, seed=42), config2_grid()
+    if args.nan:
+        fleet.srv_cur_acc[:] = 0
+        fleet.srv_cur_replicas[:] = 2
+        fleet.srv_cur_cost[:] = float("inf")
     S = fleet.n_servers
     blk = torch.zeros(10 * S, dtype=torch.int32, device="cuda")
     cols = _abi.AllocsC()
@@ -97,6 +105,9 @@ def main():
     busy = [sum(d for _, _, d in s) for s in per_step]
     print(f"device: {card()}")
     print(f"{len(per_step)} profiled steps, {launches} library launches per {args.steps} steps")
+    plan = (C.c_uint32 * 31)()
+    eng._L.wva_dbg_read_plan(eng._h, plan)  # item_count[2 * 256 + 1 ..]: [15] candidates, [16] chunks (grid_order)
+    print(f"grid_order: {plan[15]} candidates in {plan[16]} chunks")
     order = [n for n, _, _ in per_step[0]]
     for n in dict.fromkeys(order):
         print(f"  {n:<22s} {statistics.median(by_name[n]):8.1f} us")

@@ -995,11 +995,15 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     plan->n_blocks = (int)((n_cells + kSortChunk - 1) / kSortChunk);
     const size_t nc = std::max<size_t>(plan->n_cells, 1);
     // sort workspace: order u32 [n_cells] | items u64 | items_sorted u64 | item counter |
-    // per-cell records in global item order (32 x 16 bytes per item)
-    const size_t max_items = (nc + 31) / 32 + (size_t)std::max(plan->n_blocks, 1);
+    // per-cell records in global item order (32 x 16 bytes per item) | grid_order's chunk list.
+    // A sort chunk (grid_sort_local: kSortChunk cells; grid_sort_cands: up to kCandChunk candidates of one pair, so
+    // at most n_cells / kCandChunk + S*A chunks) ends with at most one partial item.
+    const size_t max_chunks = nc / kCandChunk + n_pairs;
+    const size_t max_items = (nc + 31) / 32 + std::max((size_t)std::max(plan->n_blocks, 1), max_chunks);
     Cols ws(256);
     const size_t o_order = ws.take(4 * nc), o_items = ws.take(8 * max_items), o_sorted = ws.take(8 * max_items),
-                 o_count = ws.take(4 * (2 * kClasses + 32)), o_recs = ws.take(512 * max_items);
+                 o_count = ws.take(4 * (2 * kClasses + 32)), o_recs = ws.take(512 * max_items),
+                 o_chunks = ws.take(sizeof(uint4) * max_chunks);
     CK(h->d_sort.ensure(ws.bytes));
     char* w = (char*)h->d_sort.p;
     g.order = (unsigned*)(w + o_order);
@@ -1007,6 +1011,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     g.items_sorted = (unsigned long long*)(w + o_sorted);
     g.item_count = (unsigned*)(w + o_count);
     g.recs = (uint4*)(w + o_recs);
+    g.chunks = (uint4*)(w + o_chunks);
     h->dbg_plan = g.item_count + 2 * kClasses + 1;
     const size_t n_best = std::max<size_t>((size_t)S * A * R, 1);
     CK(h->d_best.ensure(sizeof(int) * n_best));
@@ -1015,7 +1020,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     Cols rows(256);
     const size_t o_rows = rows.take((2 * sizeof(double) + sizeof(int)) * n_best + 64),  // row_acc | row_sump | row_j
         o_pair_rec = rows.take(48 * n_pairs_alloc), o_grp = rows.take(sizeof(unsigned) * n_best),
-                 o_bound = rows.take(sizeof(unsigned long long) * std::max(S, 1));
+                 o_bound = rows.take(sizeof(unsigned long long) * std::max(S, 1)), o_cand = rows.take(sizeof(int4) * n_best);
     CK(h->d_rows.ensure(rows.bytes));
     g.row_acc = (double*)((char*)h->d_rows.p + o_rows);
     g.row_sump = g.row_acc + n_best;
@@ -1023,6 +1028,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     g.pair_rec = (float4*)((char*)h->d_rows.p + o_pair_rec);
     g.row_grp = (unsigned*)((char*)h->d_rows.p + o_grp);
     g.bound = (unsigned long long*)((char*)h->d_rows.p + o_bound);
+    g.row_cand = (int4*)((char*)h->d_rows.p + o_cand);
     // grid_order ranks a server's rows in shared memory, and a cell's key holds the accelerator in 8 bits and the batch
     // size in 24; outside those limits every cell is evaluated (grid_order still walks the shared runs)
     g.prune = A <= 256 && Bmax < (1 << 24) && (long long)A * R <= kOrderMaxRows;
@@ -1067,12 +1073,13 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
         h->launches++;
         if (g.want_cells) {
             g.prune = 0;  // every cell is evaluated and stored
+            grid_sort_local<<<plan.n_blocks, kSortThreads, 0, h->stream>>>(g);
         } else {
-            // the shared-chain cells and each server's bound, before grid_sort_local skips the cells above it
+            // the shared-chain cells, each server's bound and the cells left for grid_kernel, then their sort
             grid_order<<<(unsigned)hf.S, kOrderThreads, 0, h->stream>>>(g);
             h->launches++;
+            grid_sort_cands<<<(unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads, 0, h->stream>>>(g);
         }
-        grid_sort_local<<<plan.n_blocks, kSortThreads, 0, h->stream>>>(g);
         grid_items_scatter<<<(unsigned)(16 * h->sm_count), 256, 0, h->stream>>>(g);  // warp per item (grid-stride)
         h->launches++;
         CK(cudaEventRecord(h->ev_k0, h->stream));  // wva_last_kernel_ms = the dominant kernel alone

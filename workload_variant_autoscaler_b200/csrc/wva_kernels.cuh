@@ -328,13 +328,14 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 //   grid_rows        per (pair, replica level): the chain every large-enough batch size shares
 //                    (solve_row); also the (server, replica) rate block and the batch-rank reset
 //   grid_order       without a cell table, per server: the rows' order under grid_finalize's key, the cells
-//                    that share their row's chain up to the row's first feasible one, and the server's bound
-//                    (the smallest key of a feasible cell found)
-//   grid_sort_local  per chunk of 8192 cells: gates + Analyze's rate checks; cells that share their
-//                    row's chain are left to grid_order / grid_shared, and without a cell table cells
-//                    that cannot be feasible or lie above the bound are dropped; the others get a
-//                    log-domain length estimate, an 8-bit class and a local counting sort -> warp items;
-//                    the last CTA plans grid_kernel's queues (grid_items_plan)
+//                    that share their row's chain up to the row's first feasible one, the server's bound
+//                    (the smallest key of a feasible cell found), and the cells left for grid_kernel as two
+//                    rank intervals per row, listed in chunks of at most 4096 of one pair
+//   grid_sort_local  with a cell table, per chunk of 8192 cells: gates + Analyze's rate checks; cells that
+//                    share their row's chain are left to grid_shared; the others get a log-domain length
+//                    estimate, an 8-bit class and a local counting sort -> warp items; the last CTA plans
+//                    grid_kernel's queues (grid_items_plan)
+//   grid_sort_cands  without a cell table, the same over grid_order's chunks (fixed grid, chunk per CTA at a time)
 //   grid_items_scatter  items ordered globally, longest class first
 //   grid_kernel      persistent CTA per SM; warps pull items (32 cells of nearly equal chain length)
 //                    from a long and a short queue: streaming solve, metrics, SLO feasibility,
@@ -403,6 +404,10 @@ struct GridArgs {
     unsigned long_cap;       // ... up to this many (long_per_sm x CTAs)
     unsigned* dbg_cycles;    // diagnostics: per order index, SM cycles spent in grid_kernel (or NULL)
     size_t dbg_n;            // cells; dbg_cycles[dbg_n + idx] holds the warp timeline (start ns, SM, end ns)
+    // without a cell table (grid_order -> grid_sort_cands): the cells handed to grid_kernel, row by row
+    int4* row_cand;          // [S*A*R] {row's first candidate inside its pair, n1, s2, 0}: the row's candidates are the
+                             // ranks [0, n1) and then s2, s2 + 1, ...
+    uint4* chunks;           // chunk list: {pair, first candidate inside the pair, count, place in order[]}
 };
 
 // A cell's place in grid_finalize's order (value, cost, replicas, batch, accelerator) among the cells of its server:
@@ -666,7 +671,7 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
     }
 }
 
-// Without a cell table, between grid_rows and grid_sort_local: one CTA per server.
+// Without a cell table, between grid_rows and grid_sort_cands: one CTA per server.
 //  1. Group ranks (g.prune): every (accelerator, replica level) row gets the number of rows of the server strictly
 //     below it in (value, cost, replicas), with value and cost computed as grid_finalize computes them.  A counting
 //     rank, Q threads per row.  It keeps key_better's order, ties included (-0 == +0); rows without a table take part
@@ -679,14 +684,25 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
 //     A walk step is a chain of dependent loads, and a row without a feasible shared cell walks its whole run, so
 //     the batch sizes in rank order and the pairs' RateRange.Max per rank are staged in shared memory first (in the
 //     space the ranking used).
+//  3. The candidates: the cells grid_sort_cands hands to grid_kernel, as rank intervals of each row.  Every rule that
+//     drops a cell cuts a row at one rank, since batch sizes ascend with the rank: shared cells are the ranks
+//     [lo, kK) (lo: the first rank with b >= jl + 2, B without sharing; kK: the first rank with K >= 2^23, the same
+//     for every row), and cells above the bound the ranks [hi, B) (keys grow along a row).  So the candidates are
+//     [0, min(lo, hi)) and [max(lo, kK), hi).  Rows with rt.x <= 0 and pairs without a table or with alpha > slo_itl
+//     (ITL = alpha + beta * eff >= alpha, eff >= 0, beta >= 0) have none.  A warp per pair scans its rows' counts
+//     into their first candidates, then reserves the pair's chunks of kCandChunk candidates in the chunk list and
+//     their places in order[] with one atomic.
 //
 // No pass over the shared cells is needed after grid_kernel.  Every cell that is never evaluated — a shared cell
-// after the stop of its row's walk, or a non-shared cell that grid_sort_local or grid_kernel skips — either cannot be
-// feasible (the exact gates of grid_sort_local) or has a key strictly above a feasible cell of its server.  So the
-// winner W (the smallest key among the feasible cells) is evaluated, and so is every feasible cell of W's row below W,
-// which has a smaller or equal key: best_rank of W's row is W's rank.  Any other best_rank is a feasible cell, whose
-// key is >= W's.  grid_finalize picks W exactly as when every cell is evaluated.
+// after the stop of its row's walk, or a non-shared cell that is not a candidate or that grid_sort_cands or
+// grid_kernel skips — either cannot be feasible (the exact gates above and in grid_sort_cands) or has a key strictly
+// above a feasible cell of its server.  So the winner W (the smallest key among the feasible cells) is evaluated, and
+// so is every feasible cell of W's row below W, which has a smaller or equal key: best_rank of W's row is W's rank.
+// Any other best_rank is a feasible cell, whose key is >= W's.  grid_finalize picks W exactly as when every cell is
+// evaluated.
 constexpr int kOrderThreads = 1024, kOrderG = 4, kOrderMaxRows = 2048;
+constexpr int kCandChunk = 4096;               // candidates per chunk of grid_sort_cands (never two pairs)
+constexpr int kCandResv = 2 * kClasses + 16;   // item_count[kCandResv], [kCandResv + 1]: candidates, chunks reserved
 __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
     __shared__ float s_vc[2 * kOrderMaxRows];  // ranking: values | costs; walk: RateRange.Max per (accelerator, rank)
     __shared__ int s_rep[kOrderMaxRows];        // ranking: replicas; walk: batch size per rank
@@ -829,7 +845,66 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
         }
     }
     __syncthreads();
-    if (tid == 0) g.bound[s] = prune ? s_bound : kBoundOff;
+    const unsigned long long bound = prune ? s_bound : kBoundOff;
+    if (tid == 0) g.bound[s] = bound;
+    int kK = 0;  // the first rank with K >= 2^23
+    for (int hi = B; kK < hi;) {
+        const int mid = (kK + hi) >> 1, b = batch_at(mid);
+        if (b + b * f.ratio < (1 << 23)) kK = mid + 1; else hi = mid;
+    }
+    for (int a = (int)(tid >> 5); a < A; a += kOrderThreads / 32) {
+        const int sa = s * A + a;
+        bool out = g.pair_tab_off[sa] < 0;
+        if (!out) {  // a table implies a valid model index (pair_class == PAIR_LOAD)
+            const int k = f.srv_model[s] * A + a;
+            const float slo_itl = f.srv_slo_itl[s];
+            out = slo_itl != 0.0f && f.perf_beta[k] >= 0.0f && f.perf_alpha[k] > slo_itl;
+        }
+        unsigned tot = 0;  // the pair's candidates
+        for (int r0 = 0; r0 < R && !out; r0 += 32) {
+            const int ri = r0 + (int)lane;
+            const size_t row = (size_t)sa * R + ri;
+            int n1 = 0, s2 = 0, cnt = 0;
+            if (ri < R && !(g.rt[s * R + ri].x <= 0.0f)) {
+                const int jl = g.row_j[row];
+                int lo = B, hi = B;
+                if (jl != INT_MAX) {
+                    lo = 0;
+                    for (int h = B; lo < h;) {
+                        const int mid = (lo + h) >> 1;
+                        if (batch_at(mid) < jl + 2) lo = mid + 1; else h = mid;
+                    }
+                }
+                if (bound < kBoundNone) {  // only with prune: a key <= bound exists
+                    const unsigned grp = s_grp[a * R + ri];
+                    hi = 0;
+                    for (int h = B; hi < h;) {
+                        const int mid = (hi + h) >> 1;
+                        if (cell_key(grp, batch_at(mid), a) > bound) h = mid; else hi = mid + 1;
+                    }
+                }
+                n1 = min(lo, hi);
+                s2 = max(lo, kK);
+                cnt = n1 + max(hi - s2, 0);
+            }
+            int inc = cnt;
+            for (int d = 1; d < 32; d <<= 1) {
+                const int o = __shfl_up_sync(0xffffffffu, inc, d);
+                if ((int)lane >= d) inc += o;
+            }
+            if (ri < R) g.row_cand[row] = make_int4((int)tot + inc - cnt, n1, s2, 0);
+            tot += (unsigned)__shfl_sync(0xffffffffu, inc, 31);
+        }
+        if (tot) {
+            const unsigned nch = (tot + kCandChunk - 1) / kCandChunk;
+            unsigned long long at = 0;  // candidates reserved before this pair (low word), chunks (high word)
+            if (lane == 0) at = atomicAdd((unsigned long long*)(g.item_count + kCandResv), (unsigned long long)nch << 32 | tot);
+            at = __shfl_sync(0xffffffffu, at, 0);
+            for (unsigned c = lane; c < nch; c += 32)
+                g.chunks[(at >> 32) + c] = make_uint4((unsigned)sa, c * kCandChunk, min((unsigned)kCandChunk, tot - c * kCandChunk),
+                                                      (unsigned)at + c * kCandChunk);
+        }
+    }
 }
 
 // Counter increment for lanes whose equal keys sit in CONTIGUOUS lane ranges (along a row the
@@ -852,106 +927,14 @@ __device__ __forceinline__ unsigned seg_inc(unsigned* counters, int key) {
     return base + __popc(seg_mask & ((1u << lane) - 1u));
 }
 
-// Estimate + LOCAL counting sort, one CTA per chunk of kSortChunk consecutive cells (cells of
-// one or two (server, accelerator) pairs): length classes are computed into shared memory,
-// histogrammed, scanned and scattered without leaving the CTA.  Each run of 32 sorted cells
-// becomes one warp work item tagged with its (longest) class; grid_sort_items then orders the
-// items globally, so the launch is longest-first while a pair's cells stay adjacent.
-__device__ __forceinline__ void grid_items_plan(const GridArgs& g);
-__global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
-    __shared__ uint8_t keys[kSortChunk];
-    __shared__ uint8_t sorted_keys[kSortChunk];
-    __shared__ unsigned hist[kClasses];
-    __shared__ unsigned cursor[kClasses];
+// The end of a chunk's sort, the same in both sort kernels: keys[0, n) hold the chunk's length classes (255: the
+// cell is not handed to grid_kernel) and hist their counts.  The counts are scanned into class cursors, the cells
+// are scattered into order[obase ...] by class (cell_of(k): the id of the chunk's k-th cell), and each run of 32
+// sorted cells becomes one warp work item tagged with its (longest) class.
+template <int kThreads, class CellOf>
+__device__ __forceinline__ void sort_chunk_items(const GridArgs& g, const uint8_t* keys, uint8_t* sorted_keys,
+                                                 unsigned* hist, unsigned* cursor, int n, unsigned obase, CellOf cell_of) {
     __shared__ unsigned item_base;
-    const DevFleet& f = g.f;
-    if (threadIdx.x < kClasses) hist[threadIdx.x] = 0;
-    __syncthreads();
-    const long long base = (long long)blockIdx.x * kSortChunk;
-    const int n_here = (int)min((long long)kSortChunk, g.n_cells - base);
-    // walk the chunk row by row (a row = the R replica levels of one (server, accelerator, batch)):
-    // the row's constants are decoded once per warp, lanes take the replica levels
-    {
-        const unsigned R = (unsigned)g.R, B = (unsigned)g.B, A = (unsigned)f.A;
-        const unsigned row0 = (unsigned)(base / R), row1 = (unsigned)((base + n_here - 1) / R);
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        // pair-level constants are re-read only when the walk crosses into the next pair; so are the
-        // lane's own row constants (its first two replica levels: rate, lambda, the row's shared chain)
-        struct LaneRow {
-            float4 rt;
-            int jl;
-            unsigned grp;
-        };
-        unsigned cur_sa = 0xffffffffu;
-        LaneRow c0{}, c1{};
-        unsigned sa = (row0 + warp) / B;
-        int bi = (int)(row0 + warp - sa * B);
-        int s = 0, t = 0;
-        long long toff = -1;
-        // without a cell table, cells that cannot be feasible or cannot be the server's winner are not evaluated:
-        // TPS servers above the stability limit, ITL = alpha + beta * eff >= alpha > slo_itl (eff >= 0, beta >= 0),
-        // and keys above the server's bound from grid_order
-        unsigned long long bound = kBoundOff;
-        bool tps = false, itl_out = false;
-        auto load_lane = [&](unsigned ri, LaneRow& c) {
-            if (ri >= R || toff < 0) return;
-            c.rt = g.rt[(unsigned)s * R + ri];
-            c.jl = g.row_j[(size_t)sa * R + ri];
-            if (g.prune) c.grp = g.row_grp[(size_t)sa * R + ri];
-        };
-        for (unsigned row = row0 + warp; row <= row1; row += kSortThreads / 32, bi += kSortThreads / 32) {
-            while (bi >= (int)B) {
-                bi -= (int)B;
-                ++sa;
-            }
-            if (sa != cur_sa) {
-                cur_sa = sa;
-                s = (int)(sa / A);
-                toff = g.pair_tab_off[sa];
-                if (toff >= 0) t = g.pair_tab_idx[sa];
-                if (toff >= 0 && !g.want_cells) {  // a table implies a valid model index (pair_class == PAIR_LOAD)
-                    const int k = f.srv_model[s] * (int)A + (int)(sa - (unsigned)s * A);
-                    const float slo_itl = f.srv_slo_itl[s];
-                    bound = g.bound[s];
-                    tps = f.srv_slo_tps[s] > 0.0f;
-                    itl_out = slo_itl != 0.0f && f.perf_beta[k] >= 0.0f && f.perf_alpha[k] > slo_itl;
-                }
-                load_lane(lane, c0);
-                load_lane(lane + 32, c1);
-            }
-            const int b = g.batch[bi];
-            const int K = b + b * f.ratio;
-            float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (toff >= 0) pb = g.pb[(size_t)t * g.B + bi];
-            // one cell: (row, ri) with the lane's cached row constants
-            auto do_cell = [&](unsigned ri, const LaneRow& c) {
-                const long long cell = (long long)row * R + ri;
-                if (cell < base || cell >= base + n_here) return;
-                int key = 255;
-                if (toff >= 0 && !(c.rt.x <= 0.0f) && !(c.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
-                    // a cell that shares its row's chain stays at class 255: grid_order (without a cell table) or
-                    // grid_shared (with one) evaluates it
-                    const bool shared = c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23);
-                    const bool skip = itl_out || (tps && !(c.rt.y <= feas_lim(pb.x))) ||
-                                      (bound != kBoundOff && cell_key(c.grp, b, (int)(sa - (unsigned)s * A)) > bound);
-                    if (!shared && !skip)
-                        key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, c.rt.y, c.rt.z, pb.w, pb.y, pb.z));
-                }
-                keys[cell - base] = (uint8_t)key;
-                if (key != 255) seg_inc(hist, key);  // class 255 (shared / not analysable) needs no slot
-                // (the cell table, when requested, is cleared by the host before the launch: cells that are never
-                // analysed read back as 0 without a store per cell here)
-            };
-            if ((unsigned)lane < R) do_cell(lane, c0);
-            if ((unsigned)lane + 32 < R) do_cell(lane + 32, c1);
-            for (unsigned ri = lane + 64; ri < R; ri += 32) {
-                LaneRow c;
-                load_lane(ri, c);
-                do_cell(ri, c);
-            }
-        }
-    }
-    __syncthreads();
     if (threadIdx.x < 32) {  // exclusive scan of the 256 class counts by one warp
         unsigned run = 0;
         for (int c0 = 0; c0 < kClasses; c0 += 32) {
@@ -968,26 +951,30 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
     }
     __syncthreads();
     const int n_active = (int)cursor[255];  // class 255 (not analysable) sorts last
-    for (int k = threadIdx.x; k < n_here; k += kSortThreads) {
+    for (int k = threadIdx.x; k < n; k += kThreads) {
         const int key = keys[k];
         if (key == 255) continue;
         const unsigned pos = seg_inc(cursor, key);
-        g.order[base + pos] = (unsigned)(base + k);
+        g.order[obase + pos] = cell_of(k);
         sorted_keys[pos] = (uint8_t)key;
     }
     const int n_items = (n_active + 31) >> 5;
     if (threadIdx.x == 0) item_base = n_items ? atomicAdd(g.item_count, (unsigned)n_items) : 0u;
     __syncthreads();
-    for (int w = threadIdx.x; w < n_items; w += kSortThreads) {
-        const unsigned start = (unsigned)(base + 32 * w);
+    for (int w = threadIdx.x; w < n_items; w += kThreads) {
+        const unsigned start = obase + 32 * w;
         const unsigned cnt = (unsigned)min(32, n_active - 32 * w);
         const int cls = sorted_keys[32 * w];
         g.items[item_base + w] = (unsigned long long)start | ((unsigned long long)cnt << 32) |
                                  ((unsigned long long)cls << 40);
         agg_inc(g.item_count + 1, cls);  // global items-per-class histogram (warp-aggregated)
     }
-    // the last CTA to get here turns the global histogram into class cursors and plans grid_kernel's queues
-    // (one launch less than a separate single-CTA kernel)
+}
+
+// The last CTA of a sort kernel to get here turns the global histogram into class cursors and plans grid_kernel's
+// queues (one launch less than a separate single-CTA kernel).
+__device__ __forceinline__ void grid_items_plan(const GridArgs& g);
+__device__ __forceinline__ void sort_plan_in_last_cta(const GridArgs& g) {
     __shared__ bool last_cta;
     __threadfence();
     __syncthreads();
@@ -997,6 +984,143 @@ __global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
         __threadfence();
         grid_items_plan(g);
     }
+}
+
+// With a cell table: estimate + LOCAL counting sort, one CTA per chunk of kSortChunk consecutive cells (cells of
+// one or two (server, accelerator) pairs): length classes are computed into shared memory, histogrammed, scanned and
+// scattered without leaving the CTA; grid_items_scatter then orders the items globally, so the launch is
+// longest-first while a pair's cells stay adjacent.
+__global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
+    __shared__ uint8_t keys[kSortChunk];
+    __shared__ uint8_t sorted_keys[kSortChunk];
+    __shared__ unsigned hist[kClasses];
+    __shared__ unsigned cursor[kClasses];
+    const DevFleet& f = g.f;
+    if (threadIdx.x < kClasses) hist[threadIdx.x] = 0;
+    __syncthreads();
+    const long long base = (long long)blockIdx.x * kSortChunk;
+    const int n_here = (int)min((long long)kSortChunk, g.n_cells - base);
+    // walk the chunk row by row (a row = the R replica levels of one (server, accelerator, batch)):
+    // the row's constants are decoded once per warp, lanes take the replica levels
+    {
+        const unsigned R = (unsigned)g.R, B = (unsigned)g.B, A = (unsigned)f.A;
+        const unsigned row0 = (unsigned)(base / R), row1 = (unsigned)((base + n_here - 1) / R);
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        // pair-level constants are re-read only when the walk crosses into the next pair; so are the
+        // lane's own row constants (its first two replica levels: rate, lambda, the row's shared chain)
+        struct LaneRow {
+            float4 rt;
+            int jl;
+        };
+        unsigned cur_sa = 0xffffffffu;
+        LaneRow c0{}, c1{};
+        unsigned sa = (row0 + warp) / B;
+        int bi = (int)(row0 + warp - sa * B);
+        int s = 0, t = 0;
+        long long toff = -1;
+        auto load_lane = [&](unsigned ri, LaneRow& c) {
+            if (ri >= R || toff < 0) return;
+            c.rt = g.rt[(unsigned)s * R + ri];
+            c.jl = g.row_j[(size_t)sa * R + ri];
+        };
+        for (unsigned row = row0 + warp; row <= row1; row += kSortThreads / 32, bi += kSortThreads / 32) {
+            while (bi >= (int)B) {
+                bi -= (int)B;
+                ++sa;
+            }
+            if (sa != cur_sa) {
+                cur_sa = sa;
+                s = (int)(sa / A);
+                toff = g.pair_tab_off[sa];
+                if (toff >= 0) t = g.pair_tab_idx[sa];
+                load_lane(lane, c0);
+                load_lane(lane + 32, c1);
+            }
+            const int b = g.batch[bi];
+            const int K = b + b * f.ratio;
+            float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (toff >= 0) pb = g.pb[(size_t)t * g.B + bi];
+            // one cell: (row, ri) with the lane's cached row constants
+            auto do_cell = [&](unsigned ri, const LaneRow& c) {
+                const long long cell = (long long)row * R + ri;
+                if (cell < base || cell >= base + n_here) return;
+                int key = 255;
+                if (toff >= 0 && !(c.rt.x <= 0.0f) && !(c.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
+                    // a cell that shares its row's chain stays at class 255: grid_shared evaluates it
+                    const bool shared = c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23);
+                    if (!shared)
+                        key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, c.rt.y, c.rt.z, pb.w, pb.y, pb.z));
+                }
+                keys[cell - base] = (uint8_t)key;
+                if (key != 255) seg_inc(hist, key);  // class 255 (shared / not analysable) needs no slot
+                // (the cell table is cleared by the host before the launch: cells that are never analysed read back
+                // as 0 without a store per cell here)
+            };
+            if ((unsigned)lane < R) do_cell(lane, c0);
+            if ((unsigned)lane + 32 < R) do_cell(lane + 32, c1);
+            for (unsigned ri = lane + 64; ri < R; ri += 32) {
+                LaneRow c;
+                load_lane(ri, c);
+                do_cell(ri, c);
+            }
+        }
+    }
+    __syncthreads();
+    sort_chunk_items<kSortThreads>(g, keys, sorted_keys, hist, cursor, n_here, (unsigned)base,
+                                   [&](int k) { return (unsigned)(base + k); });
+    sort_plan_in_last_cta(g);
+}
+
+// Without a cell table: grid_order's candidates, a chunk (at most kCandChunk candidates of one pair) per CTA at a
+// time over a fixed grid.  A candidate's replica level is the last row of the pair whose first candidate is at or
+// before it, and its rank follows from that row's intervals.  The gates that grid_order's intervals leave to each
+// cell — Analyze's RateRange.Max and K >= 2, and TPS servers above the stability limit — give class 255; the others
+// get the length class, and grid_sort_local's tail sorts the chunk into items.  A chunk never holds two pairs, so
+// neither does an item (grid_kernel fetches the pair record once per item).
+constexpr int kCandThreads = 256, kCandCtasPerSm = 4;
+__global__ void __launch_bounds__(kCandThreads) grid_sort_cands(GridArgs g) {
+    __shared__ unsigned cells[kCandChunk];
+    __shared__ uint8_t keys[kCandChunk];
+    __shared__ uint8_t sorted_keys[kCandChunk];
+    __shared__ unsigned hist[kClasses];
+    __shared__ unsigned cursor[kClasses];
+    const DevFleet& f = g.f;
+    const int R = g.R, B = g.B;
+    const unsigned n_chunks = g.item_count[kCandResv + 1];
+    for (unsigned ci = blockIdx.x; ci < n_chunks; ci += gridDim.x) {
+        const uint4 ch = g.chunks[ci];
+        if (threadIdx.x < kClasses) hist[threadIdx.x] = 0;
+        __syncthreads();
+        const int sa = (int)ch.x, s = sa / f.A, t = g.pair_tab_idx[sa];
+        const long long toff = g.pair_tab_off[sa];
+        const bool tps = f.srv_slo_tps[s] > 0.0f;
+        const int4* rc = g.row_cand + (size_t)sa * R;
+        for (int k = threadIdx.x; k < (int)ch.z; k += kCandThreads) {
+            const int j = (int)ch.y + k;
+            int ri = 0;
+            for (int hi = R - 1; ri < hi;) {
+                const int mid = (ri + hi + 1) >> 1;
+                if (rc[mid].x <= j) ri = mid; else hi = mid - 1;
+            }
+            const int4 row = rc[ri];
+            const int q = j - row.x;
+            const int bi = g.rank_to_bi[q < row.y ? q : row.z + (q - row.y)];
+            const int b = g.batch[bi];
+            const int K = b + b * f.ratio;
+            const float4 rt = g.rt[s * R + ri];
+            const float4 pb = g.pb[(size_t)t * B + bi];
+            int key = 255;
+            if (!(rt.x > pb.x) && K >= 2 && !(tps && !(rt.y <= feas_lim(pb.x))))  // Analyze: queueanalyzer.go:135-143
+                key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, rt.y, rt.z, pb.w, pb.y, pb.z));
+            keys[k] = (uint8_t)key;
+            cells[k] = ((unsigned)sa * (unsigned)B + (unsigned)bi) * (unsigned)R + (unsigned)ri;
+            if (key != 255) seg_inc(hist, key);  // along a row, consecutive ranks: runs of equal classes
+        }
+        __syncthreads();
+        sort_chunk_items<kCandThreads>(g, keys, sorted_keys, hist, cursor, (int)ch.z, ch.w,
+                                       [&](int k) { return cells[k]; });
+    }
+    sort_plan_in_last_cta(g);
 }
 
 // Global order of the warp items by class (longest first): class cursors from the global
@@ -1018,7 +1142,7 @@ constexpr int kGkLong = -1;    // long-item warps per CTA: automatic     // long
 __device__ __forceinline__ float class_len(int c) { return exp2f((float)(254 - c) * (1.0f / 12.0f)); }
 __device__ __forceinline__ float item_us(int c) { return 0.0987f * class_len(c) + 7.0f; }
 __device__ __forceinline__ float long_us(int c) { return 0.0564f * class_len(c) + 4.0f; }
-// Runs in ONE CTA of at least kClasses threads (the last CTA of grid_sort_local to finish); threads beyond
+// Runs in ONE CTA of at least kClasses threads (the last CTA of the sort kernel to finish); threads beyond
 // kClasses only take part in the barriers.
 __device__ __forceinline__ void grid_items_plan(const GridArgs& g) {
     __shared__ unsigned cnt[kClasses + 1];  // exclusive prefix of the class counts (cnt[kClasses] = all items)
@@ -1179,7 +1303,7 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
     const int K = N + N * f.ratio;
     const unsigned pair = cell / ((unsigned)g.B * (unsigned)g.R);
     if (g.prune) {
-        // the bound may have dropped since grid_sort_local (feasible cells found by earlier items): an item none of
+        // the bound may have dropped since grid_order (feasible cells found by earlier items): an item none of
         // whose cells can still be its server's winner is not solved
         const unsigned s = pair / (unsigned)f.A;
         const unsigned long long bound = __ldcg(g.bound + s);
