@@ -279,6 +279,56 @@ int wva_load_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const
                   wva_allocs *candidates, wva_allocs *winners);
 
 /*
+ * Load intervals: for each server, the exact float32 arrival rates in [rpm_lo[s], rpm_hi[s]] (req/min) at which
+ * wva_load_grid's winner changes its decision, and the winner on each stretch in between.  An autoscaler can
+ * skip a re-solve while the load stays inside the current interval, or publish the next scale-up and scale-down
+ * rates.
+ *
+ * The decision key of a winner record is (feasible, acc, replicas, batch, cost, value, max_rate), compared
+ * bitwise.  For server s the intervals partition [rpm_lo[s], rpm_hi[s]]: interval 0 starts at rpm_lo[s],
+ * interval j covers [start_rpm[j], start_rpm[j+1]), and start_rpm[j] is the smallest float32 rate at which the
+ * key differs from interval j-1's; adjacent stretches with the same key are one interval.  At every float32 rate
+ * of an interval wva_load_grid's winner for s has the interval's key.  Record j (index s*M + j) is byte for byte
+ * wva_load_grid's winner record for s at level start_rpm[j], latency columns (itl, ttft, rho) included; those vary
+ * inside an interval and are reported at its start only.  A stretch without a feasible candidate is an interval
+ * with a nil record.  Rate 0 is a point of its own (zeroLoadAllocation); the next interval starts at the smallest
+ * positive float32 unless it has the same key.  With a TPS target or out_tokens 0 the decision does not read the
+ * load, so such a server has one interval above rate 0.
+ *
+ * Above rate 0 each pair's key is a step function of the rate (DESIGN.md §3.10): the replica count never
+ * decreases, and at a fixed count Analyze's rate check flips at most twice.  So each step is found exactly by a
+ * bisection over float32 bit patterns, and the winner can change only where some pair steps.  The sizing runs once
+ * per (server, accelerator), as in wva_load_grid.
+ *
+ * count[s] is the number of intervals written (1..M).  truncated[s] = 1 when the decision changes again in
+ * (last start, rpm_hi[s]]: either M intervals were written first, or a pair of s would need more than INT32_MAX
+ * replicas there (the int32 replicas column and the float-to-int conversion wrap, so the steps stop being
+ * monotone).  In the second case the list stops at the last start below that rate, and count[s] = 0 when it is
+ * rpm_lo[s] itself.  A truncated list's last interval ends at that next change, which is not reported.  Records
+ * and start rates past count[s] are zero bytes.
+ *
+ * fleet->srv_arrival_rpm, fleet->unlimited and the capacities are not read.  The fleet becomes resident, and
+ * wva_summarize returns WVA_ERR_STATE afterwards, as after wva_load_grid.  Columns of out->rec may be NULL (not
+ * written).  WVA_ERR_BAD_ARG: out NULL, max_per_server < 1, rpm_lo, rpm_hi, count, truncated or start_rpm NULL
+ * with S > 0, a bound that is NaN, infinite or negative, or rpm_lo[s] > rpm_hi[s].  WVA_ERR_UNSUPPORTED:
+ * S * max_per_server >= 2^31, or a range in which wva_load_grid fails: an interval start whose solve fails the
+ * same way (a rescale loop that would not terminate, too many stored-vector fallbacks), or a positive rate below
+ * 60 * 2^-150 req/min on a server with a min_replicas-0 load pair.  There totalRate rounds to 0, the pair gets 0
+ * replicas and Analyze solves at 0/0, whose rescale loop does not terminate in wva_load_grid (the Go reference
+ * reports NaN latencies there).
+ */
+typedef struct wva_intervals {
+    int32_t max_per_server; /* M: capacity per server                                            */
+    int32_t *count;         /* [S] intervals written for server s                                */
+    uint8_t *truncated;     /* [S] 1 if the decision changes again in (last start, rpm_hi[s]]    */
+    float *start_rpm;       /* [S*M] first float32 arrival rate (req/min) of interval j           */
+    wva_allocs rec;         /* [S*M] the per-server winner record at start_rpm                    */
+} wva_intervals;
+
+int wva_load_intervals(wva_handle *h, const wva_fleet *fleet, const float *rpm_lo, const float *rpm_hi,
+                       wva_intervals *out);
+
+/*
  * Solver.SolveGreedy + the best-effort saturation policies (pkg/solver/greedy.go:35-341) over a candidate
  * table the caller already holds: `candidates` (S*A, value = transition penalty as wva_analyze returns it) is
  * read, and modified where the reference scales best-effort allocations; `winners` (S) is written.  Host only

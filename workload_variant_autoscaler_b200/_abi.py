@@ -95,6 +95,11 @@ class AllocsC(C.Structure):
     ]
 
 
+class IntervalsC(C.Structure):
+    _fields_ = [("max_per_server", C.c_int32), ("count", i32p), ("truncated", u8p), ("start_rpm", f32p),
+                ("rec", AllocsC)]
+
+
 class GridC(C.Structure):
     _fields_ = [("n_batch", C.c_int32), ("batch", i32p), ("n_replicas", C.c_int32), ("replicas", i32p)]
 

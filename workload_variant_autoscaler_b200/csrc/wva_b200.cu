@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <cfloat>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -196,7 +197,8 @@ struct wva_handle {
     // size path
     DevBuf d_sz_state, d_sz_req, d_sz_sort;
     PinBuf sz_pin;
-    DevBuf d_lg_star;  // the load grid's rateStar records
+    DevBuf d_lg_star;  // the load grid's rateStar records (shared with the load intervals)
+    DevBuf d_iv;       // the load intervals' counts, flags, starts and work list
 
     // grid path
     DevBuf d_sort, d_best, d_pb, d_rows;
@@ -790,30 +792,88 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
 }
 
 // ---- load grid: CreateAllocation and the unlimited winner at every listed load level -------------------------
-// Phase 1 sizes each candidate once: the pairs that pass the gates and are a load at some level, sorted by
-// descending N with one N-entry table each, run through the size drivers in rateStar mode.  Phase 2 (load_kernel,
-// load_fallback) is the tail per (candidate, level).  rpm [L*S] is the caller's level list; cand ([L*S*A]) and
-// winners ([L*S]) are device columns.
+// Phase 1 sizes each candidate once: the pairs that pass the gates and are a load somewhere in the caller's
+// rates, sorted by descending N with one N-entry table each, run through the size drivers in rateStar mode.  The
+// load grid and the load intervals share it (and lg_tabs / d_lg_star, which both rebuild on every call).
+//
+// prepare_load_star uploads the candidate lists with the caller's columns (laid out in c, written by fill; `pairs`
+// holds the candidates' pair ids by the time fill runs).  enqueue_load_star then builds the tables, sizes fallback
+// list 1 for the caller's tail (up to fb2_cap entries) and enqueues phase 1.
+struct LoadStar {
+    int n = 0;           // candidates
+    AllocCols star{};    // rateStar mode's records by pair id: feasible and max_rate = rateStar
+    FbRun fb2{};         // the tail's fallback list
+    SizeArgs g{};        // phase 1's candidates and tables
+};
+template <class Fill>
+int prepare_load_star(wva_handle* h, const std::vector<char>& loaded, std::vector<int>& pairs, Cols& c, Fill&& fill) {
+    const HostFleet& hf = h->hf;
+    std::vector<int> Ns;
+    int rc = sorted_pairs(h, [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, true, 1.0f) == PAIR_LOAD; },
+                          pairs, Ns);
+    if (rc) return rc;
+    return upload_tables(h, h->lg_tabs, pairs, Ns, true, c, fill);
+}
+int enqueue_load_star(wva_handle* h, long long fb2_cap, LoadStar& ls) {
+    const HostFleet& hf = h->hf;
+    const PairTables& pt = h->lg_tabs;
+    const size_t n_pairs = (size_t)hf.S * hf.A;
+    CK(h->d_lg_star.ensure(5 * n_pairs + 16));
+    ls.star = AllocCols{};
+    ls.star.max_rate = (float*)h->d_lg_star.p;
+    ls.star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
+    int rc = build_tables(h, pt);
+    if (rc) return rc;
+    // the tail's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
+    rc = prepare_fallback(h, 1, (int)std::min<long long>(fb2_cap, 1 << 22), pt.len_max, ls.fb2);
+    if (rc) return rc;
+    ls.n = pt.n;
+    SizeArgs& g = ls.g;
+    g = SizeArgs{};
+    g.f = h->df;
+    g.cand_pair = pt.pair();
+    g.cand_N = pt.len();
+    g.n_cand = pt.n;
+    g.tab = (const double*)pt.tab.p;
+    g.tab_off = pt.off();
+    g.ls = (const float*)pt.ls.p;
+    g.place = CandPlace{nullptr, nullptr};
+    g.cand = ls.star;
+    return enqueue_candidates(h, g, pt.len_max, true);
+}
+// The tail's view of phase 1: candidates, tables and rateStar records (the level list is the caller's).
+LoadArgs load_args(wva_handle* h, const LoadStar& ls) {
+    LoadArgs la{};
+    la.f = h->df;
+    la.cand_pair = ls.g.cand_pair;
+    la.cand_N = ls.g.cand_N;
+    la.tab_off = ls.g.tab_off;
+    la.tab = ls.g.tab;
+    la.star_ok = ls.star.feasible;
+    la.rate_star = ls.star.max_rate;
+    la.n_cand = ls.n;
+    la.fb = ls.fb2.list;
+    return la;
+}
+
+// Phase 2 (load_kernel, load_fallback) is the tail per (candidate, level).  rpm [L*S] is the caller's level list;
+// cand ([L*S*A]) and winners ([L*S]) are device columns.
 int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     std::vector<char> loaded(S, 0);  // server s is a load at some level (NaN and +Inf included)
     for (int l = 0; l < L; ++l)
         for (int s = 0; s < S; ++s) loaded[s] |= !(rpm[(size_t)l * S + s] < 0.0f) && rpm[(size_t)l * S + s] != 0.0f;
-    std::vector<int> pairs, Ns;
-    int rc = sorted_pairs(h, [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, true, 1.0f) == PAIR_LOAD; },
-                          pairs, Ns);
-    if (rc) return rc;
-    const int n = (int)pairs.size();
-    const long long n_items = (long long)n * L;
-    PairTables& pt = h->lg_tabs;
+    std::vector<int> pairs;
     Cols c(16);
     const size_t o_rpm = c.take(4 * (size_t)L * S);
-    rc = upload_tables(h, pt, pairs, Ns, true, c, [&](char* p) {
+    int rc = prepare_load_star(h, loaded, pairs, c, [&](char* p) {
         if ((size_t)L * S) memcpy(p + o_rpm, rpm, 4 * (size_t)L * S);
     });
     if (rc) return rc;
-    const float* d_rpm = (const float*)((const char*)pt.lists.p + o_rpm);
+    const int n = (int)pairs.size();
+    const long long n_items = (long long)n * L;
+    const float* d_rpm = (const float*)((const char*)h->lg_tabs.lists.p + o_rpm);
     rc = ensure_ctrl(h);
     if (rc) return rc;
     const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
@@ -821,45 +881,16 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
         trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(h->df, cand, d_rpm, L);
         h->launches++;
     }
-    // rateStar mode's records by pair id: feasible and max_rate = rateStar
-    const size_t n_pairs = (size_t)S * A;
-    CK(h->d_lg_star.ensure(5 * n_pairs + 16));
-    AllocCols star{};
-    star.max_rate = (float*)h->d_lg_star.p;
-    star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
-    rc = build_tables(h, pt);
+    LoadStar ls;
+    rc = enqueue_load_star(h, n_items, ls);
     if (rc) return rc;
-    // phase 2's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
-    FbRun fb2;
-    rc = prepare_fallback(h, 1, (int)std::min<long long>(n_items, 1 << 22), pt.len_max, fb2);
-    if (rc) return rc;
-    SizeArgs g{};
-    g.f = h->df;
-    g.cand_pair = pt.pair();
-    g.cand_N = pt.len();
-    g.n_cand = n;
-    g.tab = (const double*)pt.tab.p;
-    g.tab_off = pt.off();
-    g.ls = (const float*)pt.ls.p;
-    g.place = CandPlace{nullptr, nullptr};
-    g.cand = star;
-    rc = enqueue_candidates(h, g, pt.len_max, true);
-    if (rc) return rc;
+    const FbRun& fb2 = ls.fb2;
     if (n > 0 && L > 0) {
-        LoadArgs la{};
-        la.f = h->df;
-        la.cand_pair = g.cand_pair;
-        la.cand_N = g.cand_N;
-        la.tab_off = g.tab_off;
-        la.tab = g.tab;
-        la.star_ok = star.feasible;
-        la.rate_star = star.max_rate;
+        LoadArgs la = load_args(h, ls);
         la.level_rpm = d_rpm;
-        la.n_cand = n;
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
         la.cand = cand;
-        la.fb = fb2.list;
         int per_sm = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, load_kernel, 256, 0));
         per_sm = std::max(1, std::min(per_sm, 8));
@@ -875,6 +906,77 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
             h->df, cand, winners, L);
         h->launches++;
     }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- load intervals: where each server's load-grid winner changes in [lo, hi] ---------------------------------
+// The device columns of one call: count [S], truncated [S] and start [S*M] come back to the caller, the work list
+// [S*M] stays on the device.
+struct IntervalCols {
+    Cols cols{16};
+    size_t o_count = 0, o_trunc = 0, o_start = 0, o_items = 0;
+};
+
+// Phase 1 over the servers with hi > 0, interval_kernel, interval_tail and interval_fallback.  lo / hi [S] are
+// the caller's bounds; rec ([S*M]) is a device block; the other columns are in h->d_iv at iv's offsets.
+int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int M, const IntervalCols& iv,
+                           const AllocCols& rec, size_t rec_bytes) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A;
+    std::vector<char> loaded(S, 0);
+    for (int s = 0; s < S; ++s) loaded[s] = hi[s] > 0.0f;
+    std::vector<int> pairs;
+    Cols c(16);
+    const size_t o_lo = c.take(4 * (size_t)S), o_hi = c.take(4 * (size_t)S), o_cop = c.take(4 * (size_t)S * A);
+    int rc = prepare_load_star(h, loaded, pairs, c, [&](char* p) {
+        if (S) {
+            memcpy(p + o_lo, lo, 4 * (size_t)S);
+            memcpy(p + o_hi, hi, 4 * (size_t)S);
+        }
+        int* cop = (int*)(p + o_cop);
+        std::fill(cop, cop + (size_t)S * A, -1);
+        for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
+    });
+    if (rc) return rc;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    // records and starts past a server's count read back as zero
+    char* d = (char*)h->d_iv.p;
+    CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
+    CK(cudaMemsetAsync(d + iv.o_start, 0, 4 * (size_t)S * M, h->stream));
+    LoadStar ls;
+    rc = enqueue_load_star(h, (long long)S * M, ls);
+    if (rc) return rc;
+    if (S == 0) return WVA_OK;
+    const char* dl = (const char*)h->lg_tabs.lists.p;
+    IntervalArgs g{};
+    g.ld = load_args(h, ls);
+    g.cand_of_pair = (const int*)(dl + o_cop);
+    g.lo = (const float*)(dl + o_lo);
+    g.hi = (const float*)(dl + o_hi);
+    g.M = M;
+    g.count = (int*)(d + iv.o_count);
+    g.truncated = (uint8_t*)(d + iv.o_trunc);
+    g.start = (float*)(d + iv.o_start);
+    g.rec = rec;
+    g.items = FbList{(int*)h->d_ctrl.p + CTRL_COUNTER, (unsigned long long*)(d + iv.o_items), S * M};
+    g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
+    // one warp per server, A accelerator states per warp in shared memory
+    const size_t per_warp = sizeof(IvAcc) * (size_t)A;
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    if (per_warp > (size_t)optin)
+        return h->fail(WVA_ERR_UNSUPPORTED, "too many accelerators for the interval kernel's shared memory");
+    const int wpb = (int)std::max<size_t>(1, std::min<size_t>(4, (48u << 10) / std::max<size_t>(per_warp, 1)));
+    const size_t smem = per_warp * wpb;
+    if (smem > (48u << 10)) CK(cudaFuncSetAttribute(interval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    interval_kernel<<<(unsigned)((S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, ((long long)S * M + 255) / 256);
+    interval_tail<<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
+    h->launches += 2;
+    CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1 and the interval kernels
+    launch_fallback(h, interval_fallback, g, ls.fb2);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1741,6 +1843,39 @@ int wva_load_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const
     if (rc) return rc;
     scatter_block(c.cand_host, c.bc, candidates);
     scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
+int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_lo, const float* rpm_hi,
+                       wva_intervals* out) {
+    if (!h) return WVA_ERR_BAD_ARG;
+    if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
+    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
+    const int S = fleet->n_servers, M = out->max_per_server;
+    if (M < 1) return h->fail(WVA_ERR_BAD_ARG, "max_per_server below 1");
+    if (S > 0 && (!rpm_lo || !rpm_hi || !out->count || !out->truncated || !out->start_rpm))
+        return h->fail(WVA_ERR_BAD_ARG, "NULL bound or output column");
+    if ((long long)S * M >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "load intervals too large for one call (>= 2^31 records)");
+    for (int s = 0; s < S; ++s)
+        if (!std::isfinite(rpm_lo[s]) || !std::isfinite(rpm_hi[s]) || rpm_lo[s] < 0.0f || !(rpm_lo[s] <= rpm_hi[s]))
+            return h->fail(WVA_ERR_BAD_ARG, "bound NaN, infinite or negative, or rpm_lo above rpm_hi");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    IntervalCols iv;
+    iv.o_count = iv.cols.take(4 * (size_t)S, out->count);
+    iv.o_trunc = iv.cols.take((size_t)S, out->truncated);
+    iv.o_start = iv.cols.take(4 * (size_t)S * M, out->start_rpm);
+    iv.o_items = iv.cols.take(8 * (size_t)S * M);
+    CK(h->d_iv.ensure(iv.cols.bytes));
+    HostCall c{(size_t)S * M, true, false, &iv.cols, h->d_iv.p};
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
+        return enqueue_load_intervals(h, rpm_lo, rpm_hi, M, iv, dc, c.bc.bytes);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, &out->rec);
     return WVA_OK;
 }
 

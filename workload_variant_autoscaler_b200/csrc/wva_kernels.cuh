@@ -172,6 +172,11 @@ __device__ __forceinline__ float total_rate_of(const DevFleet& f, int s) {  // a
     if (f.srv_slo_tps[s] == 0.0f) return __fdiv_rn(f.srv_arrival_rpm[s], 60.0f);
     return __fdiv_rn(f.srv_slo_tps[s], (float)f.srv_out_tokens[s]);
 }
+// ... at arrival rate rpm instead of the server's own (the load intervals' points are not in memory)
+__device__ __forceinline__ float total_rate_of(const DevFleet& f, int s, float rpm) {
+    if (f.srv_slo_tps[s] == 0.0f) return __fdiv_rn(rpm, 60.0f);
+    return total_rate_of(f, s);
+}
 // The fleet as the load grid sees it at level l: the arrival rates are row l of the level list.
 __device__ __forceinline__ DevFleet at_level(const DevFleet& f, const float* level_rpm, int l) {
     DevFleet fl = f;

@@ -236,14 +236,22 @@ struct SzReplicas {
     long long nrep;
     float cost;
 };
+// ceil(totalRate / rateStar) before the conversion to int (allocation.go:141)
+__device__ __forceinline__ double sz_quotient(float total_rate, float rate_star) {
+    return ceil(__ddiv_rn((double)total_rate, (double)rate_star));
+}
+// the per-replica rate Analyze checks (allocation.go:146)
+__device__ __forceinline__ float sz_final_rate(float total_rate, long long nrep) {
+    return __fdiv_rn(total_rate, (float)nrep);
+}
 __device__ __forceinline__ bool sz_replicas(const DevFleet& f, int s, int a, float rmax, float rate_star,
                                             float total_rate, SzReplicas& r, float& lam) {
-    r.nrep = go_f64_to_int(ceil(__ddiv_rn((double)total_rate, (double)rate_star)));
+    r.nrep = go_f64_to_int(sz_quotient(total_rate, rate_star));
     const long long min_rep = f.srv_min_replicas[s];
     if (r.nrep < min_rep) r.nrep = min_rep;
     const long long total = (long long)num_instances(f, f.srv_model[s], a) * r.nrep;
     r.cost = __fmul_rn(f.acc_cost[a], (float)total);
-    return sz_gate(__fdiv_rn(total_rate, (float)r.nrep), rmax, lam);
+    return sz_gate(sz_final_rate(total_rate, r.nrep), rmax, lam);
 }
 
 // The feasible allocation (allocation.go:155-163); value = cost.
@@ -742,10 +750,11 @@ struct LoadArgs {
     FbList fb;                  // items that bailed: fb_pack(candidate, level)
 };
 
-// Candidate e's record at level l (nil, or the feasible allocation); solve(lambda, st) is Model.Solve for the
-// final Analyze.  Returns false when that solve bailed (out is then nil).
-template <class Solve>
-__device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, int l, float sN, Solve&& solve, Cand& out) {
+// Candidate e's record at totalRate total_rate(s) (nil, or the feasible allocation); solve(lambda, st) is
+// Model.Solve for the final Analyze.  Returns false when that solve bailed (out is then nil).
+template <class Total, class Solve>
+__device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, Total&& total_rate, float sN, Solve&& solve,
+                                          Cand& out) {
     const DevFleet& f = g.f;
     const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A, N = g.cand_N[e];
     out = cand_nil();
@@ -753,8 +762,7 @@ __device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, int l, float
     const float rate_star = g.rate_star[pair];
     SzReplicas r;
     float lam;
-    if (!sz_replicas(f, s, a, rate_max_of(sN), rate_star, total_rate_of(at_level(f, g.level_rpm, l), s), r, lam))
-        return true;
+    if (!sz_replicas(f, s, a, rate_max_of(sN), rate_star, total_rate(s), r, lam)) return true;
     ModelStats st;
     if (!solve(lam, st)) return false;
     const Metrics m = metrics_from(qparams_of(f, s, a), N, st);
@@ -765,6 +773,12 @@ __device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, int l, float
 __device__ __forceinline__ size_t load_record(const LoadArgs& g, int e, int l) {
     return (size_t)l * g.f.S * g.f.A + g.cand_pair[e];
 }
+// totalRate of server s at level l, for load_tail
+struct LevelRate {
+    const LoadArgs& g;
+    int l;
+    __device__ __forceinline__ float operator()(int s) const { return total_rate_of(at_level(g.f, g.level_rpm, l), s); }
+};
 
 __global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
     const DevFleet& f = g.f;
@@ -783,7 +797,8 @@ __global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
                 const int N = g.cand_N[e], K = N + N * f.ratio;
                 const double* tab = g.tab + 4 * g.tab_off[e];
                 Cand c;
-                const bool ok = load_tail(g, e, l, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
+                const bool ok = load_tail(g, e, LevelRate{g, l}, (float)tab[4 * (N - 1)],
+                                          [&](float lam, ModelStats& st) {
                     return solve_shared(tab, N, K, lam, st) == kSolveOk;
                 }, c);
                 if (!ok) fb_push(g.fb, fb_pack(e, l));
@@ -802,12 +817,264 @@ __global__ void load_fallback(LoadArgs g, FbRun r) {
         const double* tab = g.tab + 4 * g.tab_off[e];
         int rc = 0;
         Cand c;
-        if (!load_tail(g, e, l, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
+        if (!load_tail(g, e, LevelRate{g, l}, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
                 rc = solve_stored(p, tab, N, K, lam, st);
                 return rc == 0;
             }, c))
             return rc;
         store_cand(g.cand, load_record(g, e, l), c);
+        return 0;
+    });
+}
+
+// ---------------------------------------------------------------------------
+// Load intervals (DESIGN.md §3.10): per server, the float32 arrival rates in [lo, hi] at which the load grid's
+// winner changes its decision key (feasible, acc, replicas, batch, cost, value, max_rate).  Above zero load a load
+// pair's key is a function of its state (nrep, gate), and that state never decreases as the rate grows, so each
+// pair's next change is the first float32 at which a monotone predicate flips: a bisection over the bit patterns.
+// interval_kernel walks the union of the pairs' steps with one warp per server and emits an interval wherever the
+// winner's key changes; interval_tail then runs the load grid's tail (load_tail) at every interval start whose
+// winner is a load pair, and interval_fallback re-runs the items it bailed on.
+// ---------------------------------------------------------------------------
+struct IntervalArgs {
+    LoadArgs ld;               // phase 1's candidates and rateStar records (level_rpm, L and cand unused)
+    const int* cand_of_pair;   // [S * A] the pair's index in ld's candidate list, -1: not a load candidate
+    const float* lo;           // [S] range bounds (req/min)
+    const float* hi;
+    int M;                     // intervals per server
+    int* count;                // [S]
+    uint8_t* truncated;        // [S]
+    float* start;              // [S * M]
+    AllocCols rec;             // [S * M]
+    FbList items;              // interval_tail's work list: fb_pack(accelerator, record)
+    int* status;               // set when a pair has 0 replicas at a positive rate (see iv_advance)
+};
+
+// A pair's state at one rate: the key is a function of (nrep, gate), and over marks a replica count beyond
+// INT32_MAX (the int32 column and go_f64_to_int's wrap end the monotone part there).  gate: 0 the final rate is
+// not positive, 1 Analyze accepts it, 2 it is above RateRange.Max.
+struct IvState {
+    long long nrep;
+    int gate;
+    bool over;
+    __device__ bool operator!=(const IvState& o) const { return nrep != o.nrep || gate != o.gate || over != o.over; }
+};
+
+// What one accelerator of the warp's server decides at the current point, and where that changes next.
+struct IvAcc {
+    Cand key;       // the load grid's record at the point without its latency columns; value = TransitionPenalty
+    float next;     // the smallest rate above the point at which the state changes (+Inf: none up to hi)
+    float rate_star, rmax;
+    int N;
+    int tail;       // 1: a load pair, whose record needs the tail (the latency columns) at an interval start
+    bool over;
+};
+
+__device__ __forceinline__ IvState iv_state(const DevFleet& f, int s, int a, const IvAcc& p, float rpm, Cand* key) {
+    const float total = total_rate_of(f, s, rpm);
+    SzReplicas r;
+    float lam;
+    const bool ok = sz_replicas(f, s, a, p.rmax, p.rate_star, total, r, lam);
+    IvState st;
+    st.nrep = r.nrep;
+    st.gate = ok ? 1 : (sz_final_rate(total, r.nrep) <= 0.0f ? 0 : 2);
+    st.over = !(sz_quotient(total, p.rate_star) <= 2147483647.0);
+    if (key) {
+        *key = cand_nil();
+        if (ok) {
+            *key = sz_cand(a, p.N, r, p.rate_star, 0.0f, 0.0f, 0.0f);
+            key->value = penalty_of(f, s, *key);
+        }
+    }
+    return st;
+}
+
+// Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.
+__device__ __forceinline__ void iv_advance(const IntervalArgs& g, int s, int a, float x, float hi, IvAcc& p) {
+    const DevFleet& f = g.ld.f;
+    const float inf = __int_as_float(0x7f800000);
+    // the class at x: pair_class reads only whether the rate is negative or zero, and lo[s] = 0 when x = 0
+    const int cls = pair_class(at_level(f, x == 0.0f ? g.lo : g.hi, 0), s, a, true);
+    p.tail = 0;
+    p.over = false;
+    p.next = x == 0.0f && hi > 0.0f ? __int_as_float(1) : inf;  // rpm = 0 is a point of its own
+    if (cls != PAIR_LOAD) {
+        p.key = cand_nil();
+        if (cls == PAIR_ZERO) {
+            p.key = zero_load_alloc(f, s, a);
+            p.key.value = penalty_of(f, s, p.key);
+        }
+        return;
+    }
+    const int e = g.cand_of_pair[s * f.A + a];
+    if (!g.ld.star_ok[s * f.A + a]) {  // nil at every load
+        p.key = cand_nil();
+        return;
+    }
+    p.tail = 1;
+    p.N = g.ld.cand_N[e];
+    p.rate_star = g.ld.rate_star[s * f.A + a];
+    p.rmax = rate_max_of((float)g.ld.tab[4 * (g.ld.tab_off[e] + p.N - 1)]);
+    const IvState at = iv_state(f, s, a, p, x, &p.key);
+    p.over = at.over;
+    // totalRate rounds to 0 below 60 * 2^-150 req/min: with min_replicas 0 the pair has 0 replicas and Analyze
+    // solves at 0/0, whose rescale loop does not terminate, so the load grid fails at this rate; so does the call
+    if (at.nrep == 0) *g.status = 1;
+    if (f.srv_slo_tps[s] != 0.0f || at.over) return;  // a TPS target: totalRate does not read the load
+    // the first float32 in (x, hi] whose state differs from x's: the state is non-decreasing in the rate (nrep
+    // first, then gate at a fixed nrep, with over absorbing), so "differs" is a monotone predicate
+    auto differs = [&](unsigned bits) { return iv_state(f, s, a, p, __uint_as_float(bits), nullptr) != at; };
+    unsigned l = __float_as_uint(x), h = __float_as_uint(hi);
+    if (h <= l) return;
+    // The step is within a few ulps of 60 * nrep * rateStar (the count grows) or 60 * nrep * RateRange.Max (the
+    // rate check starts rejecting): when a bracket of +-64 ulps around the nearer estimate holds it, bisect there;
+    // otherwise over the whole range.  Either way the result is the predicate's first flip.
+    if (at.nrep >= 1) {
+        double est = 60.0 * (double)at.nrep * (double)p.rate_star;
+        if (at.gate == 1) est = fmin(est, 60.0 * (double)at.nrep * (double)p.rmax);
+        const unsigned e = __float_as_uint(__double2float_rn(est));
+        const unsigned bl = e > l && e - l > 64 ? e - 64 : l, bh = e < h && h - e > 64 ? e + 64 : h;
+        if (at.gate != 0 && est < 3.0e38 && bl < bh && (bl == l || !differs(bl)) && differs(bh)) {
+            l = bl;
+            h = bh;
+        } else if (!differs(h)) {
+            return;
+        }
+    } else if (!differs(h)) {
+        return;
+    }
+    while (h - l > 1) {
+        const unsigned m = l + (h - l) / 2;
+        if (differs(m)) h = m;
+        else l = m;
+    }
+    p.next = __uint_as_float(h);
+}
+
+// SolveUnlimited over the warp's accelerators: strict '<' from MaxFloat32, ties to the lower accelerator id.
+// Returns the winner's accelerator (-1: none) on every lane.
+__device__ __forceinline__ int iv_winner(const IvAcc* acc, int A, int lane) {
+    float v = 3.40282346638528859811704183484516925440e+38f;
+    int w = -1;
+    for (int a = lane; a < A; a += 32)
+        if (acc[a].key.feasible && acc[a].key.value < v) {
+            v = acc[a].key.value;
+            w = a;
+        }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, v, d);
+        const int ow = __shfl_xor_sync(0xffffffffu, w, d);
+        if (ow >= 0 && (w < 0 || ov < v || (ov == v && ow < w))) {
+            v = ov;
+            w = ow;
+        }
+    }
+    return w;
+}
+
+// The decision key's columns, bitwise.
+__device__ __forceinline__ bool iv_same_key(const Cand& x, const Cand& y) {
+    return x.feasible == y.feasible && x.acc == y.acc && x.replicas == y.replicas && x.batch == y.batch &&
+           __float_as_uint(x.cost) == __float_as_uint(y.cost) && __float_as_uint(x.value) == __float_as_uint(y.value) &&
+           __float_as_uint(x.max_rate) == __float_as_uint(y.max_rate);
+}
+
+// One warp per server; the accelerators' state lives in dynamic shared memory (A entries per warp).
+__global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
+    extern __shared__ IvAcc iv_acc[];
+    const DevFleet& f = g.ld.f;
+    const int A = f.A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int s = blockIdx.x * (blockDim.x >> 5) + wid;
+    if (s >= f.S) return;
+    IvAcc* acc = iv_acc + (size_t)wid * A;
+    const float hi = g.hi[s];
+    float x = g.lo[s];
+    bool over = false;
+    for (int a = lane; a < A; a += 32) {
+        iv_advance(g, s, a, x, hi, acc[a]);
+        over |= acc[a].over;
+    }
+    __syncwarp();
+    int n = 0;
+    bool truncated = __any_sync(0xffffffffu, over);  // a pair needs more than INT32_MAX replicas at lo
+    Cand prev = cand_nil();
+    while (!truncated) {
+        const int w = iv_winner(acc, A, lane);
+        const Cand key = w >= 0 ? acc[w].key : cand_nil();
+        if (n == 0 || !iv_same_key(key, prev)) {
+            if (n == g.M) {
+                truncated = true;
+                break;
+            }
+            if (lane == 0) {
+                const size_t r = (size_t)s * g.M + n;
+                g.start[r] = x;
+                if (w >= 0 && acc[w].tail) fb_push(g.items, fb_pack(w, (int)r));
+                else store_cand(g.rec, r, key);
+            }
+            prev = key;
+            ++n;
+        }
+        float nx = __int_as_float(0x7f800000);
+        for (int a = lane; a < A; a += 32) nx = fminf(nx, acc[a].next);
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) nx = fminf(nx, __shfl_xor_sync(0xffffffffu, nx, d));
+        if (!(nx <= hi)) break;
+        __syncwarp();
+        for (int a = lane; a < A; a += 32)
+            if (acc[a].next == nx) {
+                iv_advance(g, s, a, nx, hi, acc[a]);
+                over |= acc[a].over;
+            }
+        __syncwarp();
+        truncated = __any_sync(0xffffffffu, over);  // the list ends below the first rate that overflows
+        x = nx;
+    }
+    if (lane == 0) {
+        g.count[s] = n;
+        g.truncated[s] = truncated;
+    }
+}
+
+// The record at an interval start whose winner is a load pair: the load grid's tail at that rate, then the value.
+template <class Solve>
+__device__ __forceinline__ bool iv_tail(const IntervalArgs& g, unsigned long long item, Solve&& solve, Cand& c) {
+    const DevFleet& f = g.ld.f;
+    const int r = (int)(unsigned)item, a = (int)(item >> 32), s = r / g.M;
+    const int e = g.cand_of_pair[s * f.A + a], N = g.ld.cand_N[e];
+    const double* tab = g.ld.tab + 4 * g.ld.tab_off[e];
+    if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, g.start[r]); }, (float)tab[4 * (N - 1)],
+                   [&](float lam, ModelStats& st) { return solve(tab, N, N + N * f.ratio, lam, st); }, c))
+        return false;
+    if (c.feasible) c.value = penalty_of(f, s, c);
+    return true;
+}
+
+__global__ void __launch_bounds__(256) interval_tail(IntervalArgs g) {
+    const int n = min(*g.items.count, g.items.cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned long long item = g.items.item[i];
+        Cand c;
+        const bool ok = iv_tail(g, item, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+            return solve_shared(tab, N, K, lam, st) == kSolveOk;
+        }, c);
+        if (!ok) fb_push(g.ld.fb, item);
+        store_cand(g.rec, (unsigned)item, c);
+    }
+}
+
+// Stored-vector re-run of the interval starts interval_tail bailed on.
+__global__ void interval_fallback(IntervalArgs g, FbRun r) {
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        int rc = 0;
+        Cand c;
+        if (!iv_tail(g, item, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+                rc = solve_stored(p, tab, N, K, lam, st);
+                return rc == 0;
+            }, c))
+            return rc;
+        store_cand(g.rec, (unsigned)item, c);
         return 0;
     });
 }

@@ -151,6 +151,32 @@ class Engine:
                                           C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
+    def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
+        """Where each server's ``load_grid`` winner changes its decision in ``[rpm_lo[s], rpm_hi[s]]`` (req/min)
+        -> (count [S], truncated [S], start_rpm (S, M), records: ``Allocs`` of S * M).
+
+        Interval ``j`` of server ``s`` starts at ``start_rpm[s, j]`` and ends where interval ``j + 1`` starts;
+        record ``s * M + j`` is ``load_grid``'s winner for ``s`` at that rate.  ``truncated[s]`` is 1 when the
+        decision changes again before ``rpm_hi[s]`` (see ``wva_load_intervals`` in include/wva_b200.h);
+        ``fleet.srv_arrival_rpm`` is not read."""
+        S, M = fleet.n_servers, int(max_per_server)
+        lo = np.ascontiguousarray(rpm_lo, np.float32)
+        hi = np.ascontiguousarray(rpm_hi, np.float32)
+        for name, col in (("rpm_lo", lo), ("rpm_hi", hi)):
+            if col.shape != (S,):
+                raise ValueError(f"{name} must have shape ({S},), got {col.shape}")
+        if M < 1:
+            raise ValueError("max_per_server must be at least 1")
+        count = np.zeros(S, np.int32)
+        truncated = np.zeros(S, np.uint8)
+        start = np.zeros((S, M), np.float32)
+        rec = Allocs(S * M)
+        oc = _abi.IntervalsC(M, _abi.ptr(count), _abi.ptr(truncated), _abi.ptr(start.reshape(-1)), rec.as_c())
+        fc = fleet.as_c()
+        self._resident(fleet)
+        self._check(self._L.wva_load_intervals(self._h, C.byref(fc), _abi.ptr(lo), _abi.ptr(hi), C.byref(oc)))
+        return count, truncated, start, rec
+
     def sweep(self, fleet: Fleet, n_rates: int) -> dict:
         n = fleet.n_servers * fleet.n_acc * n_rates
         out = {"valid": np.zeros(n, np.uint8)}
