@@ -1,11 +1,12 @@
-"""The cells handed to grid_kernel without a cell table, at the edges of grid_order's rank intervals.
+"""The cells handed to grid_kernel, at the edges of grid_order's rank intervals.
 
-Without a cell table grid_order lists, per (server, accelerator, replica level) row, the cells left for grid_kernel
-as two rank intervals, [0, min(lo, hi)) and [max(lo, kK), hi): lo is the row's first shared rank (b >= j + 2), kK the
-first rank with K >= 2^23 and hi the first rank whose key (group, batch size, accelerator) lies above the server's
-bound.  Rows with no load, pairs without a table and pairs with alpha > slo_itl have none; grid_sort_cands sorts
-them in chunks of at most 4096 candidates of one pair.  Every case here is checked byte for byte against the
-oracle's winners and the winners of the cell-table path (which evaluates every cell).
+grid_order lists, per (server, accelerator, replica level) row, the cells left for grid_kernel as two rank intervals,
+[0, min(lo, hi)) and [max(lo, kK), hi): lo is the row's first shared rank (b >= j + 2), kK the first rank with
+K >= 2^23 and hi the first rank whose key (group, batch size, accelerator) lies above the server's bound (B with a
+cell table).  Rows with no load and pairs without a table have none, nor, without a cell table, do pairs with
+alpha > slo_itl; grid_sort_cands sorts them in chunks of at most 4096 candidates of one pair.  Every case here is
+checked byte for byte against the oracle's winners and the winners of the cell-table path (which evaluates every
+cell).
 
 ``wva_dbg_read_plan`` returns item_count[2·256 + 1 ..], so slots 15 and 16 are the candidates and chunks that
 grid_order listed on the last call.
@@ -18,11 +19,13 @@ import numpy as np
 import pytest
 
 from tests.test_gpu_grid_pruning import _check, _same_winners
-from tests.test_gpu_grid_shapes import INV_BATCH, INV_REPLICAS, _analyzer_of, _lambda, invariant_fleet, shape_fleet
+from tests.test_gpu_grid_shapes import (INV_BATCH, INV_REPLICAS, _analyzer_of, _lambda, _three_ways, cell_shares_row,
+                                        invariant_fleet, shape_fleet)
 from tests.test_gpu_windows import chain_profile
 from workload_variant_autoscaler_b200 import Grid, config2_grid, synth_fleet
 
 CHUNK = 4096
+f32 = np.float32
 
 
 def _listed(engine):
@@ -126,6 +129,31 @@ def test_one_server_case_has_more_than_two_chunks_of_candidates(oracle_mod):
     assert n > 2 * CHUNK, n
 
 
+def test_gates_case_has_cells_only_grid_kernel_stores(oracle_mod):
+    """Without a cell table grid_order drops the pairs with alpha > slo_itl and grid_sort_cands the TPS cells above
+    the stability limit (lambda > RateRange.Max / 1000 · 0.9); with a cell table grid_kernel stores both as analysed
+    and not feasible.  The case has cells of both kinds that do not share their row's chain."""
+    fleet, grid = gates_case()
+    cells, _ = oracle_mod.grid_solve(fleet, grid, want_cells=True)
+    S, A = fleet.n_servers, fleet.n_acc
+    flags = cells["flags"].reshape(S, A, grid.batch.size, grid.replicas.size)
+    m = fleet.srv_model
+    found = {"itl": False, "tps": False}
+    for s, a, bi, ri in zip(*np.nonzero(flags == 1)):
+        s, a, b, r = int(s), int(a), int(grid.batch[bi]), int(grid.replicas[ri])
+        itl = fleet.srv_slo_itl[s]
+        if itl != 0 and fleet.perf_beta[m[s], a] >= 0 and fleet.perf_alpha[m[s], a] > itl:
+            kind = "itl"
+        elif fleet.srv_slo_tps[s] > 0:
+            lim = f32(f32(f32(_analyzer_of(fleet, s, a, b).rate_range()[1]) / f32(1000)) * f32(f32(1) - f32(0.1)))
+            kind = "tps" if _lambda(fleet, s, r) > lim else None
+        else:
+            kind = None
+        if kind and not found[kind] and not cell_shares_row(fleet, s, a, b, r):
+            found[kind] = True
+    assert all(found.values()), found
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------
@@ -155,6 +183,21 @@ def test_one_server_several_chunks_per_pair(engine, oracle_mod):
     n, chunks = _listed(engine)
     assert n > 2 * CHUNK and chunks >= 3, (n, chunks)  # two pairs: one of them has two chunks
     _check(engine, oracle_mod, fleet, grid, "one server, several chunks per pair")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", [one_server_case, gates_case], ids=lambda c: c.__name__)
+def test_cell_table_against_oracle(engine, oracle_mod, case):
+    """With a cell table grid_order lists every cell of a loaded row with a table that does not share its row's
+    chain: one_server_case spans several chunks per pair, and gates_case has ITL-out pairs and TPS cells above the
+    stability limit, which only grid_kernel stores."""
+    fleet, grid = case()
+    cells_o, win_o = oracle_mod.grid_solve(fleet, grid, want_cells=True)
+    if case is one_server_case:
+        engine.grid_solve(fleet, grid, want_cells=True)
+        n, chunks = _listed(engine)
+        assert n > 2 * CHUNK and chunks >= 3, (n, chunks)
+    _three_ways(engine, fleet, grid, cells_o, win_o, f"{case.__name__}, cell table")
 
 
 @pytest.mark.gpu

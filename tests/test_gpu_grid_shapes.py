@@ -8,14 +8,13 @@
   while ``Bmax <= kRowsSmemEntries = 1536``;
 * ``grid_order`` ranks with ``q`` threads per row (q doubles while ``2·q·n <= 1024``, ``n = A·R``), walks 256 rows
   per pass, and stages the batch sizes only while ``B <= 2048`` and ``RateRange.Max`` only while ``A·B <= 4096``;
-* ``grid_finalize`` gives each of its 256 threads ``ceil(A·R / 256)`` keys;
-* ``grid_sort_local`` caches the row constants of a lane's first two replica levels (levels 0..63) and sorts chunks of
-  ``kSortChunk = 8192`` cells, so a row of more than 8192 replica levels spans two chunks.
+* ``grid_finalize`` gives each of its 256 threads ``ceil(A·R / 256)`` keys.
 
 ``SHAPES`` puts one case on each side of each threshold, and ``test_shape_cases_sit_on_their_sides`` restates the
-rules from the fleet and the grid alone.  Every case runs three ways on the GPU: with the cell table (``grid_shared``),
-without it (``grid_order``, its bound and ``grid_finalize``'s re-evaluation), and pruned winners against cell-table
-winners byte for byte.  ``key_order_case`` adds a winner that only a key ordering batch size before accelerator
+rules from the fleet and the grid alone.  The ``R=`` cases also set how many rows of a pair ``grid_sort_cands``
+searches for a candidate's replica level, up to 8193.  Every case runs three ways on the GPU: with the cell table
+(``grid_shared``), without it (``grid_order``, its bound and ``grid_finalize``'s re-evaluation), and pruned winners
+against cell-table winners byte for byte.  ``key_order_case`` adds a winner that only a key ordering batch size before accelerator
 keeps below grid_order's bound.
 
 The second half is numeric.  ``grid_order`` and ``grid_shared`` evaluate a shared row through ``row_invariant`` when
@@ -48,16 +47,14 @@ COLUMNS = ("feasible", "acc", "replicas", "batch", "cost", "value", "itl", "ttft
 # the host rules, restated from the fleet and the grid
 # ---------------------------------------------------------------------------------------------------------------
 def host_plan(fleet, grid):
-    """Which side of each shape threshold a call is on, by the rules of prepare_grid, enqueue_grid, grid_order,
-    grid_finalize and grid_sort_local (wva_b200.cu, wva_kernels.cuh)."""
+    """Which side of each shape threshold a call is on, by the rules of prepare_grid, enqueue_grid, grid_order and
+    grid_finalize (wva_b200.cu, wva_kernels.cuh)."""
     A, B, R = fleet.n_acc, int(grid.batch.size), int(grid.replicas.size)
     Bmax = max(1, int(grid.batch.max()))
     n = A * R
     q = 1
     while q < 32 and 2 * q * n <= 1024:
         q *= 2
-    rows = fleet.n_servers * A * B
-    starts = np.arange(rows, dtype=np.int64) * R
     return {
         "prune": A <= 256 and Bmax < (1 << 24) and A * R <= 2048,        # prepare_grid
         "rows_threads": 128 if R >= 128 else (64 if R > 32 else 32),     # enqueue_grid
@@ -67,8 +64,6 @@ def host_plan(fleet, grid):
         "stage_b": B <= 2048,                                             # grid_order: batch sizes staged
         "stage_rmax": A * B <= 4096,                                      # grid_order: RateRange.Max staged
         "finalize_keys": -(-n // 256),                                    # grid_finalize: keys per thread
-        "sort_uncached": R > 64,                                          # grid_sort_local: levels past the cache
-        "row_spans_chunks": bool(np.any(starts // 8192 != (starts + R - 1) // 8192)),  # kSortChunk
     }
 
 
@@ -135,13 +130,13 @@ SHAPES = {
     "A*B=4097": (4, 17, ("draw", 241), [1, 3], {"stage_b": True, "stage_rmax": False}),
     "Bmax=1536": (5, 2, [24, 16, 1536, 48], [1, 2, 3, 5, 8, 13], {"rows_smem": True}),
     "Bmax=1537": (5, 2, [24, 16, 1537, 48], [1, 2, 3, 5, 8, 13], {"rows_smem": False}),
-    "R=32": (5, 2, SMALL_B, np.arange(1, 33), {"rows_threads": 32, "sort_uncached": False}),
-    "R=33": (5, 2, SMALL_B, np.arange(1, 34), {"rows_threads": 64, "sort_uncached": False}),
-    "R=64": (5, 2, SMALL_B, np.arange(1, 65), {"rows_threads": 64, "sort_uncached": False}),
-    "R=65": (5, 2, SMALL_B, np.arange(1, 66), {"rows_threads": 64, "sort_uncached": True}),
-    "R=127": (5, 2, SMALL_B, np.arange(1, 128), {"rows_threads": 64, "sort_uncached": True}),
-    "R=128": (5, 2, SMALL_B, np.arange(1, 129), {"rows_threads": 128, "sort_uncached": True}),
-    "R=8193": (5, 1, [24], np.arange(1, 8194), {"prune": False, "row_spans_chunks": True}),
+    "R=32": (5, 2, SMALL_B, np.arange(1, 33), {"rows_threads": 32}),
+    "R=33": (5, 2, SMALL_B, np.arange(1, 34), {"rows_threads": 64}),
+    "R=64": (5, 2, SMALL_B, np.arange(1, 65), {"rows_threads": 64}),
+    "R=65": (5, 2, SMALL_B, np.arange(1, 66), {"rows_threads": 64}),
+    "R=127": (5, 2, SMALL_B, np.arange(1, 128), {"rows_threads": 64}),
+    "R=128": (5, 2, SMALL_B, np.arange(1, 129), {"rows_threads": 128}),
+    "R=8193": (5, 1, [24], np.arange(1, 8194), {"prune": False}),
 }
 @functools.lru_cache(maxsize=None)
 def shape_case(name):
@@ -393,7 +388,7 @@ def test_shape_cases_sit_on_their_sides():
         assert not wrong, f"{name}: {wrong}"
     # and each threshold has a case on both of its sides
     plans = [host_plan(*shape_case(n)) for n in SHAPES]
-    for key in ("prune", "rows_smem", "stage_b", "stage_rmax", "sort_uncached", "row_spans_chunks"):
+    for key in ("prune", "rows_smem", "stage_b", "stage_rmax"):
         assert {p[key] for p in plans} == {True, False}, key
     for key, values in (("rows_threads", {32, 64, 128}), ("order_q", {1, 2, 4}), ("order_passes", {1, 2, 3}),
                         ("finalize_keys", {1, 2, 3})):

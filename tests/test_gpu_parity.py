@@ -378,8 +378,8 @@ def test_size_randomised_fleets(engine, oracle_mod):
 
 
 def test_grid_wide_replica_axis_and_long_tables(engine, oracle_mod):
-    """R = 100 replica levels (the per-lane row cache of grid_sort_local covers the first 64, the rest take the
-    generic path) and a 1700-entry table (longer than grid_rows' shared-memory staging; 18,700-state chains)."""
+    """R = 100 replica levels, ascending and then descending, and a 1700-entry table (longer than grid_rows'
+    shared-memory staging; 18,700-state chains)."""
     fleet = synth_fleet(2, 2, seed=77)
     fleet.srv_arrival_rpm[:] = np.float32([900.0, 2500.0])
     _grid_check(engine, oracle_mod, fleet, Grid([3, 1700], np.arange(1, 101)))

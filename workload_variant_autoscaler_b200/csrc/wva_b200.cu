@@ -998,7 +998,6 @@ struct GridPlan {
     GridArgs args;
     FbRun fb;
     size_t n_cells;
-    int n_blocks;
     int Bmax;
     Cols cells{256};  // layout of d_cells; the copy-back goes to the caller's cell table
 };
@@ -1094,14 +1093,13 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     if (n_cells > 0xfffffff0ull) return h->fail(WVA_ERR_UNSUPPORTED, "grid too large for one call (>= 2^32 cells)");
     g.n_cells = (long long)n_cells;
     plan->n_cells = (size_t)n_cells;
-    plan->n_blocks = (int)((n_cells + kSortChunk - 1) / kSortChunk);
     const size_t nc = std::max<size_t>(plan->n_cells, 1);
     // sort workspace: order u32 [n_cells] | items u64 | items_sorted u64 | item counter |
     // per-cell records in global item order (32 x 16 bytes per item) | grid_order's chunk list.
-    // A sort chunk (grid_sort_local: kSortChunk cells; grid_sort_cands: up to kCandChunk candidates of one pair, so
-    // at most n_cells / kCandChunk + S*A chunks) ends with at most one partial item.
+    // A sort chunk (up to kCandChunk candidates of one pair, so at most n_cells / kCandChunk + S*A chunks) ends with
+    // at most one partial item.
     const size_t max_chunks = nc / kCandChunk + n_pairs;
-    const size_t max_items = (nc + 31) / 32 + std::max((size_t)std::max(plan->n_blocks, 1), max_chunks);
+    const size_t max_items = (nc + 31) / 32 + max_chunks;
     Cols ws(256);
     const size_t o_order = ws.take(4 * nc), o_items = ws.take(8 * max_items), o_sorted = ws.take(8 * max_items),
                  o_count = ws.take(4 * (2 * kClasses + 32)), o_recs = ws.take(512 * max_items),
@@ -1173,15 +1171,12 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
             grid_rows<<<(unsigned)(hf.S * hf.A), rows_threads, rows_smem, h->stream>>>(g);
         }
         h->launches++;
-        if (g.want_cells) {
-            g.prune = 0;  // every cell is evaluated and stored
-            grid_sort_local<<<plan.n_blocks, kSortThreads, 0, h->stream>>>(g);
-        } else {
-            // the shared-chain cells, each server's bound and the cells left for grid_kernel, then their sort
-            grid_order<<<(unsigned)hf.S, kOrderThreads, 0, h->stream>>>(g);
-            h->launches++;
-            grid_sort_cands<<<(unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads, 0, h->stream>>>(g);
-        }
+        if (g.want_cells) g.prune = 0;  // every cell is evaluated and stored
+        // without a cell table the shared-chain cells and each server's bound; the cells left for grid_kernel, then
+        // their sort
+        grid_order<<<(unsigned)hf.S, kOrderThreads, 0, h->stream>>>(g);
+        h->launches++;
+        grid_sort_cands<<<(unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads, 0, h->stream>>>(g);
         grid_items_scatter<<<(unsigned)(16 * h->sm_count), 256, 0, h->stream>>>(g);  // warp per item (grid-stride)
         h->launches++;
         CK(cudaEventRecord(h->ev_k0, h->stream));  // wva_last_kernel_ms = the dominant kernel alone

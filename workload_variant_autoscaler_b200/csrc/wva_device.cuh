@@ -392,8 +392,8 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
         if (STAGED && staged) {
             // steps n < nh read entry n from the window, later steps the lane's own tail entry; all lanes
             // hold the same n (they advance together or leave together).  A window in which every lane
-            // is still in its head (the usual case: grid_sort_local keeps cells of similar batch size
-            // together) needs no per-lane select; only the first window feeds the stash.
+            // is still in its head (the usual case: grid_sort_cands keeps cells of one pair and similar
+            // length together) needs no per-lane select; only the first window feeds the stash.
             const double4* tab4 = reinterpret_cast<const double4*>(tab);
             double4* tb = reinterpret_cast<double4*>(tbuf);
             const int lane = threadIdx.x & 31;

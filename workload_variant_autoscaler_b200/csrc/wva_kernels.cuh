@@ -332,15 +332,13 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 //
 //   grid_rows        per (pair, replica level): the chain every large-enough batch size shares
 //                    (solve_row); also the (server, replica) rate block and the batch-rank reset
-//   grid_order       without a cell table, per server: the rows' order under grid_finalize's key, the cells
-//                    that share their row's chain up to the row's first feasible one, the server's bound
-//                    (the smallest key of a feasible cell found), and the cells left for grid_kernel as two
+//   grid_order       per server: without a cell table, the rows' order under grid_finalize's key, the cells
+//                    that share their row's chain up to the row's first feasible one and the server's bound
+//                    (the smallest key of a feasible cell found); then the cells left for grid_kernel as two
 //                    rank intervals per row, listed in chunks of at most 4096 of one pair
-//   grid_sort_local  with a cell table, per chunk of 8192 cells: gates + Analyze's rate checks; cells that
-//                    share their row's chain are left to grid_shared; the others get a log-domain length
+//   grid_sort_cands  per chunk (fixed grid, a chunk per CTA at a time): the per-cell gates, a log-domain length
 //                    estimate, an 8-bit class and a local counting sort -> warp items; the last CTA plans
 //                    grid_kernel's queues (grid_items_plan)
-//   grid_sort_cands  without a cell table, the same over grid_order's chunks (fixed grid, chunk per CTA at a time)
 //   grid_items_scatter  items ordered globally, longest class first
 //   grid_kernel      persistent CTA per SM; warps pull items (32 cells of nearly equal chain length)
 //                    from a long and a short queue: streaming solve, metrics, SLO feasibility,
@@ -382,7 +380,7 @@ struct GridArgs {
     int* row_j;                     // last state of the shared chain (INT_MAX: no sharing)
     int Bmax;                       // table length
     long long n_cells;
-    unsigned* order;         // [n_cells] cell ids, sorted by length class inside each chunk of kSortChunk cells
+    unsigned* order;         // [n_cells] cell ids, sorted by length class inside each of grid_order's chunks
     unsigned long long* items;         // warp work items (start | count << 32 | class << 40), unsorted
     unsigned long long* items_sorted;  // the same, longest class first
     unsigned* item_count;    // [0] number of items, [1..256] items per class, [257..512] class cursors
@@ -409,7 +407,7 @@ struct GridArgs {
     unsigned long_cap;       // ... up to this many (long_per_sm x CTAs)
     unsigned* dbg_cycles;    // diagnostics: per order index, SM cycles spent in grid_kernel (or NULL)
     size_t dbg_n;            // cells; dbg_cycles[dbg_n + idx] holds the warp timeline (start ns, SM, end ns)
-    // without a cell table (grid_order -> grid_sort_cands): the cells handed to grid_kernel, row by row
+    // grid_order -> grid_sort_cands: the cells handed to grid_kernel, row by row
     int4* row_cand;          // [S*A*R] {row's first candidate inside its pair, n1, s2, 0}: the row's candidates are the
                              // ranks [0, n1) and then s2, s2 + 1, ...
     uint4* chunks;           // chunk list: {pair, first candidate inside the pair, count, place in order[]}
@@ -676,7 +674,8 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
     }
 }
 
-// Without a cell table, between grid_rows and grid_sort_cands: one CTA per server.
+// Between grid_rows and grid_sort_cands: one CTA per server.  With a cell table (pruning off) only step 3 runs:
+// grid_shared evaluates every shared cell after grid_kernel, which the walk of step 2 would only repeat.
 //  1. Group ranks (g.prune): every (accelerator, replica level) row gets the number of rows of the server strictly
 //     below it in (value, cost, replicas), with value and cost computed as grid_finalize computes them.  A counting
 //     rank, Q threads per row.  It keeps key_better's order, ties included (-0 == +0); rows without a table take part
@@ -693,20 +692,22 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
 //     drops a cell cuts a row at one rank, since batch sizes ascend with the rank: shared cells are the ranks
 //     [lo, kK) (lo: the first rank with b >= jl + 2, B without sharing; kK: the first rank with K >= 2^23, the same
 //     for every row), and cells above the bound the ranks [hi, B) (keys grow along a row).  So the candidates are
-//     [0, min(lo, hi)) and [max(lo, kK), hi).  Rows with rt.x <= 0 and pairs without a table or with alpha > slo_itl
-//     (ITL = alpha + beta * eff >= alpha, eff >= 0, beta >= 0) have none.  A warp per pair scans its rows' counts
+//     [0, min(lo, hi)) and [max(lo, kK), hi).  Rows with rt.x <= 0 and pairs without a table have none, nor, without
+//     a cell table, do pairs with alpha > slo_itl (ITL = alpha + beta * eff >= alpha, eff >= 0, beta >= 0); with a
+//     cell table grid_kernel stores their cells as analysed and not feasible.  A warp per pair scans its rows' counts
 //     into their first candidates, then reserves the pair's chunks of kCandChunk candidates in the chunk list and
 //     their places in order[] with one atomic.
 //
-// No pass over the shared cells is needed after grid_kernel.  Every cell that is never evaluated — a shared cell
-// after the stop of its row's walk, or a non-shared cell that is not a candidate or that grid_sort_cands or
-// grid_kernel skips — either cannot be feasible (the exact gates above and in grid_sort_cands) or has a key strictly
-// above a feasible cell of its server.  So the winner W (the smallest key among the feasible cells) is evaluated, and
-// so is every feasible cell of W's row below W, which has a smaller or equal key: best_rank of W's row is W's rank.
-// Any other best_rank is a feasible cell, whose key is >= W's.  grid_finalize picks W exactly as when every cell is
-// evaluated.
+// Without a cell table no pass over the shared cells is needed after grid_kernel.  Every cell that is never
+// evaluated — a shared cell after the stop of its row's walk, or a non-shared cell that is not a candidate or that
+// grid_sort_cands or grid_kernel skips — either cannot be feasible (the exact gates above and in grid_sort_cands) or
+// has a key strictly above a feasible cell of its server.  So the winner W (the smallest key among the feasible cells)
+// is evaluated, and so is every feasible cell of W's row below W, which has a smaller or equal key: best_rank of W's
+// row is W's rank.  Any other best_rank is a feasible cell, whose key is >= W's.  grid_finalize picks W exactly as
+// when every cell is evaluated.
 constexpr int kOrderThreads = 1024, kOrderG = 4, kOrderMaxRows = 2048;
 constexpr int kCandChunk = 4096;               // candidates per chunk of grid_sort_cands (never two pairs)
+constexpr int kCandThreads = 256, kCandCtasPerSm = 4;
 constexpr int kCandResv = 2 * kClasses + 16;   // item_count[kCandResv], [kCandResv + 1]: candidates, chunks reserved
 __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
     __shared__ float s_vc[2 * kOrderMaxRows];  // ranking: values | costs; walk: RateRange.Max per (accelerator, rank)
@@ -784,7 +785,7 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
     __syncthreads();
     auto batch_at = [&](int r) { return stage_b ? s_rep[r] : g.batch[g.rank_to_bi[r]]; };
     const unsigned sub = lane % kOrderG, gmask = ((1u << kOrderG) - 1u) << (lane - sub);
-    for (int base = 0; base < n; base += (int)blockDim.x / kOrderG) {
+    for (int base = 0; base < n && !g.want_cells; base += (int)blockDim.x / kOrderG) {
         const int p = base + (int)tid / kOrderG;
         const int k = p < n ? (prune ? s_at[p] : p) : 0;
         const int a = k / R, ri = k - a * R;
@@ -860,7 +861,7 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
     for (int a = (int)(tid >> 5); a < A; a += kOrderThreads / 32) {
         const int sa = s * A + a;
         bool out = g.pair_tab_off[sa] < 0;
-        if (!out) {  // a table implies a valid model index (pair_class == PAIR_LOAD)
+        if (!out && !g.want_cells) {  // a table implies a valid model index (pair_class == PAIR_LOAD)
             const int k = f.srv_model[s] * A + a;
             const float slo_itl = f.srv_slo_itl[s];
             out = slo_itl != 0.0f && f.perf_beta[k] >= 0.0f && f.perf_alpha[k] > slo_itl;
@@ -932,13 +933,13 @@ __device__ __forceinline__ unsigned seg_inc(unsigned* counters, int key) {
     return base + __popc(seg_mask & ((1u << lane) - 1u));
 }
 
-// The end of a chunk's sort, the same in both sort kernels: keys[0, n) hold the chunk's length classes (255: the
-// cell is not handed to grid_kernel) and hist their counts.  The counts are scanned into class cursors, the cells
-// are scattered into order[obase ...] by class (cell_of(k): the id of the chunk's k-th cell), and each run of 32
-// sorted cells becomes one warp work item tagged with its (longest) class.
-template <int kThreads, class CellOf>
-__device__ __forceinline__ void sort_chunk_items(const GridArgs& g, const uint8_t* keys, uint8_t* sorted_keys,
-                                                 unsigned* hist, unsigned* cursor, int n, unsigned obase, CellOf cell_of) {
+// The end of a chunk's sort: cells[0, n) hold the chunk's cell ids, keys[0, n) their length classes (255: the cell
+// is not handed to grid_kernel) and hist the class counts.  The counts are scanned into class cursors, the cells are
+// scattered into order[obase ...] by class, and each run of 32 sorted cells becomes one warp work item tagged with
+// its (longest) class.
+__device__ __forceinline__ void sort_chunk_items(const GridArgs& g, const unsigned* cells, const uint8_t* keys,
+                                                 uint8_t* sorted_keys, unsigned* hist, unsigned* cursor, int n,
+                                                 unsigned obase) {
     __shared__ unsigned item_base;
     if (threadIdx.x < 32) {  // exclusive scan of the 256 class counts by one warp
         unsigned run = 0;
@@ -956,17 +957,17 @@ __device__ __forceinline__ void sort_chunk_items(const GridArgs& g, const uint8_
     }
     __syncthreads();
     const int n_active = (int)cursor[255];  // class 255 (not analysable) sorts last
-    for (int k = threadIdx.x; k < n; k += kThreads) {
+    for (int k = threadIdx.x; k < n; k += kCandThreads) {
         const int key = keys[k];
         if (key == 255) continue;
         const unsigned pos = seg_inc(cursor, key);
-        g.order[obase + pos] = cell_of(k);
+        g.order[obase + pos] = cells[k];
         sorted_keys[pos] = (uint8_t)key;
     }
     const int n_items = (n_active + 31) >> 5;
     if (threadIdx.x == 0) item_base = n_items ? atomicAdd(g.item_count, (unsigned)n_items) : 0u;
     __syncthreads();
-    for (int w = threadIdx.x; w < n_items; w += kThreads) {
+    for (int w = threadIdx.x; w < n_items; w += kCandThreads) {
         const unsigned start = obase + 32 * w;
         const unsigned cnt = (unsigned)min(32, n_active - 32 * w);
         const int cls = sorted_keys[32 * w];
@@ -976,7 +977,7 @@ __device__ __forceinline__ void sort_chunk_items(const GridArgs& g, const uint8_
     }
 }
 
-// The last CTA of a sort kernel to get here turns the global histogram into class cursors and plans grid_kernel's
+// The last CTA of grid_sort_cands to get here turns the global histogram into class cursors and plans grid_kernel's
 // queues (one launch less than a separate single-CTA kernel).
 __device__ __forceinline__ void grid_items_plan(const GridArgs& g);
 __device__ __forceinline__ void sort_plan_in_last_cta(const GridArgs& g) {
@@ -991,98 +992,13 @@ __device__ __forceinline__ void sort_plan_in_last_cta(const GridArgs& g) {
     }
 }
 
-// With a cell table: estimate + LOCAL counting sort, one CTA per chunk of kSortChunk consecutive cells (cells of
-// one or two (server, accelerator) pairs): length classes are computed into shared memory, histogrammed, scanned and
-// scattered without leaving the CTA; grid_items_scatter then orders the items globally, so the launch is
-// longest-first while a pair's cells stay adjacent.
-__global__ void __launch_bounds__(kSortThreads, 2) grid_sort_local(GridArgs g) {
-    __shared__ uint8_t keys[kSortChunk];
-    __shared__ uint8_t sorted_keys[kSortChunk];
-    __shared__ unsigned hist[kClasses];
-    __shared__ unsigned cursor[kClasses];
-    const DevFleet& f = g.f;
-    if (threadIdx.x < kClasses) hist[threadIdx.x] = 0;
-    __syncthreads();
-    const long long base = (long long)blockIdx.x * kSortChunk;
-    const int n_here = (int)min((long long)kSortChunk, g.n_cells - base);
-    // walk the chunk row by row (a row = the R replica levels of one (server, accelerator, batch)):
-    // the row's constants are decoded once per warp, lanes take the replica levels
-    {
-        const unsigned R = (unsigned)g.R, B = (unsigned)g.B, A = (unsigned)f.A;
-        const unsigned row0 = (unsigned)(base / R), row1 = (unsigned)((base + n_here - 1) / R);
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        // pair-level constants are re-read only when the walk crosses into the next pair; so are the
-        // lane's own row constants (its first two replica levels: rate, lambda, the row's shared chain)
-        struct LaneRow {
-            float4 rt;
-            int jl;
-        };
-        unsigned cur_sa = 0xffffffffu;
-        LaneRow c0{}, c1{};
-        unsigned sa = (row0 + warp) / B;
-        int bi = (int)(row0 + warp - sa * B);
-        int s = 0, t = 0;
-        long long toff = -1;
-        auto load_lane = [&](unsigned ri, LaneRow& c) {
-            if (ri >= R || toff < 0) return;
-            c.rt = g.rt[(unsigned)s * R + ri];
-            c.jl = g.row_j[(size_t)sa * R + ri];
-        };
-        for (unsigned row = row0 + warp; row <= row1; row += kSortThreads / 32, bi += kSortThreads / 32) {
-            while (bi >= (int)B) {
-                bi -= (int)B;
-                ++sa;
-            }
-            if (sa != cur_sa) {
-                cur_sa = sa;
-                s = (int)(sa / A);
-                toff = g.pair_tab_off[sa];
-                if (toff >= 0) t = g.pair_tab_idx[sa];
-                load_lane(lane, c0);
-                load_lane(lane + 32, c1);
-            }
-            const int b = g.batch[bi];
-            const int K = b + b * f.ratio;
-            float4 pb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (toff >= 0) pb = g.pb[(size_t)t * g.B + bi];
-            // one cell: (row, ri) with the lane's cached row constants
-            auto do_cell = [&](unsigned ri, const LaneRow& c) {
-                const long long cell = (long long)row * R + ri;
-                if (cell < base || cell >= base + n_here) return;
-                int key = 255;
-                if (toff >= 0 && !(c.rt.x <= 0.0f) && !(c.rt.x > pb.x) && K >= 2) {  // Analyze: queueanalyzer.go:135-143
-                    // a cell that shares its row's chain stays at class 255: grid_shared evaluates it
-                    const bool shared = c.jl != INT_MAX && b >= c.jl + 2 && K < (1 << 23);
-                    if (!shared)
-                        key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, c.rt.y, c.rt.z, pb.w, pb.y, pb.z));
-                }
-                keys[cell - base] = (uint8_t)key;
-                if (key != 255) seg_inc(hist, key);  // class 255 (shared / not analysable) needs no slot
-                // (the cell table is cleared by the host before the launch: cells that are never analysed read back
-                // as 0 without a store per cell here)
-            };
-            if ((unsigned)lane < R) do_cell(lane, c0);
-            if ((unsigned)lane + 32 < R) do_cell(lane + 32, c1);
-            for (unsigned ri = lane + 64; ri < R; ri += 32) {
-                LaneRow c;
-                load_lane(ri, c);
-                do_cell(ri, c);
-            }
-        }
-    }
-    __syncthreads();
-    sort_chunk_items<kSortThreads>(g, keys, sorted_keys, hist, cursor, n_here, (unsigned)base,
-                                   [&](int k) { return (unsigned)(base + k); });
-    sort_plan_in_last_cta(g);
-}
-
-// Without a cell table: grid_order's candidates, a chunk (at most kCandChunk candidates of one pair) per CTA at a
-// time over a fixed grid.  A candidate's replica level is the last row of the pair whose first candidate is at or
-// before it, and its rank follows from that row's intervals.  The gates that grid_order's intervals leave to each
-// cell — Analyze's RateRange.Max and K >= 2, and TPS servers above the stability limit — give class 255; the others
-// get the length class, and grid_sort_local's tail sorts the chunk into items.  A chunk never holds two pairs, so
-// neither does an item (grid_kernel fetches the pair record once per item).
-constexpr int kCandThreads = 256, kCandCtasPerSm = 4;
+// grid_order's candidates, a chunk (at most kCandChunk candidates of one pair) per CTA at a time over a fixed grid.
+// A candidate's replica level is the last row of the pair whose first candidate is at or before it, and its rank
+// follows from that row's intervals.  The gates that grid_order's intervals leave to each cell — Analyze's
+// RateRange.Max and K >= 2, and, without a cell table, TPS servers above the stability limit (with one, grid_kernel
+// stores those cells as analysed and not feasible) — give class 255; the others get the length class, and
+// sort_chunk_items sorts the chunk into items.  A chunk never holds two pairs, so neither does an item (grid_kernel
+// fetches the pair record once per item).
 __global__ void __launch_bounds__(kCandThreads) grid_sort_cands(GridArgs g) {
     __shared__ unsigned cells[kCandChunk];
     __shared__ uint8_t keys[kCandChunk];
@@ -1098,7 +1014,7 @@ __global__ void __launch_bounds__(kCandThreads) grid_sort_cands(GridArgs g) {
         __syncthreads();
         const int sa = (int)ch.x, s = sa / f.A, t = g.pair_tab_idx[sa];
         const long long toff = g.pair_tab_off[sa];
-        const bool tps = f.srv_slo_tps[s] > 0.0f;
+        const bool tps = f.srv_slo_tps[s] > 0.0f && !g.want_cells;
         const int4* rc = g.row_cand + (size_t)sa * R;
         for (int k = threadIdx.x; k < (int)ch.z; k += kCandThreads) {
             const int j = (int)ch.y + k;
@@ -1122,8 +1038,7 @@ __global__ void __launch_bounds__(kCandThreads) grid_sort_cands(GridArgs g) {
             if (key != 255) seg_inc(hist, key);  // along a row, consecutive ranks: runs of equal classes
         }
         __syncthreads();
-        sort_chunk_items<kCandThreads>(g, keys, sorted_keys, hist, cursor, (int)ch.z, ch.w,
-                                       [&](int k) { return cells[k]; });
+        sort_chunk_items(g, cells, keys, sorted_keys, hist, cursor, (int)ch.z, ch.w);
     }
     sort_plan_in_last_cta(g);
 }
@@ -1316,10 +1231,10 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
         const bool live = valid && cell_key(grp, N, (int)(pair - s * (unsigned)f.A)) <= bound;
         if (!__any_sync(0xffffffffu, live)) return;
     }
-    // one pair per item is the rule (an item is cut from one sort chunk); then lanes 0..2 fetch its record
-    const bool one_pair = __all_sync(0xffffffffu, pair == __shfl_sync(0xffffffffu, pair, 0));
+    // an item holds one pair (a sort chunk never holds two, and a padded lane copies the item's first cell), so
+    // lanes 0..2 fetch its record
     __syncwarp();  // the previous item's readers of pair_buf are done
-    if (one_pair && lane < 3) cp_async16(pair_buf + lane, g.pair_rec + 3 * (size_t)pair + lane);
+    if (lane < 3) cp_async16(pair_buf + lane, g.pair_rec + 3 * (size_t)pair + lane);
     cp_async_commit();
     ModelStats st;
     const int rc = solve_shared_t<kGridStash, 10, true>(tab, N, K, lambda, st, stash_warp + lane, tbuf_warp);
@@ -1329,9 +1244,7 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
         if (rc != kSolveOk) {
             fb_push(FbList{g.fb_count, g.fb_cells, g.fb_cap}, cell);
         } else {
-            const float4 r0 = one_pair ? pair_buf[0] : g.pair_rec[3 * (size_t)pair + 0];
-            const float4 r1 = one_pair ? pair_buf[1] : g.pair_rec[3 * (size_t)pair + 1];
-            const float4 r2 = one_pair ? pair_buf[2] : g.pair_rec[3 * (size_t)pair + 2];
+            const float4 r0 = pair_buf[0], r1 = pair_buf[1], r2 = pair_buf[2];
             QParams q;
             q.alpha = r0.x; q.beta = r0.y; q.gamma = r0.z; q.delta = r0.w;
             q.in_tok = __float_as_int(r1.x); q.out_tok = __float_as_int(r1.y);
