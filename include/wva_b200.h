@@ -204,6 +204,16 @@ int wva_abi_version(void);
  * Replaces ModelAnalyzer.AnalyzeModel (internal/modelanalyzer/analyzer.go:25-34)
  * called in a loop at internal/controller/variantautoscaling_controller.go:149-156.
  * `candidates` has S*A entries.
+ *
+ * Queue sizes (wva_analyze, wva_solve, wva_resolve and every call below that builds queue models): a load pair,
+ * i.e. one that passes the gates with a positive arrival rate and out_tokens >= 1, builds the reference's queue
+ * model of batch size N (srv_max_batch, else max(perf_max_batch * perf_at_tokens / out_tokens, 1)) with
+ * N + N * max_queue_to_batch_ratio states.  Both are computed in 64 bits, as Go's int.  The call returns
+ * WVA_ERR_UNSUPPORTED, before any kernel is launched and with a wva_last_error text naming the cause, when such
+ * an N is above 2^20 or such a model has 2^31 states or more: the reference would need a p[] vector of 2^31
+ * doubles or more, and this library counts states in int32.  Zero-load pairs (zeroLoadAllocation reads
+ * perf_max_batch directly) and gated pairs build no model and are never refused.  wva_resolve applies the rule to
+ * the resident fleet as wva_update_load left it.
  */
 int wva_analyze(wva_handle *h, const wva_fleet *fleet, wva_allocs *candidates);
 
@@ -223,7 +233,9 @@ int wva_solve(wva_handle *h, const wva_fleet *fleet, wva_allocs *candidates,
 /*
  * Full candidate grid + per-server min-value SLO-feasible cell.
  * Winner order: value, then cost, then replicas, then batch, then accelerator id
- * (all ascending).  `cells` may be NULL.
+ * (all ascending).  `cells` may be NULL.  WVA_ERR_UNSUPPORTED (the queue-size rule of wva_analyze, for
+ * wva_grid_solve_device too): some server has a load pair, the grid has a replica level, and the largest listed
+ * batch size b has b * (1 + max_queue_to_batch_ratio) >= 2^31.
  */
 int wva_grid_solve(wva_handle *h, const wva_fleet *fleet, const wva_grid *grid,
                    wva_cells *cells, wva_allocs *winners);
@@ -246,8 +258,9 @@ int wva_grid_solve(wva_handle *h, const wva_fleet *fleet, const wva_grid *grid,
  *
  * `candidates` (S*A*n_batch entries) may be NULL; `winners` has S entries.  n_batch == 0 is valid (every
  * winner is nil).  WVA_ERR_BAD_ARG: n_batch < 0, batch NULL with n_batch > 0, or a batch size outside
- * [1, 2^20].  WVA_ERR_UNSUPPORTED: S*A*n_batch >= 2^31, or, as for wva_solve, too many candidates need the
- * stored-vector fallback or its rescale loop would not terminate.
+ * [1, 2^20].  WVA_ERR_UNSUPPORTED: S*A*n_batch >= 2^31; some server has a load pair and the largest listed
+ * batch size b has b * (1 + max_queue_to_batch_ratio) >= 2^31 (the queue-size rule of wva_analyze); or, as for
+ * wva_solve, too many candidates need the stored-vector fallback or its rescale loop would not terminate.
  */
 int wva_size_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_batch, const int32_t *batch,
                   wva_allocs *candidates, wva_allocs *winners);
@@ -273,7 +286,8 @@ int wva_size_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_batch, const 
  * n_levels*S entries.  n_levels == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG: n_levels < 0,
  * arrival_rpm NULL with n_levels > 0, or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_levels >= 2^31 (refused
  * before the fleet is read), or a level on which wva_analyze of f_l fails the same way (a NaN rate whose
- * rescale loop would not terminate, too many stored-vector fallbacks).
+ * rescale loop would not terminate, too many stored-vector fallbacks, a load pair outside wva_analyze's
+ * queue-size rule).
  */
 int wva_load_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
                   wva_allocs *candidates, wva_allocs *winners);
@@ -311,8 +325,10 @@ int wva_load_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const
  * wva_summarize returns WVA_ERR_STATE afterwards, as after wva_load_grid.  Columns of out->rec may be NULL (not
  * written).  WVA_ERR_BAD_ARG: out NULL, max_per_server < 1, rpm_lo, rpm_hi, count, truncated or start_rpm NULL
  * with S > 0, a bound that is NaN, infinite or negative, or rpm_lo[s] > rpm_hi[s].  WVA_ERR_UNSUPPORTED:
- * S * max_per_server >= 2^31, or a range in which wva_load_grid fails: an interval start whose solve fails the
- * same way (a rescale loop that would not terminate, too many stored-vector fallbacks), or a positive rate below
+ * S * max_per_server >= 2^31; a server with rpm_hi[s] > 0 and a pair outside wva_analyze's queue-size rule (the
+ * pair is a load pair at some rate of its range); or a range in which wva_load_grid fails: an interval start
+ * whose solve fails the same way (a rescale loop that would not terminate, too many stored-vector fallbacks), or a
+ * positive rate below
  * 60 * 2^-150 req/min on a server with a min_replicas-0 load pair.  There totalRate rounds to 0, the pair gets 0
  * replicas and Analyze solves at 0/0, whose rescale loop does not terminate in wva_load_grid (the Go reference
  * reports NaN latencies there).
@@ -341,7 +357,9 @@ int wva_solve_greedy(const wva_fleet *fleet, wva_allocs *candidates, wva_allocs 
 /*
  * Latency sweep of QueueAnalyzer.Analyze over n_rates rates per (server, acc).  A point whose chain leaves
  * the streaming solve's exponent windows is re-run on the stored p[0..K] vector with the reference's rescale
- * loops, like a grid cell; WVA_ERR_UNSUPPORTED only when that rescale loop would not terminate (NaN rates).
+ * loops, like a grid cell.  WVA_ERR_UNSUPPORTED when that rescale loop would not terminate (NaN rates), or when a
+ * swept pair (every pair with a profile, in_tokens >= 0 and out_tokens >= 1, whatever its rate) is outside
+ * wva_analyze's queue-size rule.
  */
 int wva_sweep(wva_handle *h, const wva_fleet *fleet, int32_t n_rates, wva_sweep_out *out);
 

@@ -128,6 +128,7 @@ def lib():
     L.wvao_calculate.argtypes = [vp, vp]
     L.wvao_last_solves.restype = C.c_int64
     L.wvao_last_states.restype = C.c_int64
+    L.wvao_take_unsupported.restype = C.c_int64
     L.wvao_solve_unlimited.argtypes = [vp, vp, vp]
     L.wvao_solve_greedy.argtypes = [vp, vp, vp]
     L.wvao_solve.argtypes = [vp, vp, vp]
@@ -294,10 +295,25 @@ def binary_search(xmin, xmax, ytarget, fn):
     return err, xs.value, ind.value
 
 
+class Unsupported(RuntimeError):
+    """The call would build a queue model of 2^31 states or more (N + N * max_queue_to_batch_ratio, in Go's 64-bit
+    int): outside the oracle's int32 domain, as it is outside the CUDA library's (WVA_ERR_UNSUPPORTED)."""
+
+
+def _refusing(call):
+    """Runs call() and raises Unsupported if the oracle refused a queue model during it."""
+    lib().wvao_take_unsupported()
+    out = call()
+    n = lib().wvao_take_unsupported()
+    if n:
+        raise Unsupported(f"{n} queue model(s) of 2^31 states or more")
+    return out
+
+
 def create_allocation(fleet, s, a) -> dict:
     rec = AllocRec()
     fc = fleet.as_c()
-    lib().wvao_create_allocation(C.addressof(fc), s, a, C.byref(rec))
+    _refusing(lambda: lib().wvao_create_allocation(C.addressof(fc), s, a, C.byref(rec)))
     return {n: getattr(rec, n) for n, _ in AllocRec._fields_}
 
 
@@ -305,7 +321,7 @@ def calculate(fleet) -> np.ndarray:
     """Server.Calculate for every server -> structured array [S, A]."""
     out = np.zeros((fleet.n_servers, fleet.n_acc), ALLOC_DTYPE)
     fc = fleet.as_c()
-    lib().wvao_calculate(C.addressof(fc), out.ctypes.data)
+    _refusing(lambda: lib().wvao_calculate(C.addressof(fc), out.ctypes.data))
     return out
 
 
@@ -344,15 +360,15 @@ def grid_solve(fleet, grid, want_cells=True):
     cells = np.zeros(n, CELL_DTYPE) if want_cells else None
     win = np.zeros(fleet.n_servers, ALLOC_DTYPE)
     fc, gc = fleet.as_c(), grid.as_c()
-    lib().wvao_grid_solve(C.addressof(fc), C.addressof(gc), cells.ctypes.data if want_cells else None,
-                          win.ctypes.data)
+    _refusing(lambda: lib().wvao_grid_solve(C.addressof(fc), C.addressof(gc),
+                                            cells.ctypes.data if want_cells else None, win.ctypes.data))
     return cells, win
 
 
 def grid_cells(fleet, grid, c0, c1):
     cells = np.zeros(c1 - c0, CELL_DTYPE)
     fc, gc = fleet.as_c(), grid.as_c()
-    lib().wvao_grid_cells(C.addressof(fc), C.addressof(gc), c0, c1, cells.ctypes.data)
+    _refusing(lambda: lib().wvao_grid_cells(C.addressof(fc), C.addressof(gc), c0, c1, cells.ctypes.data))
     return cells
 
 
@@ -362,8 +378,8 @@ def sweep(fleet, n_rates):
     for k in ("rate", "ttft", "itl", "throughput", "rho"):
         out[k] = np.zeros(n, np.float32)
     fc = fleet.as_c()
-    lib().wvao_sweep(C.addressof(fc), n_rates, *[out[k].ctypes.data for k in
-                                                  ("valid", "rate", "ttft", "itl", "throughput", "rho")])
+    _refusing(lambda: lib().wvao_sweep(C.addressof(fc), n_rates, *[out[k].ctypes.data for k in
+                                                            ("valid", "rate", "ttft", "itl", "throughput", "rho")]))
     return out
 
 

@@ -43,6 +43,27 @@ static int64_t g_solves, g_states;
 int64_t wvao_last_solves(void) { return g_solves; }
 int64_t wvao_last_states(void) { return g_states; }
 
+/* Queue models the oracle refused since the last call of this function (see queue_states). */
+static int64_t g_unsupported;
+int64_t wvao_take_unsupported(void) {
+    int64_t n = g_unsupported;
+    g_unsupported = 0;
+    return n;
+}
+
+/* BuildModel's K = MaxBatchSize + MaxQueueSize with MaxQueueSize = N * MaxQueueToBatchRatio, in Go's 64-bit int
+ * (allocation.go:88-93, queueanalyzer.go:115).  A model of 2^31 states or more has no int32 K (the analyzer here,
+ * the CUDA library and the ABI all count states in int32) and would need a p[] of 16 GiB or more: it is counted
+ * in g_unsupported and -1 is returned, and the caller builds nothing. */
+static int queue_states(int64_t N, int ratio, int *max_queue) {
+    if (N >= ((int64_t)1 << 31) || N * (1 + (int64_t)ratio) >= ((int64_t)1 << 31)) {
+        g_unsupported++;
+        return -1;
+    }
+    *max_queue = ratio < 0 ? -1 : (int)(N * ratio); /* negative: Configuration.check refuses it */
+    return 0;
+}
+
 /* ------------------------------------------------------------------------ */
 /* pkg/analyzer/queueanalyzer.go: service-time model                        */
 /* ------------------------------------------------------------------------ */
@@ -618,14 +639,16 @@ void wvao_create_allocation(const wva_fleet *f, int s, int a, wvao_alloc *o) {
         return;
     }
     int K = f->srv_out_tokens[s];
-    int N;
+    int64_t N64;
     if (f->srv_max_batch[s] > 0) {
-        N = f->srv_max_batch[s];
+        N64 = f->srv_max_batch[s];
     } else {
         int64_t t = (int64_t)f->perf_max_batch[m * A + a] * (int64_t)f->perf_at_tokens[m * A + a] / K;
-        N = (int)(t > 1 ? t : 1);
+        N64 = t > 1 ? t : 1;
     }
-    int max_queue = N * f->tun.max_queue_to_batch_ratio;
+    int max_queue;
+    if (queue_states(N64, f->tun.max_queue_to_batch_ratio, &max_queue) != 0) return;
+    int N = (int)N64;
 
     wvao_analyzer *qa = wvao_analyzer_new(N, max_queue, f->perf_alpha[m * A + a], f->perf_beta[m * A + a],
                                           f->perf_gamma[m * A + a], f->perf_delta[m * A + a],
@@ -1110,7 +1133,9 @@ static void eval_cell(const wva_fleet *f, int s, int a, int b, int r, cell_eval 
     const int A = f->n_acc;
     int m = f->srv_model[s];
     memset(ce, 0, sizeof(*ce));
-    wvao_analyzer *qa = wvao_analyzer_new(b, b * f->tun.max_queue_to_batch_ratio, f->perf_alpha[m * A + a],
+    int max_queue;
+    if (queue_states(b, f->tun.max_queue_to_batch_ratio, &max_queue) != 0) return;
+    wvao_analyzer *qa = wvao_analyzer_new(b, max_queue, f->perf_alpha[m * A + a],
                                           f->perf_beta[m * A + a], f->perf_gamma[m * A + a],
                                           f->perf_delta[m * A + a], f->srv_in_tokens[s], f->srv_out_tokens[s]);
     if (!qa) return;
@@ -1219,13 +1244,13 @@ void wvao_grid_cells(const wva_fleet *f, const wva_grid *g, int64_t c0, int64_t 
 
 /* Batch size a (server, accelerator) pair is analysed at outside the grid:
  * allocation.go:77-87. */
-static int pair_batch(const wva_fleet *f, int s, int a) {
+static int64_t pair_batch(const wva_fleet *f, int s, int a) {
     const int A = f->n_acc;
     int m = f->srv_model[s];
     if (f->srv_max_batch[s] > 0) return f->srv_max_batch[s];
     int64_t t = (int64_t)f->perf_max_batch[m * A + a] * (int64_t)f->perf_at_tokens[m * A + a] /
                 f->srv_out_tokens[s];
-    return (int)(t > 1 ? t : 1);
+    return t > 1 ? t : 1;
 }
 
 void wvao_sweep(const wva_fleet *f, int n_rates, uint8_t *valid, float *rate, float *ttft, float *itl,
@@ -1240,10 +1265,11 @@ void wvao_sweep(const wva_fleet *f, int n_rates, uint8_t *valid, float *rate, fl
             /* the sweep ignores keepAccelerator: it characterises every profile */
             int gate = f->srv_in_tokens[s] >= 0 && f->srv_out_tokens[s] >= 1 && f->srv_model[s] >= 0 &&
                        f->srv_model[s] < f->n_models && f->perf_present[f->srv_model[s] * A + a];
-            if (gate) {
+            int max_queue;
+            int64_t N = gate ? pair_batch(f, s, a) : 0;
+            if (gate && queue_states(N, f->tun.max_queue_to_batch_ratio, &max_queue) == 0) {
                 int m = f->srv_model[s];
-                int N = pair_batch(f, s, a);
-                qa = wvao_analyzer_new(N, N * f->tun.max_queue_to_batch_ratio, f->perf_alpha[m * A + a],
+                qa = wvao_analyzer_new((int)N, max_queue, f->perf_alpha[m * A + a],
                                        f->perf_beta[m * A + a], f->perf_gamma[m * A + a],
                                        f->perf_delta[m * A + a], f->srv_in_tokens[s], f->srv_out_tokens[s]);
             }

@@ -124,6 +124,11 @@ void wvao_calculate(const wva_fleet *f, wvao_alloc *out);
 /* solves performed by the last wvao_calculate / wvao_grid call (instrumentation) */
 int64_t wvao_last_solves(void);
 int64_t wvao_last_states(void);
+/* Queue models refused since the previous call, and reset to 0: a model of N + N * max_queue_to_batch_ratio
+ * >= 2^31 states (computed in 64 bits, as Go's int) is outside the int32 domain of this oracle and of the CUDA
+ * library.  Its candidate, cell or sweep points are left nil / invalid; callers treat a non-zero count as
+ * "unsupported" (the library returns WVA_ERR_UNSUPPORTED for such a call). */
+int64_t wvao_take_unsupported(void);
 
 /* ---- pkg/solver --------------------------------------------------------- */
 /* SolveUnlimited: solver.go:63-79, deterministic tie-break = lowest acc id. */

@@ -133,13 +133,17 @@ struct HostFleet {
         if (rpm == 0.0f || srv_out_tokens[s] == 0) return PAIR_ZERO;
         return PAIR_LOAD;
     }
-    // batch size of a candidate: pkg/core/allocation.go:77-87
-    int pair_batch(int s, int a) const {
+    // batch size of a candidate: pkg/core/allocation.go:77-87, in Go's 64-bit int (the AtTokens rule can exceed int32)
+    long long pair_batch(int s, int a) const {
         if (srv_max_batch[s] > 0) return srv_max_batch[s];
         const size_t k = (size_t)srv_model[s] * A + a;
         const long long t = (long long)perf_max_batch[k] * (long long)perf_at_tokens[k] / srv_out_tokens[s];
-        return (int)std::max<long long>(t, 1);
+        return std::max<long long>(t, 1);
     }
+    // The queue model of batch size N (at most 2^20) has N + N * ratio states.  The reference counts them in Go's
+    // 64-bit int; the kernels, the fallback scratch and the int32 ABI count them in int32, so a model of 2^31
+    // states or more is refused instead of being built at a wrapped size.
+    bool queue_fits(long long N) const { return N * (1 + (long long)tun.max_queue_to_batch_ratio) < (1ll << 31); }
     // limited mode charges every allocation to its accelerator's type: each accelerator needs one
     bool every_acc_typed() const {
         for (int a = 0; a < A; ++a)
@@ -372,11 +376,13 @@ int ensure_ctrl(wva_handle* h) {
 constexpr int kFbBlocks = 2, kFbThreads = 64, kFbSlots = kFbBlocks * kFbThreads;
 constexpr int kFbCount[2] = {CTRL_FB_COUNT, CTRL_FB2_COUNT};
 
-// List `list` (0 or 1) of up to cap entries, and the scratch for chains of batch size up to Nmax.  Called before the
-// kernels that use them are enqueued: a DevBuf that grows frees its old memory, and cudaFree synchronises.
+// List `list` (0 or 1) of up to cap entries, and the scratch for chains of batch size up to Nmax: the largest batch
+// size of a model the call builds (0 when it builds none), which the caller has checked with queue_fits.  Called
+// before the kernels that use them are enqueued: a DevBuf that grows frees its old memory, and cudaFree synchronises.
 int prepare_fallback(wva_handle* h, int list, int cap, int Nmax, FbRun& r) {
     CK(h->d_fb_list[list].ensure(sizeof(unsigned long long) * std::max(cap, 1)));
-    const int Kmax = Nmax + Nmax * h->hf.tun.max_queue_to_batch_ratio;
+    if (!h->hf.queue_fits(Nmax)) return h->fail(WVA_ERR_UNSUPPORTED, "queue model of 2^31 states or more");
+    const int Kmax = (int)(Nmax * (1 + (long long)h->hf.tun.max_queue_to_batch_ratio));
     CK(h->d_scratch.ensure(sizeof(double) * ((size_t)Kmax + 1) * kFbSlots));
     int* ctrl = (int*)h->d_ctrl.p;
     r.list = FbList{ctrl + kFbCount[list], (unsigned long long*)h->d_fb_list[list].p, cap};
@@ -405,9 +411,12 @@ int sorted_pairs(wva_handle* h, Keep keep, std::vector<int>& pairs, std::vector<
     for (int s = 0; s < S; ++s)
         for (int a = 0; a < A; ++a)
             if (keep(s, a)) {
-                const int n = hf.pair_batch(s, a);
+                const long long n = hf.pair_batch(s, a);
                 if (n > (1 << 20)) return h->fail(WVA_ERR_UNSUPPORTED, "batch size above 2^20");
-                Ns[(size_t)s * A + a] = n;
+                if (!hf.queue_fits(n))
+                    return h->fail(WVA_ERR_UNSUPPORTED,
+                                   "queue model of 2^31 states or more (batch size x (1 + max_queue_to_batch_ratio))");
+                Ns[(size_t)s * A + a] = (int)n;
                 pairs.push_back(s * A + a);
             }
     std::stable_sort(pairs.begin(), pairs.end(), [&](int x, int y) { return Ns[x] > Ns[y]; });
@@ -596,7 +605,7 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
 int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, bool star = false) {
     const int n = g.n_cand;
     FbRun fb;
-    const int rc = prepare_fallback(h, 0, n, Nmax, fb);
+    const int rc = prepare_fallback(h, 0, n, n ? Nmax : 0, fb);
     if (rc) return rc;
     g.fb = fb.list;
     CK(cudaEventRecord(h->ev_k0, h->stream));
@@ -741,6 +750,9 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
             if (hf.pair_class(s, a, true) == PAIR_LOAD) tab_pair.push_back(s * hf.A + a);
     const int n_tab = (int)tab_pair.size();
     if ((long long)n_tab * Bmax > 0xffffffffll) return h->fail(WVA_ERR_UNSUPPORTED, "size-grid tables above 2^32 entries");
+    if (n_tab > 0 && B > 0 && !hf.queue_fits(Bmax))
+        return h->fail(WVA_ERR_UNSUPPORTED,
+                       "queue model of 2^31 states or more (batch size x (1 + max_queue_to_batch_ratio))");
     const int n = n_tab * B;  // <= S * A * B < 2^31 (checked by the caller)
     std::vector<int> order(n);  // candidate t * B + bi of table t
     std::iota(order.begin(), order.end(), 0);
@@ -825,7 +837,7 @@ int enqueue_load_star(wva_handle* h, long long fb2_cap, LoadStar& ls) {
     int rc = build_tables(h, pt);
     if (rc) return rc;
     // the tail's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
-    rc = prepare_fallback(h, 1, (int)std::min<long long>(fb2_cap, 1 << 22), pt.len_max, ls.fb2);
+    rc = prepare_fallback(h, 1, (int)std::min<long long>(fb2_cap, 1 << 22), pt.n ? pt.len_max : 0, ls.fb2);
     if (rc) return rc;
     ls.n = pt.n;
     SizeArgs& g = ls.g;
@@ -1069,6 +1081,11 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
         pt.epoch = h->epoch_tokens;
         pt.key = std::move(key);
     }
+    // every cell of a pair with a table builds the queue model of its batch size
+    const int Nmax = pt.n > 0 && B > 0 && R > 0 ? Bmax : 0;
+    if (!hf.queue_fits(Nmax))
+        return h->fail(WVA_ERR_UNSUPPORTED,
+                       "queue model of 2^31 states or more (batch size x (1 + max_queue_to_batch_ratio))");
     // [tables x batch] constants, then the [server x replica] rate block grid_rows fills (always allocated)
     CK(h->d_pb.ensure(sizeof(float4) * ((size_t)pt.n * std::max(B, 1) + (size_t)S * std::max(R, 1) + 1)));
     const char* d = (const char*)pt.lists.p;
@@ -1133,7 +1150,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     // size in 24; outside those limits every cell is evaluated (grid_order still walks the shared runs)
     g.prune = A <= 256 && Bmax < (1 << 24) && (long long)A * R <= kOrderMaxRows;
     g.Bmax = Bmax;
-    rc = prepare_fallback(h, 0, (int)std::min<size_t>(nc, (size_t)1 << 22), Bmax, plan->fb);
+    rc = prepare_fallback(h, 0, (int)std::min<size_t>(nc, (size_t)1 << 22), Nmax, plan->fb);
     if (rc) return rc;
     g.fb_count = plan->fb.list.count;
     g.fb_cells = plan->fb.list.item;
