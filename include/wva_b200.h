@@ -293,6 +293,37 @@ int wva_load_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const
                   wva_allocs *candidates, wva_allocs *winners);
 
 /*
+ * SLO grid: Server.Calculate (as in wva_analyze) and SolveUnlimited's winner at each of n_levels caller-given
+ * rows of service-class targets, e.g. candidate ITL / TTFT / TPS targets before they are chosen.
+ *
+ * Let f_l be the fleet with srv_slo_itl, srv_slo_ttft and srv_slo_tps replaced by row l of slo_itl, slo_ttft and
+ * slo_tps (each [n_levels * S], index l*S + s, in the units of the fleet's columns).  Candidate block l (records
+ * (l*S + s)*A + a) is byte for byte what wva_analyze returns for f_l, value = TransitionPenalty included.  Winner
+ * block l (records l*S + s) is wva_solve's winner block for f_l with unlimited = 1: strict '<' from MaxFloat32,
+ * ties to the lower accelerator id.  fleet->srv_slo_*, fleet->unlimited and the capacities are not read; every
+ * other column comes from `fleet`, and srv_has_target still gates (a server without a target is nil at every
+ * level).  Each candidate block is a valid input for wva_solve_greedy, which serves limited mode.
+ *
+ * Deduplication: each bisection of QueueAnalyzer.Size reads exactly one target (the TTFT search TargetTTFT, the
+ * ITL search TargetITL) and nothing else of the service class, so a search is determined by (server, accelerator,
+ * which search, target bits).  Each distinct (server, search, target) that some level needs runs once per
+ * (server, accelerator); a level needs it when its three targets are not negative and the target is > 0 (0, -0
+ * and NaN disable a search).  Only lambda*, rateStar, the replica count, the cost and two Analyze calls run per
+ * level: an 8 x 8 ITL x TTFT grid runs 16 searches per pair instead of 128.
+ *
+ * The fleet becomes resident, as with every call that takes one; there is no single solution afterwards, so
+ * wva_summarize returns WVA_ERR_STATE.  `candidates` (n_levels*S*A entries) may be NULL; `winners` has
+ * n_levels*S entries.  n_levels == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG: n_levels < 0, a row list
+ * NULL with n_levels * S > 0, or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_levels >= 2^31 (refused before the
+ * fleet is read); 2^31 or more search records (distinct keys x A); a load pair outside wva_analyze's queue-size
+ * rule (with n_levels > 0); or exactly the levels on which wva_analyze of f_l fails the same way (a rescale loop
+ * that would not terminate, which a NaN or tiny TPS target can cause, or too many stored-vector fallbacks).  A
+ * search that no level's reference would run (the ITL search after a failed TTFT search) does not fail the call.
+ */
+int wva_slo_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *slo_itl,
+                 const float *slo_ttft, const float *slo_tps, wva_allocs *candidates, wva_allocs *winners);
+
+/*
  * Load intervals: for each server, the exact float32 arrival rates in [rpm_lo[s], rpm_hi[s]] (req/min) at which
  * wva_load_grid's winner changes its decision, and the winner on each stretch in between.  An autoscaler can
  * skip a re-solve while the load stays inside the current interval, or publish the next scale-up and scale-down

@@ -203,6 +203,7 @@ struct wva_handle {
     PinBuf sz_pin;
     DevBuf d_lg_star;  // the load grid's rateStar records (shared with the load intervals)
     DevBuf d_iv;       // the load intervals' counts, flags, starts and work list
+    DevBuf d_slo;      // the SLO grid's search records
 
     // grid path
     DevBuf d_sort, d_best, d_pb, d_rows;
@@ -510,7 +511,10 @@ int size_depth_for(int n) {
     if (const char* e = getenv("WVA_SIZE_DEPTH")) d = atoi(e);
     return std::min(std::max(d, 1), kSzMaxDepth);
 }
-int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
+// What the size drivers compute per candidate: CreateAllocation, its rateStar mode (the load grid) or its search
+// mode (the SLO grid).
+enum SizeMode { SIZE_FULL, SIZE_STAR, SIZE_SEARCH };
+int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, SizeMode mode, const SearchCols& search) {
     const int D = size_depth_for(n);
     const size_t per_cand = 2 * ((size_t)(1 << D) - 1 + 2);  // two searches: a tree each, plus the two end points
     const size_t cap = per_cand * (size_t)n;                 // requests per round, worst case
@@ -567,11 +571,13 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
     g.ws.items_sorted = (unsigned long long*)(wp + w_sorted); g.ws.item_count = (unsigned*)(wp + w_cnt);
     g.cand = sa.cand;
     g.fb = sa.fb;
+    g.search = search;
 
     const unsigned nb = (unsigned)((n + 255) / 256);
     const unsigned cks = (unsigned)chunks, items_blocks = (unsigned)((max_items + 255) / 256),
                    solve_blocks = (unsigned)((max_items * 32 + 255) / 256);
-    sz2_init<<<nb, 256, 0, h->stream>>>(g);
+    if (mode == SIZE_SEARCH) sz2_init_search<<<nb, 256, 0, h->stream>>>(g);
+    else sz2_init<<<nb, 256, 0, h->stream>>>(g);
     h->launches++;
     unsigned* pin = (unsigned*)h->sz_pin.p;
     // Rounds are enqueued in groups without looking at the device: every kernel of a round leaves at once when the
@@ -582,7 +588,8 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
     for (int round = 0; round < max_rounds; round += group) {
         for (int r = 0; r < group; ++r) {
             sz2_round_reset<<<3, 256, 0, h->stream>>>(g);
-            if (star) sz2_advance_star<<<nb, 256, 0, h->stream>>>(g);
+            if (mode == SIZE_STAR) sz2_advance_star<<<nb, 256, 0, h->stream>>>(g);
+            else if (mode == SIZE_SEARCH) sz2_advance_search<<<nb, 256, 0, h->stream>>>(g);
             else sz2_advance<<<nb, 256, 0, h->stream>>>(g);
             sz2_sort_local<<<cks, kSortThreads, 0, h->stream>>>(g);
             ws_items_scan<<<1, 256, 0, h->stream>>>(g.ws);
@@ -599,10 +606,10 @@ int run_size_rounds(wva_handle* h, const SizeArgs& sa, int n, bool star) {
     return WVA_OK;
 }
 
-// CreateAllocation for the load candidates g lists (g.cand_pair .. g.place set, batch sizes at most Nmax), or up to
-// rateStar when star is set (create_allocation's rateStar mode): the warp-per-candidate kernel or the rounds, timed
-// as the call's kernel, then the stored-vector fallback.
-int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, bool star = false) {
+// CreateAllocation for the load candidates g lists (g.cand_pair .. g.place set, batch sizes at most Nmax), up to
+// rateStar in SIZE_STAR mode, or one search each in SIZE_SEARCH mode (with `search`): the warp-per-candidate kernel
+// or the rounds, timed as the call's kernel, then the stored-vector fallback.
+int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, SizeMode mode = SIZE_FULL, const SearchCols& search = {}) {
     const int n = g.n_cand;
     FbRun fb;
     const int rc = prepare_fallback(h, 0, n, n ? Nmax : 0, fb);
@@ -612,15 +619,18 @@ int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, bool star = false) 
     int small_max = 1024;  // up to here a warp per candidate beats rounds (the GPU is mostly empty either way)
     if (const char* e = getenv("WVA_SIZE_SMALL_MAX")) small_max = atoi(e);
     if (n > 0 && n <= small_max) {
-        if (star) size_warp_star<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
-        else size_warp_kernel<<<(unsigned)((n + 3) / 4), 128, 0, h->stream>>>(g);
+        const unsigned blocks = (unsigned)((n + 3) / 4);
+        if (mode == SIZE_STAR) size_warp_star<<<blocks, 128, 0, h->stream>>>(g);
+        else if (mode == SIZE_SEARCH) size_warp_search<<<blocks, 128, 0, h->stream>>>(SearchArgs{g, search});
+        else size_warp_kernel<<<blocks, 128, 0, h->stream>>>(g);
         h->launches++;
     } else if (n > 0) {
-        const int rc = run_size_rounds(h, g, n, star);
+        const int rc = run_size_rounds(h, g, n, mode, search);
         if (rc) return rc;
     }
     CK(cudaEventRecord(h->ev_k1, h->stream));
-    if (n > 0) launch_fallback(h, star ? size_fallback_star : size_fallback, g, fb);
+    if (n > 0 && mode == SIZE_SEARCH) launch_fallback(h, size_fallback_search, SearchArgs{g, search}, fb);
+    else if (n > 0) launch_fallback(h, mode == SIZE_STAR ? size_fallback_star : size_fallback, g, fb);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -851,7 +861,7 @@ int enqueue_load_star(wva_handle* h, long long fb2_cap, LoadStar& ls) {
     g.ls = (const float*)pt.ls.p;
     g.place = CandPlace{nullptr, nullptr};
     g.cand = ls.star;
-    return enqueue_candidates(h, g, pt.len_max, true);
+    return enqueue_candidates(h, g, pt.len_max, SIZE_STAR);
 }
 // The tail's view of phase 1: candidates, tables and rateStar records (the level list is the caller's).
 LoadArgs load_args(wva_handle* h, const LoadStar& ls) {
@@ -989,6 +999,175 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     h->launches += 2;
     CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1 and the interval kernels
     launch_fallback(h, interval_fallback, g, ls.fb2);
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- SLO grid: CreateAllocation and the unlimited winner at every listed (ITL, TTFT, TPS) target row -----------
+// A bisection reads only its own target (DESIGN.md §3.11), so phase 1 runs each distinct (server, search, target
+// bits) key once per load pair of the server, in search mode; phase 2 (slo_kernel, slo_fallback) is the tail per
+// (load pair, level).  A key exists where some level needs it: the level's three targets are not negative
+// (TargetPerf.check makes the pair nil before any search), the target is > 0 (0, -0 and NaN disable a search) and
+// the server has load pairs.  Lists, tables (lg_tabs, shared with the load grid and the load intervals) and the
+// search records (d_slo) are rebuilt on every call.  itl / ttft / tps [L*S] are the caller's rows; cand ([L*S*A])
+// and winners ([L*S]) are device columns.
+int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, const float* tps,
+                     const AllocCols& cand, const AllocCols& winners) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A;
+    const size_t LS = (size_t)L * S;
+    // the tail's candidates: every load pair (none without levels), descending N, one N-entry table each
+    std::vector<int> pairs, Ns;
+    if (L > 0) {
+        const int rc = sorted_pairs(h, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
+        if (rc) return rc;
+    }
+    std::vector<int> tab_of((size_t)S * A, -1);  // the pair's table index
+    std::vector<long long> tab_entry(pairs.size());
+    long long entries = 0;
+    for (size_t t = 0; t < pairs.size(); ++t) {
+        tab_of[pairs[t]] = (int)t;
+        tab_entry[t] = entries;
+        entries += Ns[t];
+    }
+    std::vector<int> n_load(S, 0);
+    for (int p : pairs) n_load[p / A]++;
+    // the search keys: per server, its distinct (search, target bits) in that order, so a server's keys are
+    // key_begin[s] .. key_begin[s + 1] - 1
+    std::vector<int> key(2 * LS, -1), key_begin(S + 1, 0);
+    std::vector<uint8_t> key_w;
+    std::vector<float> key_t;
+    std::vector<std::pair<uint64_t, size_t>> uses;  // (search << 32 | target bits, index into key)
+    for (int s = 0; s < S; ++s) {
+        key_begin[s] = (int)key_w.size();
+        if (!n_load[s]) continue;
+        uses.clear();
+        for (int l = 0; l < L; ++l) {
+            const size_t i = (size_t)l * S + s;
+            if (itl[i] < 0.0f || ttft[i] < 0.0f || tps[i] < 0.0f) continue;
+            for (int w = 0; w < 2; ++w) {
+                const float t = w == 0 ? ttft[i] : itl[i];
+                if (!(t > 0.0f)) continue;
+                uint32_t bits;
+                memcpy(&bits, &t, 4);
+                uses.emplace_back((uint64_t)w << 32 | bits, 2 * i + w);
+            }
+        }
+        std::sort(uses.begin(), uses.end());
+        for (size_t u = 0; u < uses.size(); ++u) {
+            if (u == 0 || uses[u].first != uses[u - 1].first) {
+                const uint32_t bits = (uint32_t)uses[u].first;
+                float t;
+                memcpy(&t, &bits, 4);
+                key_w.push_back((uint8_t)(uses[u].first >> 32));
+                key_t.push_back(t);
+            }
+            key[uses[u].second] = (int)key_w.size() - 1;
+        }
+        // at most 2 * L * S keys in all; the search candidates are fewer than the records
+        if ((long long)key_w.size() * A >= (1ll << 31))
+            return h->fail(WVA_ERR_UNSUPPORTED, "SLO grid with 2^31 or more search records in one call");
+    }
+    key_begin[S] = (int)key_w.size();
+    const int n_keys = (int)key_w.size();
+    // search candidates (key, pair): the load pairs in their order (descending N), each with its server's keys
+    std::vector<std::pair<int, int>> sc;
+    for (int p : pairs)
+        for (int k = key_begin[p / A]; k < key_begin[p / A + 1]; ++k) sc.emplace_back(k, p);
+    const long long n = (long long)sc.size();
+    Cols c(16);
+    const size_t o_itl = c.take(4 * LS), o_ttft = c.take(4 * LS), o_tps = c.take(4 * LS), o_key = c.take(8 * LS);
+    const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_rec = c.take(4 * (size_t)n),
+                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_tgt = c.take(4 * (size_t)n),
+                 o_which = c.take((size_t)n);
+    int rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
+        if (LS) {
+            memcpy(p + o_itl, itl, 4 * LS);
+            memcpy(p + o_ttft, ttft, 4 * LS);
+            memcpy(p + o_tps, tps, 4 * LS);
+            memcpy(p + o_key, key.data(), 8 * LS);
+        }
+        for (size_t j = 0; j < sc.size(); ++j) {
+            const int k = sc[j].first, pair = sc[j].second, a = pair % A, t = tab_of[pair];
+            ((int*)(p + o_pair))[j] = pair;
+            ((int*)(p + o_N))[j] = Ns[t];
+            ((int*)(p + o_rec))[j] = k * A + a;
+            ((int*)(p + o_idx))[j] = t;
+            ((long long*)(p + o_off))[j] = tab_entry[t];
+            ((float*)(p + o_tgt))[j] = key_t[k];
+            ((uint8_t*)(p + o_which))[j] = key_w[k];
+        }
+    });
+    if (rc) return rc;
+    const PairTables& pt = h->lg_tabs;
+    const char* d = (const char*)pt.lists.p;
+    rc = build_tables(h, pt);
+    if (rc) return rc;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const long long n_items = (long long)pt.n * L;
+    // the tail's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
+    FbRun fb2;
+    rc = prepare_fallback(h, 1, (int)std::min<long long>(n_items, 1 << 22), pt.n ? pt.len_max : 0, fb2);
+    if (rc) return rc;
+    const size_t n_srec = (size_t)n_keys * A;
+    CK(h->d_slo.ensure(5 * n_srec + 16));
+    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
+    if (n_rec > 0) {
+        trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(h->df, cand, L);
+        h->launches++;
+    }
+    // phase 1: the searches
+    AllocCols srch{};
+    srch.max_rate = (float*)h->d_slo.p;
+    srch.feasible = (uint8_t*)h->d_slo.p + 4 * n_srec;
+    SizeArgs g{};
+    g.f = h->df;
+    g.cand_pair = (const int*)(d + o_pair);
+    g.cand_N = (const int*)(d + o_N);
+    g.n_cand = (int)n;
+    g.tab = (const double*)pt.tab.p;
+    g.tab_off = (const long long*)(d + o_off);
+    g.ls = (const float*)pt.ls.p;
+    g.place = CandPlace{(const int*)(d + o_idx), (const int*)(d + o_rec)};
+    g.cand = srch;
+    rc = enqueue_candidates(h, g, pt.len_max, SIZE_SEARCH,
+                            SearchCols{(const uint8_t*)(d + o_which), (const float*)(d + o_tgt)});
+    if (rc) return rc;
+    // phase 2: the tail per (load pair, level)
+    if (n_items > 0) {
+        SloArgs la{};
+        la.f = h->df;
+        la.cand_pair = pt.pair();
+        la.cand_N = pt.len();
+        la.tab_off = pt.off();
+        la.tab = (const double*)pt.tab.p;
+        la.slo_itl = (const float*)(d + o_itl);
+        la.slo_ttft = (const float*)(d + o_ttft);
+        la.slo_tps = (const float*)(d + o_tps);
+        la.key = (const int*)(d + o_key);
+        la.srch = srch;
+        la.n_cand = pt.n;
+        la.L = L;
+        la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+        la.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
+        la.cand = cand;
+        la.fb = fb2.list;
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, slo_kernel, 256, 0));
+        per_sm = std::max(1, std::min(per_sm, 8));
+        const long long warps = (n_items + 31) / 32;
+        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
+        slo_kernel<<<blocks, 256, 0, h->stream>>>(la);
+        h->launches++;
+        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
+        launch_fallback(h, slo_fallback, la, fb2);
+    }
+    if (S > 0 && L > 0) {
+        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
+            h->df, cand, winners, L);
+        h->launches++;
+    }
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1850,6 +2029,30 @@ int wva_load_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const
     c.win_blocks = (size_t)n_levels;
     rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
         return enqueue_load_grid(h, n_levels, arrival_rpm, dc, dw);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
+int wva_slo_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* slo_itl,
+                 const float* slo_ttft, const float* slo_tps, wva_allocs* candidates, wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * n_levels > 0 && (!slo_itl || !slo_ttft || !slo_tps))
+        return h->fail(WVA_ERR_BAD_ARG, "NULL target row list");
+    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "SLO grid too large for one call (>= 2^31 candidates)");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
+    c.win_blocks = (size_t)n_levels;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_slo_grid(h, n_levels, slo_itl, slo_ttft, slo_tps, dc, dw);
     });
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;

@@ -5,7 +5,7 @@
 //                       sort, persistent warps pulling 32-cell items, fused feasibility + batch-rank minimum
 //   grid_fallback       stored-vector re-run of the rare cells the streaming solve bails on
 //   grid_finalize  K3   per-server argmin over partials (warp shuffle -> smem -> record)
-//   trivial_kernel      nil / zero-load candidates (overload: per load level of wva_load_grid)
+//   trivial_kernel      nil / zero-load candidates (overloads: per level of wva_load_grid and wva_slo_grid)
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
 //   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
@@ -1578,6 +1578,18 @@ __global__ void trivial_kernel(DevFleet f, AllocCols cand, const float* level_rp
     const int l = i / n_pairs, pair = i - l * n_pairs;
     const int s = pair / f.A, a = pair % f.A;
     const int cls = pair_class(at_level(f, level_rpm, l), s, a, true);
+    if (cls == PAIR_LOAD) return;
+    store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
+}
+// ... of the SLO grid: L level blocks of S * A records (record l * S * A + pair); a pair's class and its nil or
+// zero-load record read no target, so every block gets the same (S * A * L < 2^31, checked on the host).
+__global__ void trivial_kernel(DevFleet f, AllocCols cand, int L) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n_pairs = f.S * f.A;
+    if (i >= n_pairs * L) return;
+    const int pair = i % n_pairs;
+    const int s = pair / f.A, a = pair % f.A;
+    const int cls = pair_class(f, s, a, true);
     if (cls == PAIR_LOAD) return;
     store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
 }

@@ -46,6 +46,12 @@ struct CandPlace {
     }
 };
 
+// Search mode's candidate columns (the SLO grid): the one search a candidate runs, and its target.
+struct SearchCols {
+    const uint8_t* which;  // [n_cand] 0: TTFT, 1: ITL
+    const float* target;   // [n_cand] the target, > 0
+};
+
 struct SizeArgs {
     DevFleet f;
     const int* cand_pair;      // [n_cand] pair ids sorted by descending N
@@ -57,6 +63,11 @@ struct SizeArgs {
     CandPlace place;
     AllocCols cand;
     FbList fb;                 // candidate indices that bailed
+};
+// ... with search mode's columns (size_warp_search, size_fallback_search)
+struct SearchArgs {
+    SizeArgs g;
+    SearchCols search;
 };
 
 // The rounds' sort workspace and its item ordering kernels.
@@ -122,6 +133,7 @@ struct Sz2Args {
     SortWs ws;
     AllocCols cand;
     FbList fb;
+    SearchCols search;     // search mode only
 };
 
 // ---------------------------------------------------------------------------
@@ -280,11 +292,32 @@ __device__ __forceinline__ Cand star_cand(float rate_star) {
     return c;
 }
 
+// Search mode's record of one search, in the feasible and max_rate columns: SEARCH_NIL (K < 2, lambda_min >
+// lambda_max, or "target is below the bounded region"), SEARCH_OK with max_rate = lambdaStar (req/ms), or
+// SEARCH_FAIL: a solve's rescale loop does not terminate (the stored-vector re-run failed).  The search fallback
+// does not raise the call's status for SEARCH_FAIL: only a caller whose reference would have run the search does.
+enum { SEARCH_NIL = 0, SEARCH_OK = 1, SEARCH_FAIL = 2 };
+__device__ __forceinline__ Cand search_cand(int status, float xs) {
+    Cand c = cand_nil();
+    c.feasible = (uint8_t)status;
+    c.max_rate = xs;
+    return c;
+}
+// The search's target: search mode's column, else the server's own (which = 0: TTFT, 1: ITL).
+template <bool kSearch>
+__device__ __forceinline__ float search_target(const DevFleet& f, const SearchCols& sc, int j, int s, int which) {
+    if constexpr (kSearch) return which == sc.which[j] ? sc.target[j] : 0.0f;
+    return which == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+}
+
 // ---------------------------------------------------------------------------
 // The rounds (more than WVA_SIZE_SMALL_MAX candidates): one thread per candidate keeps the search state in global
 // columns between rounds; both searches of a candidate emit their trees in the same round.
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
+// kSearch: search mode (the SLO grid), where a candidate runs only its one search and is nil only for K < 2 or an
+// empty range.
+template <bool kSearch>
+__device__ __forceinline__ void sz2_init_body(const Sz2Args& g) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= g.n_cand) return;
     const DevFleet& f = g.f;
@@ -292,14 +325,15 @@ __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
     const int N = g.cand_N[j], K = N + N * f.ratio;
     const double* tab = g.tab + 4 * g.tab_off[j];
     const float s1 = (float)tab[0], sN = (float)tab[4 * (N - 1)];
-    const SzStart b = sz_start(f, s, K, s1, sN);
+    SzStart b = sz_start(f, s, K, s1, sN);
+    if constexpr (kSearch) b.nil = K < 2 || b.lmin > b.lmax;
     g.rmax[j] = b.rmax;
     g.l2s0[j] = log2f(s1);
     g.l2sN[j] = log2f(sN);
     g.lsN[j] = g.place.ls_of(g.ls, g.tab_off, j)[N - 1];
     g.phase[j] = b.nil ? PH_NIL : PH_SEARCH;
     for (int w = 0; w < 2; ++w) {
-        const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+        const float target = search_target<kSearch>(f, g.search, j, s, w);
         g.xmin[2 * j + w] = b.lmin;
         g.xmax[2 * j + w] = b.lmax;
         g.xs[2 * j + w] = b.lmax;  // lambdaStar when the target is disabled (queueanalyzer.go:205,218)
@@ -312,10 +346,13 @@ __global__ void __launch_bounds__(256) sz2_init(Sz2Args g) {
     g.aslot[j] = -1;
     if (b.nil) store_cand(g.cand, g.place.record(j, pair), cand_nil());
 }
+__global__ void __launch_bounds__(256) sz2_init(Sz2Args g) { sz2_init_body<false>(g); }
+__global__ void __launch_bounds__(256) sz2_init_search(Sz2Args g) { sz2_init_body<true>(g); }
 
 // Advance every candidate: consume last round's results (walking the midpoint trees with the reference's
-// comparisons), then emit this round's requests into consecutive slots.  kStar: rateStar mode (create_allocation).
-template <bool kStar>
+// comparisons), then emit this round's requests into consecutive slots.  kStar: rateStar mode, kSearch: search
+// mode (create_allocation).
+template <bool kStar, bool kSearch = false>
 __device__ __forceinline__ void sz2_advance_body(const Sz2Args& g) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     const DevFleet& f = g.f;
@@ -345,7 +382,7 @@ __device__ __forceinline__ void sz2_advance_body(const Sz2Args& g) {
                 const int k = 2 * j + w;
                 int st = g.sst[k];
                 if (st == SZ2_DONE || st == SZ2_OFF) continue;
-                const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+                const float target = search_target<kSearch>(f, g.search, j, s, w);
                 float lo = g.xmin[k], hi = g.xmax[k];
                 if (st == SZ2_START) {
                     emit_ends[w] = true;
@@ -378,7 +415,10 @@ __device__ __forceinline__ void sz2_advance_body(const Sz2Args& g) {
             }
             if (bail) ph = PH_BAIL;
             else if (nil) ph = PH_NIL;
-            else if (all_done) {
+            else if (kSearch && all_done) {
+                store_cand(g.cand, g.place.record(j, pair), search_cand(SEARCH_OK, g.xs[2 * j + g.search.which[j]]));
+                ph = PH_DONE;
+            } else if (all_done) {
                 if (!sz_lambda(f, s, rmax, g.xs[2 * j], g.xs[2 * j + 1], an_lambda)) ph = PH_NIL;
                 else { an_kind = 2; ph = PH_WAIT_STAR; }
             }
@@ -461,6 +501,7 @@ __device__ __forceinline__ void sz2_advance_body(const Sz2Args& g) {
 }
 __global__ void __launch_bounds__(256) sz2_advance(Sz2Args g) { sz2_advance_body<false>(g); }
 __global__ void __launch_bounds__(256) sz2_advance_star(Sz2Args g) { sz2_advance_body<true>(g); }
+__global__ void __launch_bounds__(256) sz2_advance_search(Sz2Args g) { sz2_advance_body<false, true>(g); }
 
 // Local counting sort of this round's requests by length class (keys precomputed by sz2_advance); stable inside a
 // warp's 32 requests, so the requests of one candidate (consecutive slots) stay adjacent within their class.
@@ -571,11 +612,29 @@ __global__ void sz2_round_reset(Sz2Args g) {
 // kStar: rateStar mode (the load grid) stops where the tail that reads the load starts (allocation.go:134), with
 // out = nil or star_cand(rateStar).  Everything before that point (N from the tokens and srv_max_batch, the
 // bisections, lambda*, rateStar = Analyze(lambda*).Throughput) does not read the load.
+//
+// kSearch: search mode (the SLO grid) runs only the search `which` at `target` and stops where it ends, with
+// out = search_cand(SEARCH_NIL or SEARCH_OK, lambdaStar).  A search reads no other target: its bounds come from
+// RateRange and its function is EvalTTFT or EvalITL (queueanalyzer.go:204-228, utils.go:26-70).
 // ---------------------------------------------------------------------------
-template <bool kStar, class Eval>
+template <bool kStar, bool kSearch = false, class Eval>
 __device__ __forceinline__ bool create_allocation(const DevFleet& f, int s, int a, int N, int K, float s1, float sN,
-                                                  Eval& ev, Cand& out) {
+                                                  Eval& ev, Cand& out, int which = 0, float target = 0.0f) {
     out = cand_nil();
+    if constexpr (kSearch) {
+        SzStart b = sz_start(f, s, K, s1, sN);
+        if (K < 2 || b.lmin > b.lmax) return true;
+        SzSearch S{b.lmin, b.lmax, 0.0f, 0, 0, false};
+        ev.round(which, S.lo, S.hi, true);
+        int r = sz_ends(S, target, [&](int i) { return ev.end(i); });
+        while (r == SZ_MORE) {
+            r = sz_walk(S, target, ev.depth(), [&](int v) { return ev.node(v); });
+            if (r == SZ_MORE) ev.round(which, S.lo, S.hi, false);
+        }
+        if (r == SZ_BAIL) return false;
+        if (S.ind >= 0) out = search_cand(SEARCH_OK, S.xs);
+        return true;
+    }
     const SzStart b = sz_start(f, s, K, s1, sN);
     if (b.nil) return true;
     float xs_ttft = b.lmax, xs_itl = b.lmax;  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
@@ -648,8 +707,8 @@ struct WarpEval {
     }
 };
 
-template <bool kStar>
-__device__ __forceinline__ void size_warp(const SizeArgs& g) {
+template <bool kStar, bool kSearch = false>
+__device__ __forceinline__ void size_warp(const SizeArgs& g, const SearchCols& sc = SearchCols{}) {
     const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
     if (j >= g.n_cand) return;
@@ -663,7 +722,12 @@ __device__ __forceinline__ void size_warp(const SizeArgs& g) {
     ev.K = K;
     ev.lane = lane;
     Cand c;
-    const bool ok = create_allocation<kStar>(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
+    bool ok;
+    if constexpr (kSearch)
+        ok = create_allocation<kStar, true>(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c,
+                                            sc.which[j], sc.target[j]);
+    else
+        ok = create_allocation<kStar>(f, s, a, N, K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
     if (lane == 0) {
         if (!ok) fb_push(g.fb, (unsigned)j);
         store_cand(g.cand, g.place.record(j, pair), c);
@@ -671,6 +735,7 @@ __device__ __forceinline__ void size_warp(const SizeArgs& g) {
 }
 __global__ void __launch_bounds__(128) size_warp_kernel(SizeArgs g) { size_warp<false>(g); }
 __global__ void __launch_bounds__(128) size_warp_star(SizeArgs g) { size_warp<true>(g); }
+__global__ void __launch_bounds__(128) size_warp_search(SearchArgs a) { size_warp<false, true>(a.g, a.search); }
 
 // ---------------------------------------------------------------------------
 // Stored-vector re-run of the candidates that bailed: one thread per candidate evaluates exactly the reference's
@@ -726,6 +791,30 @@ __device__ __forceinline__ void size_fallback_body(const SizeArgs& g, const FbRu
 }
 __global__ void size_fallback(SizeArgs g, FbRun r) { size_fallback_body<false>(g, r); }
 __global__ void size_fallback_star(SizeArgs g, FbRun r) { size_fallback_body<true>(g, r); }
+// ... in search mode, where a search whose re-run fails is stored SEARCH_FAIL and the call's status is left to the
+// SLO grid's tail.
+__global__ void size_fallback_search(SearchArgs sa, FbRun r) {
+    const SizeArgs& g = sa.g;
+    const DevFleet& f = g.f;
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        const int j = (int)item;
+        const int pair = g.cand_pair[j];
+        const int s = pair / f.A, a = pair % f.A;
+        const int N = g.cand_N[j];
+        StoredEval ev;
+        ev.p = p;
+        ev.tab = g.tab + 4 * g.tab_off[j];
+        ev.q = qparams_of(f, s, a);
+        ev.N = N;
+        ev.K = N + N * f.ratio;
+        Cand c;
+        if (!create_allocation<false, true>(f, s, a, N, ev.K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c,
+                                            sa.search.which[j], sa.search.target[j]))
+            c = search_cand(SEARCH_FAIL, 0.0f);
+        store_cand(g.cand, g.place.record(j, pair), c);
+        return 0;
+    });
+}
 
 // ---------------------------------------------------------------------------
 // The load grid's tail (allocation.go:134-163) at every level of a caller-given load list: one lane per (candidate,
@@ -823,6 +912,124 @@ __global__ void load_fallback(LoadArgs g, FbRun r) {
             }, c))
             return rc;
         store_cand(g.cand, load_record(g, e, l), c);
+        return 0;
+    });
+}
+
+// ---------------------------------------------------------------------------
+// The SLO grid's tail (DESIGN.md §3.11): CreateAllocation of every load pair at every level of a caller-given list
+// of (ITL, TTFT, TPS) target rows, from the search records of search mode above.  A search reads only its own
+// target, so phase 1 ran each distinct (server, search, target) once per load pair; this kernel combines a level's
+// two records and runs the rest: lambda* (min with the TPS rule), rateStar = Analyze(lambda*).Throughput, the
+// replicas at the level's totalRate and the final Analyze.  One lane per (candidate, level) item, candidate-major
+// (item e * L + l), warps from a work counter, as in load_kernel.  Record (l * S + s) * A + a.
+//
+// The reference runs the ITL search only after the TTFT search succeeded, and phase 1 runs every key regardless.
+// So a SEARCH_FAIL record fails the call only where the level's reference would have consulted it: a TTFT search
+// always, an ITL search when the TTFT search is disabled or succeeded.
+// ---------------------------------------------------------------------------
+struct SloArgs {
+    DevFleet f;
+    const int* cand_pair;       // [n_cand] load pairs sorted by descending N
+    const int* cand_N;          // [n_cand]
+    const long long* tab_off;   // [n_cand] entry offset of the candidate's table (N entries)
+    const double* tab;
+    const float* slo_itl;       // [L * S] the targets of server s at level l
+    const float* slo_ttft;
+    const float* slo_tps;
+    const int* key;             // [2 * L * S] the search key of (level, server, search) (l * S + s) * 2 + which
+    AllocCols srch;             // [n_keys * A] search records by key * A + a (search_cand)
+    int n_cand, L;
+    unsigned* counter;
+    int* status;                // set where a consulted search did not terminate
+    AllocCols cand;             // [L * S * A]
+    FbList fb;                  // items that bailed: fb_pack(candidate, level)
+};
+
+// The fleet as the SLO grid sees it at level l: the targets are row l of the level lists.
+__device__ __forceinline__ DevFleet at_slo_level(const SloArgs& g, int l) {
+    DevFleet fl = g.f;
+    fl.srv_slo_itl = g.slo_itl + (size_t)l * g.f.S;
+    fl.srv_slo_ttft = g.slo_ttft + (size_t)l * g.f.S;
+    fl.srv_slo_tps = g.slo_tps + (size_t)l * g.f.S;
+    return fl;
+}
+
+// Candidate e's record at level l; solve(lambda, st) is Model.Solve for the two Analyze calls.  Returns false when
+// a solve bailed (out is then nil).
+template <class Solve>
+__device__ __forceinline__ bool slo_tail(const SloArgs& g, int e, int l, Solve&& solve, Cand& out) {
+    const DevFleet f = at_slo_level(g, l);
+    const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A;
+    const int N = g.cand_N[e], K = N + N * f.ratio;
+    const double* tab = g.tab + 4 * g.tab_off[e];
+    out = cand_nil();
+    const SzStart b = sz_start(f, s, K, (float)tab[0], (float)tab[4 * (N - 1)]);
+    if (b.nil) return true;
+    float xs[2] = {b.lmax, b.lmax};  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
+    for (int w = 0; w < 2; ++w) {
+        const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+        if (!(target > 0.0f)) continue;
+        const size_t k = (size_t)g.key[((size_t)l * f.S + s) * 2 + w] * f.A + a;
+        const int st = g.srch.feasible[k];
+        if (st == SEARCH_FAIL) {
+            atomicExch(g.status, 1);
+            return true;
+        }
+        if (st == SEARCH_NIL) return true;
+        xs[w] = g.srch.max_rate[k];
+    }
+    float lam;
+    ModelStats st;
+    if (!sz_lambda(f, s, b.rmax, xs[0], xs[1], lam)) return true;
+    if (!solve(tab, N, K, lam, st)) return false;
+    const QParams q = qparams_of(f, s, a);
+    const float rate_star = metrics_from(q, N, st).throughput;
+    SzReplicas r;
+    if (!sz_replicas(f, s, a, b.rmax, rate_star, total_rate_of(f, s), r, lam)) return true;
+    if (!solve(tab, N, K, lam, st)) return false;
+    const Metrics m = metrics_from(q, N, st);
+    out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
+    return true;
+}
+
+__device__ __forceinline__ size_t slo_record(const SloArgs& g, int e, int l) {
+    return (size_t)l * g.f.S * g.f.A + g.cand_pair[e];
+}
+
+__global__ void __launch_bounds__(256) slo_kernel(SloArgs g) {
+    const int lane = threadIdx.x & 31;
+    const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
+    for (;;) {
+        unsigned w = 0;
+        if (lane == 0) w = atomicAdd(g.counter, 1u);
+        w = __shfl_sync(0xffffffffu, w, 0);
+        if ((unsigned long long)w * 32 >= n_items) break;
+        const unsigned i = w * 32 + lane;
+        if (i < n_items) {
+            const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
+            Cand c;
+            const bool ok = slo_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+                return solve_shared(tab, N, K, lam, st) == kSolveOk;
+            }, c);
+            if (!ok) fb_push(g.fb, fb_pack(e, l));
+            store_cand(g.cand, slo_record(g, e, l), c);
+        }
+    }
+}
+
+// Stored-vector re-run of the items slo_kernel bailed on.
+__global__ void slo_fallback(SloArgs g, FbRun r) {
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        const int e = (int)(item >> 32), l = (int)(unsigned)item;
+        int rc = 0;
+        Cand c;
+        if (!slo_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+                rc = solve_stored(p, tab, N, K, lam, st);
+                return rc == 0;
+            }, c))
+            return rc;
+        store_cand(g.cand, slo_record(g, e, l), c);
         return 0;
     });
 }

@@ -151,6 +151,36 @@ class Engine:
                                           C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
+    def slo_grid(self, fleet: Fleet, slo_itl, slo_ttft, slo_tps, want_candidates: bool = False,
+                 out: Allocs | None = None):
+        """The reference's ``Server.Calculate`` and ``SolveUnlimited`` winner at each row of service-class targets
+        (``slo_itl``, ``slo_ttft``, ``slo_tps``, each of shape (L, S), in the fleet columns' units) ->
+        (candidates [L*S*A] | None, winners [L*S]), both level-major.
+
+        Candidate block ``l`` is what ``analyze`` returns for the fleet with ``srv_slo_itl``, ``srv_slo_ttft`` and
+        ``srv_slo_tps`` = row ``l``, and winner block ``l`` is ``solve``'s winners for it in unlimited mode; each
+        distinct target of a server is searched once (see ``wva_slo_grid`` in include/wva_b200.h).  The fleet's own
+        ``srv_slo_*`` are not read.  ``out``: an ``Allocs`` of ``L * S`` records to write the winners into."""
+        rows = []
+        for name, x in (("slo_itl", slo_itl), ("slo_ttft", slo_ttft), ("slo_tps", slo_tps)):
+            r = np.ascontiguousarray(x, np.float32)
+            if r.ndim != 2 or r.shape[1] != fleet.n_servers:
+                raise ValueError(f"{name} must have shape (L, {fleet.n_servers}), got {r.shape}")
+            rows.append(r)
+        L = rows[0].shape[0]
+        if any(r.shape[0] != L for r in rows):
+            raise ValueError(f"slo_itl, slo_ttft and slo_tps must have one row count, got {[r.shape for r in rows]}")
+        if out is not None and out.n != L * fleet.n_servers:
+            raise ValueError("out must hold L * fleet.n_servers records")
+        win = out if out is not None else Allocs(L * fleet.n_servers)
+        cand = Allocs(L * fleet.n_servers * fleet.n_acc) if want_candidates else None
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_slo_grid(self._h, C.byref(fc), L, *[_abi.ptr(r.reshape(-1)) for r in rows],
+                                         C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
+
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
         """Where each server's ``load_grid`` winner changes its decision in ``[rpm_lo[s], rpm_hi[s]]`` (req/min)
         -> (count [S], truncated [S], start_rpm (S, M), records: ``Allocs`` of S * M).
