@@ -324,6 +324,40 @@ int wva_slo_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const 
                  const float *slo_ttft, const float *slo_tps, wva_allocs *candidates, wva_allocs *winners);
 
 /*
+ * Workload grid: Server.Calculate (as in wva_analyze) and SolveUnlimited's winner at each of n_levels caller-given
+ * rows of (arrival rate, average input tokens, average output tokens), e.g. a forecast in which prompts or answers
+ * grow, or a daily mix of chat and batch traffic.
+ *
+ * Let f_l be the fleet with srv_arrival_rpm, srv_in_tokens and srv_out_tokens replaced by row l of arrival_rpm
+ * (req/min), in_tokens and out_tokens (each [n_levels * S], index l*S + s).  Candidate block l (records
+ * (l*S + s)*A + a) is byte for byte what wva_analyze returns for f_l, value = TransitionPenalty included.  Winner
+ * block l (records l*S + s) is wva_solve's winner block for f_l with unlimited = 1: strict '<' from MaxFloat32,
+ * ties to the lower accelerator id.  Per level a pair is nil at a negative rate or negative tokens,
+ * zeroLoadAllocation at rate 0 or out_tokens 0, and sized under load otherwise, NaN and +Inf rates included.
+ * fleet->srv_arrival_rpm, srv_in_tokens, srv_out_tokens, fleet->unlimited and the capacities are not read; every
+ * other column comes from `fleet`.  Each candidate block is a valid input for wva_solve_greedy, which serves
+ * limited mode.
+ *
+ * Deduplication: QueueAnalyzer.Size, lambda* and rateStar read a server's tokens but not its rate, so they run
+ * once per (server, accelerator, in_tokens, out_tokens) that some level uses under load (DESIGN.md §3.12).  Only
+ * the replica count, the cost and one Analyze run per level.  With the fleet's own tokens on every row the call
+ * sizes what wva_load_grid sizes, and returns the same bytes.
+ *
+ * The fleet becomes resident, as with every call that takes one; there is no single solution afterwards, so
+ * wva_summarize returns WVA_ERR_STATE.  `candidates` (n_levels*S*A entries) may be NULL; `winners` has
+ * n_levels*S entries.  n_levels == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG: n_levels < 0, a row list
+ * NULL with n_levels * S > 0, or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_levels >= 2^31 (refused before the
+ * fleet is read; the distinct keys x A are then below 2^31 as well), or exactly the levels on which wva_analyze of
+ * f_l fails the same way: a load pair outside the queue-size rule (its batch size comes from that level's
+ * out_tokens, so a small out_tokens can push it above 2^20), a rescale loop that would not terminate, or too many
+ * stored-vector fallbacks.  A token pair that no level uses under load (its levels all have rate 0, a negative
+ * rate or out_tokens 0) is never sized and does not fail the call.
+ */
+int wva_workload_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
+                      const int32_t *in_tokens, const int32_t *out_tokens, wva_allocs *candidates,
+                      wva_allocs *winners);
+
+/*
  * Load intervals: for each server, the exact float32 arrival rates in [rpm_lo[s], rpm_hi[s]] (req/min) at which
  * wva_load_grid's winner changes its decision, and the winner on each stretch in between.  An autoscaler can
  * skip a re-solve while the load stays inside the current interval, or publish the next scale-up and scale-down

@@ -401,11 +401,10 @@ void launch_fallback(wva_handle* h, void (*kernel)(Args, FbRun), const Args& g, 
     h->launches++;
 }
 
-// The (server, accelerator) pairs that keep(s, a) accepts, as ids s * A + a with their batch sizes N, sorted
+// The (server, accelerator) pairs of hf that keep(s, a) accepts, as ids s * A + a with their batch sizes N, sorted
 // by descending N (stable: equal N keep the pair order).
 template <class Keep>
-int sorted_pairs(wva_handle* h, Keep keep, std::vector<int>& pairs, std::vector<int>& N) {
-    const HostFleet& hf = h->hf;
+int sorted_pairs(wva_handle* h, const HostFleet& hf, Keep keep, std::vector<int>& pairs, std::vector<int>& N) {
     const int A = hf.A, S = hf.S;
     std::vector<int> Ns((size_t)S * A, 0);
     pairs.clear();
@@ -476,11 +475,12 @@ int upload_tables(wva_handle* h, PairTables& pt, const std::vector<int>& pair, c
     return WVA_OK;
 }
 
-// build_pair_tables over the uploaded lists; the grid passes its batch list and gets the per-(table, batch)
-// constants in pb
-int build_tables(wva_handle* h, const PairTables& pt, const int* batch = nullptr, int B = 0, float4* pb = nullptr) {
+// build_pair_tables over the uploaded lists of fleet f's pairs; the grid passes its batch list and gets the
+// per-(table, batch) constants in pb
+int build_tables(wva_handle* h, const DevFleet& f, const PairTables& pt, const int* batch = nullptr, int B = 0,
+                 float4* pb = nullptr) {
     if (pt.n == 0) return WVA_OK;
-    build_pair_tables<<<pt.n, 128, 0, h->stream>>>(h->df, pt.pair(), pt.off(), pt.len(), pt.n, (double*)pt.tab.p,
+    build_pair_tables<<<pt.n, 128, 0, h->stream>>>(f, pt.pair(), pt.off(), pt.len(), pt.n, (double*)pt.tab.p,
                                                    pt.with_ls ? (float*)pt.ls.p : nullptr, batch, B, pb);
     h->launches++;
     CK(cudaGetLastError());
@@ -494,12 +494,12 @@ int prepare_size(wva_handle* h) {
     if (pt.holds(h->epoch_tokens)) return WVA_OK;
     const HostFleet& hf = h->hf;
     std::vector<int> pairs, Ns;
-    int rc = sorted_pairs(h, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
+    int rc = sorted_pairs(h, hf, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
     if (rc) return rc;
     Cols c(16);
     rc = upload_tables(h, pt, pairs, Ns, true, c, [](char*) {});
     if (rc) return rc;
-    rc = build_tables(h, pt);
+    rc = build_tables(h, h->df, pt);
     if (rc) return rc;
     pt.epoch = h->epoch_tokens;
     return WVA_OK;
@@ -782,7 +782,7 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
         if (B) memcpy(p + o_bl, batch, 4 * (size_t)B);
     });
     if (rc) return rc;
-    rc = build_tables(h, pt);
+    rc = build_tables(h, h->df, pt);
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
@@ -816,35 +816,36 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
 // ---- load grid: CreateAllocation and the unlimited winner at every listed load level -------------------------
 // Phase 1 sizes each candidate once: the pairs that pass the gates and are a load somewhere in the caller's
 // rates, sorted by descending N with one N-entry table each, run through the size drivers in rateStar mode.  The
-// load grid and the load intervals share it (and lg_tabs / d_lg_star, which both rebuild on every call).
+// load grid, the load intervals and the workload grid share it (and lg_tabs / d_lg_star, which all rebuild on every
+// call).  Each passes the fleet it sizes: the resident one, or the workload grid's key fleet.
 //
-// prepare_load_star uploads the candidate lists with the caller's columns (laid out in c, written by fill; `pairs`
-// holds the candidates' pair ids by the time fill runs).  enqueue_load_star then builds the tables, sizes fallback
-// list 1 for the caller's tail (up to fb2_cap entries) and enqueues phase 1.
+// prepare_load_star uploads the candidate lists of fleet hf with the caller's columns (laid out in c, written by
+// fill; `pairs` holds the candidates' pair ids by the time fill runs).  enqueue_load_star then builds the tables
+// for the device image f of the same fleet, sizes fallback list 1 for the caller's tail (up to fb2_cap entries)
+// and enqueues phase 1.
 struct LoadStar {
     int n = 0;           // candidates
     AllocCols star{};    // rateStar mode's records by pair id: feasible and max_rate = rateStar
     FbRun fb2{};         // the tail's fallback list
-    SizeArgs g{};        // phase 1's candidates and tables
+    SizeArgs g{};        // phase 1's fleet, candidates and tables
 };
 template <class Fill>
-int prepare_load_star(wva_handle* h, const std::vector<char>& loaded, std::vector<int>& pairs, Cols& c, Fill&& fill) {
-    const HostFleet& hf = h->hf;
+int prepare_load_star(wva_handle* h, const HostFleet& hf, const std::vector<char>& loaded, std::vector<int>& pairs,
+                      Cols& c, Fill&& fill) {
     std::vector<int> Ns;
-    int rc = sorted_pairs(h, [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, true, 1.0f) == PAIR_LOAD; },
-                          pairs, Ns);
+    int rc = sorted_pairs(
+        h, hf, [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, true, 1.0f) == PAIR_LOAD; }, pairs, Ns);
     if (rc) return rc;
     return upload_tables(h, h->lg_tabs, pairs, Ns, true, c, fill);
 }
-int enqueue_load_star(wva_handle* h, long long fb2_cap, LoadStar& ls) {
-    const HostFleet& hf = h->hf;
+int enqueue_load_star(wva_handle* h, const HostFleet& hf, const DevFleet& f, long long fb2_cap, LoadStar& ls) {
     const PairTables& pt = h->lg_tabs;
     const size_t n_pairs = (size_t)hf.S * hf.A;
     CK(h->d_lg_star.ensure(5 * n_pairs + 16));
     ls.star = AllocCols{};
     ls.star.max_rate = (float*)h->d_lg_star.p;
     ls.star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
-    int rc = build_tables(h, pt);
+    int rc = build_tables(h, f, pt);
     if (rc) return rc;
     // the tail's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
     rc = prepare_fallback(h, 1, (int)std::min<long long>(fb2_cap, 1 << 22), pt.n ? pt.len_max : 0, ls.fb2);
@@ -852,7 +853,7 @@ int enqueue_load_star(wva_handle* h, long long fb2_cap, LoadStar& ls) {
     ls.n = pt.n;
     SizeArgs& g = ls.g;
     g = SizeArgs{};
-    g.f = h->df;
+    g.f = f;
     g.cand_pair = pt.pair();
     g.cand_N = pt.len();
     g.n_cand = pt.n;
@@ -863,10 +864,10 @@ int enqueue_load_star(wva_handle* h, long long fb2_cap, LoadStar& ls) {
     g.cand = ls.star;
     return enqueue_candidates(h, g, pt.len_max, SIZE_STAR);
 }
-// The tail's view of phase 1: candidates, tables and rateStar records (the level list is the caller's).
-LoadArgs load_args(wva_handle* h, const LoadStar& ls) {
+// The tail's view of phase 1: fleet, candidates, tables and rateStar records (the level list is the caller's).
+LoadArgs load_args(const LoadStar& ls) {
     LoadArgs la{};
-    la.f = h->df;
+    la.f = ls.g.f;
     la.cand_pair = ls.g.cand_pair;
     la.cand_N = ls.g.cand_N;
     la.tab_off = ls.g.tab_off;
@@ -889,7 +890,7 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     std::vector<int> pairs;
     Cols c(16);
     const size_t o_rpm = c.take(4 * (size_t)L * S);
-    int rc = prepare_load_star(h, loaded, pairs, c, [&](char* p) {
+    int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
         if ((size_t)L * S) memcpy(p + o_rpm, rpm, 4 * (size_t)L * S);
     });
     if (rc) return rc;
@@ -904,11 +905,11 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
         h->launches++;
     }
     LoadStar ls;
-    rc = enqueue_load_star(h, n_items, ls);
+    rc = enqueue_load_star(h, hf, h->df, n_items, ls);
     if (rc) return rc;
     const FbRun& fb2 = ls.fb2;
     if (n > 0 && L > 0) {
-        LoadArgs la = load_args(h, ls);
+        LoadArgs la = load_args(ls);
         la.level_rpm = d_rpm;
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
@@ -951,7 +952,7 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     std::vector<int> pairs;
     Cols c(16);
     const size_t o_lo = c.take(4 * (size_t)S), o_hi = c.take(4 * (size_t)S), o_cop = c.take(4 * (size_t)S * A);
-    int rc = prepare_load_star(h, loaded, pairs, c, [&](char* p) {
+    int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
         if (S) {
             memcpy(p + o_lo, lo, 4 * (size_t)S);
             memcpy(p + o_hi, hi, 4 * (size_t)S);
@@ -968,12 +969,12 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
     CK(cudaMemsetAsync(d + iv.o_start, 0, 4 * (size_t)S * M, h->stream));
     LoadStar ls;
-    rc = enqueue_load_star(h, (long long)S * M, ls);
+    rc = enqueue_load_star(h, hf, h->df, (long long)S * M, ls);
     if (rc) return rc;
     if (S == 0) return WVA_OK;
     const char* dl = (const char*)h->lg_tabs.lists.p;
     IntervalArgs g{};
-    g.ld = load_args(h, ls);
+    g.ld = load_args(ls);
     g.cand_of_pair = (const int*)(dl + o_cop);
     g.lo = (const float*)(dl + o_lo);
     g.hi = (const float*)(dl + o_hi);
@@ -1019,7 +1020,8 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
     // the tail's candidates: every load pair (none without levels), descending N, one N-entry table each
     std::vector<int> pairs, Ns;
     if (L > 0) {
-        const int rc = sorted_pairs(h, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
+        const int rc =
+            sorted_pairs(h, hf, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
         if (rc) return rc;
     }
     std::vector<int> tab_of((size_t)S * A, -1);  // the pair's table index
@@ -1101,7 +1103,7 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
     if (rc) return rc;
     const PairTables& pt = h->lg_tabs;
     const char* d = (const char*)pt.lists.p;
-    rc = build_tables(h, pt);
+    rc = build_tables(h, h->df, pt);
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
@@ -1162,6 +1164,170 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
         h->launches++;
         CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
         launch_fallback(h, slo_fallback, la, fb2);
+    }
+    if (S > 0 && L > 0) {
+        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
+            h->df, cand, winners, L);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- workload grid: CreateAllocation and the unlimited winner at every listed (rate, in, out) row --------------
+// Which lengths of WVA_FLEET_COLUMNS are per server.
+#define WVA_PER_SERVER_A 0
+#define WVA_PER_SERVER_T 0
+#define WVA_PER_SERVER_MA 0
+#define WVA_PER_SERVER_S 1
+
+// The fleet the workload grid sizes (DESIGN.md §3.12): row k is server srv[k] of the resident fleet at the key's
+// tokens, with a positive rate (phase 1 reads no rate; the tail reads the level's).  The A, T and M columns are the
+// resident fleet's.  On the device the server columns lie in an upload image of the caller's (place, write), and
+// view() points a copy of the resident DevFleet at them, so the resident arena is never written.
+struct KeyFleet {
+    HostFleet hf;
+    struct {
+#define KEY_OFFSET(abi, name, type, len) size_t name = 0;
+        WVA_FLEET_COLUMNS(KEY_OFFSET)
+#undef KEY_OFFSET
+    } off;
+    KeyFleet(const HostFleet& fleet, const std::vector<int>& srv, const std::vector<int>& in,
+             const std::vector<int>& out)
+        : hf(fleet) {
+        const size_t K = srv.size();
+        hf.S = (int)K;
+#define KEY_GATHER(abi, name, type, len)                                     \
+    if (WVA_PER_SERVER_##len) {                                              \
+        hf.name.resize(K);                                                   \
+        for (size_t k = 0; k < K; ++k) hf.name[k] = fleet.name[srv[k]];      \
+    }
+        WVA_FLEET_COLUMNS(KEY_GATHER)
+#undef KEY_GATHER
+        std::fill(hf.srv_arrival_rpm.begin(), hf.srv_arrival_rpm.end(), 1.0f);
+        hf.srv_in_tokens = in;
+        hf.srv_out_tokens = out;
+    }
+    void place(Cols& c) {
+#define KEY_PLACE(abi, name, type, len) \
+    if (WVA_PER_SERVER_##len) off.name = c.take(sizeof(type) * hf.name.size());
+        WVA_FLEET_COLUMNS(KEY_PLACE)
+#undef KEY_PLACE
+    }
+    void write(char* p) const {
+#define KEY_WRITE(abi, name, type, len) \
+    if (WVA_PER_SERVER_##len && !hf.name.empty()) memcpy(p + off.name, hf.name.data(), sizeof(type) * hf.name.size());
+        WVA_FLEET_COLUMNS(KEY_WRITE)
+#undef KEY_WRITE
+    }
+    DevFleet view(DevFleet f, const char* d) const {
+        f.S = hf.S;
+#define KEY_VIEW(abi, name, type, len) \
+    if (WVA_PER_SERVER_##len) f.name = (const type*)(d + off.name);
+        WVA_FLEET_COLUMNS(KEY_VIEW)
+#undef KEY_VIEW
+        return f;
+    }
+};
+
+// QueueAnalyzer.Size, lambda* and rateStar read a server's tokens but not its rate (DESIGN.md §3.12), so phase 1
+// is the load grid's, run once on the key fleet: one row per distinct (server, in_tokens, out_tokens) that some
+// level uses under load (rate not negative and not 0, NaN and +Inf included; in_tokens >= 0; out_tokens >= 1).
+// Phase 2 (workload_kernel, workload_fallback) is the load grid's tail per (key candidate, level of the key).  The
+// lists, the key fleet's server columns and the tables go into lg_tabs, rebuilt on every call.  rpm / in / out
+// [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device columns.
+int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                          const AllocCols& cand, const AllocCols& winners) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A;
+    const size_t LS = (size_t)L * S;
+    // the keys: per server, its distinct (in, out) in ascending order; key k's levels are lev[lev_off[k] ..
+    // lev_off[k + 1]), ascending.  There are at most L * S keys, so fewer than 2^31 key candidates.
+    std::vector<int> key_srv, key_in, key_out, lev_off{0}, lev;
+    std::vector<std::pair<uint64_t, int>> uses;  // ((in << 32) | out, level)
+    for (int s = 0; s < S; ++s) {
+        uses.clear();
+        for (int l = 0; l < L; ++l) {
+            const size_t i = (size_t)l * S + s;
+            if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1)
+                uses.emplace_back((uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], l);
+        }
+        std::sort(uses.begin(), uses.end());
+        for (size_t u = 0; u < uses.size(); ++u) {
+            if (u == 0 || uses[u].first != uses[u - 1].first) {
+                key_srv.push_back(s);
+                key_in.push_back((int)(uses[u].first >> 32));
+                key_out.push_back((int)(uint32_t)uses[u].first);
+                lev_off.push_back(lev_off.back());
+            }
+            lev.push_back(uses[u].second);
+            lev_off.back()++;
+        }
+    }
+    const int K = (int)key_srv.size();
+    KeyFleet kf(hf, key_srv, key_in, key_out);
+    Cols c(16);
+    kf.place(c);
+    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS),
+                 o_ksrv = c.take(4 * (size_t)K), o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * lev.size()),
+                 o_item = c.take(4 * ((size_t)K * A + 1));
+    std::vector<int> pairs;
+    int n_items = 0;
+    int rc = prepare_load_star(h, kf.hf, std::vector<char>(K, 1), pairs, c, [&](char* p) {
+        kf.write(p);
+        if (LS) {
+            memcpy(p + o_rpm, rpm, 4 * LS);
+            memcpy(p + o_in, in, 4 * LS);
+            memcpy(p + o_out, out, 4 * LS);
+        }
+        if (K) memcpy(p + o_ksrv, key_srv.data(), 4 * (size_t)K);
+        memcpy(p + o_loff, lev_off.data(), 4 * ((size_t)K + 1));
+        if (!lev.empty()) memcpy(p + o_lev, lev.data(), 4 * lev.size());
+        // candidate j's items: one per level of its key
+        int* item = (int*)(p + o_item);
+        item[0] = 0;
+        for (size_t j = 0; j < pairs.size(); ++j) {
+            const int k = pairs[j] / A;
+            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
+        }
+        n_items = item[pairs.size()];
+    });
+    if (rc) return rc;
+    const char* d = (const char*)h->lg_tabs.lists.p;
+    const float* d_rpm = (const float*)(d + o_rpm);
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
+    if (n_rec > 0) {
+        trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(
+            h->df, cand, d_rpm, (const int*)(d + o_in), (const int*)(d + o_out), L);
+        h->launches++;
+    }
+    LoadStar ls;
+    rc = enqueue_load_star(h, kf.hf, kf.view(h->df, d), n_items, ls);
+    if (rc) return rc;
+    if (n_items > 0) {
+        WorkloadArgs g{};
+        g.ld = load_args(ls);
+        g.ld.level_rpm = d_rpm;
+        g.ld.L = L;
+        g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+        g.ld.cand = cand;
+        g.key_srv = (const int*)(d + o_ksrv);
+        g.lev_off = (const int*)(d + o_loff);
+        g.lev = (const int*)(d + o_lev);
+        g.item_off = (const int*)(d + o_item);
+        g.S = S;
+        g.n_items = n_items;
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, workload_kernel, 256, 0));
+        per_sm = std::max(1, std::min(per_sm, 8));
+        const long long warps = ((long long)n_items + 31) / 32;
+        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
+        workload_kernel<<<blocks, 256, 0, h->stream>>>(g);
+        h->launches++;
+        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
+        launch_fallback(h, workload_fallback, g, ls.fb2);
     }
     if (S > 0 && L > 0) {
         unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
@@ -1275,7 +1441,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     g.batch_rank = g.batch + B;
     g.rank_to_bi = g.batch + 2 * B;
     g.replicas = g.batch + 3 * B;
-    int rc = build_tables(h, pt, g.batch, B, (float4*)h->d_pb.p);
+    int rc = build_tables(h, h->df, pt, g.batch, B, (float4*)h->d_pb.p);
     if (rc) return rc;
     g.B = B;
     g.R = R;
@@ -2061,6 +2227,31 @@ int wva_slo_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const 
     return WVA_OK;
 }
 
+int wva_workload_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                      const int32_t* in_tokens, const int32_t* out_tokens, wva_allocs* candidates,
+                      wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * n_levels > 0 && (!arrival_rpm || !in_tokens || !out_tokens))
+        return h->fail(WVA_ERR_BAD_ARG, "NULL row list");
+    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "workload grid too large for one call (>= 2^31 candidates)");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
+    c.win_blocks = (size_t)n_levels;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_workload_grid(h, n_levels, arrival_rpm, in_tokens, out_tokens, dc, dw);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
 int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_lo, const float* rpm_hi,
                        wva_intervals* out) {
     if (!h) return WVA_ERR_BAD_ARG;
@@ -2234,7 +2425,7 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
     const int A = hf.A, S = hf.S;
     // every (server, acc) with a profile, ignoring keepAccelerator
     std::vector<int> pairs, lens;
-    rc = sorted_pairs(h,
+    rc = sorted_pairs(h, hf,
                       [&](int s, int a) {
                           const int m = hf.srv_model[s];
                           return hf.srv_in_tokens[s] >= 0 && hf.srv_out_tokens[s] >= 1 && m >= 0 && m < hf.M &&
@@ -2264,7 +2455,7 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         Cols c(16);
         int rc = upload_tables(h, pt, pairs, lens, false, c, [](char*) {});
         if (rc) return rc;
-        rc = build_tables(h, pt);
+        rc = build_tables(h, h->df, pt);
         if (rc) return rc;
         FbRun fb;
         rc = prepare_fallback(h, 0, (int)std::min<size_t>((size_t)n * n_rates, (size_t)1 << 22), lens[0], fb);

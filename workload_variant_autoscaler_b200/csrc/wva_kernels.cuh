@@ -5,7 +5,8 @@
 //                       sort, persistent warps pulling 32-cell items, fused feasibility + batch-rank minimum
 //   grid_fallback       stored-vector re-run of the rare cells the streaming solve bails on
 //   grid_finalize  K3   per-server argmin over partials (warp shuffle -> smem -> record)
-//   trivial_kernel      nil / zero-load candidates (overloads: per level of wva_load_grid and wva_slo_grid)
+//   trivial_kernel      nil / zero-load candidates (overloads: per level of wva_load_grid, wva_slo_grid and
+//                       wva_workload_grid)
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
 //   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
@@ -1590,6 +1591,23 @@ __global__ void trivial_kernel(DevFleet f, AllocCols cand, int L) {
     const int pair = i % n_pairs;
     const int s = pair / f.A, a = pair % f.A;
     const int cls = pair_class(f, s, a, true);
+    if (cls == PAIR_LOAD) return;
+    store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
+}
+// ... of the workload grid: L level blocks of S * A records (record l * S * A + pair), each pair classed at its
+// level's rate and tokens (row l of level_rpm, level_in and level_out); a zero-load candidate reads no tokens
+// (S * A * L < 2^31, checked on the host).
+__global__ void trivial_kernel(DevFleet f, AllocCols cand, const float* level_rpm, const int* level_in,
+                               const int* level_out, int L) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n_pairs = f.S * f.A;
+    if (i >= n_pairs * L) return;
+    const int l = i / n_pairs, pair = i - l * n_pairs;
+    const int s = pair / f.A, a = pair % f.A;
+    DevFleet fl = at_level(f, level_rpm, l);
+    fl.srv_in_tokens = level_in + (size_t)l * f.S;
+    fl.srv_out_tokens = level_out + (size_t)l * f.S;
+    const int cls = pair_class(fl, s, a, true);
     if (cls == PAIR_LOAD) return;
     store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
 }

@@ -3,7 +3,8 @@
 // replica count, the feasible candidate) are written once below and driven two ways: large fleets run ROUNDS of
 // sorted solve batches with SPECULATIVE bisection (sz2_*); small fleets and the stored-vector fallback run
 // create_allocation straight through (size_warp_kernel, size_fallback).  The load grid runs the same drivers up to
-// rateStar (the part that does not read the load), then its tail per load level (load_kernel, load_fallback).
+// rateStar (the part that does not read the load), then its tail per load level (load_kernel, load_fallback); the
+// workload grid runs them on a fleet of token keys, then the same tail (workload_kernel, workload_fallback).
 //
 // The reference runs, per candidate, two sequential bisections (pkg/analyzer/utils.go:26-70) of <= 102 model
 // solves each, then two Analyze calls.  The solves of one bisection depend on each other only through ONE
@@ -1030,6 +1031,93 @@ __global__ void slo_fallback(SloArgs g, FbRun r) {
             }, c))
             return rc;
         store_cand(g.cand, slo_record(g, e, l), c);
+        return 0;
+    });
+}
+
+// ---------------------------------------------------------------------------
+// The workload grid's tail (DESIGN.md §3.12): the load grid's tail (load_tail) on the key fleet, whose row k is
+// server key_srv[k] at one (in_tokens, out_tokens) pair; phase 1 sized its load pairs k * A + a in rateStar mode.
+// One lane per (key candidate, level that uses the key) item: candidate e's items are item_off[e] ..
+// item_off[e + 1] - 1, and its j-th item is the j-th level of its key (lev[lev_off[k] + j]).  So items are
+// candidate-major and a warp reads the tables of one or a few candidates; a work counter hands out warps, as in
+// load_kernel.  totalRate is the level's rate over 60, or with a TPS target TPS over the key's out_tokens, which
+// are the level's.  Record (l * S + s) * A + a.
+// ---------------------------------------------------------------------------
+struct WorkloadArgs {
+    LoadArgs ld;           // phase 1 on the key fleet; level_rpm [L * S] by server and cand [L * S * A]
+    const int* key_srv;    // [K] the key's server
+    const int* lev_off;    // [K + 1] key k's levels are lev[lev_off[k] .. lev_off[k + 1]), ascending
+    const int* lev;
+    const int* item_off;   // [n_cand + 1] candidate e's first item
+    int S;                 // servers of the fleet (ld.f.S counts the keys)
+    int n_items;           // item_off[n_cand]: at most one per loaded (level, server, accelerator), < 2^31
+};
+
+// Item i's candidate e (the last one with item_off[e] <= i) and level l.
+__device__ __forceinline__ void workload_item(const WorkloadArgs& g, int i, int& e, int& l) {
+    int lo = 0, hi = g.ld.n_cand - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (g.item_off[mid] <= i) lo = mid;
+        else hi = mid - 1;
+    }
+    e = lo;
+    const int k = g.ld.cand_pair[e] / g.ld.f.A;
+    l = g.lev[g.lev_off[k] + (i - g.item_off[e])];
+}
+
+// Candidate e's record at level l and its index; solve(tab, N, K, lambda, st) is Model.Solve for the final
+// Analyze.  Returns false when that solve bailed (out is then nil).
+template <class Solve>
+__device__ __forceinline__ bool workload_tail(const WorkloadArgs& g, int e, int l, Solve&& solve, Cand& out,
+                                              size_t& rec) {
+    const DevFleet& f = g.ld.f;
+    const int pair = g.ld.cand_pair[e], k = pair / f.A, s = g.key_srv[k];
+    const float rpm = g.ld.level_rpm[(size_t)l * g.S + s];
+    rec = ((size_t)l * g.S + s) * f.A + pair % f.A;
+    const int N = g.ld.cand_N[e], K = N + N * f.ratio;
+    const double* tab = g.ld.tab + 4 * g.ld.tab_off[e];
+    return load_tail(g.ld, e, [&](int) { return total_rate_of(f, k, rpm); }, (float)tab[4 * (N - 1)],
+                     [&](float lam, ModelStats& st) { return solve(tab, N, K, lam, st); }, out);
+}
+
+__global__ void __launch_bounds__(256) workload_kernel(WorkloadArgs g) {
+    const int lane = threadIdx.x & 31;
+    const unsigned n_items = (unsigned)g.n_items;
+    for (;;) {
+        unsigned w = 0;
+        if (lane == 0) w = atomicAdd(g.ld.counter, 1u);
+        w = __shfl_sync(0xffffffffu, w, 0);
+        if ((unsigned long long)w * 32 >= n_items) break;
+        const unsigned i = w * 32 + lane;
+        if (i < n_items) {
+            int e, l;
+            workload_item(g, (int)i, e, l);
+            Cand c;
+            size_t rec;
+            const bool ok = workload_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+                return solve_shared(tab, N, K, lam, st) == kSolveOk;
+            }, c, rec);
+            if (!ok) fb_push(g.ld.fb, fb_pack(e, l));
+            store_cand(g.ld.cand, rec, c);
+        }
+    }
+}
+
+// Stored-vector re-run of the items workload_kernel bailed on.
+__global__ void workload_fallback(WorkloadArgs g, FbRun r) {
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        const int e = (int)(item >> 32), l = (int)(unsigned)item;
+        int rc = 0;
+        Cand c;
+        size_t rec;
+        if (!workload_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+                rc = solve_stored(p, tab, N, K, lam, st);
+                return rc == 0;
+            }, c, rec))
+            return rc;
+        store_cand(g.ld.cand, rec, c);
         return 0;
     });
 }

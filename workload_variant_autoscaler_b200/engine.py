@@ -181,6 +181,40 @@ class Engine:
                                          C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
+    def workload_grid(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None,
+                      want_candidates: bool = False, out: Allocs | None = None):
+        """The reference's ``Server.Calculate`` and ``SolveUnlimited`` winner at each row of (``arrival_rpm``
+        req/min, ``in_tokens``, ``out_tokens``), each of shape (L, S) -> (candidates [L*S*A] | None,
+        winners [L*S]), both level-major.
+
+        Candidate block ``l`` is what ``analyze`` returns for the fleet with ``srv_arrival_rpm``,
+        ``srv_in_tokens`` and ``srv_out_tokens`` = row ``l``, and winner block ``l`` is ``solve``'s winners for
+        it in unlimited mode; each distinct (server, in, out) is sized once (see ``wva_workload_grid`` in
+        include/wva_b200.h).  A token list of ``None`` is the fleet's own column at every level.  ``out``: an
+        ``Allocs`` of ``L * S`` records to write the winners into."""
+        S = fleet.n_servers
+        rpm = np.ascontiguousarray(arrival_rpm, np.float32)
+        if rpm.ndim != 2 or rpm.shape[1] != S:
+            raise ValueError(f"arrival_rpm must have shape (L, {S}), got {rpm.shape}")
+        L = rpm.shape[0]
+        rows = [rpm]
+        for name, x, own in (("in_tokens", in_tokens, fleet.srv_in_tokens),
+                             ("out_tokens", out_tokens, fleet.srv_out_tokens)):
+            r = np.ascontiguousarray(np.broadcast_to(own, (L, S)) if x is None else x, np.int32)
+            if r.shape != (L, S):
+                raise ValueError(f"{name} must have shape ({L}, {S}), got {r.shape}")
+            rows.append(r)
+        if out is not None and out.n != L * S:
+            raise ValueError("out must hold L * fleet.n_servers records")
+        win = out if out is not None else Allocs(L * S)
+        cand = Allocs(L * S * fleet.n_acc) if want_candidates else None
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_workload_grid(self._h, C.byref(fc), L, *[_abi.ptr(r.reshape(-1)) for r in rows],
+                                              C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
+
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
         """Where each server's ``load_grid`` winner changes its decision in ``[rpm_lo[s], rpm_hi[s]]`` (req/min)
         -> (count [S], truncated [S], start_rpm (S, M), records: ``Allocs`` of S * M).
