@@ -358,6 +358,51 @@ int wva_workload_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, c
                       wva_allocs *winners);
 
 /*
+ * Workload trace: the reference's reconcile replayed over n_ticks caller-given rows of (arrival rate, average input
+ * tokens, average output tokens), each tick's winner becoming the next tick's current allocation, e.g. what the
+ * autoscaler does over a recorded day or a forecast, and what it costs.  The rows are laid out as in
+ * wva_workload_grid: each is [n_ticks * S], index t*S + s.
+ *
+ * Let c_0 be the fleet's (srv_cur_acc, srv_cur_replicas, srv_cur_cost), and f_t the fleet with srv_arrival_rpm,
+ * srv_in_tokens and srv_out_tokens replaced by row t and its current-allocation columns replaced by c_t.
+ *   - Candidate block t (records (t*S + s)*A + a) is byte for byte what wva_analyze returns for f_t: value =
+ *     TransitionPenalty(c_t, .), and the keepAccelerator mask against c_t's accelerator (a masked pair is a nil
+ *     record).
+ *   - Winner block t (records t*S + s) is byte for byte wva_solve's winner block for f_t with unlimited = 1.
+ *   - c_{t+1} is winner t's (acc, replicas, cost) when that winner is feasible, and c_t otherwise.  A zero-load
+ *     winner with min_replicas 0 has accelerator WVA_ACC_NONE, 0 replicas and cost 0, and becomes exactly that.
+ * This is the reference's Server.SetLoad(row t); Server.Calculate; SolveUnlimited; Server.ApplyDesiredAlloc per
+ * tick, on a ServerSpec whose DesiredAlloc starts equal to its CurrentAlloc (the state ApplyDesiredAlloc leaves).
+ * A spec built by the WVA adapters starts with an empty DesiredAlloc instead (internal/utils/utils.go:293).  The two
+ * differ only for a server that has no winner at tick 0: the reference would then drop that server to the empty
+ * allocation, while the controller (and this call) leaves it unchanged.
+ *
+ * Only unlimited mode is traced: limited mode's greedy pass couples the servers and runs on the host, and WVA always
+ * runs unlimited (internal/utils/utils.go:170).  fleet->unlimited and the capacities are not read.  A trace can be
+ * continued: the trace over ticks 0..L-1 equals the trace over 0..k-1 followed by the trace over k..L-1 on the fleet
+ * whose srv_cur_* columns hold c_k.
+ *
+ * Sizing (DESIGN.md §3.13): CreateAllocation does not read the current allocation, so every tick's records are
+ * sized in one batched pass with the workload grid's deduplication, and only the chain (mask, value, minimum,
+ * advance) runs tick by tick, on the device.  A server is pinned when keepAccelerator is set, its current
+ * accelerator is not WVA_ACC_NONE, and either that accelerator is WVA_ACC_UNKNOWN or min_replicas != 0: its
+ * accelerator can never change, so only (s, srv_cur_acc[s]) is sized (nothing when unknown).  Every other server's
+ * pairs are all sized, keepAccelerator ignored, since its current accelerator can change along the chain.
+ *
+ * The fleet becomes resident; wva_summarize returns WVA_ERR_STATE afterwards.  `candidates` (n_ticks*S*A entries)
+ * may be NULL; `winners` has n_ticks*S entries.  n_ticks == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG:
+ * n_ticks < 0, a row list NULL with n_ticks * S > 0, or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_ticks >= 2^31
+ * (refused before the fleet is read), or the failures of wva_workload_grid for the pairs the call sizes: a load pair
+ * outside the queue-size rule, a rescale loop that would not terminate, or too many stored-vector fallbacks.  This
+ * set of refusals can be larger than the set of ticks at which wva_analyze(f_t) fails, but only through the pairs of
+ * a server that is not pinned yet has keepAccelerator set, at ticks where the chain keeps them masked.  The call
+ * never returns a result that differs from the per-tick composition.
+ */
+int wva_workload_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                       const int32_t *in_tokens, const int32_t *out_tokens, wva_allocs *candidates,
+                       wva_allocs *winners);
+
+/*
  * Load intervals: for each server, the exact float32 arrival rates in [rpm_lo[s], rpm_hi[s]] (req/min) at which
  * wva_load_grid's winner changes its decision, and the winner on each stretch in between.  An autoscaler can
  * skip a re-solve while the load stays inside the current interval, or publish the next scale-up and scale-down

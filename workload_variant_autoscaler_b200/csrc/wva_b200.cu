@@ -1230,14 +1230,27 @@ struct KeyFleet {
     }
 };
 
+// A server whose accelerator no tick of a workload trace can change (DESIGN.md §3.13): with keepAccelerator and a
+// current accelerator other than "" only that accelerator is a candidate, and its load and zero-load candidates
+// carry it unless min_replicas is 0 (a zero-load candidate is then ""); an unknown one has no candidate at all.
+// A nil winner keeps the current allocation, so neither ever moves.
+bool trace_pinned(const HostFleet& hf, int s) {
+    const int cur = hf.srv_cur_acc[s];
+    return hf.srv_keep_acc[s] && cur != WVA_ACC_NONE && (cur == WVA_ACC_UNKNOWN || hf.srv_min_replicas[s] != 0);
+}
+
 // QueueAnalyzer.Size, lambda* and rateStar read a server's tokens but not its rate (DESIGN.md §3.12), so phase 1
 // is the load grid's, run once on the key fleet: one row per distinct (server, in_tokens, out_tokens) that some
 // level uses under load (rate not negative and not 0, NaN and +Inf included; in_tokens >= 0; out_tokens >= 1).
 // Phase 2 (workload_kernel, workload_fallback) is the load grid's tail per (key candidate, level of the key).  The
 // lists, the key fleet's server columns and the tables go into lg_tabs, rebuilt on every call.  rpm / in / out
-// [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device columns.
-int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                          const AllocCols& cand, const AllocCols& winners) {
+// [L*S] are the caller's rows; cand ([L*S*A]) is a device column.
+//
+// With `trace` (the workload trace, DESIGN.md §3.13) the records are CreateAllocation without the keepAccelerator
+// mask, which trace_kernel applies tick by tick: trivial_kernel sees an all-zero keep column, and the key fleet keeps
+// keepAccelerator only on the pinned servers, so that phase 1 sizes their current accelerator alone.
+int enqueue_workload_sizing(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                            const AllocCols& cand, bool trace) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     const size_t LS = (size_t)L * S;
@@ -1266,11 +1279,14 @@ int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t*
     }
     const int K = (int)key_srv.size();
     KeyFleet kf(hf, key_srv, key_in, key_out);
+    if (trace)
+        for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, key_srv[k]);
     Cols c(16);
     kf.place(c);
     const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS),
                  o_ksrv = c.take(4 * (size_t)K), o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * lev.size()),
                  o_item = c.take(4 * ((size_t)K * A + 1));
+    const size_t o_nokeep = trace ? c.take(S) : 0;  // the trace's all-zero keep column
     std::vector<int> pairs;
     int n_items = 0;
     int rc = prepare_load_star(h, kf.hf, std::vector<char>(K, 1), pairs, c, [&](char* p) {
@@ -1291,6 +1307,7 @@ int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t*
             item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
         }
         n_items = item[pairs.size()];
+        if (trace) memset(p + o_nokeep, 0, S);
     });
     if (rc) return rc;
     const char* d = (const char*)h->lg_tabs.lists.p;
@@ -1299,8 +1316,10 @@ int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t*
     if (rc) return rc;
     const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
     if (n_rec > 0) {
+        DevFleet tf = h->df;
+        if (trace) tf.srv_keep_acc = (const uint8_t*)(d + o_nokeep);
         trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(
-            h->df, cand, d_rpm, (const int*)(d + o_in), (const int*)(d + o_out), L);
+            tf, cand, d_rpm, (const int*)(d + o_in), (const int*)(d + o_out), L);
         h->launches++;
     }
     LoadStar ls;
@@ -1329,9 +1348,34 @@ int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t*
         CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
         launch_fallback(h, workload_fallback, g, ls.fb2);
     }
-    if (S > 0 && L > 0) {
-        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
-            h->df, cand, winners, L);
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// The workload grid: the sizing above, then the unlimited winner of every level (winners [L*S], a device column).
+int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                          const AllocCols& cand, const AllocCols& winners) {
+    const int rc = enqueue_workload_sizing(h, L, rpm, in, out, cand, false);
+    if (rc) return rc;
+    if (h->hf.S > 0 && L > 0) {
+        unlimited_kernel<<<dim3((unsigned)((h->hf.S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0,
+                           h->stream>>>(h->df, cand, winners, L);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- workload trace: the reconcile replayed tick by tick (DESIGN.md §3.13) ------------------------------------
+// The workload grid's sizing of every tick in one pass, without the keepAccelerator mask, then trace_kernel's chain:
+// one thread per server applies the mask against its current allocation, picks the winner and advances.  rpm / in /
+// out [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device columns.
+int enqueue_workload_trace(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                           const AllocCols& cand, const AllocCols& winners) {
+    const int rc = enqueue_workload_sizing(h, L, rpm, in, out, cand, true);
+    if (rc) return rc;
+    if (h->hf.S > 0 && L > 0) {
+        trace_kernel<<<(unsigned)((h->hf.S + 127) / 128), 128, 0, h->stream>>>(h->df, cand, winners, L);
         h->launches++;
     }
     CK(cudaGetLastError());
@@ -2244,6 +2288,31 @@ int wva_workload_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
     c.win_blocks = (size_t)n_levels;
     rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
         return enqueue_workload_grid(h, n_levels, arrival_rpm, in_tokens, out_tokens, dc, dw);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
+int wva_workload_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                       const int32_t* in_tokens, const int32_t* out_tokens, wva_allocs* candidates,
+                       wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_ticks < 0) return h->fail(WVA_ERR_BAD_ARG, "negative tick count");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * n_ticks > 0 && (!arrival_rpm || !in_tokens || !out_tokens))
+        return h->fail(WVA_ERR_BAD_ARG, "NULL row list");
+    if ((long long)fleet->n_servers * fleet->n_acc * n_ticks >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "workload trace too large for one call (>= 2^31 candidates)");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_ticks, candidates != nullptr, true};
+    c.win_blocks = (size_t)n_ticks;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_workload_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens, dc, dw);
     });
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;

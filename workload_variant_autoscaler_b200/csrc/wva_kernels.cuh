@@ -8,6 +8,7 @@
 //   trivial_kernel      nil / zero-load candidates (overloads: per level of wva_load_grid, wva_slo_grid and
 //                       wva_workload_grid)
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
+//   trace_kernel        the same tick by tick, each tick's winner the next tick's current allocation
 //   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
 //
@@ -1651,6 +1652,46 @@ __global__ void unlimited_kernel(DevFleet f, AllocCols cand, AllocCols winners, 
     if (s >= f.S) return;
     for (int l = blockIdx.y; l < L; l += gridDim.y)
         unlimited_server(f, cols_at(cand, (size_t)l * f.S * f.A), cols_at(winners, (size_t)l * f.S), s);
+}
+
+// The workload trace's chain (DESIGN.md §3.13): one thread per server walks the L tick blocks (candidates
+// (t * S + s) * A + a, winners t * S + s) with the current allocation c_t in registers, c_0 from the fleet.  The
+// records hold CreateAllocation without the keepAccelerator mask, which does not read c_t.  Per tick: a pair the
+// mask excludes against c_t's accelerator gets a nil record (sized or not), every other feasible record gets
+// value = TransitionPenalty(c_t, .), winner t is SolveUnlimited's minimum (strict '<' from MaxFloat32, ties to the
+// lower accelerator id), and c_{t+1} is the winner's (acc, replicas, cost) when it is feasible, c_t otherwise
+// (Server.ApplyDesiredAlloc).
+__global__ void trace_kernel(DevFleet f, AllocCols cand, AllocCols winners, int L) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= f.S) return;
+    const bool keep = f.srv_keep_acc[s] != 0;
+    int cur_acc = f.srv_cur_acc[s], cur_replicas = f.srv_cur_replicas[s];
+    float cur_cost = f.srv_cur_cost[s];
+    for (int t = 0; t < L; ++t) {
+        float min_val = 3.40282346638528859811704183484516925440e+38f;
+        Cand best = cand_nil();
+        for (int a = 0; a < f.A; ++a) {
+            const size_t i = ((size_t)t * f.S + s) * f.A + a;
+            if (keep && cur_acc != -1 && cur_acc != a) {  // pair_class's keepAccelerator rule at c_t
+                store_cand(cand, i, cand_nil());
+                continue;
+            }
+            if (!cand.feasible[i]) continue;
+            Cand c = load_cand(cand, i);
+            c.value = transition_penalty(f.penalty, cur_acc, cur_replicas, cur_cost, c.acc, c.replicas, c.cost);
+            cand.value[i] = c.value;
+            if (c.value < min_val) {
+                min_val = c.value;
+                best = c;
+            }
+        }
+        store_cand(winners, (size_t)t * f.S + s, best);
+        if (best.feasible) {
+            cur_acc = best.acc;
+            cur_replicas = best.replicas;
+            cur_cost = best.cost;
+        }
+    }
 }
 
 // wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record

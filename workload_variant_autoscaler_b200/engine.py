@@ -192,6 +192,25 @@ class Engine:
         it in unlimited mode; each distinct (server, in, out) is sized once (see ``wva_workload_grid`` in
         include/wva_b200.h).  A token list of ``None`` is the fleet's own column at every level.  ``out``: an
         ``Allocs`` of ``L * S`` records to write the winners into."""
+        return self._workload_rows(self._L.wva_workload_grid, fleet, arrival_rpm, in_tokens, out_tokens,
+                                   want_candidates, out)
+
+    def workload_trace(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None,
+                       want_candidates: bool = False, out: Allocs | None = None):
+        """The reference's reconcile replayed over the ticks of (``arrival_rpm`` req/min, ``in_tokens``,
+        ``out_tokens``), each of shape (L, S): ``Server.Calculate``, ``SolveUnlimited`` and
+        ``Server.ApplyDesiredAlloc`` per tick -> (candidates [L*S*A] | None, winners [L*S]), both tick-major.
+
+        Tick ``t`` is ``workload_grid``'s level ``t`` on the fleet whose current allocation is the previous tick's
+        feasible winner (the fleet's own ``srv_cur_*`` at tick 0, and unchanged after a nil winner), i.e. ``solve``
+        on ``fleet.apply_winners`` of every earlier tick in turn (see ``wva_workload_trace`` in include/wva_b200.h).
+        A token list of ``None`` is the fleet's own column at every tick.  ``out``: an ``Allocs`` of ``L * S``
+        records to write the winners into."""
+        return self._workload_rows(self._L.wva_workload_trace, fleet, arrival_rpm, in_tokens, out_tokens,
+                                   want_candidates, out)
+
+    def _workload_rows(self, call, fleet, arrival_rpm, in_tokens, out_tokens, want_candidates, out):
+        """wva_workload_grid / wva_workload_trace over (L, S) rows; a token list of None is the fleet's own."""
         S = fleet.n_servers
         rpm = np.ascontiguousarray(arrival_rpm, np.float32)
         if rpm.ndim != 2 or rpm.shape[1] != S:
@@ -211,8 +230,8 @@ class Engine:
         fc, wc = fleet.as_c(), win.as_c()
         cc = cand.as_c() if cand is not None else None
         self._resident(fleet)
-        self._check(self._L.wva_workload_grid(self._h, C.byref(fc), L, *[_abi.ptr(r.reshape(-1)) for r in rows],
-                                              C.byref(cc) if cc is not None else None, C.byref(wc)))
+        self._check(call(self._h, C.byref(fc), L, *[_abi.ptr(r.reshape(-1)) for r in rows],
+                         C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):

@@ -143,6 +143,23 @@ class Fleet:
                 kw[n] = v.copy() if isinstance(v, np.ndarray) else v
         return Fleet(**kw)
 
+    def apply_winners(self, winners) -> "Fleet":
+        """A copy of the fleet whose current allocation is advanced by one reconcile (``Server.ApplyDesiredAlloc``,
+        pkg/core/server.go:157-161): a feasible winner's (accelerator, replicas, cost) becomes ``srv_cur_*``, and a
+        server without one keeps its current allocation.  ``winners``: S records, an ``Allocs`` or a structured
+        array with ``feasible`` / ``acc`` / ``replicas`` / ``cost`` fields (e.g. one tick of ``workload_trace``)."""
+        def col(k):
+            c = winners[k] if isinstance(winners, np.ndarray) else getattr(winners, k)
+            if len(c) != self.n_servers:
+                raise ValueError(f"winners must hold {self.n_servers} records, got {len(c)}")
+            return np.asarray(c)
+        f = self.take_servers(np.arange(self.n_servers))
+        won = col("feasible") != 0
+        f.srv_cur_acc[won] = col("acc")[won]
+        f.srv_cur_replicas[won] = col("replicas")[won]
+        f.srv_cur_cost[won] = col("cost")[won]
+        return f
+
     # ------------------------------------------------------------------
     @staticmethod
     def from_spec(spec: dict, *, max_queue_to_batch_ratio: int = 10, accel_penalty_factor: float = 0.1) -> "Fleet":
