@@ -403,6 +403,51 @@ int wva_workload_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, c
                        wva_allocs *winners);
 
 /*
+ * Rows of accelerator costs and model x accelerator performance data for wva_profile_grid.  Any pointer may be NULL:
+ * that column is the fleet's own at every level.
+ */
+typedef struct wva_profile_rows {
+    const float *acc_cost;                                            /* [L*A], index l*A + a                */
+    const uint8_t *perf_present;                                      /* [L*M*A], index (l*M + m)*A + a      */
+    const float *perf_alpha, *perf_beta, *perf_gamma, *perf_delta;    /* [L*M*A]                             */
+    const int32_t *perf_acc_count, *perf_max_batch, *perf_at_tokens;  /* [L*M*A]                             */
+} wva_profile_rows;
+
+/*
+ * Profile grid: Server.Calculate (as in wva_analyze) and SolveUnlimited's winner at each of n_levels caller-given
+ * rows of accelerator costs and performance profiles, e.g. a price change, a spot price, an error in the fitted
+ * alpha / beta / gamma / delta, or a new accelerator (listed with perf_present = 0, switched on per row).
+ *
+ * Let f_l be the fleet with acc_cost and the nine perf_* columns replaced by row l of `rows`.  Candidate block l
+ * (records (l*S + s)*A + a) is byte for byte what wva_analyze returns for f_l, value = TransitionPenalty and the
+ * keepAccelerator mask included.  Winner block l (records l*S + s) is wva_solve's winner block for f_l with
+ * unlimited = 1: strict '<' from MaxFloat32, ties to the lower accelerator id.  acc_multiplicity, acc_type, the
+ * capacities and fleet->unlimited are not read; every other column comes from `fleet`.  Each candidate block, with
+ * its level's accelerator table, is a valid input for wva_solve_greedy, which serves limited mode.
+ *
+ * The current allocation's cost is srv_cur_cost as given, not re-priced at row l: in WVA it is the VariantCost
+ * recorded in the variant's status, so block l is the decision at the first reconcile after the price change.
+ *
+ * Deduplication (DESIGN.md §3.14): CreateAllocation reads the accelerator's cost and AccCount only in the cost of
+ * the allocation.  For a pair (s, a) the batch size at level l is N = srv_max_batch, or else
+ * max(perf_max_batch * perf_at_tokens / out_tokens, 1) in 64 bits.  QueueAnalyzer.Size, rateStar, the replica count
+ * and the final Analyze run once per distinct (s, a, bits of alpha, beta, gamma, delta, N) that some level uses as
+ * a load pair; per level only the cost, the value and the minimum run.  A row list that changes only prices sizes
+ * every pair once.
+ *
+ * The fleet becomes resident, as with every call that takes one; wva_summarize returns WVA_ERR_STATE afterwards.
+ * `candidates` (n_levels*S*A entries) may be NULL; `winners` has n_levels*S entries.  n_levels == 0 is valid
+ * (nothing is written).  `rows` NULL means every column is the fleet's own.  WVA_ERR_BAD_ARG: n_levels < 0, fleet
+ * NULL or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_levels >= 2^31 or n_levels*M*A >= 2^31 (refused before the
+ * fleet is read), or exactly the levels on which wva_analyze of f_l fails the same way: a load pair outside the
+ * queue-size rule (a level's perf_max_batch and perf_at_tokens can push N above 2^20), a rescale loop that would
+ * not terminate, or too many stored-vector fallbacks.  Each key is sized only when some level uses it, so the
+ * refusals are the union of the per-level ones.
+ */
+int wva_profile_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const wva_profile_rows *rows,
+                     wva_allocs *candidates, wva_allocs *winners);
+
+/*
  * Load intervals: for each server, the exact float32 arrival rates in [rpm_lo[s], rpm_hi[s]] (req/min) at which
  * wva_load_grid's winner changes its decision, and the winner on each stretch in between.  An autoscaler can
  * skip a re-solve while the load stays inside the current interval, or publish the next scale-up and scale-down

@@ -100,6 +100,12 @@ class IntervalsC(C.Structure):
                 ("rec", AllocsC)]
 
 
+class ProfileRowsC(C.Structure):
+    _fields_ = [("acc_cost", f32p), ("perf_present", u8p), ("perf_alpha", f32p), ("perf_beta", f32p),
+                ("perf_gamma", f32p), ("perf_delta", f32p), ("perf_acc_count", i32p), ("perf_max_batch", i32p),
+                ("perf_at_tokens", i32p)]
+
+
 class GridC(C.Structure):
     _fields_ = [("n_batch", C.c_int32), ("batch", i32p), ("n_replicas", C.c_int32), ("replicas", i32p)]
 

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <cfloat>
 #include <cmath>
 #include <cstdio>
@@ -124,11 +125,16 @@ struct HostFleet {
     int pair_class(int s, int a, bool honour_keep) const { return pair_class(s, a, honour_keep, srv_arrival_rpm[s]); }
     // ... at the arrival rate rpm
     int pair_class(int s, int a, bool honour_keep, float rpm) const {
+        const int m = srv_model[s];
+        return pair_class(s, a, honour_keep, rpm, m >= 0 && m < M && perf_present[(size_t)m * A + a]);
+    }
+    // ... with `present` in place of the model's perf_present at a (the profile grid's rows)
+    int pair_class(int s, int a, bool honour_keep, float rpm, bool present) const {
         if (honour_keep && srv_keep_acc[s] && srv_cur_acc[s] != WVA_ACC_NONE && srv_cur_acc[s] != a) return 0;
         if (rpm < 0.0f || srv_in_tokens[s] < 0 || srv_out_tokens[s] < 0) return 0;
         const int m = srv_model[s];
         if (m < 0 || m >= M) return 0;
-        if (!perf_present[(size_t)m * A + a]) return 0;
+        if (!present) return 0;
         if (!srv_has_target[s]) return 0;
         if (rpm == 0.0f || srv_out_tokens[s] == 0) return PAIR_ZERO;
         return PAIR_LOAD;
@@ -204,6 +210,7 @@ struct wva_handle {
     DevBuf d_lg_star;  // the load grid's rateStar records (shared with the load intervals)
     DevBuf d_iv;       // the load intervals' counts, flags, starts and work list
     DevBuf d_slo;      // the SLO grid's search records
+    DevBuf d_prof;     // the profile grid's key records
 
     // grid path
     DevBuf d_sort, d_best, d_pb, d_rows;
@@ -1180,13 +1187,20 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
 #define WVA_PER_SERVER_T 0
 #define WVA_PER_SERVER_MA 0
 #define WVA_PER_SERVER_S 1
+// ... per (model, accelerator): a key fleet of the profile grid has its own (own_ma).
+#define WVA_PER_MODEL_A 0
+#define WVA_PER_MODEL_T 0
+#define WVA_PER_MODEL_MA 1
+#define WVA_PER_MODEL_S 0
 
 // The fleet the workload grid sizes (DESIGN.md §3.12): row k is server srv[k] of the resident fleet at the key's
 // tokens, with a positive rate (phase 1 reads no rate; the tail reads the level's).  The A, T and M columns are the
 // resident fleet's.  On the device the server columns lie in an upload image of the caller's (place, write), and
-// view() points a copy of the resident DevFleet at them, so the resident arena is never written.
+// view() points a copy of the resident DevFleet at them, so the resident arena is never written.  The profile grid
+// also gives the key fleet its own models (own_ma): M and the perf_* columns are then the key fleet's.
 struct KeyFleet {
     HostFleet hf;
+    bool own_ma = false;
     struct {
 #define KEY_OFFSET(abi, name, type, len) size_t name = 0;
         WVA_FLEET_COLUMNS(KEY_OFFSET)
@@ -1210,20 +1224,22 @@ struct KeyFleet {
     }
     void place(Cols& c) {
 #define KEY_PLACE(abi, name, type, len) \
-    if (WVA_PER_SERVER_##len) off.name = c.take(sizeof(type) * hf.name.size());
+    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) off.name = c.take(sizeof(type) * hf.name.size());
         WVA_FLEET_COLUMNS(KEY_PLACE)
 #undef KEY_PLACE
     }
     void write(char* p) const {
-#define KEY_WRITE(abi, name, type, len) \
-    if (WVA_PER_SERVER_##len && !hf.name.empty()) memcpy(p + off.name, hf.name.data(), sizeof(type) * hf.name.size());
+#define KEY_WRITE(abi, name, type, len)                                              \
+    if ((WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) && !hf.name.empty()) \
+        memcpy(p + off.name, hf.name.data(), sizeof(type) * hf.name.size());
         WVA_FLEET_COLUMNS(KEY_WRITE)
 #undef KEY_WRITE
     }
     DevFleet view(DevFleet f, const char* d) const {
         f.S = hf.S;
+        if (own_ma) f.M = hf.M;
 #define KEY_VIEW(abi, name, type, len) \
-    if (WVA_PER_SERVER_##len) f.name = (const type*)(d + off.name);
+    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) f.name = (const type*)(d + off.name);
         WVA_FLEET_COLUMNS(KEY_VIEW)
 #undef KEY_VIEW
         return f;
@@ -1376,6 +1392,262 @@ int enqueue_workload_trace(wva_handle* h, int L, const float* rpm, const int32_t
     if (rc) return rc;
     if (h->hf.S > 0 && L > 0) {
         trace_kernel<<<(unsigned)((h->hf.S + 127) / 128), 128, 0, h->stream>>>(h->df, cand, winners, L);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- profile grid: CreateAllocation and the unlimited winner at every listed (acc_cost, perf) row (DESIGN.md §3.14)
+// CreateAllocation reads the accelerator's cost and AccCount only in the allocation's cost, so a load pair's record
+// at level l is fixed by the pair and the row's (alpha, beta, gamma, delta, N).  The host ranks the distinct rows of
+// each (m, a) that the levels use (present ones only: elsewhere no pair of m is a load), and builds a key fleet:
+// key-model (m, j) holds the j-th distinct row of (m, a) at every accelerator a that has one, so its tables stay
+// within L * M * A entries, and key row k is server key_srv[k] on one key-model, at the server's own load.  Per load
+// pair (s, a) the rows with equal (alpha .. delta, N) share the lowest j's key.  Phase 1 and the workload grid's tail
+// run on the key fleet with one "level" (its own rates), writing one record per key pair; profile_kernel then writes
+// every level's records and the existing L-block unlimited_kernel the winners.  The lists, the row lists and the key
+// fleet's columns go into lg_tabs, rebuilt on every call.  cand ([L*S*A]) and winners ([L*S]) are device columns.
+int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, const AllocCols& cand,
+                         const AllocCols& winners) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A, M = hf.M;
+    const size_t MA = (size_t)M * A, LA = (size_t)L * A, LMA = (size_t)L * MA;
+    // column c of row l at entry k: the caller's list (bit c of per_level) or the fleet's own
+    const void* const lists[9] = {rows.acc_cost,     rows.perf_present,   rows.perf_alpha,
+                                  rows.perf_beta,    rows.perf_gamma,     rows.perf_delta,
+                                  rows.perf_acc_count, rows.perf_max_batch, rows.perf_at_tokens};
+    unsigned per_level = 0;
+    for (int c = 0; c < 9; ++c) per_level |= lists[c] ? 1u << c : 0u;
+    const bool perf_rows = (per_level >> 1) != 0;
+    auto at = [&](const auto* list, const auto& own, int l, size_t k) { return list ? list[l * MA + k] : own[k]; };
+    auto bits = [](float x) {
+        uint32_t u;
+        memcpy(&u, &x, 4);
+        return u;
+    };
+    using Row = std::array<uint32_t, 6>;  // bits of alpha, beta, gamma, delta; max_batch, at_tokens
+    auto row_of = [&](int l, size_t k) {
+        return Row{bits(at(rows.perf_alpha, hf.perf_alpha, l, k)), bits(at(rows.perf_beta, hf.perf_beta, l, k)),
+                   bits(at(rows.perf_gamma, hf.perf_gamma, l, k)), bits(at(rows.perf_delta, hf.perf_delta, l, k)),
+                   (uint32_t)at(rows.perf_max_batch, hf.perf_max_batch, l, k),
+                   (uint32_t)at(rows.perf_at_tokens, hf.perf_at_tokens, l, k)};
+    };
+    // the distinct present rows of (m, a) = k: row_v[row_off[k] .. row_off[k + 1]), ascending; rank [L*M*A] is row
+    // (l, k)'s index among them (-1: absent), needed only when some perf column is a row list
+    std::vector<Row> row_v;
+    std::vector<int> row_off(MA + 1, 0), rank;
+    if (perf_rows) {
+        rank.assign(LMA, -1);
+        std::vector<std::pair<Row, int>> uses;
+        for (size_t k = 0; k < MA; ++k) {
+            uses.clear();
+            for (int l = 0; l < L; ++l)
+                if (at(rows.perf_present, hf.perf_present, l, k)) uses.emplace_back(row_of(l, k), l);
+            std::sort(uses.begin(), uses.end());
+            for (size_t u = 0; u < uses.size(); ++u) {
+                if (u == 0 || uses[u].first != uses[u - 1].first) row_v.push_back(uses[u].first);
+                rank[(size_t)uses[u].second * MA + k] = (int)row_v.size() - 1 - row_off[k];
+            }
+            row_off[k + 1] = (int)row_v.size();
+        }
+    } else {
+        for (size_t k = 0; k < MA; ++k) {
+            if (L > 0 && hf.perf_present[k]) row_v.push_back(row_of(0, k));
+            row_off[k + 1] = (int)row_v.size();
+        }
+    }
+    // key-model (m, j) = moff[m] + j, j < the most distinct rows of m at any accelerator
+    std::vector<int> moff(M + 1, 0);
+    for (int m = 0; m < M; ++m) {
+        int J = 0;
+        for (int a = 0; a < A; ++a) J = std::max(J, row_off[(size_t)m * A + a + 1] - row_off[(size_t)m * A + a]);
+        moff[m + 1] = moff[m] + J;
+    }
+    // Per load pair (s, a): one key_of entry per distinct row j of (m, a), pointing at the key record of the lowest
+    // row with the same (alpha .. delta, N).  The key rows are (server, key-model) pairs numbered in server order;
+    // need[k * A + a] marks the key pairs phase 1 sizes.
+    std::vector<int> pair_off((size_t)S * A + 1, 0), key_of, key_srv, key_model;
+    std::vector<char> need;
+    std::vector<std::pair<std::array<uint64_t, 3>, int>> groups;  // ((alpha, beta), (gamma, delta), N), j
+    std::vector<int> srv_js;
+    for (int s = 0; s < S; ++s) {
+        const int m = hf.srv_model[s];
+        srv_js.clear();
+        for (int a = 0; a < A; ++a) {
+            const size_t pair = (size_t)s * A + a;
+            pair_off[pair] = (int)key_of.size();
+            // the pair's class at a level where it is present (elsewhere it is nil)
+            if (hf.pair_class(s, a, true, hf.srv_arrival_rpm[s], true) != PAIR_LOAD) continue;
+            const size_t k = (size_t)m * A + a;
+            const int J = row_off[k + 1] - row_off[k], e0 = (int)key_of.size();
+            groups.clear();
+            for (int j = 0; j < J; ++j) {
+                const Row& r = row_v[row_off[k] + j];
+                const long long t = (long long)(int32_t)r[4] * (int32_t)r[5] / hf.srv_out_tokens[s];
+                const long long N = hf.srv_max_batch[s] > 0 ? hf.srv_max_batch[s] : std::max<long long>(t, 1);
+                groups.push_back({{(uint64_t)r[0] << 32 | r[1], (uint64_t)r[2] << 32 | r[3], (uint64_t)N}, j});
+            }
+            std::sort(groups.begin(), groups.end());
+            key_of.resize(key_of.size() + J);  // the representative row for now
+            for (size_t u = 0; u < groups.size(); ++u) {
+                const bool dup = u > 0 && groups[u].first == groups[u - 1].first;
+                const int rep = dup ? key_of[e0 + groups[u - 1].second] : groups[u].second;
+                key_of[e0 + groups[u].second] = rep;
+                if (!dup) srv_js.push_back(rep);
+            }
+        }
+        std::sort(srv_js.begin(), srv_js.end());
+        srv_js.erase(std::unique(srv_js.begin(), srv_js.end()), srv_js.end());
+        const int base = (int)key_srv.size();
+        for (int j : srv_js) {
+            key_srv.push_back(s);
+            key_model.push_back(moff[m] + j);
+        }
+        need.resize(key_srv.size() * A, 0);
+        for (int a = 0; a < A; ++a) {
+            const size_t pair = (size_t)s * A + a;
+            const size_t end = a + 1 < A ? (size_t)pair_off[pair + 1] : key_of.size();
+            for (size_t e = pair_off[pair]; e < end; ++e) {
+                const int kr = base + (int)(std::lower_bound(srv_js.begin(), srv_js.end(), key_of[e]) - srv_js.begin());
+                key_of[e] = kr * A + a;
+                need[(size_t)kr * A + a] = 1;
+            }
+        }
+    }
+    pair_off[(size_t)S * A] = (int)key_of.size();
+    const int K = (int)key_srv.size();  // at most L * S * A key pairs in all (checked by the caller)
+
+    // the key fleet: key row k is server key_srv[k] on key-model key_model[k], at the server's own load
+    std::vector<int> key_in(K), key_out(K);
+    for (int k = 0; k < K; ++k) {
+        key_in[k] = hf.srv_in_tokens[key_srv[k]];
+        key_out[k] = hf.srv_out_tokens[key_srv[k]];
+    }
+    KeyFleet kf(hf, key_srv, key_in, key_out);
+    HostFleet& kh = kf.hf;
+    kf.own_ma = true;
+    for (int k = 0; k < K; ++k) {
+        kh.srv_arrival_rpm[k] = hf.srv_arrival_rpm[key_srv[k]];
+        kh.srv_model[k] = key_model[k];
+    }
+    kh.M = moff[M];
+    const size_t KMA = (size_t)kh.M * A;
+    kh.perf_present.assign(KMA, 0);
+    kh.perf_acc_count.assign(KMA, 1);
+    for (auto* col : {&kh.perf_alpha, &kh.perf_beta, &kh.perf_gamma, &kh.perf_delta}) col->assign(KMA, 0.0f);
+    kh.perf_max_batch.assign(KMA, 0);
+    kh.perf_at_tokens.assign(KMA, 0);
+    for (int m = 0; m < M; ++m)
+        for (int a = 0; a < A; ++a) {
+            const size_t k = (size_t)m * A + a;
+            for (int j = 0; j < row_off[k + 1] - row_off[k]; ++j) {
+                const Row& r = row_v[row_off[k] + j];
+                const size_t q = (size_t)(moff[m] + j) * A + a;
+                kh.perf_present[q] = 1;
+                memcpy(&kh.perf_alpha[q], &r[0], 4);
+                memcpy(&kh.perf_beta[q], &r[1], 4);
+                memcpy(&kh.perf_gamma[q], &r[2], 4);
+                memcpy(&kh.perf_delta[q], &r[3], 4);
+                kh.perf_max_batch[q] = (int32_t)r[4];
+                kh.perf_at_tokens[q] = (int32_t)r[5];
+            }
+        }
+    std::vector<int> pairs, Ns;
+    int rc = sorted_pairs(h, kh, [&](int k, int a) { return need[(size_t)k * A + a] != 0; }, pairs, Ns);
+    if (rc) return rc;
+    const int n = (int)pairs.size();
+
+    // the key records: one per key pair, written by the workload grid's tail
+    const Block kb = block_layout((size_t)K * A);
+    CK(h->d_prof.ensure(kb.bytes + 16));
+    const AllocCols key = block_cols(h->d_prof.p, kb);
+
+    Cols c(16);
+    kf.place(c);
+    static const size_t elem[9] = {4, 1, 4, 4, 4, 4, 4, 4, 4};
+    size_t o_list[9] = {};
+    for (int b = 0; b < 9; ++b)
+        if (lists[b]) o_list[b] = c.take(elem[b] * (b == 0 ? LA : LMA));
+    const size_t o_rank = c.take(4 * rank.size()), o_poff = c.take(4 * pair_off.size()),
+                 o_keyof = c.take(4 * key_of.size()), o_ksrv = c.take(4 * (size_t)K),
+                 o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * (size_t)K),
+                 o_item = c.take(4 * ((size_t)n + 1));
+    rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
+        kf.write(p);
+        for (int b = 0; b < 9; ++b)
+            if (lists[b] && L) memcpy(p + o_list[b], lists[b], elem[b] * (b == 0 ? LA : LMA));
+        if (!rank.empty()) memcpy(p + o_rank, rank.data(), 4 * rank.size());
+        memcpy(p + o_poff, pair_off.data(), 4 * pair_off.size());
+        if (!key_of.empty()) memcpy(p + o_keyof, key_of.data(), 4 * key_of.size());
+        // the tail's one level: key k is server k of the key fleet, candidate e item e
+        int* ksrv = (int*)(p + o_ksrv);
+        int* loff = (int*)(p + o_loff);
+        int* item = (int*)(p + o_item);
+        std::iota(ksrv, ksrv + K, 0);
+        std::iota(loff, loff + K + 1, 0);
+        memset(p + o_lev, 0, 4 * (size_t)K);
+        std::iota(item, item + n + 1, 0);
+    });
+    if (rc) return rc;
+    const char* d = (const char*)h->lg_tabs.lists.p;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const DevFleet kd = kf.view(h->df, d);
+    LoadStar ls;
+    rc = enqueue_load_star(h, kh, kd, n, ls);
+    if (rc) return rc;
+    if (n > 0) {
+        WorkloadArgs g{};
+        g.ld = load_args(ls);
+        g.ld.level_rpm = kd.srv_arrival_rpm;
+        g.ld.L = 1;
+        g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+        g.ld.cand = key;
+        g.key_srv = (const int*)(d + o_ksrv);
+        g.lev_off = (const int*)(d + o_loff);
+        g.lev = (const int*)(d + o_lev);
+        g.item_off = (const int*)(d + o_item);
+        g.S = K;
+        g.n_items = n;
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, workload_kernel, 256, 0));
+        per_sm = std::max(1, std::min(per_sm, 8));
+        const long long warps = ((long long)n + 31) / 32;
+        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
+        workload_kernel<<<blocks, 256, 0, h->stream>>>(g);
+        h->launches++;
+        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
+        launch_fallback(h, workload_fallback, g, ls.fb2);
+    }
+    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
+    if (n_rec > 0) {
+        ProfileArgs g{};
+        g.f = h->df;
+        g.rows = h->df;
+        const auto row = [&](int b) { return (const void*)(d + o_list[b]); };
+        if (rows.acc_cost) g.rows.acc_cost = (const float*)row(0);
+        if (rows.perf_present) g.rows.perf_present = (const uint8_t*)row(1);
+        if (rows.perf_alpha) g.rows.perf_alpha = (const float*)row(2);
+        if (rows.perf_beta) g.rows.perf_beta = (const float*)row(3);
+        if (rows.perf_gamma) g.rows.perf_gamma = (const float*)row(4);
+        if (rows.perf_delta) g.rows.perf_delta = (const float*)row(5);
+        if (rows.perf_acc_count) g.rows.perf_acc_count = (const int32_t*)row(6);
+        if (rows.perf_max_batch) g.rows.perf_max_batch = (const int32_t*)row(7);
+        if (rows.perf_at_tokens) g.rows.perf_at_tokens = (const int32_t*)row(8);
+        g.per_level = per_level;
+        g.rank = perf_rows ? (const int*)(d + o_rank) : nullptr;
+        g.pair_off = (const int*)(d + o_poff);
+        g.key_of = (const int*)(d + o_keyof);
+        g.key = key;
+        g.cand = cand;
+        g.L = L;
+        profile_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(g);
+        h->launches++;
+    }
+    if (S > 0 && L > 0) {
+        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
+            h->df, cand, winners, L);
         h->launches++;
     }
     CK(cudaGetLastError());
@@ -2313,6 +2585,30 @@ int wva_workload_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, c
     c.win_blocks = (size_t)n_ticks;
     rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
         return enqueue_workload_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens, dc, dw);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
+int wva_profile_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const wva_profile_rows* rows,
+                     wva_allocs* candidates, wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31) ||
+        (long long)n_levels * fleet->n_models * fleet->n_acc >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "profile grid too large for one call (>= 2^31 candidates or row entries)");
+    const wva_profile_rows own{};
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
+    c.win_blocks = (size_t)n_levels;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_profile_grid(h, n_levels, rows ? *rows : own, dc, dw);
     });
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;

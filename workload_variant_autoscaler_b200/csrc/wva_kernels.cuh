@@ -9,6 +9,7 @@
 //                       wva_workload_grid)
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
 //   trace_kernel        the same tick by tick, each tick's winner the next tick's current allocation
+//   profile_kernel      the profile grid's records per (level, pair) from the key records, priced at the level
 //   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
 //
@@ -1692,6 +1693,61 @@ __global__ void trace_kernel(DevFleet f, AllocCols cand, AllocCols winners, int 
             cur_cost = best.cost;
         }
     }
+}
+
+// The profile grid's records (DESIGN.md §3.14): L level blocks of S * A records (record (l * S + s) * A + a), one
+// thread per record.  f_l is f with acc_cost and the perf_* columns of row l (profile_at).  A pair is classed at f_l:
+// nil, zeroLoadAllocation at f_l, or, under load, the record its key was sized to on the key fleet (the row's
+// alpha .. delta and N), with cost = acc_cost_l[a] * NumInstances_l * replicas, the only field that reads the row's
+// cost or AccCount (S * A * L < 2^31, checked on the host).
+struct ProfileArgs {
+    DevFleet f;           // the resident fleet
+    DevFleet rows;        // acc_cost and perf_* at level 0: the caller's row lists, or the fleet's own columns ...
+    unsigned per_level;   // ... bit c (0: acc_cost, 1 .. 8: perf_* in list order) set: column c is a row list
+    const int* rank;      // [L * M * A] the row's index among the distinct rows of (m, a); NULL: 0 everywhere
+    const int* pair_off;  // [S * A] the pair's first entry in key_of, one entry per distinct row of (m, a)
+    const int* key_of;    // the key record of (pair, row index); read only where the pair is a load
+    AllocCols key;        // the key fleet's records
+    AllocCols cand;       // [L * S * A]
+    int L;
+};
+__device__ __forceinline__ DevFleet profile_at(const ProfileArgs& g, int l) {
+    DevFleet fl = g.f;
+    const size_t ra = (size_t)l * g.f.A, rma = (size_t)l * g.f.M * g.f.A;
+    fl.acc_cost = g.rows.acc_cost + (g.per_level & 1u ? ra : 0);
+#define WVA_PROFILE_ROW(name, bit) fl.name = g.rows.name + (g.per_level >> bit & 1u ? rma : 0);
+    WVA_PROFILE_ROW(perf_present, 1)
+    WVA_PROFILE_ROW(perf_alpha, 2)
+    WVA_PROFILE_ROW(perf_beta, 3)
+    WVA_PROFILE_ROW(perf_gamma, 4)
+    WVA_PROFILE_ROW(perf_delta, 5)
+    WVA_PROFILE_ROW(perf_acc_count, 6)
+    WVA_PROFILE_ROW(perf_max_batch, 7)
+    WVA_PROFILE_ROW(perf_at_tokens, 8)
+#undef WVA_PROFILE_ROW
+    return fl;
+}
+__global__ void profile_kernel(ProfileArgs g) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n_pairs = g.f.S * g.f.A;
+    if (i >= n_pairs * g.L) return;
+    const int l = i / n_pairs, pair = i - l * n_pairs;
+    const int s = pair / g.f.A, a = pair % g.f.A;
+    const DevFleet fl = profile_at(g, l);
+    const int cls = pair_class(fl, s, a, true);
+    Cand c = cand_nil();
+    if (cls == PAIR_ZERO) {
+        c = zero_load_alloc(fl, s, a);
+    } else if (cls == PAIR_LOAD) {
+        const int m = fl.srv_model[s];
+        const int j = g.rank ? g.rank[((size_t)l * fl.M + m) * fl.A + a] : 0;
+        c = load_cand(g.key, g.key_of[g.pair_off[pair] + j]);
+        if (c.feasible) {
+            c.cost = __fmul_rn(fl.acc_cost[a], (float)((long long)num_instances(fl, m, a) * (long long)c.replicas));
+            c.value = c.cost;
+        }
+    }
+    store_cand(g.cand, i, c);
 }
 
 // wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record

@@ -234,6 +234,49 @@ class Engine:
                          C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
+    def profile_grid(self, fleet: Fleet, *, acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None,
+                     perf_gamma=None, perf_delta=None, perf_acc_count=None, perf_max_batch=None, perf_at_tokens=None,
+                     want_candidates: bool = False, out: Allocs | None = None):
+        """The reference's ``Server.Calculate`` and ``SolveUnlimited`` winner at each row of accelerator costs
+        (``acc_cost``, shape (L, A)) and performance profiles (``perf_*``, shape (L, M, A)) -> (candidates
+        [L*S*A] | None, winners [L*S]), both level-major.
+
+        Candidate block ``l`` is what ``analyze`` returns for the fleet with ``acc_cost`` and the ``perf_*`` columns
+        = row ``l``, and winner block ``l`` is ``solve``'s winners for it in unlimited mode; each distinct (server,
+        accelerator, alpha, beta, gamma, delta, batch size) is sized once (see ``wva_profile_grid`` in
+        include/wva_b200.h).  A column of ``None`` is the fleet's own at every level; at least one must be given,
+        and L is their row count.  ``srv_cur_cost`` is not re-priced.  ``out``: an ``Allocs`` of ``L * S`` records
+        to write the winners into."""
+        S, A, M = fleet.n_servers, fleet.n_acc, fleet.n_models
+        given = {"acc_cost": acc_cost, "perf_present": perf_present, "perf_alpha": perf_alpha,
+                 "perf_beta": perf_beta, "perf_gamma": perf_gamma, "perf_delta": perf_delta,
+                 "perf_acc_count": perf_acc_count, "perf_max_batch": perf_max_batch, "perf_at_tokens": perf_at_tokens}
+        dtypes = {name: dt for name, dt, _ in _abi.FLEET_COLUMNS}
+        rows, L = {}, None
+        for name, x in given.items():
+            if x is None:
+                continue
+            r = np.ascontiguousarray(x, dtypes[name])
+            tail = (A,) if name == "acc_cost" else (M, A)
+            if r.ndim != 1 + len(tail) or r.shape[1:] != tail or (L is not None and r.shape[0] != L):
+                want = "L" if L is None else str(L)
+                raise ValueError(f"{name} must have shape ({want}, {', '.join(map(str, tail))}), got {r.shape}")
+            L = r.shape[0]
+            rows[name] = r
+        if L is None:
+            raise ValueError("profile_grid needs at least one row list")
+        if out is not None and out.n != L * S:
+            raise ValueError("out must hold L * fleet.n_servers records")
+        win = out if out is not None else Allocs(L * S)
+        cand = Allocs(L * S * A) if want_candidates else None
+        rc_ = _abi.ProfileRowsC(*[_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in given])
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_profile_grid(self._h, C.byref(fc), L, C.byref(rc_),
+                                             C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
+
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
         """Where each server's ``load_grid`` winner changes its decision in ``[rpm_lo[s], rpm_hi[s]]`` (req/min)
         -> (count [S], truncated [S], start_rpm (S, M), records: ``Allocs`` of S * M).
