@@ -448,6 +448,49 @@ int wva_profile_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, co
                      wva_allocs *candidates, wva_allocs *winners);
 
 /*
+ * Profile trace: wva_workload_trace over ticks that also carry accelerator costs and performance profiles, e.g.
+ * hourly spot or time-of-use prices, an accelerator brought online or withdrawn at some tick (perf_present), or a
+ * serving-stack upgrade that lowers beta from some tick on.
+ *
+ * Let f_t be the fleet with srv_arrival_rpm, srv_in_tokens and srv_out_tokens replaced by row t of the three
+ * workload lists ([L*S], index t*S + s; a NULL list is the fleet's own column at every tick), acc_cost and the nine
+ * perf_* columns by row t of `rows` (wva_profile_rows' layout; a NULL column, or rows NULL, is the fleet's own), and
+ * the current allocation (srv_cur_acc, srv_cur_replicas, srv_cur_cost) by c_t.
+ *   - c_0 is the fleet's current allocation, not re-priced (in WVA it is the recorded VariantCost).
+ *   - Candidate block t (records (t*S + s)*A + a) is byte for byte what wva_analyze returns for f_t, value =
+ *     TransitionPenalty against c_t and the keepAccelerator mask against c_t included.
+ *   - Winner block t (records t*S + s) is byte for byte wva_solve's winner block for f_t with unlimited = 1.
+ *   - c_{t+1} is winner t's (acc, replicas, cost) when that winner is feasible, and c_t otherwise.  The cost carried
+ *     forward is the winner's at tick t's prices (Server.ApplyDesiredAlloc), so the penalty at tick t+1 compares a
+ *     cost recorded at the old prices with candidates priced at the new ones, as the controller does.
+ * Only unlimited mode is traced; fleet->unlimited, the capacities, acc_type and acc_multiplicity are not read.  A
+ * trace can be continued as wva_workload_trace's: the trace over ticks 0..L-1 equals the trace over 0..k-1 followed
+ * by the trace over k..L-1 on the fleet whose srv_cur_* columns hold c_k.  With every profile column NULL the call
+ * returns wva_workload_trace's result; with one tick it returns wva_profile_grid's for that row (on the fleet's own
+ * load when the workload lists are NULL).
+ *
+ * Sizing (DESIGN.md §3.15): a load pair's record at tick t is fixed by (s, a, in_t, out_t, bits of alpha, beta,
+ * gamma, delta and N at row t); the price and AccCount of row t enter only its cost.  Each distinct such key that some
+ * tick uses as a load pair is sized once, in one batched pass, and only the chain runs tick by tick.  As in
+ * wva_workload_trace, a pinned server sizes only its current pair and every other server sizes all its pairs,
+ * keepAccelerator ignored.
+ *
+ * The fleet becomes resident; wva_summarize returns WVA_ERR_STATE afterwards.  `candidates` (n_ticks*S*A entries)
+ * may be NULL; `winners` has n_ticks*S entries.  n_ticks == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG:
+ * n_ticks < 0, fleet NULL or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_ticks >= 2^31 or n_ticks*M*A >= 2^31 (refused
+ * before the fleet is read), or the union over ticks of wva_analyze(f_t)'s failures for the pairs the call sizes: a
+ * load pair outside the queue-size rule (a tick's perf_max_batch, perf_at_tokens or out_tokens can push N above
+ * 2^20), a rescale loop that would not terminate, or too many stored-vector fallbacks.  As with wva_workload_trace,
+ * these can exceed the per-tick refusals only through the pairs of keep servers that are not pinned, and the result
+ * never differs from the per-tick composition.  With a perf column the call also refuses when its distinct keys times
+ * A reach 2^31 (at most S*A*n_ticks keys, so only with A*A*S*n_ticks >= 2^31); split the ticks over several calls
+ * (continuation).
+ */
+int wva_profile_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                      const int32_t *in_tokens, const int32_t *out_tokens, const wva_profile_rows *rows,
+                      wva_allocs *candidates, wva_allocs *winners);
+
+/*
  * Load intervals: for each server, the exact float32 arrival rates in [rpm_lo[s], rpm_hi[s]] (req/min) at which
  * wva_load_grid's winner changes its decision, and the winner on each stretch in between.  An autoscaler can
  * skip a re-solve while the load stays inside the current interval, or publish the next scale-up and scale-down

@@ -41,7 +41,7 @@ EXPORTS = (
     "wva_last_kernel_ms", "wva_last_device_ms", "wva_summarize", "wva_solve_greedy", "wva_mm1k_solve",
     "wva_xchg_create", "wva_xchg_open", "wva_xchg_publish", "wva_xchg_error", "wva_xchg_destroy", "wva_size_grid",
     "wva_load_grid", "wva_load_intervals", "wva_slo_grid", "wva_workload_grid", "wva_workload_trace",
-    "wva_profile_grid",
+    "wva_profile_grid", "wva_profile_trace",
 )
 
 _lib = None
@@ -81,6 +81,8 @@ def lib():
                                 C.POINTER(_abi.AllocsC)]),
         ("wva_profile_grid", [vp, C.POINTER(_abi.FleetC), i32, C.POINTER(_abi.ProfileRowsC), C.POINTER(_abi.AllocsC),
                               C.POINTER(_abi.AllocsC)]),
+        ("wva_profile_trace", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p, C.POINTER(_abi.ProfileRowsC),
+                               C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
         ("wva_sweep", [vp, C.POINTER(_abi.FleetC), i32, C.POINTER(_abi.SweepOutC)]),
         ("wva_upload", [vp, C.POINTER(_abi.FleetC)]),
         ("wva_update_load", [vp, f32p, i32p, i32p]),

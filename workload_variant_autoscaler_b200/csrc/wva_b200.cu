@@ -1255,6 +1255,72 @@ bool trace_pinned(const HostFleet& hf, int s) {
     return hf.srv_keep_acc[s] && cur != WVA_ACC_NONE && (cur == WVA_ACC_UNKNOWN || hf.srv_min_replicas[s] != 0);
 }
 
+// The workload grid's tail (workload_kernel, then workload_fallback) after phase 1 (ls): g's key and level lists and
+// g.n_items items, at the rates level_rpm [L * g.S], into cand.  ev_k1 is recorded after workload_kernel: the
+// call's kernel time covers both phases.
+int enqueue_workload_tail(wva_handle* h, const LoadStar& ls, WorkloadArgs& g, const float* level_rpm, int L,
+                          const AllocCols& cand) {
+    if (g.n_items <= 0) return WVA_OK;
+    g.ld = load_args(ls);
+    g.ld.level_rpm = level_rpm;
+    g.ld.L = L;
+    g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+    g.ld.cand = cand;
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, workload_kernel, 256, 0));
+    per_sm = std::max(1, std::min(per_sm, 8));
+    const long long warps = ((long long)g.n_items + 31) / 32;
+    const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
+    workload_kernel<<<blocks, 256, 0, h->stream>>>(g);
+    h->launches++;
+    CK(cudaEventRecord(h->ev_k1, h->stream));
+    launch_fallback(h, workload_fallback, g, ls.fb2);
+    return WVA_OK;
+}
+
+// The levels at which server s is a load under the rows rpm / in / out [L*S] (rate not negative and not 0, NaN and
+// +Inf included; in_tokens >= 0; out_tokens >= 1), as ((in << 32) | out, level) in `uses`, sorted; then
+// group(in, out, u0, u1) for each (in, out) in ascending order, whose levels are uses[u0 .. u1), ascending.
+template <class Group>
+void load_groups(int L, int S, int s, const float* rpm, const int32_t* in, const int32_t* out,
+                 std::vector<std::pair<uint64_t, int>>& uses, Group&& group) {
+    uses.clear();
+    for (int l = 0; l < L; ++l) {
+        const size_t i = (size_t)l * S + s;
+        if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1)
+            uses.emplace_back((uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], l);
+    }
+    std::sort(uses.begin(), uses.end());
+    for (size_t u0 = 0, u1; u0 < uses.size(); u0 = u1) {
+        for (u1 = u0; u1 < uses.size() && uses[u1].first == uses[u0].first;) ++u1;
+        group((int)(uses[u0].first >> 32), (int)(uint32_t)uses[u0].first, u0, u1);
+    }
+}
+
+// Key rows (server, in_tokens, out_tokens) with their levels: row k's are lev[lev_off[k] .. lev_off[k + 1]).
+struct TokenKeys {
+    std::vector<int> srv, in, out, lev_off{0}, lev;
+    void add(int s, int ki, int ko) {
+        srv.push_back(s);
+        in.push_back(ki);
+        out.push_back(ko);
+        lev_off.push_back(lev_off.back());
+    }
+    void add_level(int l) {
+        lev.push_back(l);
+        lev_off.back()++;
+    }
+};
+// The workload grid's keys (DESIGN.md §3.12): per server, its distinct (in, out) under load, ascending.
+void token_keys(int L, int S, const float* rpm, const int32_t* in, const int32_t* out, TokenKeys& tk) {
+    std::vector<std::pair<uint64_t, int>> uses;
+    for (int s = 0; s < S; ++s)
+        load_groups(L, S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
+            tk.add(s, ki, ko);
+            for (size_t u = u0; u < u1; ++u) tk.add_level(uses[u].second);
+        });
+}
+
 // QueueAnalyzer.Size, lambda* and rateStar read a server's tokens but not its rate (DESIGN.md §3.12), so phase 1
 // is the load grid's, run once on the key fleet: one row per distinct (server, in_tokens, out_tokens) that some
 // level uses under load (rate not negative and not 0, NaN and +Inf included; in_tokens >= 0; out_tokens >= 1).
@@ -1270,31 +1336,12 @@ int enqueue_workload_sizing(wva_handle* h, int L, const float* rpm, const int32_
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     const size_t LS = (size_t)L * S;
-    // the keys: per server, its distinct (in, out) in ascending order; key k's levels are lev[lev_off[k] ..
-    // lev_off[k + 1]), ascending.  There are at most L * S keys, so fewer than 2^31 key candidates.
-    std::vector<int> key_srv, key_in, key_out, lev_off{0}, lev;
-    std::vector<std::pair<uint64_t, int>> uses;  // ((in << 32) | out, level)
-    for (int s = 0; s < S; ++s) {
-        uses.clear();
-        for (int l = 0; l < L; ++l) {
-            const size_t i = (size_t)l * S + s;
-            if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1)
-                uses.emplace_back((uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], l);
-        }
-        std::sort(uses.begin(), uses.end());
-        for (size_t u = 0; u < uses.size(); ++u) {
-            if (u == 0 || uses[u].first != uses[u - 1].first) {
-                key_srv.push_back(s);
-                key_in.push_back((int)(uses[u].first >> 32));
-                key_out.push_back((int)(uint32_t)uses[u].first);
-                lev_off.push_back(lev_off.back());
-            }
-            lev.push_back(uses[u].second);
-            lev_off.back()++;
-        }
-    }
+    // the keys: at most L * S, so fewer than 2^31 key candidates
+    TokenKeys tk;
+    token_keys(L, S, rpm, in, out, tk);
+    const std::vector<int>&key_srv = tk.srv, &lev_off = tk.lev_off, &lev = tk.lev;
     const int K = (int)key_srv.size();
-    KeyFleet kf(hf, key_srv, key_in, key_out);
+    KeyFleet kf(hf, key_srv, tk.in, tk.out);
     if (trace)
         for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, key_srv[k]);
     Cols c(16);
@@ -1341,29 +1388,15 @@ int enqueue_workload_sizing(wva_handle* h, int L, const float* rpm, const int32_
     LoadStar ls;
     rc = enqueue_load_star(h, kf.hf, kf.view(h->df, d), n_items, ls);
     if (rc) return rc;
-    if (n_items > 0) {
-        WorkloadArgs g{};
-        g.ld = load_args(ls);
-        g.ld.level_rpm = d_rpm;
-        g.ld.L = L;
-        g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
-        g.ld.cand = cand;
-        g.key_srv = (const int*)(d + o_ksrv);
-        g.lev_off = (const int*)(d + o_loff);
-        g.lev = (const int*)(d + o_lev);
-        g.item_off = (const int*)(d + o_item);
-        g.S = S;
-        g.n_items = n_items;
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, workload_kernel, 256, 0));
-        per_sm = std::max(1, std::min(per_sm, 8));
-        const long long warps = ((long long)n_items + 31) / 32;
-        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
-        workload_kernel<<<blocks, 256, 0, h->stream>>>(g);
-        h->launches++;
-        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
-        launch_fallback(h, workload_fallback, g, ls.fb2);
-    }
+    WorkloadArgs g{};
+    g.key_srv = (const int*)(d + o_ksrv);
+    g.lev_off = (const int*)(d + o_loff);
+    g.lev = (const int*)(d + o_lev);
+    g.item_off = (const int*)(d + o_item);
+    g.S = S;
+    g.n_items = n_items;
+    rc = enqueue_workload_tail(h, ls, g, d_rpm, L, cand);
+    if (rc) return rc;
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1408,62 +1441,142 @@ int enqueue_workload_trace(wva_handle* h, int L, const float* rpm, const int32_t
 // run on the key fleet with one "level" (its own rates), writing one record per key pair; profile_kernel then writes
 // every level's records and the existing L-block unlimited_kernel the winners.  The lists, the row lists and the key
 // fleet's columns go into lg_tabs, rebuilt on every call.  cand ([L*S*A]) and winners ([L*S]) are device columns.
+// The rows of a wva_profile_rows list as the profile grid and the profile trace size them.  Per (m, a) the host ranks
+// the distinct present rows that the levels use (elsewhere no pair of m is a load); key-model (m, j) = moff[m] + j
+// holds the j-th distinct row of (m, a) at every accelerator a that has one, so a key fleet's tables stay within
+// L * M * A entries.  The caller's row lists travel in the call's upload image (place, write), and set_rows points
+// a ProfileArgs at them.
+struct ProfileRanks {
+    using Row = std::array<uint32_t, 6>;  // bits of alpha, beta, gamma, delta; max_batch, at_tokens
+    const void* lists[9];                 // column c: the caller's row list (bit c of per_level) or NULL
+    unsigned per_level = 0;
+    bool perf_rows = false;               // some perf column is a row list
+    int L, A;
+    size_t MA;
+    // the distinct present rows of (m, a) = k: row_v[row_off[k] .. row_off[k + 1]), ascending; rank [L*M*A] is row
+    // (l, k)'s index among them (-1: absent), built only when perf_rows
+    std::vector<Row> row_v;
+    std::vector<int> row_off, rank;
+    std::vector<int> moff;  // [M + 1]: key-model (m, j) = moff[m] + j, j < the most distinct rows of m at any a
+    size_t o_list[9] = {};
+
+    ProfileRanks(const HostFleet& hf, int L_, const wva_profile_rows& rows)
+        : lists{rows.acc_cost,  rows.perf_present,   rows.perf_alpha,     rows.perf_beta,     rows.perf_gamma,
+                rows.perf_delta, rows.perf_acc_count, rows.perf_max_batch, rows.perf_at_tokens},
+          L(L_), A(hf.A), MA((size_t)hf.M * hf.A), row_off(MA + 1, 0), moff(hf.M + 1, 0) {
+        for (int c = 0; c < 9; ++c) per_level |= lists[c] ? 1u << c : 0u;
+        perf_rows = (per_level >> 1) != 0;
+        // column c of row l at entry k
+        auto at = [&](const auto* list, const auto& own, int l, size_t k) { return list ? list[l * MA + k] : own[k]; };
+        auto bits = [](float x) {
+            uint32_t u;
+            memcpy(&u, &x, 4);
+            return u;
+        };
+        auto row_of = [&](int l, size_t k) {
+            return Row{bits(at(rows.perf_alpha, hf.perf_alpha, l, k)), bits(at(rows.perf_beta, hf.perf_beta, l, k)),
+                       bits(at(rows.perf_gamma, hf.perf_gamma, l, k)), bits(at(rows.perf_delta, hf.perf_delta, l, k)),
+                       (uint32_t)at(rows.perf_max_batch, hf.perf_max_batch, l, k),
+                       (uint32_t)at(rows.perf_at_tokens, hf.perf_at_tokens, l, k)};
+        };
+        if (perf_rows) {
+            rank.assign((size_t)L * MA, -1);
+            std::vector<std::pair<Row, int>> uses;
+            for (size_t k = 0; k < MA; ++k) {
+                uses.clear();
+                for (int l = 0; l < L; ++l)
+                    if (at(rows.perf_present, hf.perf_present, l, k)) uses.emplace_back(row_of(l, k), l);
+                std::sort(uses.begin(), uses.end());
+                for (size_t u = 0; u < uses.size(); ++u) {
+                    if (u == 0 || uses[u].first != uses[u - 1].first) row_v.push_back(uses[u].first);
+                    rank[(size_t)uses[u].second * MA + k] = (int)row_v.size() - 1 - row_off[k];
+                }
+                row_off[k + 1] = (int)row_v.size();
+            }
+        } else {
+            for (size_t k = 0; k < MA; ++k) {
+                if (L > 0 && hf.perf_present[k]) row_v.push_back(row_of(0, k));
+                row_off[k + 1] = (int)row_v.size();
+            }
+        }
+        for (int m = 0; m < hf.M; ++m) {
+            int J = 0;
+            for (int a = 0; a < A; ++a) J = std::max(J, row_off[(size_t)m * A + a + 1] - row_off[(size_t)m * A + a]);
+            moff[m + 1] = moff[m] + J;
+        }
+    }
+    // row (l, k)'s index among the distinct rows of k, -1 where (m, a) is absent at row l
+    int rank_at(int l, size_t k) const {
+        if (perf_rows) return rank[(size_t)l * MA + k];
+        return row_off[k + 1] > row_off[k] ? 0 : -1;
+    }
+    // What a load pair's sizing reads of row j of k = (m, a): ((alpha, beta), (gamma, delta), N), N being the
+    // server's batch size max_batch when positive and the row's AtTokens rule at out_tokens out otherwise.
+    std::array<uint64_t, 3> sizing_key(size_t k, int j, int max_batch, int out) const {
+        const Row& r = row_v[row_off[k] + j];
+        const long long t = (long long)(int32_t)r[4] * (int32_t)r[5] / out;
+        const long long N = max_batch > 0 ? max_batch : std::max<long long>(t, 1);
+        return {(uint64_t)r[0] << 32 | r[1], (uint64_t)r[2] << 32 | r[3], (uint64_t)N};
+    }
+    // the key fleet's models: M and the perf columns of the key-models (kh starts as a copy of the fleet)
+    void fill(HostFleet& kh) const {
+        kh.M = moff.back();
+        const size_t KMA = (size_t)kh.M * A;
+        kh.perf_present.assign(KMA, 0);
+        kh.perf_acc_count.assign(KMA, 1);
+        for (auto* col : {&kh.perf_alpha, &kh.perf_beta, &kh.perf_gamma, &kh.perf_delta}) col->assign(KMA, 0.0f);
+        kh.perf_max_batch.assign(KMA, 0);
+        kh.perf_at_tokens.assign(KMA, 0);
+        for (size_t m = 0; m + 1 < moff.size(); ++m)
+            for (int a = 0; a < A; ++a) {
+                const size_t k = m * A + a;
+                for (int j = 0; j < row_off[k + 1] - row_off[k]; ++j) {
+                    const Row& r = row_v[row_off[k] + j];
+                    const size_t q = (size_t)(moff[m] + j) * A + a;
+                    kh.perf_present[q] = 1;
+                    memcpy(&kh.perf_alpha[q], &r[0], 4);
+                    memcpy(&kh.perf_beta[q], &r[1], 4);
+                    memcpy(&kh.perf_gamma[q], &r[2], 4);
+                    memcpy(&kh.perf_delta[q], &r[3], 4);
+                    kh.perf_max_batch[q] = (int32_t)r[4];
+                    kh.perf_at_tokens[q] = (int32_t)r[5];
+                }
+            }
+    }
+    size_t list_bytes(int c) const {
+        static const size_t elem[9] = {4, 1, 4, 4, 4, 4, 4, 4, 4};
+        return elem[c] * (size_t)L * (c == 0 ? (size_t)A : MA);
+    }
+    void place(Cols& c) {
+        for (int b = 0; b < 9; ++b)
+            if (lists[b]) o_list[b] = c.take(list_bytes(b));
+    }
+    void write(char* p) const {
+        for (int b = 0; b < 9; ++b)
+            if (lists[b] && L) memcpy(p + o_list[b], lists[b], list_bytes(b));
+    }
+    // g.rows: g.f with the row lists uploaded at d, and per_level
+    void set_rows(ProfileArgs& g, const char* d) const {
+        g.rows = g.f;
+        const auto row = [&](int b) { return (const void*)(d + o_list[b]); };
+        if (lists[0]) g.rows.acc_cost = (const float*)row(0);
+        if (lists[1]) g.rows.perf_present = (const uint8_t*)row(1);
+        if (lists[2]) g.rows.perf_alpha = (const float*)row(2);
+        if (lists[3]) g.rows.perf_beta = (const float*)row(3);
+        if (lists[4]) g.rows.perf_gamma = (const float*)row(4);
+        if (lists[5]) g.rows.perf_delta = (const float*)row(5);
+        if (lists[6]) g.rows.perf_acc_count = (const int32_t*)row(6);
+        if (lists[7]) g.rows.perf_max_batch = (const int32_t*)row(7);
+        if (lists[8]) g.rows.perf_at_tokens = (const int32_t*)row(8);
+        g.per_level = per_level;
+    }
+};
+
 int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, const AllocCols& cand,
                          const AllocCols& winners) {
     const HostFleet& hf = h->hf;
-    const int S = hf.S, A = hf.A, M = hf.M;
-    const size_t MA = (size_t)M * A, LA = (size_t)L * A, LMA = (size_t)L * MA;
-    // column c of row l at entry k: the caller's list (bit c of per_level) or the fleet's own
-    const void* const lists[9] = {rows.acc_cost,     rows.perf_present,   rows.perf_alpha,
-                                  rows.perf_beta,    rows.perf_gamma,     rows.perf_delta,
-                                  rows.perf_acc_count, rows.perf_max_batch, rows.perf_at_tokens};
-    unsigned per_level = 0;
-    for (int c = 0; c < 9; ++c) per_level |= lists[c] ? 1u << c : 0u;
-    const bool perf_rows = (per_level >> 1) != 0;
-    auto at = [&](const auto* list, const auto& own, int l, size_t k) { return list ? list[l * MA + k] : own[k]; };
-    auto bits = [](float x) {
-        uint32_t u;
-        memcpy(&u, &x, 4);
-        return u;
-    };
-    using Row = std::array<uint32_t, 6>;  // bits of alpha, beta, gamma, delta; max_batch, at_tokens
-    auto row_of = [&](int l, size_t k) {
-        return Row{bits(at(rows.perf_alpha, hf.perf_alpha, l, k)), bits(at(rows.perf_beta, hf.perf_beta, l, k)),
-                   bits(at(rows.perf_gamma, hf.perf_gamma, l, k)), bits(at(rows.perf_delta, hf.perf_delta, l, k)),
-                   (uint32_t)at(rows.perf_max_batch, hf.perf_max_batch, l, k),
-                   (uint32_t)at(rows.perf_at_tokens, hf.perf_at_tokens, l, k)};
-    };
-    // the distinct present rows of (m, a) = k: row_v[row_off[k] .. row_off[k + 1]), ascending; rank [L*M*A] is row
-    // (l, k)'s index among them (-1: absent), needed only when some perf column is a row list
-    std::vector<Row> row_v;
-    std::vector<int> row_off(MA + 1, 0), rank;
-    if (perf_rows) {
-        rank.assign(LMA, -1);
-        std::vector<std::pair<Row, int>> uses;
-        for (size_t k = 0; k < MA; ++k) {
-            uses.clear();
-            for (int l = 0; l < L; ++l)
-                if (at(rows.perf_present, hf.perf_present, l, k)) uses.emplace_back(row_of(l, k), l);
-            std::sort(uses.begin(), uses.end());
-            for (size_t u = 0; u < uses.size(); ++u) {
-                if (u == 0 || uses[u].first != uses[u - 1].first) row_v.push_back(uses[u].first);
-                rank[(size_t)uses[u].second * MA + k] = (int)row_v.size() - 1 - row_off[k];
-            }
-            row_off[k + 1] = (int)row_v.size();
-        }
-    } else {
-        for (size_t k = 0; k < MA; ++k) {
-            if (L > 0 && hf.perf_present[k]) row_v.push_back(row_of(0, k));
-            row_off[k + 1] = (int)row_v.size();
-        }
-    }
-    // key-model (m, j) = moff[m] + j, j < the most distinct rows of m at any accelerator
-    std::vector<int> moff(M + 1, 0);
-    for (int m = 0; m < M; ++m) {
-        int J = 0;
-        for (int a = 0; a < A; ++a) J = std::max(J, row_off[(size_t)m * A + a + 1] - row_off[(size_t)m * A + a]);
-        moff[m + 1] = moff[m] + J;
-    }
+    const int S = hf.S, A = hf.A;
+    ProfileRanks pr(hf, L, rows);
     // Per load pair (s, a): one key_of entry per distinct row j of (m, a), pointing at the key record of the lowest
     // row with the same (alpha .. delta, N).  The key rows are (server, key-model) pairs numbered in server order;
     // need[k * A + a] marks the key pairs phase 1 sizes.
@@ -1480,14 +1593,10 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
             // the pair's class at a level where it is present (elsewhere it is nil)
             if (hf.pair_class(s, a, true, hf.srv_arrival_rpm[s], true) != PAIR_LOAD) continue;
             const size_t k = (size_t)m * A + a;
-            const int J = row_off[k + 1] - row_off[k], e0 = (int)key_of.size();
+            const int J = pr.row_off[k + 1] - pr.row_off[k], e0 = (int)key_of.size();
             groups.clear();
-            for (int j = 0; j < J; ++j) {
-                const Row& r = row_v[row_off[k] + j];
-                const long long t = (long long)(int32_t)r[4] * (int32_t)r[5] / hf.srv_out_tokens[s];
-                const long long N = hf.srv_max_batch[s] > 0 ? hf.srv_max_batch[s] : std::max<long long>(t, 1);
-                groups.push_back({{(uint64_t)r[0] << 32 | r[1], (uint64_t)r[2] << 32 | r[3], (uint64_t)N}, j});
-            }
+            for (int j = 0; j < J; ++j)
+                groups.push_back({pr.sizing_key(k, j, hf.srv_max_batch[s], hf.srv_out_tokens[s]), j});
             std::sort(groups.begin(), groups.end());
             key_of.resize(key_of.size() + J);  // the representative row for now
             for (size_t u = 0; u < groups.size(); ++u) {
@@ -1502,7 +1611,7 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
         const int base = (int)key_srv.size();
         for (int j : srv_js) {
             key_srv.push_back(s);
-            key_model.push_back(moff[m] + j);
+            key_model.push_back(pr.moff[m] + j);
         }
         need.resize(key_srv.size() * A, 0);
         for (int a = 0; a < A; ++a) {
@@ -1531,28 +1640,7 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
         kh.srv_arrival_rpm[k] = hf.srv_arrival_rpm[key_srv[k]];
         kh.srv_model[k] = key_model[k];
     }
-    kh.M = moff[M];
-    const size_t KMA = (size_t)kh.M * A;
-    kh.perf_present.assign(KMA, 0);
-    kh.perf_acc_count.assign(KMA, 1);
-    for (auto* col : {&kh.perf_alpha, &kh.perf_beta, &kh.perf_gamma, &kh.perf_delta}) col->assign(KMA, 0.0f);
-    kh.perf_max_batch.assign(KMA, 0);
-    kh.perf_at_tokens.assign(KMA, 0);
-    for (int m = 0; m < M; ++m)
-        for (int a = 0; a < A; ++a) {
-            const size_t k = (size_t)m * A + a;
-            for (int j = 0; j < row_off[k + 1] - row_off[k]; ++j) {
-                const Row& r = row_v[row_off[k] + j];
-                const size_t q = (size_t)(moff[m] + j) * A + a;
-                kh.perf_present[q] = 1;
-                memcpy(&kh.perf_alpha[q], &r[0], 4);
-                memcpy(&kh.perf_beta[q], &r[1], 4);
-                memcpy(&kh.perf_gamma[q], &r[2], 4);
-                memcpy(&kh.perf_delta[q], &r[3], 4);
-                kh.perf_max_batch[q] = (int32_t)r[4];
-                kh.perf_at_tokens[q] = (int32_t)r[5];
-            }
-        }
+    pr.fill(kh);
     std::vector<int> pairs, Ns;
     int rc = sorted_pairs(h, kh, [&](int k, int a) { return need[(size_t)k * A + a] != 0; }, pairs, Ns);
     if (rc) return rc;
@@ -1565,18 +1653,15 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
 
     Cols c(16);
     kf.place(c);
-    static const size_t elem[9] = {4, 1, 4, 4, 4, 4, 4, 4, 4};
-    size_t o_list[9] = {};
-    for (int b = 0; b < 9; ++b)
-        if (lists[b]) o_list[b] = c.take(elem[b] * (b == 0 ? LA : LMA));
+    pr.place(c);
+    const std::vector<int>& rank = pr.rank;
     const size_t o_rank = c.take(4 * rank.size()), o_poff = c.take(4 * pair_off.size()),
                  o_keyof = c.take(4 * key_of.size()), o_ksrv = c.take(4 * (size_t)K),
                  o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * (size_t)K),
                  o_item = c.take(4 * ((size_t)n + 1));
     rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
         kf.write(p);
-        for (int b = 0; b < 9; ++b)
-            if (lists[b] && L) memcpy(p + o_list[b], lists[b], elem[b] * (b == 0 ? LA : LMA));
+        pr.write(p);
         if (!rank.empty()) memcpy(p + o_rank, rank.data(), 4 * rank.size());
         memcpy(p + o_poff, pair_off.data(), 4 * pair_off.size());
         if (!key_of.empty()) memcpy(p + o_keyof, key_of.data(), 4 * key_of.size());
@@ -1597,46 +1682,21 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
     LoadStar ls;
     rc = enqueue_load_star(h, kh, kd, n, ls);
     if (rc) return rc;
-    if (n > 0) {
-        WorkloadArgs g{};
-        g.ld = load_args(ls);
-        g.ld.level_rpm = kd.srv_arrival_rpm;
-        g.ld.L = 1;
-        g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
-        g.ld.cand = key;
-        g.key_srv = (const int*)(d + o_ksrv);
-        g.lev_off = (const int*)(d + o_loff);
-        g.lev = (const int*)(d + o_lev);
-        g.item_off = (const int*)(d + o_item);
-        g.S = K;
-        g.n_items = n;
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, workload_kernel, 256, 0));
-        per_sm = std::max(1, std::min(per_sm, 8));
-        const long long warps = ((long long)n + 31) / 32;
-        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
-        workload_kernel<<<blocks, 256, 0, h->stream>>>(g);
-        h->launches++;
-        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
-        launch_fallback(h, workload_fallback, g, ls.fb2);
-    }
+    WorkloadArgs t{};
+    t.key_srv = (const int*)(d + o_ksrv);
+    t.lev_off = (const int*)(d + o_loff);
+    t.lev = (const int*)(d + o_lev);
+    t.item_off = (const int*)(d + o_item);
+    t.S = K;
+    t.n_items = n;
+    rc = enqueue_workload_tail(h, ls, t, kd.srv_arrival_rpm, 1, key);
+    if (rc) return rc;
     const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
     if (n_rec > 0) {
         ProfileArgs g{};
         g.f = h->df;
-        g.rows = h->df;
-        const auto row = [&](int b) { return (const void*)(d + o_list[b]); };
-        if (rows.acc_cost) g.rows.acc_cost = (const float*)row(0);
-        if (rows.perf_present) g.rows.perf_present = (const uint8_t*)row(1);
-        if (rows.perf_alpha) g.rows.perf_alpha = (const float*)row(2);
-        if (rows.perf_beta) g.rows.perf_beta = (const float*)row(3);
-        if (rows.perf_gamma) g.rows.perf_gamma = (const float*)row(4);
-        if (rows.perf_delta) g.rows.perf_delta = (const float*)row(5);
-        if (rows.perf_acc_count) g.rows.perf_acc_count = (const int32_t*)row(6);
-        if (rows.perf_max_batch) g.rows.perf_max_batch = (const int32_t*)row(7);
-        if (rows.perf_at_tokens) g.rows.perf_at_tokens = (const int32_t*)row(8);
-        g.per_level = per_level;
-        g.rank = perf_rows ? (const int*)(d + o_rank) : nullptr;
+        pr.set_rows(g, d);
+        g.rank = pr.perf_rows ? (const int*)(d + o_rank) : nullptr;
         g.pair_off = (const int*)(d + o_poff);
         g.key_of = (const int*)(d + o_keyof);
         g.key = key;
@@ -1648,6 +1708,163 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
     if (S > 0 && L > 0) {
         unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
             h->df, cand, winners, L);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- profile trace: the reconcile replayed over ticks of load and of (acc_cost, perf) rows (DESIGN.md §3.15) ------
+// CreateAllocation reads neither the current allocation (§3.13) nor, outside the cost, the price and AccCount
+// (§3.14).  So a load pair's record at tick t is fixed by its key (s, a, in_t, out_t, bits of alpha .. delta at row
+// t, N at row t), and every tick is sized in one pass.  The workload grid's tail gives every candidate of a key row
+// the row's tick list, so:
+// - with a perf column given, the key fleet has one row per key pair: server s at the key's tokens on the
+//   key-model (ProfileRanks) of a row of the key, with keepAccelerator and current accelerator a, so that
+//   prepare_load_star sizes that pair alone;
+// - with none, every accelerator of (s, in, out) has the same rows at every tick, and the key fleet is the workload
+//   trace's: rows (s, in, out) on the fleet's own models, keepAccelerator kept on the pinned servers only.  So the
+//   call sizes the same pairs, in the same order, with the same phase-1 work.
+// Phase 1 and the workload grid's tail run unchanged and write each loaded (t, s, a) record in place;
+// profile_trace_kernel then writes the nil and zero-load records and prices the tail's at row t, and the workload
+// trace's trace_kernel runs the chain.  rpm / in / out [L*S] are the caller's rows (NULL: the fleet's own column at
+// every tick); cand ([L*S*A]) and winners ([L*S]) are device columns.
+int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                          const wva_profile_rows& rows, const AllocCols& cand, const AllocCols& winners) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A, M = hf.M;
+    const size_t LS = (size_t)L * S;
+    std::vector<float> own_rpm;
+    std::vector<int32_t> own_in, own_out;
+    auto tile = [&](auto*& list, const auto& col, auto& own) {
+        if (list) return;
+        own.resize(LS);
+        for (int t = 0; t < L; ++t) std::copy(col.begin(), col.end(), own.begin() + (size_t)t * S);
+        list = own.data();
+    };
+    tile(rpm, hf.srv_arrival_rpm, own_rpm);
+    tile(in, hf.srv_in_tokens, own_in);
+    tile(out, hf.srv_out_tokens, own_out);
+    ProfileRanks pr(hf, L, rows);
+    std::vector<uint8_t> pin(S);
+    for (int s = 0; s < S; ++s) pin[s] = trace_pinned(hf, s);
+    // The keys.  Without a perf column: the workload trace's (s, in, out) rows.  With one: per server the ticks at
+    // which s is a load, grouped by (in, out) as in the workload trace; per group and accelerator the ticks at which
+    // (m, a) is present, grouped by the row's sizing key, one row per key pair.  A pinned server sizes its current
+    // pair alone.
+    TokenKeys tk;
+    std::vector<int> key_acc, key_model;  // with a perf column: key row k's accelerator and key-model
+    if (!pr.perf_rows) {
+        token_keys(L, S, rpm, in, out, tk);
+    } else {
+        std::vector<std::pair<uint64_t, int>> uses;                 // ((in << 32) | out, tick)
+        std::vector<std::pair<std::array<uint64_t, 3>, int>> prof;  // (sizing key, tick)
+        for (int s = 0; s < S; ++s) {
+            const int m = hf.srv_model[s];
+            if (m < 0 || m >= M || !hf.srv_has_target[s]) continue;
+            load_groups(L, S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
+                for (int a = 0; a < A; ++a) {
+                    if (pin[s] && hf.srv_cur_acc[s] != a) continue;
+                    const size_t k = (size_t)m * A + a;
+                    prof.clear();
+                    for (size_t u = u0; u < u1; ++u) {
+                        const int t = uses[u].second, j = pr.rank_at(t, k);
+                        if (j >= 0) prof.emplace_back(pr.sizing_key(k, j, hf.srv_max_batch[s], ko), t);
+                    }
+                    std::sort(prof.begin(), prof.end());
+                    for (size_t v = 0; v < prof.size(); ++v) {
+                        if (v == 0 || prof[v].first != prof[v - 1].first) {
+                            tk.add(s, ki, ko);
+                            key_acc.push_back(a);
+                            key_model.push_back(pr.moff[m] + pr.rank_at(prof[v].second, k));
+                        }
+                        tk.add_level(prof[v].second);
+                    }
+                }
+            });
+        }
+    }
+    const std::vector<int>&key_srv = tk.srv, &lev_off = tk.lev_off, &lev = tk.lev;
+    const int K = (int)key_srv.size();  // at most L * S * A
+    // the key fleet's pair ids k * A + a are int
+    if ((long long)K * A >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "profile trace too large for one call (>= 2^31 key pairs x accelerators)");
+    KeyFleet kf(hf, key_srv, tk.in, tk.out);
+    HostFleet& kh = kf.hf;
+    if (pr.perf_rows) {
+        kf.own_ma = true;
+        for (int k = 0; k < K; ++k) {
+            kh.srv_model[k] = key_model[k];
+            kh.srv_keep_acc[k] = 1;
+            kh.srv_cur_acc[k] = key_acc[k];
+        }
+        pr.fill(kh);
+    } else {  // the workload trace's key fleet
+        for (int k = 0; k < K; ++k) kh.srv_keep_acc[k] = pin[key_srv[k]];
+    }
+    Cols c(16);
+    kf.place(c);
+    pr.place(c);
+    // the tail's candidates: one per key row with a perf column, up to A without
+    const size_t n_cand_max = pr.perf_rows ? (size_t)K : (size_t)K * A;
+    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS), o_pin = c.take(S),
+                 o_ksrv = c.take(4 * (size_t)K), o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * lev.size()),
+                 o_item = c.take(4 * (n_cand_max + 1));
+    std::vector<int> pairs;
+    int n_items = 0;
+    int rc = prepare_load_star(h, kh, std::vector<char>(K, 1), pairs, c, [&](char* p) {
+        kf.write(p);
+        pr.write(p);
+        if (LS) {
+            memcpy(p + o_rpm, rpm, 4 * LS);
+            memcpy(p + o_in, in, 4 * LS);
+            memcpy(p + o_out, out, 4 * LS);
+        }
+        if (S) memcpy(p + o_pin, pin.data(), S);
+        if (K) memcpy(p + o_ksrv, key_srv.data(), 4 * (size_t)K);
+        memcpy(p + o_loff, lev_off.data(), 4 * ((size_t)K + 1));
+        if (!lev.empty()) memcpy(p + o_lev, lev.data(), 4 * lev.size());
+        // candidate j's items: one per tick of its key row
+        int* item = (int*)(p + o_item);
+        item[0] = 0;
+        for (size_t j = 0; j < pairs.size(); ++j) {
+            const int k = pairs[j] / A;
+            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
+        }
+        n_items = item[pairs.size()];
+    });
+    if (rc) return rc;
+    const char* d = (const char*)h->lg_tabs.lists.p;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    LoadStar ls;
+    rc = enqueue_load_star(h, kh, kf.view(h->df, d), n_items, ls);
+    if (rc) return rc;
+    WorkloadArgs g{};
+    g.key_srv = (const int*)(d + o_ksrv);
+    g.lev_off = (const int*)(d + o_loff);
+    g.lev = (const int*)(d + o_lev);
+    g.item_off = (const int*)(d + o_item);
+    g.S = S;
+    g.n_items = n_items;
+    rc = enqueue_workload_tail(h, ls, g, (const float*)(d + o_rpm), L, cand);
+    if (rc) return rc;
+    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
+    if (n_rec > 0) {
+        ProfileTraceArgs r{};
+        r.p.f = h->df;
+        r.p.f.srv_keep_acc = (const uint8_t*)(d + o_pin);
+        pr.set_rows(r.p, d);
+        r.p.cand = cand;
+        r.p.L = L;
+        r.level_rpm = (const float*)(d + o_rpm);
+        r.level_in = (const int*)(d + o_in);
+        r.level_out = (const int*)(d + o_out);
+        profile_trace_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(r);
+        h->launches++;
+    }
+    if (S > 0 && L > 0) {
+        trace_kernel<<<(unsigned)((S + 127) / 128), 128, 0, h->stream>>>(h->df, cand, winners, L);
         h->launches++;
     }
     CK(cudaGetLastError());
@@ -2609,6 +2826,31 @@ int wva_profile_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, co
     c.win_blocks = (size_t)n_levels;
     rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
         return enqueue_profile_grid(h, n_levels, rows ? *rows : own, dc, dw);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
+int wva_profile_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                      const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
+                      wva_allocs* candidates, wva_allocs* winners) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (n_ticks < 0) return h->fail(WVA_ERR_BAD_ARG, "negative tick count");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * fleet->n_acc * n_ticks >= (1ll << 31) ||
+        (long long)n_ticks * fleet->n_models * fleet->n_acc >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "profile trace too large for one call (>= 2^31 candidates or row entries)");
+    const wva_profile_rows own{};
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_ticks, candidates != nullptr, true};
+    c.win_blocks = (size_t)n_ticks;
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_profile_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens, rows ? *rows : own, dc, dw);
     });
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;

@@ -10,6 +10,7 @@
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
 //   trace_kernel        the same tick by tick, each tick's winner the next tick's current allocation
 //   profile_kernel      the profile grid's records per (level, pair) from the key records, priced at the level
+//   profile_trace_kernel  the profile trace's records per (tick, pair), the tail's records priced at the tick
 //   size_grid_finalize  the same over (accelerator x batch size) per server, one warp per server
 //   sweep_kernel        Analyze over a rate sweep per (server, acc)
 //
@@ -1727,6 +1728,15 @@ __device__ __forceinline__ DevFleet profile_at(const ProfileArgs& g, int l) {
 #undef WVA_PROFILE_ROW
     return fl;
 }
+// A load record sized at another price or AccCount, priced at fl: cost = acc_cost[a] * NumInstances(m, a) *
+// replicas and value = cost, the only fields of CreateAllocation that read either.
+__device__ __forceinline__ Cand priced_at(const DevFleet& fl, int m, int a, Cand c) {
+    if (c.feasible) {
+        c.cost = __fmul_rn(fl.acc_cost[a], (float)((long long)num_instances(fl, m, a) * (long long)c.replicas));
+        c.value = c.cost;
+    }
+    return c;
+}
 __global__ void profile_kernel(ProfileArgs g) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int n_pairs = g.f.S * g.f.A;
@@ -1741,13 +1751,39 @@ __global__ void profile_kernel(ProfileArgs g) {
     } else if (cls == PAIR_LOAD) {
         const int m = fl.srv_model[s];
         const int j = g.rank ? g.rank[((size_t)l * fl.M + m) * fl.A + a] : 0;
-        c = load_cand(g.key, g.key_of[g.pair_off[pair] + j]);
-        if (c.feasible) {
-            c.cost = __fmul_rn(fl.acc_cost[a], (float)((long long)num_instances(fl, m, a) * (long long)c.replicas));
-            c.value = c.cost;
-        }
+        c = priced_at(fl, m, a, load_cand(g.key, g.key_of[g.pair_off[pair] + j]));
     }
     store_cand(g.cand, i, c);
+}
+
+// The profile trace's records (DESIGN.md §3.15): L tick blocks of S * A records (record (t * S + s) * A + a), one
+// thread per record, after the workload grid's tail wrote every load pair's record in place at the key fleet's
+// price.  f_t is f with row t of the load rows and of the profile rows (profile_at).  A pair is classed at f_t: nil,
+// zeroLoadAllocation at f_t, or the tail's record priced at row t.  f carries keepAccelerator on the pinned servers
+// only, whose pairs the tail did not size; trace_kernel applies the rest of the mask tick by tick (S * A * L < 2^31,
+// checked on the host).
+struct ProfileTraceArgs {
+    ProfileArgs p;           // f, rows, per_level, cand and L (rank, pair_off, key_of and key are not read)
+    const float* level_rpm;  // [L * S] row t's arrival rates ...
+    const int* level_in;     // ... input tokens ...
+    const int* level_out;    // ... and output tokens
+};
+__global__ void profile_trace_kernel(ProfileTraceArgs g) {
+    const ProfileArgs& p = g.p;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n_pairs = p.f.S * p.f.A;
+    if (i >= n_pairs * p.L) return;
+    const int t = i / n_pairs, pair = i - t * n_pairs;
+    const int s = pair / p.f.A, a = pair % p.f.A;
+    DevFleet ft = profile_at(p, t);
+    ft.srv_arrival_rpm = g.level_rpm + (size_t)t * p.f.S;
+    ft.srv_in_tokens = g.level_in + (size_t)t * p.f.S;
+    ft.srv_out_tokens = g.level_out + (size_t)t * p.f.S;
+    const int cls = pair_class(ft, s, a, true);
+    Cand c = cand_nil();
+    if (cls == PAIR_ZERO) c = zero_load_alloc(ft, s, a);
+    else if (cls == PAIR_LOAD) c = priced_at(ft, ft.srv_model[s], a, load_cand(p.cand, i));
+    store_cand(p.cand, i, c);
 }
 
 // wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record

@@ -40,6 +40,37 @@ def greedy_solve(fleet: Fleet, candidates: Allocs):
     return candidates, win
 
 
+# the fleet column each load row list replaces (every other row list is named after its column)
+_ROW_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens"}
+_PROFILE_COLUMNS = ("acc_cost", "perf_present", "perf_alpha", "perf_beta", "perf_gamma", "perf_delta",
+                    "perf_acc_count", "perf_max_batch", "perf_at_tokens")
+
+
+def _row_lists(fleet: Fleet, given: dict):
+    """The row lists of a grid or trace call, by argument name -> ({name: C-contiguous array of shape (L, *the
+    column's shape) in the column's dtype}, L).  A list of None is left out; L is the lists' common first dimension,
+    None when every list is None."""
+    shape = {"S": (fleet.n_servers,), "A": (fleet.n_acc,), "MA": (fleet.n_models, fleet.n_acc)}
+    cols = {name: (dt, shape.get(n)) for name, dt, n in _abi.FLEET_COLUMNS}
+    rows, L = {}, None
+    for name, x in given.items():
+        if x is None:
+            continue
+        dt, tail = cols[_ROW_COLUMN.get(name, name)]
+        r = np.ascontiguousarray(x, dt)
+        if r.ndim != 1 + len(tail) or r.shape[1:] != tail or (L is not None and r.shape[0] != L):
+            want = "L" if L is None else str(L)
+            raise ValueError(f"{name} must have shape ({want}, {', '.join(map(str, tail))}), got {r.shape}")
+        L = r.shape[0]
+        rows[name] = r
+    return rows, L
+
+
+def _profile_rows_c(rows: dict):
+    """wva_profile_rows over the profile columns in rows (NULL for the others)."""
+    return _abi.ProfileRowsC(*[_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in _PROFILE_COLUMNS])
+
+
 class Engine:
     """One engine per GPU (one process per GPU in multi-GPU runs)."""
 
@@ -212,27 +243,29 @@ class Engine:
     def _workload_rows(self, call, fleet, arrival_rpm, in_tokens, out_tokens, want_candidates, out):
         """wva_workload_grid / wva_workload_trace over (L, S) rows; a token list of None is the fleet's own."""
         S = fleet.n_servers
-        rpm = np.ascontiguousarray(arrival_rpm, np.float32)
-        if rpm.ndim != 2 or rpm.shape[1] != S:
-            raise ValueError(f"arrival_rpm must have shape (L, {S}), got {rpm.shape}")
-        L = rpm.shape[0]
-        rows = [rpm]
-        for name, x, own in (("in_tokens", in_tokens, fleet.srv_in_tokens),
-                             ("out_tokens", out_tokens, fleet.srv_out_tokens)):
-            r = np.ascontiguousarray(np.broadcast_to(own, (L, S)) if x is None else x, np.int32)
-            if r.shape != (L, S):
-                raise ValueError(f"{name} must have shape ({L}, {S}), got {r.shape}")
-            rows.append(r)
-        if out is not None and out.n != L * S:
-            raise ValueError("out must hold L * fleet.n_servers records")
-        win = out if out is not None else Allocs(L * S)
-        cand = Allocs(L * S * fleet.n_acc) if want_candidates else None
+        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "in_tokens": in_tokens, "out_tokens": out_tokens})
+        if "arrival_rpm" not in rows:
+            raise ValueError("arrival_rpm is required")
+        for name, own in (("in_tokens", fleet.srv_in_tokens), ("out_tokens", fleet.srv_out_tokens)):
+            if name not in rows:
+                rows[name] = np.ascontiguousarray(np.broadcast_to(own, (L, S)), np.int32)
+        win, cand = self._row_outputs(fleet, L, want_candidates, out)
         fc, wc = fleet.as_c(), win.as_c()
         cc = cand.as_c() if cand is not None else None
         self._resident(fleet)
-        self._check(call(self._h, C.byref(fc), L, *[_abi.ptr(r.reshape(-1)) for r in rows],
+        self._check(call(self._h, C.byref(fc), L,
+                         *[_abi.ptr(rows[k].reshape(-1)) for k in ("arrival_rpm", "in_tokens", "out_tokens")],
                          C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
+
+    @staticmethod
+    def _row_outputs(fleet, L, want_candidates, out):
+        """The winners (``out``, or new) and candidates (or None) of an L-row call."""
+        if out is not None and out.n != L * fleet.n_servers:
+            raise ValueError("out must hold L * fleet.n_servers records")
+        win = out if out is not None else Allocs(L * fleet.n_servers)
+        cand = Allocs(L * fleet.n_servers * fleet.n_acc) if want_candidates else None
+        return win, cand
 
     def profile_grid(self, fleet: Fleet, *, acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None,
                      perf_gamma=None, perf_delta=None, perf_acc_count=None, perf_max_batch=None, perf_at_tokens=None,
@@ -247,34 +280,50 @@ class Engine:
         include/wva_b200.h).  A column of ``None`` is the fleet's own at every level; at least one must be given,
         and L is their row count.  ``srv_cur_cost`` is not re-priced.  ``out``: an ``Allocs`` of ``L * S`` records
         to write the winners into."""
-        S, A, M = fleet.n_servers, fleet.n_acc, fleet.n_models
-        given = {"acc_cost": acc_cost, "perf_present": perf_present, "perf_alpha": perf_alpha,
-                 "perf_beta": perf_beta, "perf_gamma": perf_gamma, "perf_delta": perf_delta,
-                 "perf_acc_count": perf_acc_count, "perf_max_batch": perf_max_batch, "perf_at_tokens": perf_at_tokens}
-        dtypes = {name: dt for name, dt, _ in _abi.FLEET_COLUMNS}
-        rows, L = {}, None
-        for name, x in given.items():
-            if x is None:
-                continue
-            r = np.ascontiguousarray(x, dtypes[name])
-            tail = (A,) if name == "acc_cost" else (M, A)
-            if r.ndim != 1 + len(tail) or r.shape[1:] != tail or (L is not None and r.shape[0] != L):
-                want = "L" if L is None else str(L)
-                raise ValueError(f"{name} must have shape ({want}, {', '.join(map(str, tail))}), got {r.shape}")
-            L = r.shape[0]
-            rows[name] = r
+        rows, L = _row_lists(fleet, {"acc_cost": acc_cost, "perf_present": perf_present, "perf_alpha": perf_alpha,
+                                     "perf_beta": perf_beta, "perf_gamma": perf_gamma, "perf_delta": perf_delta,
+                                     "perf_acc_count": perf_acc_count, "perf_max_batch": perf_max_batch,
+                                     "perf_at_tokens": perf_at_tokens})
         if L is None:
             raise ValueError("profile_grid needs at least one row list")
-        if out is not None and out.n != L * S:
-            raise ValueError("out must hold L * fleet.n_servers records")
-        win = out if out is not None else Allocs(L * S)
-        cand = Allocs(L * S * A) if want_candidates else None
-        rc_ = _abi.ProfileRowsC(*[_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in given])
+        win, cand = self._row_outputs(fleet, L, want_candidates, out)
+        rc_ = _profile_rows_c(rows)
         fc, wc = fleet.as_c(), win.as_c()
         cc = cand.as_c() if cand is not None else None
         self._resident(fleet)
         self._check(self._L.wva_profile_grid(self._h, C.byref(fc), L, C.byref(rc_),
                                              C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
+
+    def profile_trace(self, fleet: Fleet, arrival_rpm=None, in_tokens=None, out_tokens=None, *, acc_cost=None,
+                      perf_present=None, perf_alpha=None, perf_beta=None, perf_gamma=None, perf_delta=None,
+                      perf_acc_count=None, perf_max_batch=None, perf_at_tokens=None, want_candidates: bool = False,
+                      out: Allocs | None = None):
+        """The reference's reconcile replayed over ticks of load (``arrival_rpm`` req/min, ``in_tokens``,
+        ``out_tokens``, shape (L, S)), accelerator costs (``acc_cost``, shape (L, A)) and performance profiles
+        (``perf_*``, shape (L, M, A)): ``Server.Calculate``, ``SolveUnlimited`` and ``Server.ApplyDesiredAlloc`` per
+        tick -> (candidates [L*S*A] | None, winners [L*S]), both tick-major.
+
+        Tick ``t`` is ``solve`` in unlimited mode on the fleet with every given column = row ``t`` and the current
+        allocation advanced by ``fleet.apply_winners`` through ticks 0..t-1; the fleet's own ``srv_cur_cost`` is
+        not re-priced (see ``wva_profile_trace`` in include/wva_b200.h).  A list of ``None`` is the fleet's own
+        column at every tick; at least one must be given, and L is their common row count.  ``out``: an ``Allocs``
+        of ``L * S`` records to write the winners into."""
+        load = {"arrival_rpm": arrival_rpm, "in_tokens": in_tokens, "out_tokens": out_tokens}
+        rows, L = _row_lists(fleet, {**load, "acc_cost": acc_cost, "perf_present": perf_present,
+                                     "perf_alpha": perf_alpha, "perf_beta": perf_beta, "perf_gamma": perf_gamma,
+                                     "perf_delta": perf_delta, "perf_acc_count": perf_acc_count,
+                                     "perf_max_batch": perf_max_batch, "perf_at_tokens": perf_at_tokens})
+        if L is None:
+            raise ValueError("profile_trace needs at least one row list")
+        win, cand = self._row_outputs(fleet, L, want_candidates, out)
+        rc_ = _profile_rows_c(rows)
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_profile_trace(self._h, C.byref(fc), L,
+                                              *[_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in load],
+                                              C.byref(rc_), C.byref(cc) if cc is not None else None, C.byref(wc)))
         return cand, win
 
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
