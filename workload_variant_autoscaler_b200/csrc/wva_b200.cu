@@ -3103,7 +3103,9 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
 // ---- self-check of the exact-division primitive (not part of the public ABI) ------------------
 // Compares div_recip (Markstein correction around a double-word reciprocal) with div.rn.f64 on
 // pseudo-random operands drawn from the solver's exponent windows, including adversarial
-// divisors next to powers of two and float32-valued divisors.  Returns the mismatch count.
+// divisors next to powers of two and float32-valued divisors, and div_rate / step_rate (no
+// correction) on float32-valued divisors, random and at the least distance a quotient by a
+// float32 can have from a rounding midpoint.  Returns the mismatch count.
 __global__ void div_selfcheck_kernel(unsigned long long seed, int iters, unsigned long long* mismatches) {
     unsigned long long x = seed ^ (0x9E3779B97F4A7C15ull * (blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x + 1));
     auto next = [&]() {  // xorshift64*
@@ -3136,7 +3138,12 @@ __global__ void div_selfcheck_kernel(unsigned long long seed, int iters, unsigne
         z.yl = __dmul_rn(__fma_rn(-b, rc.yh, 1.0), rc.yh);
         const double q2 = div_recip(a, z);
         if (__double_as_longlong(q2) != __double_as_longlong(want)) ++bad;
-        // the tail step with the pre-multiplied low word (step_recip): p in [2^-280, 2^880), float32 lambda in
+        // division by a service rate (div_rate, no Markstein correction): a float32 divisor drawn as case 0 above
+        const float bf = (float)__longlong_as_double((long long)(((unsigned long long)(1023 + eb) << 52) |
+                                                                 (r0 & 0x000FFFFFE0000000ull)));
+        const RateRecip rr = make_rate_recip(bf);
+        if (__double_as_longlong(div_rate(a, rr)) != __double_as_longlong(__ddiv_rn(a, (double)bf))) ++bad;
+        // the tail step with the pre-multiplied low word (step_rate): p in [2^-280, 2^880), float32 lambda in
         // [2^-60, 2^60]
         {
             const unsigned long long r3 = next();
@@ -3145,9 +3152,36 @@ __global__ void div_selfcheck_kernel(unsigned long long seed, int iters, unsigne
             const long long el = (long long)((r3 >> 12) % 121) - 60;
             const double lam = __longlong_as_double(
                 (long long)(((unsigned long long)(1023 + el) << 52) | ((r3 >> 20) & 0x000FFFFFE0000000ull)));
-            const double got = step_recip(pp, lam, __dmul_rn(lam, rc.yl), rc);
-            const double want3 = __ddiv_rn(__dmul_rn(pp, lam), b);
+            const double got = step_rate(pp, lam, __dmul_rn(lam, rr.yl), rr);
+            const double want3 = __ddiv_rn(__dmul_rn(pp, lam), (double)bf);
             if (__double_as_longlong(got) != __double_as_longlong(want3)) ++bad;
+        }
+        // the hardest float32 divisors: b = M * 2^eb with M odd (24 bits) and a = A * 2^ea with
+        // A * 2^25 = M * O -+ 1 for an odd 54-bit O, so that a / b lies 2^-25 / M (~2^-78 relative) from the
+        // rounding midpoint O * 2^-25 (scaled); checked through div_rate and through step_rate with lambda a power
+        // of two (p = a / lambda exactly)
+        {
+            const unsigned long long r6 = next(), r7 = next();
+            const unsigned M = 0x800001u | ((unsigned)r6 & 0x7FFFFEu);  // odd, in [2^23, 2^24)
+            unsigned inv = M;  // M^-1 mod 2^25 by Newton's iteration (each step doubles the correct low bits)
+            for (int k = 0; k < 5; ++k) inv *= 2u - M * inv;
+            const bool plus = (r6 >> 24) & 1;  // A * 2^25 = M * O + 1 (O = -M^-1) or M * O - 1 (O = M^-1)
+            const unsigned long long olo = (plus ? (0u - inv) : inv) & 0x1FFFFFFu;
+            const unsigned long long ohi = (1ull << 28) | ((r6 >> 25) & 0xFFFFFFFull);  // O = ohi * 2^25 + olo
+            const unsigned long long mlo = (unsigned long long)M * olo;                // < 2^49
+            const unsigned long long A = (unsigned long long)M * ohi + ((plus ? mlo + 1 : mlo - 1) >> 25);
+            const long long ebh = (long long)(r7 % 120) - 60, eah = (long long)((r7 >> 8) % 1281) - 340;
+            const float bh = (float)ldexp((double)M, (int)ebh - 23);
+            const double ah = ldexp((double)A, (int)eah - 52);
+            const RateRecip rh = make_rate_recip(bh);
+            const double wanth = __ddiv_rn(ah, (double)bh);
+            if (__double_as_longlong(div_rate(ah, rh)) != __double_as_longlong(wanth)) ++bad;
+            const long long elh = (long long)((r7 >> 20) % 121) - 60;
+            const long long eph = eah - elh;  // p = a / lambda, kept inside [2^-280, 2^880)
+            if (eph >= -279 && eph < 880) {  // A in [2^51, 2^53): p in [2^(eph - 1), 2^(eph + 1))
+                const double lam = ldexp(1.0, (int)elh), pp = ldexp((double)A, (int)eph - 52);
+                if (__double_as_longlong(step_rate(pp, lam, __dmul_rn(lam, rh.yl), rh)) != __double_as_longlong(wanth)) ++bad;
+            }
         }
         // the division by the normalising sum: sum in [1, 2^900), p in [max(2^-280, sum * 2^-960), sum]
         {
@@ -3170,7 +3204,7 @@ __global__ void div_selfcheck_kernel(unsigned long long seed, int iters, unsigne
 
 // ---- diagnostics (not part of the public ABI) ------------------------------------------
 // Per-cell SM cycles of the last grid solve, in launch order, followed by the cell ids.
-// Runs blocks*256*iters*2 random divisions; returns the number of results that differ from div.rn.f64.
+// Runs blocks*256*iters rounds of the checks above; returns the number of results that differ from div.rn.f64.
 long long wva_dbg_div_selfcheck(wva_handle* h, unsigned long long seed, int blocks, int iters) {
     if (!h) return -1;
     cudaSetDevice(h->device);

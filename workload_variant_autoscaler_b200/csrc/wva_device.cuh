@@ -7,10 +7,11 @@
 //
 // The one place where the instruction sequence differs from the reference is IEEE
 // division by a value that is reused many times (the state-dependent service rate and
-// the normalising sum).  There the quotient is produced by a Markstein correction
-// around a pre-computed double-word reciprocal, which yields the correctly rounded
-// quotient — the same bits as the reference's DIVSD — in 4 dependent FP64 ops instead
-// of the ~10-op generic division sequence (see DESIGN.md "Exact division").
+// the normalising sum).  There the quotient is produced from a pre-computed double-word
+// reciprocal, which yields the correctly rounded quotient — the same bits as the
+// reference's DIVSD — in 2 dependent FP64 ops for a float32 service rate and 4 (with a
+// Markstein correction) for the double sum, instead of the ~10-op generic division
+// sequence (see DESIGN.md "Exact division").
 #pragma once
 #include <math_constants.h>
 #include <cuda_runtime.h>
@@ -102,18 +103,37 @@ __device__ __forceinline__ double div_recip(double a, const Recip& r) {
     double res = __fma_rn(-r.b, q0, a);
     return __fma_rn(res, r.yh, q0);
 }
+// Division by a service rate.  The rates are float32 values (servRate is []float32 in the reference), and for a
+// divisor with a 24-bit significand q0 = RN(a*yh + RN(a*yl)) is already RN(a/b): a/b - m, for any rounding midpoint
+// m = O * 2^g between doubles (O odd, 54 bits), has the nonzero integer numerator of (a - b*m) / b, and b*m has a
+// 78-bit odd part that a cannot match, so a/b lies at least ~2^-78 (relative) from every midpoint, while the
+// FMA's exact sum a*yh + t is within ~2^-103 of a/b.  Both lie strictly between the same two midpoints, so the
+// Markstein correction of div_recip can never change q0 and is dropped (proof in DESIGN.md "Exact division").
+// Preconditions: the divisor is a float32 value, and the exponent windows below keep a, t and q0 normal.  The
+// first is carried by the type: a RateRecip is built only from a float (make_rate_recip) or read back from a
+// table that make_rate_recip filled (load_recip); a double divisor (the normalising sum) stays a Recip.
+struct RateRecip {
+    double b, yh, yl;
+};
+__device__ __forceinline__ RateRecip make_rate_recip(float rate) {
+    const Recip r = make_recip((double)rate);
+    RateRecip s;
+    s.b = r.b;
+    s.yh = r.yh;
+    s.yl = r.yl;
+    return s;
+}
+// RN(a / b) for a float32-valued b: dependent chain t -> q0 (two operations)
+__device__ __forceinline__ double div_rate(double a, const RateRecip& r) {
+    return __fma_rn(a, r.yh, __dmul_rn(a, r.yl));
+}
 // One step of the recurrence, RN(RN(p * lam) / b), with the low-word product taken from p instead of from
 // a = RN(p * lam): t = RN(p * c), c = RN(lam * yl), runs in parallel with a, so the dependent chain is
-// a -> q0 -> r -> q (four operations) instead of a -> t -> q0 -> r -> q.  t only has to be accurate to a
-// few bits (it enters q0 at 2^-53 of its magnitude): q0 stays within one ulp of a / b and the final
-// Markstein correction rounds correctly exactly as in div_recip (self-check: 2 x 10^9 random steps against
-// div.rn.f64, tests/test_gpu_parity.py).  Used where lam and the divisor are loop constants (the tail).
-__device__ __forceinline__ double step_recip(double p, double lam, double c, const Recip& r) {
-    const double a = __dmul_rn(p, lam);
-    const double t = __dmul_rn(p, c);
-    const double q0 = __fma_rn(a, r.yh, t);
-    const double res = __fma_rn(-r.b, q0, a);
-    return __fma_rn(res, r.yh, q0);
+// a -> q0 (two operations).  t only has to be accurate to a few ulps: its error enters the FMA's sum at
+// ~2^-105 of the quotient, far inside the 2^-78 margin above.  Used where lam and the divisor are loop
+// constants (the tail).
+__device__ __forceinline__ double step_rate(double p, double lam, double c, const RateRecip& r) {
+    return __fma_rn(__dmul_rn(p, lam), r.yh, __dmul_rn(p, c));
 }
 
 // math.Pow(x, n) for an integer n >= 0 as the Go standard library computes it (src/math/pow.go: binary powering on
@@ -235,7 +255,7 @@ struct ModelStats {  // queuemodel.go:10-19 + mm1kmodel.go:15 + mm1modelstatedep
 // (exit test, exact division for tiny p, bail-out) lives in an outer handler.
 // tab: 4 doubles per entry {servRate[n], yh, yl, suffix-min}, at least N entries.
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void load_recip(const double* __restrict__ tab, int n, Recip& r) {
+__device__ __forceinline__ void load_recip(const double* __restrict__ tab, int n, RateRecip& r) {
     const double2 t0 = *(const double2*)(tab + 4 * n);
     r.b = t0.x;
     r.yh = t0.y;
@@ -288,7 +308,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     const unsigned warp_mask = __activemask();
     const double lam = (double)lambda;
     const int nh = N - 1;
-    Recip A, B;  // reciprocal triples of two consecutive steps (software-pipelined table loads)
+    RateRecip A, B;  // reciprocal triples of two consecutive steps (software-pipelined table loads)
     // staged head: full warp, one table.  Everything the solve reads from the table is requested here in one
     // batch: the first 64-entry window, the lane's tail entry (T stays in registers for the whole solve) and
     // entry 0.
@@ -341,7 +361,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                 !in_window(A.b, kHiRateLo, kHiRateHi);
     const bool tail_mono = rate_below(lambda, (float)tail_b);
 
-    double p = bail ? 0.0 : div_recip(lam, A);  // p[1]; RN(1*lambda) = lambda
+    double p = bail ? 0.0 : div_rate(lam, A);  // p[1]; RN(1*lambda) = lambda
     if (!(p >= 0.0) || (unsigned)__double2hiint(p) >= kHiPHi) bail = true;
     const double p1 = p;
     unsigned thr_hi = 0;
@@ -401,11 +421,11 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 #define WVA_SP1_GROUP(SEL, ST)                                                                                    \
     _Pragma("unroll") for (int u = 0; u < 4; ++u) {                                                               \
         const double4 e = *((SEL) && !(n < nh) ? (const double4*)tsave4 : (const double4*)(tb + (k + u)));       \
-        Recip R;                                                                                                  \
+        RateRecip R;                                                                                              \
         R.b = e.x;                                                                                                \
         R.yh = e.y;                                                                                               \
         R.yl = e.z;                                                                                               \
-        p = div_recip(__dmul_rn(p, lam), R);                                                                      \
+        p = div_rate(__dmul_rn(p, lam), R);                                                                       \
         sum = __dadd_rn(sum, p);                                                                                  \
         if (ST && n < STASH) stash[n * 32] = p;                                                                   \
         ++n;                                                                                                      \
@@ -440,7 +460,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
         if (n + 1 < nh) load_recip(tab, n + 1, B);
         while (n < n_stop) {
 #define WVA_P1_STEP(R)                                                      \
-    p = div_recip(__dmul_rn(p, lam), R);                                    \
+    p = div_rate(__dmul_rn(p, lam), R);                                     \
     if (n < nh) load_recip(tab, n + 2 < nh ? n + 2 : nh, R);                \
     sum = __dadd_rn(sum, p);                                                \
     if (STASH > 0 && n < STASH) stash[n * 32] = p;                          \
@@ -456,7 +476,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                     const double cA = __dmul_rn(lam, A.yl);
 #pragma unroll
                     for (int u = 0; u < 16; ++u) {
-                        p = step_recip(p, lam, cA, A);
+                        p = step_rate(p, lam, cA, A);
                         sum = __dadd_rn(sum, p);
                     }
                     n += 16;
@@ -495,7 +515,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             // rare: one step outside the fast loop (exact IEEE division when p is tiny)
             WVA_LOAD_TAIL(A)
             if (n < nh) load_recip(tab, n, A);
-            p = hp >= kHiPLo ? div_recip(__dmul_rn(p, lam), A) : __ddiv_rn(__dmul_rn(p, lam), A.b);
+            p = hp >= kHiPLo ? div_rate(__dmul_rn(p, lam), A) : __ddiv_rn(__dmul_rn(p, lam), A.b);
             sum = __dadd_rn(sum, p);
             if (STASH > 0 && n < STASH) stash[n * 32] = p;
             ++n;
@@ -593,7 +613,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
                 WVA_LOAD_TAIL(A)
                 if (i - 1 < nh) load_recip(tab, i - 1, A);
                 const double pprev = stash[(i - 2) * 32];
-                p = WVA_FASTWIN(pprev, lo2, span2) ? div_recip(__dmul_rn(pprev, lam), A)
+                p = WVA_FASTWIN(pprev, lo2, span2) ? div_rate(__dmul_rn(pprev, lam), A)
                                                                  : __ddiv_rn(__dmul_rn(pprev, lam), A.b);
             }
         }
@@ -609,13 +629,13 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 #define WVA_SP2_GROUP(SEL)                                                                                        \
     _Pragma("unroll") for (int u = 0; u < 4; ++u) {                                                               \
         const double4 e = *((SEL) && !(i < nh) ? (const double4*)tsave4 : (const double4*)(tbp + (k + u)));      \
-        Recip R;                                                                                                  \
+        RateRecip R;                                                                                              \
         R.b = e.x;                                                                                                \
         R.yh = e.y;                                                                                               \
         R.yl = e.z;                                                                                               \
         const double a_ = __dmul_rn(p, lam);                                                                      \
         pn = div_recip(p, z);                                                                                     \
-        p = div_recip(a_, R);                                                                                     \
+        p = div_rate(a_, R);                                                                                      \
         acc = __dadd_rn(acc, __dmul_rn(di, pn));                                                                  \
         di = __dadd_rn(di, 1.0);                                                                                  \
         if (SEL) {                                                                                                \
@@ -661,7 +681,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     {                                                                       \
         const double a_ = __dmul_rn(p, lam);                                \
         pn = div_recip(p, z);                                               \
-        p = div_recip(a_, R); /* p[i+1] (unused after the last state) */    \
+        p = div_rate(a_, R); /* p[i+1] (unused after the last state) */     \
         if (i < nh) load_recip(tab, i + 2 < nh ? i + 2 : nh, R);            \
         acc = __dadd_rn(acc, __dmul_rn(di, pn));                            \
         di = __dadd_rn(di, 1.0);                                            \
@@ -677,7 +697,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 #pragma unroll
                     for (int u = 0; u < 16; ++u) {
                         pn = div_recip(p, z);
-                        p = step_recip(p, lam, cA, A);
+                        p = step_rate(p, lam, cA, A);
                         acc = __dadd_rn(acc, __dmul_rn(di, pn));
                         di = __dadd_rn(di, 1.0);
                     }
@@ -759,10 +779,10 @@ __device__ __forceinline__ bool solve_row(const double* __restrict__ tab, int le
                                           double& sump_out, int& j_last) {
     const double lam = (double)lambda;
     const int nh = len - 1;
-    Recip A, B;
+    RateRecip A, B;
     load_recip(tab, 0, A);
     if (!in_window(lam, kHiRateLo, kHiRateHi) || !in_window(A.b, kHiRateLo, kHiRateHi) || nh < 2) return false;
-    double p = div_recip(lam, A);
+    double p = div_rate(lam, A);
     if (!(p >= 0.0) || (unsigned)__double2hiint(p) >= kHiPHi) return false;
     const double p1 = p;
     const unsigned thr_hi = (unsigned)__double2hiint(__dmul_rn(fmin(1.0, p1), 0x1p-78));
@@ -793,7 +813,7 @@ __device__ __forceinline__ bool solve_row(const double* __restrict__ tab, int le
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
             load_recip(tab, n + 1, B);
-            p = div_recip(__dmul_rn(p, lam), A);
+            p = div_rate(__dmul_rn(p, lam), A);
             sum = __dadd_rn(sum, p);
             A = B;
             ++n;
@@ -801,7 +821,7 @@ __device__ __forceinline__ bool solve_row(const double* __restrict__ tab, int le
     }
     while (n < nh && WVA_FASTWIN(p, lo_eff, span_eff)) {
         load_recip(tab, n + 1 < nh ? n + 1 : nh, B);
-        p = div_recip(__dmul_rn(p, lam), A);
+        p = div_rate(__dmul_rn(p, lam), A);
         sum = __dadd_rn(sum, p);
         A = B;
         ++n;
@@ -829,7 +849,7 @@ __device__ __forceinline__ bool solve_row(const double* __restrict__ tab, int le
             acc = __dadd_rn(acc, __dmul_rn(di, pn));
             di = __dadd_rn(di, 1.0);
             sum_p = __dadd_rn(sum_p, pn);
-            p = div_recip(__dmul_rn(p, lam), A);
+            p = div_rate(__dmul_rn(p, lam), A);
             A = B;
             ++i;
         }
@@ -844,7 +864,7 @@ __device__ __forceinline__ bool solve_row(const double* __restrict__ tab, int le
         acc = __dadd_rn(acc, __dmul_rn(di, pn));
         di = __dadd_rn(di, 1.0);
         sum_p = __dadd_rn(sum_p, pn);
-        p = div_recip(__dmul_rn(p, lam), A);
+        p = div_rate(__dmul_rn(p, lam), A);
         A = B;
     }
     acc_out = acc;

@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
         if (n < len) {
             const float srf = serv_rate(q, n + 1);
             const double sr = (double)srf;
-            const Recip r = make_recip(sr);
+            const RateRecip r = make_rate_recip(srf);
             out[4 * n + 0] = sr;
             out[4 * n + 1] = r.yh;
             out[4 * n + 2] = r.yl;
