@@ -408,6 +408,32 @@ void launch_fallback(wva_handle* h, void (*kernel)(Args, FbRun), const Args& g, 
     h->launches++;
 }
 
+// Enqueues kernel(args...) with one thread per record of an n_rec-record block (trivial_kernel, profile_kernel, ...).
+// The overload of kernel is the one whose parameters are exactly the arguments' types.
+template <class... Args>
+void launch_records(wva_handle* h, long long n_rec, void (*kernel)(Args...), const Args&... args) {
+    if (n_rec <= 0) return;
+    kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(args...);
+    h->launches++;
+}
+
+// Enqueues a tail kernel (load_kernel, slo_kernel, workload_kernel, sweep_kernel) whose warps take their items from
+// a work counter: at most 8 blocks of 256 threads per SM, and no more than `warps` warps.  Then records ev_k1 (the
+// call's kernel time ends with the tail) and re-runs the items it bailed on (fallback over fb).
+template <class Args>
+int launch_tail(wva_handle* h, void (*kernel)(Args), void (*fallback)(Args, FbRun), const Args& g, long long warps,
+                const FbRun& fb) {
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, 0));
+    per_sm = std::max(1, std::min(per_sm, 8));
+    const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
+    kernel<<<blocks, 256, 0, h->stream>>>(g);
+    h->launches++;
+    CK(cudaEventRecord(h->ev_k1, h->stream));
+    launch_fallback(h, fallback, g, fb);
+    return WVA_OK;
+}
+
 // The (server, accelerator) pairs of hf that keep(s, a) accepts, as ids s * A + a with their batch sizes N, sorted
 // by descending N (stable: equal N keep the pair order).
 template <class Keep>
@@ -642,21 +668,10 @@ int enqueue_candidates(wva_handle* h, SizeArgs& g, int Nmax, SizeMode mode = SIZ
     return WVA_OK;
 }
 
-// Enqueue analyze (+ unlimited solve). cand/winner columns are device pointers.
-int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners) {
-    int rc = prepare_size(h);
-    if (rc) return rc;
-    rc = ensure_ctrl(h);
-    if (rc) return rc;
-    const HostFleet& hf = h->hf;
-    const int n_pairs = hf.S * hf.A;
-    if (n_pairs > 0) {
-        trivial_kernel<<<(n_pairs + 255) / 256, 256, 0, h->stream>>>(h->df, cand, (const int*)nullptr, 1);
-        h->launches++;
-    }
-    const PairTables& pt = h->size_tabs;
+// The size drivers' arguments for fleet f: one candidate per table of pt, written into cand by pair id.
+SizeArgs size_args(const DevFleet& f, const PairTables& pt, const AllocCols& cand) {
     SizeArgs g{};
-    g.f = h->df;
+    g.f = f;
     g.cand_pair = pt.pair();
     g.cand_N = pt.len();
     g.n_cand = pt.n;
@@ -665,6 +680,19 @@ int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners)
     g.ls = (const float*)pt.ls.p;
     g.place = CandPlace{nullptr, nullptr};
     g.cand = cand;
+    return g;
+}
+
+// Enqueue analyze (+ unlimited solve). cand/winner columns are device pointers.
+int enqueue_size(wva_handle* h, const AllocCols& cand, const AllocCols* winners) {
+    int rc = prepare_size(h);
+    if (rc) return rc;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const HostFleet& hf = h->hf;
+    launch_records(h, (long long)hf.S * hf.A, trivial_kernel, h->df, cand, (const int*)nullptr, 1);
+    const PairTables& pt = h->size_tabs;
+    SizeArgs g = size_args(h->df, pt, cand);
     rc = enqueue_candidates(h, g, pt.len_max);
     if (rc) return rc;
     if (winners && hf.S > 0) {
@@ -751,6 +779,37 @@ int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
     return WVA_OK;
 }
 
+// The entry of the calls over L rows of a fleet with L candidate and L winner blocks (the load, SLO, workload and
+// profile grids, the workload and profile traces), named `name` in wva_last_error: the argument checks, the upload,
+// then enqueue(dc, dw) under run_host and both blocks back to the caller.  null_rows is the call's refusal when some
+// row list it needs is NULL (it applies when S * L > 0), or NULL; with row_entries the L * M * A entries of a
+// wva_profile_rows list are bounded as well.  A trace's rows are ticks, a grid's levels.
+template <class Enqueue>
+int run_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const char* name, const char* null_rows,
+               bool row_entries, wva_allocs* candidates, wva_allocs* winners, Enqueue&& enqueue) {
+    if (!h || !winners) return WVA_ERR_BAD_ARG;
+    if (L < 0) return h->fail(WVA_ERR_BAD_ARG, strstr(name, "trace") ? "negative tick count" : "negative level count");
+    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
+    if ((long long)fleet->n_servers * L > 0 && null_rows) return h->fail(WVA_ERR_BAD_ARG, null_rows);
+    const long long n_cand = (long long)fleet->n_servers * fleet->n_acc * L;
+    if (n_cand >= (1ll << 31) || (row_entries && (long long)L * fleet->n_models * fleet->n_acc >= (1ll << 31))) {
+        const std::string what = std::string(name) + " too large for one call (>= 2^31 candidates" +
+                                 (row_entries ? " or row entries)" : ")");
+        return h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
+    }
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    HostCall c{(size_t)n_cand, candidates != nullptr, true};
+    c.win_blocks = (size_t)L;
+    rc = run_host(h, c, enqueue);
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    scatter_block(c.win_host, c.bw, winners);
+    return WVA_OK;
+}
+
 // ---- size grid: CreateAllocation at every listed batch size --------------------------------------
 // The load pairs x the batch list, sorted by descending N (stable: pair order, then list order), with one
 // Bmax-long table per pair that the pair's candidates share.  Enqueues the nil / zero-load candidates,
@@ -793,23 +852,15 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
-    const int n_rec = hf.S * hf.A * B;
     const char* d = (const char*)pt.lists.p;
     const int* d_batch = (const int*)(d + o_bl);
-    if (n_rec > 0) {
-        trivial_kernel<<<(n_rec + 255) / 256, 256, 0, h->stream>>>(h->df, cand, d_batch, B);
-        h->launches++;
-    }
-    SizeArgs g{};
-    g.f = h->df;
+    launch_records(h, (long long)hf.S * hf.A * B, trivial_kernel, h->df, cand, d_batch, B);
+    SizeArgs g = size_args(h->df, pt, cand);
     g.cand_pair = (const int*)(d + o_pair);
     g.cand_N = (const int*)(d + o_N);
     g.n_cand = n;
-    g.tab = (const double*)pt.tab.p;
     g.tab_off = (const long long*)(d + o_off);
-    g.ls = (const float*)pt.ls.p;
     g.place = CandPlace{(const int*)(d + o_idx), (const int*)(d + o_rec)};
-    g.cand = cand;
     rc = enqueue_candidates(h, g, Bmax);
     if (rc) return rc;
     if (hf.S > 0) {
@@ -828,8 +879,8 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
 //
 // prepare_load_star uploads the candidate lists of fleet hf with the caller's columns (laid out in c, written by
 // fill; `pairs` holds the candidates' pair ids by the time fill runs).  enqueue_load_star then builds the tables
-// for the device image f of the same fleet, sizes fallback list 1 for the caller's tail (up to fb2_cap entries)
-// and enqueues phase 1.
+// for the device image f of the same fleet and sizes fallback list 1 for the caller's tail (prepare_tail, which the
+// SLO grid shares), and enqueues phase 1.
 struct LoadStar {
     int n = 0;           // candidates
     AllocCols star{};    // rateStar mode's records by pair id: feasible and max_rate = rateStar
@@ -845,6 +896,14 @@ int prepare_load_star(wva_handle* h, const HostFleet& hf, const std::vector<char
     if (rc) return rc;
     return upload_tables(h, h->lg_tabs, pairs, Ns, true, c, fill);
 }
+// Builds lg_tabs' tables for fleet f and sizes the tail's fallback list (list 1, up to fb2_cap entries) before
+// phase 1 is enqueued (which sizes the scratch for the same len_max).  Needs ensure_ctrl.
+int prepare_tail(wva_handle* h, const DevFleet& f, long long fb2_cap, FbRun& fb2) {
+    const PairTables& pt = h->lg_tabs;
+    const int rc = build_tables(h, f, pt);
+    if (rc) return rc;
+    return prepare_fallback(h, 1, (int)std::min<long long>(fb2_cap, 1 << 22), pt.n ? pt.len_max : 0, fb2);
+}
 int enqueue_load_star(wva_handle* h, const HostFleet& hf, const DevFleet& f, long long fb2_cap, LoadStar& ls) {
     const PairTables& pt = h->lg_tabs;
     const size_t n_pairs = (size_t)hf.S * hf.A;
@@ -852,24 +911,24 @@ int enqueue_load_star(wva_handle* h, const HostFleet& hf, const DevFleet& f, lon
     ls.star = AllocCols{};
     ls.star.max_rate = (float*)h->d_lg_star.p;
     ls.star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
-    int rc = build_tables(h, f, pt);
-    if (rc) return rc;
-    // the tail's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
-    rc = prepare_fallback(h, 1, (int)std::min<long long>(fb2_cap, 1 << 22), pt.n ? pt.len_max : 0, ls.fb2);
+    const int rc = prepare_tail(h, f, fb2_cap, ls.fb2);
     if (rc) return rc;
     ls.n = pt.n;
-    SizeArgs& g = ls.g;
-    g = SizeArgs{};
-    g.f = f;
-    g.cand_pair = pt.pair();
-    g.cand_N = pt.len();
-    g.n_cand = pt.n;
-    g.tab = (const double*)pt.tab.p;
-    g.tab_off = pt.off();
-    g.ls = (const float*)pt.ls.p;
-    g.place = CandPlace{nullptr, nullptr};
-    g.cand = ls.star;
-    return enqueue_candidates(h, g, pt.len_max, SIZE_STAR);
+    ls.g = size_args(f, pt, ls.star);
+    return enqueue_candidates(h, ls.g, pt.len_max, SIZE_STAR);
+}
+
+// The winners of an L-block call: per block the unlimited winner (unlimited_kernel), or with `trace` the workload
+// trace's tick chain (trace_kernel), in which block l's winners are block l + 1's current allocation.
+void enqueue_level_winners(wva_handle* h, const AllocCols& cand, const AllocCols& winners, int L, bool trace) {
+    const int S = h->hf.S;
+    if (S <= 0 || L <= 0) return;
+    if (trace)
+        trace_kernel<<<(unsigned)((S + 127) / 128), 128, 0, h->stream>>>(h->df, cand, winners, L);
+    else
+        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
+            h->df, cand, winners, L);
+    h->launches++;
 }
 // The tail's view of phase 1: fleet, candidates, tables and rateStar records (the level list is the caller's).
 LoadArgs load_args(const LoadStar& ls) {
@@ -906,36 +965,20 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     const float* d_rpm = (const float*)((const char*)h->lg_tabs.lists.p + o_rpm);
     rc = ensure_ctrl(h);
     if (rc) return rc;
-    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
-    if (n_rec > 0) {
-        trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(h->df, cand, d_rpm, L);
-        h->launches++;
-    }
+    launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, d_rpm, L);
     LoadStar ls;
     rc = enqueue_load_star(h, hf, h->df, n_items, ls);
     if (rc) return rc;
-    const FbRun& fb2 = ls.fb2;
     if (n > 0 && L > 0) {
         LoadArgs la = load_args(ls);
         la.level_rpm = d_rpm;
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
         la.cand = cand;
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, load_kernel, 256, 0));
-        per_sm = std::max(1, std::min(per_sm, 8));
-        const long long warps = (n_items + 31) / 32;
-        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
-        load_kernel<<<blocks, 256, 0, h->stream>>>(la);
-        h->launches++;
-        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
-        launch_fallback(h, load_fallback, la, fb2);
+        rc = launch_tail(h, load_kernel, load_fallback, la, (n_items + 31) / 32, ls.fb2);
+        if (rc) return rc;
     }
-    if (S > 0 && L > 0) {
-        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
-            h->df, cand, winners, L);
-        h->launches++;
-    }
+    enqueue_level_winners(h, cand, winners, L, false);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1110,36 +1153,25 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
     if (rc) return rc;
     const PairTables& pt = h->lg_tabs;
     const char* d = (const char*)pt.lists.p;
-    rc = build_tables(h, h->df, pt);
-    if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
     const long long n_items = (long long)pt.n * L;
-    // the tail's fallback list, sized before phase 1 is enqueued (which sizes the scratch for the same len_max)
     FbRun fb2;
-    rc = prepare_fallback(h, 1, (int)std::min<long long>(n_items, 1 << 22), pt.n ? pt.len_max : 0, fb2);
+    rc = prepare_tail(h, h->df, n_items, fb2);
     if (rc) return rc;
     const size_t n_srec = (size_t)n_keys * A;
     CK(h->d_slo.ensure(5 * n_srec + 16));
-    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
-    if (n_rec > 0) {
-        trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(h->df, cand, L);
-        h->launches++;
-    }
+    launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, L);
     // phase 1: the searches
     AllocCols srch{};
     srch.max_rate = (float*)h->d_slo.p;
     srch.feasible = (uint8_t*)h->d_slo.p + 4 * n_srec;
-    SizeArgs g{};
-    g.f = h->df;
+    SizeArgs g = size_args(h->df, pt, srch);
     g.cand_pair = (const int*)(d + o_pair);
     g.cand_N = (const int*)(d + o_N);
     g.n_cand = (int)n;
-    g.tab = (const double*)pt.tab.p;
     g.tab_off = (const long long*)(d + o_off);
-    g.ls = (const float*)pt.ls.p;
     g.place = CandPlace{(const int*)(d + o_idx), (const int*)(d + o_rec)};
-    g.cand = srch;
     rc = enqueue_candidates(h, g, pt.len_max, SIZE_SEARCH,
                             SearchCols{(const uint8_t*)(d + o_which), (const float*)(d + o_tgt)});
     if (rc) return rc;
@@ -1162,21 +1194,10 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
         la.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
         la.cand = cand;
         la.fb = fb2.list;
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, slo_kernel, 256, 0));
-        per_sm = std::max(1, std::min(per_sm, 8));
-        const long long warps = (n_items + 31) / 32;
-        const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
-        slo_kernel<<<blocks, 256, 0, h->stream>>>(la);
-        h->launches++;
-        CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: both phases
-        launch_fallback(h, slo_fallback, la, fb2);
+        rc = launch_tail(h, slo_kernel, slo_fallback, la, (n_items + 31) / 32, fb2);
+        if (rc) return rc;
     }
-    if (S > 0 && L > 0) {
-        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
-            h->df, cand, winners, L);
-        h->launches++;
-    }
+    enqueue_level_winners(h, cand, winners, L, false);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1266,16 +1287,7 @@ int enqueue_workload_tail(wva_handle* h, const LoadStar& ls, WorkloadArgs& g, co
     g.ld.L = L;
     g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
     g.ld.cand = cand;
-    int per_sm = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, workload_kernel, 256, 0));
-    per_sm = std::max(1, std::min(per_sm, 8));
-    const long long warps = ((long long)g.n_items + 31) / 32;
-    const unsigned blocks = (unsigned)std::min<long long>((long long)h->sm_count * per_sm, (warps + 7) / 8);
-    workload_kernel<<<blocks, 256, 0, h->stream>>>(g);
-    h->launches++;
-    CK(cudaEventRecord(h->ev_k1, h->stream));
-    launch_fallback(h, workload_fallback, g, ls.fb2);
-    return WVA_OK;
+    return launch_tail(h, workload_kernel, workload_fallback, g, ((long long)g.n_items + 31) / 32, ls.fb2);
 }
 
 // The levels at which server s is a load under the rows rpm / in / out [L*S] (rate not negative and not 0, NaN and
@@ -1297,9 +1309,13 @@ void load_groups(int L, int S, int s, const float* rpm, const int32_t* in, const
     }
 }
 
-// Key rows (server, in_tokens, out_tokens) with their levels: row k's are lev[lev_off[k] .. lev_off[k + 1]).
+// Key rows (server, in_tokens, out_tokens) with their levels: row k's are lev[lev_off[k] .. lev_off[k + 1]).  On
+// the device the workload grid's tail reads the servers, the level lists and each candidate's first item, which
+// lie in the call's upload image (place, write) and which args() hands to a WorkloadArgs.
 struct TokenKeys {
     std::vector<int> srv, in, out, lev_off{0}, lev;
+    size_t o_srv = 0, o_loff = 0, o_lev = 0, o_item = 0;
+    int n_items = 0;  // set by write
     void add(int s, int ki, int ko) {
         srv.push_back(s);
         in.push_back(ki);
@@ -1309,6 +1325,37 @@ struct TokenKeys {
     void add_level(int l) {
         lev.push_back(l);
         lev_off.back()++;
+    }
+    // room for the key rows and the item offsets of up to n_cand candidates
+    void place(Cols& c, size_t n_cand) {
+        o_srv = c.take(4 * srv.size());
+        o_loff = c.take(4 * lev_off.size());
+        o_lev = c.take(4 * lev.size());
+        o_item = c.take(4 * (n_cand + 1));
+    }
+    // The key rows, and candidate j's items: one per level of its key row pairs[j] / A.
+    void write(char* p, const std::vector<int>& pairs, int A) {
+        if (!srv.empty()) memcpy(p + o_srv, srv.data(), 4 * srv.size());
+        memcpy(p + o_loff, lev_off.data(), 4 * lev_off.size());
+        if (!lev.empty()) memcpy(p + o_lev, lev.data(), 4 * lev.size());
+        int* item = (int*)(p + o_item);
+        item[0] = 0;
+        for (size_t j = 0; j < pairs.size(); ++j) {
+            const int k = pairs[j] / A;
+            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
+        }
+        n_items = item[pairs.size()];
+    }
+    // the tail's lists uploaded at d, for levels of S servers
+    WorkloadArgs args(const char* d, int S) const {
+        WorkloadArgs g{};
+        g.key_srv = (const int*)(d + o_srv);
+        g.lev_off = (const int*)(d + o_loff);
+        g.lev = (const int*)(d + o_lev);
+        g.item_off = (const int*)(d + o_item);
+        g.S = S;
+        g.n_items = n_items;
+        return g;
     }
 };
 // The workload grid's keys (DESIGN.md §3.12): per server, its distinct (in, out) under load, ascending.
@@ -1325,51 +1372,41 @@ void token_keys(int L, int S, const float* rpm, const int32_t* in, const int32_t
 // is the load grid's, run once on the key fleet: one row per distinct (server, in_tokens, out_tokens) that some
 // level uses under load (rate not negative and not 0, NaN and +Inf included; in_tokens >= 0; out_tokens >= 1).
 // Phase 2 (workload_kernel, workload_fallback) is the load grid's tail per (key candidate, level of the key).  The
-// lists, the key fleet's server columns and the tables go into lg_tabs, rebuilt on every call.  rpm / in / out
-// [L*S] are the caller's rows; cand ([L*S*A]) is a device column.
+// lists, the key fleet's server columns and the tables go into lg_tabs, rebuilt on every call.  Then the unlimited
+// winner of every level.  rpm / in / out [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device
+// columns.
 //
 // With `trace` (the workload trace, DESIGN.md §3.13) the records are CreateAllocation without the keepAccelerator
 // mask, which trace_kernel applies tick by tick: trivial_kernel sees an all-zero keep column, and the key fleet keeps
-// keepAccelerator only on the pinned servers, so that phase 1 sizes their current accelerator alone.
-int enqueue_workload_sizing(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                            const AllocCols& cand, bool trace) {
+// keepAccelerator only on the pinned servers, so that phase 1 sizes their current accelerator alone.  trace_kernel's
+// chain then picks the winners: one thread per server applies the mask against its current allocation, picks the
+// winner and advances.
+int enqueue_workload(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                     const AllocCols& cand, const AllocCols& winners, bool trace) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     const size_t LS = (size_t)L * S;
     // the keys: at most L * S, so fewer than 2^31 key candidates
     TokenKeys tk;
     token_keys(L, S, rpm, in, out, tk);
-    const std::vector<int>&key_srv = tk.srv, &lev_off = tk.lev_off, &lev = tk.lev;
-    const int K = (int)key_srv.size();
-    KeyFleet kf(hf, key_srv, tk.in, tk.out);
+    const int K = (int)tk.srv.size();
+    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
     if (trace)
-        for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, key_srv[k]);
+        for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, tk.srv[k]);
     Cols c(16);
     kf.place(c);
-    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS),
-                 o_ksrv = c.take(4 * (size_t)K), o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * lev.size()),
-                 o_item = c.take(4 * ((size_t)K * A + 1));
+    tk.place(c, (size_t)K * A);
+    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS);
     const size_t o_nokeep = trace ? c.take(S) : 0;  // the trace's all-zero keep column
     std::vector<int> pairs;
-    int n_items = 0;
     int rc = prepare_load_star(h, kf.hf, std::vector<char>(K, 1), pairs, c, [&](char* p) {
         kf.write(p);
+        tk.write(p, pairs, A);
         if (LS) {
             memcpy(p + o_rpm, rpm, 4 * LS);
             memcpy(p + o_in, in, 4 * LS);
             memcpy(p + o_out, out, 4 * LS);
         }
-        if (K) memcpy(p + o_ksrv, key_srv.data(), 4 * (size_t)K);
-        memcpy(p + o_loff, lev_off.data(), 4 * ((size_t)K + 1));
-        if (!lev.empty()) memcpy(p + o_lev, lev.data(), 4 * lev.size());
-        // candidate j's items: one per level of its key
-        int* item = (int*)(p + o_item);
-        item[0] = 0;
-        for (size_t j = 0; j < pairs.size(); ++j) {
-            const int k = pairs[j] / A;
-            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
-        }
-        n_items = item[pairs.size()];
         if (trace) memset(p + o_nokeep, 0, S);
     });
     if (rc) return rc;
@@ -1377,56 +1414,17 @@ int enqueue_workload_sizing(wva_handle* h, int L, const float* rpm, const int32_
     const float* d_rpm = (const float*)(d + o_rpm);
     rc = ensure_ctrl(h);
     if (rc) return rc;
-    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
-    if (n_rec > 0) {
-        DevFleet tf = h->df;
-        if (trace) tf.srv_keep_acc = (const uint8_t*)(d + o_nokeep);
-        trivial_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(
-            tf, cand, d_rpm, (const int*)(d + o_in), (const int*)(d + o_out), L);
-        h->launches++;
-    }
+    DevFleet tf = h->df;
+    if (trace) tf.srv_keep_acc = (const uint8_t*)(d + o_nokeep);
+    launch_records(h, (long long)S * A * L, trivial_kernel, tf, cand, d_rpm, (const int*)(d + o_in),
+                   (const int*)(d + o_out), L);
     LoadStar ls;
-    rc = enqueue_load_star(h, kf.hf, kf.view(h->df, d), n_items, ls);
+    rc = enqueue_load_star(h, kf.hf, kf.view(h->df, d), tk.n_items, ls);
     if (rc) return rc;
-    WorkloadArgs g{};
-    g.key_srv = (const int*)(d + o_ksrv);
-    g.lev_off = (const int*)(d + o_loff);
-    g.lev = (const int*)(d + o_lev);
-    g.item_off = (const int*)(d + o_item);
-    g.S = S;
-    g.n_items = n_items;
+    WorkloadArgs g = tk.args(d, S);
     rc = enqueue_workload_tail(h, ls, g, d_rpm, L, cand);
     if (rc) return rc;
-    CK(cudaGetLastError());
-    return WVA_OK;
-}
-
-// The workload grid: the sizing above, then the unlimited winner of every level (winners [L*S], a device column).
-int enqueue_workload_grid(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                          const AllocCols& cand, const AllocCols& winners) {
-    const int rc = enqueue_workload_sizing(h, L, rpm, in, out, cand, false);
-    if (rc) return rc;
-    if (h->hf.S > 0 && L > 0) {
-        unlimited_kernel<<<dim3((unsigned)((h->hf.S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0,
-                           h->stream>>>(h->df, cand, winners, L);
-        h->launches++;
-    }
-    CK(cudaGetLastError());
-    return WVA_OK;
-}
-
-// ---- workload trace: the reconcile replayed tick by tick (DESIGN.md §3.13) ------------------------------------
-// The workload grid's sizing of every tick in one pass, without the keepAccelerator mask, then trace_kernel's chain:
-// one thread per server applies the mask against its current allocation, picks the winner and advances.  rpm / in /
-// out [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device columns.
-int enqueue_workload_trace(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                           const AllocCols& cand, const AllocCols& winners) {
-    const int rc = enqueue_workload_sizing(h, L, rpm, in, out, cand, true);
-    if (rc) return rc;
-    if (h->hf.S > 0 && L > 0) {
-        trace_kernel<<<(unsigned)((h->hf.S + 127) / 128), 128, 0, h->stream>>>(h->df, cand, winners, L);
-        h->launches++;
-    }
+    enqueue_level_winners(h, cand, winners, L, trace);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1665,7 +1663,8 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
         if (!rank.empty()) memcpy(p + o_rank, rank.data(), 4 * rank.size());
         memcpy(p + o_poff, pair_off.data(), 4 * pair_off.size());
         if (!key_of.empty()) memcpy(p + o_keyof, key_of.data(), 4 * key_of.size());
-        // the tail's one level: key k is server k of the key fleet, candidate e item e
+        // the tail's one level: key k is server k of the key fleet, candidate e item e (written in place: building
+        // them as TokenKeys costs the host measurably more at 10^5 keys)
         int* ksrv = (int*)(p + o_ksrv);
         int* loff = (int*)(p + o_loff);
         int* item = (int*)(p + o_item);
@@ -1691,25 +1690,17 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
     t.n_items = n;
     rc = enqueue_workload_tail(h, ls, t, kd.srv_arrival_rpm, 1, key);
     if (rc) return rc;
-    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
-    if (n_rec > 0) {
-        ProfileArgs g{};
-        g.f = h->df;
-        pr.set_rows(g, d);
-        g.rank = pr.perf_rows ? (const int*)(d + o_rank) : nullptr;
-        g.pair_off = (const int*)(d + o_poff);
-        g.key_of = (const int*)(d + o_keyof);
-        g.key = key;
-        g.cand = cand;
-        g.L = L;
-        profile_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(g);
-        h->launches++;
-    }
-    if (S > 0 && L > 0) {
-        unlimited_kernel<<<dim3((unsigned)((S + 127) / 128), (unsigned)std::min(L, 65535)), 128, 0, h->stream>>>(
-            h->df, cand, winners, L);
-        h->launches++;
-    }
+    ProfileArgs g{};
+    g.f = h->df;
+    pr.set_rows(g, d);
+    g.rank = pr.perf_rows ? (const int*)(d + o_rank) : nullptr;
+    g.pair_off = (const int*)(d + o_poff);
+    g.key_of = (const int*)(d + o_keyof);
+    g.key = key;
+    g.cand = cand;
+    g.L = L;
+    launch_records(h, (long long)S * A * L, profile_kernel, g);
+    enqueue_level_winners(h, cand, winners, L, false);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -1784,12 +1775,11 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
             });
         }
     }
-    const std::vector<int>&key_srv = tk.srv, &lev_off = tk.lev_off, &lev = tk.lev;
-    const int K = (int)key_srv.size();  // at most L * S * A
+    const int K = (int)tk.srv.size();  // at most L * S * A
     // the key fleet's pair ids k * A + a are int
     if ((long long)K * A >= (1ll << 31))
         return h->fail(WVA_ERR_UNSUPPORTED, "profile trace too large for one call (>= 2^31 key pairs x accelerators)");
-    KeyFleet kf(hf, key_srv, tk.in, tk.out);
+    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
     HostFleet& kh = kf.hf;
     if (pr.perf_rows) {
         kf.own_ma = true;
@@ -1800,73 +1790,47 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
         }
         pr.fill(kh);
     } else {  // the workload trace's key fleet
-        for (int k = 0; k < K; ++k) kh.srv_keep_acc[k] = pin[key_srv[k]];
+        for (int k = 0; k < K; ++k) kh.srv_keep_acc[k] = pin[tk.srv[k]];
     }
     Cols c(16);
     kf.place(c);
     pr.place(c);
     // the tail's candidates: one per key row with a perf column, up to A without
-    const size_t n_cand_max = pr.perf_rows ? (size_t)K : (size_t)K * A;
-    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS), o_pin = c.take(S),
-                 o_ksrv = c.take(4 * (size_t)K), o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * lev.size()),
-                 o_item = c.take(4 * (n_cand_max + 1));
+    tk.place(c, pr.perf_rows ? (size_t)K : (size_t)K * A);
+    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS), o_pin = c.take(S);
     std::vector<int> pairs;
-    int n_items = 0;
     int rc = prepare_load_star(h, kh, std::vector<char>(K, 1), pairs, c, [&](char* p) {
         kf.write(p);
         pr.write(p);
+        tk.write(p, pairs, A);
         if (LS) {
             memcpy(p + o_rpm, rpm, 4 * LS);
             memcpy(p + o_in, in, 4 * LS);
             memcpy(p + o_out, out, 4 * LS);
         }
         if (S) memcpy(p + o_pin, pin.data(), S);
-        if (K) memcpy(p + o_ksrv, key_srv.data(), 4 * (size_t)K);
-        memcpy(p + o_loff, lev_off.data(), 4 * ((size_t)K + 1));
-        if (!lev.empty()) memcpy(p + o_lev, lev.data(), 4 * lev.size());
-        // candidate j's items: one per tick of its key row
-        int* item = (int*)(p + o_item);
-        item[0] = 0;
-        for (size_t j = 0; j < pairs.size(); ++j) {
-            const int k = pairs[j] / A;
-            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
-        }
-        n_items = item[pairs.size()];
     });
     if (rc) return rc;
     const char* d = (const char*)h->lg_tabs.lists.p;
     rc = ensure_ctrl(h);
     if (rc) return rc;
     LoadStar ls;
-    rc = enqueue_load_star(h, kh, kf.view(h->df, d), n_items, ls);
+    rc = enqueue_load_star(h, kh, kf.view(h->df, d), tk.n_items, ls);
     if (rc) return rc;
-    WorkloadArgs g{};
-    g.key_srv = (const int*)(d + o_ksrv);
-    g.lev_off = (const int*)(d + o_loff);
-    g.lev = (const int*)(d + o_lev);
-    g.item_off = (const int*)(d + o_item);
-    g.S = S;
-    g.n_items = n_items;
+    WorkloadArgs g = tk.args(d, S);
     rc = enqueue_workload_tail(h, ls, g, (const float*)(d + o_rpm), L, cand);
     if (rc) return rc;
-    const long long n_rec = (long long)S * A * L;  // < 2^31 (checked by the caller)
-    if (n_rec > 0) {
-        ProfileTraceArgs r{};
-        r.p.f = h->df;
-        r.p.f.srv_keep_acc = (const uint8_t*)(d + o_pin);
-        pr.set_rows(r.p, d);
-        r.p.cand = cand;
-        r.p.L = L;
-        r.level_rpm = (const float*)(d + o_rpm);
-        r.level_in = (const int*)(d + o_in);
-        r.level_out = (const int*)(d + o_out);
-        profile_trace_kernel<<<(unsigned)((n_rec + 255) / 256), 256, 0, h->stream>>>(r);
-        h->launches++;
-    }
-    if (S > 0 && L > 0) {
-        trace_kernel<<<(unsigned)((S + 127) / 128), 128, 0, h->stream>>>(h->df, cand, winners, L);
-        h->launches++;
-    }
+    ProfileTraceArgs r{};
+    r.p.f = h->df;
+    r.p.f.srv_keep_acc = (const uint8_t*)(d + o_pin);
+    pr.set_rows(r.p, d);
+    r.p.cand = cand;
+    r.p.L = L;
+    r.level_rpm = (const float*)(d + o_rpm);
+    r.level_in = (const int*)(d + o_in);
+    r.level_out = (const int*)(d + o_out);
+    launch_records(h, (long long)S * A * L, profile_trace_kernel, r);
+    enqueue_level_winners(h, cand, winners, L, true);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -2715,148 +2679,61 @@ int wva_size_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_batch, const 
 
 int wva_load_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                   wva_allocs* candidates, wva_allocs* winners) {
-    if (!h || !winners) return WVA_ERR_BAD_ARG;
-    if (n_levels < 0 || (n_levels > 0 && !arrival_rpm))
+    if (h && winners && (n_levels < 0 || (n_levels > 0 && !arrival_rpm)))
         return h->fail(WVA_ERR_BAD_ARG, "negative level count or NULL level list");
-    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
-    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "load grid too large for one call (>= 2^31 candidates)");
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
-    c.win_blocks = (size_t)n_levels;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
-        return enqueue_load_grid(h, n_levels, arrival_rpm, dc, dw);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, candidates);
-    scatter_block(c.win_host, c.bw, winners);
-    return WVA_OK;
+    return run_levels(h, fleet, n_levels, "load grid", nullptr, false, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_load_grid(h, n_levels, arrival_rpm, dc, dw);
+                      });
 }
 
 int wva_slo_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* slo_itl,
                  const float* slo_ttft, const float* slo_tps, wva_allocs* candidates, wva_allocs* winners) {
-    if (!h || !winners) return WVA_ERR_BAD_ARG;
-    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
-    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
-    if ((long long)fleet->n_servers * n_levels > 0 && (!slo_itl || !slo_ttft || !slo_tps))
-        return h->fail(WVA_ERR_BAD_ARG, "NULL target row list");
-    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "SLO grid too large for one call (>= 2^31 candidates)");
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
-    c.win_blocks = (size_t)n_levels;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
-        return enqueue_slo_grid(h, n_levels, slo_itl, slo_ttft, slo_tps, dc, dw);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, candidates);
-    scatter_block(c.win_host, c.bw, winners);
-    return WVA_OK;
+    const char* null_rows = !slo_itl || !slo_ttft || !slo_tps ? "NULL target row list" : nullptr;
+    return run_levels(h, fleet, n_levels, "SLO grid", null_rows, false, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_slo_grid(h, n_levels, slo_itl, slo_ttft, slo_tps, dc, dw);
+                      });
 }
 
 int wva_workload_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                       const int32_t* in_tokens, const int32_t* out_tokens, wva_allocs* candidates,
                       wva_allocs* winners) {
-    if (!h || !winners) return WVA_ERR_BAD_ARG;
-    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
-    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
-    if ((long long)fleet->n_servers * n_levels > 0 && (!arrival_rpm || !in_tokens || !out_tokens))
-        return h->fail(WVA_ERR_BAD_ARG, "NULL row list");
-    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "workload grid too large for one call (>= 2^31 candidates)");
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
-    c.win_blocks = (size_t)n_levels;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
-        return enqueue_workload_grid(h, n_levels, arrival_rpm, in_tokens, out_tokens, dc, dw);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, candidates);
-    scatter_block(c.win_host, c.bw, winners);
-    return WVA_OK;
+    const char* null_rows = !arrival_rpm || !in_tokens || !out_tokens ? "NULL row list" : nullptr;
+    return run_levels(h, fleet, n_levels, "workload grid", null_rows, false, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_workload(h, n_levels, arrival_rpm, in_tokens, out_tokens, dc, dw, false);
+                      });
 }
 
 int wva_workload_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                        const int32_t* in_tokens, const int32_t* out_tokens, wva_allocs* candidates,
                        wva_allocs* winners) {
-    if (!h || !winners) return WVA_ERR_BAD_ARG;
-    if (n_ticks < 0) return h->fail(WVA_ERR_BAD_ARG, "negative tick count");
-    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
-    if ((long long)fleet->n_servers * n_ticks > 0 && (!arrival_rpm || !in_tokens || !out_tokens))
-        return h->fail(WVA_ERR_BAD_ARG, "NULL row list");
-    if ((long long)fleet->n_servers * fleet->n_acc * n_ticks >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "workload trace too large for one call (>= 2^31 candidates)");
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_ticks, candidates != nullptr, true};
-    c.win_blocks = (size_t)n_ticks;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
-        return enqueue_workload_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens, dc, dw);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, candidates);
-    scatter_block(c.win_host, c.bw, winners);
-    return WVA_OK;
+    const char* null_rows = !arrival_rpm || !in_tokens || !out_tokens ? "NULL row list" : nullptr;
+    return run_levels(h, fleet, n_ticks, "workload trace", null_rows, false, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_workload(h, n_ticks, arrival_rpm, in_tokens, out_tokens, dc, dw, true);
+                      });
 }
 
 int wva_profile_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const wva_profile_rows* rows,
                      wva_allocs* candidates, wva_allocs* winners) {
-    if (!h || !winners) return WVA_ERR_BAD_ARG;
-    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
-    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
-    if ((long long)fleet->n_servers * fleet->n_acc * n_levels >= (1ll << 31) ||
-        (long long)n_levels * fleet->n_models * fleet->n_acc >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "profile grid too large for one call (>= 2^31 candidates or row entries)");
     const wva_profile_rows own{};
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_levels, candidates != nullptr, true};
-    c.win_blocks = (size_t)n_levels;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
-        return enqueue_profile_grid(h, n_levels, rows ? *rows : own, dc, dw);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, candidates);
-    scatter_block(c.win_host, c.bw, winners);
-    return WVA_OK;
+    return run_levels(h, fleet, n_levels, "profile grid", nullptr, true, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_profile_grid(h, n_levels, rows ? *rows : own, dc, dw);
+                      });
 }
 
 int wva_profile_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                       const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
                       wva_allocs* candidates, wva_allocs* winners) {
-    if (!h || !winners) return WVA_ERR_BAD_ARG;
-    if (n_ticks < 0) return h->fail(WVA_ERR_BAD_ARG, "negative tick count");
-    if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
-    if ((long long)fleet->n_servers * fleet->n_acc * n_ticks >= (1ll << 31) ||
-        (long long)n_ticks * fleet->n_models * fleet->n_acc >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "profile trace too large for one call (>= 2^31 candidates or row entries)");
     const wva_profile_rows own{};
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    HostCall c{(size_t)fleet->n_servers * fleet->n_acc * n_ticks, candidates != nullptr, true};
-    c.win_blocks = (size_t)n_ticks;
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
-        return enqueue_profile_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens, rows ? *rows : own, dc, dw);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, candidates);
-    scatter_block(c.win_host, c.bw, winners);
-    return WVA_OK;
+    return run_levels(h, fleet, n_ticks, "profile trace", nullptr, true, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_profile_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens,
+                                                       rows ? *rows : own, dc, dw);
+                      });
 }
 
 int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_lo, const float* rpm_hi,
@@ -3084,17 +2961,11 @@ int wva_sweep(wva_handle* h, const wva_fleet* fleet, int32_t n_rates, wva_sweep_
         g.throughput = (float*)(p + o_thr);
         g.rho = (float*)(p + o_rho);
         g.fb = fb.list;
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sweep_kernel, 256, 0));
-        per_sm = std::max(1, std::min(per_sm, 8));
-        const unsigned items = (unsigned)n * g.n_chunks;
-        unsigned blocks = std::min<unsigned>((unsigned)(h->sm_count * per_sm), (items + 7) / 8);
         CK(cudaEventRecord(h->ev_k0, h->stream));
-        sweep_kernel<<<blocks, 256, 0, h->stream>>>(g);
-        h->launches++;
-        CK(cudaEventRecord(h->ev_k1, h->stream));
-        // the points whose chain left the streaming solve's window: stored vector, as the reference
-        launch_fallback(h, sweep_fallback, g, fb);
+        // one warp per (pair, chunk) item; the points whose chain left the streaming solve's window are re-run with
+        // the stored vector, as the reference
+        rc = launch_tail(h, sweep_kernel, sweep_fallback, g, (long long)((unsigned)n * g.n_chunks), fb);
+        if (rc) return rc;
         CK(cudaGetLastError());
         return WVA_OK;
     });

@@ -870,32 +870,39 @@ struct LevelRate {
     __device__ __forceinline__ float operator()(int s) const { return total_rate_of(at_level(g.f, g.level_rpm, l), s); }
 };
 
-__global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
-    const DevFleet& f = g.f;
+// The tails' work loop: each warp takes the next 32 items from the work counter until all n_items are handed out,
+// and lane i of a warp runs fn(item) on its item (lanes past n_items idle).
+template <class Fn>
+__device__ __forceinline__ void for_each_warp_item(unsigned* counter, unsigned n_items, Fn&& fn) {
     const int lane = threadIdx.x & 31;
-    const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
     for (;;) {
         unsigned w = 0;
-        if (lane == 0) w = atomicAdd(g.counter, 1u);
+        if (lane == 0) w = atomicAdd(counter, 1u);
         w = __shfl_sync(0xffffffffu, w, 0);
         if ((unsigned long long)w * 32 >= n_items) break;
         const unsigned i = w * 32 + lane;
-        if (i < n_items) {
-            const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
-            const float rpm = g.level_rpm[(size_t)l * f.S + g.cand_pair[e] / f.A];
-            if (!(rpm < 0.0f) && rpm != 0.0f) {  // else trivial_kernel's nil / zero-load record
-                const int N = g.cand_N[e], K = N + N * f.ratio;
-                const double* tab = g.tab + 4 * g.tab_off[e];
-                Cand c;
-                const bool ok = load_tail(g, e, LevelRate{g, l}, (float)tab[4 * (N - 1)],
-                                          [&](float lam, ModelStats& st) {
-                    return solve_shared(tab, N, K, lam, st) == kSolveOk;
-                }, c);
-                if (!ok) fb_push(g.fb, fb_pack(e, l));
-                store_cand(g.cand, load_record(g, e, l), c);
-            }
-        }
+        if (i < n_items) fn(i);
     }
+}
+
+__global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
+    const DevFleet& f = g.f;
+    const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
+    for_each_warp_item(g.counter, n_items, [&](unsigned i) {
+        const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
+        const float rpm = g.level_rpm[(size_t)l * f.S + g.cand_pair[e] / f.A];
+        if (!(rpm < 0.0f) && rpm != 0.0f) {  // else trivial_kernel's nil / zero-load record
+            const int N = g.cand_N[e], K = N + N * f.ratio;
+            const double* tab = g.tab + 4 * g.tab_off[e];
+            Cand c;
+            const bool ok = load_tail(g, e, LevelRate{g, l}, (float)tab[4 * (N - 1)],
+                                      [&](float lam, ModelStats& st) {
+                return solve_shared(tab, N, K, lam, st) == kSolveOk;
+            }, c);
+            if (!ok) fb_push(g.fb, fb_pack(e, l));
+            store_cand(g.cand, load_record(g, e, l), c);
+        }
+    });
 }
 
 // Stored-vector re-run of the items load_kernel bailed on.
@@ -999,24 +1006,16 @@ __device__ __forceinline__ size_t slo_record(const SloArgs& g, int e, int l) {
 }
 
 __global__ void __launch_bounds__(256) slo_kernel(SloArgs g) {
-    const int lane = threadIdx.x & 31;
     const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
-    for (;;) {
-        unsigned w = 0;
-        if (lane == 0) w = atomicAdd(g.counter, 1u);
-        w = __shfl_sync(0xffffffffu, w, 0);
-        if ((unsigned long long)w * 32 >= n_items) break;
-        const unsigned i = w * 32 + lane;
-        if (i < n_items) {
-            const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
-            Cand c;
-            const bool ok = slo_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-                return solve_shared(tab, N, K, lam, st) == kSolveOk;
-            }, c);
-            if (!ok) fb_push(g.fb, fb_pack(e, l));
-            store_cand(g.cand, slo_record(g, e, l), c);
-        }
-    }
+    for_each_warp_item(g.counter, n_items, [&](unsigned i) {
+        const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
+        Cand c;
+        const bool ok = slo_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+            return solve_shared(tab, N, K, lam, st) == kSolveOk;
+        }, c);
+        if (!ok) fb_push(g.fb, fb_pack(e, l));
+        store_cand(g.cand, slo_record(g, e, l), c);
+    });
 }
 
 // Stored-vector re-run of the items slo_kernel bailed on.
@@ -1083,26 +1082,17 @@ __device__ __forceinline__ bool workload_tail(const WorkloadArgs& g, int e, int 
 }
 
 __global__ void __launch_bounds__(256) workload_kernel(WorkloadArgs g) {
-    const int lane = threadIdx.x & 31;
-    const unsigned n_items = (unsigned)g.n_items;
-    for (;;) {
-        unsigned w = 0;
-        if (lane == 0) w = atomicAdd(g.ld.counter, 1u);
-        w = __shfl_sync(0xffffffffu, w, 0);
-        if ((unsigned long long)w * 32 >= n_items) break;
-        const unsigned i = w * 32 + lane;
-        if (i < n_items) {
-            int e, l;
-            workload_item(g, (int)i, e, l);
-            Cand c;
-            size_t rec;
-            const bool ok = workload_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-                return solve_shared(tab, N, K, lam, st) == kSolveOk;
-            }, c, rec);
-            if (!ok) fb_push(g.ld.fb, fb_pack(e, l));
-            store_cand(g.ld.cand, rec, c);
-        }
-    }
+    for_each_warp_item(g.ld.counter, (unsigned)g.n_items, [&](unsigned i) {
+        int e, l;
+        workload_item(g, (int)i, e, l);
+        Cand c;
+        size_t rec;
+        const bool ok = workload_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
+            return solve_shared(tab, N, K, lam, st) == kSolveOk;
+        }, c, rec);
+        if (!ok) fb_push(g.ld.fb, fb_pack(e, l));
+        store_cand(g.ld.cand, rec, c);
+    });
 }
 
 // Stored-vector re-run of the items workload_kernel bailed on.

@@ -40,8 +40,9 @@ def greedy_solve(fleet: Fleet, candidates: Allocs):
     return candidates, win
 
 
-# the fleet column each load row list replaces (every other row list is named after its column)
-_ROW_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens"}
+# the fleet column each load or target row list replaces (every other row list is named after its column)
+_ROW_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens",
+               "slo_itl": "srv_slo_itl", "slo_ttft": "srv_slo_ttft", "slo_tps": "srv_slo_tps"}
 _PROFILE_COLUMNS = ("acc_cost", "perf_present", "perf_alpha", "perf_beta", "perf_gamma", "perf_delta",
                     "perf_acc_count", "perf_max_batch", "perf_at_tokens")
 
@@ -167,20 +168,11 @@ class Engine:
         winner block ``l`` is ``solve``'s winners for it in unlimited mode (see ``wva_load_grid`` in
         include/wva_b200.h); ``fleet.srv_arrival_rpm`` is not read.  ``out``: an ``Allocs`` of ``L * S`` records
         to write the winners into."""
-        rpm = np.ascontiguousarray(arrival_rpm, np.float32)
-        if rpm.ndim != 2 or rpm.shape[1] != fleet.n_servers:
-            raise ValueError(f"arrival_rpm must have shape (L, {fleet.n_servers}), got {rpm.shape}")
-        L = rpm.shape[0]
-        if out is not None and out.n != L * fleet.n_servers:
-            raise ValueError("out must hold L * fleet.n_servers records")
-        win = out if out is not None else Allocs(L * fleet.n_servers)
-        cand = Allocs(L * fleet.n_servers * fleet.n_acc) if want_candidates else None
-        fc, wc = fleet.as_c(), win.as_c()
-        cc = cand.as_c() if cand is not None else None
-        self._resident(fleet)
-        self._check(self._L.wva_load_grid(self._h, C.byref(fc), L, _abi.ptr(rpm.reshape(-1)),
-                                          C.byref(cc) if cc is not None else None, C.byref(wc)))
-        return cand, win
+        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm})
+        if L is None:
+            raise ValueError("arrival_rpm is required")
+        return self._level_call(self._L.wva_load_grid, fleet, L, [_abi.ptr(rows["arrival_rpm"].reshape(-1))],
+                                want_candidates, out)
 
     def slo_grid(self, fleet: Fleet, slo_itl, slo_ttft, slo_tps, want_candidates: bool = False,
                  out: Allocs | None = None):
@@ -192,25 +184,12 @@ class Engine:
         ``srv_slo_tps`` = row ``l``, and winner block ``l`` is ``solve``'s winners for it in unlimited mode; each
         distinct target of a server is searched once (see ``wva_slo_grid`` in include/wva_b200.h).  The fleet's own
         ``srv_slo_*`` are not read.  ``out``: an ``Allocs`` of ``L * S`` records to write the winners into."""
-        rows = []
-        for name, x in (("slo_itl", slo_itl), ("slo_ttft", slo_ttft), ("slo_tps", slo_tps)):
-            r = np.ascontiguousarray(x, np.float32)
-            if r.ndim != 2 or r.shape[1] != fleet.n_servers:
-                raise ValueError(f"{name} must have shape (L, {fleet.n_servers}), got {r.shape}")
-            rows.append(r)
-        L = rows[0].shape[0]
-        if any(r.shape[0] != L for r in rows):
-            raise ValueError(f"slo_itl, slo_ttft and slo_tps must have one row count, got {[r.shape for r in rows]}")
-        if out is not None and out.n != L * fleet.n_servers:
-            raise ValueError("out must hold L * fleet.n_servers records")
-        win = out if out is not None else Allocs(L * fleet.n_servers)
-        cand = Allocs(L * fleet.n_servers * fleet.n_acc) if want_candidates else None
-        fc, wc = fleet.as_c(), win.as_c()
-        cc = cand.as_c() if cand is not None else None
-        self._resident(fleet)
-        self._check(self._L.wva_slo_grid(self._h, C.byref(fc), L, *[_abi.ptr(r.reshape(-1)) for r in rows],
-                                         C.byref(cc) if cc is not None else None, C.byref(wc)))
-        return cand, win
+        names = ("slo_itl", "slo_ttft", "slo_tps")
+        rows, L = _row_lists(fleet, dict(zip(names, (slo_itl, slo_ttft, slo_tps))))
+        if len(rows) != len(names):
+            raise ValueError("slo_itl, slo_ttft and slo_tps are required")
+        return self._level_call(self._L.wva_slo_grid, fleet, L, [_abi.ptr(rows[k].reshape(-1)) for k in names],
+                                want_candidates, out)
 
     def workload_grid(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None,
                       want_candidates: bool = False, out: Allocs | None = None):
@@ -249,23 +228,22 @@ class Engine:
         for name, own in (("in_tokens", fleet.srv_in_tokens), ("out_tokens", fleet.srv_out_tokens)):
             if name not in rows:
                 rows[name] = np.ascontiguousarray(np.broadcast_to(own, (L, S)), np.int32)
-        win, cand = self._row_outputs(fleet, L, want_candidates, out)
-        fc, wc = fleet.as_c(), win.as_c()
-        cc = cand.as_c() if cand is not None else None
-        self._resident(fleet)
-        self._check(call(self._h, C.byref(fc), L,
-                         *[_abi.ptr(rows[k].reshape(-1)) for k in ("arrival_rpm", "in_tokens", "out_tokens")],
-                         C.byref(cc) if cc is not None else None, C.byref(wc)))
-        return cand, win
+        return self._level_call(call, fleet, L,
+                                [_abi.ptr(rows[k].reshape(-1)) for k in ("arrival_rpm", "in_tokens", "out_tokens")],
+                                want_candidates, out)
 
-    @staticmethod
-    def _row_outputs(fleet, L, want_candidates, out):
-        """The winners (``out``, or new) and candidates (or None) of an L-row call."""
+    def _level_call(self, call, fleet, L, row_ptrs, want_candidates, out):
+        """call(handle, fleet, L, *row_ptrs, candidates, winners) for an L-row call -> (candidates [L*S*A] | None,
+        winners [L*S]); the winners go into ``out`` when given."""
         if out is not None and out.n != L * fleet.n_servers:
             raise ValueError("out must hold L * fleet.n_servers records")
         win = out if out is not None else Allocs(L * fleet.n_servers)
         cand = Allocs(L * fleet.n_servers * fleet.n_acc) if want_candidates else None
-        return win, cand
+        fc, wc = fleet.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(call(self._h, C.byref(fc), L, *row_ptrs, C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return cand, win
 
     def profile_grid(self, fleet: Fleet, *, acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None,
                      perf_gamma=None, perf_delta=None, perf_acc_count=None, perf_max_batch=None, perf_at_tokens=None,
@@ -286,14 +264,8 @@ class Engine:
                                      "perf_at_tokens": perf_at_tokens})
         if L is None:
             raise ValueError("profile_grid needs at least one row list")
-        win, cand = self._row_outputs(fleet, L, want_candidates, out)
         rc_ = _profile_rows_c(rows)
-        fc, wc = fleet.as_c(), win.as_c()
-        cc = cand.as_c() if cand is not None else None
-        self._resident(fleet)
-        self._check(self._L.wva_profile_grid(self._h, C.byref(fc), L, C.byref(rc_),
-                                             C.byref(cc) if cc is not None else None, C.byref(wc)))
-        return cand, win
+        return self._level_call(self._L.wva_profile_grid, fleet, L, [C.byref(rc_)], want_candidates, out)
 
     def profile_trace(self, fleet: Fleet, arrival_rpm=None, in_tokens=None, out_tokens=None, *, acc_cost=None,
                       perf_present=None, perf_alpha=None, perf_beta=None, perf_gamma=None, perf_delta=None,
@@ -316,15 +288,9 @@ class Engine:
                                      "perf_max_batch": perf_max_batch, "perf_at_tokens": perf_at_tokens})
         if L is None:
             raise ValueError("profile_trace needs at least one row list")
-        win, cand = self._row_outputs(fleet, L, want_candidates, out)
         rc_ = _profile_rows_c(rows)
-        fc, wc = fleet.as_c(), win.as_c()
-        cc = cand.as_c() if cand is not None else None
-        self._resident(fleet)
-        self._check(self._L.wva_profile_trace(self._h, C.byref(fc), L,
-                                              *[_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in load],
-                                              C.byref(rc_), C.byref(cc) if cc is not None else None, C.byref(wc)))
-        return cand, win
+        row_ptrs = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in load] + [C.byref(rc_)]
+        return self._level_call(self._L.wva_profile_trace, fleet, L, row_ptrs, want_candidates, out)
 
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
         """Where each server's ``load_grid`` winner changes its decision in ``[rpm_lo[s], rpm_hi[s]]`` (req/min)
