@@ -649,7 +649,8 @@ int wva_synchronize(wva_handle *h);
 /* Number of kernel launches issued by this handle since creation. */
 int64_t wva_launch_count(const wva_handle *h);
 /* Device time (ms, CUDA events on the handle's stream) of the dominant kernel in
- * the most recent call, and of the whole call's device work. */
+ * the most recent call with host results, and of the whole call's device work
+ * (the *_device calls do not time themselves). */
 float wva_last_kernel_ms(const wva_handle *h);
 float wva_last_device_ms(const wva_handle *h);
 

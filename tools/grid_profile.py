@@ -2,7 +2,9 @@
 
 torch.profiler with CUDA activities records every kernel and memset of K steps after a warm-up; each step is the
 L2 flush that bench.py runs followed by one wva_grid_solve_device.  Prints, per launch, the median device time
-over the steps, then the median step span (first launch start to last launch end) and the idle time inside it.
+over the steps and the median time it adds to the step (its end minus the previous launch's end: with programmatic
+dependent launch a kernel starts while its predecessor drains, and its device time includes that wait), then the
+median step span (first launch start to last launch end) and the idle time inside it (no launch running).
 With --cells, also the median wall time of engine.grid_solve(..., want_cells=True) (cell table copied back).
 With --nan, every server gets an infinite current cost on accelerator 0, which makes the value of its other
 accelerators NaN and turns pruning off: every non-shared cell of a loaded row is a candidate (the worst case of
@@ -94,23 +96,35 @@ def main():
         elif cur is not None:
             cur.append((n, float(e["ts"]), float(e["dur"])))
     per_step = [s for s in per_step if s]
-    by_name = {}
+    by_name, adds = {}, {}
     for s in per_step:
-        seen = {}
-        for n, _, d in s:
+        seen, added, prev_end = {}, {}, s[0][1]
+        for n, t, d in s:
             seen[n] = seen.get(n, 0.0) + d
+            added[n] = added.get(n, 0.0) + max(t + d - prev_end, 0.0)
+            prev_end = max(prev_end, t + d)
         for n, d in seen.items():
             by_name.setdefault(n, []).append(d)
-    spans = [s[-1][1] + s[-1][2] - s[0][1] for s in per_step]
-    busy = [sum(d for _, _, d in s) for s in per_step]
+            adds.setdefault(n, []).append(added[n])
+    spans = [max(t + d for _, t, d in s) - s[0][1] for s in per_step]
+
+    def busy_of(s):  # length of the union of the launches' intervals
+        tot, end = 0.0, s[0][1]
+        for _, t, d in sorted(s, key=lambda x: x[1]):
+            if t + d > end:
+                tot += t + d - max(t, end)
+                end = t + d
+        return tot
+    busy = [busy_of(s) for s in per_step]
     print(f"device: {card()}")
     print(f"{len(per_step)} profiled steps, {launches} library launches per {args.steps} steps")
     plan = (C.c_uint32 * 31)()
     eng._L.wva_dbg_read_plan(eng._h, plan)  # item_count[2 * 256 + 1 ..]: [15] candidates, [16] chunks (grid_order)
     print(f"grid_order: {plan[15]} candidates in {plan[16]} chunks")
     order = [n for n, _, _ in per_step[0]]
+    print(f"  {'launch':<22s} {'device':>8s} {'adds':>8s}")
     for n in dict.fromkeys(order):
-        print(f"  {n:<22s} {statistics.median(by_name[n]):8.1f} us")
+        print(f"  {n:<22s} {statistics.median(by_name[n]):8.1f} {statistics.median(adds[n]):8.1f} us")
     print(f"  {'step span':<22s} {statistics.median(spans):8.1f} us")
     print(f"  {'idle inside span':<22s} {statistics.median([a - b for a, b in zip(spans, busy)]):8.1f} us")
     if args.cells:

@@ -401,11 +401,33 @@ int prepare_fallback(wva_handle* h, int list, int cap, int Nmax, FbRun& r) {
     return WVA_OK;
 }
 
-// Enqueues a re-run kernel (grid_fallback, size_fallback, ...) over r's list.
+// Enqueues kernel<<<grid, block, smem>>>(args...) with programmatic dependent launch: the kernel may start while the
+// kernel before it in the stream runs, and reads nothing that kernel writes before its pdl_wait().
+template <class... Params, class... Args>
+int launch_pdl(wva_handle* h, void (*kernel)(Params...), unsigned grid, unsigned block, size_t smem, Args&&... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = h->stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    CK(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
+    h->launches++;
+    return WVA_OK;
+}
+
+// Enqueues a re-run kernel (grid_fallback, size_fallback, ...) over r's list; with pdl, by launch_pdl (the kernel
+// calls pdl_wait() first).
 template <class Args>
-void launch_fallback(wva_handle* h, void (*kernel)(Args, FbRun), const Args& g, const FbRun& r) {
+int launch_fallback(wva_handle* h, void (*kernel)(Args, FbRun), const Args& g, const FbRun& r, bool pdl = false) {
+    if (pdl) return launch_pdl(h, kernel, kFbBlocks, kFbThreads, 0, g, r);
     kernel<<<kFbBlocks, kFbThreads, 0, h->stream>>>(g, r);
     h->launches++;
+    return WVA_OK;
 }
 
 // Enqueues kernel(args...) with one thread per record of an n_rec-record block (trivial_kernel, profile_kernel, ...).
@@ -509,12 +531,13 @@ int upload_tables(wva_handle* h, PairTables& pt, const std::vector<int>& pair, c
 }
 
 // build_pair_tables over the uploaded lists of fleet f's pairs; the grid passes its batch list and gets the
-// per-(table, batch) constants in pb
+// per-(table, batch) constants in pb, and its n_zero step counters are zeroed (by one CTA when there is no table)
 int build_tables(wva_handle* h, const DevFleet& f, const PairTables& pt, const int* batch = nullptr, int B = 0,
-                 float4* pb = nullptr) {
-    if (pt.n == 0) return WVA_OK;
-    build_pair_tables<<<pt.n, 128, 0, h->stream>>>(f, pt.pair(), pt.off(), pt.len(), pt.n, (double*)pt.tab.p,
-                                                   pt.with_ls ? (float*)pt.ls.p : nullptr, batch, B, pb);
+                 float4* pb = nullptr, unsigned* zero = nullptr, int n_zero = 0) {
+    if (pt.n == 0 && n_zero == 0) return WVA_OK;
+    build_pair_tables<<<std::max(pt.n, 1), 128, 0, h->stream>>>(f, pt.pair(), pt.off(), pt.len(), pt.n,
+                                                                (double*)pt.tab.p, pt.with_ls ? (float*)pt.ls.p : nullptr,
+                                                                batch, B, pb, zero, n_zero);
     h->launches++;
     CK(cudaGetLastError());
     return WVA_OK;
@@ -1928,7 +1951,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     if (!hf.queue_fits(Nmax))
         return h->fail(WVA_ERR_UNSUPPORTED,
                        "queue model of 2^31 states or more (batch size x (1 + max_queue_to_batch_ratio))");
-    // [tables x batch] constants, then the [server x replica] rate block grid_rows fills (always allocated)
+    // [tables x batch] constants, then the [server x replica] rate block grid_order fills (always allocated)
     CK(h->d_pb.ensure(sizeof(float4) * ((size_t)pt.n * std::max(B, 1) + (size_t)S * std::max(R, 1) + 1)));
     const char* d = (const char*)pt.lists.p;
     GridArgs& g = plan->args;
@@ -1938,8 +1961,6 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     g.batch_rank = g.batch + B;
     g.rank_to_bi = g.batch + 2 * B;
     g.replicas = g.batch + 3 * B;
-    int rc = build_tables(h, h->df, pt, g.batch, B, (float4*)h->d_pb.p);
-    if (rc) return rc;
     g.B = B;
     g.R = R;
     g.tab = (const double*)pt.tab.p;
@@ -1992,7 +2013,7 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
     // size in 24; outside those limits every cell is evaluated (grid_order still walks the shared runs)
     g.prune = A <= 256 && Bmax < (1 << 24) && (long long)A * R <= kOrderMaxRows;
     g.Bmax = Bmax;
-    rc = prepare_fallback(h, 0, (int)std::min<size_t>(nc, (size_t)1 << 22), Nmax, plan->fb);
+    int rc = prepare_fallback(h, 0, (int)std::min<size_t>(nc, (size_t)1 << 22), Nmax, plan->fb);
     if (rc) return rc;
     g.fb_count = plan->fb.list.count;
     g.fb_cells = plan->fb.list.item;
@@ -2015,37 +2036,42 @@ int prepare_grid(wva_handle* h, const wva_grid* grid, GridPlan* plan) {
         h->dbg_n = nc;
     }
     plan->Bmax = Bmax;
-    return WVA_OK;
+    // the step's first kernel, enqueued after every buffer it or the step uses is in place (a DevBuf that grows frees
+    // its old memory)
+    return build_tables(h, h->df, pt, g.batch, B, (float4*)h->d_pb.p, g.item_count, kItemCountWords);
 }
 
-int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
+// timed: record ev_k0 / ev_k1 around grid_kernel for wva_last_kernel_ms, and launch grid_kernel ordinarily.  A record
+// of a timing event between two kernels makes the second wait for the first to finish (no programmatic overlap), so
+// only calls that read the timing (those with host results) record them.
+int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners, bool timed) {
     GridArgs& g = plan.args;
     const HostFleet& hf = h->hf;
-    if (plan.n_cells == 0) CK(cudaEventRecord(h->ev_k0, h->stream));
+    int rc = WVA_OK;
+    if (timed && plan.n_cells == 0) CK(cudaEventRecord(h->ev_k0, h->stream));
     if (plan.n_cells > 0) {
-        CK(cudaMemsetAsync(g.item_count, 0, sizeof(unsigned) * (2 * kClasses + 32), h->stream));
-        {
-            const int rows_threads = g.R >= 128 ? 128 : (g.R > 32 ? 64 : 32);
-            const size_t rows_smem = g.Bmax <= kRowsSmemEntries ? (size_t)g.Bmax * 32 : 0;
-            grid_rows<<<(unsigned)(hf.S * hf.A), rows_threads, rows_smem, h->stream>>>(g);
-        }
-        h->launches++;
         if (g.want_cells) g.prune = 0;  // every cell is evaluated and stored
-        // without a cell table the shared-chain cells and each server's bound; the cells left for grid_kernel, then
-        // their sort
-        grid_order<<<(unsigned)hf.S, kOrderThreads, 0, h->stream>>>(g);
-        h->launches++;
-        grid_sort_cands<<<(unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads, 0, h->stream>>>(g);
-        grid_items_scatter<<<(unsigned)(16 * h->sm_count), 256, 0, h->stream>>>(g);  // warp per item (grid-stride)
-        h->launches++;
-        CK(cudaEventRecord(h->ev_k0, h->stream));  // wva_last_kernel_ms = the dominant kernel alone
+        // the rows; without a cell table the shared-chain cells and each server's bound; the cells left for
+        // grid_kernel, then their sort
+        const size_t order_smem = (long long)hf.A * g.Bmax <= kOrderTabEntries ? (size_t)hf.A * g.Bmax * 32 : 0;
+        rc = launch_pdl(h, grid_order, (unsigned)hf.S, kOrderThreads, order_smem, g);
+        if (!rc) rc = launch_pdl(h, grid_sort_cands, (unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads, 0, g);
+        if (!rc) rc = launch_pdl(h, grid_items_scatter, (unsigned)(16 * h->sm_count), 256, 0, g);  // warp per item
+        if (rc) return rc;
         const size_t smem = (size_t)kGkWarps * kGkWarpD * sizeof(double);
-        grid_kernel<<<(unsigned)h->sm_count, kGkThreads, smem, h->stream>>>(g);
-        h->launches += 2;
+        if (timed) {  // wva_last_kernel_ms = the dominant kernel alone; after the record there is no overlap to gain
+            CK(cudaEventRecord(h->ev_k0, h->stream));
+            grid_kernel<<<(unsigned)h->sm_count, kGkThreads, smem, h->stream>>>(g);
+            h->launches++;
+        } else {
+            rc = launch_pdl(h, grid_kernel, (unsigned)h->sm_count, kGkThreads, smem, g);
+            if (rc) return rc;
+        }
     }
-    CK(cudaEventRecord(h->ev_k1, h->stream));
+    if (timed) CK(cudaEventRecord(h->ev_k1, h->stream));
     if (plan.n_cells > 0) {
-        launch_fallback(h, grid_fallback, g, plan.fb);
+        rc = launch_fallback(h, grid_fallback, g, plan.fb, true);
+        if (rc) return rc;
         if (g.want_cells) {  // the shared-chain cells with a cell table: one warp per 32 rows and slice of ranks
             const size_t n_warps = ((size_t)hf.S * hf.A * g.R + 31) / 32 * ((size_t)(g.B + kSharedSlice - 1) / kSharedSlice);
             const unsigned ctas = (unsigned)((n_warps + kSharedThreads / 32 - 1) / (kSharedThreads / 32));
@@ -2054,8 +2080,8 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners) {
         }
     }
     if (hf.S > 0) {
-        grid_finalize<<<hf.S, 256, 0, h->stream>>>(g, winners);
-        h->launches++;
+        rc = launch_pdl(h, grid_finalize, (unsigned)hf.S, 256, 0, g, winners);
+        if (rc) return rc;
     }
     CK(cudaGetLastError());
     return WVA_OK;
@@ -2351,6 +2377,7 @@ int wva_create(wva_handle** out, int device) {
     h->device = device;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) h->sm_count = prop.multiProcessorCount;
+    cudaFuncSetAttribute(grid_order, cudaFuncAttributeMaxDynamicSharedMemorySize, kOrderTabEntries * 32);
     cudaFuncSetAttribute(grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)((size_t)kGkWarps * kGkWarpD * sizeof(double)));
     if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
@@ -2623,11 +2650,8 @@ int wva_grid_solve_device(wva_handle* h, const wva_grid* grid, wva_allocs* winne
     if (rc) return rc;
     rc = ensure_cells(h, plan, nullptr);
     if (rc) return rc;
-    CK(cudaEventRecord(h->ev_d0, h->stream));
-    rc = enqueue_grid(h, plan, cols_from_abi(winners_dev));
-    if (rc) return rc;
-    CK(cudaEventRecord(h->ev_d1, h->stream));
-    return WVA_OK;
+    // untimed: nothing reads the timing events after a call without host results
+    return enqueue_grid(h, plan, cols_from_abi(winners_dev), false);
 }
 
 int wva_grid_solve(wva_handle* h, const wva_fleet* fleet, const wva_grid* grid, wva_cells* cells, wva_allocs* winners) {
@@ -2647,7 +2671,7 @@ int wva_grid_solve(wva_handle* h, const wva_fleet* fleet, const wva_grid* grid, 
     if (plan.args.want_cells && plan.n_cells)  // cells that are never analysed must read back as 0
         CK(cudaMemsetAsync(h->d_cells.p, 0, plan.cells.bytes, h->stream));
     HostCall c{0, false, true, &plan.cells, h->d_cells.p};
-    rc = run_host(h, c, [&](const AllocCols&, const AllocCols& dw) { return enqueue_grid(h, plan, dw); });
+    rc = run_host(h, c, [&](const AllocCols&, const AllocCols& dw) { return enqueue_grid(h, plan, dw, true); });
     if (rc) return rc;
     scatter_block(c.win_host, c.bw, winners);
     h->last_kind = 1;

@@ -772,7 +772,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 // needs IEEE division, a chain that reaches the table end, window violations) just reports
 // "no sharing" and the cells go through grid_kernel as usual.
 // ---------------------------------------------------------------------------
-// Inlined into its two call sites so that the shared-memory call compiles to LDS (grid_rows stages the
+// Inlined into its two call sites so that the shared-memory call compiles to LDS (grid_order stages the
 // pair's table).  Both passes run 4 steps per window test where the exponent bounds allow it
 // (solve_shared_t's argument); lanes are independent rows, so there is no warp vote here.
 __device__ __forceinline__ bool solve_row(const double* __restrict__ tab, int len, float lambda, double& acc_out,

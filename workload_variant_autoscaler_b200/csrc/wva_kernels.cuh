@@ -216,6 +216,14 @@ __device__ __forceinline__ Cand zero_load_alloc(const DevFleet& f, int s, int a)
     return zero_load_alloc(f, s, a, f.srv_max_batch[s] > 0 ? f.srv_max_batch[s] : f.perf_max_batch[k]);
 }
 
+// Programmatic dependent launch (sm_90): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization
+// may start while the kernel before it in the stream still runs.  pdl_wait() blocks until that kernel has finished
+// and its memory is visible, so nothing it writes may be read before; without the attribute it returns at once.
+// pdl_launch_dependents() lets the next such kernel start.  Called only after pdl_wait(), it never lets work of one
+// step overlap the kernels of the step before.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // ---------------------------------------------------------------------------
 // Shared head tables: entry n (0-based) of table t = {servRate[n], yh, yl} as doubles + {min(servRate[n..]),
 // max(servRate[0..n])} as floats (32 B, two 16 B loads per head step), plus a float column
@@ -224,15 +232,21 @@ __device__ __forceinline__ Cand zero_load_alloc(const DevFleet& f, int s, int a)
 // Per (table, batch index) constants shared by the 64 replica levels of a pair:
 // x = RateRange.Max (req/s) for N = batch, y = log2 servRate[N-1], z = ls[N-1], w = log2 servRate[0].
 // Per (server, replica index): x = rate (req/s), y = lambda (req/ms), z = log2 lambda.
+// The grid step's first kernel: it lets the next one (grid_order) start at once, and CTA 0 zeroes the step's n_zero
+// counters, which grid_order reads only after its pdl_wait().  Launched with at least one CTA when there is a reset.
 __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* __restrict__ tab_pair,
                                                          const long long* __restrict__ tab_off,
                                                          const int* __restrict__ tab_len, int n_tab,
                                                          double* __restrict__ tab, float* __restrict__ ls,
                                                          const int* __restrict__ batch, int B,
-                                                         float4* __restrict__ pb) {
+                                                         float4* __restrict__ pb, unsigned* __restrict__ zero,
+                                                         int n_zero) {
     __shared__ double wsum[4];
     __shared__ double carry_s;
+    pdl_launch_dependents();
     const int t = blockIdx.x;
+    if (t == 0)
+        for (int i = threadIdx.x; i < n_zero; i += blockDim.x) zero[i] = 0;
     if (t >= n_tab) return;
     const int pair = tab_pair[t];
     const int s = pair / f.A, a = pair % f.A;
@@ -334,12 +348,12 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 // ---------------------------------------------------------------------------
 // K2: candidate grid.
 //
-//   grid_rows        per (pair, replica level): the chain every large-enough batch size shares
-//                    (solve_row); also the (server, replica) rate block and the batch-rank reset
-//   grid_order       per server: without a cell table, the rows' order under grid_finalize's key, the cells
-//                    that share their row's chain up to the row's first feasible one and the server's bound
-//                    (the smallest key of a feasible cell found); then the cells left for grid_kernel as two
-//                    rank intervals per row, listed in chunks of at most 4096 of one pair
+//   grid_order       per server: the (server, replica) rate block, the batch-rank reset and, per (pair, replica
+//                    level), the chain every large-enough batch size shares (solve_row); without a cell table, the
+//                    rows' order under grid_finalize's key, the cells that share their row's chain up to the row's
+//                    first feasible one and the server's bound (the smallest key of a feasible cell found); then
+//                    the cells left for grid_kernel as two rank intervals per row, listed in chunks of at most 4096
+//                    of one pair
 //   grid_sort_cands  per chunk (fixed grid, a chunk per CTA at a time): the per-cell gates, a log-domain length
 //                    estimate, an 8-bit class and a local counting sort -> warp items; the last CTA plans
 //                    grid_kernel's queues (grid_items_plan)
@@ -352,6 +366,10 @@ __global__ void __launch_bounds__(128) build_pair_tables(DevFleet f, const int* 
 //   grid_fallback   stored-vector re-run of the rare cells the streaming solve bails on
 //   grid_shared     with a cell table, per (pair, replica level): every cell that shares the row's chain
 //   grid_finalize   per-server argmin (warp shuffle -> shared memory -> winner record)
+//
+// build_pair_tables opens the step with an ordinary launch; every kernel above except grid_shared (and grid_kernel
+// when the call times it) follows with programmatic dependent launch (pdl_wait above): it starts while its
+// predecessor drains and waits for it before reading what the step has written.
 //
 // For a fixed (server, accelerator, replica level) the transition penalty and the cost do
 // not depend on the batch size, so the winner among batch sizes is the smallest feasible
@@ -598,93 +616,23 @@ __device__ __forceinline__ Metrics shared_cell_metrics_inv(const PairConst& pc, 
     return m;
 }
 
-// One CTA per (server, accelerator) pair, one lane per replica level: the chain every large-enough
-// batch size shares.  The pair's table is staged in shared memory first (coalesced), so the serial
-// chains read it at shared-memory latency instead of waiting for L2 on every step.
-constexpr int kRowsSmemEntries = 1536;  // 48 KB of 32-byte entries; longer tables are read from global
-__global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
-    extern __shared__ double rows_tab[];
-    const DevFleet& f = g.f;
-    const int sa = blockIdx.x;
-    const int s = sa / f.A;
-    const long long toff = g.pair_tab_off[sa];
-    const double* tab = toff >= 0 ? g.tab + 4 * toff : nullptr;
-    const bool staged = toff >= 0 && g.Bmax <= kRowsSmemEntries;
-    if (staged) {
-        // all of a thread's loads first, then its stores: one L2 round trip instead of one per iteration
-        const double2* src = (const double2*)tab;
-        double2* dst = (double2*)rows_tab;
-        const int n16 = 2 * g.Bmax;
-        for (int i0 = threadIdx.x; i0 < n16; i0 += 8 * blockDim.x) {
-            double2 v[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                const int i = i0 + u * blockDim.x;
-                if (i < n16) v[u] = src[i];
-            }
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                const int i = i0 + u * blockDim.x;
-                if (i < n16) dst[i] = v[u];
-            }
-        }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {  // the pair's constants as one record (grid_kernel reads it once per item)
-        const int a = sa - s * f.A;
-        const int m = f.srv_model[s];
-        float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (m >= 0 && m < f.M) {
-            const int k = m * f.A + a;
-            r0 = make_float4(f.perf_alpha[k], f.perf_beta[k], f.perf_gamma[k], f.perf_delta[k]);
-        }
-        g.pair_rec[3 * sa + 0] = r0;
-        g.pair_rec[3 * sa + 1] = make_float4(__int_as_float(f.srv_in_tokens[s]), __int_as_float(f.srv_out_tokens[s]),
-                                             f.srv_slo_ttft[s], f.srv_slo_itl[s]);
-        g.pair_rec[3 * sa + 2] = make_float4(__int_as_float(f.srv_min_replicas[s]),
-                                             __int_as_float(f.srv_slo_tps[s] > 0.0f ? 1 : 0), 0.f, 0.f);
-    }
-    float l2s0 = 0.f, ls_end = 0.f;
-    if (toff >= 0) {
-        l2s0 = log2f((float)tab[0]);
-        ls_end = (g.ls + toff + g.pair_tab_idx[sa])[g.Bmax - 1];
-    }
-    for (int ri = threadIdx.x; ri < g.R; ri += blockDim.x) {
-        const size_t row = (size_t)sa * g.R + ri;
-        int j = INT_MAX;
-        double acc = 0.0, sump = 0.0;
-        // per-replica rate, lambda and log2(lambda) of the server (rate = total / replicas, lambda = rate / 1000): every pair CTA
-        // derives its own copy, the CTA of accelerator 0 publishes it for the later kernels; the
-        // (pair, replica) slot of the batch-rank minimum is reset here too
-        const float rate = __fdiv_rn(total_rate_of(f, s), (float)g.replicas[ri]);
-        const float lambda = __fdiv_rn(rate, 1000.0f);
-        const float4 rt = make_float4(rate, lambda, log2f(lambda), 0.0f);
-        if (sa == s * f.A) g.rt[s * g.R + ri] = rt;
-        g.best_rank[row] = INT_MAX;
-        if (toff >= 0 && rt.x > 0.0f) {
-            // skip rows whose chain is (by the log-domain estimate) still far from negligible at the end of
-            // the table: they cannot be shared and would only burn Bmax steps to find that out
-            const float thr = -78.0f + fminf(0.0f, rt.z - l2s0);
-            const float Lend = (float)(g.Bmax - 1) * rt.z - ls_end;
-            int jl = 0;
-            if (Lend < thr + 8.0f) {
-                const bool ok = staged ? solve_row(rows_tab, g.Bmax, rt.y, acc, sump, jl) : solve_row(tab, g.Bmax, rt.y, acc, sump, jl);
-                if (ok) j = jl;
-            }
-        }
-        g.row_j[row] = j;
-        g.row_acc[row] = acc;
-        g.row_sump[row] = sump;
-    }
-}
-
-// Between grid_rows and grid_sort_cands: one CTA per server.  With a cell table (pruning off) only step 3 runs:
-// grid_shared evaluates every shared cell after grid_kernel, which the walk of step 2 would only repeat.
-//  1. Group ranks (g.prune): every (accelerator, replica level) row gets the number of rows of the server strictly
-//     below it in (value, cost, replicas), with value and cost computed as grid_finalize computes them.  A counting
-//     rank, Q threads per row.  It keeps key_better's order, ties included (-0 == +0); rows without a table take part
-//     with a fixed key, which does not change the order of the others.  A NaN value or cost would make the order
-//     depend on the reduction, so it turns pruning off for the server (bound = kBoundOff).
+// After build_pair_tables, before grid_sort_cands: one CTA per server.  With a cell table (pruning off) the rows are
+// solved and then only step 3 runs: grid_shared evaluates every shared cell after grid_kernel, which the walk of step 2
+// would only repeat.
+//  0. Before the tables exist (ahead of griddepcontrol.wait, while build_pair_tables may still run): the pair records,
+//     the (server, replica) rate block, the batch-rank reset and the ranking's values and costs.  These read the
+//     uploaded fleet and grid only.
+//  1. The rows (solve_row): per (accelerator, replica level) the chain every large-enough batch size shares.  The
+//     server's tables are staged in shared memory when A * Bmax <= kOrderTabEntries, so the serial chains read them at
+//     shared-memory latency; longer ones are read from global memory.  A row whose chain is (by the log-domain
+//     estimate) still far from negligible at the end of the table is skipped: it cannot be shared.  Warps take 32
+//     rows at a time from a shared counter.
+//     Group ranks (g.prune), at the same time on the other warps, which take rows once the ranking is done: every row
+//     gets the number of rows of the server strictly below it in (value, cost, replicas), with value and cost
+//     computed as grid_finalize computes them.  A counting rank, Q threads per row.  It keeps key_better's order, ties
+//     included (-0 == +0); rows without a table take part with a fixed key, which does not change the order of the
+//     others.  A NaN value or cost would make the order depend on the reduction, so it turns pruning off for the
+//     server (bound = kBoundOff).
 //  2. The shared runs (b >= jl + 2, K < 2^23): each row is walked from its first shared rank up to its first feasible
 //     cell, which lowers best_rank; the smallest key among those cells is the server's bound.  Rows are taken in group
 //     order, kOrderG lanes per row, and a row's walk also stops at the first cell whose key is above the bound so far
@@ -700,7 +648,7 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
 //     a cell table, do pairs with alpha > slo_itl (ITL = alpha + beta * eff >= alpha, eff >= 0, beta >= 0); with a
 //     cell table grid_kernel stores their cells as analysed and not feasible.  A warp per pair scans its rows' counts
 //     into their first candidates, then reserves the pair's chunks of kCandChunk candidates in the chunk list and
-//     their places in order[] with one atomic.
+//     their places in order[] with one atomic (build_pair_tables zeroed the counters).
 //
 // Without a cell table no pass over the shared cells is needed after grid_kernel.  Every cell that is never
 // evaluated — a shared cell after the stop of its row's walk, or a non-shared cell that is not a candidate or that
@@ -710,10 +658,14 @@ __global__ void __launch_bounds__(128) grid_rows(GridArgs g) {
 // row is W's rank.  Any other best_rank is a feasible cell, whose key is >= W's.  grid_finalize picks W exactly as
 // when every cell is evaluated.
 constexpr int kOrderThreads = 1024, kOrderG = 4, kOrderMaxRows = 2048;
+constexpr int kOrderTabEntries = 4096;         // 128 KB of 32-byte table entries per server; more are read from global
+constexpr int kOrderRowWarps = 8;              // with g.prune, warps that start on the rows while the others rank
 constexpr int kCandChunk = 4096;               // candidates per chunk of grid_sort_cands (never two pairs)
 constexpr int kCandThreads = 256, kCandCtasPerSm = 4;
 constexpr int kCandResv = 2 * kClasses + 16;   // item_count[kCandResv], [kCandResv + 1]: candidates, chunks reserved
+constexpr int kItemCountWords = 2 * kClasses + 32;  // item_count[]: the step's counters, zeroed by build_pair_tables
 __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
+    extern __shared__ __align__(16) double order_tab[];  // [A][Bmax] table entries when staged
     __shared__ float s_vc[2 * kOrderMaxRows];  // ranking: values | costs; walk: RateRange.Max per (accelerator, rank)
     __shared__ int s_rep[kOrderMaxRows];        // ranking: replicas; walk: batch size per rank
     float* s_val = s_vc;
@@ -721,14 +673,39 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
     __shared__ unsigned s_grp[kOrderMaxRows];
     __shared__ unsigned short s_at[kOrderMaxRows];  // the row at each position of the group order
     __shared__ unsigned long long s_bound;
+    __shared__ int s_next_row;
     const DevFleet& f = g.f;
     const int s = blockIdx.x, A = f.A, R = g.R, B = g.B, n = A * R;
     const size_t row0 = (size_t)s * n;
     const unsigned tid = threadIdx.x, lane = tid & 31;
-    if (tid == 0) s_bound = kBoundNone;
+    if (tid == 0) {
+        s_bound = kBoundNone;
+        s_next_row = 0;
+    }
+    const float total = total_rate_of(f, s);
+    for (int a = (int)tid; a < A; a += blockDim.x) {  // the pair's constants as one record (grid_kernel reads it once per item)
+        const int sa = s * A + a, m = f.srv_model[s];
+        float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (m >= 0 && m < f.M) {
+            const int k = m * A + a;
+            r0 = make_float4(f.perf_alpha[k], f.perf_beta[k], f.perf_gamma[k], f.perf_delta[k]);
+        }
+        g.pair_rec[3 * sa + 0] = r0;
+        g.pair_rec[3 * sa + 1] = make_float4(__int_as_float(f.srv_in_tokens[s]), __int_as_float(f.srv_out_tokens[s]),
+                                             f.srv_slo_ttft[s], f.srv_slo_itl[s]);
+        g.pair_rec[3 * sa + 2] = make_float4(__int_as_float(f.srv_min_replicas[s]),
+                                             __int_as_float(f.srv_slo_tps[s] > 0.0f ? 1 : 0), 0.f, 0.f);
+    }
+    // per-replica rate, lambda and log2(lambda) of the server (rate = total / replicas, lambda = rate / 1000)
+    for (int ri = (int)tid; ri < R; ri += blockDim.x) {
+        const float rate = __fdiv_rn(total, (float)g.replicas[ri]);
+        const float lambda = __fdiv_rn(rate, 1000.0f);
+        g.rt[s * R + ri] = make_float4(rate, lambda, log2f(lambda), 0.0f);
+    }
     int nan = 0;
-    if (g.prune) {
-        for (int k = tid; k < n; k += blockDim.x) {
+    for (int k = (int)tid; k < n; k += blockDim.x) {
+        g.best_rank[row0 + k] = INT_MAX;
+        if (g.prune) {
             const int a = k / R, ri = k - a * R;
             float v = INFINITY, c = INFINITY;
             int r = INT_MAX;
@@ -745,18 +722,44 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
             s_rep[k] = r;
         }
     }
-    const bool prune = g.prune && !__syncthreads_or(nan);
-    if (prune) {
+    // the tables, pb, and the counters are written by the kernels before this one
+    pdl_wait();
+    pdl_launch_dependents();
+    const int Bmax = g.Bmax;
+    const bool staged = (long long)A * Bmax <= kOrderTabEntries;
+    if (staged) {
+        // all of a thread's loads first, then its stores: one L2 round trip instead of one per iteration
+        const int n16 = 2 * Bmax;  // 16-byte halves of the entries of one pair
+        for (int i0 = (int)tid; i0 < A * n16; i0 += 4 * (int)blockDim.x) {
+            double2 v[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int i = i0 + u * (int)blockDim.x, a = i / n16;
+                const long long toff = i < A * n16 ? g.pair_tab_off[s * A + a] : -1;
+                if (toff >= 0) v[u] = ((const double2*)(g.tab + 4 * toff))[i - a * n16];
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int i = i0 + u * (int)blockDim.x, a = i / n16;
+                if (i < A * n16 && g.pair_tab_off[s * A + a] >= 0) ((double2*)order_tab)[i] = v[u];
+            }
+        }
+    }
+    const bool any_nan = __syncthreads_or(nan);  // also: the staged tables and s_next_row are in place
+    const bool prune = g.prune && !any_nan;
+    const int rank_first = min((n + 31) / 32, kOrderRowWarps);  // with prune, the warps from here on rank first
+    if (prune && (int)(tid >> 5) >= rank_first) {
+        const int rtid = (int)tid - 32 * rank_first, threads = (int)blockDim.x - 32 * rank_first;
         int q = 1;  // threads per row: a power of two <= 32, so that they are lanes of one warp
-        while (q < 32 && 2 * q * n <= (int)blockDim.x) q *= 2;
-        const int per = (int)blockDim.x / q;
+        while (q < 32 && 2 * q * n <= threads) q *= 2;
+        const int per = threads / q;
         for (int base = 0; base < n; base += per) {
-            const int i = base + (int)tid / q;
+            const int i = base + rtid / q;
             unsigned lt = 0, eq = 0;  // rows strictly below row i; equal rows before it (its place among its ties)
             if (i < n) {
                 const float vi = s_val[i], ci = s_cost[i];
                 const int ri = s_rep[i];
-                for (int j = (int)tid % q; j < n; j += q) {
+                for (int j = rtid % q; j < n; j += q) {
                     const float vj = s_val[j], cj = s_cost[j];
                     const int rj = s_rep[j];
                     lt += vj < vi || (vj == vi && (cj < ci || (cj == ci && rj < ri)));
@@ -767,16 +770,45 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
                 lt += __shfl_xor_sync(0xffffffffu, lt, d);
                 eq += __shfl_xor_sync(0xffffffffu, eq, d);
             }
-            if (i < n && (int)tid % q == 0) {
+            if (i < n && rtid % q == 0) {
                 s_grp[i] = lt;
                 s_at[lt + eq] = (unsigned short)i;
                 g.row_grp[row0 + i] = lt;
             }
         }
-    } else if (g.prune) {
-        for (int k = tid; k < n; k += blockDim.x) g.row_grp[row0 + k] = 0;
+    } else if (g.prune && !prune) {
+        for (int k = (int)tid; k < n; k += blockDim.x) g.row_grp[row0 + k] = 0;
+    }
+    for (;;) {  // the rows, 32 per warp at a time
+        int k0 = 0;
+        if (lane == 0) k0 = atomicAdd(&s_next_row, 32);
+        k0 = __shfl_sync(0xffffffffu, k0, 0);
+        if (k0 >= n) break;
+        const int k = k0 + (int)lane, a = k / R, ri = k - a * R, sa = s * A + a;
+        const long long toff = k < n ? g.pair_tab_off[sa] : -1;
+        int j = INT_MAX;
+        double acc = 0.0, sump = 0.0;
+        if (toff >= 0) {
+            const float rate = __fdiv_rn(total, (float)g.replicas[ri]), lambda = __fdiv_rn(rate, 1000.0f);  // rt.x, rt.y
+            const double* tab = g.tab + 4 * toff;
+            const double* stab = order_tab + 4 * (size_t)a * Bmax;
+            const float l2lam = log2f(lambda), l2s0 = log2f((float)(staged ? stab[0] : tab[0]));
+            const float thr = -78.0f + fminf(0.0f, l2lam - l2s0);
+            const float Lend = (float)(Bmax - 1) * l2lam - (g.ls + toff + g.pair_tab_idx[sa])[Bmax - 1];
+            int jl = 0;
+            if (rate > 0.0f && Lend < thr + 8.0f) {
+                const bool ok = staged ? solve_row(stab, Bmax, lambda, acc, sump, jl) : solve_row(tab, Bmax, lambda, acc, sump, jl);
+                if (ok) j = jl;
+            }
+        }
+        if (k < n) {
+            g.row_j[row0 + k] = j;
+            g.row_acc[row0 + k] = acc;
+            g.row_sump[row0 + k] = sump;
+        }
     }
     __syncthreads();
+
     const bool stage_b = B <= kOrderMaxRows, stage_rmax = A * B <= 2 * kOrderMaxRows;
     if (stage_b)
         for (int r = tid; r < B; r += blockDim.x) s_rep[r] = g.batch[g.rank_to_bi[r]];
@@ -795,7 +827,7 @@ __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
         const int a = k / R, ri = k - a * R;
         const size_t row = row0 + k;
         const unsigned grp = prune ? s_grp[k] : 0u;
-        const int jl = p < n ? g.row_j[row] : INT_MAX;  // a shared chain implies a table and a positive rate (grid_rows)
+        const int jl = p < n ? g.row_j[row] : INT_MAX;  // a shared chain implies a table and a positive rate (step 1)
         int lo = 0;
         bool active = false;
         float4 rt;
@@ -1011,6 +1043,8 @@ __global__ void __launch_bounds__(kCandThreads) grid_sort_cands(GridArgs g) {
     __shared__ unsigned cursor[kClasses];
     const DevFleet& f = g.f;
     const int R = g.R, B = g.B;
+    pdl_wait();
+    pdl_launch_dependents();
     const unsigned n_chunks = g.item_count[kCandResv + 1];
     for (unsigned ci = blockIdx.x; ci < n_chunks; ci += gridDim.x) {
         const uint4 ch = g.chunks[ci];
@@ -1153,6 +1187,8 @@ __device__ __forceinline__ void grid_items_plan(const GridArgs& g) {
 // chunk) is padded with copies of its first cell, flagged, so that the whole warp takes part in the staged loads.
 __global__ void __launch_bounds__(256) grid_items_scatter(GridArgs g) {
     const DevFleet& f = g.f;
+    pdl_wait();
+    pdl_launch_dependents();
     const unsigned n = *g.item_count;
     const unsigned lane = threadIdx.x & 31;
     const unsigned warps = (gridDim.x * blockDim.x) >> 5;
@@ -1287,6 +1323,8 @@ __global__ void __launch_bounds__(kGkThreads, 1) grid_kernel(GridArgs g) {
     extern __shared__ __align__(16) double grid_smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     double* warp_smem = grid_smem + (size_t)warp * kGkWarpD;
+    pdl_wait();
+    pdl_launch_dependents();
     const unsigned n_items = g.item_count[0], n_long = g.item_count[kQLongN];
     const bool sub0 = (warp & 3) == 0;
     // the long items are spread over as few CTAs as possible (long_per_sm per CTA): the other CTAs keep all
@@ -1329,6 +1367,8 @@ __global__ void __launch_bounds__(kGkThreads, 1) grid_kernel(GridArgs g) {
 // Stored-vector re-run of the cells grid_kernel bailed on (r.list holds cell ids).
 __global__ void grid_fallback(GridArgs g, FbRun r) {
     const DevFleet& f = g.f;
+    pdl_wait();
+    pdl_launch_dependents();
     fb_rerun(r, [&](unsigned long long cell, double* p) {
         int s, a, bi, ri;
         decode_cell(g, (long long)cell, s, a, bi, ri);
@@ -1377,7 +1417,7 @@ __global__ void __launch_bounds__(kSharedThreads) grid_shared(GridArgs g) {
     bool todo = false;
     if (my_row < (size_t)f.S * f.A * R) {
         const size_t row = my_row;
-        const int jl = g.row_j[row];  // a shared chain implies a table and a positive rate (grid_rows)
+        const int jl = g.row_j[row];  // a shared chain implies a table and a positive rate (grid_order)
         SharedRow& x = rows[warp][lane];
         x.lo = 0;
         x.end = r_end;
@@ -1470,6 +1510,7 @@ __device__ __forceinline__ GridKey key_warp_min(GridKey c) {
 __global__ void __launch_bounds__(256) grid_finalize(GridArgs g, AllocCols winners) {
     const DevFleet& f = g.f;
     const int s = blockIdx.x;
+    pdl_wait();
     GridKey best{};
     best.acc = -1;
     for (int k = threadIdx.x; k < f.A * g.R; k += blockDim.x) {
