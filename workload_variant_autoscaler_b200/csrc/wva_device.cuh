@@ -942,6 +942,22 @@ __device__ __noinline__ int solve_stored(double* p, const double* tab, int N, in
     return 0;
 }
 
+// The two solves behind one signature, true when the solve succeeded: a streaming kernel solves with SharedSolve,
+// and its stored-vector re-run with StoredSolve on its scratch slot, which keeps the code of the last solve.
+struct SharedSolve {
+    __device__ __forceinline__ bool operator()(const double* tab, int N, int K, float lambda, ModelStats& st) const {
+        return solve_shared(tab, N, K, lambda, st) == kSolveOk;
+    }
+};
+struct StoredSolve {
+    double* p;
+    int rc;  // solve_stored's code of the last solve
+    __device__ __forceinline__ bool operator()(const double* tab, int N, int K, float lambda, ModelStats& st) {
+        rc = solve_stored(p, tab, N, K, lambda, st);
+        return rc == 0;
+    }
+};
+
 // The entries a streaming kernel bailed on, for the stored-vector re-run.  Each path packs its entry into 64 bits
 // (fb_pack for two ints).  An append past cap is counted but not stored; fb_rerun reports it.
 struct FbList {

@@ -704,7 +704,7 @@ struct WarpEval {
     __device__ __forceinline__ SzPt end(int i) const { return at(i); }
     __device__ __forceinline__ SzPt node(int v) const { return at(first ? v + 1 : v - 1); }
     __device__ __forceinline__ bool solve(float lambda, ModelStats& st) const {
-        return solve_shared(tab, N, K, lambda, st) == kSolveOk;
+        return SharedSolve{}(tab, N, K, lambda, st);
     }
 };
 
@@ -743,11 +743,10 @@ __global__ void __launch_bounds__(128) size_warp_search(SearchArgs a) { size_war
 // points, one at a time, with the literal restatement solve_stored on its scratch slot.
 // ---------------------------------------------------------------------------
 struct StoredEval {
-    double* p;
+    StoredSolve stored;
     const double* tab;
     QParams q;
     int N, K;
-    int rc;  // solve_stored's code of the last solve
     int which;
     float lo, hi;
     __device__ __forceinline__ int depth() const { return 1; }
@@ -763,59 +762,44 @@ struct StoredEval {
     }
     __device__ __forceinline__ SzPt end(int i) { return at(i ? hi : lo); }
     __device__ __forceinline__ SzPt node(int) { return at(sz_mid(lo, hi)); }
-    __device__ __forceinline__ bool solve(float lambda, ModelStats& st) {
-        rc = solve_stored(p, tab, N, K, lambda, st);
-        return rc == 0;
-    }
+    __device__ __forceinline__ bool solve(float lambda, ModelStats& st) { return stored(tab, N, K, lambda, st); }
 };
 
-// A candidate whose re-run fails is stored nil, as the drivers store a candidate that bailed.
-template <bool kStar>
-__device__ __forceinline__ void size_fallback_body(const SizeArgs& g, const FbRun& r) {
+// A candidate whose re-run fails is stored nil, as the drivers store a candidate that bailed, and returns the
+// solve's code; in search mode it is stored SEARCH_FAIL instead and the call's status is left to the SLO grid's tail.
+template <bool kStar, bool kSearch = false>
+__device__ __forceinline__ void size_fallback_body(const SizeArgs& g, const FbRun& r,
+                                                   const SearchCols& sc = SearchCols{}) {
     const DevFleet& f = g.f;
     fb_rerun(r, [&](unsigned long long item, double* p) {
         const int j = (int)item;
-        const int pair = g.cand_pair[j];
-        const int s = pair / f.A, a = pair % f.A;
+        const int pair = g.cand_pair[j], s = pair / f.A, a = pair % f.A;
         const int N = g.cand_N[j];
         StoredEval ev;
-        ev.p = p;
+        ev.stored.p = p;
         ev.tab = g.tab + 4 * g.tab_off[j];
         ev.q = qparams_of(f, s, a);
         ev.N = N;
         ev.K = N + N * f.ratio;
         Cand c;
-        const bool ok = create_allocation<kStar>(f, s, a, N, ev.K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
+        bool ok;
+        if constexpr (kSearch)
+            ok = create_allocation<kStar, true>(f, s, a, N, ev.K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c,
+                                                sc.which[j], sc.target[j]);
+        else
+            ok = create_allocation<kStar>(f, s, a, N, ev.K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c);
+        int rc = ok ? 0 : ev.stored.rc;
+        if (kSearch && !ok) {
+            c = search_cand(SEARCH_FAIL, 0.0f);
+            rc = 0;
+        }
         store_cand(g.cand, g.place.record(j, pair), c);
-        return ok ? 0 : ev.rc;
+        return rc;
     });
 }
 __global__ void size_fallback(SizeArgs g, FbRun r) { size_fallback_body<false>(g, r); }
 __global__ void size_fallback_star(SizeArgs g, FbRun r) { size_fallback_body<true>(g, r); }
-// ... in search mode, where a search whose re-run fails is stored SEARCH_FAIL and the call's status is left to the
-// SLO grid's tail.
-__global__ void size_fallback_search(SearchArgs sa, FbRun r) {
-    const SizeArgs& g = sa.g;
-    const DevFleet& f = g.f;
-    fb_rerun(r, [&](unsigned long long item, double* p) {
-        const int j = (int)item;
-        const int pair = g.cand_pair[j];
-        const int s = pair / f.A, a = pair % f.A;
-        const int N = g.cand_N[j];
-        StoredEval ev;
-        ev.p = p;
-        ev.tab = g.tab + 4 * g.tab_off[j];
-        ev.q = qparams_of(f, s, a);
-        ev.N = N;
-        ev.K = N + N * f.ratio;
-        Cand c;
-        if (!create_allocation<false, true>(f, s, a, N, ev.K, (float)ev.tab[0], (float)ev.tab[4 * (N - 1)], ev, c,
-                                            sa.search.which[j], sa.search.target[j]))
-            c = search_cand(SEARCH_FAIL, 0.0f);
-        store_cand(g.cand, g.place.record(j, pair), c);
-        return 0;
-    });
-}
+__global__ void size_fallback_search(SearchArgs sa, FbRun r) { size_fallback_body<false, true>(sa.g, r, sa.search); }
 
 // ---------------------------------------------------------------------------
 // The load grid's tail (allocation.go:134-163) at every level of a caller-given load list: one lane per (candidate,
@@ -840,28 +824,30 @@ struct LoadArgs {
     FbList fb;                  // items that bailed: fb_pack(candidate, level)
 };
 
-// Candidate e's record at totalRate total_rate(s) (nil, or the feasible allocation); solve(lambda, st) is
-// Model.Solve for the final Analyze.  Returns false when that solve bailed (out is then nil).
+// Candidate e's record at totalRate total_rate(s) (nil, or the feasible allocation); solve(tab, N, K, lambda, st)
+// is Model.Solve for the final Analyze.  Returns false when that solve bailed (out is then nil).
 template <class Total, class Solve>
-__device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, Total&& total_rate, float sN, Solve&& solve,
-                                          Cand& out) {
+__device__ __forceinline__ bool load_tail(const LoadArgs& g, int e, Total&& total_rate, Solve&& solve, Cand& out) {
     const DevFleet& f = g.f;
     const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A, N = g.cand_N[e];
+    const double* tab = g.tab + 4 * g.tab_off[e];
     out = cand_nil();
     if (!g.star_ok[pair]) return true;
     const float rate_star = g.rate_star[pair];
     SzReplicas r;
     float lam;
-    if (!sz_replicas(f, s, a, rate_max_of(sN), rate_star, total_rate(s), r, lam)) return true;
+    if (!sz_replicas(f, s, a, rate_max_of((float)tab[4 * (N - 1)]), rate_star, total_rate(s), r, lam)) return true;
     ModelStats st;
-    if (!solve(lam, st)) return false;
+    if (!solve(tab, N, N + N * f.ratio, lam, st)) return false;
     const Metrics m = metrics_from(qparams_of(f, s, a), N, st);
     out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
     return true;
 }
 
-__device__ __forceinline__ size_t load_record(const LoadArgs& g, int e, int l) {
-    return (size_t)l * g.f.S * g.f.A + g.cand_pair[e];
+// The record of item fb_pack(e, l) in the level blocks: (l * S + s) * A + a, where s * A + a is candidate e's pair.
+__device__ __forceinline__ size_t level_record(const DevFleet& f, const int* cand_pair, unsigned long long item) {
+    const int e = (int)(item >> 32), l = (int)(unsigned)item;
+    return (size_t)l * f.S * f.A + cand_pair[e];
 }
 // totalRate of server s at level l, for load_tail
 struct LevelRate {
@@ -885,44 +871,53 @@ __device__ __forceinline__ void for_each_warp_item(unsigned* counter, unsigned n
     }
 }
 
+// The two sides of every tail.  A tail evaluates a packed item, eval(item, solve, out): false when a solve bailed
+// (out is then nil); eval.record(item) is the index of its record.  The streaming side runs it with SharedSolve,
+// appends the item to fb on a bail and stores the record either way; the re-run runs it with StoredSolve and stores
+// the record only when every solve succeeded, else returns the failed solve's code.
+template <class Eval>
+__device__ __forceinline__ void tail_item(const FbList& fb, const AllocCols& cand, unsigned long long item,
+                                          const Eval& eval) {
+    Cand c;
+    if (!eval(item, SharedSolve{}, c)) fb_push(fb, item);
+    store_cand(cand, eval.record(item), c);
+}
+template <class Eval>
+__device__ __forceinline__ void tail_rerun(const FbRun& r, const AllocCols& cand, const Eval& eval) {
+    fb_rerun(r, [&](unsigned long long item, double* p) {
+        StoredSolve solve{p, 0};
+        Cand c;
+        if (!eval(item, solve, c)) return solve.rc;
+        store_cand(cand, eval.record(item), c);
+        return 0;
+    });
+}
+
+// The load grid's item fb_pack(e, l): candidate e at level l.
+struct LoadTail {
+    const LoadArgs& g;
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        return load_tail(g, (int)(item >> 32), LevelRate{g, (int)(unsigned)item}, solve, out);
+    }
+    __device__ __forceinline__ size_t record(unsigned long long item) const {
+        return level_record(g.f, g.cand_pair, item);
+    }
+};
+
 __global__ void __launch_bounds__(256) load_kernel(LoadArgs g) {
     const DevFleet& f = g.f;
     const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
     for_each_warp_item(g.counter, n_items, [&](unsigned i) {
         const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
         const float rpm = g.level_rpm[(size_t)l * f.S + g.cand_pair[e] / f.A];
-        if (!(rpm < 0.0f) && rpm != 0.0f) {  // else trivial_kernel's nil / zero-load record
-            const int N = g.cand_N[e], K = N + N * f.ratio;
-            const double* tab = g.tab + 4 * g.tab_off[e];
-            Cand c;
-            const bool ok = load_tail(g, e, LevelRate{g, l}, (float)tab[4 * (N - 1)],
-                                      [&](float lam, ModelStats& st) {
-                return solve_shared(tab, N, K, lam, st) == kSolveOk;
-            }, c);
-            if (!ok) fb_push(g.fb, fb_pack(e, l));
-            store_cand(g.cand, load_record(g, e, l), c);
-        }
+        // a level without load keeps trivial_kernel's nil / zero-load record
+        if (!(rpm < 0.0f) && rpm != 0.0f) tail_item(g.fb, g.cand, fb_pack(e, l), LoadTail{g});
     });
 }
 
 // Stored-vector re-run of the items load_kernel bailed on.
-__global__ void load_fallback(LoadArgs g, FbRun r) {
-    const DevFleet& f = g.f;
-    fb_rerun(r, [&](unsigned long long item, double* p) {
-        const int e = (int)(item >> 32), l = (int)(unsigned)item;
-        const int N = g.cand_N[e], K = N + N * f.ratio;
-        const double* tab = g.tab + 4 * g.tab_off[e];
-        int rc = 0;
-        Cand c;
-        if (!load_tail(g, e, LevelRate{g, l}, (float)tab[4 * (N - 1)], [&](float lam, ModelStats& st) {
-                rc = solve_stored(p, tab, N, K, lam, st);
-                return rc == 0;
-            }, c))
-            return rc;
-        store_cand(g.cand, load_record(g, e, l), c);
-        return 0;
-    });
-}
+__global__ void load_fallback(LoadArgs g, FbRun r) { tail_rerun(r, g.cand, LoadTail{g}); }
 
 // ---------------------------------------------------------------------------
 // The SLO grid's tail (DESIGN.md §3.11): CreateAllocation of every load pair at every level of a caller-given list
@@ -963,76 +958,60 @@ __device__ __forceinline__ DevFleet at_slo_level(const SloArgs& g, int l) {
     return fl;
 }
 
-// Candidate e's record at level l; solve(lambda, st) is Model.Solve for the two Analyze calls.  Returns false when
-// a solve bailed (out is then nil).
-template <class Solve>
-__device__ __forceinline__ bool slo_tail(const SloArgs& g, int e, int l, Solve&& solve, Cand& out) {
-    const DevFleet f = at_slo_level(g, l);
-    const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A;
-    const int N = g.cand_N[e], K = N + N * f.ratio;
-    const double* tab = g.tab + 4 * g.tab_off[e];
-    out = cand_nil();
-    const SzStart b = sz_start(f, s, K, (float)tab[0], (float)tab[4 * (N - 1)]);
-    if (b.nil) return true;
-    float xs[2] = {b.lmax, b.lmax};  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
-    for (int w = 0; w < 2; ++w) {
-        const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
-        if (!(target > 0.0f)) continue;
-        const size_t k = (size_t)g.key[((size_t)l * f.S + s) * 2 + w] * f.A + a;
-        const int st = g.srch.feasible[k];
-        if (st == SEARCH_FAIL) {
-            atomicExch(g.status, 1);
-            return true;
-        }
-        if (st == SEARCH_NIL) return true;
-        xs[w] = g.srch.max_rate[k];
+// The SLO grid's item fb_pack(e, l): candidate e at level l; solve is Model.Solve for the two Analyze calls.
+struct SloTail {
+    const SloArgs& g;
+    __device__ __forceinline__ size_t record(unsigned long long item) const {
+        return level_record(g.f, g.cand_pair, item);
     }
-    float lam;
-    ModelStats st;
-    if (!sz_lambda(f, s, b.rmax, xs[0], xs[1], lam)) return true;
-    if (!solve(tab, N, K, lam, st)) return false;
-    const QParams q = qparams_of(f, s, a);
-    const float rate_star = metrics_from(q, N, st).throughput;
-    SzReplicas r;
-    if (!sz_replicas(f, s, a, b.rmax, rate_star, total_rate_of(f, s), r, lam)) return true;
-    if (!solve(tab, N, K, lam, st)) return false;
-    const Metrics m = metrics_from(q, N, st);
-    out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
-    return true;
-}
-
-__device__ __forceinline__ size_t slo_record(const SloArgs& g, int e, int l) {
-    return (size_t)l * g.f.S * g.f.A + g.cand_pair[e];
-}
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        const int e = (int)(item >> 32), l = (int)(unsigned)item;
+        const DevFleet f = at_slo_level(g, l);
+        const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A;
+        const int N = g.cand_N[e], K = N + N * f.ratio;
+        const double* tab = g.tab + 4 * g.tab_off[e];
+        out = cand_nil();
+        const SzStart b = sz_start(f, s, K, (float)tab[0], (float)tab[4 * (N - 1)]);
+        if (b.nil) return true;
+        float xs[2] = {b.lmax, b.lmax};  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
+        for (int w = 0; w < 2; ++w) {
+            const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+            if (!(target > 0.0f)) continue;
+            const size_t k = (size_t)g.key[((size_t)l * f.S + s) * 2 + w] * f.A + a;
+            const int st = g.srch.feasible[k];
+            if (st == SEARCH_FAIL) {
+                atomicExch(g.status, 1);
+                return true;
+            }
+            if (st == SEARCH_NIL) return true;
+            xs[w] = g.srch.max_rate[k];
+        }
+        float lam;
+        ModelStats st;
+        if (!sz_lambda(f, s, b.rmax, xs[0], xs[1], lam)) return true;
+        if (!solve(tab, N, K, lam, st)) return false;
+        const QParams q = qparams_of(f, s, a);
+        const float rate_star = metrics_from(q, N, st).throughput;
+        SzReplicas r;
+        if (!sz_replicas(f, s, a, b.rmax, rate_star, total_rate_of(f, s), r, lam)) return true;
+        if (!solve(tab, N, K, lam, st)) return false;
+        const Metrics m = metrics_from(q, N, st);
+        out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
+        return true;
+    }
+};
 
 __global__ void __launch_bounds__(256) slo_kernel(SloArgs g) {
     const unsigned n_items = (unsigned)g.n_cand * (unsigned)g.L;  // <= S * A * L < 2^31
     for_each_warp_item(g.counter, n_items, [&](unsigned i) {
         const int e = (int)(i / (unsigned)g.L), l = (int)(i - (unsigned)e * g.L);
-        Cand c;
-        const bool ok = slo_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-            return solve_shared(tab, N, K, lam, st) == kSolveOk;
-        }, c);
-        if (!ok) fb_push(g.fb, fb_pack(e, l));
-        store_cand(g.cand, slo_record(g, e, l), c);
+        tail_item(g.fb, g.cand, fb_pack(e, l), SloTail{g});
     });
 }
 
 // Stored-vector re-run of the items slo_kernel bailed on.
-__global__ void slo_fallback(SloArgs g, FbRun r) {
-    fb_rerun(r, [&](unsigned long long item, double* p) {
-        const int e = (int)(item >> 32), l = (int)(unsigned)item;
-        int rc = 0;
-        Cand c;
-        if (!slo_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-                rc = solve_stored(p, tab, N, K, lam, st);
-                return rc == 0;
-            }, c))
-            return rc;
-        store_cand(g.cand, slo_record(g, e, l), c);
-        return 0;
-    });
-}
+__global__ void slo_fallback(SloArgs g, FbRun r) { tail_rerun(r, g.cand, SloTail{g}); }
 
 // ---------------------------------------------------------------------------
 // The workload grid's tail (DESIGN.md §3.12): the load grid's tail (load_tail) on the key fleet, whose row k is
@@ -1066,51 +1045,33 @@ __device__ __forceinline__ void workload_item(const WorkloadArgs& g, int i, int&
     l = g.lev[g.lev_off[k] + (i - g.item_off[e])];
 }
 
-// Candidate e's record at level l and its index; solve(tab, N, K, lambda, st) is Model.Solve for the final
-// Analyze.  Returns false when that solve bailed (out is then nil).
-template <class Solve>
-__device__ __forceinline__ bool workload_tail(const WorkloadArgs& g, int e, int l, Solve&& solve, Cand& out,
-                                              size_t& rec) {
-    const DevFleet& f = g.ld.f;
-    const int pair = g.ld.cand_pair[e], k = pair / f.A, s = g.key_srv[k];
-    const float rpm = g.ld.level_rpm[(size_t)l * g.S + s];
-    rec = ((size_t)l * g.S + s) * f.A + pair % f.A;
-    const int N = g.ld.cand_N[e], K = N + N * f.ratio;
-    const double* tab = g.ld.tab + 4 * g.ld.tab_off[e];
-    return load_tail(g.ld, e, [&](int) { return total_rate_of(f, k, rpm); }, (float)tab[4 * (N - 1)],
-                     [&](float lam, ModelStats& st) { return solve(tab, N, K, lam, st); }, out);
-}
+// The workload grid's item fb_pack(e, l): candidate e at level l, from workload_item.
+struct WorkloadTail {
+    const WorkloadArgs& g;
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        const int e = (int)(item >> 32), l = (int)(unsigned)item;
+        const int k = g.ld.cand_pair[e] / g.ld.f.A;
+        const float rpm = g.ld.level_rpm[(size_t)l * g.S + g.key_srv[k]];
+        return load_tail(g.ld, e, [&](int) { return total_rate_of(g.ld.f, k, rpm); }, solve, out);
+    }
+    // record (l * S + s) * A + a of the key's server s
+    __device__ __forceinline__ size_t record(unsigned long long item) const {
+        const int pair = g.ld.cand_pair[item >> 32], l = (int)(unsigned)item;
+        return ((size_t)l * g.S + g.key_srv[pair / g.ld.f.A]) * g.ld.f.A + pair % g.ld.f.A;
+    }
+};
 
 __global__ void __launch_bounds__(256) workload_kernel(WorkloadArgs g) {
     for_each_warp_item(g.ld.counter, (unsigned)g.n_items, [&](unsigned i) {
         int e, l;
         workload_item(g, (int)i, e, l);
-        Cand c;
-        size_t rec;
-        const bool ok = workload_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-            return solve_shared(tab, N, K, lam, st) == kSolveOk;
-        }, c, rec);
-        if (!ok) fb_push(g.ld.fb, fb_pack(e, l));
-        store_cand(g.ld.cand, rec, c);
+        tail_item(g.ld.fb, g.ld.cand, fb_pack(e, l), WorkloadTail{g});
     });
 }
 
 // Stored-vector re-run of the items workload_kernel bailed on.
-__global__ void workload_fallback(WorkloadArgs g, FbRun r) {
-    fb_rerun(r, [&](unsigned long long item, double* p) {
-        const int e = (int)(item >> 32), l = (int)(unsigned)item;
-        int rc = 0;
-        Cand c;
-        size_t rec;
-        if (!workload_tail(g, e, l, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-                rc = solve_stored(p, tab, N, K, lam, st);
-                return rc == 0;
-            }, c, rec))
-            return rc;
-        store_cand(g.ld.cand, rec, c);
-        return 0;
-    });
-}
+__global__ void workload_fallback(WorkloadArgs g, FbRun r) { tail_rerun(r, g.ld.cand, WorkloadTail{g}); }
 
 // ---------------------------------------------------------------------------
 // Load intervals (DESIGN.md §3.10): per server, the float32 arrival rates in [lo, hi] at which the load grid's
@@ -1322,46 +1283,29 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     }
 }
 
-// The record at an interval start whose winner is a load pair: the load grid's tail at that rate, then the value.
-template <class Solve>
-__device__ __forceinline__ bool iv_tail(const IntervalArgs& g, unsigned long long item, Solve&& solve, Cand& c) {
-    const DevFleet& f = g.ld.f;
-    const int r = (int)(unsigned)item, a = (int)(item >> 32), s = r / g.M;
-    const int e = g.cand_of_pair[s * f.A + a], N = g.ld.cand_N[e];
-    const double* tab = g.ld.tab + 4 * g.ld.tab_off[e];
-    if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, g.start[r]); }, (float)tab[4 * (N - 1)],
-                   [&](float lam, ModelStats& st) { return solve(tab, N, N + N * f.ratio, lam, st); }, c))
-        return false;
-    if (c.feasible) c.value = penalty_of(f, s, c);
-    return true;
-}
+// The item fb_pack(a, r): the record r at an interval start whose winner is the load pair of accelerator a, the load
+// grid's tail at that rate, then the value.
+struct IvTail {
+    const IntervalArgs& g;
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        const DevFleet& f = g.ld.f;
+        const int r = (int)(unsigned)item, a = (int)(item >> 32), s = r / g.M;
+        const int e = g.cand_of_pair[s * f.A + a];
+        if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, g.start[r]); }, solve, out)) return false;
+        if (out.feasible) out.value = penalty_of(f, s, out);
+        return true;
+    }
+    __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
+};
 
 __global__ void __launch_bounds__(256) interval_tail(IntervalArgs g) {
     const int n = min(*g.items.count, g.items.cap);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const unsigned long long item = g.items.item[i];
-        Cand c;
-        const bool ok = iv_tail(g, item, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-            return solve_shared(tab, N, K, lam, st) == kSolveOk;
-        }, c);
-        if (!ok) fb_push(g.ld.fb, item);
-        store_cand(g.rec, (unsigned)item, c);
-    }
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        tail_item(g.ld.fb, g.rec, g.items.item[i], IvTail{g});
 }
 
 // Stored-vector re-run of the interval starts interval_tail bailed on.
-__global__ void interval_fallback(IntervalArgs g, FbRun r) {
-    fb_rerun(r, [&](unsigned long long item, double* p) {
-        int rc = 0;
-        Cand c;
-        if (!iv_tail(g, item, [&](const double* tab, int N, int K, float lam, ModelStats& st) {
-                rc = solve_stored(p, tab, N, K, lam, st);
-                return rc == 0;
-            }, c))
-            return rc;
-        store_cand(g.rec, (unsigned)item, c);
-        return 0;
-    });
-}
+__global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec, IvTail{g}); }
 
 }  // namespace wva
