@@ -543,6 +543,36 @@ int wva_load_intervals(wva_handle *h, const wva_fleet *fleet, const float *rpm_l
                        wva_intervals *out);
 
 /*
+ * Price thresholds: for each server s and accelerator a, the exact accelerator price at which s's unlimited
+ * winner leaves a.  Let f(p) be the fleet with acc_cost[a] = p, solved in unlimited mode.
+ *
+ * threshold[s*A + a] is the smallest float32 p in [+0, MaxFloat32] at which s's wva_solve winner on f(p) is not
+ * a's candidate, and +Inf when a's candidate wins at every such p.  a's candidate wins at every price below the
+ * threshold (DESIGN.md §3.16): CreateAllocation reads p only in the cost of a's own candidates (cost = p *
+ * NumInstances * replicas), the current cost srv_cur_cost is not re-priced (as in wva_profile_grid), and
+ * TransitionPenalty of a's candidate never decreases as p grows.  So 0 means a never wins at a non-negative
+ * price: a nil or keepAccelerator-masked pair, a NaN value, or a candidate beaten at cost 0.  A candidate whose
+ * value does not read p (same accelerator and replica count as the current allocation, penalty 0) gets 0 or
+ * +Inf.  Negative prices are outside the contract.  Column a of threshold does not depend on the fleet's own
+ * acc_cost[a].
+ *
+ * above[s*A + a] is byte for byte wva_profile_grid's winner record for s at the row acc_cost[a] = threshold:
+ * where s goes once a is too expensive (a nil record when no other candidate can win).  It is zero bytes where
+ * the threshold is +Inf.  candidates (S*A) is byte for byte what wva_analyze returns for the fleet.  above and
+ * candidates may be NULL, and so may any of their columns (not written).
+ *
+ * Only unlimited mode is covered: fleet->unlimited and the capacities are not read.  The fleet becomes
+ * resident, and wva_summarize returns WVA_ERR_STATE afterwards.  WVA_ERR_BAD_ARG: threshold NULL with S*A > 0.
+ * WVA_ERR_UNSUPPORTED: whatever wva_analyze refuses (the queue-size rule, a rescale loop that would not
+ * terminate, too many stored-vector fallbacks), and, before any kernel is launched, the inputs on which a
+ * candidate's value could decrease as its price grows: a penalty factor (tun.accel_penalty_factor) that is NaN,
+ * negative or infinite, or an srv_cur_cost that is NaN or infinite on a server with a pair wva_analyze does not
+ * class nil (a pair it sizes, or a zero-load candidate).
+ */
+int wva_price_thresholds(wva_handle *h, const wva_fleet *fleet, float *threshold /* [S*A] */,
+                         wva_allocs *above /* [S*A], may be NULL */, wva_allocs *candidates /* [S*A], may be NULL */);
+
+/*
  * Solver.SolveGreedy + the best-effort saturation policies (pkg/solver/greedy.go:35-341) over a candidate
  * table the caller already holds: `candidates` (S*A, value = transition penalty as wva_analyze returns it) is
  * read, and modified where the reference scales best-effort allocations; `winners` (S) is written.  Host only

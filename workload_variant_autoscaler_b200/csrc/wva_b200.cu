@@ -211,6 +211,7 @@ struct wva_handle {
     DevBuf d_iv;       // the load intervals' counts, flags, starts and work list
     DevBuf d_slo;      // the SLO grid's search records
     DevBuf d_prof;     // the profile grid's key records
+    DevBuf d_price;    // the price thresholds
 
     // grid path
     DevBuf d_sort, d_best, d_pb, d_rows;
@@ -1858,6 +1859,35 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
     return WVA_OK;
 }
 
+// ---- price thresholds: the price of each accelerator at which each server's winner leaves it (DESIGN.md §3.16) --
+// The inputs on which a pair's value can decrease as its price grows, so that its winning prices need not be one
+// interval from 0: a penalty factor that is NaN, negative or infinite, or a non-finite current cost on a server
+// that has a candidate (a pair wva_analyze does not class nil).  nullptr when there is none.
+const char* price_refusal(const HostFleet& hf) {
+    const float f = hf.tun.accel_penalty_factor;
+    if (!(f >= 0.0f) || std::isinf(f)) return "penalty factor NaN, negative or infinite";
+    for (int s = 0; s < hf.S; ++s) {
+        if (std::isfinite(hf.srv_cur_cost[s])) continue;
+        for (int a = 0; a < hf.A; ++a)
+            if (hf.pair_class(s, a, true)) return "current cost NaN or infinite on a server with a candidate";
+    }
+    return nullptr;
+}
+
+// wva_analyze's sizing and values into cand ([S*A]), then price_kernel: threshold ([S*A], device) and above
+// ([S*A] records; at least S, which the sizing's winners use first).
+int enqueue_price_thresholds(wva_handle* h, float* threshold, const AllocCols& cand, const AllocCols& above) {
+    int rc = enqueue_size(h, cand, &above);
+    if (rc) return rc;
+    const HostFleet& hf = h->hf;
+    if ((long long)hf.S * hf.A > 0) {
+        price_kernel<<<(hf.S + 3) / 4, 128, 0, h->stream>>>(h->df, cand, threshold, above);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
 // ---- grid path (K2 + K3) ----------------------------------------------------
 int validate_grid(wva_handle* h, const wva_grid* g) {
     if (!g) return h->fail(WVA_ERR_BAD_ARG, "grid is NULL");
@@ -2790,6 +2820,31 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;
     scatter_block(c.cand_host, c.bc, &out->rec);
+    return WVA_OK;
+}
+
+int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold, wva_allocs* above,
+                         wva_allocs* candidates) {
+    if (!h) return WVA_ERR_BAD_ARG;
+    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
+    const long long n = (long long)fleet->n_servers * fleet->n_acc;
+    if (n > 0 && !threshold) return h->fail(WVA_ERR_BAD_ARG, "threshold is NULL");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    if (const char* what = price_refusal(h->hf)) return h->fail(WVA_ERR_UNSUPPORTED, what);
+    Cols th(16);
+    th.take(4 * (size_t)n, threshold);
+    CK(h->d_price.ensure(th.bytes));
+    HostCall c{(size_t)n, candidates != nullptr, above != nullptr && n > 0, &th, h->d_price.p};
+    c.win_blocks = (size_t)std::max(fleet->n_acc, 1);  // above, and the sizing's S winners before it
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols& dw) {
+        return enqueue_price_thresholds(h, (float*)h->d_price.p, dc, dw);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    scatter_block(c.cand_host, c.bc, candidates);
+    if (c.win_host) scatter_block(c.win_host, c.bw, above);
     return WVA_OK;
 }
 

@@ -1769,11 +1769,16 @@ __device__ __forceinline__ DevFleet profile_at(const ProfileArgs& g, int l) {
 #undef WVA_PROFILE_ROW
     return fl;
 }
+// CreateAllocation's cost of `replicas` replicas of model m on accelerator a at price `price`
+// (allocation.go:144-145, zeroLoadAllocation :274-275).
+__device__ __forceinline__ float cost_at(const DevFleet& fl, int m, int a, int replicas, float price) {
+    return __fmul_rn(price, (float)((long long)num_instances(fl, m, a) * (long long)replicas));
+}
 // A load record sized at another price or AccCount, priced at fl: cost = acc_cost[a] * NumInstances(m, a) *
 // replicas and value = cost, the only fields of CreateAllocation that read either.
 __device__ __forceinline__ Cand priced_at(const DevFleet& fl, int m, int a, Cand c) {
     if (c.feasible) {
-        c.cost = __fmul_rn(fl.acc_cost[a], (float)((long long)num_instances(fl, m, a) * (long long)c.replicas));
+        c.cost = cost_at(fl, m, a, c.replicas, fl.acc_cost[a]);
         c.value = c.cost;
     }
     return c;
@@ -1825,6 +1830,85 @@ __global__ void profile_trace_kernel(ProfileTraceArgs g) {
     if (cls == PAIR_ZERO) c = zero_load_alloc(ft, s, a);
     else if (cls == PAIR_LOAD) c = priced_at(ft, ft.srv_model[s], a, load_cand(p.cand, i));
     store_cand(p.cand, i, c);
+}
+
+// The price thresholds (DESIGN.md §3.16): one warp per server over wva_analyze's records (value = TransitionPenalty),
+// lane l owning accelerators l, l + 32, ...  SolveUnlimited picks the least (value, accelerator id) among the
+// feasible records whose value is below MaxFloat32, so a wins at price p iff V_a(p) < MaxFloat32 and (V_a(p), a)
+// precedes the best other record w: the server's best record, or its second best where a is the best.  V_a(p) is
+// TransitionPenalty of a's record at cost_at(.., p), and no other record reads p.  It never decreases as p grows
+// (a NaN counted as +Inf), so a wins on [+0, threshold), found by bisecting the non-negative float32 bit patterns.
+// above is w's record (nil without one), zero bytes where the threshold is +Inf.
+struct PriceBest {  // a record's (value, accelerator id); id INT_MAX: none
+    float v;
+    int a;
+};
+__device__ __forceinline__ bool price_before(float v, int a, const PriceBest& b) {
+    return v < b.v || (v == b.v && a < b.a);
+}
+__device__ __forceinline__ PriceBest shfl_xor_best(const PriceBest& b, int d) {
+    return PriceBest{__shfl_xor_sync(0xffffffffu, b.v, d), __shfl_xor_sync(0xffffffffu, b.a, d)};
+}
+__global__ void __launch_bounds__(128) price_kernel(DevFleet f, AllocCols cand, float* threshold, AllocCols above) {
+    const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (s >= f.S) return;  // whole warps
+    const float max_f32 = 3.40282346638528859811704183484516925440e+38f;
+    const unsigned max_bits = 0x7f7fffffu;
+    const PriceBest none{__int_as_float(0x7f800000), INT_MAX};
+    // the server's two best records: each lane's own, then merged across the warp (accelerator ids are distinct)
+    PriceBest b1 = none, b2 = none;
+    for (int a = lane; a < f.A; a += 32) {
+        const size_t i = (size_t)s * f.A + a;
+        if (!cand.feasible[i]) continue;
+        const float v = cand.value[i];
+        if (!(v < max_f32)) continue;
+        if (price_before(v, a, b1)) {
+            b2 = b1;
+            b1 = PriceBest{v, a};
+        } else if (price_before(v, a, b2)) {
+            b2 = PriceBest{v, a};
+        }
+    }
+    for (int d = 16; d > 0; d >>= 1) {
+        const PriceBest o1 = shfl_xor_best(b1, d), o2 = shfl_xor_best(b2, d);
+        if (price_before(o1.v, o1.a, b1)) {
+            b2 = price_before(b1.v, b1.a, o2) ? b1 : o2;
+            b1 = o1;
+        } else if (price_before(o1.v, o1.a, b2)) {
+            b2 = o1;
+        }
+    }
+    const int m = f.srv_model[s], cur_acc = f.srv_cur_acc[s], cur_replicas = f.srv_cur_replicas[s];
+    const float cur_cost = f.srv_cur_cost[s];
+    for (int a = lane; a < f.A; a += 32) {
+        const size_t i = (size_t)s * f.A + a;
+        const PriceBest w = b1.a == a ? b2 : b1;
+        float t = 0.0f;  // a never wins: nil, masked, or beaten at every price
+        if (cand.feasible[i]) {
+            const int acc = cand.acc[i], replicas = cand.replicas[i];
+            const auto wins = [&](unsigned bits) {
+                const float v = transition_penalty(f.penalty, cur_acc, cur_replicas, cur_cost, acc, replicas,
+                                                   cost_at(f, m, a, replicas, __uint_as_float(bits)));
+                return v < max_f32 && price_before(v, a, w);
+            };
+            if (wins(max_bits)) {
+                t = __int_as_float(0x7f800000);
+            } else if (wins(0u)) {
+                unsigned lo = 0u, hi = max_bits;  // a wins at lo, not at hi
+                while (hi - lo > 1u) {
+                    const unsigned mid = lo + (hi - lo) / 2u;
+                    if (wins(mid)) lo = mid;
+                    else hi = mid;
+                }
+                t = __uint_as_float(hi);
+            }
+        }
+        threshold[i] = t;
+        Cand r = {};
+        if (!isinf(t)) r = w.a == INT_MAX ? cand_nil() : load_cand(cand, (size_t)s * f.A + w.a);
+        store_cand(above, i, r);
+    }
 }
 
 // wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record

@@ -40,6 +40,37 @@ def greedy_solve(fleet: Fleet, candidates: Allocs):
     return candidates, win
 
 
+def accelerator_demand(fleet: Fleet, threshold, candidates: Allocs, a: int):
+    """The fleet's demand curve for accelerator ``a`` in unlimited mode, from ``Engine.price_thresholds``' output
+    (host only, no GPU) -> (breakpoints, units).
+
+    ``breakpoints`` are the ascending distinct thresholds of column ``a`` in (0, MaxFloat32].  They cut the prices
+    [+0, MaxFloat32] into ``len(breakpoints) + 1`` stretches: [0, b_0), [b_0, b_1), ..., [b_last, MaxFloat32].
+    ``units[j]`` (int64) is the number of ``a``'s units the unlimited winners use at every price of stretch ``j``,
+    counted as ``System.AllocateByType`` counts them (pkg/core/system.go:271-300): replicas * NumInstances *
+    multiplicity over the servers whose winner is ``a``'s candidate, i.e. whose threshold lies above the price.  A
+    zero-replica candidate (accelerator "") uses no units."""
+    S, A = fleet.n_servers, fleet.n_acc
+    if not 0 <= a < A:
+        raise ValueError(f"accelerator {a} out of range [0, {A})")
+    th = np.ascontiguousarray(threshold, np.float32)
+    if th.shape != (S, A) or candidates.n != S * A:
+        raise ValueError("threshold must have shape (n_servers, n_acc) and candidates n_servers * n_acc records")
+    col = th[:, a]
+    idx = np.arange(S) * A + a
+    m = fleet.srv_model
+    on_a = candidates.acc[idx] == a  # a feasible record in column a is on a, or on "" with 0 replicas
+    inst = np.maximum(fleet.perf_acc_count[np.where(on_a, m, 0), a].astype(np.int64), 1)
+    units = np.where(on_a, candidates.replicas[idx].astype(np.int64) * inst, 0) * int(fleet.acc_multiplicity[a])
+    breakpoints = np.unique(col[(col > 0) & np.isfinite(col)])
+    starts = np.concatenate([[np.float32(0.0)], breakpoints]).astype(np.float32)
+    # server s wins on the stretches that start below threshold[s]: the first k[s] of them
+    k = np.searchsorted(starts, col, side="left")
+    per_k = np.zeros(starts.size + 1, np.int64)
+    np.add.at(per_k, k, units)
+    return breakpoints, np.cumsum(per_k[::-1])[::-1][1:]
+
+
 # the fleet column each load or target row list replaces (every other row list is named after its column)
 _ROW_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens",
                "slo_itl": "srv_slo_itl", "slo_ttft": "srv_slo_ttft", "slo_tps": "srv_slo_tps"}
@@ -317,6 +348,27 @@ class Engine:
         self._resident(fleet)
         self._check(self._L.wva_load_intervals(self._h, C.byref(fc), _abi.ptr(lo), _abi.ptr(hi), C.byref(oc)))
         return count, truncated, start, rec
+
+    def price_thresholds(self, fleet: Fleet, want_candidates: bool = False):
+        """The exact price of each accelerator at which each server's unlimited winner leaves it -> (threshold
+        (S, A) float32, above: ``Allocs`` of S * A, candidates [S*A] | None).
+
+        ``threshold[s, a]`` is the smallest float32 price ``p`` in [+0, MaxFloat32] at which ``solve``'s winner for
+        ``s`` on the fleet with ``acc_cost[a] = p`` is not ``a``'s candidate (+Inf when it is at every price; 0 when
+        it never is).  Record ``s * A + a`` of ``above`` is ``profile_grid``'s winner for ``s`` at that price (zero
+        bytes where the threshold is +Inf), and ``candidates`` is what ``analyze`` returns.  ``srv_cur_cost`` is not
+        re-priced; ``fleet.unlimited`` and the capacities are not read (see ``wva_price_thresholds`` in
+        include/wva_b200.h).  ``accelerator_demand`` turns a column into a demand curve."""
+        S, A = fleet.n_servers, fleet.n_acc
+        threshold = np.zeros((S, A), np.float32)
+        above = Allocs(S * A)
+        cand = Allocs(S * A) if want_candidates else None
+        fc, ac = fleet.as_c(), above.as_c()
+        cc = cand.as_c() if cand is not None else None
+        self._resident(fleet)
+        self._check(self._L.wva_price_thresholds(self._h, C.byref(fc), _abi.ptr(threshold.reshape(-1)), C.byref(ac),
+                                                 C.byref(cc) if cc is not None else None))
+        return threshold, above, cand
 
     def sweep(self, fleet: Fleet, n_rates: int) -> dict:
         n = fleet.n_servers * fleet.n_acc * n_rates
