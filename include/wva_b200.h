@@ -403,6 +403,48 @@ int wva_workload_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, c
                        wva_allocs *winners);
 
 /*
+ * SLO trace: wva_workload_trace over ticks that also carry service-class targets, e.g. a time-of-day SLO schedule (a
+ * premium class whose ITL is tightened during business hours and relaxed overnight), or a proposed target change
+ * replayed over recorded traffic.  The controller re-reads the service classes on every reconcile, so a target edit
+ * takes effect at the next tick, as a load change does.
+ *
+ * Let f_t be the fleet with srv_arrival_rpm, srv_in_tokens, srv_out_tokens, srv_slo_itl, srv_slo_ttft and srv_slo_tps
+ * replaced by row t of the six lists (each [n_ticks * S], index t*S + s, in the units of the fleet's columns; a NULL
+ * list is the fleet's own column at every tick) and its current allocation (srv_cur_acc, srv_cur_replicas,
+ * srv_cur_cost) by c_t.
+ *   - Candidate block t (records (t*S + s)*A + a) is byte for byte what wva_analyze returns for f_t, value =
+ *     TransitionPenalty against c_t and the keepAccelerator mask against c_t included.
+ *   - Winner block t (records t*S + s) is byte for byte wva_solve's winner block for f_t with unlimited = 1.
+ *   - c_0 is the fleet's current allocation; c_{t+1} is winner t's (acc, replicas, cost) when that winner is
+ *     feasible, and c_t otherwise (wva_workload_trace's rule).
+ * Only unlimited mode is traced; fleet->unlimited and the capacities are not read.  A trace can be continued as
+ * wva_workload_trace's: ticks 0..L-1 equal ticks 0..k-1 followed by ticks k..L-1 on the fleet whose srv_cur_* hold
+ * c_k.  With the three target lists NULL the call returns wva_workload_trace's result on the same load rows; with one
+ * tick it returns wva_slo_grid's for that row on the fleet whose load columns are the tick's.
+ *
+ * Sizing (DESIGN.md §3.17): Size, lambda* and rateStar read the tokens but not the rate, and each bisection reads only
+ * its own target, so a search is fixed by (server, accelerator, in, out, which search, target bits).  Each distinct
+ * search that some tick needs (its three targets not negative, the search's target > 0) runs once, in one batched
+ * pass; per tick only lambda*, rateStar, the replica count and the final Analyze run, then the chain.  As in
+ * wva_workload_trace, a pinned server sizes only its current pair and every other server sizes all its pairs,
+ * keepAccelerator ignored.  With the fleet's own tokens, an ITL schedule of two values over 24 ticks runs three
+ * searches per pair (one TTFT, two ITL) instead of 48.
+ *
+ * The fleet becomes resident; wva_summarize returns WVA_ERR_STATE afterwards.  `candidates` (n_ticks*S*A entries)
+ * may be NULL; `winners` has n_ticks*S entries.  n_ticks == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG:
+ * n_ticks < 0, fleet NULL or winners NULL.  WVA_ERR_UNSUPPORTED: S*A*n_ticks >= 2^31 (refused before the fleet is
+ * read); 2^31 or more search records (distinct search keys x A); or the union over ticks of wva_analyze(f_t)'s
+ * failures for the pairs the call sizes: a load pair outside the queue-size rule, a rescale loop that would not
+ * terminate (a NaN or tiny TPS target can cause one), or too many stored-vector fallbacks.  As with
+ * wva_workload_trace, these can exceed the per-tick refusals only through the pairs of keep servers that are not
+ * pinned, and the result never differs from the per-tick composition.  As in wva_slo_grid, a search that no tick's
+ * reference would run (the ITL search after a failed TTFT search) does not fail the call.
+ */
+int wva_slo_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                  const int32_t *in_tokens, const int32_t *out_tokens, const float *slo_itl, const float *slo_ttft,
+                  const float *slo_tps, wva_allocs *candidates, wva_allocs *winners);
+
+/*
  * Rows of accelerator costs and model x accelerator performance data for wva_profile_grid.  Any pointer may be NULL:
  * that column is the fleet's own at every level.
  */

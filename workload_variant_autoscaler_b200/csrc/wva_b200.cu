@@ -1086,77 +1086,101 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
 // the server has load pairs.  Lists, tables (lg_tabs, shared with the load grid and the load intervals) and the
 // search records (d_slo) are rebuilt on every call.  itl / ttft / tps [L*S] are the caller's rows; cand ([L*S*A])
 // and winners ([L*S]) are device columns.
-int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, const float* tps,
-                     const AllocCols& cand, const AllocCols& winners) {
-    const HostFleet& hf = h->hf;
-    const int S = hf.S, A = hf.A;
-    const size_t LS = (size_t)L * S;
-    // the tail's candidates: every load pair (none without levels), descending N, one N-entry table each
-    std::vector<int> pairs, Ns;
-    if (L > 0) {
-        const int rc =
-            sorted_pairs(h, hf, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
-        if (rc) return rc;
-    }
-    std::vector<int> tab_of((size_t)S * A, -1);  // the pair's table index
-    std::vector<long long> tab_entry(pairs.size());
-    long long entries = 0;
-    for (size_t t = 0; t < pairs.size(); ++t) {
-        tab_of[pairs[t]] = (int)t;
-        tab_entry[t] = entries;
-        entries += Ns[t];
-    }
-    std::vector<int> n_load(S, 0);
-    for (int p : pairs) n_load[p / A]++;
-    // the search keys: per server, its distinct (search, target bits) in that order, so a server's keys are
-    // key_begin[s] .. key_begin[s + 1] - 1
-    std::vector<int> key(2 * LS, -1), key_begin(S + 1, 0);
-    std::vector<uint8_t> key_w;
-    std::vector<float> key_t;
-    std::vector<std::pair<uint64_t, size_t>> uses;  // (search << 32 | target bits, index into key)
-    for (int s = 0; s < S; ++s) {
-        key_begin[s] = (int)key_w.size();
-        if (!n_load[s]) continue;
-        uses.clear();
-        for (int l = 0; l < L; ++l) {
-            const size_t i = (size_t)l * S + s;
-            if (itl[i] < 0.0f || ttft[i] < 0.0f || tps[i] < 0.0f) continue;
-            for (int w = 0; w < 2; ++w) {
-                const float t = w == 0 ? ttft[i] : itl[i];
-                if (!(t > 0.0f)) continue;
-                uint32_t bits;
-                memcpy(&bits, &t, 4);
-                uses.emplace_back((uint64_t)w << 32 | bits, 2 * i + w);
+//
+// SloKeys holds phase 1's searches for the SLO grid and the SLO trace: a search is fixed by (key row, accelerator,
+// which search, target bits), where a key row is one (server, tokens) with the rows at which it applies.  The grid's
+// key rows are the resident servers, each at every level; the trace's are the workload trace's token keys, each at
+// the ticks that use its tokens under load.  build() lists, per key row with load pairs, its distinct (search, target
+// bits) in that order and crosses them with the row's load pairs (the tail's candidates `pairs`, descending N, one
+// N-entry table each): the search candidates, still in descending N.  The target row lists and the key of each (row,
+// server, search) travel in the call's upload image (place, write); enqueue() runs the searches in search mode over
+// the tables of lg_tabs, records in d_slo.
+struct SloKeys {
+    std::vector<int> key;        // [2 * L * S] key of (row l, server s, search w) at (l * S + s) * 2 + w; -1: none
+    std::vector<uint8_t> key_w;  // per key: its search (0: TTFT, 1: ITL) ...
+    std::vector<float> key_t;    // ... and target
+    std::vector<std::pair<int, int>> sc;  // the search candidates (key, pair)
+    std::vector<int> tab_of;              // a pair's table index
+    std::vector<long long> tab_entry;     // a table's first entry
+    size_t o_itl = 0, o_ttft = 0, o_tps = 0, o_key = 0, o_pair = 0, o_N = 0, o_rec = 0, o_idx = 0, o_off = 0,
+           o_tgt = 0, o_which = 0;
+    AllocCols srch{};  // the search records by key * A + a, set by enqueue
+
+    // R key rows: row r is server srv(r) and applies at the rows ticks(r, fn) hands to fn, ascending; pairs r * A + a.
+    // Refuses 2^31 or more search records (`what` names the call).
+    template <class Srv, class Ticks>
+    int build(wva_handle* h, const char* what, int L, int S, int A, int R, Srv&& srv, Ticks&& ticks,
+              const float* itl, const float* ttft, const float* tps, const std::vector<int>& pairs,
+              const std::vector<int>& Ns) {
+        tab_of.assign((size_t)R * A, -1);
+        tab_entry.resize(pairs.size());
+        long long entries = 0;
+        for (size_t t = 0; t < pairs.size(); ++t) {
+            tab_of[pairs[t]] = (int)t;
+            tab_entry[t] = entries;
+            entries += Ns[t];
+        }
+        std::vector<int> n_load(R, 0);
+        for (int p : pairs) n_load[p / A]++;
+        // a row's keys are key_begin[r] .. key_begin[r + 1] - 1
+        std::vector<int> key_begin(R + 1, 0);
+        key.assign(2 * (size_t)L * S, -1);
+        std::vector<std::pair<uint64_t, size_t>> uses;  // (search << 32 | target bits, index into key)
+        for (int r = 0; r < R; ++r) {
+            key_begin[r] = (int)key_w.size();
+            if (!n_load[r]) continue;
+            const int s = srv(r);
+            uses.clear();
+            ticks(r, [&](int l) {
+                const size_t i = (size_t)l * S + s;
+                if (itl[i] < 0.0f || ttft[i] < 0.0f || tps[i] < 0.0f) return;
+                for (int w = 0; w < 2; ++w) {
+                    const float t = w == 0 ? ttft[i] : itl[i];
+                    if (!(t > 0.0f)) continue;
+                    uint32_t bits;
+                    memcpy(&bits, &t, 4);
+                    uses.emplace_back((uint64_t)w << 32 | bits, 2 * i + w);
+                }
+            });
+            std::sort(uses.begin(), uses.end());
+            for (size_t u = 0; u < uses.size(); ++u) {
+                if (u == 0 || uses[u].first != uses[u - 1].first) {
+                    const uint32_t bits = (uint32_t)uses[u].first;
+                    float t;
+                    memcpy(&t, &bits, 4);
+                    key_w.push_back((uint8_t)(uses[u].first >> 32));
+                    key_t.push_back(t);
+                }
+                key[uses[u].second] = (int)key_w.size() - 1;
+            }
+            // at most 2 * L * S keys in all; the search candidates are fewer than the records
+            if ((long long)key_w.size() * A >= (1ll << 31)) {
+                const std::string msg = std::string(what) + " with 2^31 or more search records in one call";
+                return h->fail(WVA_ERR_UNSUPPORTED, msg.c_str());
             }
         }
-        std::sort(uses.begin(), uses.end());
-        for (size_t u = 0; u < uses.size(); ++u) {
-            if (u == 0 || uses[u].first != uses[u - 1].first) {
-                const uint32_t bits = (uint32_t)uses[u].first;
-                float t;
-                memcpy(&t, &bits, 4);
-                key_w.push_back((uint8_t)(uses[u].first >> 32));
-                key_t.push_back(t);
-            }
-            key[uses[u].second] = (int)key_w.size() - 1;
-        }
-        // at most 2 * L * S keys in all; the search candidates are fewer than the records
-        if ((long long)key_w.size() * A >= (1ll << 31))
-            return h->fail(WVA_ERR_UNSUPPORTED, "SLO grid with 2^31 or more search records in one call");
+        key_begin[R] = (int)key_w.size();
+        // the load pairs in their order (descending N), each with its row's keys
+        for (int p : pairs)
+            for (int k = key_begin[p / A]; k < key_begin[p / A + 1]; ++k) sc.emplace_back(k, p);
+        return WVA_OK;
     }
-    key_begin[S] = (int)key_w.size();
-    const int n_keys = (int)key_w.size();
-    // search candidates (key, pair): the load pairs in their order (descending N), each with its server's keys
-    std::vector<std::pair<int, int>> sc;
-    for (int p : pairs)
-        for (int k = key_begin[p / A]; k < key_begin[p / A + 1]; ++k) sc.emplace_back(k, p);
-    const long long n = (long long)sc.size();
-    Cols c(16);
-    const size_t o_itl = c.take(4 * LS), o_ttft = c.take(4 * LS), o_tps = c.take(4 * LS), o_key = c.take(8 * LS);
-    const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_rec = c.take(4 * (size_t)n),
-                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_tgt = c.take(4 * (size_t)n),
-                 o_which = c.take((size_t)n);
-    int rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
+    void place(Cols& c, size_t LS) {
+        const size_t n = sc.size();
+        o_itl = c.take(4 * LS);
+        o_ttft = c.take(4 * LS);
+        o_tps = c.take(4 * LS);
+        o_key = c.take(8 * LS);
+        o_pair = c.take(4 * n);
+        o_N = c.take(4 * n);
+        o_rec = c.take(4 * n);
+        o_idx = c.take(4 * n);
+        o_off = c.take(8 * n);
+        o_tgt = c.take(4 * n);
+        o_which = c.take(n);
+    }
+    void write(char* p, size_t LS, const float* itl, const float* ttft, const float* tps, const std::vector<int>& Ns,
+               int A) const {
         if (LS) {
             memcpy(p + o_itl, itl, 4 * LS);
             memcpy(p + o_ttft, ttft, 4 * LS);
@@ -1173,7 +1197,55 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
             ((float*)(p + o_tgt))[j] = key_t[k];
             ((uint8_t*)(p + o_which))[j] = key_w[k];
         }
-    });
+    }
+    // d_slo for the records; call before enqueue
+    int reserve(wva_handle* h) {
+        const size_t n_srec = key_w.size() * (size_t)h->hf.A;
+        CK(h->d_slo.ensure(5 * n_srec + 16));
+        srch = AllocCols{};
+        srch.max_rate = (float*)h->d_slo.p;
+        srch.feasible = (uint8_t*)h->d_slo.p + 4 * n_srec;
+        return WVA_OK;
+    }
+    // phase 1: the searches on fleet f (whose tables are lg_tabs', uploaded at d)
+    int enqueue(wva_handle* h, const DevFleet& f, const char* d) const {
+        const PairTables& pt = h->lg_tabs;
+        SizeArgs g = size_args(f, pt, srch);
+        g.cand_pair = (const int*)(d + o_pair);
+        g.cand_N = (const int*)(d + o_N);
+        g.n_cand = (int)sc.size();
+        g.tab_off = (const long long*)(d + o_off);
+        g.place = CandPlace{(const int*)(d + o_idx), (const int*)(d + o_rec)};
+        return enqueue_candidates(h, g, pt.len_max, SIZE_SEARCH,
+                                  SearchCols{(const uint8_t*)(d + o_which), (const float*)(d + o_tgt)});
+    }
+};
+
+int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, const float* tps,
+                     const AllocCols& cand, const AllocCols& winners) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A;
+    const size_t LS = (size_t)L * S;
+    // the tail's candidates: every load pair (none without levels), descending N, one N-entry table each
+    std::vector<int> pairs, Ns;
+    if (L > 0) {
+        const int rc =
+            sorted_pairs(h, hf, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
+        if (rc) return rc;
+    }
+    // one key row per server, at every level
+    SloKeys sk;
+    int rc = sk.build(
+        h, "SLO grid", L, S, A, S, [](int s) { return s; },
+        [&](int, auto&& fn) {
+            for (int l = 0; l < L; ++l) fn(l);
+        },
+        itl, ttft, tps, pairs, Ns);
+    if (rc) return rc;
+    Cols c(16);
+    sk.place(c, LS);
+    rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c,
+                       [&](char* p) { sk.write(p, LS, itl, ttft, tps, Ns, A); });
     if (rc) return rc;
     const PairTables& pt = h->lg_tabs;
     const char* d = (const char*)pt.lists.p;
@@ -1183,21 +1255,11 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
     FbRun fb2;
     rc = prepare_tail(h, h->df, n_items, fb2);
     if (rc) return rc;
-    const size_t n_srec = (size_t)n_keys * A;
-    CK(h->d_slo.ensure(5 * n_srec + 16));
+    rc = sk.reserve(h);
+    if (rc) return rc;
     launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, L);
     // phase 1: the searches
-    AllocCols srch{};
-    srch.max_rate = (float*)h->d_slo.p;
-    srch.feasible = (uint8_t*)h->d_slo.p + 4 * n_srec;
-    SizeArgs g = size_args(h->df, pt, srch);
-    g.cand_pair = (const int*)(d + o_pair);
-    g.cand_N = (const int*)(d + o_N);
-    g.n_cand = (int)n;
-    g.tab_off = (const long long*)(d + o_off);
-    g.place = CandPlace{(const int*)(d + o_idx), (const int*)(d + o_rec)};
-    rc = enqueue_candidates(h, g, pt.len_max, SIZE_SEARCH,
-                            SearchCols{(const uint8_t*)(d + o_which), (const float*)(d + o_tgt)});
+    rc = sk.enqueue(h, h->df, d);
     if (rc) return rc;
     // phase 2: the tail per (load pair, level)
     if (n_items > 0) {
@@ -1207,11 +1269,11 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
         la.cand_N = pt.len();
         la.tab_off = pt.off();
         la.tab = (const double*)pt.tab.p;
-        la.slo_itl = (const float*)(d + o_itl);
-        la.slo_ttft = (const float*)(d + o_ttft);
-        la.slo_tps = (const float*)(d + o_tps);
-        la.key = (const int*)(d + o_key);
-        la.srch = srch;
+        la.slo_itl = (const float*)(d + sk.o_itl);
+        la.slo_ttft = (const float*)(d + sk.o_ttft);
+        la.slo_tps = (const float*)(d + sk.o_tps);
+        la.key = (const int*)(d + sk.o_key);
+        la.srch = sk.srch;
         la.n_cand = pt.n;
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
@@ -1449,6 +1511,121 @@ int enqueue_workload(wva_handle* h, int L, const float* rpm, const int32_t* in, 
     rc = enqueue_workload_tail(h, ls, g, d_rpm, L, cand);
     if (rc) return rc;
     enqueue_level_winners(h, cand, winners, L, trace);
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- SLO trace: the reconcile replayed over ticks of load and service-class targets (DESIGN.md §3.17) -------------
+// Size, lambda* and rateStar read the tokens but not the rate (§3.12), and each bisection reads only its own target
+// (§3.11), so a search is fixed by (server, accelerator, in, out, which search, target bits).  The key rows are the
+// workload trace's (server, in, out) rows under load, on a key fleet that keeps keepAccelerator only on the pinned
+// servers; SloKeys runs each distinct search of a key row once per load pair of the row.  The tail (slo_trace_kernel,
+// slo_trace_fallback) then runs per (key candidate, tick of its row) at f_t, the workload trace's trivial_kernel writes
+// the nil and zero-load records, and trace_kernel runs the chain.  The six row lists (NULL: the fleet's own column at
+// every tick) are in the call's upload image; lists, key fleet columns and tables go into lg_tabs, rebuilt on every
+// call.  cand ([L*S*A]) and winners ([L*S]) are device columns.
+int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out, const float* itl,
+                      const float* ttft, const float* tps, const AllocCols& cand, const AllocCols& winners) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A;
+    const size_t LS = (size_t)L * S;
+    std::vector<float> own_rpm, own_itl, own_ttft, own_tps;
+    std::vector<int32_t> own_in, own_out;
+    auto tile = [&](auto*& list, const auto& col, auto& own) {
+        if (list) return;
+        own.resize(LS);
+        for (int t = 0; t < L; ++t) std::copy(col.begin(), col.end(), own.begin() + (size_t)t * S);
+        list = own.data();
+    };
+    tile(rpm, hf.srv_arrival_rpm, own_rpm);
+    tile(in, hf.srv_in_tokens, own_in);
+    tile(out, hf.srv_out_tokens, own_out);
+    tile(itl, hf.srv_slo_itl, own_itl);
+    tile(ttft, hf.srv_slo_ttft, own_ttft);
+    tile(tps, hf.srv_slo_tps, own_tps);
+    // the key rows: at most L * S
+    TokenKeys tk;
+    token_keys(L, S, rpm, in, out, tk);
+    const int K = (int)tk.srv.size();
+    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
+    for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, tk.srv[k]);
+    // the tail's candidates: the key fleet's load pairs, descending N, one N-entry table each
+    const HostFleet& kh = kf.hf;
+    std::vector<int> pairs, Ns;
+    int rc = sorted_pairs(h, kh, [&](int k, int a) { return kh.pair_class(k, a, true) == PAIR_LOAD; }, pairs, Ns);
+    if (rc) return rc;
+    SloKeys sk;
+    rc = sk.build(
+        h, "SLO trace", L, S, A, K, [&](int k) { return tk.srv[k]; },
+        [&](int k, auto&& fn) {
+            for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j) fn(tk.lev[j]);
+        },
+        itl, ttft, tps, pairs, Ns);
+    if (rc) return rc;
+    Cols c(16);
+    kf.place(c);
+    tk.place(c, pairs.size());
+    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS), o_nokeep = c.take(S);
+    sk.place(c, LS);
+    rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
+        kf.write(p);
+        tk.write(p, pairs, A);
+        if (LS) {
+            memcpy(p + o_rpm, rpm, 4 * LS);
+            memcpy(p + o_in, in, 4 * LS);
+            memcpy(p + o_out, out, 4 * LS);
+        }
+        memset(p + o_nokeep, 0, S);
+        sk.write(p, LS, itl, ttft, tps, Ns, A);
+    });
+    if (rc) return rc;
+    const PairTables& pt = h->lg_tabs;
+    const char* d = (const char*)pt.lists.p;
+    const float* d_rpm = (const float*)(d + o_rpm);
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    const DevFleet kd = kf.view(h->df, d);
+    FbRun fb2;
+    rc = prepare_tail(h, kd, tk.n_items, fb2);
+    if (rc) return rc;
+    rc = sk.reserve(h);
+    if (rc) return rc;
+    // the workload trace's nil and zero-load records: no keepAccelerator mask (trace_kernel applies it), no target read
+    DevFleet tf = h->df;
+    tf.srv_keep_acc = (const uint8_t*)(d + o_nokeep);
+    launch_records(h, (long long)S * A * L, trivial_kernel, tf, cand, d_rpm, (const int*)(d + o_in),
+                   (const int*)(d + o_out), L);
+    // phase 1: the searches
+    rc = sk.enqueue(h, kd, d);
+    if (rc) return rc;
+    // phase 2: the tail per (key candidate, tick of its key row)
+    if (tk.n_items > 0) {
+        SloTraceArgs g{};
+        g.w = tk.args(d, S);
+        g.w.ld.f = kd;
+        g.w.ld.cand_pair = pt.pair();
+        g.w.ld.cand_N = pt.len();
+        g.w.ld.tab_off = pt.off();
+        g.w.ld.tab = (const double*)pt.tab.p;
+        g.w.ld.level_rpm = d_rpm;
+        g.w.ld.n_cand = pt.n;
+        g.w.ld.L = L;
+        g.w.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+        g.w.ld.cand = cand;
+        g.w.ld.fb = fb2.list;
+        g.f = h->df;
+        g.tick_in = (const int*)(d + o_in);
+        g.tick_out = (const int*)(d + o_out);
+        g.slo_itl = (const float*)(d + sk.o_itl);
+        g.slo_ttft = (const float*)(d + sk.o_ttft);
+        g.slo_tps = (const float*)(d + sk.o_tps);
+        g.key = (const int*)(d + sk.o_key);
+        g.srch = sk.srch;
+        g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
+        rc = launch_tail(h, slo_trace_kernel, slo_trace_fallback, g, ((long long)tk.n_items + 31) / 32, fb2);
+        if (rc) return rc;
+    }
+    enqueue_level_winners(h, cand, winners, L, true);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -2767,6 +2944,16 @@ int wva_workload_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, c
     return run_levels(h, fleet, n_ticks, "workload trace", null_rows, false, candidates, winners,
                       [&](const AllocCols& dc, const AllocCols& dw) {
                           return enqueue_workload(h, n_ticks, arrival_rpm, in_tokens, out_tokens, dc, dw, true);
+                      });
+}
+
+int wva_slo_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                  const int32_t* in_tokens, const int32_t* out_tokens, const float* slo_itl, const float* slo_ttft,
+                  const float* slo_tps, wva_allocs* candidates, wva_allocs* winners) {
+    return run_levels(h, fleet, n_ticks, "SLO trace", nullptr, false, candidates, winners,
+                      [&](const AllocCols& dc, const AllocCols& dw) {
+                          return enqueue_slo_trace(h, n_ticks, arrival_rpm, in_tokens, out_tokens, slo_itl, slo_ttft,
+                                                   slo_tps, dc, dw);
                       });
 }
 

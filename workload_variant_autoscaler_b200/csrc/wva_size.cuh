@@ -958,7 +958,46 @@ __device__ __forceinline__ DevFleet at_slo_level(const SloArgs& g, int l) {
     return fl;
 }
 
-// The SLO grid's item fb_pack(e, l): candidate e at level l; solve is Model.Solve for the two Analyze calls.
+// CreateAllocation of pair (s, a) of f (the fleet at one level or tick: its targets, rate and tokens) from phase 1's
+// search records: the sign gate, the level's two search records (key[kb + w] * A + a, where w = 0: TTFT, 1: ITL),
+// lambda* (min with the TPS rule), rateStar = Analyze(lambda*).Throughput, the replicas at f's totalRate and the
+// final Analyze.  tab is the pair's N-entry table; solve is Model.Solve for the two Analyze calls.  Returns false
+// when a solve bailed (out is then nil).  The SLO grid and the SLO trace share it.
+template <class Solve>
+__device__ __forceinline__ bool slo_tail(const DevFleet& f, int s, int a, int N, const double* tab, const int* key,
+                                         size_t kb, const AllocCols& srch, int* status, Solve&& solve, Cand& out) {
+    const int K = N + N * f.ratio;
+    out = cand_nil();
+    const SzStart b = sz_start(f, s, K, (float)tab[0], (float)tab[4 * (N - 1)]);
+    if (b.nil) return true;
+    float xs[2] = {b.lmax, b.lmax};  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
+    for (int w = 0; w < 2; ++w) {
+        const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
+        if (!(target > 0.0f)) continue;
+        const size_t k = (size_t)key[kb + w] * f.A + a;
+        const int st = srch.feasible[k];
+        if (st == SEARCH_FAIL) {
+            atomicExch(status, 1);
+            return true;
+        }
+        if (st == SEARCH_NIL) return true;
+        xs[w] = srch.max_rate[k];
+    }
+    float lam;
+    ModelStats st;
+    if (!sz_lambda(f, s, b.rmax, xs[0], xs[1], lam)) return true;
+    if (!solve(tab, N, K, lam, st)) return false;
+    const QParams q = qparams_of(f, s, a);
+    const float rate_star = metrics_from(q, N, st).throughput;
+    SzReplicas r;
+    if (!sz_replicas(f, s, a, b.rmax, rate_star, total_rate_of(f, s), r, lam)) return true;
+    if (!solve(tab, N, K, lam, st)) return false;
+    const Metrics m = metrics_from(q, N, st);
+    out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
+    return true;
+}
+
+// The SLO grid's item fb_pack(e, l): candidate e at level l.
 struct SloTail {
     const SloArgs& g;
     __device__ __forceinline__ size_t record(unsigned long long item) const {
@@ -968,37 +1007,9 @@ struct SloTail {
     __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
         const int e = (int)(item >> 32), l = (int)(unsigned)item;
         const DevFleet f = at_slo_level(g, l);
-        const int pair = g.cand_pair[e], s = pair / f.A, a = pair % f.A;
-        const int N = g.cand_N[e], K = N + N * f.ratio;
-        const double* tab = g.tab + 4 * g.tab_off[e];
-        out = cand_nil();
-        const SzStart b = sz_start(f, s, K, (float)tab[0], (float)tab[4 * (N - 1)]);
-        if (b.nil) return true;
-        float xs[2] = {b.lmax, b.lmax};  // lambdaStar when a target is disabled (queueanalyzer.go:205,218)
-        for (int w = 0; w < 2; ++w) {
-            const float target = w == 0 ? f.srv_slo_ttft[s] : f.srv_slo_itl[s];
-            if (!(target > 0.0f)) continue;
-            const size_t k = (size_t)g.key[((size_t)l * f.S + s) * 2 + w] * f.A + a;
-            const int st = g.srch.feasible[k];
-            if (st == SEARCH_FAIL) {
-                atomicExch(g.status, 1);
-                return true;
-            }
-            if (st == SEARCH_NIL) return true;
-            xs[w] = g.srch.max_rate[k];
-        }
-        float lam;
-        ModelStats st;
-        if (!sz_lambda(f, s, b.rmax, xs[0], xs[1], lam)) return true;
-        if (!solve(tab, N, K, lam, st)) return false;
-        const QParams q = qparams_of(f, s, a);
-        const float rate_star = metrics_from(q, N, st).throughput;
-        SzReplicas r;
-        if (!sz_replicas(f, s, a, b.rmax, rate_star, total_rate_of(f, s), r, lam)) return true;
-        if (!solve(tab, N, K, lam, st)) return false;
-        const Metrics m = metrics_from(q, N, st);
-        out = sz_cand(a, N, r, rate_star, m.ttft, m.avg_token_time, m.rho);
-        return true;
+        const int pair = g.cand_pair[e], s = pair / f.A;
+        return slo_tail(f, s, pair % f.A, g.cand_N[e], g.tab + 4 * g.tab_off[e], g.key, ((size_t)l * f.S + s) * 2,
+                        g.srch, g.status, solve, out);
     }
 };
 
@@ -1072,6 +1083,64 @@ __global__ void __launch_bounds__(256) workload_kernel(WorkloadArgs g) {
 
 // Stored-vector re-run of the items workload_kernel bailed on.
 __global__ void workload_fallback(WorkloadArgs g, FbRun r) { tail_rerun(r, g.ld.cand, WorkloadTail{g}); }
+
+// ---------------------------------------------------------------------------
+// The SLO trace's tail (DESIGN.md §3.17): the SLO grid's tail (slo_tail) on the workload trace's key fleet, whose row
+// k is server key_srv[k] at one (in_tokens, out_tokens) pair.  Phase 1 ran each distinct (key row, search, target
+// bits) once per load pair of the row, in search mode.  One lane per (key candidate, tick of its key row) item,
+// located as workload_item locates them, warps from a work counter.  Item (e, t) evaluates the pair at f_t, the
+// resident fleet with the rate, tokens and targets of row t (the key row's tokens are row t's), with the search
+// records of tick t.  Record (t * S + s) * A + a.
+// ---------------------------------------------------------------------------
+struct SloTraceArgs {
+    WorkloadArgs w;            // the key rows, their ticks and candidates, and the tables (w.ld, on the key fleet)
+    DevFleet f;                // the resident fleet
+    const int* tick_in;        // [L * S] row t of in_tokens and out_tokens (w.ld.level_rpm: of arrival_rpm)
+    const int* tick_out;
+    const float* slo_itl;      // [L * S] row t of the targets
+    const float* slo_ttft;
+    const float* slo_tps;
+    const int* key;            // [2 * L * S] the search key of (tick, server, search) (t * S + s) * 2 + which
+    AllocCols srch;            // search records by key * A + a (search_cand)
+    int* status;               // set where a consulted search did not terminate
+};
+
+// f_t: the resident fleet with row t of the six row lists.
+__device__ __forceinline__ DevFleet at_tick(const SloTraceArgs& g, int t) {
+    const size_t o = (size_t)t * g.f.S;
+    DevFleet ft = g.f;
+    ft.srv_arrival_rpm = g.w.ld.level_rpm + o;
+    ft.srv_in_tokens = g.tick_in + o;
+    ft.srv_out_tokens = g.tick_out + o;
+    ft.srv_slo_itl = g.slo_itl + o;
+    ft.srv_slo_ttft = g.slo_ttft + o;
+    ft.srv_slo_tps = g.slo_tps + o;
+    return ft;
+}
+
+// The SLO trace's item fb_pack(e, t): key candidate e at tick t, from workload_item.
+struct SloTraceTail {
+    const SloTraceArgs& g;
+    __device__ __forceinline__ size_t record(unsigned long long item) const { return WorkloadTail{g.w}.record(item); }
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        const int e = (int)(item >> 32), t = (int)(unsigned)item;
+        const int pair = g.w.ld.cand_pair[e], s = g.w.key_srv[pair / g.f.A];
+        return slo_tail(at_tick(g, t), s, pair % g.f.A, g.w.ld.cand_N[e], g.w.ld.tab + 4 * g.w.ld.tab_off[e], g.key,
+                        ((size_t)t * g.f.S + s) * 2, g.srch, g.status, solve, out);
+    }
+};
+
+__global__ void __launch_bounds__(256) slo_trace_kernel(SloTraceArgs g) {
+    for_each_warp_item(g.w.ld.counter, (unsigned)g.w.n_items, [&](unsigned i) {
+        int e, t;
+        workload_item(g.w, (int)i, e, t);
+        tail_item(g.w.ld.fb, g.w.ld.cand, fb_pack(e, t), SloTraceTail{g});
+    });
+}
+
+// Stored-vector re-run of the items slo_trace_kernel bailed on.
+__global__ void slo_trace_fallback(SloTraceArgs g, FbRun r) { tail_rerun(r, g.w.ld.cand, SloTraceTail{g}); }
 
 // ---------------------------------------------------------------------------
 // Load intervals (DESIGN.md §3.10): per server, the float32 arrival rates in [lo, hi] at which the load grid's

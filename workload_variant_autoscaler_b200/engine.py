@@ -323,6 +323,26 @@ class Engine:
         row_ptrs = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in load] + [C.byref(rc_)]
         return self._level_call(self._L.wva_profile_trace, fleet, L, row_ptrs, want_candidates, out)
 
+    def slo_trace(self, fleet: Fleet, arrival_rpm=None, in_tokens=None, out_tokens=None, *, slo_itl=None,
+                  slo_ttft=None, slo_tps=None, want_candidates: bool = False, out: Allocs | None = None):
+        """The reference's reconcile replayed over ticks of load (``arrival_rpm`` req/min, ``in_tokens``,
+        ``out_tokens``) and service-class targets (``slo_itl``, ``slo_ttft``, ``slo_tps``, in the fleet columns'
+        units), each of shape (L, S): ``Server.Calculate``, ``SolveUnlimited`` and ``Server.ApplyDesiredAlloc`` per
+        tick -> (candidates [L*S*A] | None, winners [L*S]), both tick-major.
+
+        Tick ``t`` is ``solve`` in unlimited mode on the fleet with every given column = row ``t`` and the current
+        allocation advanced by ``fleet.apply_winners`` through ticks 0..t-1; each distinct (server, tokens, search,
+        target) is searched once (see ``wva_slo_trace`` in include/wva_b200.h).  A list of ``None`` is the fleet's
+        own column at every tick; at least one must be given, and L is their common row count.  ``out``: an
+        ``Allocs`` of ``L * S`` records to write the winners into."""
+        names = ("arrival_rpm", "in_tokens", "out_tokens", "slo_itl", "slo_ttft", "slo_tps")
+        rows, L = _row_lists(fleet, dict(zip(names, (arrival_rpm, in_tokens, out_tokens, slo_itl, slo_ttft,
+                                                     slo_tps))))
+        if L is None:
+            raise ValueError("slo_trace needs at least one row list")
+        row_ptrs = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in names]
+        return self._level_call(self._L.wva_slo_trace, fleet, L, row_ptrs, want_candidates, out)
+
     def load_intervals(self, fleet: Fleet, rpm_lo, rpm_hi, max_per_server: int):
         """Where each server's ``load_grid`` winner changes its decision in ``[rpm_lo[s], rpm_hi[s]]`` (req/min)
         -> (count [S], truncated [S], start_rpm (S, M), records: ``Allocs`` of S * M).
