@@ -72,20 +72,32 @@ struct PinBuf {
 inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
 // Columns packed into one buffer, each starting on an `align`-byte boundary (an empty column still gets an
-// address of its own).  The offsets take() returns hand out the device pointers, and take() records where a
-// column with a host destination lies, so the layout and the copy-back cannot disagree.
+// address of its own).  The offsets take() and put() return hand out the device pointers.  take() records where a
+// column with a host destination lies, so the layout and the copy-back cannot disagree.  put() lays out a column
+// whose host bytes are src, and upload_tables copies every such column into the host image before its fill runs:
+// src must stay alive, and must not be resized, until upload_tables returns.
 struct Cols {
     struct Col {
         size_t off, bytes;
         void* dst;
     };
+    struct Src {
+        size_t off, bytes;
+        const void* src;
+    };
     size_t align, bytes = 0;
     std::vector<Col> out;  // the columns that have a host destination
+    std::vector<Src> in;   // the columns copied verbatim from host memory
     explicit Cols(size_t a) : align(a) {}
     size_t take(size_t n, void* dst = nullptr) {
         const size_t at = bytes;
         if (dst) out.push_back({at, n, dst});
         bytes = align_up(at + std::max<size_t>(n, 1), align);
+        return at;
+    }
+    size_t put(const void* src, size_t n) {
+        const size_t at = take(n);
+        if (n) in.push_back({at, n, src});
         return at;
     }
     // device buffer `dev` -> the destinations, enqueued on `st`
@@ -483,8 +495,9 @@ int sorted_pairs(wva_handle* h, const HostFleet& hf, Keep keep, std::vector<int>
 
 // ---- shared service-rate tables ---------------------------------------------
 // Upload the lists of one set of tables: table t is pair[t]'s first len[t] service rates, in the caller's order,
-// at entry offset len[0] + .. + len[t-1].  The columns the caller laid out in `c` come first in the same image and
-// fill(host image) writes them; the table lists follow.  One H2D copy, then tab (and ls when with_ls) are sized.
+// at entry offset len[0] + .. + len[t-1].  The columns the caller laid out in `c` come first in the same image:
+// those put() there are copied in, then fill(host image) writes the rest; the table lists follow.  One H2D copy,
+// then tab (and ls when with_ls) are sized.
 // The instance is left keyed kUncached; a path that caches sets the key once its tables are built.
 //
 // Every entry point that takes a fleet calls upload_fleet, which bumps epoch_tokens, so only the resident calls can
@@ -518,6 +531,7 @@ int upload_tables(wva_handle* h, PairTables& pt, const std::vector<int>& pair, c
         entries += len[t];
         pt.len_max = std::max(pt.len_max, len[t]);
     }
+    for (const Cols::Src& s : c.in) memcpy(p + s.off, s.src, s.bytes);
     fill(p);
     CK(pt.lists.ensure(c.bytes));
     // pageable source: cudaMemcpyAsync has consumed it by the time it returns
@@ -859,7 +873,7 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return batch[x % B] > batch[y % B]; });
     Cols c(16);
     const size_t o_pair = c.take(4 * (size_t)n), o_N = c.take(4 * (size_t)n), o_rec = c.take(4 * (size_t)n),
-                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_bl = c.take(4 * (size_t)B);
+                 o_idx = c.take(4 * (size_t)n), o_off = c.take(8 * (size_t)n), o_bl = c.put(batch, 4 * (size_t)B);
     int rc = upload_tables(h, pt, tab_pair, std::vector<int>(n_tab, Bmax), true, c, [&](char* p) {
         for (int j = 0; j < n; ++j) {
             const int t = order[j] / B, bi = order[j] % B;
@@ -869,7 +883,6 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
             ((int*)(p + o_idx))[j] = t;
             ((long long*)(p + o_off))[j] = (long long)t * Bmax;
         }
-        if (B) memcpy(p + o_bl, batch, 4 * (size_t)B);
     });
     if (rc) return rc;
     rc = build_tables(h, h->df, pt);
@@ -906,7 +919,6 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
 // for the device image f of the same fleet and sizes fallback list 1 for the caller's tail (prepare_tail, which the
 // SLO grid shares), and enqueues phase 1.
 struct LoadStar {
-    int n = 0;           // candidates
     AllocCols star{};    // rateStar mode's records by pair id: feasible and max_rate = rateStar
     FbRun fb2{};         // the tail's fallback list
     SizeArgs g{};        // phase 1's fleet, candidates and tables
@@ -937,7 +949,6 @@ int enqueue_load_star(wva_handle* h, const HostFleet& hf, const DevFleet& f, lon
     ls.star.feasible = (uint8_t*)h->d_lg_star.p + 4 * n_pairs;
     const int rc = prepare_tail(h, f, fb2_cap, ls.fb2);
     if (rc) return rc;
-    ls.n = pt.n;
     ls.g = size_args(f, pt, ls.star);
     return enqueue_candidates(h, ls.g, pt.len_max, SIZE_STAR);
 }
@@ -954,20 +965,72 @@ void enqueue_level_winners(wva_handle* h, const AllocCols& cand, const AllocCols
             h->df, cand, winners, L);
     h->launches++;
 }
+// A tail's fleet f, and its candidates and tables: those of pt, one per table.
+template <class Args>
+void set_tables(Args& g, const DevFleet& f, const PairTables& pt) {
+    g.f = f;
+    g.cand_pair = pt.pair();
+    g.cand_N = pt.len();
+    g.tab_off = pt.off();
+    g.tab = (const double*)pt.tab.p;
+    g.n_cand = pt.n;
+}
 // The tail's view of phase 1: fleet, candidates, tables and rateStar records (the level list is the caller's).
-LoadArgs load_args(const LoadStar& ls) {
+LoadArgs load_args(wva_handle* h, const LoadStar& ls) {
     LoadArgs la{};
-    la.f = ls.g.f;
-    la.cand_pair = ls.g.cand_pair;
-    la.cand_N = ls.g.cand_N;
-    la.tab_off = ls.g.tab_off;
-    la.tab = ls.g.tab;
+    set_tables(la, ls.g.f, h->lg_tabs);
     la.star_ok = ls.star.feasible;
     la.rate_star = ls.star.max_rate;
-    la.n_cand = ls.n;
     la.fb = ls.fb2.list;
     return la;
 }
+
+// One call's [L*S] lists of the server columns that a grid or trace replaces by row: arrival_rpm, in / out tokens
+// and the ITL / TTFT / TPS targets.  The put_* calls put the lists the call reads into its upload image c, a NULL
+// list tiled from the resident column (the calls that refuse NULL lists do so in run_levels).  After the upload, a
+// list's dev() is its device pointer (NULL: not put) and load() the records' load rows.  The tiled lists live
+// here, so a RowLists outlives the upload.
+struct RowLists {
+    template <class T>
+    struct List {
+        const T* host = nullptr;  // the caller's list or own
+        size_t off = 0;
+        bool placed = false;
+        std::vector<T> own;
+        const T* dev(const char* d) const { return placed ? (const T*)(d + off) : nullptr; }
+    };
+    const HostFleet& hf;
+    int L;
+    Cols& c;
+    List<float> rpm, itl, ttft, tps;
+    List<int32_t> in, out;
+
+    void put_rpm(const float* r) { put(rpm, r, hf.srv_arrival_rpm); }
+    void put_tokens(const int32_t* i, const int32_t* o) {
+        put(in, i, hf.srv_in_tokens);
+        put(out, o, hf.srv_out_tokens);
+    }
+    void put_targets(const float* i, const float* t, const float* p) {
+        put(itl, i, hf.srv_slo_itl);
+        put(ttft, t, hf.srv_slo_ttft);
+        put(tps, p, hf.srv_slo_tps);
+    }
+    LoadRows load(const char* d) const { return LoadRows{rpm.dev(d), in.dev(d), out.dev(d)}; }
+
+  private:
+    template <class T>
+    void put(List<T>& r, const T* list, const std::vector<T>& col) {
+        const size_t S = col.size();
+        if (!list) {
+            r.own.resize((size_t)L * S);
+            for (int l = 0; l < L; ++l) std::copy(col.begin(), col.end(), r.own.begin() + (size_t)l * S);
+            list = r.own.data();
+        }
+        r.host = list;
+        r.off = c.put(list, sizeof(T) * (size_t)L * S);
+        r.placed = true;
+    }
+};
 
 // Phase 2 (load_kernel, load_fallback) is the tail per (candidate, level).  rpm [L*S] is the caller's level list;
 // cand ([L*S*A]) and winners ([L*S]) are device columns.
@@ -979,23 +1042,22 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
         for (int s = 0; s < S; ++s) loaded[s] |= !(rpm[(size_t)l * S + s] < 0.0f) && rpm[(size_t)l * S + s] != 0.0f;
     std::vector<int> pairs;
     Cols c(16);
-    const size_t o_rpm = c.take(4 * (size_t)L * S);
-    int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
-        if ((size_t)L * S) memcpy(p + o_rpm, rpm, 4 * (size_t)L * S);
-    });
+    RowLists lists{hf, L, c};
+    lists.put_rpm(rpm);
+    int rc = prepare_load_star(h, hf, loaded, pairs, c, [](char*) {});
     if (rc) return rc;
     const int n = (int)pairs.size();
     const long long n_items = (long long)n * L;
-    const float* d_rpm = (const float*)((const char*)h->lg_tabs.lists.p + o_rpm);
+    const char* d = (const char*)h->lg_tabs.lists.p;
     rc = ensure_ctrl(h);
     if (rc) return rc;
-    launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, d_rpm, L);
+    launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, lists.load(d), L);
     LoadStar ls;
     rc = enqueue_load_star(h, hf, h->df, n_items, ls);
     if (rc) return rc;
     if (n > 0 && L > 0) {
-        LoadArgs la = load_args(ls);
-        la.level_rpm = d_rpm;
+        LoadArgs la = load_args(h, ls);
+        la.level_rpm = lists.rpm.dev(d);
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
         la.cand = cand;
@@ -1025,12 +1087,8 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     for (int s = 0; s < S; ++s) loaded[s] = hi[s] > 0.0f;
     std::vector<int> pairs;
     Cols c(16);
-    const size_t o_lo = c.take(4 * (size_t)S), o_hi = c.take(4 * (size_t)S), o_cop = c.take(4 * (size_t)S * A);
+    const size_t o_lo = c.put(lo, 4 * (size_t)S), o_hi = c.put(hi, 4 * (size_t)S), o_cop = c.take(4 * (size_t)S * A);
     int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
-        if (S) {
-            memcpy(p + o_lo, lo, 4 * (size_t)S);
-            memcpy(p + o_hi, hi, 4 * (size_t)S);
-        }
         int* cop = (int*)(p + o_cop);
         std::fill(cop, cop + (size_t)S * A, -1);
         for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
@@ -1048,7 +1106,7 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     if (S == 0) return WVA_OK;
     const char* dl = (const char*)h->lg_tabs.lists.p;
     IntervalArgs g{};
-    g.ld = load_args(ls);
+    g.ld = load_args(h, ls);
     g.cand_of_pair = (const int*)(dl + o_cop);
     g.lo = (const float*)(dl + o_lo);
     g.hi = (const float*)(dl + o_hi);
@@ -1092,8 +1150,8 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
 // key rows are the resident servers, each at every level; the trace's are the workload trace's token keys, each at
 // the ticks that use its tokens under load.  build() lists, per key row with load pairs, its distinct (search, target
 // bits) in that order and crosses them with the row's load pairs (the tail's candidates `pairs`, descending N, one
-// N-entry table each): the search candidates, still in descending N.  The target row lists and the key of each (row,
-// server, search) travel in the call's upload image (place, write); enqueue() runs the searches in search mode over
+// N-entry table each): the search candidates, still in descending N.  The key of each (row, server, search) and the
+// search candidates travel in the call's upload image (place, write); enqueue() runs the searches in search mode over
 // the tables of lg_tabs, records in d_slo.
 struct SloKeys {
     std::vector<int> key;        // [2 * L * S] key of (row l, server s, search w) at (l * S + s) * 2 + w; -1: none
@@ -1102,8 +1160,7 @@ struct SloKeys {
     std::vector<std::pair<int, int>> sc;  // the search candidates (key, pair)
     std::vector<int> tab_of;              // a pair's table index
     std::vector<long long> tab_entry;     // a table's first entry
-    size_t o_itl = 0, o_ttft = 0, o_tps = 0, o_key = 0, o_pair = 0, o_N = 0, o_rec = 0, o_idx = 0, o_off = 0,
-           o_tgt = 0, o_which = 0;
+    size_t o_key = 0, o_pair = 0, o_N = 0, o_rec = 0, o_idx = 0, o_off = 0, o_tgt = 0, o_which = 0;
     AllocCols srch{};  // the search records by key * A + a, set by enqueue
 
     // R key rows: row r is server srv(r) and applies at the rows ticks(r, fn) hands to fn, ascending; pairs r * A + a.
@@ -1165,12 +1222,9 @@ struct SloKeys {
             for (int k = key_begin[p / A]; k < key_begin[p / A + 1]; ++k) sc.emplace_back(k, p);
         return WVA_OK;
     }
-    void place(Cols& c, size_t LS) {
+    void place(Cols& c) {
         const size_t n = sc.size();
-        o_itl = c.take(4 * LS);
-        o_ttft = c.take(4 * LS);
-        o_tps = c.take(4 * LS);
-        o_key = c.take(8 * LS);
+        o_key = c.put(key.data(), 4 * key.size());
         o_pair = c.take(4 * n);
         o_N = c.take(4 * n);
         o_rec = c.take(4 * n);
@@ -1179,14 +1233,7 @@ struct SloKeys {
         o_tgt = c.take(4 * n);
         o_which = c.take(n);
     }
-    void write(char* p, size_t LS, const float* itl, const float* ttft, const float* tps, const std::vector<int>& Ns,
-               int A) const {
-        if (LS) {
-            memcpy(p + o_itl, itl, 4 * LS);
-            memcpy(p + o_ttft, ttft, 4 * LS);
-            memcpy(p + o_tps, tps, 4 * LS);
-            memcpy(p + o_key, key.data(), 8 * LS);
-        }
+    void write(char* p, const std::vector<int>& Ns, int A) const {
         for (size_t j = 0; j < sc.size(); ++j) {
             const int k = sc[j].first, pair = sc[j].second, a = pair % A, t = tab_of[pair];
             ((int*)(p + o_pair))[j] = pair;
@@ -1225,7 +1272,6 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
                      const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
-    const size_t LS = (size_t)L * S;
     // the tail's candidates: every load pair (none without levels), descending N, one N-entry table each
     std::vector<int> pairs, Ns;
     if (L > 0) {
@@ -1233,6 +1279,9 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
             sorted_pairs(h, hf, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
         if (rc) return rc;
     }
+    Cols c(16);
+    RowLists lists{hf, L, c};
+    lists.put_targets(itl, ttft, tps);
     // one key row per server, at every level
     SloKeys sk;
     int rc = sk.build(
@@ -1242,10 +1291,8 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
         },
         itl, ttft, tps, pairs, Ns);
     if (rc) return rc;
-    Cols c(16);
-    sk.place(c, LS);
-    rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c,
-                       [&](char* p) { sk.write(p, LS, itl, ttft, tps, Ns, A); });
+    sk.place(c);
+    rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) { sk.write(p, Ns, A); });
     if (rc) return rc;
     const PairTables& pt = h->lg_tabs;
     const char* d = (const char*)pt.lists.p;
@@ -1257,24 +1304,19 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
     if (rc) return rc;
     rc = sk.reserve(h);
     if (rc) return rc;
-    launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, L);
+    launch_records(h, (long long)S * A * L, trivial_kernel, h->df, cand, lists.load(d), L);
     // phase 1: the searches
     rc = sk.enqueue(h, h->df, d);
     if (rc) return rc;
     // phase 2: the tail per (load pair, level)
     if (n_items > 0) {
         SloArgs la{};
-        la.f = h->df;
-        la.cand_pair = pt.pair();
-        la.cand_N = pt.len();
-        la.tab_off = pt.off();
-        la.tab = (const double*)pt.tab.p;
-        la.slo_itl = (const float*)(d + sk.o_itl);
-        la.slo_ttft = (const float*)(d + sk.o_ttft);
-        la.slo_tps = (const float*)(d + sk.o_tps);
+        set_tables(la, h->df, pt);
+        la.slo_itl = lists.itl.dev(d);
+        la.slo_ttft = lists.ttft.dev(d);
+        la.slo_tps = lists.tps.dev(d);
         la.key = (const int*)(d + sk.o_key);
         la.srch = sk.srch;
-        la.n_cand = pt.n;
         la.L = L;
         la.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
         la.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
@@ -1302,7 +1344,7 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
 
 // The fleet the workload grid sizes (DESIGN.md §3.12): row k is server srv[k] of the resident fleet at the key's
 // tokens, with a positive rate (phase 1 reads no rate; the tail reads the level's).  The A, T and M columns are the
-// resident fleet's.  On the device the server columns lie in an upload image of the caller's (place, write), and
+// resident fleet's.  On the device the server columns lie in an upload image of the caller's (place), and
 // view() points a copy of the resident DevFleet at them, so the resident arena is never written.  The profile grid
 // also gives the key fleet its own models (own_ma): M and the perf_* columns are then the key fleet's.
 struct KeyFleet {
@@ -1330,17 +1372,11 @@ struct KeyFleet {
         hf.srv_out_tokens = out;
     }
     void place(Cols& c) {
-#define KEY_PLACE(abi, name, type, len) \
-    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) off.name = c.take(sizeof(type) * hf.name.size());
+#define KEY_PLACE(abi, name, type, len)                            \
+    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) \
+        off.name = c.put(hf.name.data(), sizeof(type) * hf.name.size());
         WVA_FLEET_COLUMNS(KEY_PLACE)
 #undef KEY_PLACE
-    }
-    void write(char* p) const {
-#define KEY_WRITE(abi, name, type, len)                                              \
-    if ((WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) && !hf.name.empty()) \
-        memcpy(p + off.name, hf.name.data(), sizeof(type) * hf.name.size());
-        WVA_FLEET_COLUMNS(KEY_WRITE)
-#undef KEY_WRITE
     }
     DevFleet view(DevFleet f, const char* d) const {
         f.S = hf.S;
@@ -1353,13 +1389,18 @@ struct KeyFleet {
     }
 };
 
-// A server whose accelerator no tick of a workload trace can change (DESIGN.md §3.13): with keepAccelerator and a
-// current accelerator other than "" only that accelerator is a candidate, and its load and zero-load candidates
-// carry it unless min_replicas is 0 (a zero-load candidate is then ""); an unknown one has no candidate at all.
-// A nil winner keeps the current allocation, so neither ever moves.
-bool trace_pinned(const HostFleet& hf, int s) {
-    const int cur = hf.srv_cur_acc[s];
-    return hf.srv_keep_acc[s] && cur != WVA_ACC_NONE && (cur == WVA_ACC_UNKNOWN || hf.srv_min_replicas[s] != 0);
+// The servers whose accelerator no tick of a trace can change (DESIGN.md §3.13), as flags [S]: with keepAccelerator
+// and a current accelerator other than "" only that accelerator is a candidate, and its load and zero-load
+// candidates carry it unless min_replicas is 0 (a zero-load candidate is then ""); an unknown one has no candidate at
+// all.  A nil winner keeps the current allocation, so neither ever moves.  A trace's records carry keepAccelerator on
+// these servers only: trace_kernel applies the rest of the mask tick by tick.
+std::vector<uint8_t> trace_pinned(const HostFleet& hf) {
+    std::vector<uint8_t> pin(hf.S);
+    for (int s = 0; s < hf.S; ++s) {
+        const int cur = hf.srv_cur_acc[s];
+        pin[s] = hf.srv_keep_acc[s] && cur != WVA_ACC_NONE && (cur == WVA_ACC_UNKNOWN || hf.srv_min_replicas[s] != 0);
+    }
+    return pin;
 }
 
 // The workload grid's tail (workload_kernel, then workload_fallback) after phase 1 (ls): g's key and level lists and
@@ -1368,7 +1409,7 @@ bool trace_pinned(const HostFleet& hf, int s) {
 int enqueue_workload_tail(wva_handle* h, const LoadStar& ls, WorkloadArgs& g, const float* level_rpm, int L,
                           const AllocCols& cand) {
     if (g.n_items <= 0) return WVA_OK;
-    g.ld = load_args(ls);
+    g.ld = load_args(h, ls);
     g.ld.level_rpm = level_rpm;
     g.ld.L = L;
     g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
@@ -1412,18 +1453,15 @@ struct TokenKeys {
         lev.push_back(l);
         lev_off.back()++;
     }
-    // room for the key rows and the item offsets of up to n_cand candidates
+    // the key rows, and room for the item offsets of up to n_cand candidates
     void place(Cols& c, size_t n_cand) {
-        o_srv = c.take(4 * srv.size());
-        o_loff = c.take(4 * lev_off.size());
-        o_lev = c.take(4 * lev.size());
+        o_srv = c.put(srv.data(), 4 * srv.size());
+        o_loff = c.put(lev_off.data(), 4 * lev_off.size());
+        o_lev = c.put(lev.data(), 4 * lev.size());
         o_item = c.take(4 * (n_cand + 1));
     }
-    // The key rows, and candidate j's items: one per level of its key row pairs[j] / A.
+    // candidate j's items: one per level of its key row pairs[j] / A
     void write(char* p, const std::vector<int>& pairs, int A) {
-        if (!srv.empty()) memcpy(p + o_srv, srv.data(), 4 * srv.size());
-        memcpy(p + o_loff, lev_off.data(), 4 * lev_off.size());
-        if (!lev.empty()) memcpy(p + o_lev, lev.data(), 4 * lev.size());
         int* item = (int*)(p + o_item);
         item[0] = 0;
         for (size_t j = 0; j < pairs.size(); ++j) {
@@ -1444,14 +1482,21 @@ struct TokenKeys {
         return g;
     }
 };
-// The workload grid's keys (DESIGN.md §3.12): per server, its distinct (in, out) under load, ascending.
-void token_keys(int L, int S, const float* rpm, const int32_t* in, const int32_t* out, TokenKeys& tk) {
+// The workload grid's keys (DESIGN.md §3.12) of the rows rpm / in / out into tk: per server, its distinct (in, out)
+// under load, ascending.  Returns their key fleet, which with pin (a trace's trace_pinned flags) keeps
+// keepAccelerator on the pinned servers only, so that phase 1 sizes their current accelerator alone.
+KeyFleet workload_keys(const HostFleet& hf, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                       const uint8_t* pin, TokenKeys& tk) {
     std::vector<std::pair<uint64_t, int>> uses;
-    for (int s = 0; s < S; ++s)
-        load_groups(L, S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
+    for (int s = 0; s < hf.S; ++s)
+        load_groups(L, hf.S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
             tk.add(s, ki, ko);
             for (size_t u = u0; u < u1; ++u) tk.add_level(uses[u].second);
         });
+    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
+    if (pin)
+        for (size_t k = 0; k < tk.srv.size(); ++k) kf.hf.srv_keep_acc[k] = pin[tk.srv[k]];
+    return kf;
 }
 
 // QueueAnalyzer.Size, lambda* and rateStar read a server's tokens but not its rate (DESIGN.md §3.12), so phase 1
@@ -1462,53 +1507,39 @@ void token_keys(int L, int S, const float* rpm, const int32_t* in, const int32_t
 // winner of every level.  rpm / in / out [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device
 // columns.
 //
-// With `trace` (the workload trace, DESIGN.md §3.13) the records are CreateAllocation without the keepAccelerator
-// mask, which trace_kernel applies tick by tick: trivial_kernel sees an all-zero keep column, and the key fleet keeps
-// keepAccelerator only on the pinned servers, so that phase 1 sizes their current accelerator alone.  trace_kernel's
-// chain then picks the winners: one thread per server applies the mask against its current allocation, picks the
-// winner and advances.
+// With `trace` (the workload trace, DESIGN.md §3.13) the records carry keepAccelerator on the pinned servers only
+// (trace_pinned), in trivial_kernel and in the key fleet alike.  trace_kernel's chain then picks the winners: one
+// thread per server applies the mask against its current allocation, picks the winner and advances.
 int enqueue_workload(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
                      const AllocCols& cand, const AllocCols& winners, bool trace) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
-    const size_t LS = (size_t)L * S;
+    Cols c(16);
+    RowLists lists{hf, L, c};
+    lists.put_rpm(rpm);
+    lists.put_tokens(in, out);
+    const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
+    const size_t o_pin = trace ? c.put(pin.data(), S) : 0;
     // the keys: at most L * S, so fewer than 2^31 key candidates
     TokenKeys tk;
-    token_keys(L, S, rpm, in, out, tk);
+    KeyFleet kf = workload_keys(hf, L, rpm, in, out, trace ? pin.data() : nullptr, tk);
     const int K = (int)tk.srv.size();
-    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
-    if (trace)
-        for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, tk.srv[k]);
-    Cols c(16);
     kf.place(c);
     tk.place(c, (size_t)K * A);
-    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS);
-    const size_t o_nokeep = trace ? c.take(S) : 0;  // the trace's all-zero keep column
     std::vector<int> pairs;
-    int rc = prepare_load_star(h, kf.hf, std::vector<char>(K, 1), pairs, c, [&](char* p) {
-        kf.write(p);
-        tk.write(p, pairs, A);
-        if (LS) {
-            memcpy(p + o_rpm, rpm, 4 * LS);
-            memcpy(p + o_in, in, 4 * LS);
-            memcpy(p + o_out, out, 4 * LS);
-        }
-        if (trace) memset(p + o_nokeep, 0, S);
-    });
+    int rc = prepare_load_star(h, kf.hf, std::vector<char>(K, 1), pairs, c, [&](char* p) { tk.write(p, pairs, A); });
     if (rc) return rc;
     const char* d = (const char*)h->lg_tabs.lists.p;
-    const float* d_rpm = (const float*)(d + o_rpm);
     rc = ensure_ctrl(h);
     if (rc) return rc;
     DevFleet tf = h->df;
-    if (trace) tf.srv_keep_acc = (const uint8_t*)(d + o_nokeep);
-    launch_records(h, (long long)S * A * L, trivial_kernel, tf, cand, d_rpm, (const int*)(d + o_in),
-                   (const int*)(d + o_out), L);
+    if (trace) tf.srv_keep_acc = (const uint8_t*)(d + o_pin);
+    launch_records(h, (long long)S * A * L, trivial_kernel, tf, cand, lists.load(d), L);
     LoadStar ls;
     rc = enqueue_load_star(h, kf.hf, kf.view(h->df, d), tk.n_items, ls);
     if (rc) return rc;
     WorkloadArgs g = tk.args(d, S);
-    rc = enqueue_workload_tail(h, ls, g, d_rpm, L, cand);
+    rc = enqueue_workload_tail(h, ls, g, lists.rpm.dev(d), L, cand);
     if (rc) return rc;
     enqueue_level_winners(h, cand, winners, L, trace);
     CK(cudaGetLastError());
@@ -1528,27 +1559,17 @@ int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in,
                       const float* ttft, const float* tps, const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
-    const size_t LS = (size_t)L * S;
-    std::vector<float> own_rpm, own_itl, own_ttft, own_tps;
-    std::vector<int32_t> own_in, own_out;
-    auto tile = [&](auto*& list, const auto& col, auto& own) {
-        if (list) return;
-        own.resize(LS);
-        for (int t = 0; t < L; ++t) std::copy(col.begin(), col.end(), own.begin() + (size_t)t * S);
-        list = own.data();
-    };
-    tile(rpm, hf.srv_arrival_rpm, own_rpm);
-    tile(in, hf.srv_in_tokens, own_in);
-    tile(out, hf.srv_out_tokens, own_out);
-    tile(itl, hf.srv_slo_itl, own_itl);
-    tile(ttft, hf.srv_slo_ttft, own_ttft);
-    tile(tps, hf.srv_slo_tps, own_tps);
+    Cols c(16);
+    RowLists lists{hf, L, c};
+    lists.put_rpm(rpm);
+    lists.put_tokens(in, out);
+    lists.put_targets(itl, ttft, tps);
+    const std::vector<uint8_t> pin = trace_pinned(hf);
+    const size_t o_pin = c.put(pin.data(), S);
     // the key rows: at most L * S
     TokenKeys tk;
-    token_keys(L, S, rpm, in, out, tk);
+    KeyFleet kf = workload_keys(hf, L, lists.rpm.host, lists.in.host, lists.out.host, pin.data(), tk);
     const int K = (int)tk.srv.size();
-    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
-    for (int k = 0; k < K; ++k) kf.hf.srv_keep_acc[k] = trace_pinned(hf, tk.srv[k]);
     // the tail's candidates: the key fleet's load pairs, descending N, one N-entry table each
     const HostFleet& kh = kf.hf;
     std::vector<int> pairs, Ns;
@@ -1560,28 +1581,18 @@ int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in,
         [&](int k, auto&& fn) {
             for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j) fn(tk.lev[j]);
         },
-        itl, ttft, tps, pairs, Ns);
+        lists.itl.host, lists.ttft.host, lists.tps.host, pairs, Ns);
     if (rc) return rc;
-    Cols c(16);
     kf.place(c);
     tk.place(c, pairs.size());
-    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS), o_nokeep = c.take(S);
-    sk.place(c, LS);
+    sk.place(c);
     rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
-        kf.write(p);
         tk.write(p, pairs, A);
-        if (LS) {
-            memcpy(p + o_rpm, rpm, 4 * LS);
-            memcpy(p + o_in, in, 4 * LS);
-            memcpy(p + o_out, out, 4 * LS);
-        }
-        memset(p + o_nokeep, 0, S);
-        sk.write(p, LS, itl, ttft, tps, Ns, A);
+        sk.write(p, Ns, A);
     });
     if (rc) return rc;
     const PairTables& pt = h->lg_tabs;
     const char* d = (const char*)pt.lists.p;
-    const float* d_rpm = (const float*)(d + o_rpm);
     rc = ensure_ctrl(h);
     if (rc) return rc;
     const DevFleet kd = kf.view(h->df, d);
@@ -1590,11 +1601,10 @@ int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in,
     if (rc) return rc;
     rc = sk.reserve(h);
     if (rc) return rc;
-    // the workload trace's nil and zero-load records: no keepAccelerator mask (trace_kernel applies it), no target read
+    // the workload trace's nil and zero-load records: keepAccelerator on the pinned servers only, no target read
     DevFleet tf = h->df;
-    tf.srv_keep_acc = (const uint8_t*)(d + o_nokeep);
-    launch_records(h, (long long)S * A * L, trivial_kernel, tf, cand, d_rpm, (const int*)(d + o_in),
-                   (const int*)(d + o_out), L);
+    tf.srv_keep_acc = (const uint8_t*)(d + o_pin);
+    launch_records(h, (long long)S * A * L, trivial_kernel, tf, cand, lists.load(d), L);
     // phase 1: the searches
     rc = sk.enqueue(h, kd, d);
     if (rc) return rc;
@@ -1602,23 +1612,18 @@ int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in,
     if (tk.n_items > 0) {
         SloTraceArgs g{};
         g.w = tk.args(d, S);
-        g.w.ld.f = kd;
-        g.w.ld.cand_pair = pt.pair();
-        g.w.ld.cand_N = pt.len();
-        g.w.ld.tab_off = pt.off();
-        g.w.ld.tab = (const double*)pt.tab.p;
-        g.w.ld.level_rpm = d_rpm;
-        g.w.ld.n_cand = pt.n;
+        set_tables(g.w.ld, kd, pt);
+        g.w.ld.level_rpm = lists.rpm.dev(d);
         g.w.ld.L = L;
         g.w.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
         g.w.ld.cand = cand;
         g.w.ld.fb = fb2.list;
         g.f = h->df;
-        g.tick_in = (const int*)(d + o_in);
-        g.tick_out = (const int*)(d + o_out);
-        g.slo_itl = (const float*)(d + sk.o_itl);
-        g.slo_ttft = (const float*)(d + sk.o_ttft);
-        g.slo_tps = (const float*)(d + sk.o_tps);
+        g.tick_in = lists.in.dev(d);
+        g.tick_out = lists.out.dev(d);
+        g.slo_itl = lists.itl.dev(d);
+        g.slo_ttft = lists.ttft.dev(d);
+        g.slo_tps = lists.tps.dev(d);
         g.key = (const int*)(d + sk.o_key);
         g.srch = sk.srch;
         g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
@@ -1643,8 +1648,8 @@ int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in,
 // The rows of a wva_profile_rows list as the profile grid and the profile trace size them.  Per (m, a) the host ranks
 // the distinct present rows that the levels use (elsewhere no pair of m is a load); key-model (m, j) = moff[m] + j
 // holds the j-th distinct row of (m, a) at every accelerator a that has one, so a key fleet's tables stay within
-// L * M * A entries.  The caller's row lists travel in the call's upload image (place, write), and set_rows points
-// a ProfileArgs at them.
+// L * M * A entries.  The caller's row lists travel in the call's upload image (place), and set_rows points a
+// ProfileArgs at them.
 struct ProfileRanks {
     using Row = std::array<uint32_t, 6>;  // bits of alpha, beta, gamma, delta; max_batch, at_tokens
     const void* lists[9];                 // column c: the caller's row list (bit c of per_level) or NULL
@@ -1748,11 +1753,7 @@ struct ProfileRanks {
     }
     void place(Cols& c) {
         for (int b = 0; b < 9; ++b)
-            if (lists[b]) o_list[b] = c.take(list_bytes(b));
-    }
-    void write(char* p) const {
-        for (int b = 0; b < 9; ++b)
-            if (lists[b] && L) memcpy(p + o_list[b], lists[b], list_bytes(b));
+            if (lists[b]) o_list[b] = c.put(lists[b], list_bytes(b));
     }
     // g.rows: g.f with the row lists uploaded at d, and per_level
     void set_rows(ProfileArgs& g, const char* d) const {
@@ -1854,16 +1855,11 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
     kf.place(c);
     pr.place(c);
     const std::vector<int>& rank = pr.rank;
-    const size_t o_rank = c.take(4 * rank.size()), o_poff = c.take(4 * pair_off.size()),
-                 o_keyof = c.take(4 * key_of.size()), o_ksrv = c.take(4 * (size_t)K),
+    const size_t o_rank = c.put(rank.data(), 4 * rank.size()), o_poff = c.put(pair_off.data(), 4 * pair_off.size()),
+                 o_keyof = c.put(key_of.data(), 4 * key_of.size()), o_ksrv = c.take(4 * (size_t)K),
                  o_loff = c.take(4 * ((size_t)K + 1)), o_lev = c.take(4 * (size_t)K),
                  o_item = c.take(4 * ((size_t)n + 1));
     rc = upload_tables(h, h->lg_tabs, pairs, Ns, true, c, [&](char* p) {
-        kf.write(p);
-        pr.write(p);
-        if (!rank.empty()) memcpy(p + o_rank, rank.data(), 4 * rank.size());
-        memcpy(p + o_poff, pair_off.data(), 4 * pair_off.size());
-        if (!key_of.empty()) memcpy(p + o_keyof, key_of.data(), 4 * key_of.size());
         // the tail's one level: key k is server k of the key fleet, candidate e item e (written in place: building
         // them as TokenKeys costs the host measurably more at 10^5 keys)
         int* ksrv = (int*)(p + o_ksrv);
@@ -1925,30 +1921,23 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
                           const wva_profile_rows& rows, const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A, M = hf.M;
-    const size_t LS = (size_t)L * S;
-    std::vector<float> own_rpm;
-    std::vector<int32_t> own_in, own_out;
-    auto tile = [&](auto*& list, const auto& col, auto& own) {
-        if (list) return;
-        own.resize(LS);
-        for (int t = 0; t < L; ++t) std::copy(col.begin(), col.end(), own.begin() + (size_t)t * S);
-        list = own.data();
-    };
-    tile(rpm, hf.srv_arrival_rpm, own_rpm);
-    tile(in, hf.srv_in_tokens, own_in);
-    tile(out, hf.srv_out_tokens, own_out);
+    Cols c(16);
+    RowLists lists{hf, L, c};
+    lists.put_rpm(rpm);
+    lists.put_tokens(in, out);
+    rpm = lists.rpm.host;  // from here on: the caller's lists or the tiled columns
+    in = lists.in.host;
+    out = lists.out.host;
     ProfileRanks pr(hf, L, rows);
-    std::vector<uint8_t> pin(S);
-    for (int s = 0; s < S; ++s) pin[s] = trace_pinned(hf, s);
+    const std::vector<uint8_t> pin = trace_pinned(hf);
+    const size_t o_pin = c.put(pin.data(), S);
     // The keys.  Without a perf column: the workload trace's (s, in, out) rows.  With one: per server the ticks at
     // which s is a load, grouped by (in, out) as in the workload trace; per group and accelerator the ticks at which
     // (m, a) is present, grouped by the row's sizing key, one row per key pair.  A pinned server sizes its current
     // pair alone.
     TokenKeys tk;
     std::vector<int> key_acc, key_model;  // with a perf column: key row k's accelerator and key-model
-    if (!pr.perf_rows) {
-        token_keys(L, S, rpm, in, out, tk);
-    } else {
+    if (pr.perf_rows) {
         std::vector<std::pair<uint64_t, int>> uses;                 // ((in << 32) | out, tick)
         std::vector<std::pair<std::array<uint64_t, 3>, int>> prof;  // (sizing key, tick)
         for (int s = 0; s < S; ++s) {
@@ -1975,12 +1964,13 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
                 }
             });
         }
+        // at most L * S * A key rows; the key fleet's pair ids k * A + a are int
+        if ((long long)tk.srv.size() * A >= (1ll << 31))
+            return h->fail(WVA_ERR_UNSUPPORTED,
+                           "profile trace too large for one call (>= 2^31 key pairs x accelerators)");
     }
-    const int K = (int)tk.srv.size();  // at most L * S * A
-    // the key fleet's pair ids k * A + a are int
-    if ((long long)K * A >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "profile trace too large for one call (>= 2^31 key pairs x accelerators)");
-    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
+    KeyFleet kf = pr.perf_rows ? KeyFleet(hf, tk.srv, tk.in, tk.out) : workload_keys(hf, L, rpm, in, out, pin.data(), tk);
+    const int K = (int)tk.srv.size();
     HostFleet& kh = kf.hf;
     if (pr.perf_rows) {
         kf.own_ma = true;
@@ -1990,27 +1980,13 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
             kh.srv_cur_acc[k] = key_acc[k];
         }
         pr.fill(kh);
-    } else {  // the workload trace's key fleet
-        for (int k = 0; k < K; ++k) kh.srv_keep_acc[k] = pin[tk.srv[k]];
     }
-    Cols c(16);
     kf.place(c);
     pr.place(c);
     // the tail's candidates: one per key row with a perf column, up to A without
     tk.place(c, pr.perf_rows ? (size_t)K : (size_t)K * A);
-    const size_t o_rpm = c.take(4 * LS), o_in = c.take(4 * LS), o_out = c.take(4 * LS), o_pin = c.take(S);
     std::vector<int> pairs;
-    int rc = prepare_load_star(h, kh, std::vector<char>(K, 1), pairs, c, [&](char* p) {
-        kf.write(p);
-        pr.write(p);
-        tk.write(p, pairs, A);
-        if (LS) {
-            memcpy(p + o_rpm, rpm, 4 * LS);
-            memcpy(p + o_in, in, 4 * LS);
-            memcpy(p + o_out, out, 4 * LS);
-        }
-        if (S) memcpy(p + o_pin, pin.data(), S);
-    });
+    int rc = prepare_load_star(h, kh, std::vector<char>(K, 1), pairs, c, [&](char* p) { tk.write(p, pairs, A); });
     if (rc) return rc;
     const char* d = (const char*)h->lg_tabs.lists.p;
     rc = ensure_ctrl(h);
@@ -2019,7 +1995,7 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
     rc = enqueue_load_star(h, kh, kf.view(h->df, d), tk.n_items, ls);
     if (rc) return rc;
     WorkloadArgs g = tk.args(d, S);
-    rc = enqueue_workload_tail(h, ls, g, (const float*)(d + o_rpm), L, cand);
+    rc = enqueue_workload_tail(h, ls, g, lists.rpm.dev(d), L, cand);
     if (rc) return rc;
     ProfileTraceArgs r{};
     r.p.f = h->df;
@@ -2027,9 +2003,7 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
     pr.set_rows(r.p, d);
     r.p.cand = cand;
     r.p.L = L;
-    r.level_rpm = (const float*)(d + o_rpm);
-    r.level_in = (const int*)(d + o_in);
-    r.level_out = (const int*)(d + o_out);
+    r.rows = lists.load(d);
     launch_records(h, (long long)S * A * L, profile_trace_kernel, r);
     enqueue_level_winners(h, cand, winners, L, true);
     CK(cudaGetLastError());

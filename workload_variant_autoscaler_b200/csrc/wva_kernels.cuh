@@ -5,8 +5,7 @@
 //                       sort, persistent warps pulling 32-cell items, fused feasibility + batch-rank minimum
 //   grid_fallback       stored-vector re-run of the rare cells the streaming solve bails on
 //   grid_finalize  K3   per-server argmin over partials (warp shuffle -> smem -> record)
-//   trivial_kernel      nil / zero-load candidates (overloads: per level of wva_load_grid, wva_slo_grid and
-//                       wva_workload_grid)
+//   trivial_kernel      nil / zero-load candidates (overload: per level of the load rows of the level calls)
 //   unlimited_kernel    Server.Calculate value + SolveUnlimited argmin per server (overload: per load level)
 //   trace_kernel        the same tick by tick, each tick's winner the next tick's current allocation
 //   profile_kernel      the profile grid's records per (level, pair) from the key records, priced at the level
@@ -185,6 +184,19 @@ __device__ __forceinline__ float total_rate_of(const DevFleet& f, int s, float r
 __device__ __forceinline__ DevFleet at_level(const DevFleet& f, const float* level_rpm, int l) {
     DevFleet fl = f;
     fl.srv_arrival_rpm = level_rpm + (size_t)l * f.S;
+    return fl;
+}
+// [L * S] lists of a call's arrival rates and input and output tokens by row; NULL: the fleet's own column
+struct LoadRows {
+    const float* rpm;
+    const int* in;
+    const int* out;
+};
+// The fleet at row l of the load rows.
+__device__ __forceinline__ DevFleet at_rows(const DevFleet& f, const LoadRows& rows, int l) {
+    DevFleet fl = rows.rpm ? at_level(f, rows.rpm, l) : f;
+    if (rows.in) fl.srv_in_tokens = rows.in + (size_t)l * f.S;
+    if (rows.out) fl.srv_out_tokens = rows.out + (size_t)l * f.S;
     return fl;
 }
 __device__ __forceinline__ float penalty_of(const DevFleet& f, int s, const Cand& c) {
@@ -1613,45 +1625,16 @@ __global__ void trivial_kernel(DevFleet f, AllocCols cand, const int* batch, int
     if (cls == PAIR_ZERO) c = batch ? zero_load_alloc(f, s, a, batch[bi]) : zero_load_alloc(f, s, a);
     store_cand(cand, i, c);
 }
-// ... of the load grid: L level blocks of S * A records (record l * S * A + pair), each pair classed at its
-// level's rate level_rpm[l * S + s]; a zero-load candidate at the pair's own batch size (S * A * L < 2^31, checked
-// on the host).
-__global__ void trivial_kernel(DevFleet f, AllocCols cand, const float* level_rpm, int L) {
+// ... of a level call: L level blocks of S * A records (record l * S * A + pair), each pair classed at row l of the
+// load rows (the SLO grid has none: a pair's class and its nil or zero-load record read no target); a zero-load
+// candidate at the pair's own batch size reads no load (S * A * L < 2^31, checked on the host).
+__global__ void trivial_kernel(DevFleet f, AllocCols cand, LoadRows rows, int L) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int n_pairs = f.S * f.A;
     if (i >= n_pairs * L) return;
     const int l = i / n_pairs, pair = i - l * n_pairs;
     const int s = pair / f.A, a = pair % f.A;
-    const int cls = pair_class(at_level(f, level_rpm, l), s, a, true);
-    if (cls == PAIR_LOAD) return;
-    store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
-}
-// ... of the SLO grid: L level blocks of S * A records (record l * S * A + pair); a pair's class and its nil or
-// zero-load record read no target, so every block gets the same (S * A * L < 2^31, checked on the host).
-__global__ void trivial_kernel(DevFleet f, AllocCols cand, int L) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int n_pairs = f.S * f.A;
-    if (i >= n_pairs * L) return;
-    const int pair = i % n_pairs;
-    const int s = pair / f.A, a = pair % f.A;
-    const int cls = pair_class(f, s, a, true);
-    if (cls == PAIR_LOAD) return;
-    store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
-}
-// ... of the workload grid: L level blocks of S * A records (record l * S * A + pair), each pair classed at its
-// level's rate and tokens (row l of level_rpm, level_in and level_out); a zero-load candidate reads no tokens
-// (S * A * L < 2^31, checked on the host).
-__global__ void trivial_kernel(DevFleet f, AllocCols cand, const float* level_rpm, const int* level_in,
-                               const int* level_out, int L) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int n_pairs = f.S * f.A;
-    if (i >= n_pairs * L) return;
-    const int l = i / n_pairs, pair = i - l * n_pairs;
-    const int s = pair / f.A, a = pair % f.A;
-    DevFleet fl = at_level(f, level_rpm, l);
-    fl.srv_in_tokens = level_in + (size_t)l * f.S;
-    fl.srv_out_tokens = level_out + (size_t)l * f.S;
-    const int cls = pair_class(fl, s, a, true);
+    const int cls = pair_class(at_rows(f, rows, l), s, a, true);
     if (cls == PAIR_LOAD) return;
     store_cand(cand, i, cls == PAIR_ZERO ? zero_load_alloc(f, s, a) : cand_nil());
 }
@@ -1804,15 +1787,13 @@ __global__ void profile_kernel(ProfileArgs g) {
 
 // The profile trace's records (DESIGN.md §3.15): L tick blocks of S * A records (record (t * S + s) * A + a), one
 // thread per record, after the workload grid's tail wrote every load pair's record in place at the key fleet's
-// price.  f_t is f with row t of the load rows and of the profile rows (profile_at).  A pair is classed at f_t: nil,
-// zeroLoadAllocation at f_t, or the tail's record priced at row t.  f carries keepAccelerator on the pinned servers
-// only, whose pairs the tail did not size; trace_kernel applies the rest of the mask tick by tick (S * A * L < 2^31,
-// checked on the host).
+// price.  f_t is f with row t of the load rows (at_rows) and of the profile rows (profile_at).  A pair is classed at
+// f_t: nil, zeroLoadAllocation at f_t, or the tail's record priced at row t.  f carries keepAccelerator on the pinned
+// servers only, whose pairs the tail did not size; trace_kernel applies the rest of the mask tick by tick
+// (S * A * L < 2^31, checked on the host).
 struct ProfileTraceArgs {
-    ProfileArgs p;           // f, rows, per_level, cand and L (rank, pair_off, key_of and key are not read)
-    const float* level_rpm;  // [L * S] row t's arrival rates ...
-    const int* level_in;     // ... input tokens ...
-    const int* level_out;    // ... and output tokens
+    ProfileArgs p;  // f, rows, per_level, cand and L (rank, pair_off, key_of and key are not read)
+    LoadRows rows;
 };
 __global__ void profile_trace_kernel(ProfileTraceArgs g) {
     const ProfileArgs& p = g.p;
@@ -1821,10 +1802,7 @@ __global__ void profile_trace_kernel(ProfileTraceArgs g) {
     if (i >= n_pairs * p.L) return;
     const int t = i / n_pairs, pair = i - t * n_pairs;
     const int s = pair / p.f.A, a = pair % p.f.A;
-    DevFleet ft = profile_at(p, t);
-    ft.srv_arrival_rpm = g.level_rpm + (size_t)t * p.f.S;
-    ft.srv_in_tokens = g.level_in + (size_t)t * p.f.S;
-    ft.srv_out_tokens = g.level_out + (size_t)t * p.f.S;
+    const DevFleet ft = at_rows(profile_at(p, t), g.rows, t);
     const int cls = pair_class(ft, s, a, true);
     Cand c = cand_nil();
     if (cls == PAIR_ZERO) c = zero_load_alloc(ft, s, a);
