@@ -615,6 +615,45 @@ int wva_price_thresholds(wva_handle *h, const wva_fleet *fleet, float *threshold
                          wva_allocs *above /* [S*A], may be NULL */, wva_allocs *candidates /* [S*A], may be NULL */);
 
 /*
+ * SLO bounds: for each (server s, accelerator a) and search w (0: TTFT, 1: ITL), the exact targets at which the
+ * reference's candidate turns nil and at which its target stops binding.  Entry (s*A + a)*2 + w of each column.
+ *
+ * BinarySearch (utils.go:26-70) decides from the target t > 0 and two values that do not depend on it, y_lo =
+ * eval(lambda_min) and y_hi = eval(lambda_max) (EvalTTFT or EvalITL, both from one Model.Solve at that lambda in
+ * req/ms), which class t falls in:
+ *   NIL       "target is below the bounded region": Size fails and the candidate is nil;
+ *   FREE      lambda* = lambda_max exactly (within tolerance of y_hi, or above the bounded region);
+ *   SEARCHED  within tolerance of y_lo, or the bisection runs.
+ * Over the positive float32 targets up to +Inf the classes come in one order (DESIGN.md §3.18): rising (y_lo <
+ * y_hi) NIL, SEARCHED, FREE; otherwise FREE, SEARCHED, NIL.  Any stretch may be empty.  b1 <= b2 split them: t is
+ * in the first stretch when !(t >= b1), in the last when t >= b2, else in the middle one.  b1 or b2 is NaN where
+ * the stretches before it reach through +Inf (no positive target is past it).  Two consequences are exact:
+ *   - t in the NIL stretch of w: the candidate is nil whatever the other targets are;
+ *   - t in the FREE stretch of w: the candidate is byte for byte the one with w's target 0 and the other targets
+ *     unchanged (lambda* is lambda_max, bit for bit, in both).
+ * So a server whose candidates are all NIL at t has a nil winner, and one whose candidates that read the target
+ * are all FREE at t has its winner at target 0.
+ *
+ * kind: 0 target not read (a pair that is not a load pair, or a model of fewer than 2 states: the candidate does
+ * not depend on t); 1 every positive target nil (lambda_min > lambda_max, or lambda_min < 0, where the model is
+ * invalid at the first evaluation); 2 rising; 3 not rising.  y_lo, y_hi, b1 and b2 are 0 for kinds 0 and 1.
+ *
+ * The bounds belong to the pair: srv_slo_* are not read (srv_has_target and the other gates decide kind 0), nor
+ * are fleet->unlimited and the capacities.  Any column of out may be NULL (not written).  The fleet becomes
+ * resident, and wva_summarize returns WVA_ERR_STATE afterwards.  WVA_ERR_BAD_ARG: out NULL.  WVA_ERR_UNSUPPORTED:
+ * the queue-size rule, before any kernel is launched, as wva_analyze refuses it; a boundary solve whose rescale
+ * loop does not terminate (wva_last_error names the pair and the end).
+ */
+typedef struct wva_slo_bounds_out {
+    uint8_t *kind; /* [S*A*2] */
+    float *y_lo;   /* [S*A*2] */
+    float *y_hi;   /* [S*A*2] */
+    float *b1;     /* [S*A*2] */
+    float *b2;     /* [S*A*2] */
+} wva_slo_bounds_out;
+int wva_slo_bounds(wva_handle *h, const wva_fleet *fleet, wva_slo_bounds_out *out);
+
+/*
  * Solver.SolveGreedy + the best-effort saturation policies (pkg/solver/greedy.go:35-341) over a candidate
  * table the caller already holds: `candidates` (S*A, value = transition penalty as wva_analyze returns it) is
  * read, and modified where the reference scales best-effort allocations; `winners` (S) is written.  Host only

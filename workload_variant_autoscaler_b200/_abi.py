@@ -100,6 +100,10 @@ class IntervalsC(C.Structure):
                 ("rec", AllocsC)]
 
 
+class SloBoundsC(C.Structure):
+    _fields_ = [("kind", u8p), ("y_lo", f32p), ("y_hi", f32p), ("b1", f32p), ("b2", f32p)]
+
+
 class ProfileRowsC(C.Structure):
     _fields_ = [("acc_cost", f32p), ("perf_present", u8p), ("perf_alpha", f32p), ("perf_beta", f32p),
                 ("perf_gamma", f32p), ("perf_delta", f32p), ("perf_acc_count", i32p), ("perf_max_batch", i32p),

@@ -224,6 +224,7 @@ struct wva_handle {
     DevBuf d_slo;      // the SLO grid's search records
     DevBuf d_prof;     // the profile grid's key records
     DevBuf d_price;    // the price thresholds
+    DevBuf d_bounds;   // the SLO bounds' end records and entries
 
     // grid path
     DevBuf d_sort, d_best, d_pb, d_rows;
@@ -2039,6 +2040,47 @@ int enqueue_price_thresholds(wva_handle* h, float* threshold, const AllocCols& c
     return WVA_OK;
 }
 
+// ---- SLO bounds: where each load pair's two searches turn nil and stop binding (DESIGN.md §3.18) ----------------
+// The load pairs (pairs, batch sizes Ns, sorted by descending N) get one N-entry table each in lg_tabs, as the level
+// calls build them.  bounds_tail solves both ends of every pair into the end records, the stored-vector re-run takes
+// the items it bailed on, and bounds_kernel writes the entries.  g carries the device columns of the call's buffer
+// (ends, out); the launches do not depend on the fleet once it has a load pair.
+int enqueue_slo_bounds(wva_handle* h, const std::vector<int>& pairs, const std::vector<int>& Ns,
+                       const std::vector<int>& cand_of_pair, BoundsArgs& g) {
+    const HostFleet& hf = h->hf;
+    int rc = ensure_ctrl(h);
+    if (rc) return rc;
+    PairTables& pt = h->lg_tabs;
+    Cols c(16);
+    const size_t o_cop = c.put(cand_of_pair.data(), 4 * cand_of_pair.size());
+    rc = upload_tables(h, pt, pairs, Ns, false, c, [](char*) {});
+    if (rc) return rc;
+    rc = build_tables(h, h->df, pt);
+    if (rc) return rc;
+    const int n = pt.n;
+    FbRun fb;
+    rc = prepare_fallback(h, 0, 2 * n, n ? pt.len_max : 0, fb);
+    if (rc) return rc;
+    set_tables(g, h->df, pt);
+    g.cand_of_pair = (const int*)((const char*)pt.lists.p + o_cop);
+    g.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
+    g.fb = fb.list;
+    CK(cudaEventRecord(h->ev_k0, h->stream));
+    if (n > 0) {
+        rc = launch_tail(h, bounds_tail, bounds_fallback, g, (2ll * n + 31) / 32, fb);
+        if (rc) return rc;
+    } else {
+        CK(cudaEventRecord(h->ev_k1, h->stream));
+    }
+    const long long n_out = 2ll * hf.S * hf.A;
+    if (n_out > 0) {
+        bounds_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, h->stream>>>(g);
+        h->launches++;
+    }
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
 // ---- grid path (K2 + K3) ----------------------------------------------------
 int validate_grid(wva_handle* h, const wva_grid* g) {
     if (!g) return h->fail(WVA_ERR_BAD_ARG, "grid is NULL");
@@ -3007,6 +3049,53 @@ int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold
     scatter_block(c.cand_host, c.bc, candidates);
     if (c.win_host) scatter_block(c.win_host, c.bw, above);
     return WVA_OK;
+}
+
+int wva_slo_bounds(wva_handle* h, const wva_fleet* fleet, wva_slo_bounds_out* out) {
+    if (!h) return WVA_ERR_BAD_ARG;
+    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
+    if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    const HostFleet& hf = h->hf;
+    std::vector<int> pairs, Ns;
+    rc = sorted_pairs(h, hf, [&](int s, int a) { return hf.pair_class(s, a, true) == PAIR_LOAD; }, pairs, Ns);
+    if (rc) return rc;
+    const size_t n = pairs.size(), n_out = 2 * (size_t)hf.S * hf.A;
+    std::vector<int> cand_of_pair((size_t)hf.S * hf.A, -1);
+    for (size_t e = 0; e < n; ++e) cand_of_pair[pairs[e]] = (int)e;
+    // the end records (their feasible column comes back to name a pair whose solve failed), then the entries
+    std::vector<uint8_t> solved(2 * n, 1);
+    Cols b(16);
+    const size_t o_solved = b.take(2 * n, solved.data()), o_ttft = b.take(8 * n), o_itl = b.take(8 * n);
+    const size_t o_kind = b.take(n_out, out->kind), o_ylo = b.take(4 * n_out, out->y_lo),
+                 o_yhi = b.take(4 * n_out, out->y_hi), o_b1 = b.take(4 * n_out, out->b1),
+                 o_b2 = b.take(4 * n_out, out->b2);
+    CK(h->d_bounds.ensure(b.bytes));
+    char* d = (char*)h->d_bounds.p;
+    BoundsArgs g{};
+    g.ends.feasible = (uint8_t*)(d + o_solved);
+    g.ends.ttft = (float*)(d + o_ttft);
+    g.ends.itl = (float*)(d + o_itl);
+    g.out = BoundsOut{(uint8_t*)(d + o_kind), (float*)(d + o_ylo), (float*)(d + o_yhi), (float*)(d + o_b1),
+                      (float*)(d + o_b2)};
+    HostCall c{0, false, false, &b, d};
+    rc = run_host(h, c, [&](const AllocCols&, const AllocCols&) {
+        return enqueue_slo_bounds(h, pairs, Ns, cand_of_pair, g);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc == WVA_ERR_UNSUPPORTED)
+        for (size_t i = 0; i < 2 * n; ++i)
+            if (solved[i] == 0) {
+                const int s = pairs[i / 2] / hf.A, a = pairs[i / 2] % hf.A;
+                const std::string what = "boundary solve at lambda_" + std::string(i % 2 ? "max" : "min") +
+                                         " of server " + std::to_string(s) + ", accelerator " + std::to_string(a) +
+                                         ": input outside the supported numeric domain (rescale loop does not "
+                                         "terminate)";
+                return h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
+            }
+    return rc;
 }
 
 // System.AllocateByType + CreateAllocationDiff over the most recent solution (include/wva_b200.h).

@@ -172,11 +172,16 @@ struct SzStart {
     float rmax, lmin, lmax;
     bool nil;
 };
+// RateRange in req/s and the bisection bounds lambda_min / lambda_max in req/ms (queueanalyzer.go:197-198) from a
+// table's first and last service rates.
+__device__ __forceinline__ void sz_range(float s1, float sN, float& rmax, float& lmin, float& lmax) {
+    rmax = rate_max_of(sN);
+    lmin = __fdiv_rn(rate_min_of(s1), 1000.0f);
+    lmax = __fdiv_rn(rmax, 1000.0f);
+}
 __device__ __forceinline__ SzStart sz_start(const DevFleet& f, int s, int K, float s1, float sN) {
     SzStart b;
-    b.rmax = rate_max_of(sN);
-    b.lmin = __fdiv_rn(rate_min_of(s1), 1000.0f);
-    b.lmax = __fdiv_rn(b.rmax, 1000.0f);
+    sz_range(s1, sN, b.rmax, b.lmin, b.lmax);
     const float slo_ttft = f.srv_slo_ttft[s], slo_itl = f.srv_slo_itl[s], slo_tps = f.srv_slo_tps[s];
     b.nil = K < 2 || slo_itl < 0.0f || slo_ttft < 0.0f || slo_tps < 0.0f ||
             (b.lmin > b.lmax && (slo_ttft > 0.0f || slo_itl > 0.0f));
@@ -191,7 +196,7 @@ struct SzSearch {
 };
 
 // The two boundary evaluations (utils.go:36-51); end(0) / end(1) = the points at lo / hi.  A bail-out at hi
-// counts only when the point at lo was not within tolerance.
+// counts only when the point at lo was not within tolerance.  The SLO bounds class their targets with it too.
 template <class End>
 __device__ __forceinline__ int sz_ends(SzSearch& S, float target, End&& end) {
     const SzPt p0 = end(0);
@@ -1141,6 +1146,138 @@ __global__ void __launch_bounds__(256) slo_trace_kernel(SloTraceArgs g) {
 
 // Stored-vector re-run of the items slo_trace_kernel bailed on.
 __global__ void slo_trace_fallback(SloTraceArgs g, FbRun r) { tail_rerun(r, g.w.ld.cand, SloTraceTail{g}); }
+
+// ---------------------------------------------------------------------------
+// SLO bounds (DESIGN.md §3.18): per (load pair, search), the two breakpoints in the target at which BinarySearch's
+// boundary checks change their verdict.  Those checks read the target and y0 = eval(lambda_min), y1 =
+// eval(lambda_max), and EvalTTFT and EvalITL come from one Model.Solve, so two solves per pair give both searches'
+// bounds for every target.  bounds_tail solves one item fb_pack(candidate, end) per (pair, end), end 1 (lambda_max,
+// the pair's longest chain) for every candidate first, and bounds_kernel classifies each (pair, search).
+// ---------------------------------------------------------------------------
+struct BoundsOut {  // [S * A * 2] by (s * A + a) * 2 + which
+    uint8_t* kind;
+    float *y_lo, *y_hi, *b1, *b2;
+};
+enum { BOUNDS_UNREAD = 0, BOUNDS_NIL = 1, BOUNDS_RISING = 2, BOUNDS_FALLING = 3 };
+
+struct BoundsArgs {
+    DevFleet f;
+    const int* cand_pair;       // [n_cand] load pairs sorted by descending N
+    const int* cand_N;          // [n_cand]
+    const long long* tab_off;   // [n_cand] entry offset of the candidate's table (N entries)
+    const double* tab;
+    const int* cand_of_pair;    // [S * A] the pair's candidate, -1: not a load pair
+    int n_cand;
+    unsigned* counter;
+    AllocCols ends;             // [2 * n_cand] record 2e + end: feasible 1 once solved (ttft / itl: the two
+                                // metrics), 2 where no solve runs, 0 where the solve did not terminate
+    FbList fb;                  // items that bailed: fb_pack(candidate, end)
+    BoundsOut out;
+};
+
+// Candidate e's bisection bounds and whether its boundary solves run: not for K < 2 (sz_start's nil), an empty
+// range (BinarySearch's error before any evaluation) or lambda_min < 0, where Model.Solve marks the model invalid
+// (queuemodel.go:27-37) and the first evaluation fails.  Every other model of K >= 2 states is valid: rho = 1 - p[0]
+// of the previous solve lies in [0, 1] (NaN passes the check).
+__device__ __forceinline__ bool bounds_range(const BoundsArgs& g, int e, float& lmin, float& lmax, bool& nil) {
+    const int N = g.cand_N[e], K = N + N * g.f.ratio;
+    const double* tab = g.tab + 4 * g.tab_off[e];
+    float rmax;
+    sz_range((float)tab[0], (float)tab[4 * (N - 1)], rmax, lmin, lmax);
+    nil = lmin > lmax || lmin < 0.0f;
+    return K >= 2;
+}
+
+// Item fb_pack(e, end): Model.Solve(lambda, 1) at lambda = lambda_min (end 0) or lambda_max (end 1), in req/ms as
+// BinarySearch evaluates them, then EvalTTFT and EvalITL (target_value) from that one solve.
+struct BoundsTail {
+    const BoundsArgs& g;
+    __device__ __forceinline__ size_t record(unsigned long long item) const {
+        return 2 * (size_t)(item >> 32) + (unsigned)item;
+    }
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        const int e = (int)(item >> 32), end = (int)(unsigned)item;
+        out = cand_nil();
+        float lmin, lmax;
+        bool nil;
+        if (!bounds_range(g, e, lmin, lmax, nil) || nil) {
+            out.feasible = 2;
+            return true;
+        }
+        const int pair = g.cand_pair[e], N = g.cand_N[e], K = N + N * g.f.ratio;
+        ModelStats st;
+        if (!solve(g.tab + 4 * g.tab_off[e], N, K, end ? lmax : lmin, st)) return false;
+        const QParams q = qparams_of(g.f, pair / g.f.A, pair % g.f.A);
+        out.feasible = 1;
+        out.ttft = target_value(q, 0, N, st);
+        out.itl = target_value(q, 1, N, st);
+        return true;
+    }
+};
+
+__global__ void __launch_bounds__(256) bounds_tail(BoundsArgs g) {
+    const unsigned n = (unsigned)g.n_cand;  // 2 * n < 2^31 (n <= S * A)
+    for_each_warp_item(g.counter, 2 * n, [&](unsigned i) {
+        tail_item(g.fb, g.ends, i < n ? fb_pack((int)i, 1) : fb_pack((int)(i - n), 0), BoundsTail{g});
+    });
+}
+
+// Stored-vector re-run of the items bounds_tail bailed on.
+__global__ void bounds_fallback(BoundsArgs g, FbRun r) { tail_rerun(r, g.ends, BoundsTail{g}); }
+
+// The class of target t for a search with boundary values y0, y1, decided by sz_ends itself over the stand-in range
+// (lo, hi) = (0, 1): NIL where it ends with ind -1, FREE where it ends at hi, SEARCHED where it ends at lo with ind
+// 0 or bisects.  As a rank that never decreases as t grows (DESIGN.md §3.18): rising (y0 < y1) NIL 0, SEARCHED 1,
+// FREE 2; otherwise FREE 0, SEARCHED 1, NIL 2.
+__device__ __forceinline__ int bounds_rank(float y0, float y1, bool rising, float t) {
+    SzSearch S{0.0f, 1.0f, 0.0f, 0, 0, false};
+    const int r = sz_ends(S, t, [&](int i) { return SzPt{i ? y1 : y0, false}; });
+    const int cls = r == SZ_MORE ? 1 : (S.ind < 0 ? 0 : (S.xs == S.hi ? 2 : 1));  // NIL 0, SEARCHED 1, FREE 2
+    return rising ? cls : 2 - cls;
+}
+// The smallest positive float32 target (bits 1 .. 0x7f800000 = +Inf) of rank >= k, or NaN when +Inf's rank is
+// below k: a bisection over the bit patterns, which are ordered like the values.
+__device__ __forceinline__ float bounds_first(float y0, float y1, bool rising, int k) {
+    const unsigned inf = 0x7f800000u;
+    if (bounds_rank(y0, y1, rising, __uint_as_float(inf)) < k) return __uint_as_float(0x7fc00000u);
+    if (bounds_rank(y0, y1, rising, __uint_as_float(1u)) >= k) return __uint_as_float(1u);
+    unsigned lo = 1u, hi = inf;  // rank(lo) < k <= rank(hi)
+    while (hi - lo > 1u) {
+        const unsigned mid = lo + (hi - lo) / 2u;
+        if (bounds_rank(y0, y1, rising, __uint_as_float(mid)) >= k) hi = mid;
+        else lo = mid;
+    }
+    return __uint_as_float(hi);
+}
+
+// One thread per (pair, search) entry (s * A + a) * 2 + which.
+__global__ void __launch_bounds__(256) bounds_kernel(BoundsArgs g) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 2ll * g.f.S * g.f.A) return;
+    const int which = (int)(i & 1), e = g.cand_of_pair[i >> 1];
+    int kind = BOUNDS_UNREAD;
+    float y0 = 0.0f, y1 = 0.0f, b1 = 0.0f, b2 = 0.0f;
+    float lmin, lmax;
+    bool nil;
+    if (e >= 0 && bounds_range(g, e, lmin, lmax, nil)) {
+        kind = BOUNDS_NIL;
+        if (!nil) {
+            const AllocCols& r = g.ends;
+            y0 = which ? r.itl[2 * (size_t)e] : r.ttft[2 * (size_t)e];
+            y1 = which ? r.itl[2 * (size_t)e + 1] : r.ttft[2 * (size_t)e + 1];
+            const bool rising = y0 < y1;
+            kind = rising ? BOUNDS_RISING : BOUNDS_FALLING;
+            b1 = bounds_first(y0, y1, rising, 1);
+            b2 = bounds_first(y0, y1, rising, 2);
+        }
+    }
+    if (g.out.kind) g.out.kind[i] = (uint8_t)kind;
+    if (g.out.y_lo) g.out.y_lo[i] = y0;
+    if (g.out.y_hi) g.out.y_hi[i] = y1;
+    if (g.out.b1) g.out.b1[i] = b1;
+    if (g.out.b2) g.out.b2[i] = b2;
+}
 
 // ---------------------------------------------------------------------------
 // Load intervals (DESIGN.md §3.10): per server, the float32 arrival rates in [lo, hi] at which the load grid's

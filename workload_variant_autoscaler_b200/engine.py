@@ -71,6 +71,80 @@ def accelerator_demand(fleet: Fleet, threshold, candidates: Allocs, a: int):
     return breakpoints, np.cumsum(per_k[::-1])[::-1][1:]
 
 
+# The smallest positive float32 target, and the position past +Inf as a uint32 key (its float is a NaN): the SLO
+# bounds order targets by their bit patterns, which are ordered like the positive values.
+_MIN_TARGET = np.float32(np.finfo(np.float32).smallest_subnormal)
+_PAST_INF = np.uint32(0x7F800001)
+
+
+def _target_keys(x):
+    """Bit patterns of positive float32 targets or NaN (past +Inf) as ordered uint32 keys."""
+    x = np.ascontiguousarray(x, np.float32)
+    return np.where(np.isnan(x), _PAST_INF, x.view(np.uint32)).astype(np.uint32)
+
+
+def _key_targets(k):
+    k = np.ascontiguousarray(k, np.uint32)
+    return np.where(k == _PAST_INF, np.float32(np.nan), k.view(np.float32)).astype(np.float32)
+
+
+def _zero_load_pairs(fleet: Fleet):
+    """(S, A) bool: the pairs whose candidate is zeroLoadAllocation (pkg/core/allocation.go:42-75 with the
+    keepAccelerator rule of server.go:70-82): feasible at every target, since neither search runs."""
+    S, A = fleet.n_servers, fleet.n_acc
+    acc = np.arange(A)[None, :]
+    m = fleet.srv_model.astype(np.int64)
+    known = (m >= 0) & (m < fleet.n_models)
+    present = np.zeros((S, A), bool)
+    present[known] = fleet.perf_present[m[known]] != 0
+    cur = fleet.srv_cur_acc[:, None]
+    masked = (fleet.srv_keep_acc[:, None] != 0) & (cur != -1) & (cur != acc)
+    rpm, tin, tout = fleet.srv_arrival_rpm, fleet.srv_in_tokens, fleet.srv_out_tokens
+    gated = (rpm < 0) | (tin < 0) | (tout < 0) | (fleet.srv_has_target == 0)
+    zero = (rpm == 0) | (tout == 0)
+    return present & ~masked & (~gated & zero)[:, None]
+
+
+def slo_envelope(fleet: Fleet, bounds, which: int):
+    """Per server, the targets of search ``which`` (0: TTFT, 1: ITL) between which its winner depends on that
+    target, from ``Engine.slo_bounds``' output (host only, no GPU) -> (floor [S], ceiling [S]) float32.
+
+    Both are exact statements about ``solve``'s unlimited winner of server ``s`` on the fleet with ``s``'s target
+    of search ``which`` set to ``t`` (any positive float32 up to +Inf) and every other column unchanged:
+
+    * ``floor[s]`` is the smallest positive target at which some candidate of ``s`` is not NIL (a zero-load
+      candidate is never NIL).  At every target below it (``not t >= floor[s]``) every candidate is nil whatever
+      the other targets are, so ``s``'s winner is nil.
+    * ``ceiling[s]`` is the smallest target from which on every candidate of ``s`` that reads the target (kinds 1
+      to 3) is FREE.  At every target ``t >= ceiling[s]`` each candidate, and so ``s``'s winner, is byte for byte
+      the one with that target set to 0.  A server with no such candidate gets the smallest positive target.
+
+    +Inf is itself a target, so where no target qualifies the value is NaN, as for the bounds' b1 and b2: the
+    position past +Inf, which no comparison ``t >= x`` reaches."""
+    kind, _, _, b1, b2 = (np.asarray(x) for x in bounds)
+    S, A = fleet.n_servers, fleet.n_acc
+    if which not in (0, 1):
+        raise ValueError("which must be 0 (TTFT) or 1 (ITL)")
+    if kind.shape != (S, A, 2):
+        raise ValueError("bounds must have shape (n_servers, n_acc, 2)")
+    k, k1, k2 = kind[..., which], _target_keys(b1[..., which]), _target_keys(b2[..., which])
+    lo = _target_keys(_MIN_TARGET)
+    # first target at which the candidate is not NIL: rising after its NIL stretch, falling from the start unless
+    # its NIL stretch is everything
+    not_nil = np.full((S, A), _PAST_INF, np.uint32)
+    not_nil[k == 2] = k1[k == 2]
+    not_nil[(k == 3) & (k2 > lo)] = lo
+    not_nil[_zero_load_pairs(fleet)] = lo
+    # first target from which on the candidate is FREE: rising from b2, falling only when FREE is every target
+    free = np.full((S, A), lo, np.uint32)
+    free[k == 1] = _PAST_INF
+    free[k == 2] = k2[k == 2]
+    free[k == 3] = np.where(k1[k == 3] == _PAST_INF, lo, _PAST_INF)
+    floor = not_nil.min(axis=1) if A else np.full(S, _PAST_INF, np.uint32)
+    ceiling = free.max(axis=1) if A else np.full(S, lo, np.uint32)
+    return _key_targets(floor), _key_targets(ceiling)
+
+
 # the fleet column each load or target row list replaces (every other row list is named after its column)
 _ROW_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens",
                "slo_itl": "srv_slo_itl", "slo_ttft": "srv_slo_ttft", "slo_tps": "srv_slo_tps"}
@@ -389,6 +463,25 @@ class Engine:
         self._check(self._L.wva_price_thresholds(self._h, C.byref(fc), _abi.ptr(threshold.reshape(-1)), C.byref(ac),
                                                  C.byref(cc) if cc is not None else None))
         return threshold, above, cand
+
+    def slo_bounds(self, fleet: Fleet):
+        """Where each load pair's TTFT and ITL searches turn the candidate nil and stop binding -> (kind, y_lo, y_hi,
+        b1, b2), each of shape (S, A, 2), index [s, a, w] with w = 0: TTFT, 1: ITL.
+
+        ``kind`` (uint8): 0 the target is not read, 1 every positive target nil, 2 rising (stretches NIL,
+        SEARCHED, FREE), 3 not rising (FREE, SEARCHED, NIL).  ``y_lo`` / ``y_hi`` are EvalTTFT / EvalITL at
+        lambda_min / lambda_max.  A target ``t`` is in the first stretch when ``not t >= b1``, in the last when
+        ``t >= b2``, else in the middle; NaN is past +Inf.  ``srv_slo_*``, ``fleet.unlimited`` and the capacities
+        are not read (see ``wva_slo_bounds`` in include/wva_b200.h).  ``slo_envelope`` turns them into per-server
+        statements."""
+        S, A = fleet.n_servers, fleet.n_acc
+        kind = np.zeros((S, A, 2), np.uint8)
+        cols = [np.zeros((S, A, 2), np.float32) for _ in range(4)]
+        oc = _abi.SloBoundsC(_abi.ptr(kind.reshape(-1)), *(_abi.ptr(c.reshape(-1)) for c in cols))
+        fc = fleet.as_c()
+        self._resident(fleet)
+        self._check(self._L.wva_slo_bounds(self._h, C.byref(fc), C.byref(oc)))
+        return (kind, *cols)
 
     def sweep(self, fleet: Fleet, n_rates: int) -> dict:
         n = fleet.n_servers * fleet.n_acc * n_rates
