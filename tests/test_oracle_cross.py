@@ -4,9 +4,10 @@ Float outputs under load are pinned by no reference test (SURVEY.md §8c), so tw
 agreeing is what stands in for the Go binary here.  The first three tests are small random cases.  The families after
 them run the restatement on the inputs the GPU tests judge the kernels with, taken from those modules by import: the
 exponent windows (test_gpu_windows), the grid's shape thresholds and stored-vector fallbacks (test_gpu_grid_shapes),
-the adversarial fleets and the queue-size rule (test_gpu_adversarial_paths), and the rows of the SLO, workload and
-profile grids.  A kernel that matches the oracle bit for bit is only as right as the oracle, so a misreading of the Go
-code at one of these edges would otherwise pass every GPU test.
+the adversarial fleets and the queue-size rule (test_gpu_adversarial_paths), the rows of the SLO, workload and
+profile grids, and the rows that put the level calls' tails on the exponent windows (test_gpu_tail_windows).  A
+kernel that matches the oracle bit for bit is only as right as the oracle, so a misreading of the Go code at one of
+these edges would otherwise pass every GPU test.
 
 Comparison: feasible, accelerator, replicas and batch size exactly; cost, ITL, TTFT, rho and max_rate (and a cell's
 or sweep point's TTFT, ITL, rho and throughput) by their float32 bits, NaN equal to NaN; probability vectors by their
@@ -506,3 +507,48 @@ def test_level_rows_cross(oracle_mod, case):
         for l in range(2):
             cross_fleet(oracle_mod, at_profile(g, {"perf_max_batch": mb}, l), t, f"perf batch row {l}")
         t.report(case, min_feasible=150, min_infeasible=40, **{"refused (batch)": 1})
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the level calls' tails at the exponent windows (test_gpu_tail_windows)
+# ---------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("case", ["load", "slo", "profile", "bounds"])
+def test_tail_windows_cross(oracle_mod, case):
+    """The rows test_gpu_tail_windows steers the tails' solves onto the exponent windows with (their bands are
+    asserted there), each applied to a copy of the fleet as the level calls' compositions apply it: an even sample of
+    the load levels and of the SLO grid's TTFT and TPS rows, every edge row, one level of the K >= 2^23 candidate,
+    a sample of the perf_alpha rows, and a sample of the bounds' batch sizes at their own load (Size at lambda_max,
+    then the final Analyze).  The bounds' rate-edge pairs are left out: at a load they need more than 2^31 replicas,
+    which the record's int32 does not hold."""
+    from tests import test_gpu_tail_windows as T
+    from tests.test_gpu_load_grid import at_level
+    from tests.test_gpu_profile_grid import at_profile
+    from tests.test_gpu_slo_grid import at_slo
+    t = Tally()
+    sample = lambda n, k: np.unique(np.linspace(0, n - 1, k).round().astype(int))  # noqa: E731
+    if case == "load":
+        (main, rpm), (long, lrpm), (edge, erpm) = T.load_cases()
+        for l in sample(rpm.shape[0], 16):
+            cross_fleet(oracle_mod, at_level(main, rpm[l]), t, f"load level {l}")
+        cross_fleet(oracle_mod, at_level(long, lrpm[len(lrpm) // 2]), t, "K >= 2^23")
+        for l in range(erpm.shape[0]):
+            cross_fleet(oracle_mod, at_level(edge, erpm[l]), t, f"edge level {l}")
+        t.report(case, min_feasible=40, min_infeasible=0)
+    elif case == "slo":
+        (main, (itl, ttft, tps)), (edge, erows) = T.slo_cases()[:2]
+        L1 = int((ttft[:, 0] > 0).sum())
+        for l in list(sample(L1, 6)) + list(L1 + sample(itl.shape[0] - L1, 6)):
+            cross_fleet(oracle_mod, at_slo(main, itl[l], ttft[l], tps[l]), t, f"SLO row {l}")
+        for l in range(erows[0].shape[0]):
+            cross_fleet(oracle_mod, at_slo(edge, *(r[l] for r in erows)), t, f"edge row {l}")
+        t.report(case, min_feasible=30, min_infeasible=0)
+    elif case == "profile":
+        for fleet, rows in T.profile_cases():
+            L = rows["perf_alpha"].shape[0]
+            for l in sample(L, 12):
+                cross_fleet(oracle_mod, at_profile(fleet, rows, l), t, f"perf_alpha row {l}")
+        t.report(case, min_feasible=40, min_infeasible=0)
+    else:
+        main = T.bounds_cases()[0]
+        cross_fleet(oracle_mod, main, t, "bounds", pairs=[(int(s), 0) for s in sample(main.n_servers, 24)])
+        t.report(case, min_feasible=20, min_infeasible=0)
