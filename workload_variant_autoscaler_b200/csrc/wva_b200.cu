@@ -2278,7 +2278,10 @@ int enqueue_grid(wva_handle* h, GridPlan& plan, const AllocCols& winners, bool t
         // grid_kernel, then their sort
         const size_t order_smem = (long long)hf.A * g.Bmax <= kOrderTabEntries ? (size_t)hf.A * g.Bmax * 32 : 0;
         rc = launch_pdl(h, grid_order, (unsigned)hf.S, kOrderThreads, order_smem, g);
-        if (!rc) rc = launch_pdl(h, grid_sort_cands, (unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads, 0, g);
+        const long long cand_smem = cand_stage_bytes(g.B, g.R, g.Bmax);
+        if (!rc)
+            rc = launch_pdl(h, grid_sort_cands, (unsigned)(kCandCtasPerSm * h->sm_count), kCandThreads,
+                            cand_smem <= kCandStageBytes ? (size_t)cand_smem : 0, g);
         if (!rc) rc = launch_pdl(h, grid_items_scatter, (unsigned)(16 * h->sm_count), 256, 0, g);  // warp per item
         if (rc) return rc;
         const size_t smem = (size_t)kGkWarps * kGkWarpD * sizeof(double);

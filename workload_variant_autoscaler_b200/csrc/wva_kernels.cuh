@@ -673,7 +673,14 @@ constexpr int kOrderThreads = 1024, kOrderG = 4, kOrderMaxRows = 2048;
 constexpr int kOrderTabEntries = 4096;         // 128 KB of 32-byte table entries per server; more are read from global
 constexpr int kOrderRowWarps = 8;              // with g.prune, warps that start on the rows while the others rank
 constexpr int kCandChunk = 4096;               // candidates per chunk of grid_sort_cands (never two pairs)
-constexpr int kCandThreads = 256, kCandCtasPerSm = 4;
+// A chunk's time is its candidates' chains of dependent loads run 8 deep per thread; 2 x 512 keeps 64 registers
+// (4 x 512 or 2 x 1024 spill at 32) and 264 CTAs, more than config 2's 145 chunks (DESIGN.md §5)
+constexpr int kCandThreads = 512, kCandCtasPerSm = 2;
+// grid_sort_cands stages a chunk's tables in shared memory up to this many bytes (cand_stage_bytes)
+constexpr int kCandStageBytes = 16384;
+__host__ __device__ constexpr long long cand_stage_bytes(int B, int R, int Bmax) {
+    return 24ll * B + 32ll * R + 4ll * Bmax;
+}
 constexpr int kCandResv = 2 * kClasses + 16;   // item_count[kCandResv], [kCandResv + 1]: candidates, chunks reserved
 constexpr int kItemCountWords = 2 * kClasses + 32;  // item_count[]: the step's counters, zeroed by build_pair_tables
 __global__ void __launch_bounds__(kOrderThreads) grid_order(GridArgs g) {
@@ -1040,55 +1047,140 @@ __device__ __forceinline__ void sort_plan_in_last_cta(const GridArgs& g) {
     }
 }
 
+// Inclusive max-scan of v[0, kCandChunk) in place by the whole CTA: a contiguous run of kCandScan entries per thread
+// (16-byte loads), a warp scan of the run maxima, then a scan of the warp maxima by warp 0.
+constexpr int kCandScan = kCandChunk / kCandThreads;
+static_assert(kCandScan % 4 == 0, "cta_max_scan reads its runs as uint4");
+__device__ __forceinline__ void cta_max_scan(unsigned* v) {
+    __shared__ unsigned warp_max[kCandThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint4* run4 = (uint4*)v + threadIdx.x * (kCandScan / 4);
+    uint4 r[kCandScan / 4];
+    unsigned run = 0;
+#pragma unroll
+    for (int e = 0; e < kCandScan / 4; ++e) {
+        r[e] = run4[e];
+        run = max(run, max(max(r[e].x, r[e].y), max(r[e].z, r[e].w)));
+    }
+    unsigned inc = run;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const unsigned o = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc = max(inc, o);
+    }
+    if (lane == 31) warp_max[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned w = lane < kCandThreads / 32 ? warp_max[lane] : 0u;
+#pragma unroll
+        for (int d = 1; d < kCandThreads / 32; d <<= 1) {
+            const unsigned o = __shfl_up_sync(0xffffffffu, w, d);
+            if (lane >= d) w = max(w, o);
+        }
+        if (lane < kCandThreads / 32) warp_max[lane] = w;
+    }
+    __syncthreads();
+    const unsigned prev = __shfl_up_sync(0xffffffffu, inc, 1);
+    unsigned m = max(warp > 0 ? warp_max[warp - 1] : 0u, lane > 0 ? prev : 0u);
+#pragma unroll
+    for (int e = 0; e < kCandScan / 4; ++e) {
+        r[e].x = m = max(m, r[e].x);
+        r[e].y = m = max(m, r[e].y);
+        r[e].z = m = max(m, r[e].z);
+        r[e].w = m = max(m, r[e].w);
+        run4[e] = r[e];
+    }
+    __syncthreads();
+}
+
 // grid_order's candidates, a chunk (at most kCandChunk candidates of one pair) per CTA at a time over a fixed grid.
-// A candidate's replica level is the last row of the pair whose first candidate is at or before it, and its rank
-// follows from that row's intervals.  The gates that grid_order's intervals leave to each cell — Analyze's
-// RateRange.Max and K >= 2, and, without a cell table, TPS servers above the stability limit (with one, grid_kernel
-// stores those cells as analysed and not feasible) — give class 255; the others get the length class, and
-// sort_chunk_items sorts the chunk into items.  A chunk never holds two pairs, so neither does an item (grid_kernel
-// fetches the pair record once per item).
-__global__ void __launch_bounds__(kCandThreads) grid_sort_cands(GridArgs g) {
-    __shared__ unsigned cells[kCandChunk];
+// A chunk is a run of the pair's rows, cut at both ends: each row whose candidates reach into the chunk writes its
+// replica level at its first place in the chunk, and a max-scan carries it over the row's other places (a row's first
+// candidate grows with the level).  A candidate's rank follows from its row's intervals.  The tables a candidate
+// reads — batch index and size by rank, the pair's (table, batch) constants by batch index, the table's prefix log2
+// sums (estimate_len searches them) and the server's rate block and the pair's rows by replica level — are staged in
+// shared memory once per chunk with coalesced loads when they fit in kCandStageBytes, so that a candidate's chain of
+// dependent loads runs at shared-memory latency; larger shapes read them from global memory.  The gates that
+// grid_order's intervals leave to each cell — Analyze's RateRange.Max and K >= 2, and, without a cell table, TPS
+// servers above the stability limit (with one, grid_kernel stores those cells as analysed and not feasible) — give
+// class 255; the others get the length class, and sort_chunk_items sorts the chunk into items.  A chunk never holds two
+// pairs, so neither does an item (grid_kernel fetches the pair record once per item).
+__global__ void __launch_bounds__(kCandThreads, kCandCtasPerSm) grid_sort_cands(GridArgs g) {
+    extern __shared__ __align__(16) float4 cand_stage[];  // cand_stage_bytes(B, R, Bmax) when staged
+    __shared__ __align__(16) unsigned cells[kCandChunk];  // the candidate's replica level, then its cell id
     __shared__ uint8_t keys[kCandChunk];
     __shared__ uint8_t sorted_keys[kCandChunk];
     __shared__ unsigned hist[kClasses];
     __shared__ unsigned cursor[kClasses];
     const DevFleet& f = g.f;
     const int R = g.R, B = g.B;
+    const bool staged = cand_stage_bytes(B, R, g.Bmax) <= kCandStageBytes;
+    float4* s_pb = cand_stage;                       // [B] by batch index
+    float4* s_rt = s_pb + B;                         // [R]
+    int4* s_rc = (int4*)(s_rt + R);                  // [R]
+    int2* s_bb = (int2*)(s_rc + R);                  // [B] by rank: batch size, batch index
+    float* s_ls = (float*)(s_bb + B);                // [Bmax]
     pdl_wait();
     pdl_launch_dependents();
     const unsigned n_chunks = g.item_count[kCandResv + 1];
     for (unsigned ci = blockIdx.x; ci < n_chunks; ci += gridDim.x) {
         const uint4 ch = g.chunks[ci];
-        if (threadIdx.x < kClasses) hist[threadIdx.x] = 0;
-        __syncthreads();
+        const int j0 = (int)ch.y, n = (int)ch.z;
         const int sa = (int)ch.x, s = sa / f.A, t = g.pair_tab_idx[sa];
         const long long toff = g.pair_tab_off[sa];
         const bool tps = f.srv_slo_tps[s] > 0.0f && !g.want_cells;
         const int4* rc = g.row_cand + (size_t)sa * R;
-        for (int k = threadIdx.x; k < (int)ch.z; k += kCandThreads) {
-            const int j = (int)ch.y + k;
-            int ri = 0;
-            for (int hi = R - 1; ri < hi;) {
-                const int mid = (ri + hi + 1) >> 1;
-                if (rc[mid].x <= j) ri = mid; else hi = mid - 1;
+        if (threadIdx.x < kClasses) hist[threadIdx.x] = 0;
+        for (int k = threadIdx.x; k < kCandChunk; k += kCandThreads) cells[k] = 0;
+        if (staged) {
+            for (int i = threadIdx.x; i < B; i += kCandThreads) {
+                const int bi = g.rank_to_bi[i];
+                s_bb[i] = make_int2(g.batch[bi], bi);
+                s_pb[i] = g.pb[(size_t)t * B + i];
             }
+            for (int i = threadIdx.x; i < g.Bmax; i += kCandThreads) s_ls[i] = g.ls[toff + t + i];
+            for (int i = threadIdx.x; i < R; i += kCandThreads) s_rt[i] = g.rt[s * R + i];
+        }
+        __syncthreads();
+        for (int ri = threadIdx.x; ri < R; ri += kCandThreads) {
             const int4 row = rc[ri];
-            const int q = j - row.x;
-            const int bi = g.rank_to_bi[q < row.y ? q : row.z + (q - row.y)];
-            const int b = g.batch[bi];
+            const int next = ri + 1 < R ? rc[ri + 1].x : INT_MAX;  // the next row's first candidate
+            const int p = max(row.x, j0) - j0;
+            if (p < n && next > j0 + p) cells[p] = (unsigned)ri;
+            if (staged) s_rc[ri] = row;
+        }
+        __syncthreads();
+        cta_max_scan(cells);
+        const int4* rows = staged ? s_rc : rc;
+        const float4* rts = staged ? s_rt : g.rt + s * R;
+        const float4* pbs = staged ? s_pb : g.pb + (size_t)t * B;
+        const float* lss = staged ? s_ls : g.ls + toff + t;
+        for (int k = threadIdx.x; k < n; k += kCandThreads) {
+            const int ri = (int)cells[k];
+            const int4 row = rows[ri];
+            const int q = j0 + k - row.x;
+            const int rank = q < row.y ? q : row.z + (q - row.y);
+            int b, bi;
+            if (staged) {
+                const int2 bb = s_bb[rank];
+                b = bb.x;
+                bi = bb.y;
+            } else {
+                bi = g.rank_to_bi[rank];
+                b = g.batch[bi];
+            }
             const int K = b + b * f.ratio;
-            const float4 rt = g.rt[s * R + ri];
-            const float4 pb = g.pb[(size_t)t * B + bi];
+            const float4 rt = rts[ri];
+            const float4 pb = pbs[bi];
             int key = 255;
             if (!(rt.x > pb.x) && K >= 2 && !(tps && !(rt.y <= feas_lim(pb.x))))  // Analyze: queueanalyzer.go:135-143
-                key = length_class(estimate_len(g.tab + 4 * toff, g.ls + toff + t, b, K, rt.y, rt.z, pb.w, pb.y, pb.z));
+                key = length_class(estimate_len(g.tab + 4 * toff, lss, b, K, rt.y, rt.z, pb.w, pb.y, pb.z));
             keys[k] = (uint8_t)key;
             cells[k] = ((unsigned)sa * (unsigned)B + (unsigned)bi) * (unsigned)R + (unsigned)ri;
             if (key != 255) seg_inc(hist, key);  // along a row, consecutive ranks: runs of equal classes
         }
         __syncthreads();
-        sort_chunk_items(g, cells, keys, sorted_keys, hist, cursor, (int)ch.z, ch.w);
+        sort_chunk_items(g, cells, keys, sorted_keys, hist, cursor, n, ch.w);
     }
     sort_plan_in_last_cta(g);
 }
