@@ -6,34 +6,9 @@ minNumReplicas on its current accelerator (optimizer_test.go "scaled to %d witho
 import numpy as np
 import pytest
 
+from tests.levels import ACC_CM, SC_CM, _va
 from workload_variant_autoscaler_b200 import Fleet, adapters
 from workload_variant_autoscaler_b200.adapters import go_parse_float32
-
-ACC_CM = {  # CreateAcceleratorUnitCostConfigMap, JSON-decoded as readAccFunc does (optimizer_test.go:72-86)
-    "A100": {"device": "NVIDIA-A100-PCIE-80GB", "cost": "40.00"},
-    "MI300X": {"device": "AMD-MI300X-192GB", "cost": "65.00"},
-    "G2": {"device": "Intel-Gaudi-2-96GB", "cost": "23.00"},
-}
-SC_CM = {  # CreateServiceClassConfigMap
-    "premium.yaml": "name: Premium\npriority: 1\ndata:\n  - model: default/default\n    slo-tpot: 24\n    slo-ttft: 500\n"
-                    "  - model: meta/llama0-70b\n    slo-tpot: 80\n    slo-ttft: 500",
-    "freemium.yaml": "name: Freemium\npriority: 10\ndata:\n  - model: ibm/granite-13b\n    slo-tpot: 200\n    slo-ttft: 2000\n"
-                     "  - model: meta/llama0-7b\n    slo-tpot: 150\n    slo-ttft: 1500",
-}
-
-
-def _va(i, *, arrival="0.00", replicas=1):
-    return {
-        "metadata": {"name": f"test-variantautoscaling-{i}", "namespace": "default",
-                     "labels": {"inference.optimization/acceleratorName": "A100"}},
-        "spec": {"modelID": "meta/llama0-70b", "modelProfile": {"accelerators": [{
-            "acc": "A100", "accCount": 1, "maxBatchSize": 4,
-            "perfParms": {"decodeParms": {"alpha": "20.28", "beta": "0.72"}, "prefillParms": {"gamma": "0", "delta": "0"}}}]}},
-        "status": {"currentAlloc": {"accelerator": "A100", "numReplicas": replicas, "maxBatch": 4, "variantCost": "40.00",
-                                    "itlAverage": "0.00", "ttftAverage": "0.00",
-                                    "load": {"arrivalRate": arrival, "avgInputTokens": "0.00", "avgOutputTokens": "0.00"}}},
-    }
-
 
 def test_parse_float32_is_go_strconv():
     f32 = np.float32

@@ -7,6 +7,7 @@ import sys
 
 import numpy as np
 import torch.multiprocessing as mp
+from tests.levels import limited_fleet
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -46,7 +47,6 @@ def _limited_worker(rank, world, port, out_dir):
     import torch.distributed as dist
 
     import oracle
-    from tests.test_greedy import limited_fleet
     from workload_variant_autoscaler_b200 import Allocs, parallel
     from workload_variant_autoscaler_b200._abi import ALLOC_COLUMNS, SAT_PRIORITY_ROUND_ROBIN
     os.environ["MASTER_ADDR"] = "127.0.0.1"
@@ -72,7 +72,6 @@ def _limited_worker(rank, world, port, out_dir):
 def test_two_rank_limited_mode_matches_single_greedy(tmp_path, oracle_mod):
     """Limited mode at world_size 2: candidates generated per shard, one all-gather of the candidate tables, the
     product's SolveGreedy (host C++) run redundantly on both ranks; both equal the oracle's single-process greedy."""
-    from tests.test_greedy import limited_fleet
     from workload_variant_autoscaler_b200._abi import SAT_PRIORITY_ROUND_ROBIN
     world = 2
     mp.spawn(_limited_worker, args=(world, _free_port(), str(tmp_path)), nprocs=world, join=True)
@@ -91,7 +90,6 @@ def test_two_rank_limited_mode_matches_single_greedy(tmp_path, oracle_mod):
 
 
 def test_sharded_unlimited_refuses_limited_fleet():
-    from tests.test_greedy import limited_fleet
     from workload_variant_autoscaler_b200 import parallel
     import pytest
     with pytest.raises(ValueError):

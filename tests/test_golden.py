@@ -6,11 +6,11 @@ import sys
 import numpy as np
 import pytest
 
-from tests.util import assert_allocs_equal, assert_f32_bits_equal
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden as mg  # noqa: E402
+from tests.util import assert_allocs_equal, assert_f32_bits_equal
 
 GOLD = np.load(os.path.join(HERE, "golden", "golden_r01.npz"))
 

@@ -1,8 +1,8 @@
 """The size grid, load grid, load intervals, sweep and streaming paths on adversarial fleets, and the queue-size rule.
 
-The fleets come from test_gpu_parity's _adversarial_fleet (coefficients over many decades or exactly 0, token counts
+The fleets come from levels._adversarial_fleet (coefficients over many decades or exactly 0, token counts
 0 / 1 / 100000, SLOs 0 / tiny / 1e7, loads from 1e-3 to 1e6 req/min), each path with a seed stream of its own.  The
-expected values are the oracle compositions the other test modules pin: ref_size_grid, ref_load_grid,
+expected values are the oracle compositions the other test modules pin: ref_size_grid, ref_grid,
 ref_intervals and the oracle's sweep and solve.  The load intervals are also checked without the monotonicity
 argument of DESIGN.md §3.10 that ref_intervals restates: a load grid over samples spread over every decade of each
 range must give every sample the key of the interval that contains it.
@@ -13,56 +13,21 @@ model with N above 2^20 (library) or K of 2^31 or more (both) is refused instead
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import pair_batch, rates_at_rate_star, ref_load_grid
-from tests.test_gpu_load_intervals import KEY_FIELDS, _bits, _f, load_pair, ref_intervals
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.test_gpu_size_grid import ref_size_grid
-from tests.test_gpu_table_cache import device_winners
+from tests.grid_cases import device_winners
+from tests.levels import (F32, KEY_FIELDS, QUEUE_CASES, _adversarial_fleet, _levels_to_rows, _rate_star_rates,
+                          from_bits, go_queue, load_grid_cases, load_pair, pair_batch, queue_fleet, ref_grid,
+                          ref_intervals, ref_size_grid, size_grid_cases, u32_bits)
 from tests.util import ALLOC_FIELDS, assert_allocs_equal, assert_f32_bits_equal
 from workload_variant_autoscaler_b200 import Grid, WvaError, _abi, synth_fleet
 
-F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-TINY_TOTAL = F32(60) * F32(2.0 ** -149)  # below this positive rate totalRate rounds to 0
 SWEEP_COLS = ("rate", "ttft", "itl", "throughput", "rho")
 
 
-def _same(a, b):
+def same_bytes(a, b):
     return np.ascontiguousarray(a).tobytes() == np.ascontiguousarray(b).tobytes()
 
 
-def _levels_to_rows(cols):
-    """[L, S] rows from one list of rates per server, each padded with its own last rate."""
-    L = max(1, max(len(c) for c in cols))
-    rows = np.zeros((L, len(cols)), np.float32)
-    for s, c in enumerate(cols):
-        if c:
-            rows[:, s] = c[-1]
-            rows[:len(c), s] = c
-    return rows
-
-
 # ---- size grid ---------------------------------------------------------------------------------------
-
-N_SIZE = 60
-
-
-def size_grid_cases():
-    """(fleet, batch list, rounds) per case: unsorted, repeated lists with 1 and 2, and every 15th case a long
-    batch size (1024 or 2049) with ratio 1 so that the oracle stays fast."""
-    rng = np.random.default_rng(0x51CE)
-    out = []
-    for case in range(N_SIZE):
-        fleet = _adversarial_fleet(rng, 20000 + case)
-        batches = [1, 2] + rng.integers(1, 65, int(rng.integers(0, 5))).tolist()
-        batches += [batches[int(rng.integers(0, len(batches)))]]  # a repeat
-        if case % 15 == 7:
-            batches.append(1024 if case % 30 == 7 else 2049)
-            fleet.max_queue_to_batch_ratio = 1
-        rng.shuffle(batches)
-        out.append((fleet, np.array(batches, np.int32), bool(case % 2)))
-    return out
-
 
 @pytest.mark.gpu
 def test_size_grid_adversarial(engine, oracle_mod, monkeypatch):
@@ -82,40 +47,6 @@ def test_size_grid_adversarial(engine, oracle_mod, monkeypatch):
 
 
 # ---- load grid ---------------------------------------------------------------------------------------
-
-N_LOAD = 60
-
-
-def _rate_star_rates(oracle_mod, fleet, s):
-    """rates_at_rate_star for every pair of server s that has a rateStar (the others have no such rates)."""
-    out = []
-    for a in range(fleet.n_acc):
-        if load_pair(oracle_mod, fleet, s, a) is None:
-            continue
-        try:
-            out += rates_at_rate_star(oracle_mod, fleet, s, a)
-        except AssertionError:  # no float32 rate lands exactly at 60 k rateStar (rateStar tiny or huge)
-            pass
-    return out
-
-
-def load_levels(oracle_mod, fleet):
-    """Per server: 0, -1, 1e-3, 0.5x, x, 2x, 1e3 x of its load, MaxFloat32, +Inf, and the rates at and one ulp
-    under 60 nrep rateStar (nrep = 1..3) of each of its pairs.  No NaN (test_nan_level_fails_as_analyze_does), and
-    no positive rate below 60 * 2^-149 (the header's min_replicas-0 case)."""
-    cols = []
-    for s in range(fleet.n_servers):
-        x = F32(fleet.srv_arrival_rpm[s])
-        lv = [F32(0), F32(-1), F32(1e-3), x * F32(0.5), x, x * F32(2), x * F32(1e3), F32_MAX, F32(np.inf)]
-        lv += [F32(r) for r in _rate_star_rates(oracle_mod, fleet, s)]
-        cols.append([v for v in lv if not (0 < v < TINY_TOTAL)])
-    return _levels_to_rows(cols)
-
-
-def load_grid_cases(oracle_mod):
-    rng = np.random.default_rng(0x10AD)
-    return [(f, load_levels(oracle_mod, f)) for f in (_adversarial_fleet(rng, 30000 + c) for c in range(N_LOAD))]
-
 
 @pytest.fixture(scope="module")
 def load_cases(oracle_mod):
@@ -141,7 +72,7 @@ def test_load_grid_adversarial(engine, oracle_mod, monkeypatch, load_cases):
             monkeypatch.setenv("WVA_SIZE_SMALL_MAX", "0")
         else:
             monkeypatch.delenv("WVA_SIZE_SMALL_MAX", raising=False)
-        cand_o, win_o = ref_load_grid(oracle_mod, fleet, rpm)
+        cand_o, win_o = ref_grid(oracle_mod, fleet, {"arrival_rpm": rpm})
         cand_g, win_g = engine.load_grid(fleet, rpm, want_candidates=True)
         assert_allocs_equal(cand_g, cand_o, f"load grid, case {case}: candidates")
         assert_allocs_equal(win_g, win_o, f"load grid, case {case}: winners")
@@ -231,12 +162,12 @@ def test_load_intervals_adversarial(engine, interval_cases):
             what = f"intervals, case {case}, M = {M}"
             assert np.array_equal(count, count_o), f"{what}: count {count} vs {count_o}"
             assert np.array_equal(trunc, trunc_o), f"{what}: truncated {trunc} vs {trunc_o}"
-            assert _same(start, start_o), f"{what}: start_rpm"
+            assert same_bytes(start, start_o), f"{what}: start_rpm"
             assert_allocs_equal(rec, rec_o, f"{what}: records")
 
 
 def _key(win, i):
-    return tuple(_bits(getattr(win, k)[i]) if k in ("cost", "value", "max_rate") else int(getattr(win, k)[i])
+    return tuple(u32_bits(getattr(win, k)[i]) if k in ("cost", "value", "max_rate") else int(getattr(win, k)[i])
                  for k in KEY_FIELDS)
 
 
@@ -254,8 +185,8 @@ def test_load_intervals_against_sampled_load_grid(engine, oracle_mod, interval_c
         for s in range(S):
             n = int(count[s])
             st = [F32(v) for v in start[s, :n]]
-            b_lo, b_hi = _bits(lo[s]), _bits(hi[s])
-            pts = [_f(int(b)) for b in rng.integers(b_lo, b_hi + 1, 256)]
+            b_lo, b_hi = u32_bits(lo[s]), u32_bits(hi[s])
+            pts = [from_bits(int(b)) for b in rng.integers(b_lo, b_hi + 1, 256)]
             for x in st:
                 pts += [x, np.nextafter(x, F32(-np.inf)), np.nextafter(x, F32(np.inf))]
             pts = [p for p in pts if lo[s] <= p <= hi[s]]
@@ -276,11 +207,11 @@ def test_load_intervals_against_sampled_load_grid(engine, oracle_mod, interval_c
                 assert _key(win, i) == _key(rec, s * M + j), (case, s, float(p), j)
                 if p == start[s, j]:
                     for k in ALLOC_FIELDS:
-                        assert _same(getattr(win, k)[i:i + 1], getattr(rec, k)[s * M + j:s * M + j + 1]), (case, s, j, k)
+                        assert same_bytes(getattr(win, k)[i:i + 1], getattr(rec, k)[s * M + j:s * M + j + 1]), (case, s, j, k)
                 checked += 1
         # a random subset of the load-grid winners against the oracle
         pick = np.sort(rng.choice(rows.shape[0], min(64, rows.shape[0]), replace=False))
-        _, win_o = ref_load_grid(oracle_mod, fleet, rows[pick])
+        _, win_o = ref_grid(oracle_mod, fleet, {"arrival_rpm": rows[pick]})
         idx = (pick[:, None] * S + np.arange(S)[None, :]).reshape(-1)
         for k in ALLOC_FIELDS:
             got = getattr(win, k)[idx]
@@ -458,37 +389,17 @@ def test_streaming_adversarial(engine, oracle_mod, unlimited):
             engine.synchronize()
             dev = _device_block_columns(blk, S)
             for k in ALLOC_FIELDS:
-                assert _same(dev[k], getattr(win_g, k)), f"{what}: resolve_device {k}"
+                assert same_bytes(dev[k], getattr(win_g, k)), f"{what}: resolve_device {k}"
     assert feasible > 100
 
 
 # ---- the queue-size rule -----------------------------------------------------------------------------
-
-def go_queue(perf_max_batch, at_tokens, out_tokens, srv_max_batch, ratio):
-    """(N, K) of a load pair as Go computes them, in 64-bit int (allocation.go:77-93)."""
-    i64 = np.int64
-    if srv_max_batch > 0:
-        N = i64(srv_max_batch)
-    else:
-        N = max(i64(perf_max_batch) * i64(at_tokens) // i64(out_tokens), i64(1))
-    return N, N + N * i64(ratio)
-
 
 def _wrap32(x):
     return int(np.array([x], np.int64).astype(np.int32)[0])
 
 
 # (name, perf_max_batch, at_tokens, out_tokens, srv_max_batch, ratio, refused by the library)
-QUEUE_CASES = [
-    ("at_tokens_wrap", 65536, 65537, 1, 0, 10, True),       # N = 4,295,032,832: int32 sees 65536
-    ("ratio_wrap", 8, 512, 1, 4, 1 << 30, True),            # K = 2^32 + 4: int32 sees 4
-    ("n_2p20", 1024, 1024, 1, 0, 10, False),                # N = 2^20: the largest batch size
-    ("n_above_2p20", 1025, 1024, 1, 0, 10, True),           # N = 2^20 + 1024
-    ("k_just_below_2p31", 8, 512, 1, 1 << 20, 2046, False),  # K = 2^31 - 2^20
-    ("k_2p31", 8, 512, 1, 1 << 20, 2047, True),             # K = 2^31 exactly
-]
-
-
 def test_queue_cases_sit_where_they_are_meant_to():
     for name, pmb, at, out, smb, ratio, refused in QUEUE_CASES:
         N, K = go_queue(pmb, at, out, smb, ratio)
@@ -503,21 +414,6 @@ def test_queue_cases_sit_where_they_are_meant_to():
             assert K == (1 << 31) - (1 << 20)
         if name == "k_2p31":
             assert K == (1 << 31) and _wrap32(K) < 0
-
-
-def queue_fleet(name, n_servers=3):
-    """A small fleet whose server 0 carries the named case of QUEUE_CASES on every accelerator (the others
-    ordinary; ratio applies to all)."""
-    _, pmb, at, out, smb, ratio, _ = next(c for c in QUEUE_CASES if c[0] == name)
-    f = synth_fleet(n_servers, 2, seed=7, server_batch=False, zero_load_frac=0.0, tps_frac=0.0,
-                    max_batch_choices=(4, 8, 16))
-    m = int(f.srv_model[0])
-    f.perf_max_batch[m, :] = pmb
-    f.perf_at_tokens[m, :] = at
-    f.srv_out_tokens[0] = out
-    f.srv_max_batch[0] = smb
-    f.max_queue_to_batch_ratio = ratio
-    return f
 
 
 @pytest.mark.parametrize("name", ["at_tokens_wrap", "ratio_wrap"])
@@ -619,7 +515,7 @@ def test_zero_load_pair_outside_int32_is_not_refused(engine, oracle_mod):
     assert_allocs_equal(win_g, win_o, "winners")
     assert int(np.asarray(cand_g.batch)[0]) == 65536
     rpm = np.stack([f.srv_arrival_rpm, f.srv_arrival_rpm * F32(3)]).astype(np.float32)
-    cand_o, win_o = ref_load_grid(oracle_mod, f, rpm)
+    cand_o, win_o = ref_grid(oracle_mod, f, {"arrival_rpm": rpm})
     cand_g, win_g = engine.load_grid(f, rpm, want_candidates=True)
     assert_allocs_equal(cand_g, cand_o, "load-grid candidates")
     assert_allocs_equal(win_g, win_o, "load-grid winners")
@@ -627,7 +523,7 @@ def test_zero_load_pair_outside_int32_is_not_refused(engine, oracle_mod):
     hi = (f.srv_arrival_rpm * F32(1.1)).astype(np.float32)
     count_o, trunc_o, start_o, rec_o, _ = ref_intervals(oracle_mod, f, lo, hi, 16)
     count, trunc, start, rec = engine.load_intervals(f, lo, hi, 16)
-    assert np.array_equal(count, count_o) and np.array_equal(trunc, trunc_o) and _same(start, start_o)
+    assert np.array_equal(count, count_o) and np.array_equal(trunc, trunc_o) and same_bytes(start, start_o)
     assert_allocs_equal(rec, rec_o, "interval records")
     engine.upload(f)
     _, win_r = engine.resolve()

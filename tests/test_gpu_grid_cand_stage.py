@@ -13,7 +13,7 @@ import functools
 
 import pytest
 
-from tests.test_gpu_grid_shapes import STAGE_B, _batches, _three_ways, shape_fleet, winner_mix
+from tests.grid_cases import STAGE_B, _batches, _three_ways, shape_fleet, winner_mix
 from workload_variant_autoscaler_b200 import Grid, config2_grid
 
 STAGE_CAP = 16384  # kCandStageBytes

@@ -18,10 +18,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_grid_pruning import _check, _same_winners
-from tests.test_gpu_grid_shapes import (INV_BATCH, INV_REPLICAS, _analyzer_of, _lambda, _three_ways, cell_shares_row,
-                                        invariant_fleet, shape_fleet)
-from tests.test_gpu_windows import chain_profile
+from tests.grid_cases import (INV_BATCH, INV_REPLICAS, _analyzer_of, _lambda, _same_winners, _three_ways,
+                              cell_shares_row, chain_profile, check_pruning, invariant_fleet, shape_fleet)
 from workload_variant_autoscaler_b200 import Grid, config2_grid, synth_fleet
 
 CHUNK = 4096
@@ -161,7 +159,7 @@ def test_gates_case_has_cells_only_grid_kernel_stores(oracle_mod):
 @pytest.mark.parametrize("case", [tied_repeated_case, gates_case, k_limit_case], ids=lambda c: c.__name__)
 def test_candidate_intervals_against_oracle(engine, oracle_mod, case):
     fleet, grid = case()
-    _check(engine, oracle_mod, fleet, grid, case.__name__)
+    check_pruning(engine, oracle_mod, fleet, grid, case.__name__)
 
 
 @pytest.mark.gpu
@@ -182,7 +180,7 @@ def test_one_server_several_chunks_per_pair(engine, oracle_mod):
     _, win_p = engine.grid_solve(fleet, grid)
     n, chunks = _listed(engine)
     assert n > 2 * CHUNK and chunks >= 3, (n, chunks)  # two pairs: one of them has two chunks
-    _check(engine, oracle_mod, fleet, grid, "one server, several chunks per pair")
+    check_pruning(engine, oracle_mod, fleet, grid, "one server, several chunks per pair")
 
 
 @pytest.mark.gpu

@@ -19,8 +19,7 @@ import functools
 import numpy as np
 import pytest
 
-from tests.test_gpu_grid_shapes import _three_ways, shape_fleet
-from tests.test_gpu_table_cache import device_winners
+from tests.grid_cases import _cells_equal, _three_ways, device_winners, shape_fleet
 from tests.util import assert_allocs_equal
 from workload_variant_autoscaler_b200 import Grid
 
@@ -104,7 +103,6 @@ def test_back_to_back_steps(engine, oracle_mod):
     want[5] = (f2, g2)
     engine.synchronize()
 
-    from tests.test_gpu_windows import _cells_equal
     cells_o, win_o = oracle_mod.grid_solve(f2, g2, want_cells=True)
     _cells_equal(cells_g, cells_o, "cell-table call between device steps")
     assert_allocs_equal(win_c, win_o, "cell-table call between device steps: winners")

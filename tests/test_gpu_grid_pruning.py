@@ -11,29 +11,13 @@ import os
 import numpy as np
 import pytest
 
-from tests.util import assert_allocs_equal
+from tests.grid_cases import _same_winners, check_pruning
+from tests.util import ALLOC_FIELDS
 from workload_variant_autoscaler_b200 import Grid, config2_grid, synth_fleet
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "grid_winners_config2.npz")
-COLUMNS = ("feasible", "acc", "replicas", "batch", "cost", "value", "itl", "ttft", "rho", "max_rate")
-
-
-def _same_winners(a, b, what):
-    for f in COLUMNS:
-        x, y = np.asarray(getattr(a, f)), np.asarray(getattr(b, f))
-        assert x.dtype == y.dtype and np.array_equal(x.view(np.uint8), y.view(np.uint8)), f"{what}: field {f}"
-
-
-def _check(engine, oracle_mod, fleet, grid, what):
-    _, win_o = oracle_mod.grid_solve(fleet, grid, want_cells=False)
-    _, win_p = engine.grid_solve(fleet, grid)
-    _, win_c = engine.grid_solve(fleet, grid, want_cells=True)
-    assert_allocs_equal(win_p, win_o, what + " (pruned)")
-    _same_winners(win_p, win_c, what + ": pruned vs cell table")
-
-
 @pytest.mark.parametrize("seed", range(42, 50))
 def test_pruned_winners_at_bench_size(engine, seed):
     fleet, grid = synth_fleet(100, 4, seed=seed), config2_grid()
@@ -41,7 +25,7 @@ def test_pruned_winners_at_bench_size(engine, seed):
     _, win_c = engine.grid_solve(fleet, grid, want_cells=True)
     _same_winners(win_p, win_c, f"seed {seed}")
     ref = np.load(GOLDEN)
-    for f in COLUMNS:
+    for f in ALLOC_FIELDS:
         want = ref[f"s{seed}_{f}"]
         got = np.asarray(getattr(win_p, f))
         assert np.array_equal(got.astype(want.dtype).view(np.uint8), want.view(np.uint8)), f"seed {seed}: field {f}"
@@ -56,7 +40,7 @@ def test_tied_rows_across_accelerators(engine, oracle_mod):
     fleet.srv_cur_acc[:] = -1
     fleet.srv_cur_replicas[:] = 0
     fleet.srv_cur_cost[:] = 0.0
-    _check(engine, oracle_mod, fleet, Grid([1, 2, 4, 8, 16, 32, 64, 128], np.arange(1, 25)), "tied rows")
+    check_pruning(engine, oracle_mod, fleet, Grid([1, 2, 4, 8, 16, 32, 64, 128], np.arange(1, 25)), "tied rows")
 
 
 def test_repeated_unsorted_batches_and_current_allocations(engine, oracle_mod):
@@ -67,8 +51,8 @@ def test_repeated_unsorted_batches_and_current_allocations(engine, oracle_mod):
     fleet.srv_cur_replicas[:] = 1 + np.arange(16) % 5
     fleet.srv_cur_cost[:] = np.float32(5000.0)
     batch = np.array([64, 3, 17, 3, 128, 1, 64, 9, 255, 2, 17, 40])
-    _check(engine, oracle_mod, fleet, Grid(batch, np.arange(1, 31)), "repeated batches, value <= 0")
-    _check(engine, oracle_mod, fleet, Grid(batch[::-1], np.arange(30, 0, -1)), "reversed lists")
+    check_pruning(engine, oracle_mod, fleet, Grid(batch, np.arange(1, 31)), "repeated batches, value <= 0")
+    check_pruning(engine, oracle_mod, fleet, Grid(batch[::-1], np.arange(30, 0, -1)), "reversed lists")
 
 
 def test_no_feasible_shared_cell_tps_and_itl_gates(engine, oracle_mod):
@@ -79,7 +63,7 @@ def test_no_feasible_shared_cell_tps_and_itl_gates(engine, oracle_mod):
     cells_o, _ = oracle_mod.grid_solve(fleet, Grid(np.arange(1, 97), np.arange(1, 41)))
     feas = ((cells_o["flags"] >> 1) & 1).reshape(14, -1).any(axis=1)
     assert not feas[[0, 5, 9]].any() and feas.sum() >= 3
-    _check(engine, oracle_mod, fleet, Grid(np.arange(1, 97), np.arange(1, 41)), "ITL / TPS gates")
+    check_pruning(engine, oracle_mod, fleet, Grid(np.arange(1, 97), np.arange(1, 41)), "ITL / TPS gates")
 
 
 def test_cells_beyond_two_pow_23_next_to_shared_runs(engine, oracle_mod):
@@ -87,7 +71,7 @@ def test_cells_beyond_two_pow_23_next_to_shared_runs(engine, oracle_mod):
     fleet = synth_fleet(4, 2, seed=41, zero_load_frac=0.0, tps_frac=0.0, max_batch_choices=(64,))
     fleet.srv_arrival_rpm[:] = np.float32([30.0, 600.0, 120.0, 2400.0])
     fleet.max_queue_to_batch_ratio = 4000
-    _check(engine, oracle_mod, fleet, Grid([1, 2, 50, 2000, 2097, 2100], [1, 2, 3, 5]), "K >= 2^23")
+    check_pruning(engine, oracle_mod, fleet, Grid([1, 2, 50, 2000, 2097, 2100], [1, 2, 3, 5]), "K >= 2^23")
 
 
 def test_nan_value_turns_pruning_off(engine):

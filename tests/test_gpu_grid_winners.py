@@ -8,7 +8,7 @@ grid_solve(want_cells=False), plus grids built to reach the walk's edge cases.
 import numpy as np
 import pytest
 
-from tests.test_gpu_parity import _adversarial_fleet
+from tests.levels import _adversarial_fleet
 from tests.util import assert_allocs_equal
 from workload_variant_autoscaler_b200 import Grid, synth_fleet
 

@@ -3,7 +3,7 @@
 The expected intervals come from ref_intervals, a Python composition over the CPU oracle: one Analyzer.size per
 pair gives rateStar and RateRange.Max; each load pair's state (replica count, Analyze's rate check) is stepped
 through the range by float32 bit bisection with the arithmetic of the load-grid test's `tail`; the union of the
-step points is then evaluated with the oracle's Server.Calculate + Solver.Solve (ref_load_grid), and an interval
+step points is then evaluated with the oracle's Server.Calculate + Solver.Solve (ref_grid), and an interval
 starts wherever the winner's decision key changes.  The CPU tests pin that composition against the oracle at the
 starts, one ulp below them, at the steps that start nothing and at random interior points; the GPU tests compare
 the CUDA path with it, and with wva_load_grid, bit for bit."""
@@ -12,155 +12,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.util import assert_allocs_equal
-from tests.test_gpu_load_grid import (at_level, go_f64_to_int, mixed_fleet, overflow_fleet, pair_batch,
-                                      rates_at_rate_star, ref_load_grid, tail)
+from tests.levels import (F32, KEY_FIELDS, TINY, at_row, check_intervals, from_bits, load_pair, mixed_fleet,
+                          overflow_fleet, pair_state, rates_at_rate_star, rec_key, ref_intervals, u32_bits, winners_at)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
+                        same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, synth_fleet
 
-F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-TINY = F32(np.nextafter(F32(0), F32(1)))
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-ALLOC_FIELDS = ("feasible", "acc", "replicas", "batch", "cost", "value", "itl", "ttft", "rho", "max_rate")
-KEY_FIELDS = ("feasible", "acc", "replicas", "batch", "cost", "value", "max_rate")
-INT32_MAX = 2147483647
-
-
-def _bits(x):
-    return int(np.array([x], np.float32).view(np.uint32)[0])
-
-
-def _f(bits):
-    return F32(np.array([bits], np.uint32).view(np.float32)[0])
-
-
-def rec_key(r):
-    return tuple(_bits(r[k]) if k in ("cost", "value", "max_rate") else int(r[k]) for k in KEY_FIELDS)
-
-
 # ---- the oracle composition ---------------------------------------------------------------------
-
-def load_pair(oracle_mod, fleet, s, a):
-    """(rateStar, RateRange.Max) of a pair whose key reads the load above rate 0, else None: the gates of
-    CreateAllocation, the candidate rule, a TPS target (totalRate does not read the load) and a failed Size."""
-    m = int(fleet.srv_model[s])
-    if fleet.srv_keep_acc[s] and fleet.srv_cur_acc[s] != -1 and fleet.srv_cur_acc[s] != a:
-        return None
-    if m < 0 or m >= fleet.n_models or not fleet.perf_present[m, a] or not fleet.srv_has_target[s]:
-        return None
-    if fleet.srv_in_tokens[s] < 0 or fleet.srv_out_tokens[s] <= 0 or fleet.srv_slo_tps[s] != 0:
-        return None
-    N = pair_batch(fleet, s, a)
-    try:
-        qa = oracle_mod.Analyzer(N, N * fleet.max_queue_to_batch_ratio, float(fleet.perf_alpha[m, a]),
-                                 float(fleet.perf_beta[m, a]), float(fleet.perf_gamma[m, a]),
-                                 float(fleet.perf_delta[m, a]), int(fleet.srv_in_tokens[s]),
-                                 int(fleet.srv_out_tokens[s]))
-    except ValueError:
-        return None
-    err, _, met, _ = qa.size(float(fleet.srv_slo_ttft[s]), float(fleet.srv_slo_itl[s]), float(fleet.srv_slo_tps[s]))
-    if err:
-        return None
-    return F32(met["throughput"]), F32(qa.rate_range()[1]), qa, N
-
-
-def pair_state(fleet, s, rate_star, rmax, rpm):
-    """(replicas, gate, over) at rpm > 0 with `tail`'s arithmetic: gate 0 = the final rate is not positive, 1 =
-    Analyze accepts it, 2 = above RateRange.Max; over = more than INT32_MAX replicas."""
-    with np.errstate(all="ignore"):
-        total = F32(rpm) / F32(60)
-        q = np.ceil(np.float64(total) / np.float64(rate_star))
-        over = not (q <= INT32_MAX)
-        nrep = max(go_f64_to_int(q), int(fleet.srv_min_replicas[s]))
-        rate = total / np.array([nrep], np.int64).astype(F32)[0]
-    ok = not (rate <= 0 or rate > rmax)
-    return nrep, (1 if ok else (0 if rate <= 0 else 2)), over
-
-
-def next_step(fleet, s, rate_star, rmax, x, hi):
-    """The smallest float32 in (x, hi] whose state differs from x's (None: none)."""
-    at = pair_state(fleet, s, rate_star, rmax, x)
-    lo_b, hi_b = _bits(x), _bits(hi)
-    if hi_b <= lo_b or pair_state(fleet, s, rate_star, rmax, _f(hi_b)) == at:
-        return None
-    while hi_b - lo_b > 1:
-        mid = (lo_b + hi_b) // 2
-        if pair_state(fleet, s, rate_star, rmax, _f(mid)) != at:
-            hi_b = mid
-        else:
-            lo_b = mid
-    return _f(hi_b)
-
-
-def server_steps(oracle_mod, fleet, s, lo, hi):
-    """(the points to evaluate in [lo, hi], the first rate at which a pair overflows or None)."""
-    pts = {F32(lo)}
-    lo_pos = F32(lo) if lo > 0 else TINY
-    if lo == 0 and hi > 0:
-        pts.add(TINY)
-    over_at = None
-    for a in range(fleet.n_acc):
-        p = load_pair(oracle_mod, fleet, s, a) if hi > 0 else None
-        if p is None:
-            continue
-        rs, rmax = p[0], p[1]
-        x = lo_pos
-        if pair_state(fleet, s, rs, rmax, x)[2]:
-            over_at = x if over_at is None else min(over_at, x)
-            continue
-        while True:
-            y = next_step(fleet, s, rs, rmax, x, F32(hi))
-            if y is None:
-                break
-            if pair_state(fleet, s, rs, rmax, y)[2]:
-                over_at = y if over_at is None else min(over_at, y)
-                break
-            pts.add(y)
-            x = y
-    pts = sorted(p for p in pts if over_at is None or p < over_at)
-    return pts, over_at
-
-
-def winners_at(oracle_mod, fleet, points):
-    """The oracle's unlimited winner of server s at each rate of points[s] (a list per server)."""
-    S = fleet.n_servers
-    L = max(1, max(len(p) for p in points))
-    rows = np.zeros((L, S), np.float32)
-    for s, p in enumerate(points):
-        if p:
-            rows[:, s] = p[-1]
-            rows[:len(p), s] = p
-    _, win = ref_load_grid(oracle_mod, fleet, rows)
-    win = win.reshape(L, S)
-    return [[win[l, s] for l in range(len(p))] for s, p in enumerate(points)]
-
-
-def ref_intervals(oracle_mod, fleet, lo, hi, M):
-    """(count [S], truncated [S], start (S, M), records [S*M], the step points of each server)."""
-    S = fleet.n_servers
-    count = np.zeros(S, np.int32)
-    trunc = np.zeros(S, np.uint8)
-    start = np.zeros((S, M), np.float32)
-    rec = np.zeros(S * M, oracle_mod.ALLOC_DTYPE)
-    steps = [server_steps(oracle_mod, fleet, s, lo[s], hi[s]) for s in range(S)]
-    wins = winners_at(oracle_mod, fleet, [p for p, _ in steps])
-    for s in range(S):
-        pts, over_at = steps[s]
-        trunc[s] = over_at is not None
-        prev = None
-        for x, w in zip(pts, wins[s]):
-            k = rec_key(w)
-            if k == prev:
-                continue
-            if count[s] == M:
-                trunc[s] = 1
-                break
-            start[s, count[s]] = x
-            rec[s * M + count[s]] = w
-            count[s] += 1
-            prev = k
-    return count, trunc, start, rec, [p for p, _ in steps]
-
 
 def ranges(fleet, seed):
     """[0.5x, 2x] of each server's load, with lo = hi on one loaded server and lo = 0 on another."""
@@ -173,10 +31,6 @@ def ranges(fleet, seed):
     lo[i] = hi[i] = x[i]
     lo[j] = 0
     return lo, hi
-
-
-def _same(a, b):
-    return np.ascontiguousarray(a).tobytes() == np.ascontiguousarray(b).tobytes()
 
 
 # ---- CPU: the composition against the oracle ----------------------------------------------------
@@ -224,7 +78,7 @@ def test_truncation_at_M_and_lo_equal_hi(oracle_mod):
     for s in range(fleet.n_servers):
         assert count[s] == min(M, full[0][s])
         assert trunc[s] == (full[0][s] > M)
-        assert _same(start[s], full[2][s, :M])
+        assert same_bytes(start[s], full[2][s, :M])
         if lo[s] == hi[s]:
             assert count[s] == 1
     assert trunc.any()
@@ -237,21 +91,11 @@ def test_tail_at_a_tiny_rate_is_zero_replicas(oracle_mod):
     fleet.srv_min_replicas[:] = 0
     for rpm in (TINY, F32(4.2e-44)):
         assert F32(rpm) / F32(60) == 0
-        cand = oracle_mod.calculate(at_level(fleet, np.full(3, rpm, np.float32))).reshape(-1)
+        cand = oracle_mod.calculate(at_row(fleet, {"arrival_rpm": [np.full(3, rpm, np.float32)]}, 0)).reshape(-1)
         assert (cand["feasible"] == 1).all() and (cand["replicas"] == 0).all() and (cand["cost"] == 0).all()
 
 
 # ---- GPU: bit for bit -------------------------------------------------------------------------------
-
-def _check(engine, oracle_mod, fleet, lo, hi, M, what):
-    count_o, trunc_o, start_o, rec_o, _ = ref_intervals(oracle_mod, fleet, lo, hi, M)
-    count, trunc, start, rec = engine.load_intervals(fleet, lo, hi, M)
-    assert np.array_equal(count, count_o), f"{what}: count {count} vs {count_o}"
-    assert np.array_equal(trunc, trunc_o), f"{what}: truncated {trunc} vs {trunc_o}"
-    assert _same(start, start_o), f"{what}: start_rpm"
-    assert_allocs_equal(rec, rec_o, f"{what}: records")
-    return count_o, trunc_o
-
 
 def cross_check_load_grid(engine, fleet, lo, hi, M, seed, max_levels=None):
     """One wva_load_grid over every start, every start's predecessor and random interior points reproduces the
@@ -260,7 +104,7 @@ def cross_check_load_grid(engine, fleet, lo, hi, M, seed, max_levels=None):
     S = fleet.n_servers
     rng = np.random.default_rng(seed)
     pts, want = [[] for _ in range(S)], [[] for _ in range(S)]
-    keys = [[tuple(_bits(getattr(rec, k)[s * M + j]) if k in ("cost", "value", "max_rate")
+    keys = [[tuple(u32_bits(getattr(rec, k)[s * M + j]) if k in ("cost", "value", "max_rate")
                    else int(getattr(rec, k)[s * M + j]) for k in KEY_FIELDS) for j in range(count[s])] for s in range(S)]
     for s in range(S):
         n = int(count[s])
@@ -288,9 +132,9 @@ def cross_check_load_grid(engine, fleet, lo, hi, M, seed, max_levels=None):
             i = l * S + s
             if kind == "start":
                 for k in ALLOC_FIELDS:
-                    assert _same(getattr(win, k)[i:i + 1], getattr(rec, k)[s * M + j:s * M + j + 1]), (s, j, k)
+                    assert same_bytes(getattr(win, k)[i:i + 1], getattr(rec, k)[s * M + j:s * M + j + 1]), (s, j, k)
             else:
-                got = tuple(_bits(getattr(win, k)[i]) if k in ("cost", "value", "max_rate") else int(getattr(win, k)[i])
+                got = tuple(u32_bits(getattr(win, k)[i]) if k in ("cost", "value", "max_rate") else int(getattr(win, k)[i])
                             for k in KEY_FIELDS)
                 assert got == keys[s][j], (s, j, v)
     return int(count.sum())
@@ -304,7 +148,7 @@ def test_small_fleet(engine, oracle_mod, monkeypatch, keep, rounds):
         monkeypatch.setenv("WVA_SIZE_SMALL_MAX", "0")
     fleet = mixed_fleet(14, 3, 31, keep)
     lo, hi = ranges(fleet, 7)
-    count, _ = _check(engine, oracle_mod, fleet, lo, hi, 64, f"small, keep = {keep}, rounds = {rounds}")
+    count, _ = check_intervals(engine, oracle_mod, fleet, lo, hi, 64, f"small, keep = {keep}, rounds = {rounds}")
     assert count.max() >= 4
     cross_check_load_grid(engine, fleet, lo, hi, 64, 1)
 
@@ -325,7 +169,7 @@ def test_rounds_every_tree_depth(engine, rounds_case, monkeypatch, depth):
     fleet, lo, hi, (count_o, trunc_o, start_o, rec_o, _) = rounds_case
     count, trunc, start, rec = engine.load_intervals(fleet, lo, hi, 32)
     assert np.array_equal(count, count_o) and np.array_equal(trunc, trunc_o)
-    assert _same(start, start_o)
+    assert same_bytes(start, start_o)
     assert_allocs_equal(rec, rec_o, f"D = {depth}: records")
 
 
@@ -342,16 +186,16 @@ def test_configs3_shape_against_the_load_grid(engine):
 def test_many_accelerators(engine, oracle_mod, n_acc):
     fleet = mixed_fleet(6, n_acc, 43, False)
     lo, hi = ranges(fleet, 13)
-    _check(engine, oracle_mod, fleet, lo, hi, 64, f"A = {n_acc}")
+    check_intervals(engine, oracle_mod, fleet, lo, hi, 64, f"A = {n_acc}")
 
 
 @pytest.mark.gpu
 def test_M_one_and_tight_M(engine, oracle_mod):
     fleet = mixed_fleet(12, 3, 71, False)
     lo, hi = ranges(fleet, 5)
-    count, trunc = _check(engine, oracle_mod, fleet, lo, hi, 1, "M = 1")
+    count, trunc = check_intervals(engine, oracle_mod, fleet, lo, hi, 1, "M = 1")
     assert (count[hi > 0] == 1).all() and trunc.any()
-    count, trunc = _check(engine, oracle_mod, fleet, lo, hi, 3, "M = 3")
+    count, trunc = check_intervals(engine, oracle_mod, fleet, lo, hi, 3, "M = 3")
     assert trunc.any()
 
 
@@ -361,19 +205,19 @@ def test_replica_overflow_stops_the_list(engine, oracle_mod):
     s, a = 0, 0
     rs, rmax, _, _ = load_pair(oracle_mod, fleet, s, a)
     # the first rate at which ceil(totalRate / rateStar) exceeds INT32_MAX, found on the oracle's rateStar
-    lo_b, hi_b = _bits(F32(1)), _bits(F32_MAX)
+    lo_b, hi_b = u32_bits(F32(1)), u32_bits(F32_MAX)
     while hi_b - lo_b > 1:
         m = (lo_b + hi_b) // 2
-        if pair_state(fleet, s, rs, rmax, _f(m))[2]:
+        if pair_state(fleet, s, rs, rmax, from_bits(m))[2]:
             hi_b = m
         else:
             lo_b = m
-    over = _f(hi_b)
+    over = from_bits(hi_b)
     lo = fleet.srv_arrival_rpm.astype(np.float32).copy()
     hi = lo.copy()
-    lo[s] = _f(hi_b - 6)
-    hi[s] = _f(hi_b + 6)
-    count, trunc = _check(engine, oracle_mod, fleet, lo, hi, 64, "overflow")
+    lo[s] = from_bits(hi_b - 6)
+    hi[s] = from_bits(hi_b + 6)
+    count, trunc = check_intervals(engine, oracle_mod, fleet, lo, hi, 64, "overflow")
     _, _, start, _ = engine.load_intervals(fleet, lo, hi, 64)
     assert trunc[s] == 1 and 1 <= count[s] <= 6 and start[s, count[s] - 1] < over
     lo[s] = over  # overflow at rpm_lo itself: nothing is written
@@ -391,7 +235,7 @@ def test_nan_and_huge_values_and_ties(engine, oracle_mod):
     for k in ("perf_beta", "perf_gamma", "perf_delta", "perf_acc_count"):
         getattr(fleet, k)[:, 2] = getattr(fleet, k)[:, 1]
     lo, hi = ranges(fleet, 17)
-    _check(engine, oracle_mod, fleet, lo, hi, 64, "NaN / huge values and ties")
+    check_intervals(engine, oracle_mod, fleet, lo, hi, 64, "NaN / huge values and ties")
 
 
 @pytest.mark.gpu
@@ -401,7 +245,7 @@ def test_stored_vector_fallback_at_the_starts(engine, oracle_mod):
     fleet = base.take_servers(np.zeros(len(rates), np.int64))
     lo = np.array(rates, np.float32)
     hi = np.array([np.nextafter(F32(r), F32(np.inf)) for r in rates], np.float32)
-    count, _ = _check(engine, oracle_mod, fleet, lo, hi, 4, "stored-vector fallback")
+    count, _ = check_intervals(engine, oracle_mod, fleet, lo, hi, 4, "stored-vector fallback")
     assert count.sum() >= len(rates)
     cross_check_load_grid(engine, fleet, lo, hi, 4, 3)
 
@@ -415,7 +259,7 @@ def test_tiny_rates_where_total_rate_underflows(engine, oracle_mod):
     fleet.srv_min_replicas[:] = np.maximum(fleet.srv_min_replicas, 1)
     lo = np.array([0, TINY, 0, 0], np.float32)
     hi = np.array([1e-40, 1e-42, 1e-40, 5.0], np.float32)
-    _check(engine, oracle_mod, fleet, lo, hi, 16, "tiny rates")
+    check_intervals(engine, oracle_mod, fleet, lo, hi, 16, "tiny rates")
     count, _, start, rec = engine.load_intervals(fleet, lo, hi, 16)
     # server 0: rate 0, then nil while totalRate is 0, then feasible
     assert count[0] >= 3 and start[0, 1] == TINY and rec.feasible[1] == 0 and rec.feasible[2] == 1
@@ -480,9 +324,9 @@ def test_cache_interplay_on_one_handle(engine):
             for x, y in zip(call(engine), call(fresh)):
                 if isinstance(x, Allocs):
                     for k in ALLOC_FIELDS:
-                        assert _same(getattr(x, k), getattr(y, k)), f"{what}: {k}"
+                        assert same_bytes(getattr(x, k), getattr(y, k)), f"{what}: {k}"
                 elif x is not None:
-                    assert _same(x, y), what
+                    assert same_bytes(x, y), what
 
         solve = lambda e: e.solve(fleet)  # noqa: E731
         size_grid = lambda e: e.size_grid(fleet, [4, 16, 64], want_candidates=True)  # noqa: E731

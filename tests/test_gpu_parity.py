@@ -7,6 +7,7 @@ float32 ulp is 6e-8, so the bar actually enforced is bit-exactness).
 import numpy as np
 import pytest
 
+from tests.levels import ACC_CM, SC_CM, _adversarial_fleet, _va
 from tests.util import assert_allocs_equal, assert_f32_bits_equal
 from workload_variant_autoscaler_b200 import Grid, synth_fleet
 
@@ -318,7 +319,6 @@ def test_reference_flow_from_kubernetes_objects(engine, oracle_mod):
     """SURVEY.md 8f ranks 1 + 3 around the CUDA path: ConfigMaps + VariantAutoscalings (the reference's
     optimizer_test.go fixture, with load on two variants) -> adapters -> fleet -> wva_solve -> AllocationSolution ->
     optimized allocs; identical to the same flow through the oracle."""
-    from tests.test_adapters import ACC_CM, SC_CM, _va
     from workload_variant_autoscaler_b200 import Fleet, adapters
     sd = adapters.create_system_data(ACC_CM, SC_CM)
     vas = [_va(1), _va(2, arrival="600.0", replicas=2), _va(3, arrival="4200.5", replicas=1)]
@@ -408,37 +408,6 @@ def test_size_small_fleet_kernel_on_a_larger_fleet(engine, oracle_mod, monkeypat
     cand_g, win_g = engine.solve(fleet)
     assert_allocs_equal(cand_g, cand_o, "size candidates (warp per candidate)")
     assert_allocs_equal(win_g, win_o, "winners (warp per candidate)")
-
-
-def _adversarial_fleet(rng, case):
-    """Small fleet whose parameters sit at the edges the reference never exercises on purpose: coefficients spread
-    over many decades (and exactly 0), token counts 0 / 1 / huge, SLOs 0 / tiny / loose, loads from 1e-3 to 1e6
-    requests per minute, TPS targets, batch sizes 1 and 2."""
-    S, A = int(rng.integers(1, 7)), int(rng.integers(1, 4))
-    f = synth_fleet(S, A, seed=9000 + case, zero_load_frac=0.1, tps_frac=0.3, server_batch=bool(case % 2),
-                    max_batch_choices=(1, 2, 3, 8, 33, 120) if case % 25 else (2, 150, 400))
-    M = f.n_models
-
-    def logu(lo, hi, shape):
-        return np.exp(rng.uniform(np.log(lo), np.log(hi), shape)).astype(np.float32)
-    f.perf_alpha[:] = logu(1e-3, 1e3, (M, A))
-    f.perf_beta[:] = logu(1e-5, 1e2, (M, A))
-    f.perf_gamma[:] = logu(1e-3, 1e4, (M, A))
-    f.perf_delta[:] = logu(1e-7, 1.0, (M, A))
-    zero = rng.random((M, A))
-    f.perf_beta[zero < 0.1] = 0.0
-    f.perf_gamma[(zero > 0.1) & (zero < 0.2)] = 0.0
-    f.perf_delta[(zero > 0.2) & (zero < 0.3)] = 0.0
-    f.srv_in_tokens[:] = rng.choice([0, 1, 7, 512, 100000], S)
-    f.srv_out_tokens[:] = rng.choice([1, 2, 9, 300, 50000], S)
-    f.srv_arrival_rpm[:] = logu(1e-3, 1e6, S)
-    f.srv_arrival_rpm[rng.random(S) < 0.15] = 0.0
-    f.srv_slo_itl[:] = rng.choice([0.0, 1e-3, 5.0, 80.0, 1e6], S).astype(np.float32)
-    f.srv_slo_ttft[:] = rng.choice([0.0, 1e-2, 50.0, 2000.0, 1e7], S).astype(np.float32)
-    f.srv_slo_tps[:] = rng.choice([0.0, 0.0, 1.0, 500.0, 1e6], S).astype(np.float32)
-    f.srv_min_replicas[:] = rng.integers(0, 3, S)
-    f.max_queue_to_batch_ratio = int(rng.choice([1, 3, 10]))
-    return f
 
 
 def test_adversarial_parameters_size_and_grid(engine, oracle_mod):

@@ -12,10 +12,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, _same, mixed_fleet, overflow_fleet, rates_at_rate_star
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.test_gpu_workload_trace import transition_penalty
-from tests.util import ALLOC_FIELDS, assert_allocs_equal, assert_f32_bits_equal
+from tests.levels import _adversarial_fleet, mixed_fleet, overflow_fleet, rates_at_rate_star, transition_penalty
+from tests.util import ALLOC_FIELDS, assert_allocs_equal, assert_f32_bits_equal, error_code, same_bytes
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, accelerator_demand, synth_fleet
 
 F32 = np.float32
@@ -159,7 +157,7 @@ def test_repriced_table_is_calculate_at_the_price(oracle_mod, seed, factor):
             got = cand.copy()
             for s in range(fleet.n_servers):
                 got[s, a] = priced(fleet, s, a, cand[s, a], p)
-            assert _same(got, want), (a, p)
+            assert same_bytes(got, want), (a, p)
             checked += 1
     assert checked > 30
 
@@ -315,7 +313,7 @@ N_ADV = 30
 
 @pytest.mark.gpu
 def test_price_thresholds_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet, half of them on the rounds.  Where wva_analyze refuses the
+    """Fleets from levels._adversarial_fleet, half of them on the rounds.  Where wva_analyze refuses the
     fleet, the thresholds refuse too."""
     rng = np.random.default_rng(0xB1D)
     checked = refused = 0
@@ -325,9 +323,9 @@ def test_price_thresholds_adversarial(engine, oracle_mod, monkeypatch):
             monkeypatch.setenv("WVA_SIZE_SMALL_MAX", "0")
         else:
             monkeypatch.delenv("WVA_SIZE_SMALL_MAX", raising=False)
-        code = _code(lambda: engine.analyze(fleet))[0]
+        code = error_code(lambda: engine.analyze(fleet))[0]
         if code:
-            assert _code(lambda: engine.price_thresholds(fleet))[0] == code, case
+            assert error_code(lambda: engine.price_thresholds(fleet))[0] == code, case
             refused += 1
             continue
         _check(engine, oracle_mod, fleet, f"adversarial case {case}")
@@ -347,7 +345,7 @@ def test_profile_grid_at_every_threshold(engine):
     th, above, cand = engine.price_thresholds(fleet, want_candidates=True)
     analyze = engine.analyze(fleet)
     for k in ALLOC_FIELDS:
-        assert _same(getattr(cand, k), getattr(analyze, k)), k
+        assert same_bytes(getattr(cand, k), getattr(analyze, k)), k
     rows, index = [], {}
     for a in range(A):
         for t in np.unique(th[:, a][(th[:, a] > 0) & np.isfinite(th[:, a])]):
@@ -368,7 +366,7 @@ def test_profile_grid_at_every_threshold(engine):
             assert win.feasible[below] == 1 and win.acc[below] == a, (s, a)
             assert not (win.feasible[at] == 1 and win.acc[at] == a), (s, a)
             for k in ALLOC_FIELDS:
-                assert _same(getattr(win, k)[at], getattr(above, k)[s * A + a]), (s, a, k)
+                assert same_bytes(getattr(win, k)[at], getattr(above, k)[s * A + a]), (s, a, k)
             pairs += 1
     assert pairs >= 40
     inf = np.isinf(th).reshape(-1)
@@ -378,7 +376,7 @@ def test_profile_grid_at_every_threshold(engine):
         f = fleet.take_servers(np.arange(S))
         f.acc_cost[a] *= F32(3.0) if a % 2 else F32(0.25)
         th2 = engine.price_thresholds(f)[0]
-        assert _same(th2[:, a], th[:, a]), a
+        assert same_bytes(th2[:, a], th[:, a]), a
 
 
 # ---- GPU: API ---------------------------------------------------------------------------------
@@ -395,27 +393,27 @@ def test_argument_errors_and_refusals(engine):
     # above and candidates NULL: the thresholds alone
     th = np.zeros(fleet.n_servers * fleet.n_acc, F32)
     assert L.wva_price_thresholds(h, C.byref(fc), th.ctypes.data_as(C.POINTER(C.c_float)), None, None) == 0
-    assert _same(th, engine.price_thresholds(fleet)[0].reshape(-1))
+    assert same_bytes(th, engine.price_thresholds(fleet)[0].reshape(-1))
     for factor in (np.nan, -0.5, np.inf):
         f = fleet.take_servers(np.arange(fleet.n_servers))
         f.accel_penalty_factor = factor
-        assert _code(lambda: engine.price_thresholds(f))[0] == WVA_ERR_UNSUPPORTED, factor
+        assert error_code(lambda: engine.price_thresholds(f))[0] == WVA_ERR_UNSUPPORTED, factor
     f = fleet.take_servers(np.arange(fleet.n_servers))
     f.accel_penalty_factor = 0.0
-    assert _code(lambda: engine.price_thresholds(f))[0] == 0
+    assert error_code(lambda: engine.price_thresholds(f))[0] == 0
     for cost in (np.nan, np.inf, -np.inf):
         f = fleet.take_servers(np.arange(fleet.n_servers))
         f.srv_cur_cost[0] = cost
-        assert _code(lambda: engine.price_thresholds(f))[0] == WVA_ERR_UNSUPPORTED, cost
+        assert error_code(lambda: engine.price_thresholds(f))[0] == WVA_ERR_UNSUPPORTED, cost
         f.srv_model[0] = -1  # no candidate on that server: nothing to refuse
-        assert _code(lambda: engine.price_thresholds(f))[0] == 0, cost
+        assert error_code(lambda: engine.price_thresholds(f))[0] == 0, cost
     # the queue-size rule refuses as wva_analyze does
     big = synth_fleet(2, 2, seed=83, zero_load_frac=0.0)
     big.srv_max_batch[:] = 1 << 20
     big.max_queue_to_batch_ratio = 1 << 12
-    code = _code(lambda: engine.analyze(big))[0]
+    code = error_code(lambda: engine.analyze(big))[0]
     assert code == WVA_ERR_UNSUPPORTED
-    assert _code(lambda: engine.price_thresholds(big))[0] == code
+    assert error_code(lambda: engine.price_thresholds(big))[0] == code
 
 
 @pytest.mark.gpu
@@ -448,10 +446,10 @@ def test_one_handle_with_the_other_paths(engine):
     try:
         def same(x, y, what):
             if isinstance(x, np.ndarray):
-                assert _same(x, y), what
+                assert same_bytes(x, y), what
                 return
             for k in ALLOC_FIELDS:
-                assert _same(getattr(x, k), getattr(y, k)), f"{what}: {k}"
+                assert same_bytes(getattr(x, k), getattr(y, k)), f"{what}: {k}"
 
         def check(call, what):
             for x, y in zip(call(engine), call(fresh)):

@@ -11,82 +11,21 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, _f32_bits, _same, mixed_fleet, overflow_fleet, rates_at_rate_star
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.util import ALLOC_FIELDS, assert_allocs_equal
+from tests.levels import (COLUMNS, F32, PERF, _adversarial_fleet, at_row, check_level_call, mixed_fleet, overflow_fleet,
+                          profile_fleet, profile_rows, rates_at_rate_star, ref_grid)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
+                        error_code, f32_bits, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, greedy_solve, synth_fleet
-
-F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-PERF = ("perf_present", "perf_alpha", "perf_beta", "perf_gamma", "perf_delta", "perf_acc_count", "perf_max_batch",
-        "perf_at_tokens")
-COLUMNS = ("acc_cost",) + PERF
-
-
-def n_levels(rows):
-    return next(len(v) for v in rows.values())
-
-
-def at_profile(fleet, rows, l, unlimited=True):
-    """A copy of the fleet with acc_cost and the perf_* columns of row l (a column missing from rows is the
-    fleet's own)."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    for k, v in rows.items():
-        getattr(f, k)[:] = v[l]
-    f.unlimited = unlimited
-    return f
-
-
-def ref_profile_grid(oracle_mod, fleet, rows):
-    """(candidates [L*S*A], winners [L*S]): Server.Calculate and Solver.Solve (unlimited) per level."""
-    cands, wins = [np.zeros(0, oracle_mod.ALLOC_DTYPE)], [np.zeros(0, oracle_mod.ALLOC_DTYPE)]
-    for l in range(n_levels(rows)):
-        f = at_profile(fleet, rows, l)
-        cand = oracle_mod.calculate(f)
-        cands.append(cand.reshape(-1))
-        wins.append(oracle_mod.solve(f, cand)[1])
-    return np.concatenate(cands), np.concatenate(wins)
-
-
-def profile_fleet(n_servers, n_acc, seed, keep):
-    """mixed_fleet with every other server's batch size from the perf data, perf batch sizes kept small, and a few
-    servers sharing a model so that rows of one model reach several servers."""
-    f = mixed_fleet(n_servers, n_acc, seed, keep)
-    f.srv_max_batch[::2] = 0
-    f.perf_max_batch[:] = np.minimum(f.perf_max_batch, 64)
-    f.srv_model[5::4] = f.srv_model[0]
-    return f
-
-
-def profile_rows(fleet, L, seed):
-    """Mixed rows: per level a price change of every accelerator, a +-10 % change of one profile coefficient on
-    some (model, accelerator) entries, AccCount changes (0 and negative included), perf batch sizes, and a level
-    that turns the last accelerator off or on."""
-    rng = np.random.default_rng(seed)
-    M, A = fleet.n_models, fleet.n_acc
-    rows = {k: np.repeat(getattr(fleet, k)[None], L, axis=0).copy() for k in COLUMNS}
-    rows["acc_cost"] *= rng.choice([0.5, 0.8, 1.0, 1.0, 1.25], (L, A)).astype(F32)
-    for l in range(1, L):
-        k = PERF[1 + (l - 1) % 4]
-        mask = rng.random((M, A)) < 0.4
-        rows[k][l] = np.where(mask, rows[k][l] * rng.choice([F32(0.9), F32(1.1)], (M, A)), rows[k][l])
-    rows["perf_acc_count"][L // 2] = rng.choice([-3, 0, 1, 2, 4], (M, A))
-    rows["perf_max_batch"][-1] = np.maximum(rows["perf_max_batch"][-1] // 2, 1)
-    rows["perf_at_tokens"][min(2, L - 1)] *= 2
-    rows["perf_present"][min(1, L - 1), :, A - 1] ^= 1
-    return rows
-
 
 # ---- CPU: the composition and the split --------------------------------------------------------
 
 @pytest.mark.parametrize("keep", [False, True])
 def test_one_level_is_the_oracle_solve(oracle_mod, keep):
     fleet = profile_fleet(12, 3, 5, keep)
-    cand, win = ref_profile_grid(oracle_mod, fleet, {"acc_cost": fleet.acc_cost[None]})
-    cand_o, win_o = oracle_mod.solve(at_profile(fleet, {}, 0))
-    assert _same(cand, cand_o.reshape(-1))
-    assert _same(win, win_o)
+    cand, win = ref_grid(oracle_mod, fleet, {"acc_cost": fleet.acc_cost[None]})
+    cand_o, win_o = oracle_mod.solve(at_row(fleet, {}, 0))
+    assert same_bytes(cand, cand_o.reshape(-1))
+    assert same_bytes(win, win_o)
     assert win["feasible"].sum() >= 4
 
 
@@ -103,8 +42,8 @@ def test_cost_and_acc_count_enter_only_the_cost(oracle_mod, seed):
     rows["perf_acc_count"][2] = rng.choice([-1, 0, 3, 8], rows["perf_acc_count"][2].shape)
     checked = 0
     for l in range(L):
-        fl = at_profile(fleet, rows, l)
-        fk = at_profile(fleet, {k: v for k, v in rows.items() if k not in ("acc_cost", "perf_acc_count")}, l)
+        fl = at_row(fleet, rows, l)
+        fk = at_row(fleet, {k: v for k, v in rows.items() if k not in ("acc_cost", "perf_acc_count")}, l)
         for s in range(fleet.n_servers):
             m = int(fleet.srv_model[s])
             if m < 0 or not fleet.srv_has_target[s] or not (fleet.srv_arrival_rpm[s] > 0):
@@ -123,7 +62,7 @@ def test_cost_and_acc_count_enter_only_the_cost(oracle_mod, seed):
                     checked += 1
                 for k in ALLOC_FIELDS:
                     if k in ("cost", "value", "itl", "ttft", "rho", "max_rate"):
-                        assert _f32_bits(got[k]) == _f32_bits(want[k]), (l, s, a, k)
+                        assert f32_bits(got[k]) == f32_bits(want[k]), (l, s, a, k)
                     else:
                         assert int(got[k]) == int(want[k]), (l, s, a, k)
     assert checked >= 40
@@ -131,19 +70,11 @@ def test_cost_and_acc_count_enter_only_the_cost(oracle_mod, seed):
 
 # ---- GPU: bit for bit against the composition -------------------------------------------------
 
-def _check(engine, oracle_mod, fleet, rows, what):
-    cand_o, win_o = ref_profile_grid(oracle_mod, fleet, rows)
-    cand_g, win_g = engine.profile_grid(fleet, **rows, want_candidates=True)
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return cand_o, win_o
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
     fleet = profile_fleet(14, 3, 31, keep)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, profile_rows(fleet, 7, 3), f"warp path, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "profile_grid", fleet, profile_rows(fleet, 7, 3), f"warp path, keep = {keep}")
     assert cand_o["feasible"].sum() > 40
     assert len(set(win_o["acc"][win_o["feasible"] == 1].tolist())) >= 2
 
@@ -153,7 +84,7 @@ def rounds_case(oracle_mod):
     fleet = profile_fleet(120, 4, 37, False)
     fleet.srv_keep_acc[::2] = 1
     rows = profile_rows(fleet, 5, 11)
-    return fleet, rows, ref_profile_grid(oracle_mod, fleet, rows)
+    return fleet, rows, ref_grid(oracle_mod, fleet, rows)
 
 
 @pytest.mark.gpu
@@ -183,7 +114,7 @@ def test_cost_only_rows(engine, oracle_mod, monkeypatch, rounds):
                [1.0, F32_MAX, F32_MAX]]
     sweep = [np.concatenate([[base[0] * F32(f)], base[1:]]) for f in (1.0, 0.3, 0.1, 0.03, 0.01, 3.0, 10.0)]
     acc = np.array(special + sweep, F32)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, {"acc_cost": acc}, f"cost rows, rounds = {rounds}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "profile_grid", fleet, {"acc_cost": acc}, f"cost rows, rounds = {rounds}")
     S = fleet.n_servers
     w = win_o.reshape(len(acc), S)
     fe = w["feasible"] == 1
@@ -218,7 +149,7 @@ def test_perf_rows(engine, oracle_mod):
     rows["perf_acc_count"][6, :, 1] = -2
     rows["perf_max_batch"][7] = np.maximum(rows["perf_max_batch"][7] // 4, 1)
     rows["perf_at_tokens"][7] *= 3
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, "perf rows")
+    cand_o, _ = check_level_call(engine, oracle_mod, "profile_grid", fleet, rows, "perf rows")
     c = cand_o.reshape(L, fleet.n_servers, A)
     assert (c[0, :, 0]["feasible"] > c[4, :, 0]["feasible"]).any()
     assert not c[0, :, 2]["feasible"].any() and c[5, :, 2]["feasible"].any()
@@ -238,7 +169,7 @@ def test_zero_load_servers(engine, oracle_mod):
     fleet.srv_min_replicas[2::4] = 1
     fleet.srv_slo_tps[1::3] = F32(500.0)
     rows = profile_rows(fleet, 5, 7)
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, "zero load")
+    cand_o, _ = check_level_call(engine, oracle_mod, "profile_grid", fleet, rows, "zero load")
     c = cand_o.reshape(5, fleet.n_servers, fleet.n_acc)
     z = c[:, ::2]
     assert (z["feasible"] == 1).sum() > 10 and (z["rho"] == 0).all()
@@ -250,14 +181,14 @@ def test_repeated_rows_give_identical_blocks(engine, oracle_mod):
     fleet = profile_fleet(14, 3, 53, True)
     rows = profile_rows(fleet, 3, 9)
     rep = {k: v[[0, 1, 0, 2, 1, 1]] for k, v in rows.items()}
-    _check(engine, oracle_mod, fleet, rep, "repeated rows")
+    check_level_call(engine, oracle_mod, "profile_grid", fleet, rep, "repeated rows")
     cand, win = engine.profile_grid(fleet, **rep, want_candidates=True)
     S, A = fleet.n_servers, fleet.n_acc
     for k in ALLOC_FIELDS:
         c = getattr(cand, k).reshape(6, S * A)
         w = getattr(win, k).reshape(6, S)
         for x, y in ((0, 2), (1, 4), (1, 5)):
-            assert _same(c[x], c[y]) and _same(w[x], w[y]), (k, x, y)
+            assert same_bytes(c[x], c[y]) and same_bytes(w[x], w[y]), (k, x, y)
 
 
 @pytest.mark.gpu
@@ -272,7 +203,7 @@ def test_stored_vector_fallback(engine, oracle_mod):
     L = 4
     rows = {"acc_cost": np.array([[1.0], [2.5], [1.0], [0.25]], F32),
             "perf_max_batch": np.array([1024, 1024, 512, 2048], np.int32).reshape(L, 1, 1).repeat(fleet.n_models, 1)}
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, "stored-vector fallback")
+    cand_o, _ = check_level_call(engine, oracle_mod, "profile_grid", fleet, rows, "stored-vector fallback")
     assert cand_o["feasible"].sum() >= L
 
 
@@ -285,18 +216,18 @@ def test_against_the_existing_calls(engine, oracle_mod):
     S, A = fleet.n_servers, fleet.n_acc
     cand0, win0 = engine.profile_grid(fleet, acc_cost=np.zeros((0, A), F32), want_candidates=True)
     assert cand0.n == 0 and win0.n == 0
-    cand_s, win_s = engine.solve(at_profile(fleet, {}, 0))
+    cand_s, win_s = engine.solve(at_row(fleet, {}, 0))
     cand1, win1 = engine.profile_grid(fleet, perf_beta=fleet.perf_beta[None], want_candidates=True)
     for k in ALLOC_FIELDS:
-        assert _same(getattr(cand1, k), getattr(cand_s, k)) and _same(getattr(win1, k), getattr(win_s, k)), k
+        assert same_bytes(getattr(cand1, k), getattr(cand_s, k)) and same_bytes(getattr(win1, k), getattr(win_s, k)), k
     rows = profile_rows(fleet, 5, 13)
     cand_g, win_g = engine.profile_grid(fleet, **rows, want_candidates=True)
     for l in range(5):
-        cand_l, win_l = engine.solve(at_profile(fleet, rows, l))
+        cand_l, win_l = engine.solve(at_row(fleet, rows, l))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[l * S * A:(l + 1) * S * A], getattr(cand_l, k)), (l, k)
-            assert _same(getattr(win_g, k)[l * S:(l + 1) * S], getattr(win_l, k)), (l, k)
-        fl = at_profile(fleet, rows, l, unlimited=False)
+            assert same_bytes(getattr(cand_g, k)[l * S * A:(l + 1) * S * A], getattr(cand_l, k)), (l, k)
+            assert same_bytes(getattr(win_g, k)[l * S:(l + 1) * S], getattr(win_l, k)), (l, k)
+        fl = at_row(fleet, rows, l, unlimited=False)
         block = Allocs(S * A)
         for k in ALLOC_FIELDS:
             getattr(block, k)[:] = getattr(cand_g, k)[l * S * A:(l + 1) * S * A]
@@ -340,17 +271,17 @@ def test_batch_size_refusal_at_its_level_only(engine):
     m0 = int(fleet.srv_model[0])
     mb = np.repeat(fleet.perf_max_batch[None], 3, axis=0).copy()
     mb[1, m0, 0] = 1 << 16  # N = 2^16 * 2^12 / 2^7 = 2^21
-    code = _code(lambda: engine.analyze(at_profile(fleet, {"perf_max_batch": mb}, 1)))[0]
+    code = error_code(lambda: engine.analyze(at_row(fleet, {"perf_max_batch": mb}, 1)))[0]
     assert code == WVA_ERR_UNSUPPORTED
-    assert _code(lambda: engine.profile_grid(fleet, perf_max_batch=mb))[0] == code
-    assert _code(lambda: engine.profile_grid(fleet, perf_max_batch=mb[[0, 2]]))[0] == 0
+    assert error_code(lambda: engine.profile_grid(fleet, perf_max_batch=mb))[0] == code
+    assert error_code(lambda: engine.profile_grid(fleet, perf_max_batch=mb[[0, 2]]))[0] == 0
     # the same row where it cannot reach a loaded pair: server 0 on a fixed batch size, or accelerator 0 absent
     fixed = fleet.take_servers(np.arange(fleet.n_servers))
     fixed.srv_max_batch[0] = 8
-    assert _code(lambda: engine.profile_grid(fixed, perf_max_batch=mb))[0] == 0
+    assert error_code(lambda: engine.profile_grid(fixed, perf_max_batch=mb))[0] == 0
     absent = np.repeat(fleet.perf_present[None], 3, axis=0).copy()
     absent[1, m0, 0] = 0
-    assert _code(lambda: engine.profile_grid(fleet, perf_max_batch=mb, perf_present=absent))[0] == 0
+    assert error_code(lambda: engine.profile_grid(fleet, perf_max_batch=mb, perf_present=absent))[0] == 0
 
 
 @pytest.mark.gpu
@@ -407,7 +338,7 @@ def test_argument_errors(engine, oracle_mod):
     assert L.wva_profile_grid(h, C.byref(fc), 3, None, None, C.byref(win3.as_c())) == 0
     _, win_s = engine.solve(fleet)
     for k in ALLOC_FIELDS:
-        assert _same(getattr(win3, k), np.tile(getattr(win_s, k), 3)), k
+        assert same_bytes(getattr(win3, k), np.tile(getattr(win_s, k), 3)), k
     # S * A * L = 2^20 * 2^6 * 32 = 2^31, and L * M * A = 2^25 * 2^6 = 2^31: refused before the fleet is read
     big = fleet.as_c()
     big.n_servers, big.n_acc, big.n_types = 1 << 20, 1 << 6, 0
@@ -430,7 +361,7 @@ N_ADV = 30
 
 @pytest.mark.gpu
 def test_profile_grid_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet with random rows: prices from an edge set and profiles
+    """Fleets from levels._adversarial_fleet with random rows: prices from an edge set and profiles
     redrawn from the same decades, half of them on the rounds.  Where some level's wva_analyze refuses the level,
     the grid must refuse too."""
     rng = np.random.default_rng(0x9F0)
@@ -457,12 +388,12 @@ def test_profile_grid_adversarial(engine, oracle_mod, monkeypatch):
         if L > 2:
             for k in COLUMNS:
                 rows[k][2] = rows[k][1]
-        codes = [_code(lambda: engine.analyze(at_profile(fleet, rows, l)))[0] for l in range(L)]
+        codes = [error_code(lambda: engine.analyze(at_row(fleet, rows, l)))[0] for l in range(L)]
         if any(codes):
-            got, _ = _code(lambda: engine.profile_grid(fleet, **rows))
+            got, _ = error_code(lambda: engine.profile_grid(fleet, **rows))
             assert got == next(c for c in codes if c), (case, codes, got)
             refused += 1
             continue
-        _, win_o = _check(engine, oracle_mod, fleet, rows, f"adversarial case {case}")
+        _, win_o = check_level_call(engine, oracle_mod, "profile_grid", fleet, rows, f"adversarial case {case}")
         feasible += int(win_o["feasible"].sum())
     assert feasible > 30 and refused < N_ADV // 2

@@ -13,53 +13,18 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, _f32_bits, _same, overflow_fleet, rates_at_rate_star
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.test_gpu_profile_grid import COLUMNS, PERF, profile_fleet, profile_rows
-from tests.test_gpu_workload_grid import workload_levels
-from tests.test_gpu_workload_trace import _moves, _records, pinned, transition_penalty
-from tests.util import ALLOC_FIELDS, assert_allocs_equal
+from tests.levels import (COLUMNS, LOAD, PERF, ROW_COLUMN, _adversarial_fleet, _moves, _records, at_row, check_level_call, overflow_fleet,
+                          pinned, profile_fleet, profile_rows, rates_at_rate_star, ref_trace, transition_penalty,
+                          workload_levels)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
+                        error_code, f32_bits, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, synth_fleet
 
 F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-ACC_NONE = -1
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-LOAD_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens"}
-
-
-def n_ticks(rows):
-    return next(len(v) for v in rows.values())
-
-
-def at_tick(fleet, rows, t):
-    """A copy of the fleet with row t of every list in rows (load lists by argument name, profile lists by column
-    name); unlimited mode."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    for k, v in rows.items():
-        getattr(f, LOAD_COLUMN.get(k, k))[:] = v[t]
-    f.unlimited = True
-    return f
-
-
-def ref_profile_trace(oracle_mod, fleet, rows):
-    """(candidates [L*S*A], winners [L*S], the fleet with c_L): per tick, Server.Calculate and Solver.Solve
-    (unlimited) on the fleet with row t and current allocation c_t, then c_{t+1} = apply_winners."""
-    cands, wins = [np.zeros(0, oracle_mod.ALLOC_DTYPE)], [np.zeros(0, oracle_mod.ALLOC_DTYPE)]
-    cur = fleet
-    for t in range(n_ticks(rows)):
-        f = at_tick(cur, rows, t)
-        cand = oracle_mod.calculate(f)
-        win = oracle_mod.solve(f, cand)[1]
-        cands.append(cand.reshape(-1))
-        wins.append(win)
-        cur = cur.apply_winners(win)
-    return np.concatenate(cands), np.concatenate(wins), cur
-
-
 def load_rows(fleet, L, seed, special=True):
     rpm, in_tok, out_tok = workload_levels(fleet, L, seed, special=special)
     return {"arrival_rpm": rpm, "in_tokens": in_tok, "out_tokens": out_tok}
+LOAD_COLUMN = {k: ROW_COLUMN[k] for k in LOAD}
 
 
 def hourly_prices(fleet, L, seed):
@@ -70,14 +35,6 @@ def hourly_prices(fleet, L, seed):
     phase, depth = rng.uniform(0, 2 * np.pi, A), rng.uniform(0.2, 0.8, A)
     curve = 1.0 + depth * np.sin(2 * np.pi * t / 24.0 + phase) + rng.normal(0, 0.03, (L, A))
     return (fleet.acc_cost[None] * np.maximum(curve, 0.05)).astype(F32)
-
-
-def _check(engine, oracle_mod, fleet, rows, what):
-    cand_o, win_o, _ = ref_profile_trace(oracle_mod, fleet, rows)
-    cand_g, win_g = engine.profile_trace(fleet, **rows, want_candidates=True)
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return cand_o, win_o
 
 
 def _bytes_equal(got, want, what):
@@ -92,10 +49,10 @@ def test_one_tick_is_the_oracle_solve(oracle_mod, keep):
     fleet = profile_fleet(12, 3, 5, keep)
     rows = {"arrival_rpm": fleet.srv_arrival_rpm[None] * F32(1.5), "acc_cost": fleet.acc_cost[None] * F32(0.7)}
     rows["perf_beta"] = fleet.perf_beta[None] * F32(0.9)
-    cand, win, _ = ref_profile_trace(oracle_mod, fleet, rows)
-    cand_o, win_o = oracle_mod.solve(at_tick(fleet, rows, 0))
-    assert _same(cand, cand_o.reshape(-1))
-    assert _same(win, win_o)
+    cand, win, _ = ref_trace(oracle_mod, fleet, rows)
+    cand_o, win_o = oracle_mod.solve(at_row(fleet, rows, 0))
+    assert same_bytes(cand, cand_o.reshape(-1))
+    assert same_bytes(win, win_o)
     assert win["feasible"].sum() >= 4
 
 
@@ -112,7 +69,7 @@ def test_price_change_carries_the_winners_allocation(oracle_mod, seed):
     S, A = fleet.n_servers, fleet.n_acc
     cur, carried, repriced = fleet, 0, 0
     for t in range(L):
-        f = at_tick(cur, rows, t)
+        f = at_row(cur, rows, t)
         cand = oracle_mod.calculate(f)
         win = oracle_mod.solve(f, cand)[1]
         if t > 0:
@@ -123,18 +80,18 @@ def test_price_change_carries_the_winners_allocation(oracle_mod, seed):
                         continue
                     want = transition_penalty(f.accel_penalty_factor, cur.srv_cur_acc[s], cur.srv_cur_replicas[s],
                                               cur.srv_cur_cost[s], c["acc"], c["replicas"], c["cost"])
-                    assert _f32_bits(c["value"]) == _f32_bits(want), (t, s, a)
+                    assert f32_bits(c["value"]) == f32_bits(want), (t, s, a)
                     if a == cur.srv_cur_acc[s] and c["replicas"] == cur.srv_cur_replicas[s]:
-                        repriced += _f32_bits(c["cost"]) != _f32_bits(cur.srv_cur_cost[s])
+                        repriced += f32_bits(c["cost"]) != f32_bits(cur.srv_cur_cost[s])
         nxt = cur.apply_winners(win)
         for s in range(S):
             if win[s]["feasible"]:
                 assert (nxt.srv_cur_acc[s], nxt.srv_cur_replicas[s]) == (win[s]["acc"], win[s]["replicas"])
-                assert _f32_bits(nxt.srv_cur_cost[s]) == _f32_bits(win[s]["cost"])
+                assert f32_bits(nxt.srv_cur_cost[s]) == f32_bits(win[s]["cost"])
                 carried += 1
             else:
                 assert (nxt.srv_cur_acc[s], nxt.srv_cur_replicas[s]) == (cur.srv_cur_acc[s], cur.srv_cur_replicas[s])
-                assert _f32_bits(nxt.srv_cur_cost[s]) == _f32_bits(cur.srv_cur_cost[s])
+                assert f32_bits(nxt.srv_cur_cost[s]) == f32_bits(cur.srv_cur_cost[s])
         cur = nxt
     assert carried >= 20 and repriced >= 5
 
@@ -146,7 +103,7 @@ def test_price_change_carries_the_winners_allocation(oracle_mod, seed):
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
     fleet = profile_fleet(14, 3, 31, keep)
     rows = {**load_rows(fleet, 7, 3), **profile_rows(fleet, 7, 3)}
-    cand_o, win_o = _check(engine, oracle_mod, fleet, rows, f"warp path, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"warp path, keep = {keep}")
     assert cand_o["feasible"].sum() > 40
     assert len(set(win_o["acc"][win_o["feasible"] == 1].tolist())) >= 2
 
@@ -157,7 +114,7 @@ def rounds_case(oracle_mod):
     fleet.srv_keep_acc[::2] = 1
     fleet.accel_penalty_factor = 0.02
     rows = {**load_rows(fleet, 5, 11), **profile_rows(fleet, 5, 11)}
-    return fleet, rows, ref_profile_trace(oracle_mod, fleet, rows)
+    return fleet, rows, ref_trace(oracle_mod, fleet, rows)
 
 
 @pytest.mark.gpu
@@ -196,11 +153,11 @@ def test_hourly_price_rows(engine, oracle_mod, monkeypatch, keep, penalty, round
     hourly[7:, 0] = base[0] * F32(20.0)
     acc = np.concatenate([hourly[:2], np.array(special, F32), hourly[2:]]).astype(F32)
     rows = {"acc_cost": acc}
-    _, win_o = _check(engine, oracle_mod, fleet, rows, f"price rows, keep = {keep}, penalty = {penalty}")
+    _, win_o = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"price rows, keep = {keep}, penalty = {penalty}")
     S = fleet.n_servers
     _, win_trace = engine.profile_trace(fleet, **rows)
     _, win_grid = engine.profile_grid(fleet, **rows)
-    assert any(not _same(getattr(win_trace, k), getattr(win_grid, k)) for k in ALLOC_FIELDS)
+    assert any(not same_bytes(getattr(win_trace, k), getattr(win_grid, k)) for k in ALLOC_FIELDS)
     if not keep:
         assert _moves(win_o[(len(special) + 2) * S:], S) >= 1
 
@@ -218,7 +175,7 @@ def test_price_and_workload_rows(engine, oracle_mod, keep):
     rows = load_rows(fleet, L, 29, special=False)
     rows["arrival_rpm"][3::4, ::3] = 0.0
     rows["acc_cost"] = hourly_prices(fleet, L, 7)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, rows, f"prices and load, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"prices and load, keep = {keep}")
     S, A = fleet.n_servers, fleet.n_acc
     c = cand_o.reshape(L, S, A)
     zero = 0
@@ -231,7 +188,7 @@ def test_price_and_workload_rows(engine, oracle_mod, keep):
                 if r["feasible"] and r["replicas"] > 0:
                     m = fleet.srv_model[s]
                     inst = max(int(fleet.perf_acc_count[m, a]), 1) * int(r["replicas"])
-                    assert _f32_bits(r["cost"]) == _f32_bits(F32(rows["acc_cost"][t, a]) * F32(inst)), (t, s, a)
+                    assert f32_bits(r["cost"]) == f32_bits(F32(rows["acc_cost"][t, a]) * F32(inst)), (t, s, a)
                     zero += 1
     assert zero >= 10
     assert _moves(win_o, S) >= 3
@@ -262,7 +219,7 @@ def test_accelerator_switched_on_and_off(engine, oracle_mod, keep):
     for k in PERF[1:]:
         rows[k][on:off, :, 2] = rows[k][on:off, :, 1]
     rows["acc_cost"][:, 2] = fleet.acc_cost.min() * F32(0.05)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, rows, f"accelerator on and off, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"accelerator on and off, keep = {keep}")
     w = win_o.reshape(L, -1)
     if keep:
         assert pinned(fleet)[sit].all()
@@ -299,7 +256,7 @@ def test_profile_changes_from_a_tick(engine, oracle_mod, keep):
     rows["perf_max_batch"][7] = np.maximum(rows["perf_max_batch"][7] // 4, 1)
     rows["perf_at_tokens"][7] *= 3
     rows.update(load_rows(fleet, L, 13, special=False))
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, f"profile changes, keep = {keep}")
+    cand_o, _ = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"profile changes, keep = {keep}")
     c = cand_o.reshape(L, fleet.n_servers, fleet.n_acc)
     assert (c[3, :, 0]["feasible"] > c[4, :, 0]["feasible"]).any()
     srv_n = fleet.srv_max_batch == 0
@@ -328,7 +285,7 @@ def test_stored_vector_fallback_both_phases(engine, oracle_mod):
             "acc_cost": (np.arange(1, L + 1, dtype=F32)[:, None] * F32(0.75)).astype(F32),
             "perf_max_batch": np.where(np.arange(L) % 3 == 2, 512, 1024).astype(np.int32)[:, None, None]
             .repeat(fleet.n_models, 1)}
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, "stored-vector fallback")
+    cand_o, _ = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, "stored-vector fallback")
     assert cand_o["feasible"].sum() >= L
 
 
@@ -381,11 +338,11 @@ def test_model_without_profiles(engine, oracle_mod):
     for g, w in zip(got, want):
         _bytes_equal(g, w, "no perf column")
     assert n1 - n0 == n2 - n1
-    cand_o, win_o = _check(engine, oracle_mod, fleet, {**load, "acc_cost": hourly_prices(fleet, L, 5)}, "prices")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "profile_trace", fleet, {**load, "acc_cost": hourly_prices(fleet, L, 5)}, "prices")
     assert not cand_o.reshape(L, 4, 2)[:, 0]["feasible"].any() and win_o["feasible"].sum() >= 2 * L
     beta = np.repeat(fleet.perf_beta[None], L, axis=0).copy()
     beta[1:] *= F32(1.1)
-    _check(engine, oracle_mod, fleet, {**load, "perf_beta": beta}, "perf rows")
+    check_level_call(engine, oracle_mod, "profile_trace", fleet, {**load, "perf_beta": beta}, "perf rows")
 
 
 @pytest.mark.gpu
@@ -410,10 +367,10 @@ def test_each_tick_is_solve_on_the_advanced_fleet(engine):
     S, A = fleet.n_servers, fleet.n_acc
     cur = fleet
     for t in range(L):
-        cand_s, win_s = engine.solve(at_tick(cur, rows, t))
+        cand_s, win_s = engine.solve(at_row(cur, rows, t))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
-            assert _same(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
+            assert same_bytes(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
+            assert same_bytes(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
         cur = cur.apply_winners(win_s)
 
 
@@ -436,8 +393,8 @@ def test_continuation(engine, k):
         cur = cur.apply_winners(_records(win_a)[t * S:(t + 1) * S])
     cand_b, win_b = engine.profile_trace(cur, **{n: r[k:] for n, r in rows.items()}, want_candidates=True)
     for n in ALLOC_FIELDS:
-        assert _same(getattr(cand, n), np.concatenate([getattr(cand_a, n), getattr(cand_b, n)])), n
-        assert _same(getattr(win, n), np.concatenate([getattr(win_a, n), getattr(win_b, n)])), n
+        assert same_bytes(getattr(cand, n), np.concatenate([getattr(cand_a, n), getattr(cand_b, n)])), n
+        assert same_bytes(getattr(win, n), np.concatenate([getattr(win_a, n), getattr(win_b, n)])), n
     assert _moves(_records(win), S) >= 1
 
 
@@ -458,10 +415,10 @@ def test_batch_size_refusal_and_the_pinned_pair(engine):
     mb = np.repeat(fleet.perf_max_batch[None], L, axis=0).copy()
     mb[1, m0, 0] = 1 << 16
     rows = {"perf_max_batch": mb, "acc_cost": hourly_prices(fleet, L, 3)}
-    code = _code(lambda: engine.analyze(at_tick(fleet, rows, 1)))[0]
+    code = error_code(lambda: engine.analyze(at_row(fleet, rows, 1)))[0]
     assert code == WVA_ERR_UNSUPPORTED
-    assert _code(lambda: engine.profile_trace(fleet, **rows))[0] == code
-    assert _code(lambda: engine.profile_trace(fleet, **{k: v[[0, 2]] for k, v in rows.items()}))[0] == 0
+    assert error_code(lambda: engine.profile_trace(fleet, **rows))[0] == code
+    assert error_code(lambda: engine.profile_trace(fleet, **{k: v[[0, 2]] for k, v in rows.items()}))[0] == 0
     pin = fleet.take_servers(np.arange(fleet.n_servers))
     pin.srv_keep_acc[0] = 1
     pin.srv_cur_acc[0] = 1
@@ -472,10 +429,10 @@ def test_batch_size_refusal_and_the_pinned_pair(engine):
     S, A = pin.n_servers, pin.n_acc
     cur = pin
     for t in range(L):
-        cand_s, win_s = engine.solve(at_tick(cur, rows, t))
+        cand_s, win_s = engine.solve(at_row(cur, rows, t))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
-            assert _same(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
+            assert same_bytes(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
+            assert same_bytes(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
         cur = cur.apply_winners(win_s)
     assert (win_g.acc[0::S][win_g.feasible[0::S] == 1] == 1).all()
 
@@ -561,7 +518,7 @@ N_ADV = 30
 
 @pytest.mark.gpu
 def test_profile_trace_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet, keep on half the servers, with random load rows from the
+    """Fleets from levels._adversarial_fleet, keep on half the servers, with random load rows from the
     workload grid's edge sets and random profile rows from the profile grid's, half of them on the rounds.  Where
     the per-tick wva_solve loop refuses a tick, the trace must refuse too; it may refuse beyond that only through a
     keep server that is not pinned."""
@@ -598,11 +555,11 @@ def test_profile_trace_adversarial(engine, oracle_mod, monkeypatch):
         # the per-tick wva_solve loop
         code, cur = 0, fleet
         for t in range(L):
-            code, res = _code(lambda: engine.solve(at_tick(cur, rows, t)))
+            code, res = error_code(lambda: engine.solve(at_row(cur, rows, t)))
             if code:
                 break
             cur = cur.apply_winners(res[1])
-        got, _ = _code(lambda: engine.profile_trace(fleet, **rows))
+        got, _ = error_code(lambda: engine.profile_trace(fleet, **rows))
         if code:
             assert got == code, (case, code, got)
             refused += 1
@@ -611,6 +568,6 @@ def test_profile_trace_adversarial(engine, oracle_mod, monkeypatch):
             assert got == WVA_ERR_UNSUPPORTED and ((fleet.srv_keep_acc != 0) & ~pinned(fleet)).any(), (case, got)
             extra += 1
             continue
-        _, win_o = _check(engine, oracle_mod, fleet, rows, f"adversarial case {case}")
+        _, win_o = check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"adversarial case {case}")
         feasible += int(win_o["feasible"].sum())
     assert feasible > 30 and refused + extra < N_ADV // 2

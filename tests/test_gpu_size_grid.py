@@ -11,73 +11,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.util import assert_allocs_equal
+from tests.levels import mixed_fleet, ref_candidates, ref_size_grid, ref_winners, with_batch
+from tests.util import F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_UNSUPPORTED, assert_allocs_equal, same_bytes
 from workload_variant_autoscaler_b200 import Engine, synth_fleet
-
-F32_MAX = np.float32(np.finfo(np.float32).max)
-WVA_ERR_BAD_ARG, WVA_ERR_UNSUPPORTED = -1, -6
-
-
-def with_batch(fleet, b):
-    """A copy of the fleet with every server's MaxBatchSize override set to b."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    f.srv_max_batch[:] = b
-    return f
-
-
-def ref_candidates(oracle_mod, fleet, batches):
-    """[S, A, B]: Server.Calculate at each batch size."""
-    cand = np.zeros((fleet.n_servers, fleet.n_acc, len(batches)), oracle_mod.ALLOC_DTYPE)
-    for bi, b in enumerate(batches):
-        cand[:, :, bi] = oracle_mod.calculate(with_batch(fleet, int(b)))
-    return cand
-
-
-def ref_winners(oracle_mod, cand, batches):
-    """Per server: the feasible candidate with the smallest value, strict '<' from MaxFloat32 (a NaN value or one
-    not below MaxFloat32 never wins); ties to the smaller batch size, then the lower accelerator id."""
-    S, A, B = cand.shape
-    win = np.zeros(S, oracle_mod.ALLOC_DTYPE)
-    win["acc"] = -1
-    for s in range(S):
-        best = None  # (value, batch, a, bi)
-        for a in range(A):
-            for bi in range(B):
-                c = cand[s, a, bi]
-                if not c["feasible"]:
-                    continue
-                v = np.float32(c["value"])
-                if not v < F32_MAX:
-                    continue
-                key = (int(batches[bi]), a, bi)
-                if best is None or v < best[0] or (v == best[0] and key < best[1:]):
-                    best = (v,) + key
-        if best is not None:
-            win[s] = cand[s, best[2], best[3]]
-    return win
-
-
-def ref_size_grid(oracle_mod, fleet, batches):
-    cand = ref_candidates(oracle_mod, fleet, batches)
-    return cand.reshape(-1), ref_winners(oracle_mod, cand, batches)
-
-
-def mixed_fleet(n_servers, n_acc, seed, keep):
-    """Zero load, TPS targets, an unknown model, a server without a target, a missing profile, min_replicas = 0,
-    an unknown current accelerator, keepAccelerator on or off."""
-    f = synth_fleet(n_servers, n_acc, seed=seed, keep_accelerator=keep, zero_load_frac=0.2, tps_frac=0.3)
-    f.srv_min_replicas[::3] = 0
-    f.perf_present[1, n_acc - 1] = 0
-    f.srv_has_target[2] = 0
-    f.srv_model[3] = -1
-    f.srv_cur_acc[4] = -2
-    f.srv_keep_acc[4] = 1
-    return f
-
-
-def _same(a, b):
-    return np.ascontiguousarray(a).tobytes() == np.ascontiguousarray(b).tobytes()
-
 
 # ---- CPU: the composition itself --------------------------------------------------------------
 
@@ -88,8 +24,8 @@ def test_one_batch_size_is_the_oracle_solve(oracle_mod, seed, keep):
     for b in (4, 32):
         cand, win = ref_size_grid(oracle_mod, fleet, [b])
         cand_o, win_o = oracle_mod.solve(with_batch(fleet, b))
-        assert _same(cand, cand_o.reshape(-1)), f"candidates, b = {b}"
-        assert _same(win, win_o), f"winners, b = {b}"
+        assert same_bytes(cand, cand_o.reshape(-1)), f"candidates, b = {b}"
+        assert same_bytes(win, win_o), f"winners, b = {b}"
         assert win["feasible"].sum() >= 4
 
 
@@ -128,10 +64,10 @@ def test_winner_order_on_hand_built_ties(oracle_mod):
 def test_repeated_batch_sizes_give_identical_records(oracle_mod):
     fleet = mixed_fleet(10, 3, 5, False)
     cand = ref_candidates(oracle_mod, fleet, [8, 4, 8])
-    assert _same(cand[:, :, 0], cand[:, :, 2])
+    assert same_bytes(cand[:, :, 0], cand[:, :, 2])
     win = ref_winners(oracle_mod, cand, [8, 4, 8])
     win1 = ref_winners(oracle_mod, cand[:, :, :2].copy(), [8, 4])
-    assert _same(win, win1)
+    assert same_bytes(win, win1)
 
 
 # ---- GPU: bit for bit against the composition -------------------------------------------------

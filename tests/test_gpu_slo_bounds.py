@@ -11,118 +11,14 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, mixed_fleet, overflow_fleet, pair_batch
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.util import ALLOC_FIELDS, assert_f32_bits_equal
+from tests.levels import (F32, FREE, INF_BITS, NIL, PAST, SEARCHED, _adversarial_fleet, analyzer, check_slo_bounds,
+                          from_bits, lam_range, mixed_fleet, overflow_fleet, ref_slo_bounds, u32_bits)
+from tests.util import ALLOC_FIELDS, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, error_code
 from workload_variant_autoscaler_b200 import Engine, WvaError, slo_envelope, synth_fleet
 from workload_variant_autoscaler_b200 import _abi
 
-F32 = np.float32
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-INF_BITS, PAST = 0x7F800000, 0x7F800001
-NIL, SEARCHED, FREE = 0, 1, 2
-
-
-def _f(bits):
-    return np.array([bits], np.uint32).view(np.float32)[0]
-
-
-def _bits(x):
-    return int(np.array([x], np.float32).view(np.uint32)[0])
-
-
 def _key(x):
-    return PAST if np.isnan(x) else _bits(x)
-
-
-def is_load_pair(fleet, s, a):
-    """CreateAllocation's gates and the candidate rule (allocation.go:42-75, server.go:70-82): a pair it sizes."""
-    if fleet.srv_keep_acc[s] and fleet.srv_cur_acc[s] != -1 and fleet.srv_cur_acc[s] != a:
-        return False
-    rpm, m = fleet.srv_arrival_rpm[s], int(fleet.srv_model[s])
-    if rpm < 0 or fleet.srv_in_tokens[s] < 0 or fleet.srv_out_tokens[s] < 0 or not 0 <= m < fleet.n_models:
-        return False
-    if not fleet.perf_present[m, a] or not fleet.srv_has_target[s]:
-        return False
-    return rpm != 0 and fleet.srv_out_tokens[s] != 0
-
-
-def analyzer(oracle_mod, fleet, s, a):
-    m, N = int(fleet.srv_model[s]), pair_batch(fleet, s, a)
-    return oracle_mod.Analyzer(N, N * fleet.max_queue_to_batch_ratio, float(fleet.perf_alpha[m, a]),
-                               float(fleet.perf_beta[m, a]), float(fleet.perf_gamma[m, a]),
-                               float(fleet.perf_delta[m, a]), int(fleet.srv_in_tokens[s]),
-                               int(fleet.srv_out_tokens[s]))
-
-
-def lam_range(qa):
-    rmin, rmax = qa.rate_range()
-    return F32(rmin) / F32(1000), F32(rmax) / F32(1000)  # queueanalyzer.go:197-198
-
-
-class Classifier:
-    """BinarySearch's boundary checks (utils.go:36-51) restated with the oracle's WithinTolerance."""
-
-    def __init__(self, oracle_mod):
-        self.wt = oracle_mod.lib().wvao_within_tolerance
-
-    def cls(self, y0, y1, t):
-        if self.wt(y0, t, 1e-6):
-            return SEARCHED
-        if self.wt(y1, t, 1e-6):
-            return FREE
-        inc = y0 < y1
-        if (inc and t < y0) or (not inc and t > y0):
-            return NIL
-        if (inc and t > y1) or (not inc and t < y1):
-            return FREE
-        return SEARCHED
-
-    def rank(self, y0, y1, t):
-        c = self.cls(y0, y1, t)
-        return c if y0 < y1 else 2 - c
-
-    def first(self, y0, y1, k):
-        """Smallest positive float32 target of rank >= k, NaN past +Inf."""
-        if self.rank(y0, y1, _f(INF_BITS)) < k:
-            return F32(np.nan)
-        if self.rank(y0, y1, _f(1)) >= k:
-            return _f(1)
-        lo, hi = 1, INF_BITS
-        while hi - lo > 1:
-            mid = (lo + hi) // 2
-            if self.rank(y0, y1, _f(mid)) >= k:
-                hi = mid
-            else:
-                lo = mid
-        return _f(hi)
-
-
-def ref_slo_bounds(oracle_mod, fleet):
-    """(kind, y_lo, y_hi, b1, b2), each (S, A, 2), from the oracle."""
-    S, A = fleet.n_servers, fleet.n_acc
-    kind = np.zeros((S, A, 2), np.uint8)
-    y_lo, y_hi, b1, b2 = (np.zeros((S, A, 2), np.float32) for _ in range(4))
-    cl = Classifier(oracle_mod)
-    for s in range(S):
-        for a in range(A):
-            if not is_load_pair(fleet, s, a):
-                continue
-            N = pair_batch(fleet, s, a)
-            if N + N * fleet.max_queue_to_batch_ratio < 2:
-                continue
-            qa = analyzer(oracle_mod, fleet, s, a)
-            lmin, lmax = lam_range(qa)
-            ends = [(qa.eval_ttft(float(x)), qa.eval_itl(float(x))) for x in (lmin, lmax)]
-            if lmin > lmax or ends[0][0][0]:
-                kind[s, a] = 1  # BinarySearch's range error, or an invalid model at the first evaluation
-                continue
-            for w in range(2):
-                y0, y1 = F32(ends[0][w][1]), F32(ends[1][w][1])
-                kind[s, a, w] = 2 if y0 < y1 else 3
-                y_lo[s, a, w], y_hi[s, a, w] = y0, y1
-                b1[s, a, w], b2[s, a, w] = cl.first(y0, y1, 1), cl.first(y0, y1, 2)
-    return kind, y_lo, y_hi, b1, b2
+    return PAST if np.isnan(x) else u32_bits(x)
 
 
 def stretch(kind, b1, b2, t):
@@ -148,16 +44,16 @@ def probe_targets(y0, y1, b1, b2, rng):
     keys = {1, 2, 0x00400000, 0x7F7FFFFF, INF_BITS}
     for b in (b1, b2):
         if not np.isnan(b):
-            keys |= {_bits(b), max(_bits(b) - 1, 1)}
+            keys |= {u32_bits(b), max(u32_bits(b) - 1, 1)}
     for y in (y0, y1):
         if y > 0 and np.isfinite(y):
-            keys |= {k for k in range(_bits(y) - 64, _bits(y) + 65, 8) if 0 < k <= INF_BITS}
-            keys |= {_bits(y) - 1, _bits(y), _bits(y) + 1}
+            keys |= {k for k in range(u32_bits(y) - 64, u32_bits(y) + 65, 8) if 0 < k <= INF_BITS}
+            keys |= {u32_bits(y) - 1, u32_bits(y), u32_bits(y) + 1}
     edges = sorted({1} | {_key(b) for b in (b1, b2)} | {INF_BITS + 1})
     for lo, hi in zip(edges, edges[1:]):
         if hi - 1 > lo:
             keys |= set(int(k) for k in rng.integers(lo, min(hi, INF_BITS + 1), 3))
-    return [_f(k) for k in sorted(keys) if 0 < k <= INF_BITS]
+    return [from_bits(k) for k in sorted(keys) if 0 < k <= INF_BITS]
 
 
 # ---- CPU: the composition against the oracle's own search ------------------------------------------
@@ -187,7 +83,7 @@ def test_composition_is_binary_search_and_size(oracle_mod, seed):
                     if err:
                         raise ValueError("invalid model")
                     return y
-                ts = [_f(1), _f(INF_BITS), F32(1.0), F32(100.0)] if k == 1 else \
+                ts = [from_bits(1), from_bits(INF_BITS), F32(1.0), F32(100.0)] if k == 1 else \
                     probe_targets(y_lo[s, a, w], y_hi[s, a, w], b1[s, a, w], b2[s, a, w], rng)
                 err0, r0, _, _ = qa.size(0.0, 0.0, 0.0)
                 for t in ts:
@@ -204,8 +100,8 @@ def test_composition_is_binary_search_and_size(oracle_mod, seed):
                     if c == FREE:
                         assert not err0
                         name = "rate_ttft" if w == 0 else "rate_itl"
-                        assert _bits(rates[name]) == _bits(r0[name]), (s, a, w, t)
-                        assert _bits(xs) == _bits(lmax), (s, a, w, t)
+                        assert u32_bits(rates[name]) == u32_bits(r0[name]), (s, a, w, t)
+                        assert u32_bits(xs) == u32_bits(lmax), (s, a, w, t)
     assert seen[1] >= 1 and seen[2] >= 4 and seen[3] >= 2, seen
     assert {(2, NIL), (2, SEARCHED), (2, FREE)} <= classes, classes
 
@@ -223,7 +119,7 @@ def test_flat_itl_and_tolerance_edges(oracle_mod):
         y = y_lo[s, a, 1]
         assert b1[s, a, 1] <= y < b2[s, a, 1]
         qa = analyzer(oracle_mod, fleet, s, a)
-        for t in (b1[s, a, 1], _f(_bits(b1[s, a, 1]) - 1), _f(_bits(b2[s, a, 1]) - 1), b2[s, a, 1]):
+        for t in (b1[s, a, 1], from_bits(u32_bits(b1[s, a, 1]) - 1), from_bits(u32_bits(b2[s, a, 1]) - 1), b2[s, a, 1]):
             err, rates, _, _ = qa.size(0.0, float(t), 0.0)
             c = stretch(3, b1[s, a, 1], b2[s, a, 1], t)
             assert (c == NIL) == (err != 0)
@@ -231,29 +127,20 @@ def test_flat_itl_and_tolerance_edges(oracle_mod):
 
 # ---- GPU: bit for bit against the composition ---------------------------------------------------
 
-def _check(engine, oracle_mod, fleet, what):
-    want = ref_slo_bounds(oracle_mod, fleet)
-    got = engine.slo_bounds(fleet)
-    assert np.array_equal(got[0], want[0]), f"{what}: kind"
-    for name, g, w in zip(("y_lo", "y_hi", "b1", "b2"), got[1:], want[1:]):
-        assert_f32_bits_equal(g.reshape(-1), w.reshape(-1), f"{what}: {name}")
-    return want
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("rounds", [False, True])
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet(engine, oracle_mod, monkeypatch, keep, rounds):
     if rounds:
         monkeypatch.setenv("WVA_SIZE_SMALL_MAX", "0")
-    kind = _check(engine, oracle_mod, edge_fleet(31, keep), f"keep = {keep}, rounds = {rounds}")[0]
+    kind = check_slo_bounds(engine, oracle_mod, edge_fleet(31, keep), f"keep = {keep}, rounds = {rounds}")[0]
     assert (kind == 0).any() and (kind == 1).any() and (kind == 2).any() and (kind == 3).any()
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("n_acc", [32, 33])
 def test_many_accelerators(engine, oracle_mod, n_acc):
-    _check(engine, oracle_mod, synth_fleet(4, n_acc, seed=41 + n_acc, zero_load_frac=0.2), f"A = {n_acc}")
+    check_slo_bounds(engine, oracle_mod, synth_fleet(4, n_acc, seed=41 + n_acc, zero_load_frac=0.2), f"A = {n_acc}")
 
 
 @pytest.mark.gpu
@@ -262,27 +149,27 @@ def test_stored_vector_fallback(engine, oracle_mod):
     vector."""
     fleet = overflow_fleet()
     fleet.srv_arrival_rpm[:] = 600.0
-    kind = _check(engine, oracle_mod, fleet, "stored-vector fallback")[0]
+    kind = check_slo_bounds(engine, oracle_mod, fleet, "stored-vector fallback")[0]
     assert (kind >= 2).all()
 
 
 @pytest.mark.gpu
 def test_adversarial(engine, oracle_mod):
-    """test_gpu_parity's adversarial fleets: where the call refuses, wva_analyze with every target positive
+    """levels._adversarial_fleet's fleets: where the call refuses, wva_analyze with every target positive
     refuses too."""
     rng = np.random.default_rng(0x5B0)
     checked = 0
     for case in range(24):
         fleet = _adversarial_fleet(rng, 80000 + case)
-        code = _code(lambda: engine.slo_bounds(fleet))[0]
+        code = error_code(lambda: engine.slo_bounds(fleet))[0]
         if code:
             assert code == WVA_ERR_UNSUPPORTED, case
             f = fleet.take_servers(np.arange(fleet.n_servers))
             f.srv_slo_itl[:] = 1.0
             f.srv_slo_ttft[:] = 1.0
-            assert _code(lambda: engine.analyze(f))[0] == WVA_ERR_UNSUPPORTED, case
+            assert error_code(lambda: engine.analyze(f))[0] == WVA_ERR_UNSUPPORTED, case
             continue
-        _check(engine, oracle_mod, fleet, f"adversarial case {case}")
+        check_slo_bounds(engine, oracle_mod, fleet, f"adversarial case {case}")
         checked += 1
     assert checked >= 12
 
@@ -308,7 +195,7 @@ def test_statements_on_the_slo_grid(engine):
                 pts += [np.where(ok, b, 0).astype(F32), np.where(ok & (below > 0), below, 0).astype(F32)]
         floor, ceiling = slo_envelope(fleet, bounds, w)
         fc = lambda x: np.where(np.isfinite(x), x, 0).astype(F32)  # noqa: E731
-        pts += [fc(floor), fc(np.where(floor > _f(1), (floor.view(np.uint32) - 1).view(F32), 0)), fc(ceiling),
+        pts += [fc(floor), fc(np.where(floor > from_bits(1), (floor.view(np.uint32) - 1).view(F32), 0)), fc(ceiling),
                 fc(ceiling * F32(2))]
         rows = np.stack([np.zeros(S, F32)] + pts)
         own = {"slo_itl": fleet.srv_slo_itl, "slo_ttft": fleet.srv_slo_ttft, "slo_tps": fleet.srv_slo_tps}
@@ -356,9 +243,9 @@ def test_argument_errors_and_refusals(engine):
     big.srv_max_batch[:] = 1 << 20
     big.max_queue_to_batch_ratio = 1 << 12
     n0 = engine.launch_count
-    assert _code(lambda: engine.slo_bounds(big))[0] == WVA_ERR_UNSUPPORTED
+    assert error_code(lambda: engine.slo_bounds(big))[0] == WVA_ERR_UNSUPPORTED
     assert engine.launch_count == n0  # refused before any launch
-    assert _code(lambda: engine.analyze(big))[0] == WVA_ERR_UNSUPPORTED
+    assert error_code(lambda: engine.analyze(big))[0] == WVA_ERR_UNSUPPORTED
 
 
 @pytest.mark.gpu

@@ -11,79 +11,25 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, _f32_bits, _same, mixed_fleet, overflow_fleet, pair_batch, tail
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.util import ALLOC_FIELDS, assert_allocs_equal
+from tests.levels import (F32, SLO, TARGETS, TPS_TARGETS, _adversarial_fleet, _search, at_row, check_level_call,
+                          mixed_fleet, overflow_fleet, pair_batch, ref_grid, slo_levels, tail)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
+                        error_code, f32_bits, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, greedy_solve, synth_fleet
 
-F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
 # ITL / TTFT targets at the edges: 0, -0 and NaN disable a search, a negative one makes the pair nil, the others run
-TARGETS = (0.0, -0.0, np.nan, -1.0, 1e-30, 1e-40, np.inf, float(F32_MAX))
 # TPS targets: no NaN (totalRate NaN) and no tiny positive one (totalRate 0, so a min_replicas-0 pair solves at 0/0):
 # the library refuses some such levels, see test_nan_or_tiny_tps_level_fails_as_solve_does
-TPS_TARGETS = (0.0, -0.0, -1.0, np.inf, float(F32_MAX))
-
-
-def at_slo(fleet, itl, ttft, tps, unlimited=True):
-    """A copy of the fleet with the targets of row (itl, ttft, tps)."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    f.srv_slo_itl[:] = itl
-    f.srv_slo_ttft[:] = ttft
-    f.srv_slo_tps[:] = tps
-    f.unlimited = unlimited
-    return f
-
-
-def ref_slo_grid(oracle_mod, fleet, itl, ttft, tps):
-    """(candidates [L*S*A], winners [L*S]): Server.Calculate and Solver.Solve (unlimited) per level."""
-    cands, wins = [np.zeros(0, oracle_mod.ALLOC_DTYPE)], [np.zeros(0, oracle_mod.ALLOC_DTYPE)]
-    for l in range(itl.shape[0]):
-        f = at_slo(fleet, itl[l], ttft[l], tps[l])
-        cand = oracle_mod.calculate(f)
-        cands.append(cand.reshape(-1))
-        wins.append(oracle_mod.solve(f, cand)[1])
-    return np.concatenate(cands), np.concatenate(wins)
-
-
-def slo_levels(fleet, L, seed, special=True):
-    """(itl, ttft, tps), each [L, S]: every server's own targets times a seeded factor per (level, server), so the
-    rows are per-server and non-monotone, with the edge values of TARGETS and TPS_TARGETS scattered over them."""
-    rng = np.random.default_rng(seed)
-    S = fleet.n_servers
-    factors = np.array([0.5, 0.75, 1.0, 1.5, 2.0], np.float32)
-    rows = []
-    for col in (fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps):
-        rows.append((col[None, :] * rng.choice(factors, (L, S))).astype(np.float32))
-    itl, ttft, tps = rows
-    if special:
-        for k, v in enumerate(TARGETS):
-            itl[k % L, k % S::3 + k] = v
-            ttft[(k + 1) % L, (k + 1) % S::4 + k] = v
-        for k, v in enumerate(TPS_TARGETS):
-            tps[(k + 2) % L, (2 * k) % S::5 + k] = v
-    return itl, ttft, tps
-
-
-def _check(engine, oracle_mod, fleet, rows, what):
-    cand_o, win_o = ref_slo_grid(oracle_mod, fleet, *rows)
-    cand_g, win_g = engine.slo_grid(fleet, *rows, want_candidates=True)
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return cand_o, win_o
-
-
 # ---- CPU: the composition and the premise -------------------------------------------------------
 
 @pytest.mark.parametrize("keep", [False, True])
 def test_one_level_is_the_oracle_solve(oracle_mod, keep):
     fleet = mixed_fleet(12, 3, 5, keep)
     rows = [c[None, :] for c in (fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps)]
-    cand, win = ref_slo_grid(oracle_mod, fleet, *rows)
-    cand_o, win_o = oracle_mod.solve(at_slo(fleet, fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps))
-    assert _same(cand, cand_o.reshape(-1))
-    assert _same(win, win_o)
+    cand, win = ref_grid(oracle_mod, fleet, dict(zip(SLO, rows)))
+    cand_o, win_o = oracle_mod.solve(at_row(fleet, {}, 0))
+    assert same_bytes(cand, cand_o.reshape(-1))
+    assert same_bytes(win, win_o)
     assert win["feasible"].sum() >= 4
 
 
@@ -94,24 +40,6 @@ def _analyzer(oracle_mod, fleet, s, a):
                                   float(fleet.perf_beta[m, a]), float(fleet.perf_gamma[m, a]),
                                   float(fleet.perf_delta[m, a]), int(fleet.srv_in_tokens[s]),
                                   int(fleet.srv_out_tokens[s]))
-
-
-def _search(oracle_mod, qa, which, target):
-    """One BinarySearch of Size (queueanalyzer.go:204-228) on its own: (ok, lambdaStar); ok False when it errs or
-    the target is below the bounded region."""
-    lo, hi = qa.rate_range()
-    lmin, lmax = F32(lo) / F32(1000), F32(hi) / F32(1000)
-    if not target > 0:
-        return True, lmax
-    ev = qa.eval_ttft if which == 0 else qa.eval_itl
-
-    def fn(x):
-        err, y = ev(x)
-        if err:
-            raise ValueError(err)
-        return y
-    err, xs, ind = oracle_mod.binary_search(float(lmin), float(lmax), float(target), fn)
-    return (err == 0 and ind >= 0), F32(xs)
 
 
 def test_each_search_reads_only_its_own_target(oracle_mod):
@@ -132,23 +60,23 @@ def test_each_search_reads_only_its_own_target(oracle_mod):
             if not fleet.perf_present[m, a]:
                 continue
             N, qa = _analyzer(oracle_mod, fleet, s, a)
-            one_t = {_f32_bits(t): qa.size(t, 0.0, 0.0) for t in ttfts}
-            one_i = {_f32_bits(t): qa.size(0.0, t, 0.0) for t in itls}
-            srch_t = {_f32_bits(t): _search(oracle_mod, qa, 0, t) for t in ttfts}
-            srch_i = {_f32_bits(t): _search(oracle_mod, qa, 1, t) for t in itls}
+            one_t = {f32_bits(t): qa.size(t, 0.0, 0.0) for t in ttfts}
+            one_i = {f32_bits(t): qa.size(0.0, t, 0.0) for t in itls}
+            srch_t = {f32_bits(t): _search(oracle_mod, qa, 0, t) for t in ttfts}
+            srch_i = {f32_bits(t): _search(oracle_mod, qa, 1, t) for t in itls}
             for tt in ttfts:
                 for ti in itls:
                     for tp in TPS_TARGETS + (tps_typ,):
                         err, rates, _, _ = qa.size(tt, ti, tp)
                         neg = tt < 0 or ti < 0 or tp < 0
-                        ok_t, xs_t = srch_t[_f32_bits(tt)]
-                        ok_i, xs_i = srch_i[_f32_bits(ti)]
+                        ok_t, xs_t = srch_t[f32_bits(tt)]
+                        ok_i, xs_i = srch_i[f32_bits(ti)]
                         assert (err != 0) == (neg or not ok_t or not ok_i), (s, a, tt, ti, tp, err)
                         if err == 0:
-                            assert _f32_bits(rates["rate_ttft"]) == _f32_bits(one_t[_f32_bits(tt)][1]["rate_ttft"])
-                            assert _f32_bits(rates["rate_itl"]) == _f32_bits(one_i[_f32_bits(ti)][1]["rate_itl"])
+                            assert f32_bits(rates["rate_ttft"]) == f32_bits(one_t[f32_bits(tt)][1]["rate_ttft"])
+                            assert f32_bits(rates["rate_itl"]) == f32_bits(one_i[f32_bits(ti)][1]["rate_itl"])
                         # the tail from the two searches reproduces CreateAllocation at this level
-                        f_l = at_slo(fleet, fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps)
+                        f_l = at_row(fleet, {}, 0)
                         f_l.srv_slo_ttft[s], f_l.srv_slo_itl[s], f_l.srv_slo_tps[s] = tt, ti, tp
                         want = oracle_mod.create_allocation(f_l, s, a)
                         got = None
@@ -164,7 +92,7 @@ def test_each_search_reads_only_its_own_target(oracle_mod):
                             continue
                         for k in ALLOC_FIELDS:
                             if k in ("cost", "value", "itl", "ttft", "rho", "max_rate"):
-                                assert _f32_bits(got[k]) == _f32_bits(want[k]), (s, a, tt, ti, tp, k)
+                                assert f32_bits(got[k]) == f32_bits(want[k]), (s, a, tt, ti, tp, k)
                             else:
                                 assert int(got[k]) == int(want[k]), (s, a, tt, ti, tp, k)
                         checked += 1
@@ -178,7 +106,7 @@ def test_each_search_reads_only_its_own_target(oracle_mod):
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
     fleet = mixed_fleet(14, 3, 31, keep)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, slo_levels(fleet, 7, 3), f"small, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "slo_grid", fleet, dict(zip(SLO, slo_levels(fleet, 7, 3))), f"small, keep = {keep}")
     assert cand_o["feasible"].sum() > 40
     assert len(set(win_o["replicas"][win_o["feasible"] == 1].tolist())) >= 3
 
@@ -188,7 +116,7 @@ def rounds_case(oracle_mod):
     fleet = mixed_fleet(60, 3, 37, False)
     fleet.srv_keep_acc[::2] = 1
     rows = slo_levels(fleet, 4, 11)
-    return fleet, rows, ref_slo_grid(oracle_mod, fleet, *rows)
+    return fleet, rows, ref_grid(oracle_mod, fleet, dict(zip(SLO, rows)))
 
 
 @pytest.mark.gpu
@@ -220,7 +148,7 @@ def test_cartesian_itl_ttft_tps_grid(engine, oracle_mod, monkeypatch, rounds):
                 ttft.append(fleet.srv_slo_ttft * ft)
                 tps.append(tps_on if use_tps else np.zeros(S, np.float32))
     rows = tuple(np.array(x, np.float32) for x in (itl, ttft, tps))
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, f"Cartesian, rounds = {rounds}")
+    cand_o, _ = check_level_call(engine, oracle_mod, "slo_grid", fleet, dict(zip(SLO, rows)), f"Cartesian, rounds = {rounds}")
     assert cand_o["feasible"].sum() > 100
 
 
@@ -229,10 +157,10 @@ def test_own_targets_are_wva_solve(engine):
     fleet = mixed_fleet(30, 4, 43, True)
     rows = [c[None, :] for c in (fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps)]
     cand1, win1 = engine.slo_grid(fleet, *rows, want_candidates=True)
-    cand_s, win_s = engine.solve(at_slo(fleet, fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps))
+    cand_s, win_s = engine.solve(at_row(fleet, {}, 0))
     for k in ALLOC_FIELDS:
-        assert _same(getattr(cand1, k), getattr(cand_s, k)), k
-        assert _same(getattr(win1, k), getattr(win_s, k)), k
+        assert same_bytes(getattr(cand1, k), getattr(cand_s, k)), k
+        assert same_bytes(getattr(win1, k), getattr(win_s, k)), k
 
 
 @pytest.mark.gpu
@@ -257,7 +185,7 @@ def test_stored_vector_fallback_both_phases(engine, oracle_mod):
         rows_ttft.append(ttft_near * F32(ft))
     L = len(rows_itl)
     rows = (np.array(rows_itl, np.float32), np.array(rows_ttft, np.float32), np.zeros((L, S), np.float32))
-    cand_o, _ = _check(engine, oracle_mod, fleet, rows, "stored-vector fallback")
+    cand_o, _ = check_level_call(engine, oracle_mod, "slo_grid", fleet, dict(zip(SLO, rows)), "stored-vector fallback")
     assert cand_o["feasible"].sum() >= L
 
 
@@ -270,7 +198,7 @@ def test_nan_and_huge_values_and_ties(engine, oracle_mod):
     fleet.perf_alpha[:, 2] = fleet.perf_alpha[:, 1]  # accelerators 1 and 2 identical: ties on value
     for k in ("perf_beta", "perf_gamma", "perf_delta", "perf_acc_count"):
         getattr(fleet, k)[:, 2] = getattr(fleet, k)[:, 1]
-    _check(engine, oracle_mod, fleet, slo_levels(fleet, 4, 17), "NaN / huge values and ties")
+    check_level_call(engine, oracle_mod, "slo_grid", fleet, dict(zip(SLO, slo_levels(fleet, 4, 17))), "NaN / huge values and ties")
 
 
 @pytest.mark.gpu
@@ -343,7 +271,7 @@ def test_each_block_is_the_greedy_input_of_its_level(engine, oracle_mod):
     cand_g, _ = engine.slo_grid(fleet, *rows, want_candidates=True)
     S, A = fleet.n_servers, fleet.n_acc
     for l in range(4):
-        fl = at_slo(fleet, rows[0][l], rows[1][l], rows[2][l], unlimited=False)
+        fl = at_row(fleet, dict(zip(SLO, rows)), l, unlimited=False)
         block = Allocs(S * A)
         for k in ALLOC_FIELDS:
             getattr(block, k)[:] = getattr(cand_g, k)[l * S * A:(l + 1) * S * A]
@@ -393,16 +321,16 @@ def test_nan_or_tiny_tps_level_fails_as_solve_does(engine, s, value, fails):
     assert fleet.srv_arrival_rpm[s] > 0 and fleet.srv_min_replicas[s] == 0
     itl, ttft, tps = slo_levels(fleet, 3, 19, special=False)
     tps[1, s] = value
-    want, res = _code(lambda: engine.solve(at_slo(fleet, itl[1], ttft[1], tps[1])))
-    got, grid = _code(lambda: engine.slo_grid(fleet, itl, ttft, tps, want_candidates=True))
+    want, res = error_code(lambda: engine.solve(at_row(fleet, dict(zip(SLO, (itl, ttft, tps))), 1)))
+    got, grid = error_code(lambda: engine.slo_grid(fleet, itl, ttft, tps, want_candidates=True))
     assert got == want == (WVA_ERR_UNSUPPORTED if fails else 0)
     if want == 0:
         S, A = fleet.n_servers, fleet.n_acc
         for k in ALLOC_FIELDS:
-            assert _same(getattr(grid[0], k)[S * A:2 * S * A], getattr(res[0], k)), k
-            assert _same(getattr(grid[1], k)[S:2 * S], getattr(res[1], k)), k
+            assert same_bytes(getattr(grid[0], k)[S * A:2 * S * A], getattr(res[0], k)), k
+            assert same_bytes(getattr(grid[1], k)[S:2 * S], getattr(res[1], k)), k
     keep = [0, 2]
-    assert _code(lambda: engine.slo_grid(fleet, itl[keep], ttft[keep], tps[keep]))[0] == 0
+    assert error_code(lambda: engine.slo_grid(fleet, itl[keep], ttft[keep], tps[keep]))[0] == 0
 
 
 N_ADV = 36
@@ -410,7 +338,7 @@ N_ADV = 36
 
 @pytest.mark.gpu
 def test_slo_grid_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet with random target rows from the same edge sets (0, tiny,
+    """Fleets from levels._adversarial_fleet with random target rows from the same edge sets (0, tiny,
     loose; some rows with a target negative or disabled), half of them on the rounds."""
     rng = np.random.default_rng(0x510)
     feasible = 0
@@ -429,6 +357,6 @@ def test_slo_grid_adversarial(engine, oracle_mod, monkeypatch):
         itl[0], ttft[0], tps[0] = fleet.srv_slo_itl, fleet.srv_slo_ttft, fleet.srv_slo_tps
         if L > 2:
             itl[2], ttft[2], tps[2] = itl[1], ttft[1], tps[1]  # a repeated row
-        _, win_o = _check(engine, oracle_mod, fleet, (itl, ttft, tps), f"adversarial case {case}")
+        _, win_o = check_level_call(engine, oracle_mod, "slo_grid", fleet, dict(zip(SLO, (itl, ttft, tps))), f"adversarial case {case}")
         feasible += int(win_o["feasible"].sum())
     assert feasible > 60

@@ -13,41 +13,15 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, _f32_bits, _same, mixed_fleet, overflow_fleet, pair_batch, \
-    rates_at_rate_star
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.test_gpu_slo_grid import TARGETS, TPS_TARGETS, _search, at_slo, slo_levels
-from tests.test_gpu_workload_grid import at_level, token_fleet, workload_levels
-from tests.test_gpu_workload_trace import _moves, _records, low_penalty_fleet, pinned, ref_trace, wva_fleet
-from tests.util import ALLOC_FIELDS, assert_allocs_equal
+from tests.levels import (LOAD, SLO, TARGETS, TPS_TARGETS, Tally, _adversarial_fleet, _moves, _records, _search, at_row,
+                          check_level_call, cross_fleet, low_penalty_fleet, mixed_fleet, overflow_fleet, pair_batch,
+                          pinned, rates_at_rate_star, ref_trace, slo_levels, token_fleet, workload_levels, wva_fleet)
+from tests.util import (ACC_NONE, ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED,
+                        assert_allocs_equal, error_code, f32_bits, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, synth_fleet
 
 F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-ACC_NONE = -1
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-NAMES = ("arrival_rpm", "in_tokens", "out_tokens", "slo_itl", "slo_ttft", "slo_tps")
-
-
-def at_tick(fleet, rows, t):
-    """f_t without the current allocation: a copy of the fleet with the six columns at row t (unlimited)."""
-    rpm, in_tok, out_tok, itl, ttft, tps = rows
-    return at_slo(at_level(fleet, rpm[t], in_tok[t], out_tok[t]), itl[t], ttft[t], tps[t])
-
-
-def ref_slo_trace(oracle_mod, fleet, rows):
-    """(candidates [L*S*A], winners [L*S]): per tick, the workload trace's composition (Server.Calculate, Solver.Solve
-    unlimited, apply_winners) on the fleet whose targets are row t."""
-    rpm, in_tok, out_tok, itl, ttft, tps = rows
-    cands, wins = [np.zeros(0, oracle_mod.ALLOC_DTYPE)], [np.zeros(0, oracle_mod.ALLOC_DTYPE)]
-    cur = fleet
-    for t in range(rpm.shape[0]):
-        one = slice(t, t + 1)
-        cand, win, cur = ref_trace(oracle_mod, at_slo(cur, itl[t], ttft[t], tps[t]), rpm[one], in_tok[one],
-                                   out_tok[one])
-        cands.append(cand)
-        wins.append(win)
-    return np.concatenate(cands), np.concatenate(wins)
+NAMES = LOAD + SLO
 
 
 def slo_trace_rows(fleet, L, seed, special=True):
@@ -74,17 +48,9 @@ def _call(engine, fleet, rows, **kw):
     return engine.slo_trace(fleet, **dict(zip(NAMES, rows)), **kw)
 
 
-def _check(engine, oracle_mod, fleet, rows, what):
-    cand_o, win_o = ref_slo_trace(oracle_mod, fleet, rows)
-    cand_g, win_g = _call(engine, fleet, rows, want_candidates=True)
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return cand_o, win_o
-
-
 def _same_allocs(got, want, what):
     for k in ALLOC_FIELDS:
-        assert _same(getattr(got, k), getattr(want, k)), f"{what}: {k}"
+        assert same_bytes(getattr(got, k), getattr(want, k)), f"{what}: {k}"
 
 
 # ---- CPU: the composition, the premise and the restatement -------------------------------------------
@@ -94,10 +60,10 @@ def test_one_tick_is_the_oracle_solve(oracle_mod, keep):
     fleet = token_fleet(12, 3, 5, keep)
     rows = slo_trace_rows(fleet, 3, 9, special=False)
     one = tuple(r[1:2] for r in rows)
-    cand, win = ref_slo_trace(oracle_mod, fleet, one)
-    cand_o, win_o = oracle_mod.solve(at_tick(fleet, one, 0))
-    assert _same(cand, cand_o.reshape(-1))
-    assert _same(win, win_o)
+    cand, win, _ = ref_trace(oracle_mod, fleet, dict(zip(NAMES, one)))
+    cand_o, win_o = oracle_mod.solve(at_row(fleet, dict(zip(NAMES, one)), 0))
+    assert same_bytes(cand, cand_o.reshape(-1))
+    assert same_bytes(win, win_o)
     assert win["feasible"].sum() >= 3
 
 
@@ -111,7 +77,7 @@ def test_search_reads_neither_rate_nor_tps_nor_the_other_target(oracle_mod):
     checked = 0
     for s in range(fleet.n_servers):
         for t in range(L):
-            f = at_tick(fleet, rows, t)
+            f = at_row(fleet, dict(zip(NAMES, rows)), t)
             m = int(f.srv_model[s])
             if m < 0 or not f.srv_has_target[s] or f.srv_out_tokens[s] <= 0 or f.srv_in_tokens[s] < 0 or \
                     not f.srv_arrival_rpm[s] > 0 or pair_batch(f, s, 0) > 4096:
@@ -137,23 +103,22 @@ def test_search_reads_neither_rate_nor_tps_nor_the_other_target(oracle_mod):
                         if neg or err:
                             continue
                         assert own and lone[0] == 0, (s, t, a, u, key)
-                        assert _f32_bits(rates[key]) == _f32_bits(lone[1][key]), (s, t, a, u, key)
+                        assert f32_bits(rates[key]) == f32_bits(lone[1][key]), (s, t, a, u, key)
                         checked += 1
     assert checked >= 100, checked
 
 
 def test_oracle_agrees_with_the_restatement_on_schedule_ticks(oracle_mod):
     """oracle/restate_np.py against the oracle on a sample of this file's tick fleets f_t (cross_fleet)."""
-    from tests.test_oracle_cross import Tally, cross_fleet
     t = Tally()
     f = token_fleet(10, 3, 41, False)
     rows = slo_trace_rows(f, 6, 43)
     for k in (0, 2, 5):
-        cross_fleet(oracle_mod, at_tick(f, rows, k), t, f"edge rows, tick {k}")
+        cross_fleet(oracle_mod, at_row(f, dict(zip(NAMES, rows)), k), t, f"edge rows, tick {k}")
     g = low_penalty_fleet(10, 3, 45, True)
     rows = schedule(g, 8, 47)
     for k in (0, 3, 7):
-        cross_fleet(oracle_mod, at_tick(g, rows, k), t, f"schedule, tick {k}")
+        cross_fleet(oracle_mod, at_row(g, dict(zip(NAMES, rows)), k), t, f"schedule, tick {k}")
     t.report("SLO trace ticks", min_feasible=40, min_infeasible=10)
 
 
@@ -163,7 +128,7 @@ def test_oracle_agrees_with_the_restatement_on_schedule_ticks(oracle_mod):
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
     fleet = token_fleet(14, 3, 31, keep)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, slo_trace_rows(fleet, 7, 3), f"warp path, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, slo_trace_rows(fleet, 7, 3))), f"warp path, keep = {keep}")
     assert cand_o["feasible"].sum() > 30
     assert len(set(win_o["replicas"][win_o["feasible"] == 1].tolist())) >= 3
 
@@ -174,7 +139,7 @@ def rounds_case(oracle_mod):
     fleet.srv_keep_acc[::2] = 1
     fleet.accel_penalty_factor = 0.02
     rows = slo_trace_rows(fleet, 4, 11)
-    return fleet, rows, ref_slo_trace(oracle_mod, fleet, rows)
+    return fleet, rows, ref_trace(oracle_mod, fleet, dict(zip(NAMES, rows)))[:2]
 
 
 @pytest.mark.gpu
@@ -205,7 +170,7 @@ def test_schedule_moves_winners_and_back(engine, oracle_mod, monkeypatch, keep, 
         rows[k] = np.repeat(rows[k][:1], L, 0)  # one load: only the targets move
     rows[3][3:6] = rows[3][3:6] * F32(0.5)
     rows[0][7, ::3] = 0.0
-    _, win_o = _check(engine, oracle_mod, fleet, tuple(rows), f"schedule, keep = {keep}")
+    _, win_o = check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, tuple(rows))), f"schedule, keep = {keep}")
     assert _moves(win_o, S) >= (2 if keep else 4)
 
 
@@ -214,7 +179,7 @@ def test_wva_configuration_every_server_pinned(engine, oracle_mod):
     fleet = wva_fleet(60, 4, 97)
     assert pinned(fleet).all()
     rows = schedule(fleet, 6, 31)
-    _, win_o = _check(engine, oracle_mod, fleet, rows, "WVA configuration")
+    _, win_o = check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, rows)), "WVA configuration")
     win = win_o.reshape(6, -1)
     for t in range(6):
         f = win[t]["feasible"] != 0
@@ -240,7 +205,7 @@ def test_edge_targets_with_edge_loads(engine, oracle_mod):
     rpm[1, ::4] = 0.0
     rpm[2, 1::6] = -1.0
     out_tok[3, 2::6] = 0
-    cand_o, win_o = _check(engine, oracle_mod, fleet, tuple(rows), "edge targets and loads")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, tuple(rows))), "edge targets and loads")
     win = win_o.reshape(L, S)
     assert (win["feasible"] == 0).sum() >= 10
     assert ((win["feasible"] == 1) & (win["acc"] == ACC_NONE)).sum() >= 1
@@ -265,7 +230,7 @@ def test_stored_vector_fallback_both_phases(engine, oracle_mod):
     tps = np.zeros((L, S), F32)
     itl[::3] = 1e6
     ttft[1::3] = 1e9
-    cand_o, _ = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok, itl, ttft, tps), "stored-vector fallback")
+    cand_o, _ = check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, (rpm, in_tok, out_tok, itl, ttft, tps))), "stored-vector fallback")
     assert cand_o["feasible"].sum() >= L
 
 
@@ -279,7 +244,7 @@ def test_nan_and_huge_values_and_ties(engine, oracle_mod, keep):
     fleet.perf_alpha[:, 2] = fleet.perf_alpha[:, 1]
     for k in ("perf_beta", "perf_gamma", "perf_delta", "perf_acc_count"):
         getattr(fleet, k)[:, 2] = getattr(fleet, k)[:, 1]
-    _check(engine, oracle_mod, fleet, slo_trace_rows(fleet, 5, 17), f"NaN / huge values and ties, keep = {keep}")
+    check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, slo_trace_rows(fleet, 5, 17))), f"NaN / huge values and ties, keep = {keep}")
 
 
 @pytest.mark.gpu
@@ -294,17 +259,17 @@ def test_nan_or_tiny_tps_tick_fails_as_solve_does(engine, s, value, fails):
     tps[1, s] = value
     rows = (None, None, None, itl, ttft, tps)
     cur = fleet
-    _, res0 = _code(lambda: engine.solve(at_slo(cur, itl[0], ttft[0], tps[0])))
+    _, res0 = error_code(lambda: engine.solve(at_row(cur, dict(zip(SLO, (itl, ttft, tps))), 0)))
     cur = fleet.apply_winners(res0[1])
-    want, res = _code(lambda: engine.solve(at_slo(cur, itl[1], ttft[1], tps[1])))
-    got, tr = _code(lambda: _call(engine, fleet, rows, want_candidates=True))
+    want, res = error_code(lambda: engine.solve(at_row(cur, dict(zip(SLO, (itl, ttft, tps))), 1)))
+    got, tr = error_code(lambda: _call(engine, fleet, rows, want_candidates=True))
     assert got == want == (WVA_ERR_UNSUPPORTED if fails else 0)
     if want == 0:
         for k in ALLOC_FIELDS:
-            assert _same(getattr(tr[0], k)[S * A:2 * S * A], getattr(res[0], k)), k
-            assert _same(getattr(tr[1], k)[S:2 * S], getattr(res[1], k)), k
+            assert same_bytes(getattr(tr[0], k)[S * A:2 * S * A], getattr(res[0], k)), k
+            assert same_bytes(getattr(tr[1], k)[S:2 * S], getattr(res[1], k)), k
     keep = [0, 2]
-    assert _code(lambda: engine.slo_trace(fleet, slo_itl=itl[keep], slo_ttft=ttft[keep], slo_tps=tps[keep]))[0] == 0
+    assert error_code(lambda: engine.slo_trace(fleet, slo_itl=itl[keep], slo_ttft=ttft[keep], slo_tps=tps[keep]))[0] == 0
 
 
 # ---- GPU: against the library's other calls ---------------------------------------------------------
@@ -337,7 +302,7 @@ def test_one_tick_is_the_slo_grid(engine, monkeypatch, rounds):
     for t in range(3):
         one = [r[t:t + 1] for r in rows]
         got = _call(engine, fleet, one, want_candidates=True)
-        want = engine.slo_grid(at_level(fleet, rows[0][t], rows[1][t], rows[2][t]), *one[3:], want_candidates=True)
+        want = engine.slo_grid(at_row(fleet, dict(zip(LOAD, rows)), t), *one[3:], want_candidates=True)
         _same_allocs(got[0], want[0], f"tick {t}: candidates")
         _same_allocs(got[1], want[1], f"tick {t}: winners")
 
@@ -357,8 +322,8 @@ def test_continuation(engine, k):
         cur = cur.apply_winners(_records(win_a)[t * S:(t + 1) * S])
     cand_b, win_b = _call(engine, cur, [r[k:] for r in rows], want_candidates=True)
     for n in ALLOC_FIELDS:
-        assert _same(getattr(cand, n), np.concatenate([getattr(cand_a, n), getattr(cand_b, n)])), n
-        assert _same(getattr(win, n), np.concatenate([getattr(win_a, n), getattr(win_b, n)])), n
+        assert same_bytes(getattr(cand, n), np.concatenate([getattr(cand_a, n), getattr(cand_b, n)])), n
+        assert same_bytes(getattr(win, n), np.concatenate([getattr(win_a, n), getattr(win_b, n)])), n
     assert _moves(_records(win), S) >= 1
 
 
@@ -370,10 +335,10 @@ def test_each_tick_is_solve_on_the_advanced_fleet(engine):
     cand_g, win_g = _call(engine, fleet, rows, want_candidates=True)
     cur = fleet
     for t in range(L):
-        cand_s, win_s = engine.solve(at_tick(cur, rows, t))
+        cand_s, win_s = engine.solve(at_row(cur, dict(zip(NAMES, rows)), t))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
-            assert _same(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
+            assert same_bytes(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
+            assert same_bytes(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
         cur = cur.apply_winners(win_s)
     assert win_g.feasible.sum() >= L * S // 4
 
@@ -430,7 +395,7 @@ def test_argument_errors_and_refusals(engine):
     g.perf_at_tokens[:] = 1 << 12
     out_tok = np.full((2, 4), 1 << 16, np.int32)
     out_tok[1, 0] = 1
-    assert _code(lambda: engine.slo_trace(g, out_tokens=out_tok))[0] == WVA_ERR_UNSUPPORTED
+    assert error_code(lambda: engine.slo_trace(g, out_tokens=out_tok))[0] == WVA_ERR_UNSUPPORTED
     engine.solve(fleet)
 
 
@@ -474,7 +439,7 @@ N_ADV = 30
 
 @pytest.mark.gpu
 def test_slo_trace_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet, keep on half the servers, with random load and target rows
+    """Fleets from levels._adversarial_fleet, keep on half the servers, with random load and target rows
     from the edge sets, half of them on the rounds.  Where the per-tick wva_solve loop refuses a tick the trace
     refuses too; it may refuse beyond that only through a keep server that is not pinned."""
     rng = np.random.default_rng(0x5107)
@@ -501,11 +466,11 @@ def test_slo_trace_adversarial(engine, oracle_mod, monkeypatch):
         rows = (rpm, in_tok, out_tok, itl, ttft, tps)
         code, cur = 0, fleet
         for t in range(L):
-            code, res = _code(lambda: engine.solve(at_tick(cur, rows, t)))
+            code, res = error_code(lambda: engine.solve(at_row(cur, dict(zip(NAMES, rows)), t)))
             if code:
                 break
             cur = cur.apply_winners(res[1])
-        got, _ = _code(lambda: _call(engine, fleet, rows))
+        got, _ = error_code(lambda: _call(engine, fleet, rows))
         if code:
             assert got == code, (case, code, got)
             refused += 1
@@ -514,6 +479,6 @@ def test_slo_trace_adversarial(engine, oracle_mod, monkeypatch):
             assert got == WVA_ERR_UNSUPPORTED and ((fleet.srv_keep_acc != 0) & ~pinned(fleet)).any(), (case, got)
             extra += 1
             continue
-        _, win_o = _check(engine, oracle_mod, fleet, rows, f"adversarial case {case}")
+        _, win_o = check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(NAMES, rows)), f"adversarial case {case}")
         feasible += int(win_o["feasible"].sum())
     assert feasible > 30 and refused + extra < N_ADV // 2

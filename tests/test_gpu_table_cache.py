@@ -4,28 +4,13 @@ Each path keeps its tables in a set of its own (the solve path, the size grid, t
 sweep builds into the grid's.  These tests interleave every path on one handle and compare each result byte for
 byte with the same call on a fresh handle, and pin, through the launch count, which calls rebuild their tables:
 the solve path only when the token epoch changes, the grid on every call."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import ALLOC_FIELDS, load_levels, mixed_fleet
-from workload_variant_autoscaler_b200 import Engine, Grid, _abi, synth_fleet
-
-
-def device_winners(S):
-    """(tensor, AllocsC): a zeroed device winner block of S records and its columns."""
-    import torch
-    blk = torch.zeros(10 * S, dtype=torch.int32, device="cuda")
-    cols = _abi.AllocsC()
-    b = blk.data_ptr()
-    cols.feasible = C.cast(b, _abi.u8p)
-    for k, name in enumerate(("acc", "replicas", "batch"), start=1):
-        setattr(cols, name, C.cast(b + 4 * S * k, _abi.i32p))
-    for k, name in enumerate(("cost", "value", "itl", "ttft", "rho", "max_rate"), start=4):
-        setattr(cols, name, C.cast(b + 4 * S * k, _abi.f32p))
-    torch.cuda.synchronize()  # the zero fill runs on torch's stream, the engine on its own
-    return blk, cols
+from tests.grid_cases import device_winners
+from tests.levels import load_levels, mixed_fleet
+from tests.util import ALLOC_FIELDS
+from workload_variant_autoscaler_b200 import Engine, Grid, synth_fleet
 
 
 def grid_device(eng, grid, S):

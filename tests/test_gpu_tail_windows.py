@@ -35,7 +35,7 @@ Bands per tail (E = binary exponent, "edge - 1 / edge"):
   stayed inside the windows, so only those final solves are counted.  TPS-only rows on the main fleet (lambda* = 0.9
   lambda_max overflows float64) place the final rate on every band; there the whole item, final Analyze included,
   runs in slo_fallback's stored re-run.  The SLO grid also has two K >= 2^23 candidates (a TPS row on
-  test_gpu_windows.long_queue_fleet) whose lambda* solves run the pass-2 IEEE path.
+  grid_cases.long_queue_fleet) whose lambda* solves run the pass-2 IEEE path.
 * bounds: E(max p) 879 / 880, E(sum) 679 / 680 and 899 / 900 and float64 overflow at lambda_max; the rate edges and
   lambda_min exactly on 2^-60 and just below; lambda_max exactly on 2^60 and just below (the float32 values one ulp
   under a power of two are finer than the steps of lambda_min = 0.001 servRate[0] and lambda_max = 0.999
@@ -61,46 +61,22 @@ Not reachable, and so left out:
 """
 from __future__ import annotations
 
-import functools
-
 import numpy as np
 import pytest
-
-from tests.test_gpu_load_grid import ref_load_grid
-from tests.test_gpu_load_intervals import _check as intervals_check, ref_intervals
-from tests.test_gpu_profile_grid import _check as profile_grid_check, ref_profile_grid
-from tests.test_gpu_profile_trace import _check as profile_trace_check, ref_profile_trace
-from tests.test_gpu_slo_bounds import _check as bounds_check, lam_range, ref_slo_bounds
-from tests.test_gpu_slo_grid import ref_slo_grid
-from tests.test_gpu_slo_trace import _check as slo_trace_check, ref_slo_trace
-from tests.test_gpu_windows import (BELOW, LONG_RATIO, P60, SIZE_RATIO, _analyzer, _concat, _fleet, _lam_of_rate,
-                                    _lam_star, _rate_edge_models, _rpm_for_lambda, chain_profile, long_queue_fleet,
-                                    wide_bands, _rate_bands)
-from tests.test_gpu_workload_grid import _check as workload_grid_check, ref_workload_grid
-from tests.test_gpu_workload_trace import _check as workload_trace_check, ref_trace
+from tests.grid_cases import (DELTA, MAIN_N, P60, SIZE_RATIO, XS, _concat, _edge_fleet, _edge_rpm, _fleet, _lam_of_rate,
+                              _lam_star, _model, _qa, _rate_bands, _x_rpm, bounds_cases, chain_profile, f32, load_cases,
+                              profile_cases, slo_cases, wide_bands)
+from tests.levels import (LOAD, SLO, check_intervals, check_level_call, check_slo_bounds, lam_range, ref_grid,
+                          ref_intervals, ref_slo_bounds, ref_trace)
 from tests.util import assert_allocs_equal
 
-f32 = np.float32
-DELTA = 1e-5
+
 FB_SLOTS = 128  # kFbBlocks * kFbThreads: the threads of every re-run kernel
 # x = lambda * alpha of the levels: E(sum) 679 / 680 near x = 472; E(max p) 879 / 880, the pass-2 IEEE band and
 # E(sum) 899 / 900 between 604 and 632; float64 overflow above ~705
-XS = np.concatenate([np.arange(466.0, 482.0, 0.25), np.arange(604.0, 632.0, 0.125), np.arange(690.0, 740.0, 2.5)])
-MAIN_N = (1024, 900)
-LONG_XS = np.arange(612.0, 613.5, 0.5)  # the K >= 2^23 candidate's final solves, around the pass-2 IEEE band
-EDGE_N = 16
-EDGE_XS = (0.5, 3.0, 9.0)
-LAM_EDGE_ALPHAS = (2.0 ** 50, 2.0 ** 52, 2.0 ** 54)
-
-
 # ---------------------------------------------------------------------------------------------------------------
 # the solves a tail runs, with their profiles
 # ---------------------------------------------------------------------------------------------------------------
-@functools.lru_cache(maxsize=None)
-def _qa(N, alpha, delta, in_tok, out_tok, ratio):
-    return _analyzer(N, alpha, 0.0, delta, in_tok, out_tok, ratio)
-
-
 class _Solves:
     """(rates, K, lambda, candidate) of every streaming solve a tail runs, profiled in one vectorised pass."""
 
@@ -121,13 +97,6 @@ class _Solves:
         P["K"] = np.array(self.K)
         P["cand"] = list(self.cand)
         return P
-
-
-def _model(fleet, s, row=None):
-    """(N, alpha, delta, in, out, ratio) of server s's only pair; row: (in, out) in place of the fleet's tokens."""
-    it, ot = (int(fleet.srv_in_tokens[s]), int(fleet.srv_out_tokens[s])) if row is None else row
-    return (int(fleet.srv_max_batch[s]), float(fleet.perf_alpha[s, 0]), float(fleet.perf_delta[s, 0]), it, ot,
-            int(fleet.max_queue_to_batch_ratio))
 
 
 def _final_lam(rpm, tps, out_tok, replicas):
@@ -174,45 +143,6 @@ def _lam_star_max(qa):
 # ---------------------------------------------------------------------------------------------------------------
 # fleets and rows
 # ---------------------------------------------------------------------------------------------------------------
-def _main_fleet(n=MAIN_N, delta=DELTA):
-    """One server per batch size, alpha = 1, no target, min_replicas 1, queue ratio 10."""
-    return _fleet(1.0, 0.0, np.ones(len(n)), list(n), delta=delta, ratio=SIZE_RATIO)
-
-
-def _x_rpm(xs):
-    """Arrival rates whose one-replica lambda is exactly f32(x) (x = lambda at alpha = 1)."""
-    return np.array([_rpm_for_lambda(f32(x)) for x in xs], np.float32)
-
-
-def _edge_fleet():
-    """N = 16, delta = 0: the four rate-edge models (one server each) and the three lambda-edge models."""
-    alphas = [a for a, _ in _rate_edge_models(EDGE_N)] + list(LAM_EDGE_ALPHAS)
-    return _fleet(alphas, 0.0, np.ones(len(alphas)), EDGE_N, ratio=SIZE_RATIO)
-
-
-def _edge_rpm(fleet):
-    """[3, S] rows of the edge fleet: x in EDGE_XS on the rate-edge servers; lambda on 2^-60, one ulp below, on
-    2^-60 on the lambda-edge servers."""
-    cols = []
-    for s in range(fleet.n_servers):
-        c = np.float64(f32(fleet.perf_alpha[s, 0]))
-        if s < 4:
-            cols.append([_rpm_for_lambda(x / c) for x in EDGE_XS])
-        else:
-            cols.append([_rpm_for_lambda(v) for v in (2.0 ** -60, BELOW(2.0 ** -60), 2.0 ** -60)])
-    return np.array(cols, np.float32).T.copy()
-
-
-def load_cases():
-    """(fleet, rpm [L, S]) of the load grid: the main fleet at XS (both servers), the K >= 2^23 candidate at
-    LONG_XS, the edge fleet."""
-    main = _main_fleet()
-    rpm = np.repeat(_x_rpm(XS)[:, None], main.n_servers, axis=1)
-    long = _fleet(1.0, 0.0, [1.0], [682], delta=0.0, ratio=LONG_RATIO)
-    edge = _edge_fleet()
-    return [(main, rpm), (long, _x_rpm(LONG_XS)[:, None].copy()), (edge, _edge_rpm(edge))]
-
-
 def interval_cases():
     """(fleet, lo, hi, M): one server per x of XS (and more near E(sum) 680), N alternating 1024 / 900, with lo = hi
     (one interval, starting at lo); two N = 1024 servers from x = 400 to 3.5 and 2.5 rateStar, whose starts at 2, 3
@@ -249,69 +179,6 @@ def workload_cases():
     return out
 
 
-def profile_cases():
-    """(fleet, rows): lambda fixed at 1 req/ms (rpm 60000), rows of perf_alpha = XS, so x = alpha; the edge models
-    with their own rate and alpha fixed, and the lambda-edge models at lambda = 2^-60 with alpha 2^50 .. 2^54."""
-    main = _main_fleet()
-    main.srv_arrival_rpm[:] = f32(60000.0)
-    alpha = np.repeat(XS.astype(np.float32)[:, None, None], main.n_servers, axis=1)
-    out = [(main, {"perf_alpha": alpha})]
-    # edge: one server per (rate-edge model, x) and per lambda edge; rows of alpha (3 rows)
-    ea, erpm, rows = [], [], []
-    for a, _ in _rate_edge_models(EDGE_N):
-        c = np.float64(f32(a))
-        for x in EDGE_XS:
-            ea.append(a)
-            erpm.append(_rpm_for_lambda(x / c))
-            rows.append([a] * 3)
-    for lam in (2.0 ** -60, BELOW(2.0 ** -60)):
-        ea.append(LAM_EDGE_ALPHAS[0])
-        erpm.append(_rpm_for_lambda(lam))
-        rows.append(list(LAM_EDGE_ALPHAS))
-    edge = _fleet(ea, 0.0, erpm, EDGE_N, ratio=SIZE_RATIO)
-    out.append((edge, {"perf_alpha": np.array(rows, np.float32).T[:, :, None].copy()}))
-    return out
-
-
-def _ttft_targets(qa, xs):
-    return [f32(qa.eval_ttft(float(f32(x)))[1]) for x in xs]
-
-
-def slo_cases():
-    """(fleet, (itl, ttft, tps) [L, S]): the main fleet at 60 req/min with TTFT rows whose searched lambda* lands on
-    XS (all of its E(sum) 680 block, every other x above it), then TPS-only rows whose final rate is x = XS (lambda* =
-    0.9 lambda_max overflows, so these items run in the stored re-run); the edge fleet with TPS-only rows; the
-    K >= 2^23 candidates with one TPS row."""
-    main = _main_fleet()
-    main.srv_arrival_rpm[:] = 60.0
-    S = main.n_servers
-    qa = _qa(*_model(main, 0))
-    ttft = np.array(_ttft_targets(qa, np.concatenate([XS[XS < 500], XS[XS > 500][::2]])), np.float32)
-    L1 = ttft.size
-    tps = (f32(2000) * XS.astype(np.float32)).astype(np.float32)
-    L = L1 + tps.size
-    itl_r = np.zeros((L, S), np.float32)
-    ttft_r = np.zeros((L, S), np.float32)
-    tps_r = np.zeros((L, S), np.float32)
-    ttft_r[:L1] = ttft[:, None]
-    tps_r[L1:] = tps[:, None]
-    out = [(main, (itl_r, ttft_r, tps_r))]
-    edge = _edge_fleet()
-    et = np.zeros((3, edge.n_servers), np.float32)
-    for s in range(edge.n_servers):
-        a = float(edge.perf_alpha[s, 0])
-        if s < 4:
-            ls = float(_lam_star(_qa(EDGE_N, a, 0.0, 1, 2, SIZE_RATIO)))
-            et[:, s] = [f32(2.0 * ls * 1000.0 * fr) for fr in (0.2, 0.5, 0.9)]
-        else:
-            et[:, s] = [f32(np.float64(f32(v)) * 2000.0) for v in (2.0 ** -60, BELOW(2.0 ** -60), 2.0 ** -60)]
-    out.append((edge, (np.zeros_like(et), np.zeros_like(et), et)))
-    lq = long_queue_fleet().take_servers(np.array([0, 1]))
-    tp = lq.srv_slo_tps[None, :].copy()
-    out.append((lq, (np.zeros_like(tp), np.zeros_like(tp), tp)))
-    return out
-
-
 def slo_trace_rows(fleet, rows):
     """The six row lists of wva_slo_trace for an SLO grid case: the fleet's own load at every tick."""
     itl, ttft, tps = rows
@@ -321,46 +188,13 @@ def slo_trace_rows(fleet, rows):
             rep(fleet.srv_out_tokens).astype(np.int32), itl, ttft, tps)
 
 
-def _alpha_for(N, which, edge, below):
-    """A float32 alpha whose lambda_min (which 0) or lambda_max (which 1) is exactly edge, or with below, the
-    nearest reachable float32 under it (delta = 0)."""
-    a0 = int(np.array([0.001 / edge if which == 0 else N * 0.999 / edge], np.float32).view(np.uint32)[0])
-    for k in sorted(range(-512, 513), key=abs):
-        a = np.array([a0 + k], np.uint32).view(np.float32)[0]
-        v = lam_range(_qa(N, float(a), 0.0, 1, 2, SIZE_RATIO))[which]
-        if (v < f32(edge) and v >= f32(edge * (1 - 2.0 ** -20))) if below else v == f32(edge):
-            return float(a)
-    raise AssertionError(f"no alpha puts lambda {'min max'.split()[which]} on {edge!r} (below: {below})")
-
-
-def bounds_cases():
-    """Fleets of wva_slo_bounds: N from 465 to 481 (E(sum) 680 at lambda_max), 608 to 632 (E(max p) 880, E(sum) 900)
-    and every other N from 700 to 740 (float64 overflow), each at delta 1e-5 .. 6e-5; the rate edges at N = 16, 24
-    and 32; lambda_min on 2^-60 and just below, lambda_max on 2^60 and just below."""
-    Ns = list(range(465, 481)) + list(range(608, 632)) + list(range(700, 740, 2))
-    rows = [(N, d) for N in Ns for d in (1e-5, 2e-5, 3e-5, 4e-5, 5e-5, 6e-5)]
-    main = _fleet(1.0, 0.0, np.full(len(rows), 600.0), [r[0] for r in rows], delta=[r[1] for r in rows],
-                  ratio=SIZE_RATIO)
-    ea, en = [], []
-    for N in (16, 24, 32):
-        for a, _ in _rate_edge_models(N):
-            ea.append(a)
-            en.append(N)
-        for which, edge in ((0, 2.0 ** -60), (1, P60)):
-            for below in (False, True):
-                ea.append(_alpha_for(N, which, edge, below))
-                en.append(N)
-    edge = _fleet(ea, 0.0, np.full(len(ea), 600.0), en, ratio=SIZE_RATIO)
-    return [main, edge]
-
-
 # ---------------------------------------------------------------------------------------------------------------
 # the oracle's results and the solves behind them, once per module
 # ---------------------------------------------------------------------------------------------------------------
 def _load_solves(oracle_mod):
     S, calls = _Solves(), []
     for k, (fleet, rpm) in enumerate(load_cases()):
-        cand, win = ref_load_grid(oracle_mod, fleet, rpm)
+        cand, win = ref_grid(oracle_mod, fleet, {"arrival_rpm": rpm})
         calls.append((cand, win))
         _add_finals(S, cand, fleet, rpm, np.zeros_like(rpm), lambda l, s, f=fleet: (1, 2), ("load", k))
     return S.profile(), calls
@@ -383,7 +217,7 @@ def _interval_solves(oracle_mod):
 def _workload_solves(oracle_mod, trace):
     S, calls = _Solves(), []
     for k, (fleet, (rpm, it, ot)) in enumerate(workload_cases()):
-        got = (ref_trace if trace else ref_workload_grid)(oracle_mod, fleet, rpm, it, ot)
+        got = (ref_trace if trace else ref_grid)(oracle_mod, fleet, dict(zip(LOAD, (rpm, it, ot))))
         calls.append(got[:2])
         _add_finals(S, got[0], fleet, rpm, np.zeros_like(rpm), lambda l, s: (int(it[l, s]), int(ot[l, s])),
                     ("wl", k))
@@ -394,9 +228,9 @@ def _profile_solves(oracle_mod, trace):
     S, calls = _Solves(), []
     for k, (fleet, rows) in enumerate(profile_cases()):
         if trace:
-            got = ref_profile_trace(oracle_mod, fleet, rows)
+            got = ref_trace(oracle_mod, fleet, rows)
         else:
-            got = ref_profile_grid(oracle_mod, fleet, rows)
+            got = ref_grid(oracle_mod, fleet, rows)
         calls.append(got[:2])
         L, Sn = rows["perf_alpha"].shape[:2]
         c = got[0].reshape(L, Sn)
@@ -430,9 +264,9 @@ def _slo_solves(oracle_mod, trace):
     for k, (fleet, rows) in enumerate(slo_cases()):
         itl, ttft, tps = rows
         if trace:
-            got = ref_slo_trace(oracle_mod, fleet, slo_trace_rows(fleet, rows))
+            got = ref_trace(oracle_mod, fleet, dict(zip(LOAD + SLO, slo_trace_rows(fleet, rows))))[:2]
         else:
-            got = ref_slo_grid(oracle_mod, fleet, *rows)
+            got = ref_grid(oracle_mod, fleet, dict(zip(SLO, rows)))
         calls.append(got)
         L, Sn = itl.shape
         c = got[0].reshape(L, Sn)
@@ -650,10 +484,10 @@ def grid_refs(oracle_mod):
         if (what, case) not in cache:
             if what == "load":
                 fleet, rpm = load_cases()[case]
-                cache[what, case] = fleet, rpm, ref_load_grid(oracle_mod, fleet, rpm)
+                cache[what, case] = fleet, rpm, ref_grid(oracle_mod, fleet, {"arrival_rpm": rpm})
             else:
                 fleet, rows = slo_cases()[case]
-                cache[what, case] = fleet, rows, ref_slo_grid(oracle_mod, fleet, *rows)
+                cache[what, case] = fleet, rows, ref_grid(oracle_mod, fleet, dict(zip(SLO, rows)))
         return cache[what, case]
     return get
 
@@ -677,7 +511,7 @@ def test_load_grid_at_window_edges(engine, grid_refs, monkeypatch, case, phase1)
 @pytest.mark.parametrize("case", range(2))
 def test_load_intervals_at_window_edges(engine, oracle_mod, case):
     fleet, lo, hi, M = interval_cases()[case]
-    count, _ = intervals_check(engine, oracle_mod, fleet, lo, hi, M, f"intervals case {case}")
+    count, _ = check_intervals(engine, oracle_mod, fleet, lo, hi, M, f"intervals case {case}")
     assert count.sum() >= fleet.n_servers
 
 
@@ -686,8 +520,8 @@ def test_load_intervals_at_window_edges(engine, oracle_mod, case):
 @pytest.mark.parametrize("case", range(2))
 def test_workload_at_window_edges(engine, oracle_mod, case, trace):
     fleet, rows = workload_cases()[case]
-    check = workload_trace_check if trace else workload_grid_check
-    check(engine, oracle_mod, fleet, rows, f"workload {'trace' if trace else 'grid'} case {case}")
+    check_level_call(engine, oracle_mod, "workload_trace" if trace else "workload_grid", fleet, dict(zip(LOAD, rows)),
+                     f"workload {'trace' if trace else 'grid'} case {case}")
 
 
 @pytest.mark.gpu
@@ -696,9 +530,9 @@ def test_workload_at_window_edges(engine, oracle_mod, case, trace):
 def test_profile_at_window_edges(engine, oracle_mod, case, trace):
     fleet, rows = profile_cases()[case]
     if trace:
-        profile_trace_check(engine, oracle_mod, fleet, rows, f"profile trace case {case}")
+        check_level_call(engine, oracle_mod, "profile_trace", fleet, rows, f"profile trace case {case}")
     else:
-        profile_grid_check(engine, oracle_mod, fleet, rows, f"profile grid case {case}")
+        check_level_call(engine, oracle_mod, "profile_grid", fleet, rows, f"profile grid case {case}")
 
 
 @pytest.mark.gpu
@@ -716,11 +550,12 @@ def test_slo_grid_at_window_edges(engine, grid_refs, monkeypatch, case, phase1):
 @pytest.mark.parametrize("case", range(2))
 def test_slo_trace_at_window_edges(engine, oracle_mod, case):
     fleet, rows = slo_cases()[case]
-    slo_trace_check(engine, oracle_mod, fleet, slo_trace_rows(fleet, rows), f"SLO trace case {case}")
+    check_level_call(engine, oracle_mod, "slo_trace", fleet, dict(zip(LOAD + SLO, slo_trace_rows(fleet, rows))),
+                     f"SLO trace case {case}")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", range(2))
 def test_slo_bounds_at_window_edges(engine, oracle_mod, case):
-    kind = bounds_check(engine, oracle_mod, bounds_cases()[case], f"bounds case {case}")[0]
+    kind = check_slo_bounds(engine, oracle_mod, bounds_cases()[case], f"bounds case {case}")[0]
     assert (kind >= 2).any()

@@ -12,80 +12,23 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import (_code, _f32_bits, _same, load_levels, mixed_fleet, overflow_fleet, pair_batch,
-                                      rates_at_rate_star, tail)
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.util import ALLOC_FIELDS, assert_allocs_equal
+from tests.levels import (LOAD, _adversarial_fleet, at_row, check_level_call, load_levels, mixed_fleet, overflow_fleet,
+                          pair_batch, rates_at_rate_star, ref_grid, tail, token_fleet, workload_levels)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
+                        error_code, f32_bits, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, greedy_solve, synth_fleet
 
 F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-
-
-def at_level(fleet, rpm, in_tok, out_tok, unlimited=True):
-    """A copy of the fleet with the load of row (rpm, in_tok, out_tok)."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    f.srv_arrival_rpm[:] = rpm
-    f.srv_in_tokens[:] = in_tok
-    f.srv_out_tokens[:] = out_tok
-    f.unlimited = unlimited
-    return f
-
-
-def ref_workload_grid(oracle_mod, fleet, rpm, in_tok, out_tok):
-    """(candidates [L*S*A], winners [L*S]): Server.Calculate and Solver.Solve (unlimited) per level."""
-    cands, wins = [np.zeros(0, oracle_mod.ALLOC_DTYPE)], [np.zeros(0, oracle_mod.ALLOC_DTYPE)]
-    for l in range(rpm.shape[0]):
-        f = at_level(fleet, rpm[l], in_tok[l], out_tok[l])
-        cand = oracle_mod.calculate(f)
-        cands.append(cand.reshape(-1))
-        wins.append(oracle_mod.solve(f, cand)[1])
-    return np.concatenate(cands), np.concatenate(wins)
-
-
-def token_fleet(n_servers, n_acc, seed, keep):
-    """mixed_fleet with every other server's batch size from the perf data (N = MaxBatchSize * AtTokens /
-    out_tokens, so N follows the level's out_tokens), and perf batch sizes kept small so that out_tokens 1 stays a
-    cheap model."""
-    f = mixed_fleet(n_servers, n_acc, seed, keep)
-    f.srv_max_batch[::2] = 0
-    f.perf_max_batch[:] = np.minimum(f.perf_max_batch, 32)
-    return f
-
-
-def workload_levels(fleet, L, seed, special=True):
-    """(rpm, in, out), each [L, S]: per (level, server) a rate-only, token-only or joint change of the server's own
-    load (non-monotone over the levels), out_tokens from {0.75, 1, 1.5} x own, and with `special` the edge tokens
-    scattered over them: in -1, out -1, out 0, in 0, in large, out 1 and out large enough for N = 1."""
-    rng = np.random.default_rng(seed)
-    S = fleet.n_servers
-    rpm = load_levels(fleet, L, seed + 1)
-    own_in = np.broadcast_to(fleet.srv_in_tokens, (L, S))
-    own_out = np.broadcast_to(fleet.srv_out_tokens, (L, S))
-    in_f = rng.choice([0.5, 1.0, 2.0], (L, S))
-    out_f = rng.choice([0.75, 1.0, 1.5], (L, S))
-    mode = rng.integers(0, 3, (L, S))  # 0: rate only, 1: tokens only, 2: both
-    in_tok = np.where(mode == 0, own_in, np.maximum(own_in * in_f, 0)).astype(np.int32)
-    out_tok = np.where(mode == 0, own_out, np.maximum(own_out * out_f, 1)).astype(np.int32)
-    rpm = np.where(mode == 1, fleet.srv_arrival_rpm[None, :], rpm).astype(np.float32)
-    if special:
-        for k, (col, v) in enumerate((("in", -1), ("out", -1), ("out", 0), ("in", 0), ("in", 100000), ("out", 1),
-                                      ("out", 20000))):
-            (in_tok if col == "in" else out_tok)[(k + 1) % L, k % 3::4 + k] = v
-    return rpm, in_tok, out_tok
-
-
 # ---- CPU: the composition and the split --------------------------------------------------------
 
 @pytest.mark.parametrize("keep", [False, True])
 def test_one_level_is_the_oracle_solve(oracle_mod, keep):
     fleet = token_fleet(12, 3, 5, keep)
     rows = [c[None, :] for c in (fleet.srv_arrival_rpm, fleet.srv_in_tokens, fleet.srv_out_tokens)]
-    cand, win = ref_workload_grid(oracle_mod, fleet, *rows)
-    cand_o, win_o = oracle_mod.solve(at_level(fleet, *[r[0] for r in rows]))
-    assert _same(cand, cand_o.reshape(-1))
-    assert _same(win, win_o)
+    cand, win = ref_grid(oracle_mod, fleet, dict(zip(LOAD, rows)))
+    cand_o, win_o = oracle_mod.solve(at_row(fleet, dict(zip(LOAD, rows)), 0))
+    assert same_bytes(cand, cand_o.reshape(-1))
+    assert same_bytes(win, win_o)
     assert win["feasible"].sum() >= 4
 
 
@@ -127,11 +70,11 @@ def test_size_once_per_token_key_then_the_tail_is_create_allocation(oracle_mod, 
             if not fleet.perf_present[m, a]:
                 continue
             for in_tok, out_tok in sorted(keys):
-                fk = at_level(fleet, fleet.srv_arrival_rpm, np.full(S, in_tok), np.full(S, out_tok))
+                fk = at_row(fleet, {"in_tokens": [np.full(S, in_tok)], "out_tokens": [np.full(S, out_tok)]}, 0)
                 sz = _size(oracle_mod, fk, s, a)
                 sized += 1
                 for rpm in rates:
-                    want = oracle_mod.create_allocation(at_level(fk, np.full(S, rpm, F32), in_tok, out_tok), s, a)
+                    want = oracle_mod.create_allocation(at_row(fk, {"arrival_rpm": [np.full(S, rpm, F32)], "in_tokens": [in_tok], "out_tokens": [out_tok]}, 0), s, a)
                     if rpm <= 0:
                         assert want["feasible"] == int(rpm == 0), (s, a, rpm)  # nil, or zeroLoadAllocation
                         continue
@@ -145,7 +88,7 @@ def test_size_once_per_token_key_then_the_tail_is_create_allocation(oracle_mod, 
                         continue
                     for k in ALLOC_FIELDS:
                         if k in ("cost", "value", "itl", "ttft", "rho", "max_rate"):
-                            assert _f32_bits(got[k]) == _f32_bits(want[k]), (s, a, rpm, in_tok, out_tok, k)
+                            assert f32_bits(got[k]) == f32_bits(want[k]), (s, a, rpm, in_tok, out_tok, k)
                         else:
                             assert int(got[k]) == int(want[k]), (s, a, rpm, in_tok, out_tok, k)
                     checked += int(want["feasible"])
@@ -156,7 +99,7 @@ def test_same_tokens_give_the_same_rate_star_at_every_rate(oracle_mod):
     fleet = token_fleet(20, 3, 7, False)
     L = 8
     rpm, in_tok, out_tok = workload_levels(fleet, L, 9, special=False)
-    cand, _ = ref_workload_grid(oracle_mod, fleet, rpm, in_tok, out_tok)
+    cand, _ = ref_grid(oracle_mod, fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))))
     cand = cand.reshape(L, fleet.n_servers, fleet.n_acc)
     load = ~(rpm < 0) & (rpm != 0)
     keys = multi = 0
@@ -165,7 +108,7 @@ def test_same_tokens_give_the_same_rate_star_at_every_rate(oracle_mod):
             by_key = {}
             for l in range(L):
                 if load[l, s] and cand[l, s, a]["feasible"]:
-                    by_key.setdefault((in_tok[l, s], out_tok[l, s]), set()).add(_f32_bits(cand[l, s, a]["max_rate"]))
+                    by_key.setdefault((in_tok[l, s], out_tok[l, s]), set()).add(f32_bits(cand[l, s, a]["max_rate"]))
             assert all(len(v) == 1 for v in by_key.values()), (s, a, by_key)
             keys += len(by_key)
             multi += len(set().union(*by_key.values())) > 1 if by_key else 0
@@ -174,19 +117,11 @@ def test_same_tokens_give_the_same_rate_star_at_every_rate(oracle_mod):
 
 # ---- GPU: bit for bit against the composition -------------------------------------------------
 
-def _check(engine, oracle_mod, fleet, rows, what):
-    cand_o, win_o = ref_workload_grid(oracle_mod, fleet, *rows)
-    cand_g, win_g = engine.workload_grid(fleet, *rows, want_candidates=True)
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return cand_o, win_o
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
     fleet = token_fleet(14, 3, 31, keep)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, workload_levels(fleet, 7, 3), f"warp path, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "workload_grid", fleet, dict(zip(LOAD, workload_levels(fleet, 7, 3))), f"warp path, keep = {keep}")
     assert cand_o["feasible"].sum() > 40
     assert len(set(win_o["replicas"][win_o["feasible"] == 1].tolist())) >= 3
 
@@ -196,7 +131,7 @@ def rounds_case(oracle_mod):
     fleet = token_fleet(120, 4, 37, False)
     fleet.srv_keep_acc[::2] = 1
     rows = workload_levels(fleet, 4, 11)
-    return fleet, rows, ref_workload_grid(oracle_mod, fleet, *rows)
+    return fleet, rows, ref_grid(oracle_mod, fleet, dict(zip(LOAD, rows)))
 
 
 @pytest.mark.gpu
@@ -224,7 +159,7 @@ def test_cartesian_rate_by_out_tokens_grid(engine, oracle_mod, monkeypatch, roun
             rows[2].append(np.maximum(fleet.srv_out_tokens * fo, 1).astype(np.int32))
     rows = [np.array(r) for r in rows]
     rows[0] = rows[0].astype(np.float32)
-    _check(engine, oracle_mod, fleet, rows, f"rate x out_tokens, rounds = {rounds}")
+    check_level_call(engine, oracle_mod, "workload_grid", fleet, dict(zip(LOAD, rows)), f"rate x out_tokens, rounds = {rounds}")
 
 
 @pytest.mark.gpu
@@ -244,7 +179,7 @@ def test_edge_tokens(engine, oracle_mod):
     in_tok[3] = 0
     out_tok[4] = fleet.srv_out_tokens * 2
     out_tok[5] = np.maximum(fleet.srv_out_tokens // 3, 1)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), "edge tokens")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "workload_grid", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), "edge tokens")
     cand_o = cand_o.reshape(6, S, fleet.n_acc)
     assert not cand_o[0]["feasible"].any() and not cand_o[1]["feasible"].any()
     assert (cand_o[2]["rho"] == 0).all() and cand_o[2]["feasible"].sum() >= S
@@ -270,7 +205,7 @@ def test_stored_vector_fallback_both_phases(engine, oracle_mod):
     out_tok[1::4] = 128
     out_tok[3::7, 0] = 32
     in_tok = np.full((L, S), 64, np.int32)
-    cand_o, _ = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), "stored-vector fallback")
+    cand_o, _ = check_level_call(engine, oracle_mod, "workload_grid", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), "stored-vector fallback")
     assert cand_o["feasible"].sum() >= L
 
 
@@ -283,7 +218,7 @@ def test_nan_and_huge_values_and_ties(engine, oracle_mod):
     fleet.perf_alpha[:, 2] = fleet.perf_alpha[:, 1]  # accelerators 1 and 2 identical: ties on value
     for k in ("perf_beta", "perf_gamma", "perf_delta", "perf_acc_count"):
         getattr(fleet, k)[:, 2] = getattr(fleet, k)[:, 1]
-    _check(engine, oracle_mod, fleet, workload_levels(fleet, 4, 17), "NaN / huge values and ties")
+    check_level_call(engine, oracle_mod, "workload_grid", fleet, dict(zip(LOAD, workload_levels(fleet, 4, 17))), "NaN / huge values and ties")
 
 
 @pytest.mark.gpu
@@ -294,7 +229,7 @@ def test_each_block_is_the_greedy_input_of_its_level(engine, oracle_mod):
     cand_g, _ = engine.workload_grid(fleet, *rows, want_candidates=True)
     S, A = fleet.n_servers, fleet.n_acc
     for l in range(4):
-        fl = at_level(fleet, rows[0][l], rows[1][l], rows[2][l], unlimited=False)
+        fl = at_row(fleet, dict(zip(LOAD, rows)), l, unlimited=False)
         block = Allocs(S * A)
         for k in ALLOC_FIELDS:
             getattr(block, k)[:] = getattr(cand_g, k)[l * S * A:(l + 1) * S * A]
@@ -318,8 +253,8 @@ def test_own_tokens_are_the_load_grid(engine, monkeypatch, rounds):
     cand_w, win_w = engine.workload_grid(fleet, rpm, want_candidates=True)
     n2 = engine.launch_count
     for k in ALLOC_FIELDS:
-        assert _same(getattr(cand_w, k), getattr(cand_l, k)), k
-        assert _same(getattr(win_w, k), getattr(win_l, k)), k
+        assert same_bytes(getattr(cand_w, k), getattr(cand_l, k)), k
+        assert same_bytes(getattr(win_w, k), getattr(win_l, k)), k
     assert n2 - n1 == n1 - n0
 
 
@@ -334,8 +269,8 @@ def test_each_level_is_update_load_and_resolve(engine):
         engine.update_load(rows[0][l], rows[1][l], rows[2][l])
         cand_r, win_r = engine.resolve(want_candidates=True)
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[l * S * A:(l + 1) * S * A], getattr(cand_r, k)), (l, k)
-            assert _same(getattr(win_g, k)[l * S:(l + 1) * S], getattr(win_r, k)), (l, k)
+            assert same_bytes(getattr(cand_g, k)[l * S * A:(l + 1) * S * A], getattr(cand_r, k)), (l, k)
+            assert same_bytes(getattr(win_g, k)[l * S:(l + 1) * S], getattr(win_r, k)), (l, k)
 
 
 @pytest.mark.gpu
@@ -447,15 +382,15 @@ def test_small_out_tokens_fail_only_under_load(engine):
     out_tok[2, 1] = 1         # server 1 takes its batch size from the fleet: out_tokens 1 is fine there
     cand_g, _ = engine.workload_grid(fleet, rpm, in_tok, out_tok, want_candidates=True)
     for l in range(3):
-        cand_a = engine.analyze(at_level(fleet, rpm[l], in_tok[l], out_tok[l]))
+        cand_a = engine.analyze(at_row(fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), l))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[l * S * 2:(l + 1) * S * 2], getattr(cand_a, k)), (l, k)
+            assert same_bytes(getattr(cand_g, k)[l * S * 2:(l + 1) * S * 2], getattr(cand_a, k)), (l, k)
     rpm[1, 0] = 5.0
-    want, _ = _code(lambda: engine.analyze(at_level(fleet, rpm[1], in_tok[1], out_tok[1])))
+    want, _ = error_code(lambda: engine.analyze(at_row(fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), 1)))
     assert want == WVA_ERR_UNSUPPORTED
-    assert _code(lambda: engine.workload_grid(fleet, rpm, in_tok, out_tok))[0] == want
+    assert error_code(lambda: engine.workload_grid(fleet, rpm, in_tok, out_tok))[0] == want
     out_tok[1, 0] = 0  # out_tokens 0: zeroLoadAllocation at a positive rate
-    assert _code(lambda: engine.workload_grid(fleet, rpm, in_tok, out_tok))[0] == 0
+    assert error_code(lambda: engine.workload_grid(fleet, rpm, in_tok, out_tok))[0] == 0
 
 
 N_ADV = 36
@@ -463,7 +398,7 @@ N_ADV = 36
 
 @pytest.mark.gpu
 def test_workload_grid_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet with random (rate, in, out) rows from the same edge sets,
+    """Fleets from levels._adversarial_fleet with random (rate, in, out) rows from the same edge sets,
     half of them on the rounds.  Where some level's wva_analyze refuses the level, the grid must refuse too."""
     rng = np.random.default_rng(0x70C)
     feasible = refused = 0
@@ -482,12 +417,12 @@ def test_workload_grid_adversarial(engine, oracle_mod, monkeypatch):
         rpm[0], in_tok[0], out_tok[0] = fleet.srv_arrival_rpm, fleet.srv_in_tokens, fleet.srv_out_tokens
         if L > 2:
             in_tok[2], out_tok[2] = in_tok[1], out_tok[1]  # a repeated token row at other rates
-        codes = [_code(lambda: engine.analyze(at_level(fleet, rpm[l], in_tok[l], out_tok[l])))[0] for l in range(L)]
+        codes = [error_code(lambda: engine.analyze(at_row(fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), l)))[0] for l in range(L)]
         if any(codes):
-            got, _ = _code(lambda: engine.workload_grid(fleet, rpm, in_tok, out_tok))
+            got, _ = error_code(lambda: engine.workload_grid(fleet, rpm, in_tok, out_tok))
             assert got == next(c for c in codes if c), (case, codes, got)
             refused += 1
             continue
-        _, win_o = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), f"adversarial case {case}")
+        _, win_o = check_level_call(engine, oracle_mod, "workload_grid", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), f"adversarial case {case}")
         feasible += int(win_o["feasible"].sum())
     assert feasible > 40 and refused < N_ADV // 2

@@ -13,70 +13,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_load_grid import _code, _f32_bits, _same, mixed_fleet, overflow_fleet, rates_at_rate_star
-from tests.test_gpu_parity import _adversarial_fleet
-from tests.test_gpu_workload_grid import at_level, token_fleet, workload_levels
-from tests.util import ALLOC_FIELDS, assert_allocs_equal
+from tests.levels import (LOAD, _adversarial_fleet, _moves, _records, at_row, check_level_call, low_penalty_fleet,
+                          mixed_fleet, overflow_fleet, pinned, rates_at_rate_star, ref_trace, token_fleet,
+                          transition_penalty, workload_levels, wva_fleet)
+from tests.util import (ACC_NONE, ACC_UNKNOWN, ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE,
+                        WVA_ERR_UNSUPPORTED, assert_allocs_equal, error_code, f32_bits, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, synth_fleet
-
-F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-ACC_NONE, ACC_UNKNOWN = -1, -2
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-
-
-def ref_trace(oracle_mod, fleet, rpm, in_tok, out_tok):
-    """(candidates [L*S*A], winners [L*S], the fleet with c_L): per tick, Server.Calculate and Solver.Solve
-    (unlimited) on the fleet with row t and current allocation c_t, then c_{t+1} = apply_winners."""
-    cands, wins = [np.zeros(0, oracle_mod.ALLOC_DTYPE)], [np.zeros(0, oracle_mod.ALLOC_DTYPE)]
-    cur = fleet
-    for t in range(rpm.shape[0]):
-        f = at_level(cur, rpm[t], in_tok[t], out_tok[t])
-        cand = oracle_mod.calculate(f)
-        win = oracle_mod.solve(f, cand)[1]
-        cands.append(cand.reshape(-1))
-        wins.append(win)
-        cur = cur.apply_winners(win)
-    return np.concatenate(cands), np.concatenate(wins), cur
-
-
-def pinned(fleet):
-    """The servers whose accelerator no tick can change (include/wva_b200.h, wva_workload_trace)."""
-    cur = fleet.srv_cur_acc
-    return (fleet.srv_keep_acc != 0) & (cur != ACC_NONE) & ((cur == ACC_UNKNOWN) | (fleet.srv_min_replicas != 0))
-
-
-def transition_penalty(factor, cur_acc, cur_rep, cur_cost, acc, rep, cost):
-    """allocation.go:291-300 in float32; an unknown accelerator name equals no candidate's."""
-    cur_cost, cost = F32(cur_cost), F32(cost)
-    with np.errstate(all="ignore"):
-        if cur_acc == acc and cur_acc != ACC_UNKNOWN:
-            return F32(0.0) if cur_rep == rep else F32(cost - cur_cost)
-        return F32(F32(F32(factor) * F32(cur_cost + cost)) + F32(cost - cur_cost))
-
-
-def low_penalty_fleet(n_servers, n_acc, seed, keep):
-    """token_fleet with AccelPenaltyFactor 0 and every min_replicas 1: the cheapest feasible accelerator wins, so the
-    winners move between accelerators as the load moves."""
-    f = token_fleet(n_servers, n_acc, seed, keep)
-    f.accel_penalty_factor = 0.0
-    f.srv_min_replicas[:] = 1
-    return f
-
-
-def wva_fleet(n_servers, n_acc, seed):
-    """WVA's production configuration: keepAccelerator and min_replicas 1 on every server, each current accelerator
-    a real one with its cost (internal/utils/utils.go:290)."""
-    f = synth_fleet(n_servers, n_acc, seed=seed, keep_accelerator=True)
-    rng = np.random.default_rng(seed)
-    f.srv_min_replicas[:] = 1
-    none = f.srv_cur_acc < 0
-    f.srv_cur_acc[none] = rng.integers(0, n_acc, int(none.sum()))
-    f.srv_cur_replicas[none] = 1
-    a = f.srv_cur_acc
-    f.srv_cur_cost[:] = (f.acc_cost[a] * f.perf_acc_count[f.srv_model, a] * f.srv_cur_replicas).astype(np.float32)
-    return f
-
 
 # ---- CPU: the composition, the state transition and the split ---------------------------------
 
@@ -84,10 +26,10 @@ def wva_fleet(n_servers, n_acc, seed):
 def test_one_tick_is_the_oracle_solve(oracle_mod, keep):
     fleet = token_fleet(12, 3, 5, keep)
     rows = [c[None, :] for c in (fleet.srv_arrival_rpm, fleet.srv_in_tokens, fleet.srv_out_tokens)]
-    cand, win, _ = ref_trace(oracle_mod, fleet, *rows)
-    cand_o, win_o = oracle_mod.solve(at_level(fleet, *[r[0] for r in rows]))
-    assert _same(cand, cand_o.reshape(-1))
-    assert _same(win, win_o)
+    cand, win, _ = ref_trace(oracle_mod, fleet, dict(zip(LOAD, rows)))
+    cand_o, win_o = oracle_mod.solve(at_row(fleet, dict(zip(LOAD, rows)), 0))
+    assert same_bytes(cand, cand_o.reshape(-1))
+    assert same_bytes(win, win_o)
     assert win["feasible"].sum() >= 4
 
 
@@ -112,12 +54,12 @@ def test_apply_winners_hand_built():
     # a copy: the fleet itself and every other column are unchanged
     assert fleet.srv_cur_acc.tolist() == [0, 2, 1] and fleet.srv_cur_cost.tolist() == [23.0, 260.0, 80.0]
     for n in ("srv_arrival_rpm", "srv_keep_acc", "srv_min_replicas", "acc_cost", "perf_alpha"):
-        assert _same(getattr(nxt, n), getattr(fleet, n)), n
+        assert same_bytes(getattr(nxt, n), getattr(fleet, n)), n
     # the oracle's structured winners work the same way
     rec = np.zeros(3, [("feasible", "<i4"), ("acc", "<i4"), ("replicas", "<i4"), ("cost", "<f4")])
     for k in rec.dtype.names:
         rec[k] = getattr(win, k)
-    assert _same(fleet.apply_winners(rec).srv_cur_cost, nxt.srv_cur_cost)
+    assert same_bytes(fleet.apply_winners(rec).srv_cur_cost, nxt.srv_cur_cost)
     with pytest.raises(ValueError):
         fleet.apply_winners(Allocs(2))
 
@@ -142,14 +84,14 @@ def test_create_allocation_does_not_read_the_current_allocation(oracle_mod, seed
             for a in range(A):
                 rec = oracle_mod.create_allocation(f, s, a)
                 for k in ALLOC_FIELDS:
-                    assert _f32_bits(rec[k]) == _f32_bits(base[s][a][k]), (trial, s, a, k)
+                    assert f32_bits(rec[k]) == f32_bits(base[s][a][k]), (trial, s, a, k)
                 for k in ALLOC_FIELDS:
                     if k != "value":
-                        assert _f32_bits(cand[s, a][k]) == _f32_bits(rec[k]), (trial, s, a, k)
+                        assert f32_bits(cand[s, a][k]) == f32_bits(rec[k]), (trial, s, a, k)
                 if rec["feasible"]:
                     want = transition_penalty(f.accel_penalty_factor, f.srv_cur_acc[s], f.srv_cur_replicas[s],
                                               f.srv_cur_cost[s], rec["acc"], rec["replicas"], rec["cost"])
-                    assert _f32_bits(cand[s, a]["value"]) == _f32_bits(want), (trial, s, a)
+                    assert f32_bits(cand[s, a]["value"]) == f32_bits(want), (trial, s, a)
                     checked += 1
     assert checked >= 60
 
@@ -167,7 +109,7 @@ def test_pinned_servers_never_move(oracle_mod, seed):
     rpm[2, ::4] = 0.0  # zero-load ticks release the min_replicas 0 servers
     pin = pinned(fleet)
     assert pin.sum() >= 8 and (~pin & (fleet.srv_keep_acc != 0)).sum() >= 4 and pin[4] and pin[5]
-    cand, win, _ = ref_trace(oracle_mod, fleet, rpm, in_tok, out_tok)
+    cand, win, _ = ref_trace(oracle_mod, fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))))
     S, A = fleet.n_servers, fleet.n_acc
     cand, win = cand.reshape(L, S, A), win.reshape(L, S)
     cur = fleet.srv_cur_acc.copy()
@@ -187,34 +129,11 @@ def test_pinned_servers_never_move(oracle_mod, seed):
 
 # ---- GPU: bit for bit against the composition -------------------------------------------------
 
-def _check(engine, oracle_mod, fleet, rows, what):
-    cand_o, win_o, _ = ref_trace(oracle_mod, fleet, *rows)
-    cand_g, win_g = engine.workload_trace(fleet, *rows, want_candidates=True)
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return cand_o, win_o
-
-
-def _records(allocs):
-    """An Allocs as a structured array (the oracle's layout)."""
-    return np.rec.fromarrays([getattr(allocs, k) for k in ALLOC_FIELDS], names=",".join(ALLOC_FIELDS))
-
-
-def _moves(win, S):
-    """(tick, server) pairs at which a feasible winner sits on another real accelerator than the last feasible one."""
-    win = win.reshape(-1, S)
-    n = 0
-    for s in range(S):
-        accs = [int(a) for a, f in zip(win[:, s]["acc"], win[:, s]["feasible"]) if f and a >= 0]
-        n += sum(x != y for x, y in zip(accs, accs[1:]))
-    return n
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
     fleet = token_fleet(14, 3, 31, keep)
-    cand_o, win_o = _check(engine, oracle_mod, fleet, workload_levels(fleet, 7, 3), f"warp path, keep = {keep}")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, workload_levels(fleet, 7, 3))), f"warp path, keep = {keep}")
     assert cand_o["feasible"].sum() > 40
     assert len(set(win_o["replicas"][win_o["feasible"] == 1].tolist())) >= 3
 
@@ -225,7 +144,7 @@ def rounds_case(oracle_mod):
     fleet.srv_keep_acc[::2] = 1
     fleet.accel_penalty_factor = 0.02
     rows = workload_levels(fleet, 4, 11)
-    return fleet, rows, ref_trace(oracle_mod, fleet, *rows)
+    return fleet, rows, ref_trace(oracle_mod, fleet, dict(zip(LOAD, rows)))
 
 
 @pytest.mark.gpu
@@ -252,7 +171,7 @@ def test_winners_move_between_accelerators(engine, oracle_mod, monkeypatch, keep
         fleet.srv_min_replicas[::2] = 0
     rpm, in_tok, out_tok = workload_levels(fleet, 10, 29, special=False)
     rpm[3::4, ::3] = 0.0
-    _, win_o = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), f"moving, keep = {keep}")
+    _, win_o = check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), f"moving, keep = {keep}")
     assert _moves(win_o, fleet.n_servers) >= (3 if keep else 10)
 
 
@@ -261,7 +180,7 @@ def test_wva_configuration_every_server_pinned(engine, oracle_mod):
     fleet = wva_fleet(60, 4, 97)
     assert pinned(fleet).all()
     rows = workload_levels(fleet, 6, 31, special=False)
-    _, win_o = _check(engine, oracle_mod, fleet, rows, "WVA configuration")
+    _, win_o = check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, rows)), "WVA configuration")
     win = win_o.reshape(6, -1)
     for t in range(6):
         f = win[t]["feasible"] != 0
@@ -292,18 +211,18 @@ def test_chain_edges(engine, oracle_mod):
     rpm[0, 0] = -1.0
     rpm[2, 1] = -1.0
     rpm[1, 4] = rpm[1, 5] = 0.0
-    cand_o, win_o = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), "chain edges")
+    cand_o, win_o = check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), "chain edges")
     cand_o, win_o = cand_o.reshape(L, S, A), win_o.reshape(L, S)
     # 0: a nil winner at tick 0, so tick 1's values are against c_0
     assert not win_o[0, 0]["feasible"] and win_o[1, 0]["feasible"]
     c1 = cand_o[1, 0][cand_o[1, 0]["feasible"] != 0][0]
-    assert _f32_bits(c1["value"]) == _f32_bits(transition_penalty(0.0, 1, 2, 80.0, c1["acc"], c1["replicas"],
+    assert f32_bits(c1["value"]) == f32_bits(transition_penalty(0.0, 1, 2, 80.0, c1["acc"], c1["replicas"],
                                                                   c1["cost"]))
     # 1: tick 3 is valued against winner 1
     assert win_o[1, 1]["feasible"] and not win_o[2, 1]["feasible"] and win_o[3, 1]["feasible"]
     w1 = win_o[1, 1]
     c3 = cand_o[3, 1][cand_o[3, 1]["feasible"] != 0][0]
-    assert _f32_bits(c3["value"]) == _f32_bits(transition_penalty(0.0, w1["acc"], w1["replicas"], w1["cost"],
+    assert f32_bits(c3["value"]) == f32_bits(transition_penalty(0.0, w1["acc"], w1["replicas"], w1["cost"],
                                                                   c3["acc"], c3["replicas"], c3["cost"]))
     # 2 and 3
     assert not cand_o[:, 2]["feasible"].any() and not win_o[:, 2]["feasible"].any()
@@ -331,7 +250,7 @@ def test_stored_vector_fallback_both_phases(engine, oracle_mod):
     out_tok[1::4] = 128
     out_tok[3::7, 0] = 32
     in_tok = np.full((L, S), 64, np.int32)
-    cand_o, _ = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), "stored-vector fallback")
+    cand_o, _ = check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), "stored-vector fallback")
     assert cand_o["feasible"].sum() >= L
 
 
@@ -345,7 +264,7 @@ def test_nan_and_huge_values_and_ties(engine, oracle_mod, keep):
     fleet.perf_alpha[:, 2] = fleet.perf_alpha[:, 1]  # accelerators 1 and 2 identical: ties on value
     for k in ("perf_beta", "perf_gamma", "perf_delta", "perf_acc_count"):
         getattr(fleet, k)[:, 2] = getattr(fleet, k)[:, 1]
-    _check(engine, oracle_mod, fleet, workload_levels(fleet, 5, 17), f"NaN / huge values and ties, keep = {keep}")
+    check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, workload_levels(fleet, 5, 17))), f"NaN / huge values and ties, keep = {keep}")
 
 
 @pytest.mark.gpu
@@ -360,16 +279,16 @@ def test_each_tick_is_solve_on_the_advanced_fleet(engine):
     S, A = fleet.n_servers, fleet.n_acc
     cur = fleet
     for t in range(L):
-        cand_s, win_s = engine.solve(at_level(cur, rows[0][t], rows[1][t], rows[2][t]))
+        cand_s, win_s = engine.solve(at_row(cur, dict(zip(LOAD, rows)), t))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
-            assert _same(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
+            assert same_bytes(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
+            assert same_bytes(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
         cur = cur.apply_winners(win_s)
     one = [r[:1] for r in rows]
     for got, want in zip(engine.workload_trace(fleet, *one, want_candidates=True),
                          engine.workload_grid(fleet, *one, want_candidates=True)):
         for k in ALLOC_FIELDS:
-            assert _same(getattr(got, k), getattr(want, k)), k
+            assert same_bytes(getattr(got, k), getattr(want, k)), k
 
 
 @pytest.mark.gpu
@@ -389,8 +308,8 @@ def test_continuation(engine, k):
         cur = cur.apply_winners(_records(win_a)[t * S:(t + 1) * S])
     cand_b, win_b = engine.workload_trace(cur, *[r[k:] for r in rows], want_candidates=True)
     for n in ALLOC_FIELDS:
-        assert _same(getattr(cand, n), np.concatenate([getattr(cand_a, n), getattr(cand_b, n)])), n
-        assert _same(getattr(win, n), np.concatenate([getattr(win_a, n), getattr(win_b, n)])), n
+        assert same_bytes(getattr(cand, n), np.concatenate([getattr(cand_a, n), getattr(cand_b, n)])), n
+        assert same_bytes(getattr(win, n), np.concatenate([getattr(win_a, n), getattr(win_b, n)])), n
     assert _moves(_records(win), S) >= 1
 
 
@@ -418,15 +337,15 @@ def test_pair_excluded_at_every_tick_does_not_fail(engine):
     S, A = fleet.n_servers, fleet.n_acc
     cur = fleet
     for t in range(L):
-        cand_s, win_s = engine.solve(at_level(cur, rpm[t], in_tok[t], out_tok[t]))
+        cand_s, win_s = engine.solve(at_row(cur, dict(zip(LOAD, (rpm, in_tok, out_tok))), t))
         for k in ALLOC_FIELDS:
-            assert _same(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
-            assert _same(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
+            assert same_bytes(getattr(cand_g, k)[t * S * A:(t + 1) * S * A], getattr(cand_s, k)), (t, k)
+            assert same_bytes(getattr(win_g, k)[t * S:(t + 1) * S], getattr(win_s, k)), (t, k)
         cur = cur.apply_winners(win_s)
     assert win_g.feasible[S] == 1 and win_g.acc[S] == 0
     free = fleet.take_servers(np.arange(S))
     free.srv_keep_acc[0] = 0
-    assert _code(lambda: engine.workload_trace(free, rpm, in_tok, out_tok))[0] == WVA_ERR_UNSUPPORTED
+    assert error_code(lambda: engine.workload_trace(free, rpm, in_tok, out_tok))[0] == WVA_ERR_UNSUPPORTED
 
 
 @pytest.mark.gpu
@@ -505,7 +424,7 @@ N_ADV = 30
 
 @pytest.mark.gpu
 def test_workload_trace_adversarial(engine, oracle_mod, monkeypatch):
-    """Fleets from test_gpu_parity's _adversarial_fleet, keep on half the servers, with random (rate, in, out) rows
+    """Fleets from levels._adversarial_fleet, keep on half the servers, with random (rate, in, out) rows
     from the workload grid's edge sets, half of them on the rounds.  Where the per-tick wva_solve loop refuses a
     tick, the trace must refuse too; the trace may refuse beyond that only through a keep server that is not
     pinned."""
@@ -530,11 +449,11 @@ def test_workload_trace_adversarial(engine, oracle_mod, monkeypatch):
         # the per-tick wva_solve loop
         code, cur = 0, fleet
         for t in range(L):
-            code, res = _code(lambda: engine.solve(at_level(cur, rpm[t], in_tok[t], out_tok[t])))
+            code, res = error_code(lambda: engine.solve(at_row(cur, dict(zip(LOAD, (rpm, in_tok, out_tok))), t)))
             if code:
                 break
             cur = cur.apply_winners(res[1])
-        got, _ = _code(lambda: engine.workload_trace(fleet, rpm, in_tok, out_tok))
+        got, _ = error_code(lambda: engine.workload_trace(fleet, rpm, in_tok, out_tok))
         if code:
             assert got == code, (case, code, got)
             refused += 1
@@ -543,6 +462,6 @@ def test_workload_trace_adversarial(engine, oracle_mod, monkeypatch):
             assert got == WVA_ERR_UNSUPPORTED and ((fleet.srv_keep_acc != 0) & ~pinned(fleet)).any(), (case, got)
             extra += 1
             continue
-        _, win_o = _check(engine, oracle_mod, fleet, (rpm, in_tok, out_tok), f"adversarial case {case}")
+        _, win_o = check_level_call(engine, oracle_mod, "workload_trace", fleet, dict(zip(LOAD, (rpm, in_tok, out_tok))), f"adversarial case {case}")
         feasible += int(win_o["feasible"].sum())
     assert feasible > 30 and refused + extra < N_ADV // 2

@@ -6,20 +6,10 @@ GPU: the product's host greedy over device-computed candidates equals the oracle
 import numpy as np
 import pytest
 
+from tests.levels import limited_fleet
 from tests.util import assert_allocs_equal
-from workload_variant_autoscaler_b200 import synth_fleet
 from workload_variant_autoscaler_b200._abi import (SAT_NONE, SAT_PRIORITY_EXHAUSTIVE, SAT_PRIORITY_ROUND_ROBIN,
                                                    SAT_ROUND_ROBIN)
-
-
-def limited_fleet(seed, cap, policy=SAT_NONE, delayed=False, n=24, n_acc=3):
-    f = synth_fleet(n, n_acc, seed=seed, max_batch_choices=(2, 4, 8, 16), zero_load_frac=0.1)
-    f.unlimited = False
-    f.saturation_policy = policy
-    f.delayed_best_effort = delayed
-    f.type_capacity[:] = cap
-    f.srv_priority[:] = np.random.default_rng(seed).choice([1, 5, 10], f.n_servers)
-    return f
 
 
 def used_units(f, win):

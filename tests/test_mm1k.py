@@ -4,8 +4,8 @@ import math
 
 import numpy as np
 import pytest
-
 from tests.util import assert_f32_bits_equal
+
 
 
 def test_go_pow_matches_libm_to_the_accuracy_of_binary_powering(oracle_mod):

@@ -19,25 +19,16 @@ with NaN and the library refuses it, so there is nothing to agree on.
 
 Sampling is deterministic.  Pairs whose batch size comes out above 4096 under the AtTokens rule are left out of the
 adversarial and level-row samples (a Size there costs the restatement seconds); the windows family covers large N."""
-import collections
-
 import numpy as np
 import pytest
 
+from tests import grid_cases, levels
+from tests.levels import (F, LOAD, SLO, TARGETS, TPS_TARGETS, Tally, _restated, at_row, cross_fleet, mixed_fleet,
+                          pair_n, profile_fleet, profile_rows, same_f32, slo_levels, token_fleet, workload_levels)
 from workload_variant_autoscaler_b200 import synth_fleet
 
-F = np.float32
-ALLOC_FLOATS = ("cost", "itl", "ttft", "rho", "max_rate")
 CELL_FLOATS = ("ttft", "itl", "rho", "throughput")
 SWEEP_FLOATS = ("ttft", "itl", "throughput", "rho")
-BIG_N = 4096
-
-
-def _same(a, b):
-    a, b = F(a), F(b)
-    return (np.isnan(a) and np.isnan(b)) or a.view(np.uint32) == b.view(np.uint32)
-
-
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_create_allocation_cross(oracle_mod, seed):
     from oracle import restate_np as R
@@ -54,7 +45,7 @@ def test_create_allocation_cross(oracle_mod, seed):
             n_feas += 1
             assert (o["acc"], o["replicas"], o["batch"]) == (r["acc"], r["replicas"], r["batch"]), (s, a, o, r)
             for k in ("cost", "itl", "ttft", "rho", "max_rate"):
-                assert _same(o[k], r[k]), (s, a, k, o[k], r[k])
+                assert same_f32(o[k], r[k]), (s, a, k, o[k], r[k])
     assert n_feas >= 15
 
 
@@ -70,7 +61,7 @@ def test_analyze_and_solve_cross(oracle_mod):
         rq = R.QA(N, 10 * N, al, be, ga, de, it, ot)
         assert np.array_equal(qa.serv_rate().view(np.uint32), rq.sr.view(np.uint32))
         rmin, rmax = qa.rate_range()
-        assert _same(rmin, rq.rmin) and _same(rmax, rq.rmax)
+        assert same_f32(rmin, rq.rmin) and same_f32(rmax, rq.rmax)
         for frac in (0.0, 0.3, 0.7, 1.0):
             rate = F(rmin + F(frac) * (rmax - rmin))
             err, m = qa.analyze(float(rate))
@@ -78,9 +69,9 @@ def test_analyze_and_solve_cross(oracle_mod):
             assert (err == 0) == (mr is not None)
             if mr is None:
                 continue
-            assert _same(m["throughput"], mr["throughput"]) and _same(m["avg_wait_time"], mr["wait"])
-            assert _same(m["avg_prefill_time"], mr["prefill"]) and _same(m["avg_token_time"], mr["itl"])
-            assert _same(m["rho"], mr["rho"])
+            assert same_f32(m["throughput"], mr["throughput"]) and same_f32(m["avg_wait_time"], mr["wait"])
+            assert same_f32(m["avg_prefill_time"], mr["prefill"]) and same_f32(m["avg_token_time"], mr["itl"])
+            assert same_f32(m["rho"], mr["rho"])
             assert np.array_equal(qa.probs().view(np.uint64), rq.p.view(np.uint64))
 
 
@@ -96,57 +87,12 @@ def test_overflow_rescale_cross(oracle_mod):
     mr = rq.analyze(rate)
     assert err == 0 and mr is not None
     assert np.array_equal(qa.probs().view(np.uint64), rq.p.view(np.uint64))
-    assert _same(m["avg_wait_time"], mr["wait"]) and _same(m["rho"], mr["rho"])
+    assert same_f32(m["avg_wait_time"], mr["wait"]) and same_f32(m["rho"], mr["rho"])
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # the comparison of one point
 # ---------------------------------------------------------------------------------------------------------------
-class Tally:
-    """Points a family covered: feasible / infeasible records (or cells, or sweep points), refusals by reason,
-    probability vectors compared, and pairs left out for their batch size."""
-
-    def __init__(self):
-        self.n = collections.Counter()
-
-    def report(self, what, min_feasible=1, min_infeasible=1, **at_least):
-        print(f"{what}: {dict(self.n)}")
-        assert self.n["feasible"] >= min_feasible, (what, dict(self.n))
-        assert self.n["infeasible"] >= min_infeasible, (what, dict(self.n))
-        for k, v in at_least.items():
-            assert self.n[k] >= v, (what, k, dict(self.n))
-
-
-def _restated(call, oracle_mod, oracle_call, tally):
-    """call() on the restatement; on Unsupported, the oracle's side of the refusal (see the module docstring) and
-    None."""
-    from oracle import restate_np as R
-    try:
-        return call()
-    except R.Unsupported as e:
-        tally.n[f"refused ({e.reason})"] += 1
-        if e.reason == "states":
-            with pytest.raises(oracle_mod.Unsupported):
-                oracle_call()
-        return None
-
-
-def cross_alloc(oracle_mod, f, s, a, tally, what=""):
-    from oracle import restate_np as R
-    r = _restated(lambda: R.create_allocation(f, s, a), oracle_mod, lambda: oracle_mod.create_allocation(f, s, a),
-                  tally)
-    if r is None:
-        return
-    o = oracle_mod.create_allocation(f, s, a)
-    assert o["feasible"] == r["feasible"], (what, s, a, o, r)
-    tally.n["feasible" if o["feasible"] else "infeasible"] += 1
-    if not o["feasible"]:
-        return
-    assert (o["acc"], o["replicas"], o["batch"]) == (r["acc"], r["replicas"], r["batch"]), (what, s, a, o, r)
-    for k in ALLOC_FLOATS:
-        assert _same(o[k], r[k]), (what, s, a, k, o[k], r[k])
-
-
 def _cell_index(fleet, grid, ci):
     R_, B = grid.replicas.size, grid.batch.size
     ri, bi = ci % R_, (ci // R_) % B
@@ -165,7 +111,7 @@ def cross_cell(oracle_mod, fleet, grid, ci, cell_o, tally, what="", probs=False)
     assert int(cell_o["flags"]) == c["flags"], (what, (s, a, b, r), cell_o, c)
     tally.n[("feasible" if c["flags"] & 2 else "infeasible") if c["flags"] & 1 else "not analysed"] += 1
     for k in CELL_FLOATS:
-        assert _same(cell_o[k], c[k]), (what, (s, a, b, r), k, cell_o[k], c[k])
+        assert same_f32(cell_o[k], c[k]), (what, (s, a, b, r), k, cell_o[k], c[k])
     if probs and c["flags"] & 1:
         m = int(fleet.srv_model[s])
         args = (b, b * fleet.max_queue_to_batch_ratio, float(fleet.perf_alpha[m, a]), float(fleet.perf_beta[m, a]),
@@ -201,7 +147,7 @@ def cross_sweep(oracle_mod, fleet, n_rates, o, points, tally, what="", probs=())
         got = {"ttft": met["wait"] + met["prefill"], "itl": met["itl"], "throughput": met["throughput"],
                "rho": met["rho"]}
         for k in SWEEP_FLOATS:
-            assert _same(o[k][i], got[k]), (what, int(i), k, o[k][i], got[k])
+            assert same_f32(o[k][i], got[k]), (what, int(i), k, o[k][i], got[k])
         if i in probs:
             m = int(fleet.srv_model[s])
             qa = oracle_mod.Analyzer(rq.N, rq.Q, float(fleet.perf_alpha[m, a]), float(fleet.perf_beta[m, a]),
@@ -210,31 +156,6 @@ def cross_sweep(oracle_mod, fleet, n_rates, o, points, tally, what="", probs=())
             assert qa.analyze(float(o["rate"][i]))[0] == 0
             assert np.array_equal(qa.probs().view(np.uint64), rq.p.view(np.uint64)), (what, int(i))
             tally.n["probability vectors"] += 1
-
-
-def pair_n(f, s, a):
-    """The batch size N of a load pair (allocation.go:77-87), in Python's unbounded int."""
-    if f.srv_max_batch[s] > 0:
-        return int(f.srv_max_batch[s])
-    m = int(f.srv_model[s])
-    return max(int(f.perf_max_batch[m, a]) * int(f.perf_at_tokens[m, a]) // int(f.srv_out_tokens[s]), 1)
-
-
-def _too_long(f, s, a):
-    """A load pair whose N is above BIG_N but within the restated domain: left out of the samples for time."""
-    m = int(f.srv_model[s])
-    if m < 0 or not f.perf_present[m, a] or not (f.srv_arrival_rpm[s] > 0) or f.srv_out_tokens[s] <= 0:
-        return False
-    return BIG_N < pair_n(f, s, a) <= (1 << 20)
-
-
-def cross_fleet(oracle_mod, f, tally, what="", pairs=None):
-    """cross_alloc on every (server, accelerator) of f, or on the given pairs."""
-    for s, a in (pairs if pairs is not None else ((s, a) for s in range(f.n_servers) for a in range(f.n_acc))):
-        if _too_long(f, s, a):
-            tally.n["left out (N > 4096)"] += 1
-            continue
-        cross_alloc(oracle_mod, f, s, a, tally, what)
 
 
 def _pick(rng, idx, k):
@@ -254,11 +175,10 @@ def test_windows_cross(oracle_mod, case):
     every analysable grid cell and a sample of the others, with a sample of probability vectors; every size
     candidate; one of the K >= 2^23 candidates (a chain of 8.5 M states costs the restatement seconds); the two
     overflowing-search fleets; and sweep points chosen per band from chain_profile, plus an even spread."""
-    from tests import test_gpu_windows as W
     rng = np.random.default_rng(WINDOWS.index(case) + 11)
     t = Tally()
     if case.startswith("grid"):
-        fleet, grid = W.grid_cases()[int(case[-1])]
+        fleet, grid = grid_cases.grid_cases()[int(case[-1])]
         cells, _ = oracle_mod.grid_solve(fleet, grid, want_cells=True)
         ok = np.nonzero(cells["flags"] & 1)[0]
         rest = np.nonzero(~cells["flags"] & 1)[0]
@@ -269,22 +189,22 @@ def test_windows_cross(oracle_mod, case):
                  **{"probability vectors": min(6, ok.size)})
         assert t.n["feasible"] + t.n["infeasible"] == ok.size >= 6
     elif case == "size":
-        fleet = W.size_fleet()
+        fleet = grid_cases.size_fleet()
         cross_fleet(oracle_mod, fleet, t, case)
         t.report(case, min_feasible=700, min_infeasible=0)
     elif case == "long-queue":
-        fleet = W.long_queue_fleet()
+        fleet = grid_cases.long_queue_fleet()
         cross_fleet(oracle_mod, fleet, t, case, pairs=[(int(rng.integers(fleet.n_servers)), 0)])
         t.report(case, min_infeasible=0)
     elif case.startswith("overflow-search"):
-        fleet = W.overflow_search_fleet(*W.OVERFLOW_SEARCHES[int(case[-1])][:2])
+        fleet = grid_cases.overflow_search_fleet(*grid_cases.OVERFLOW_SEARCHES[int(case[-1])][:2])
         cross_fleet(oracle_mod, fleet, t, case)
         t.report(case, min_feasible=2, min_infeasible=0)
     else:
-        fleet, n = W.sweep_fleet(), W.SWEEP_RATES
+        fleet, n = grid_cases.sweep_fleet(), grid_cases.SWEEP_RATES
         o = oracle_mod.sweep(fleet, n)
         valid = np.nonzero(o["valid"])[0]
-        P = W.sweep_points(fleet, n, o["valid"])  # in the order of `valid`
+        P = grid_cases.sweep_points(fleet, n, o["valid"])  # in the order of `valid`
         ok = ~P["over"]
         bands = [P["over"], P["steep880"], ok & (P["emax"] == 879), ok & (P["emax"] == 880),
                  ok & (P["esum"] == 679), ok & (P["esum"] == 680), ok & (P["esum"] == 899), ok & (P["esum"] == 900),
@@ -304,12 +224,7 @@ def test_windows_cross(oracle_mod, case):
 # ---------------------------------------------------------------------------------------------------------------
 # grid shapes and stored-vector fallbacks (test_gpu_grid_shapes)
 # ---------------------------------------------------------------------------------------------------------------
-def _shape_names():
-    from tests.test_gpu_grid_shapes import SHAPES
-    return list(SHAPES)
-
-
-SHAPE_CASES = _shape_names() + ["tiny-acc", "invariant", "grid-fallback", "sweep-fallback", "size-fallback"]
+SHAPE_CASES = list(grid_cases.SHAPES) + ["tiny-acc", "invariant", "grid-fallback", "sweep-fallback", "size-fallback"]
 
 
 def _sample_cells(rng, cells, k_feas=6, k_infeas=4, k_none=3):
@@ -324,43 +239,42 @@ def test_grid_shapes_cross(oracle_mod, case):
     """A deterministic sample of cells of every shape case (feasible, analysed and infeasible, not analysed), the
     tiny-acc and batch-invariant cases (with the cell whose TTFT is its server's target), the fallback cases past
     their 128 slots (cells, sweep points and size candidates)."""
-    from tests import test_gpu_grid_shapes as G
     rng = np.random.default_rng(SHAPE_CASES.index(case) + 101)
     t = Tally()
     if case == "sweep-fallback":
-        fleet, n = G.sweep_fallback_fleet(), G.SWEEP_FB_RATES
+        fleet, n = grid_cases.sweep_fallback_fleet(), grid_cases.SWEEP_FB_RATES
         o = oracle_mod.sweep(fleet, n)
         pts = sorted(set(range(0, n, n // 24)) | set(range(n - 8, n)))
         cross_sweep(oracle_mod, fleet, n, o, pts, t, case, probs={pts[-1], pts[len(pts) // 2]})
         t.report(case, min_feasible=20, min_infeasible=0, **{"probability vectors": 2})
         return
     if case == "size-fallback":
-        fleet = G.size_fallback_fleet()
+        fleet = grid_cases.size_fallback_fleet()
         cross_fleet(oracle_mod, fleet, t, case, pairs=[(0, 0), (1, 0), (fleet.n_servers - 1, 0)])
         t.report(case, min_feasible=3, min_infeasible=0)
         return
     if case == "tiny-acc":
-        fleet, grid = G.tiny_acc_case()
+        fleet, grid = grid_cases.tiny_acc_case()
         extra = ()
     elif case == "invariant":
-        fleet, grid, s, (r, b) = G.invariant_case()
+        fleet, grid, s, (r, b) = grid_cases.invariant_case()
         B, R_ = grid.batch.size, grid.replicas.size
         extra = ((s * B + list(grid.batch).index(b)) * R_ + list(grid.replicas).index(r),)
     elif case == "grid-fallback":
-        fleet, grid = G.grid_fallback_case()
+        fleet, grid = grid_cases.grid_fallback_case()
         extra = ()
     else:
-        fleet, grid = G.shape_case(case)
+        fleet, grid = grid_cases.shape_case(case)
         extra = ()
     cells, _ = (oracle_mod.grid_solve(fleet, grid, want_cells=True) if case in ("tiny-acc", "invariant",
                                                                                    "grid-fallback")
-                else G.shape_oracle(case))
+                else grid_cases.shape_oracle(case))
     pick = np.unique(np.concatenate([_sample_cells(rng, cells), np.array(extra, np.int64)]))
     probs = set(_pick(rng, pick[(cells["flags"][pick] & 1) == 1], 2).tolist())
     for ci in pick:
         cross_cell(oracle_mod, fleet, grid, int(ci), cells[ci], t, case, probs=int(ci) in probs)
     t.report(case, min_feasible=1, min_infeasible=0, **{"probability vectors": 1})
-    if case in G.SHAPES:  # zero load and a missing profile: cells that are not analysed
+    if case in grid_cases.SHAPES:  # zero load and a missing profile: cells that are not analysed
         assert t.n["not analysed"] >= 1
 
 
@@ -376,11 +290,10 @@ def test_adversarial_cross(oracle_mod, case):
     whose totalRate / rateStar lies just past 2^63, where any replica count that kept the quotient's size would bring
     the per-replica rate back under RateRange.Max."""
     from oracle import restate_np as R
-    from tests import test_gpu_adversarial_paths as P
     t = Tally()
     if case == "size-grid":
         rng = np.random.default_rng(0x51CE + 1)
-        for k, (fleet, batches, _) in enumerate(P.size_grid_cases()):
+        for k, (fleet, batches, _) in enumerate(levels.size_grid_cases()):
             S, A = fleet.n_servers, fleet.n_acc
             for j in _pick(rng, np.arange(len(batches) * S * A), 8):
                 bi, sa = divmod(int(j), S * A)
@@ -390,7 +303,7 @@ def test_adversarial_cross(oracle_mod, case):
         t.report(case, min_feasible=100, min_infeasible=50)
     elif case == "load-levels":
         rng = np.random.default_rng(0x10AD + 1)
-        for k, (fleet, rpm) in enumerate(P.load_grid_cases(oracle_mod)):
+        for k, (fleet, rpm) in enumerate(levels.load_grid_cases(oracle_mod)):
             S, A = fleet.n_servers, fleet.n_acc
             for j in _pick(rng, np.arange(rpm.shape[0] * S * A), 8):
                 l, sa = divmod(int(j), S * A)
@@ -399,14 +312,14 @@ def test_adversarial_cross(oracle_mod, case):
                 cross_fleet(oracle_mod, f, t, f"load case {k}, level {l}", pairs=[divmod(sa, A)])
         t.report(case, min_feasible=100, min_infeasible=50)
     elif case == "queue-cases":
-        for name, pmb, at, out, smb, ratio, refused in P.QUEUE_CASES:
-            N, _ = P.go_queue(pmb, at, out, smb, ratio)
+        for name, pmb, at, out, smb, ratio, refused in levels.QUEUE_CASES:
+            N, _ = levels.go_queue(pmb, at, out, smb, ratio)
             try:
                 R.queue_states(int(N), ratio)
                 assert not refused, name
             except R.Unsupported:
                 assert refused, name
-            f = P.queue_fleet(name)
+            f = levels.queue_fleet(name)
             # server 0 carries the case; a model of N = 2^20 (K up to 2^31 - 2^20) is within both domains but far
             # too large to solve here, so only the other servers are compared for those two
             pairs = [(s, a) for s in range(f.n_servers) for a in range(f.n_acc)
@@ -430,7 +343,7 @@ def test_adversarial_cross(oracle_mod, case):
     else:
         f = synth_fleet(4, 2, seed=13, zero_load_frac=0.0, tps_frac=0.0, max_batch_choices=(4, 8))
         f.srv_min_replicas[:] = [0, 1, 0, 2]
-        for rpm in (P.TINY_TOTAL, np.nextafter(P.TINY_TOTAL, F(0)), F(2.0 ** -149), F(1e-30)):
+        for rpm in (levels.TINY_TOTAL, np.nextafter(levels.TINY_TOTAL, F(0)), F(2.0 ** -149), F(1e-30)):
             g = f.take_servers(np.arange(4))
             g.srv_arrival_rpm[:] = rpm
             cross_fleet(oracle_mod, g, t, f"rate {rpm!r}")
@@ -450,22 +363,19 @@ def test_level_rows_cross(oracle_mod, case):
     batch size that puts N at 2^21."""
     t = Tally()
     if case == "slo":
-        from tests.test_gpu_load_grid import mixed_fleet
-        from tests.test_gpu_slo_grid import TARGETS, TPS_TARGETS, at_slo, slo_levels
         f = synth_fleet(4, 2, seed=5, max_batch_choices=(1, 2, 4, 8, 16))
-        own = (f.srv_slo_itl, f.srv_slo_ttft)
         for itl in TARGETS:
             for ttft in TARGETS:
-                cross_fleet(oracle_mod, at_slo(f, itl, ttft, 0.0), t, f"itl {itl}, ttft {ttft}")
+                cross_fleet(oracle_mod, at_row(f, {"slo_itl": [itl], "slo_ttft": [ttft], "slo_tps": [0.0]}, 0), t, f"itl {itl}, ttft {ttft}")
         for tps in TPS_TARGETS:
             # FLT_MAX / out_tokens over rateStar leaves int64: int() is MinInt64, then min_replicas (allocation.go:140)
-            cross_fleet(oracle_mod, at_slo(f, *own, tps), t, f"tps {tps}")
+            cross_fleet(oracle_mod, at_row(f, {"slo_tps": [tps]}, 0), t, f"tps {tps}")
         g = mixed_fleet(12, 3, 47, False)
-        for l, row in enumerate(zip(*slo_levels(g, 4, 17))):
-            cross_fleet(oracle_mod, at_slo(g, *row), t, f"slo_levels row {l}")
+        rows = dict(zip(SLO, slo_levels(g, 4, 17)))
+        for l in range(4):
+            cross_fleet(oracle_mod, at_row(g, rows, l), t, f"slo_levels row {l}")
         t.report(case, min_feasible=150, min_infeasible=150)
     elif case == "workload":
-        from tests.test_gpu_workload_grid import at_level, token_fleet, workload_levels
         f = token_fleet(12, 3, 43, True)
         rpm, it, ot = workload_levels(f, 7, 13)
         assert {0, 1, 20000} <= set(ot.ravel().tolist()) and 0 in it
@@ -474,7 +384,7 @@ def test_level_rows_cross(oracle_mod, case):
         ot = np.concatenate([ot, np.full((1, f.n_servers), 20000, np.int32)])
         n1 = 0
         for l in range(rpm.shape[0]):
-            fl = at_level(f, rpm[l], it[l], ot[l])
+            fl = at_row(f, dict(zip(LOAD, (rpm, it, ot))), l)
             cross_fleet(oracle_mod, fl, t, f"workload row {l}")
             n1 += sum(fl.srv_max_batch[s] == 0 and fl.srv_arrival_rpm[s] > 0 and fl.srv_out_tokens[s] > 0 and
                       fl.srv_model[s] >= 0 and pair_n(fl, s, 0) == 1 for s in range(f.n_servers))
@@ -491,12 +401,11 @@ def test_level_rows_cross(oracle_mod, case):
             cross_fleet(oracle_mod, h, t, f"N = 2^21 server, rate {rate}, out {out}")
         t.report(case, min_feasible=100, min_infeasible=40, **{"refused (batch)": 2})
     else:
-        from tests.test_gpu_profile_grid import at_profile, profile_fleet, profile_rows
         f = profile_fleet(14, 3, 31, False)
         rows = profile_rows(f, 7, 3)
         rows["perf_acc_count"][3] = np.where(np.arange(f.n_acc) % 2, 0, -2)[None, :]
         for l in range(7):
-            cross_fleet(oracle_mod, at_profile(f, rows, l), t, f"profile row {l}")
+            cross_fleet(oracle_mod, at_row(f, rows, l), t, f"profile row {l}")
         g = synth_fleet(4, 2, seed=83, zero_load_frac=0.0)
         g.srv_max_batch[0] = 0
         g.perf_at_tokens[:] = 1 << 12
@@ -505,7 +414,7 @@ def test_level_rows_cross(oracle_mod, case):
         mb = np.repeat(g.perf_max_batch[None], 2, axis=0).copy()
         mb[1, int(g.srv_model[0]), 0] = 1 << 16  # N = 2^16 * 2^12 / 2^7 = 2^21
         for l in range(2):
-            cross_fleet(oracle_mod, at_profile(g, {"perf_max_batch": mb}, l), t, f"perf batch row {l}")
+            cross_fleet(oracle_mod, at_row(g, {"perf_max_batch": mb}, l), t, f"perf batch row {l}")
         t.report(case, min_feasible=150, min_infeasible=40, **{"refused (batch)": 1})
 
 
@@ -520,35 +429,31 @@ def test_tail_windows_cross(oracle_mod, case):
     a sample of the perf_alpha rows, and a sample of the bounds' batch sizes at their own load (Size at lambda_max,
     then the final Analyze).  The bounds' rate-edge pairs are left out: at a load they need more than 2^31 replicas,
     which the record's int32 does not hold."""
-    from tests import test_gpu_tail_windows as T
-    from tests.test_gpu_load_grid import at_level
-    from tests.test_gpu_profile_grid import at_profile
-    from tests.test_gpu_slo_grid import at_slo
     t = Tally()
     sample = lambda n, k: np.unique(np.linspace(0, n - 1, k).round().astype(int))  # noqa: E731
     if case == "load":
-        (main, rpm), (long, lrpm), (edge, erpm) = T.load_cases()
+        (main, rpm), (long, lrpm), (edge, erpm) = grid_cases.load_cases()
         for l in sample(rpm.shape[0], 16):
-            cross_fleet(oracle_mod, at_level(main, rpm[l]), t, f"load level {l}")
-        cross_fleet(oracle_mod, at_level(long, lrpm[len(lrpm) // 2]), t, "K >= 2^23")
+            cross_fleet(oracle_mod, at_row(main, {"arrival_rpm": rpm}, l), t, f"load level {l}")
+        cross_fleet(oracle_mod, at_row(long, {"arrival_rpm": lrpm}, len(lrpm) // 2), t, "K >= 2^23")
         for l in range(erpm.shape[0]):
-            cross_fleet(oracle_mod, at_level(edge, erpm[l]), t, f"edge level {l}")
+            cross_fleet(oracle_mod, at_row(edge, {"arrival_rpm": erpm}, l), t, f"edge level {l}")
         t.report(case, min_feasible=40, min_infeasible=0)
     elif case == "slo":
-        (main, (itl, ttft, tps)), (edge, erows) = T.slo_cases()[:2]
+        (main, (itl, ttft, tps)), (edge, erows) = grid_cases.slo_cases()[:2]
         L1 = int((ttft[:, 0] > 0).sum())
         for l in list(sample(L1, 6)) + list(L1 + sample(itl.shape[0] - L1, 6)):
-            cross_fleet(oracle_mod, at_slo(main, itl[l], ttft[l], tps[l]), t, f"SLO row {l}")
+            cross_fleet(oracle_mod, at_row(main, dict(zip(SLO, (itl, ttft, tps))), l), t, f"SLO row {l}")
         for l in range(erows[0].shape[0]):
-            cross_fleet(oracle_mod, at_slo(edge, *(r[l] for r in erows)), t, f"edge row {l}")
+            cross_fleet(oracle_mod, at_row(edge, dict(zip(SLO, erows)), l), t, f"edge row {l}")
         t.report(case, min_feasible=30, min_infeasible=0)
     elif case == "profile":
-        for fleet, rows in T.profile_cases():
+        for fleet, rows in grid_cases.profile_cases():
             L = rows["perf_alpha"].shape[0]
             for l in sample(L, 12):
-                cross_fleet(oracle_mod, at_profile(fleet, rows, l), t, f"perf_alpha row {l}")
+                cross_fleet(oracle_mod, at_row(fleet, rows, l), t, f"perf_alpha row {l}")
         t.report(case, min_feasible=40, min_infeasible=0)
     else:
-        main = T.bounds_cases()[0]
+        main = grid_cases.bounds_cases()[0]
         cross_fleet(oracle_mod, main, t, "bounds", pairs=[(int(s), 0) for s in sample(main.n_servers, 24)])
         t.report(case, min_feasible=20, min_infeasible=0)

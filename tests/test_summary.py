@@ -7,6 +7,8 @@ GPU: Engine.summarize() (summary_kernel, or the host loops after a greedy solve)
 import numpy as np
 import pytest
 
+from tests.grid_cases import check_summary
+from tests.levels import limited_fleet
 from workload_variant_autoscaler_b200 import Grid, synth_fleet
 from workload_variant_autoscaler_b200._abi import ACC_ABSENT, ACC_NONE
 
@@ -56,21 +58,6 @@ def test_allocate_by_type_hand_computed(oracle_mod):
     assert oracle_mod.allocate_by_type(f2, w2)["cost"][0] == want == np.float32(1.0)
 
 
-def _check(engine, oracle_mod, f, win_o):
-    got = engine.summarize(f.n_types)
-    t = oracle_mod.allocate_by_type(f, win_o)
-    d = oracle_mod.allocation_diffs(f, win_o)
-    assert np.array_equal(got["by_type"]["present"], t["present"].astype(np.uint8))
-    assert np.array_equal(got["by_type"]["count"], t["count"])
-    assert np.array_equal(got["by_type"]["limit"], t["limit"])
-    assert np.array_equal(got["by_type"]["cost"].view(np.uint32), np.ascontiguousarray(t["cost"]).view(np.uint32))
-    for k_g, k_o in (("old_acc", "old_acc"), ("new_acc", "new_acc"), ("old_replicas", "old_replicas"),
-                     ("new_replicas", "new_replicas")):
-        assert np.array_equal(got["diff"][k_g], d[k_o]), k_g
-    assert np.array_equal(got["diff"]["cost"].view(np.uint32), np.ascontiguousarray(d["cost_diff"]).view(np.uint32))
-    return t, d
-
-
 @pytest.mark.gpu
 def test_summary_after_unlimited_solve(engine, oracle_mod):
     f = synth_fleet(1500, 5, seed=31, max_batch_choices=(2, 4, 8, 16), zero_load_frac=0.1)
@@ -81,18 +68,17 @@ def test_summary_after_unlimited_solve(engine, oracle_mod):
     f.srv_has_target[5] = 0            # a server without any allocation ("none")
     _, win_o = oracle_mod.solve(f)
     engine.solve(f)
-    t, d = _check(engine, oracle_mod, f, win_o)
+    t, d = check_summary(engine, oracle_mod, f, win_o)
     assert t["present"].sum() >= 2 and (d["new_acc"] == ACC_ABSENT).sum() >= 1 and (d["new_acc"] == ACC_NONE).sum() >= 1
 
 
 @pytest.mark.gpu
 def test_summary_after_greedy_solve(engine, oracle_mod):
-    from tests.test_greedy import limited_fleet
     from workload_variant_autoscaler_b200._abi import SAT_PRIORITY_ROUND_ROBIN
     f = limited_fleet(17, 9, SAT_PRIORITY_ROUND_ROBIN, delayed=True)
     _, win_o = oracle_mod.solve(f)
     engine.solve(f)
-    t, _ = _check(engine, oracle_mod, f, win_o)
+    t, _ = check_summary(engine, oracle_mod, f, win_o)
     assert (t["count"] <= t["limit"]).all()
 
 
@@ -103,7 +89,7 @@ def test_summary_after_grid_solve_and_state_errors(engine, oracle_mod):
     grid = Grid([1, 2, 4, 8], [1, 2, 3, 4, 6, 8])
     _, win_o = oracle_mod.grid_solve(f, grid, want_cells=False)
     engine.grid_solve(f, grid)
-    _check(engine, oracle_mod, f, win_o)
+    check_summary(engine, oracle_mod, f, win_o)
     engine.upload(f)                   # a new upload invalidates the previous solution
     with pytest.raises(WvaError):
         engine.summarize(f.n_types)

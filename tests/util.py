@@ -1,8 +1,31 @@
-"""Bit-exact comparison helpers shared by the parity tests."""
+"""Bit-exact comparison helpers and the ABI constants shared by the parity tests."""
 import numpy as np
 
 ALLOC_FIELDS = ("feasible", "acc", "replicas", "batch", "cost", "value", "itl", "ttft", "rho", "max_rate")
 FLOAT_FIELDS = ("cost", "value", "itl", "ttft", "rho", "max_rate")
+F32_MAX = np.float32(np.finfo(np.float32).max)
+# include/wva_b200.h, written out so that the tests pin the values rather than read them from _abi
+WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
+ACC_NONE, ACC_UNKNOWN = -1, -2
+
+
+def same_bytes(a, b):
+    return np.ascontiguousarray(a).tobytes() == np.ascontiguousarray(b).tobytes()
+
+
+def f32_bits(x):
+    """The bits of float32(x), any NaN as the quiet NaN."""
+    v = np.float32(x)
+    return 0x7FC00000 if np.isnan(v) else int(np.array([v]).view(np.uint32)[0])
+
+
+def error_code(fn):
+    """(0, fn()) or (the WvaError's code, None)."""
+    from workload_variant_autoscaler_b200 import WvaError
+    try:
+        return 0, fn()
+    except WvaError as e:
+        return e.code, None
 
 
 def bits(a):
