@@ -585,6 +585,59 @@ int wva_load_intervals(wva_handle *h, const wva_fleet *fleet, const float *rpm_l
                        wva_intervals *out);
 
 /*
+ * Load margins: for each level l and server s, the exact stretch of float32 arrival rates around the level's rate
+ * on which wva_load_grid's winner keeps its decision.  A controller can publish "scale down below lo_rpm, scale up
+ * at hi_rpm" next to the desired replica count, or skip a re-solve while the load stays inside the stretch, and a
+ * planner can see how far the real load may stray from each row of a forecast before the planned decision is wrong.
+ *
+ * Level l has wva_load_grid's semantics: the fleet with srv_arrival_rpm set to row l (index l*S + s; arrival_rpm
+ * NULL is the fleet's own column at every level), against the fleet's own current allocation, solved in unlimited
+ * mode.  The decision key is wva_load_intervals' (feasible, acc, replicas, batch, cost, value, max_rate), compared
+ * bitwise.  Let r be row l's rate for s.  [lo_rpm, hi_rpm) is the maximal stretch of float32 rates in
+ * [rpm_lo, rpm_hi] (entry l*S + s of each) that contains r and on which the key equals the key at r.  It is exactly
+ * the interval that wva_load_intervals over the same window, with max_per_server large enough, reports as containing
+ * r, and hi_rpm is the start of the next interval in that list.  Rate 0 is a point of its own, as there.
+ *
+ * at, below and above are byte for byte wva_load_grid's winner records at r, at nextafterf(lo_rpm, 0) and at
+ * hi_rpm, latency columns included (taken at those exact rates).  Flags:
+ *   WVA_MARGIN_LO_OPEN    no change in [rpm_lo, r]: lo_rpm = rpm_lo, `below` is zero bytes;
+ *   WVA_MARGIN_HI_OPEN    no change in (r, rpm_hi]: hi_rpm = +Inf, `above` is zero bytes;
+ *   WVA_MARGIN_TRUNCATED  a pair of s would need more than INT32_MAX replicas (where the steps stop being monotone,
+ *                         see wva_load_intervals) at hi_rpm, which is then the first such rate above r, or at r
+ *                         itself, where lo_rpm = hi_rpm = r and `below` is zero bytes.  `above` is zero bytes.
+ *
+ * Each pair's state is a step function of the rate (DESIGN.md §3.10), so the call walks from r up to the first
+ * change of the winner's key and down to the last one, each step found by a bisection over float32 bit patterns
+ * (§3.19).  The sizing runs once per (server, accelerator), as in wva_load_grid.
+ *
+ * fleet->unlimited and the capacities are not read; fleet->srv_arrival_rpm only when arrival_rpm is NULL.  The
+ * fleet becomes resident, and wva_summarize returns WVA_ERR_STATE afterwards.  Columns of at, below and above may be
+ * NULL (not written).  n_levels == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG: n_levels < 0, out NULL,
+ * rpm_lo, rpm_hi, lo_rpm, hi_rpm or flags NULL with S*n_levels > 0, a rate, rpm_lo or rpm_hi that is NaN, infinite
+ * or negative, or rpm_lo > r or r > rpm_hi.  WVA_ERR_UNSUPPORTED: 3*S*n_levels >= 2^31 (three records per level and
+ * server; refused before the fleet is read), or where wva_load_intervals refuses, for the servers with some level whose rpm_hi > 0: a pair outside
+ * wva_analyze's queue-size rule, a solve at r, below lo_rpm or at hi_rpm whose rescale loop would not terminate, too
+ * many stored-vector fallbacks, or a window holding a positive rate below 60 * 2^-150 req/min on a server with a
+ * min_replicas-0 load pair.
+ */
+#define WVA_MARGIN_LO_OPEN 1
+#define WVA_MARGIN_HI_OPEN 2
+#define WVA_MARGIN_TRUNCATED 4
+
+typedef struct wva_margins {
+    float *lo_rpm;    /* [L*S] first float32 rate of the stretch that holds the level's rate                   */
+    float *hi_rpm;    /* [L*S] first float32 rate above it at which the decision key differs (+Inf: none)    */
+    uint8_t *flags;   /* [L*S] WVA_MARGIN_*                                                                   */
+    wva_allocs at;    /* [L*S] wva_load_grid's winner record at the level's rate                              */
+    wva_allocs below; /* [L*S] wva_load_grid's winner record at the largest float32 below lo_rpm              */
+    wva_allocs above; /* [L*S] wva_load_grid's winner record at hi_rpm                                        */
+} wva_margins;
+
+int wva_load_margins(wva_handle *h, const wva_fleet *fleet, int32_t n_levels,
+                     const float *arrival_rpm /* [L*S], NULL: the fleet's own column at every level */,
+                     const float *rpm_lo, const float *rpm_hi /* [L*S] search window, req/min */, wva_margins *out);
+
+/*
  * Price thresholds: for each server s and accelerator a, the exact accelerator price at which s's unlimited
  * winner leaves a.  Let f(p) be the fleet with acc_cost[a] = p, solved in unlimited mode.
  *

@@ -21,6 +21,8 @@ ACC_NONE = -1      # accelerator name "" (pkg/core/allocation.go:264)
 ACC_UNKNOWN = -2   # a name missing from the accelerator table
 ACC_ABSENT = -3    # no allocation at all: CreateAllocationDiff's "none" (pkg/core/allocation.go:357-358)
 
+MARGIN_LO_OPEN, MARGIN_HI_OPEN, MARGIN_TRUNCATED = 1, 2, 4  # wva_margins.flags
+
 SAT_NONE, SAT_PRIORITY_EXHAUSTIVE, SAT_PRIORITY_ROUND_ROBIN, SAT_ROUND_ROBIN = 0, 1, 2, 3
 SAT_BY_NAME = {  # pkg/config/config.go:28-41
     "None": SAT_NONE,
@@ -98,6 +100,11 @@ class AllocsC(C.Structure):
 class IntervalsC(C.Structure):
     _fields_ = [("max_per_server", C.c_int32), ("count", i32p), ("truncated", u8p), ("start_rpm", f32p),
                 ("rec", AllocsC)]
+
+
+class MarginsC(C.Structure):
+    _fields_ = [("lo_rpm", f32p), ("hi_rpm", f32p), ("flags", u8p), ("at", AllocsC), ("below", AllocsC),
+                ("above", AllocsC)]
 
 
 class SloBoundsC(C.Structure):

@@ -220,7 +220,7 @@ struct wva_handle {
     DevBuf d_sz_state, d_sz_req, d_sz_sort;
     PinBuf sz_pin;
     DevBuf d_lg_star;  // the load grid's rateStar records (shared with the load intervals)
-    DevBuf d_iv;       // the load intervals' counts, flags, starts and work list
+    DevBuf d_iv;       // the load intervals' and load margins' output columns and work list
     DevBuf d_slo;      // the SLO grid's search records
     DevBuf d_prof;     // the profile grid's key records
     DevBuf d_price;    // the price thresholds
@@ -308,6 +308,16 @@ void scatter_block(const void* host_block, const Block& b, const wva_allocs* out
     if (out->name) memcpy(out->name, (const char*)host_block + b.off.name, sizeof(type) * b.n);
     WVA_ALLOC_COLUMNS(BLOCK_SCATTER)
 #undef BLOCK_SCATTER
+}
+// Records [k * n, (k + 1) * n) of block b, as a block of n records (a call that returns several record lists in one
+// block scatters each through its own view)
+Block sub_block(const Block& b, size_t k, size_t n) {
+    Block s = b;
+#define SUB_OFFSET(name, type, required) s.off.name += sizeof(type) * k * n;
+    WVA_ALLOC_COLUMNS(SUB_OFFSET)
+#undef SUB_OFFSET
+    s.n = n;
+    return s;
 }
 AllocCols cols_from_abi(const wva_allocs* a) {
     AllocCols c{};
@@ -1133,6 +1143,79 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     h->launches += 2;
     CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1 and the interval kernels
     launch_fallback(h, interval_fallback, g, ls.fb2);
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// ---- load margins: the stretch around each level's rate on which the load-grid winner keeps its decision -------
+static_assert(MG_LO_OPEN == WVA_MARGIN_LO_OPEN && MG_HI_OPEN == WVA_MARGIN_HI_OPEN &&
+              MG_TRUNCATED == WVA_MARGIN_TRUNCATED, "margin flags");
+
+// The device columns of one call: lo_out, hi_out and flags [n] come back to the caller, the work list [3n] stays
+// on the device.
+struct MarginCols {
+    Cols cols{16};
+    size_t o_lo = 0, o_hi = 0, o_flags = 0, o_items = 0;
+};
+
+// Phase 1 over the servers with some window top > 0, margin_kernel, margin_tail and margin_fallback.  rate / lo /
+// hi [L*S] are the caller's rows (rate NULL: the fleet's own column); rec ([3*L*S]) is a device block; the other
+// columns are in h->d_iv at mc's offsets.
+int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* lo, const float* hi,
+                         const MarginCols& mc, const AllocCols& rec, size_t rec_bytes) {
+    const HostFleet& hf = h->hf;
+    const int S = hf.S, A = hf.A, n = S * L;
+    std::vector<char> loaded(S, 0);
+    for (int i = 0; i < n; ++i) loaded[i % S] |= hi[i] > 0.0f;
+    std::vector<int> pairs;
+    Cols c(16);
+    RowLists lists{hf, L, c};
+    lists.put_rpm(rate);
+    const size_t o_lo = c.put(lo, 4 * (size_t)n), o_hi = c.put(hi, 4 * (size_t)n), o_cop = c.take(4 * (size_t)S * A);
+    int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
+        int* cop = (int*)(p + o_cop);
+        std::fill(cop, cop + (size_t)S * A, -1);
+        for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
+    });
+    if (rc) return rc;
+    rc = ensure_ctrl(h);
+    if (rc) return rc;
+    // below and above are zero bytes where the walk writes none
+    if (n > 0) CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
+    LoadStar ls;
+    rc = enqueue_load_star(h, hf, h->df, 3ll * n, ls);
+    if (rc) return rc;
+    if (n == 0) return WVA_OK;
+    const char* dl = (const char*)h->lg_tabs.lists.p;
+    char* d = (char*)h->d_iv.p;
+    MarginArgs g{};
+    g.ld = load_args(h, ls);
+    g.cand_of_pair = (const int*)(dl + o_cop);
+    g.rate = lists.rpm.dev(dl);
+    g.lo = (const float*)(dl + o_lo);
+    g.hi = (const float*)(dl + o_hi);
+    g.n = n;
+    g.lo_out = (float*)(d + mc.o_lo);
+    g.hi_out = (float*)(d + mc.o_hi);
+    g.flags = (uint8_t*)(d + mc.o_flags);
+    g.rec = rec;
+    g.items = FbList{(int*)h->d_ctrl.p + CTRL_COUNTER, (unsigned long long*)(d + mc.o_items), 3 * n};
+    g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
+    // one warp per (level, server), A accelerator states and stretch starts per warp in shared memory
+    const size_t per_warp = (sizeof(IvAcc) + sizeof(float)) * (size_t)A;
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    if (per_warp > (size_t)optin)
+        return h->fail(WVA_ERR_UNSUPPORTED, "too many accelerators for the margin kernel's shared memory");
+    const int wpb = (int)std::max<size_t>(1, std::min<size_t>(4, (48u << 10) / std::max<size_t>(per_warp, 1)));
+    const size_t smem = per_warp * wpb;
+    if (smem > (48u << 10)) CK(cudaFuncSetAttribute(margin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    margin_kernel<<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, (3ll * n + 255) / 256);
+    margin_tail<<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
+    h->launches += 2;
+    CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1 and the margin kernels
+    launch_fallback(h, margin_fallback, g, ls.fb2);
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -3026,6 +3109,46 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;
     scatter_block(c.cand_host, c.bc, &out->rec);
+    return WVA_OK;
+}
+
+int wva_load_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                     const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
+    if (!h) return WVA_ERR_BAD_ARG;
+    if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
+    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
+    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
+    const int S = fleet->n_servers, L = n_levels;
+    // three records per (level, server), each indexed in int32
+    if (3ll * S * L >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "load margins too large for one call (>= 2^31 records)");
+    const int n = S * L;
+    if (n > 0 && (!rpm_lo || !rpm_hi || !out->lo_rpm || !out->hi_rpm || !out->flags))
+        return h->fail(WVA_ERR_BAD_ARG, "NULL window or output column");
+    for (int i = 0; i < n; ++i) {
+        const float r = arrival_rpm ? arrival_rpm[i] : fleet->srv_arrival_rpm[i % S], lo = rpm_lo[i], hi = rpm_hi[i];
+        if (!std::isfinite(r) || !std::isfinite(lo) || !std::isfinite(hi) || r < 0.0f || lo < 0.0f || hi < 0.0f ||
+            lo > r || r > hi)
+            return h->fail(WVA_ERR_BAD_ARG, "rate or window NaN, infinite or negative, or the rate outside its window");
+    }
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    MarginCols mc;
+    mc.o_lo = mc.cols.take(4 * (size_t)n, out->lo_rpm);
+    mc.o_hi = mc.cols.take(4 * (size_t)n, out->hi_rpm);
+    mc.o_flags = mc.cols.take((size_t)n, out->flags);
+    mc.o_items = mc.cols.take(8 * 3 * (size_t)n);
+    CK(h->d_iv.ensure(mc.cols.bytes));
+    HostCall c{3 * (size_t)n, n > 0, false, &mc.cols, h->d_iv.p};
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
+        return enqueue_load_margins(h, L, arrival_rpm, rpm_lo, rpm_hi, mc, dc, c.bc.bytes);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    const wva_allocs* recs[3] = {&out->at, &out->below, &out->above};
+    if (n > 0)
+        for (int k = 0; k < 3; ++k) scatter_block(c.cand_host, sub_block(c.bc, k, n), recs[k]);
     return WVA_OK;
 }
 

@@ -1341,12 +1341,15 @@ __device__ __forceinline__ IvState iv_state(const DevFleet& f, int s, int a, con
     return st;
 }
 
-// Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.
-__device__ __forceinline__ void iv_advance(const IntervalArgs& g, int s, int a, float x, float hi, IvAcc& p) {
+// Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.  g is the call's
+// IntervalArgs or MarginArgs; the window of x is row `row` of its bound lists g.lo / g.hi (the load intervals have
+// one row).
+template <class Args>
+__device__ __forceinline__ void iv_advance(const Args& g, int row, int s, int a, float x, float hi, IvAcc& p) {
     const DevFleet& f = g.ld.f;
     const float inf = __int_as_float(0x7f800000);
-    // the class at x: pair_class reads only whether the rate is negative or zero, and lo[s] = 0 when x = 0
-    const int cls = pair_class(at_level(f, x == 0.0f ? g.lo : g.hi, 0), s, a, true);
+    // the class at x: pair_class reads only whether the rate is negative or zero, and lo is 0 when x = 0
+    const int cls = pair_class(at_level(f, x == 0.0f ? g.lo : g.hi, row), s, a, true);
     p.tail = 0;
     p.over = false;
     p.next = x == 0.0f && hi > 0.0f ? __int_as_float(1) : inf;  // rpm = 0 is a point of its own
@@ -1444,7 +1447,7 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     float x = g.lo[s];
     bool over = false;
     for (int a = lane; a < A; a += 32) {
-        iv_advance(g, s, a, x, hi, acc[a]);
+        iv_advance(g, 0, s, a, x, hi, acc[a]);
         over |= acc[a].over;
     }
     __syncwarp();
@@ -1476,7 +1479,7 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
         __syncwarp();
         for (int a = lane; a < A; a += 32)
             if (acc[a].next == nx) {
-                iv_advance(g, s, a, nx, hi, acc[a]);
+                iv_advance(g, 0, s, a, nx, hi, acc[a]);
                 over |= acc[a].over;
             }
         __syncwarp();
@@ -1513,5 +1516,224 @@ __global__ void __launch_bounds__(256) interval_tail(IntervalArgs g) {
 
 // Stored-vector re-run of the interval starts interval_tail bailed on.
 __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec, IvTail{g}); }
+
+// ---------------------------------------------------------------------------
+// Load margins (DESIGN.md §3.19): per (level, server), the stretch of float32 rates in the window [lo, hi] around
+// the level's rate r on which the load grid's winner keeps its decision key.  margin_kernel runs one warp per
+// (level, server) and walks up from r as interval_kernel walks (iv_advance) to the first change of the winner's key.
+// Then it walks down: a pair's state at x holds on a stretch [start, x], found by one bisection, because the state
+// never decreases as the rate grows.  The warp maximum y of the starts is the next rate below which some pair
+// changes, and the walk stops at the first such y whose float below changes the key.  margin_tail then runs the load
+// grid's tail at the records (at r, below lo, at hi) whose winner is a load pair, and margin_fallback re-runs the
+// items it bailed on.
+// ---------------------------------------------------------------------------
+enum { MG_LO_OPEN = 1, MG_HI_OPEN = 2, MG_TRUNCATED = 4 };  // the header's WVA_MARGIN_*
+
+struct MarginArgs {
+    LoadArgs ld;               // phase 1's candidates and rateStar records (level_rpm, L and cand unused)
+    const int* cand_of_pair;   // [S * A] the pair's index in ld's candidate list, -1: not a load candidate
+    const float* rate;         // [n] the levels' rates, index l * S + s (req/min)
+    const float* lo;           // [n] the windows
+    const float* hi;
+    int n;                     // L * S, with 3 * n < 2^31
+    float* lo_out;             // [n]
+    float* hi_out;             // [n]
+    uint8_t* flags;            // [n]
+    AllocCols rec;             // [3 * n]: at (k = 0), below (1), above (2), record k * n + i
+    FbList items;              // margin_tail's work list: fb_pack(accelerator, record)
+    int* status;               // set when a window holds a rate at which a pair has 0 replicas (see iv_advance)
+};
+
+// nextafterf(x, 0) for x > 0
+__device__ __forceinline__ float mg_below(float x) { return __uint_as_float(__float_as_uint(x) - 1u); }
+
+// Accelerator a of server s at rate x in (0, r], where bottom is the window's smallest positive rate: its key at x
+// and the smallest rate in [bottom, x] at which its state is its state at x.  A pair that is not a load pair, or
+// one with a TPS target, has one key at every positive rate (iv_advance set it at r).
+__device__ __forceinline__ float mg_start(const DevFleet& f, int s, int a, IvAcc& p, float x, float bottom) {
+    if (!p.tail) return bottom;
+    const IvState at = iv_state(f, s, a, p, x, &p.key);
+    if (f.srv_slo_tps[s] != 0.0f) return bottom;
+    // "same state as at x" is false below the start and true from it on up to x: a monotone predicate
+    auto same = [&](unsigned bits) { return !(iv_state(f, s, a, p, __uint_as_float(bits), nullptr) != at); };
+    unsigned l = __float_as_uint(bottom), h = __float_as_uint(x);
+    if (h <= l || same(l)) return bottom;
+    // !same(l), same(h).  The start is within a few ulps of 60 * (nrep - 1) * rateStar (the count reached nrep) or,
+    // at a rate the check rejects, 60 * nrep * RateRange.Max (the rejection started): when a bracket of +-64 ulps
+    // around that estimate holds it, bisect there; otherwise over the whole range.
+    if (at.nrep >= 1 && at.gate != 0) {
+        double est = 60.0 * (double)(at.nrep - 1) * (double)p.rate_star;
+        if (at.gate == 2) est = fmax(est, 60.0 * (double)at.nrep * (double)p.rmax);
+        const unsigned e = __float_as_uint(__double2float_rn(est));
+        const unsigned bl = e > l && e - l > 64 ? e - 64 : l, bh = e < h && h - e > 64 ? e + 64 : h;
+        if (est < 3.0e38 && bl < bh && (bl == l || !same(bl)) && (bh == h || same(bh))) {
+            l = bl;
+            h = bh;
+        }
+    }
+    while (h - l > 1) {
+        const unsigned m = l + (h - l) / 2;
+        if (same(m)) h = m;
+        else l = m;
+    }
+    return __uint_as_float(h);
+}
+
+// Accelerator a of server s at rate 0 of row `row` (the window's bottom lo = 0): its zero-load record or nil, as
+// iv_advance sets it there.
+__device__ __forceinline__ void mg_at_zero(const DevFleet& f, const float* lo, int row, int s, int a, IvAcc& p) {
+    const int cls = pair_class(at_level(f, lo, row), s, a, true);
+    p.tail = 0;
+    p.key = cand_nil();
+    if (cls == PAIR_ZERO) {
+        p.key = zero_load_alloc(f, s, a);
+        p.key.value = penalty_of(f, s, p.key);
+    }
+}
+
+// Record k (0: at, 1: below, 2: above) of item i is winner w's record at the walk's point: a load pair's goes to
+// margin_tail, any other is stored as it is (a zero-load record or nil).  Lane 0 calls it.
+__device__ __forceinline__ void mg_emit(const MarginArgs& g, int k, int i, int w, const IvAcc* acc) {
+    const int r = k * g.n + i;
+    if (w >= 0 && acc[w].tail) fb_push(g.items, fb_pack(w, r));
+    else store_cand(g.rec, r, w >= 0 ? acc[w].key : cand_nil());
+}
+
+// One warp per (level, server) item i = l * S + s; the accelerators' IvAcc states, then their stretch starts, live
+// in dynamic shared memory (A entries of each per warp).  Launched with up to 128 threads; with
+// __launch_bounds__(128) ptxas keeps it at 72 registers and spills, with room for 96 it uses 80 and does not.
+__global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
+    extern __shared__ IvAcc iv_acc[];
+    const DevFleet& f = g.ld.f;
+    const int A = f.A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+    const int i = blockIdx.x * wpb + wid;
+    if (i >= g.n) return;
+    const int l = i / f.S, s = i - l * f.S;
+    IvAcc* acc = iv_acc + (size_t)wid * A;
+    float* start = (float*)(iv_acc + (size_t)wpb * A) + (size_t)wid * A;
+    const float r = g.rate[i], lo = g.lo[i], hi = g.hi[i];
+    const float inf = __int_as_float(0x7f800000);
+    auto advance = [&](int a, float x) { iv_advance(g, l, s, a, x, hi, acc[a]); };
+    bool over = false;
+    for (int a = lane; a < A; a += 32) {
+        advance(a, r);
+        over |= acc[a].over;
+    }
+    __syncwarp();
+    // The load intervals over the window visit its smallest positive rate, where a min_replicas-0 pair may have 0
+    // replicas; the call refuses the window as they do (r = 0 steps there first, see below).
+    const float bottom = lo > 0.0f ? lo : __int_as_float(1);
+    if (r > 0.0f && bottom < r)
+        for (int a = lane; a < A; a += 32)
+            if (acc[a].tail && iv_state(f, s, a, acc[a], bottom, nullptr).nrep == 0) *g.status = 1;
+    const int w0 = iv_winner(acc, A, lane);
+    const Cand key = w0 >= 0 ? acc[w0].key : cand_nil();
+    if (lane == 0) mg_emit(g, 0, i, w0, acc);
+    int flags = 0;
+    float lo_out = r, hi_out = r;
+    if (__any_sync(0xffffffffu, over)) {
+        flags = MG_TRUNCATED;  // a pair needs more than INT32_MAX replicas at r
+    } else {
+        // up: the union of the pairs' steps above r, as interval_kernel walks it
+        for (;;) {
+            float nx = inf;
+            for (int a = lane; a < A; a += 32) nx = fminf(nx, acc[a].next);
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) nx = fminf(nx, __shfl_xor_sync(0xffffffffu, nx, d));
+            if (!(nx <= hi)) {
+                flags |= MG_HI_OPEN;
+                hi_out = inf;
+                break;
+            }
+            __syncwarp();
+            for (int a = lane; a < A; a += 32)
+                if (acc[a].next == nx) {
+                    advance(a, nx);
+                    over |= acc[a].over;
+                }
+            __syncwarp();
+            hi_out = nx;
+            if (__any_sync(0xffffffffu, over)) {  // the stretch ends below the first rate that overflows
+                flags |= MG_TRUNCATED;
+                break;
+            }
+            const int w = iv_winner(acc, A, lane);
+            if (!iv_same_key(w >= 0 ? acc[w].key : cand_nil(), key)) {
+                if (lane == 0) mg_emit(g, 2, i, w, acc);
+                break;
+            }
+        }
+        // down: from r to the first rate below which the key differs
+        if (!(r > 0.0f)) {
+            flags |= MG_LO_OPEN;  // r = 0 is the window's bottom
+            lo_out = lo;
+        } else {
+            // Every pair's key and stretch at r first (x = y = r); then at each step down the pairs whose stretch
+            // starts at y take their key and stretch at x, the float below y.  Below the smallest positive rate
+            // lies rate 0, a point of its own.
+            for (int a = lane; a < A; a += 32) start[a] = r;
+            float x = r, y = r;
+            for (;;) {
+                const bool at_zero = !(x > 0.0f);
+                __syncwarp();
+                for (int a = lane; a < A; a += 32) {
+                    if (at_zero) mg_at_zero(f, g.lo, l, s, a, acc[a]);
+                    else if (start[a] == y) start[a] = mg_start(f, s, a, acc[a], x, bottom);
+                }
+                __syncwarp();
+                if (x != r) {
+                    const int w = iv_winner(acc, A, lane);
+                    if (!iv_same_key(w >= 0 ? acc[w].key : cand_nil(), key)) {
+                        lo_out = y;
+                        if (lane == 0) mg_emit(g, 1, i, w, acc);
+                        break;
+                    }
+                }
+                y = bottom;
+                for (int a = lane; a < A; a += 32) y = fmaxf(y, start[a]);
+#pragma unroll
+                for (int d = 16; d > 0; d >>= 1) y = fmaxf(y, __shfl_xor_sync(0xffffffffu, y, d));
+                // no pair changes its state in [bottom, x]: the stretch reaches the window's bottom
+                if (at_zero || (y == bottom && lo > 0.0f)) {
+                    flags |= MG_LO_OPEN;
+                    lo_out = lo;
+                    break;
+                }
+                x = mg_below(y);
+            }
+        }
+    }
+    if (lane == 0) {
+        g.lo_out[i] = lo_out;
+        g.hi_out[i] = hi_out;
+        g.flags[i] = (uint8_t)flags;
+    }
+}
+
+// The item fb_pack(a, k * n + i): record k of item i, whose winner is the load pair of accelerator a, the load
+// grid's tail at the record's rate (r, the float below lo_out, or hi_out), then the value.
+struct MgTail {
+    const MarginArgs& g;
+    template <class Solve>
+    __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
+        const DevFleet& f = g.ld.f;
+        const int r = (int)(unsigned)item, a = (int)(item >> 32), k = r / g.n, i = r - k * g.n, s = i % f.S;
+        const float x = k == 0 ? g.rate[i] : (k == 1 ? mg_below(g.lo_out[i]) : g.hi_out[i]);
+        const int e = g.cand_of_pair[s * f.A + a];
+        if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, x); }, solve, out)) return false;
+        if (out.feasible) out.value = penalty_of(f, s, out);
+        return true;
+    }
+    __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
+};
+
+__global__ void __launch_bounds__(256) margin_tail(MarginArgs g) {
+    const int n = min(*g.items.count, g.items.cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        tail_item(g.ld.fb, g.rec, g.items.item[i], MgTail{g});
+}
+
+// Stored-vector re-run of the records margin_tail bailed on.
+__global__ void margin_fallback(MarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail{g}); }
 
 }  // namespace wva

@@ -145,9 +145,28 @@ def slo_envelope(fleet: Fleet, bounds, which: int):
     return _key_targets(floor), _key_targets(ceiling)
 
 
+def within_margins(lo, hi, flags, new_rpm, rpm_hi):
+    """The (L, S) mask of servers whose new arrival rate lies inside the stretch ``Engine.load_margins`` returned
+    for them (host only, no GPU).  For those servers ``load_grid`` at the new rate returns the decision key of
+    ``at``, so a reconcile loop can skip their re-solve.
+
+    The stretch is ``[lo, hi)``.  An open end is the window's edge, not a change: below ``rpm_lo`` (= ``lo`` with
+    ``MARGIN_LO_OPEN``) and above ``rpm_hi`` (the window tops the margins were computed over, needed because ``hi``
+    is +Inf with ``MARGIN_HI_OPEN``) nothing is known, so a rate there is outside.  A stretch truncated at the rate
+    itself (``lo == hi``) holds nothing; NaN is never inside."""
+    lo, hi, top, x = (np.asarray(v, np.float32) for v in (lo, hi, rpm_hi, new_rpm))
+    flags = np.asarray(flags, np.uint8)
+    if not lo.shape == hi.shape == flags.shape == top.shape == x.shape:
+        raise ValueError("lo, hi, flags, new_rpm and rpm_hi must have one shape")
+    hi_open = (flags & _abi.MARGIN_HI_OPEN) != 0
+    return (lo <= x) & np.where(hi_open, x <= top, x < hi)
+
+
 # the fleet column each load or target row list replaces (every other row list is named after its column)
+# (the load margins' window rows are rates, shaped and typed like the arrival rates)
 _ROW_COLUMN = {"arrival_rpm": "srv_arrival_rpm", "in_tokens": "srv_in_tokens", "out_tokens": "srv_out_tokens",
-               "slo_itl": "srv_slo_itl", "slo_ttft": "srv_slo_ttft", "slo_tps": "srv_slo_tps"}
+               "slo_itl": "srv_slo_itl", "slo_ttft": "srv_slo_ttft", "slo_tps": "srv_slo_tps",
+               "rpm_lo": "srv_arrival_rpm", "rpm_hi": "srv_arrival_rpm"}
 _PROFILE_COLUMNS = ("acc_cost", "perf_present", "perf_alpha", "perf_beta", "perf_gamma", "perf_delta",
                     "perf_acc_count", "perf_max_batch", "perf_at_tokens")
 
@@ -442,6 +461,34 @@ class Engine:
         self._resident(fleet)
         self._check(self._L.wva_load_intervals(self._h, C.byref(fc), _abi.ptr(lo), _abi.ptr(hi), C.byref(oc)))
         return count, truncated, start, rec
+
+    def load_margins(self, fleet: Fleet, arrival_rpm=None, rpm_lo=None, rpm_hi=None):
+        """The stretch of arrival rates around each level's rate on which ``load_grid``'s winner keeps its decision
+        -> (lo (L, S), hi (L, S), flags (L, S), at, below, above), the records ``Allocs`` of L * S.
+
+        Level ``l`` is ``load_grid``'s row ``l`` of ``arrival_rpm`` (shape (L, S), req/min; ``None``: one level at
+        the fleet's own load).  ``[lo[l, s], hi[l, s])`` is the largest float32 stretch inside the window
+        ``[rpm_lo, rpm_hi]`` (shape (L, S); by default ``[0, 2 * rate]``) that holds the rate and on which the
+        winner's decision key does not change; ``at``, ``below`` and ``above`` are ``load_grid``'s winners at the
+        rate, one float32 below ``lo`` and at ``hi``.  ``flags`` holds ``MARGIN_LO_OPEN`` (no change down to
+        ``rpm_lo``), ``MARGIN_HI_OPEN`` (none up to ``rpm_hi``, ``hi`` = +Inf) and ``MARGIN_TRUNCATED`` (see
+        ``wva_load_margins`` in include/wva_b200.h).  ``within_margins`` tests new rates against the result."""
+        S = fleet.n_servers
+        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "rpm_lo": rpm_lo, "rpm_hi": rpm_hi})
+        L = 1 if L is None else L
+        rate = rows.get("arrival_rpm", np.ascontiguousarray(np.broadcast_to(fleet.srv_arrival_rpm, (L, S)), np.float32))
+        lo = rows.get("rpm_lo", np.zeros((L, S), np.float32))
+        hi = rows.get("rpm_hi", (rate * np.float32(2)).astype(np.float32))
+        lo_out, hi_out = np.zeros((L, S), np.float32), np.zeros((L, S), np.float32)
+        flags = np.zeros((L, S), np.uint8)
+        at, below, above = Allocs(L * S), Allocs(L * S), Allocs(L * S)
+        oc = _abi.MarginsC(_abi.ptr(lo_out.reshape(-1)), _abi.ptr(hi_out.reshape(-1)), _abi.ptr(flags.reshape(-1)),
+                           at.as_c(), below.as_c(), above.as_c())
+        fc = fleet.as_c()
+        self._resident(fleet)
+        self._check(self._L.wva_load_margins(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)),
+                                             _abi.ptr(lo.reshape(-1)), _abi.ptr(hi.reshape(-1)), C.byref(oc)))
+        return lo_out, hi_out, flags, at, below, above
 
     def price_thresholds(self, fleet: Fleet, want_candidates: bool = False):
         """The exact price of each accelerator at which each server's unlimited winner leaves it -> (threshold
