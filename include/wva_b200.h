@@ -668,6 +668,47 @@ int wva_price_thresholds(wva_handle *h, const wva_fleet *fleet, float *threshold
                          wva_allocs *above /* [S*A], may be NULL */, wva_allocs *candidates /* [S*A], may be NULL */);
 
 /*
+ * Price threshold grid and trace: wva_price_thresholds at every row of a forecast, e.g. how many units of
+ * accelerator a the fleet uses at each price of a in each hour.  The rows are laid out as in wva_workload_grid:
+ * arrival_rpm, in_tokens and out_tokens are [L*S], index l*S + s, with L = n_levels or n_ticks.  arrival_rpm is
+ * required; a NULL token list is the fleet's own column at every row.  Output block l of threshold, above and
+ * candidates is records (l*S + s)*A + a; of winners, l*S + s.
+ *
+ *   - Grid, level l.  Let f_l be the fleet with row l of the three lists.  Block l of threshold, above and
+ *     candidates is byte for byte what wva_price_thresholds(f_l) returns, and winner block l is wva_workload_grid's.
+ *   - Trace, tick t.  Let f_t be the fleet with row t and current allocation c_t, the current allocation
+ *     wva_workload_trace carries into tick t (the last feasible winner of ticks 0..t-1, the fleet's own without
+ *     one).  Block t is byte for byte wva_price_thresholds(f_t), and winners are wva_workload_trace's.  So the price
+ *     of a changes at tick t only: the ticks before t do not read it, c_t does not move, and the argument of
+ *     wva_price_thresholds applies to f_t as it stands.  A price that changes at every tick is not offered: through
+ *     the chain a's winning at tick t-1 changes c_t, and nothing shows its winning prices are then one interval
+ *     (DESIGN.md §3.20).
+ *
+ * Only unlimited mode is covered: fleet->unlimited and the capacities are not read.  The fleet becomes resident,
+ * and wva_summarize returns WVA_ERR_STATE afterwards.  above and candidates may be NULL, and so may any of their
+ * columns (not written); winners may not.  L == 0 is valid (nothing is written).  WVA_ERR_BAD_ARG: L < 0, winners
+ * NULL, arrival_rpm NULL with L*S > 0, threshold NULL with L*S*A > 0.  WVA_ERR_UNSUPPORTED, with wva_last_error
+ * naming the rule and, for a current cost, the server and the level or tick:
+ *   - whatever wva_workload_grid (grid) or wva_workload_trace (trace) refuses on the same rows, and L*S*A >= 2^31;
+ *   - before any launch, a penalty factor that is NaN, negative or infinite;
+ *   - grid, before any launch: an srv_cur_cost that is NaN or infinite on a server with a pair that wva_analyze(f_l)
+ *     does not class nil at some level l;
+ *   - trace, after the winners are known: a c_t cost that is NaN or infinite on a server with a pair that
+ *     wva_analyze(f_t) does not class nil.  A carried cost can be +Inf: a winner with c_t's accelerator and replica
+ *     count has value 0 whatever its cost, and an acc_cost near MaxFloat32 makes that cost overflow.  The outputs
+ *     are then unspecified.
+ * Each is a case in which wva_price_thresholds refuses some level's or tick's fleet.
+ */
+int wva_price_threshold_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
+                             const int32_t *in_tokens, const int32_t *out_tokens, float *threshold /* [L*S*A] */,
+                             wva_allocs *above /* [L*S*A], may be NULL */,
+                             wva_allocs *candidates /* [L*S*A], may be NULL */, wva_allocs *winners /* [L*S] */);
+int wva_price_threshold_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                              const int32_t *in_tokens, const int32_t *out_tokens, float *threshold /* [L*S*A] */,
+                              wva_allocs *above /* [L*S*A], may be NULL */,
+                              wva_allocs *candidates /* [L*S*A], may be NULL */, wva_allocs *winners /* [L*S] */);
+
+/*
  * SLO bounds: for each (server s, accelerator a) and search w (0: TTFT, 1: ITL), the exact targets at which the
  * reference's candidate turns nil and at which its target stops binding.  Entry (s*A + a)*2 + w of each column.
  *

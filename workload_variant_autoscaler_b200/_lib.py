@@ -42,7 +42,7 @@ EXPORTS = (
     "wva_xchg_create", "wva_xchg_open", "wva_xchg_publish", "wva_xchg_error", "wva_xchg_destroy", "wva_size_grid",
     "wva_load_grid", "wva_load_intervals", "wva_load_margins", "wva_slo_grid", "wva_workload_grid",
     "wva_workload_trace", "wva_profile_grid", "wva_profile_trace", "wva_price_thresholds", "wva_slo_bounds",
-    "wva_slo_trace",
+    "wva_slo_trace", "wva_price_threshold_grid", "wva_price_threshold_trace",
 )
 
 _lib = None
@@ -88,6 +88,10 @@ def lib():
         ("wva_profile_trace", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p, C.POINTER(_abi.ProfileRowsC),
                                C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
         ("wva_price_thresholds", [vp, C.POINTER(_abi.FleetC), f32p, C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
+        ("wva_price_threshold_grid", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p, f32p, C.POINTER(_abi.AllocsC),
+                                      C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
+        ("wva_price_threshold_trace", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p, f32p, C.POINTER(_abi.AllocsC),
+                                       C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
         ("wva_slo_bounds", [vp, C.POINTER(_abi.FleetC), C.POINTER(_abi.SloBoundsC)]),
         ("wva_sweep", [vp, C.POINTER(_abi.FleetC), i32, C.POINTER(_abi.SweepOutC)]),
         ("wva_upload", [vp, C.POINTER(_abi.FleetC)]),

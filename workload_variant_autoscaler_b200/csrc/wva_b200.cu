@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <numeric>
 #include <string>
 #include <vector>
@@ -142,13 +143,21 @@ struct HostFleet {
     }
     // ... with `present` in place of the model's perf_present at a (the profile grid's rows)
     int pair_class(int s, int a, bool honour_keep, float rpm, bool present) const {
-        if (honour_keep && srv_keep_acc[s] && srv_cur_acc[s] != WVA_ACC_NONE && srv_cur_acc[s] != a) return 0;
-        if (rpm < 0.0f || srv_in_tokens[s] < 0 || srv_out_tokens[s] < 0) return 0;
+        return pair_class(s, a, honour_keep, rpm, srv_in_tokens[s], srv_out_tokens[s], srv_cur_acc[s], present);
+    }
+    // ... at a row's tokens in / out and current accelerator cur (a level's or a trace tick's)
+    int pair_class(int s, int a, bool honour_keep, float rpm, int in, int out, int cur) const {
+        const int m = srv_model[s];
+        return pair_class(s, a, honour_keep, rpm, in, out, cur, m >= 0 && m < M && perf_present[(size_t)m * A + a]);
+    }
+    int pair_class(int s, int a, bool honour_keep, float rpm, int in, int out, int cur, bool present) const {
+        if (honour_keep && srv_keep_acc[s] && cur != WVA_ACC_NONE && cur != a) return 0;
+        if (rpm < 0.0f || in < 0 || out < 0) return 0;
         const int m = srv_model[s];
         if (m < 0 || m >= M) return 0;
         if (!present) return 0;
         if (!srv_has_target[s]) return 0;
-        if (rpm == 0.0f || srv_out_tokens[s] == 0) return PAIR_ZERO;
+        if (rpm == 0.0f || out == 0) return PAIR_ZERO;
         return PAIR_LOAD;
     }
     // batch size of a candidate: pkg/core/allocation.go:77-87, in Go's 64-bit int (the AtTokens rule can exceed int32)
@@ -832,10 +841,16 @@ int run_size_host(wva_handle* h, wva_allocs* candidates, wva_allocs* winners) {
 // profile grids, the workload and profile traces), named `name` in wva_last_error: the argument checks, the upload,
 // then enqueue(dc, dw) under run_host and both blocks back to the caller.  null_rows is the call's refusal when some
 // row list it needs is NULL (it applies when S * L > 0), or NULL; with row_entries the L * M * A entries of a
-// wva_profile_rows list are bounded as well.  A trace's rows are ticks, a grid's levels.
+// wva_profile_rows list are bounded as well.  A trace's rows are ticks, a grid's levels.  A call with outputs beyond
+// the two blocks (the price threshold grid and trace) passes `more`.
+struct LevelMore {
+    std::function<int(HostCall&)> place;        // after the upload, before any launch: refuse, or set c.extra
+    std::function<int(const HostCall&)> check;  // after the sync, before the blocks reach the caller: refuse
+};
 template <class Enqueue>
 int run_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const char* name, const char* null_rows,
-               bool row_entries, wva_allocs* candidates, wva_allocs* winners, Enqueue&& enqueue) {
+               bool row_entries, wva_allocs* candidates, wva_allocs* winners, Enqueue&& enqueue,
+               const LevelMore& more = LevelMore{}) {
     if (!h || !winners) return WVA_ERR_BAD_ARG;
     if (L < 0) return h->fail(WVA_ERR_BAD_ARG, strstr(name, "trace") ? "negative tick count" : "negative level count");
     if (!fleet) return h->fail(WVA_ERR_BAD_ARG, "fleet is NULL");
@@ -851,9 +866,11 @@ int run_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const char* nam
     if (rc) return rc;
     HostCall c{(size_t)n_cand, candidates != nullptr, true};
     c.win_blocks = (size_t)L;
+    if (more.place && (rc = more.place(c))) return rc;
     rc = run_host(h, c, enqueue);
     // no single solution to summarise (upload_fleet cleared last_kind)
     if (rc) return rc;
+    if (more.check && (rc = more.check(c))) return rc;
     scatter_block(c.cand_host, c.bc, candidates);
     scatter_block(c.win_host, c.bw, winners);
     return WVA_OK;
@@ -1588,8 +1605,8 @@ KeyFleet workload_keys(const HostFleet& hf, int L, const float* rpm, const int32
 // level uses under load (rate not negative and not 0, NaN and +Inf included; in_tokens >= 0; out_tokens >= 1).
 // Phase 2 (workload_kernel, workload_fallback) is the load grid's tail per (key candidate, level of the key).  The
 // lists, the key fleet's server columns and the tables go into lg_tabs, rebuilt on every call.  Then the unlimited
-// winner of every level.  rpm / in / out [L*S] are the caller's rows; cand ([L*S*A]) and winners ([L*S]) are device
-// columns.
+// winner of every level.  rpm / in / out [L*S] are the caller's rows (a NULL token list: the fleet's own column at
+// every row); cand ([L*S*A]) and winners ([L*S]) are device columns.
 //
 // With `trace` (the workload trace, DESIGN.md §3.13) the records carry keepAccelerator on the pinned servers only
 // (trace_pinned), in trivial_kernel and in the key fleet alike.  trace_kernel's chain then picks the winners: one
@@ -1606,7 +1623,7 @@ int enqueue_workload(wva_handle* h, int L, const float* rpm, const int32_t* in, 
     const size_t o_pin = trace ? c.put(pin.data(), S) : 0;
     // the keys: at most L * S, so fewer than 2^31 key candidates
     TokenKeys tk;
-    KeyFleet kf = workload_keys(hf, L, rpm, in, out, trace ? pin.data() : nullptr, tk);
+    KeyFleet kf = workload_keys(hf, L, rpm, lists.in.host, lists.out.host, trace ? pin.data() : nullptr, tk);
     const int K = (int)tk.srv.size();
     kf.place(c);
     tk.place(c, (size_t)K * A);
@@ -2097,16 +2114,51 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
 // ---- price thresholds: the price of each accelerator at which each server's winner leaves it (DESIGN.md §3.16) --
 // The inputs on which a pair's value can decrease as its price grows, so that its winning prices need not be one
 // interval from 0: a penalty factor that is NaN, negative or infinite, or a non-finite current cost on a server
-// that has a candidate (a pair wva_analyze does not class nil).  nullptr when there is none.
-const char* price_refusal(const HostFleet& hf) {
+// that has a candidate (a pair wva_analyze does not class nil).  The first rule is the fleet's; the second is
+// checked per row of L rows (the single call's one row is the fleet itself): at row l server s has the arrival rate
+// rpm[l*S + s], the tokens in / out[l*S + s] (NULL: the fleet's own column) and the current allocation cur(l, s) ->
+// (accelerator, cost).  Each returns its refusal, empty when there is none.
+std::string price_factor_refusal(const HostFleet& hf) {
     const float f = hf.tun.accel_penalty_factor;
-    if (!(f >= 0.0f) || std::isinf(f)) return "penalty factor NaN, negative or infinite";
-    for (int s = 0; s < hf.S; ++s) {
-        if (std::isfinite(hf.srv_cur_cost[s])) continue;
-        for (int a = 0; a < hf.A; ++a)
-            if (hf.pair_class(s, a, true)) return "current cost NaN or infinite on a server with a candidate";
-    }
-    return nullptr;
+    return !(f >= 0.0f) || std::isinf(f) ? "penalty factor NaN, negative or infinite" : "";
+}
+template <class Cur>
+std::string price_cost_refusal(const HostFleet& hf, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                               const char* row, Cur&& cur) {
+    const int S = hf.S;
+    for (int l = 0; l < L; ++l)
+        for (int s = 0; s < S; ++s) {
+            const std::pair<int, float> c = cur(l, s);
+            if (std::isfinite(c.second)) continue;
+            const size_t i = (size_t)l * S + s;
+            const int ki = in ? in[i] : hf.srv_in_tokens[s], ko = out ? out[i] : hf.srv_out_tokens[s];
+            for (int a = 0; a < hf.A; ++a)
+                if (hf.pair_class(s, a, true, rpm[i], ki, ko, c.first)) {
+                    std::string what = "current cost NaN or infinite on a server with a candidate (server " +
+                                       std::to_string(s);
+                    return row ? what + ", " + row + " " + std::to_string(l) + ")" : what + ")";
+                }
+        }
+    return "";
+}
+std::string price_refusal(const HostFleet& hf) {
+    const std::string what = price_factor_refusal(hf);
+    if (!what.empty()) return what;
+    return price_cost_refusal(hf, 1, hf.srv_arrival_rpm.data(), nullptr, nullptr, nullptr,
+                              [&](int, int s) { return std::make_pair(hf.srv_cur_acc[s], hf.srv_cur_cost[s]); });
+}
+
+// price_kernel over L candidate blocks whose values are set (DESIGN.md §3.16, §3.20): threshold and above
+// ([L*S*A], device; a NULL above column is not written), the current allocation the fleet's, or with `chain` the
+// trace's c_l from its winner blocks ([L*S]).
+void enqueue_price(wva_handle* h, int L, const AllocCols& cand, float* threshold, const AllocCols& above,
+                   const AllocCols* chain) {
+    const HostFleet& hf = h->hf;
+    const long long warps = (long long)L * hf.S;
+    if (warps * hf.A <= 0) return;
+    price_kernel<<<(unsigned)((warps + 3) / 4), 128, 0, h->stream>>>(
+        PriceArgs{h->df, cand, threshold, above, chain ? *chain : AllocCols{}, L});
+    h->launches++;
 }
 
 // wva_analyze's sizing and values into cand ([S*A]), then price_kernel: threshold ([S*A], device) and above
@@ -2114,13 +2166,76 @@ const char* price_refusal(const HostFleet& hf) {
 int enqueue_price_thresholds(wva_handle* h, float* threshold, const AllocCols& cand, const AllocCols& above) {
     int rc = enqueue_size(h, cand, &above);
     if (rc) return rc;
-    const HostFleet& hf = h->hf;
-    if ((long long)hf.S * hf.A > 0) {
-        price_kernel<<<(hf.S + 3) / 4, 128, 0, h->stream>>>(h->df, cand, threshold, above);
-        h->launches++;
-    }
+    enqueue_price(h, 1, cand, threshold, above, nullptr);
     CK(cudaGetLastError());
     return WVA_OK;
+}
+
+// The price threshold grid and trace (DESIGN.md §3.20): wva_workload_grid's or wva_workload_trace's call with
+// price_kernel after the winners.  threshold and above's columns are the call's further device columns in d_price,
+// copied straight to the caller.  The cost rule is checked per level before any launch; for a trace c_t is known only
+// from the winners, so it is checked per tick after the sync, on the winner block's host copy.
+int run_price_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const float* rpm, const int32_t* in,
+                     const int32_t* out, float* threshold, wva_allocs* above, wva_allocs* candidates,
+                     wva_allocs* winners, bool trace) {
+    if (h && winners && fleet && L > 0 && (long long)fleet->n_servers * fleet->n_acc > 0 && !threshold)
+        return h->fail(WVA_ERR_BAD_ARG, "threshold is NULL");
+    const char* name = trace ? "price threshold trace" : "price threshold grid";
+    Cols cols(16);
+    AllocCols dab{};  // above's device columns, set by place
+    LevelMore more;
+    more.place = [&](HostCall& c) {
+        const HostFleet& hf = h->hf;
+        std::string what = price_factor_refusal(hf);
+        if (what.empty() && !trace)
+            what = price_cost_refusal(hf, L, rpm, in, out, "level", [&](int, int s) {
+                return std::make_pair(hf.srv_cur_acc[s], hf.srv_cur_cost[s]);
+            });
+        if (!what.empty()) return h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
+        // threshold first, at the buffer's start; then the above columns the caller wants (SIZE_MAX: not placed)
+        const size_t n = c.n_cand;
+        cols.take(4 * n, threshold);
+        Block ab{};
+#define PRICE_ABOVE(name, type, required) \
+    ab.off.name = above && above->name ? cols.take(sizeof(type) * n, above->name) : SIZE_MAX;
+        WVA_ALLOC_COLUMNS(PRICE_ABOVE)
+#undef PRICE_ABOVE
+        CK(h->d_price.ensure(cols.bytes));
+        char* d = (char*)h->d_price.p;
+#define PRICE_ABOVE_DEV(name, type, required) dab.name = ab.off.name == SIZE_MAX ? nullptr : (type*)(d + ab.off.name);
+        WVA_ALLOC_COLUMNS(PRICE_ABOVE_DEV)
+#undef PRICE_ABOVE_DEV
+        c.extra = &cols;
+        c.extra_dev = d;
+        return WVA_OK;
+    };
+    if (trace)
+        more.check = [&](const HostCall& c) {
+            const HostFleet& hf = h->hf;
+            const uint8_t* feasible = (const uint8_t*)(c.win_host + c.bw.off.feasible);
+            const int32_t* acc = (const int32_t*)(c.win_host + c.bw.off.acc);
+            const float* cost = (const float*)(c.win_host + c.bw.off.cost);
+            // c_t per server, advanced tick by tick as price_cost_refusal walks the rows in order
+            std::vector<std::pair<int, float>> cur(hf.S);
+            for (int s = 0; s < hf.S; ++s) cur[s] = {hf.srv_cur_acc[s], hf.srv_cur_cost[s]};
+            const std::string what = price_cost_refusal(hf, L, rpm, in, out, "tick", [&](int t, int s) {
+                const std::pair<int, float> ct = cur[s];
+                const size_t j = (size_t)t * hf.S + s;
+                if (feasible[j]) cur[s] = {acc[j], cost[j]};
+                return ct;
+            });
+            return what.empty() ? WVA_OK : h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
+        };
+    return run_levels(
+        h, fleet, L, name, rpm ? nullptr : "NULL arrival rate list", false, candidates, winners,
+        [&](const AllocCols& dc, const AllocCols& dw) {
+            const int rc = enqueue_workload(h, L, rpm, in, out, dc, dw, trace);
+            if (rc) return rc;
+            enqueue_price(h, L, dc, (float*)h->d_price.p, dab, trace ? &dw : nullptr);
+            CK(cudaGetLastError());
+            return WVA_OK;
+        },
+        more);
 }
 
 // ---- SLO bounds: where each load pair's two searches turn nil and stop binding (DESIGN.md §3.18) ----------------
@@ -3161,7 +3276,8 @@ int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold
     CK(cudaSetDevice(h->device));
     int rc = upload_fleet(h, fleet);
     if (rc) return rc;
-    if (const char* what = price_refusal(h->hf)) return h->fail(WVA_ERR_UNSUPPORTED, what);
+    const std::string what = price_refusal(h->hf);
+    if (!what.empty()) return h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
     Cols th(16);
     th.take(4 * (size_t)n, threshold);
     CK(h->d_price.ensure(th.bytes));
@@ -3175,6 +3291,20 @@ int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold
     scatter_block(c.cand_host, c.bc, candidates);
     if (c.win_host) scatter_block(c.win_host, c.bw, above);
     return WVA_OK;
+}
+
+int wva_price_threshold_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                             const int32_t* in_tokens, const int32_t* out_tokens, float* threshold, wva_allocs* above,
+                             wva_allocs* candidates, wva_allocs* winners) {
+    return run_price_levels(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, threshold, above, candidates,
+                            winners, false);
+}
+
+int wva_price_threshold_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                              const int32_t* in_tokens, const int32_t* out_tokens, float* threshold, wva_allocs* above,
+                              wva_allocs* candidates, wva_allocs* winners) {
+    return run_price_levels(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, threshold, above, candidates,
+                            winners, true);
 }
 
 int wva_slo_bounds(wva_handle* h, const wva_fleet* fleet, wva_slo_bounds_out* out) {

@@ -1909,6 +1909,11 @@ __global__ void profile_trace_kernel(ProfileTraceArgs g) {
 // TransitionPenalty of a's record at cost_at(.., p), and no other record reads p.  It never decreases as p grows
 // (a NaN counted as +Inf), so a wins on [+0, threshold), found by bisecting the non-negative float32 bit patterns.
 // above is w's record (nil without one), zero bytes where the threshold is +Inf.
+//
+// The level calls (DESIGN.md §3.20) run the same per level: one warp per (level l, server s) over candidate block l,
+// whose values are TransitionPenalty against the level's current allocation.  That is the fleet's for the single call
+// and the grid.  For the trace it is c_l, the last feasible winner of the ticks before l (the fleet's without one),
+// which the warp finds by scanning the trace's winner blocks backwards, 32 ticks per ballot.
 struct PriceBest {  // a record's (value, accelerator id); id INT_MAX: none
     float v;
     int a;
@@ -1919,10 +1924,24 @@ __device__ __forceinline__ bool price_before(float v, int a, const PriceBest& b)
 __device__ __forceinline__ PriceBest shfl_xor_best(const PriceBest& b, int d) {
     return PriceBest{__shfl_xor_sync(0xffffffffu, b.v, d), __shfl_xor_sync(0xffffffffu, b.a, d)};
 }
-__global__ void __launch_bounds__(128) price_kernel(DevFleet f, AllocCols cand, float* threshold, AllocCols above) {
-    const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+struct PriceArgs {
+    DevFleet f;
+    AllocCols cand;     // [L * S * A] records (l * S + s) * A + a, value = TransitionPenalty
+    float* threshold;   // [L * S * A]
+    AllocCols above;    // [L * S * A]; a NULL column is not written
+    AllocCols chain;    // a trace's winners [L * S], tick-major; chain.feasible NULL: the fleet's current allocation
+    int L;
+};
+__global__ void __launch_bounds__(128) price_kernel(PriceArgs g) {
+    const DevFleet& f = g.f;
+    const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    if (s >= f.S) return;  // whole warps
+    if (w >= (long long)g.L * f.S) return;  // whole warps
+    const int l = (int)(w / f.S), s = (int)(w - (long long)l * f.S);
+    // block l, indexed by s * A + a below
+    const size_t block = (size_t)l * f.S * f.A;
+    const AllocCols cand = cols_at(g.cand, block), above = cols_at(g.above, block);
+    float* const threshold = g.threshold + block;
     const float max_f32 = 3.40282346638528859811704183484516925440e+38f;
     const unsigned max_bits = 0x7f7fffffu;
     const PriceBest none{__int_as_float(0x7f800000), INT_MAX};
@@ -1949,8 +1968,23 @@ __global__ void __launch_bounds__(128) price_kernel(DevFleet f, AllocCols cand, 
             b2 = o1;
         }
     }
-    const int m = f.srv_model[s], cur_acc = f.srv_cur_acc[s], cur_replicas = f.srv_cur_replicas[s];
-    const float cur_cost = f.srv_cur_cost[s];
+    const int m = f.srv_model[s];
+    int cur_acc = f.srv_cur_acc[s], cur_replicas = f.srv_cur_replicas[s];
+    float cur_cost = f.srv_cur_cost[s];
+    if (g.chain.feasible) {
+        // lane k looks at tick t0 - k; the lowest set bit is the latest feasible winner (l is warp-uniform)
+        for (int t0 = l - 1; t0 >= 0; t0 -= 32) {
+            const int t = t0 - lane;
+            const unsigned hit = __ballot_sync(0xffffffffu, t >= 0 && g.chain.feasible[(size_t)t * f.S + s]);
+            if (hit) {
+                const size_t j = (size_t)(t0 - (__ffs(hit) - 1)) * f.S + s;
+                cur_acc = g.chain.acc[j];
+                cur_replicas = g.chain.replicas[j];
+                cur_cost = g.chain.cost[j];
+                break;
+            }
+        }
+    }
     for (int a = lane; a < f.A; a += 32) {
         const size_t i = (size_t)s * f.A + a;
         const PriceBest w = b1.a == a ? b2 : b1;

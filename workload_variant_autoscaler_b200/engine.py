@@ -71,6 +71,35 @@ def accelerator_demand(fleet: Fleet, threshold, candidates: Allocs, a: int):
     return breakpoints, np.cumsum(per_k[::-1])[::-1][1:]
 
 
+def demand_by_level(fleet: Fleet, threshold, candidates: Allocs, a: int):
+    """The demand curve for accelerator ``a`` at every row of ``Engine.price_threshold_grid`` or
+    ``price_threshold_trace`` (host only, no GPU) -> (breakpoints, units (L, len(breakpoints) + 1) int64).
+
+    ``breakpoints`` is the ascending union over the rows of column ``a``'s distinct thresholds in (0, MaxFloat32];
+    it cuts the prices [+0, MaxFloat32] into stretches as ``accelerator_demand`` does.  ``units[l, j]`` is
+    ``accelerator_demand``'s count for row ``l`` (threshold block ``l`` and candidate block ``l``, which for a trace
+    is tick ``l``'s block, masked against its current allocation) on stretch ``j`` of the union."""
+    S, A = fleet.n_servers, fleet.n_acc
+    th = np.ascontiguousarray(threshold, np.float32)
+    if th.ndim != 3 or th.shape[1:] != (S, A) or candidates.n != th.shape[0] * S * A:
+        raise ValueError("threshold must have shape (L, n_servers, n_acc) and candidates L * n_servers * n_acc "
+                         "records")
+    n = S * A
+    per_level = []
+    for l in range(th.shape[0]):
+        block = Allocs(n)
+        for k in block.columns():
+            getattr(block, k)[:] = getattr(candidates, k)[l * n:(l + 1) * n]
+        per_level.append(accelerator_demand(fleet, th[l], block, a))
+    breakpoints = np.unique(np.concatenate([bp for bp, _ in per_level] + [np.zeros(0, np.float32)]))
+    starts = np.concatenate([[np.float32(0.0)], breakpoints]).astype(np.float32)
+    units = np.zeros((th.shape[0], starts.size), np.int64)
+    for l, (bp, u) in enumerate(per_level):
+        # the level's own stretch that holds each union stretch: the number of its breakpoints at or below the start
+        units[l] = u[np.searchsorted(bp, starts, side="right")]
+    return breakpoints, units
+
+
 # The smallest positive float32 target, and the position past +Inf as a uint32 key (its float is a NaN): the SLO
 # bounds order targets by their bit patterns, which are ordered like the positive values.
 _MIN_TARGET = np.float32(np.finfo(np.float32).smallest_subnormal)
@@ -510,6 +539,47 @@ class Engine:
         self._check(self._L.wva_price_thresholds(self._h, C.byref(fc), _abi.ptr(threshold.reshape(-1)), C.byref(ac),
                                                  C.byref(cc) if cc is not None else None))
         return threshold, above, cand
+
+    def price_threshold_grid(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None,
+                             want_candidates: bool = False):
+        """``price_thresholds`` at every row of (``arrival_rpm`` req/min, ``in_tokens``, ``out_tokens``), each of
+        shape (L, S) -> (threshold (L, S, A) float32, above: ``Allocs`` of L * S * A, candidates [L*S*A] | None,
+        winners [L*S]).
+
+        Block ``l`` of threshold, above and candidates is ``price_thresholds`` on the fleet with row ``l``, and
+        winner block ``l`` is ``workload_grid``'s (see ``wva_price_threshold_grid`` in include/wva_b200.h).  A token
+        list of ``None`` is the fleet's own column at every level.  ``demand_by_level`` turns a column into demand
+        curves."""
+        return self._price_rows(self._L.wva_price_threshold_grid, fleet, arrival_rpm, in_tokens, out_tokens,
+                                want_candidates)
+
+    def price_threshold_trace(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None,
+                              want_candidates: bool = False):
+        """``price_thresholds`` at every tick of ``workload_trace`` -> (threshold (L, S, A) float32, above:
+        ``Allocs`` of L * S * A, candidates [L*S*A] | None, winners [L*S]).
+
+        Block ``t`` is ``price_thresholds`` on the fleet with row ``t`` and the current allocation the trace carries
+        into tick ``t`` (``fleet.apply_winners`` of every earlier tick in turn): the price changes at tick ``t``
+        only.  Winners are ``workload_trace``'s (see ``wva_price_threshold_trace`` in include/wva_b200.h)."""
+        return self._price_rows(self._L.wva_price_threshold_trace, fleet, arrival_rpm, in_tokens, out_tokens,
+                                want_candidates)
+
+    def _price_rows(self, call, fleet, arrival_rpm, in_tokens, out_tokens, want_candidates):
+        S, A = fleet.n_servers, fleet.n_acc
+        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "in_tokens": in_tokens, "out_tokens": out_tokens})
+        if "arrival_rpm" not in rows:
+            raise ValueError("arrival_rpm is required")
+        threshold = np.zeros((L, S, A), np.float32)
+        above, win = Allocs(L * S * A), Allocs(L * S)
+        cand = Allocs(L * S * A) if want_candidates else None
+        fc, ac, wc = fleet.as_c(), above.as_c(), win.as_c()
+        cc = cand.as_c() if cand is not None else None
+        ptrs = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None
+                for k in ("arrival_rpm", "in_tokens", "out_tokens")]
+        self._resident(fleet)
+        self._check(call(self._h, C.byref(fc), L, *ptrs, _abi.ptr(threshold.reshape(-1)), C.byref(ac),
+                         C.byref(cc) if cc is not None else None, C.byref(wc)))
+        return threshold, above, cand, win
 
     def slo_bounds(self, fleet: Fleet):
         """Where each load pair's TTFT and ITL searches turn the candidate nil and stop binding -> (kind, y_lo, y_hi,
