@@ -79,11 +79,12 @@ def ref_trace(oracle_mod, fleet, rows):
     return np.concatenate(cands), np.concatenate(wins), cur
 
 
-def check_level_call(engine, oracle_mod, name, fleet, rows, what):
-    """Engine.<name> against its composition (ref_trace for a trace, ref_grid for a grid), bit for bit: the
-    oracle's (candidates, winners)."""
-    ref = ref_trace if name.endswith("_trace") else ref_grid
-    cand_o, win_o = ref(oracle_mod, fleet, rows)[:2]
+def check_level_call(engine, oracle_mod, name, fleet, rows, what, ref=None):
+    """Engine.<name> against its composition (ref_trace for a trace, ref_grid for a grid; or `ref`, its result),
+    bit for bit: the oracle's (candidates, winners)."""
+    if ref is None:
+        ref = (ref_trace if name.endswith("_trace") else ref_grid)(oracle_mod, fleet, rows)
+    cand_o, win_o = ref[:2]
     cand_g, win_g = getattr(engine, name)(fleet, **rows, want_candidates=True)
     assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
     assert_allocs_equal(win_g, win_o, f"{what}: winners")
@@ -870,6 +871,244 @@ def _adversarial_fleet(rng, case):
     f.srv_min_replicas[:] = rng.integers(0, 3, S)
     f.max_queue_to_batch_ratio = int(rng.choice([1, 3, 10]))
     return f
+
+
+# ---- price thresholds: wva_price_thresholds' composition at one fleet, and at each level's or tick's fleet ----
+
+PRICE_MAX_BITS = 0x7F7FFFFF
+
+
+def pred(x):
+    """The largest float32 below x (x > 0)."""
+    return from_bits(u32_bits(x) - 1)
+
+
+def at_price(fleet, a, p):
+    """A copy of the fleet with acc_cost[a] = p, unlimited."""
+    f = fleet.take_servers(np.arange(fleet.n_servers))
+    f.acc_cost[a] = p
+    f.unlimited = True
+    return f
+
+
+def priced(fleet, s, a, rec, p):
+    """a's record of server s at price p: cost = p * f32(NumInstances * replicas), value = TransitionPenalty against
+    the fleet's current allocation (allocation.go:144-145, :274-275, :291-300); a nil record is unchanged."""
+    r = rec.copy()
+    if not r["feasible"]:
+        return r
+    inst = int(fleet.perf_acc_count[int(fleet.srv_model[s]), a])
+    inst = 1 if inst <= 0 else inst
+    with np.errstate(all="ignore"):
+        r["cost"] = F32(p) * F32(inst * int(r["replicas"]))
+    r["value"] = transition_penalty(F32(fleet.accel_penalty_factor), int(fleet.srv_cur_acc[s]),
+                                    int(fleet.srv_cur_replicas[s]), fleet.srv_cur_cost[s], int(r["acc"]),
+                                    int(r["replicas"]), r["cost"])
+    return r
+
+
+class PriceServer:
+    """One server's winner as a's price moves: Server.Calculate's row with a's record re-priced, decided by the
+    oracle's Solver.Solve on the one-server fleet.  SolveUnlimited reads only feasible and value, so the solve sees
+    each record with its column id in the batch field, which names the winning column."""
+
+    def __init__(self, oracle_mod, fleet, cand, s):
+        self.o, self.fleet, self.row, self.s = oracle_mod, fleet, cand[s], s
+        self.f1 = fleet.take_servers(np.array([s]))
+        self.f1.unlimited = True
+
+    def winner(self, a, p):
+        """(winning column or -1, winner record) with a's record at price p."""
+        row = self.row.copy()
+        row[a] = priced(self.fleet, self.s, a, row[a], p)
+        tagged = row.copy()
+        tagged["batch"] = np.arange(row.size)
+        w = self.o.solve(self.f1, tagged[None])[1][0]
+        if not w["feasible"]:
+            return -1, w
+        return int(w["batch"]), row[int(w["batch"])]
+
+    def wins(self, a, p):
+        return self.winner(a, p)[0] == a
+
+    def threshold(self, a):
+        """The first float32 price in [+0, MaxFloat32] at which a stops winning, by bisecting the bit patterns."""
+        if self.wins(a, from_bits(PRICE_MAX_BITS)):
+            return F32(np.inf)
+        if not self.wins(a, F32(0.0)):
+            return F32(0.0)
+        lo, hi = 0, PRICE_MAX_BITS
+        while hi - lo > 1:
+            mid = (lo + hi) // 2
+            if self.wins(a, from_bits(mid)):
+                lo = mid
+            else:
+                hi = mid
+        return from_bits(hi)
+
+
+def ref_price_fleet(oracle_mod, fleet):
+    """(threshold [S, A], above [S*A], candidates [S*A], winners [S]) of one fleet: wva_price_thresholds' contract
+    composed from the oracle."""
+    cand = oracle_mod.calculate(fleet)
+    S, A = fleet.n_servers, fleet.n_acc
+    th = np.zeros((S, A), F32)
+    above = np.zeros(S * A, oracle_mod.ALLOC_DTYPE)
+    for s in range(S):
+        sp = PriceServer(oracle_mod, fleet, cand, s)
+        for a in range(A):
+            th[s, a] = sp.threshold(a)
+            if np.isfinite(th[s, a]):
+                above[s * A + a] = sp.winner(a, th[s, a])[1]
+    return th, above, cand.reshape(-1), oracle_mod.solve(fleet, cand)[1]
+
+
+def ref_price_rows(oracle_mod, fleet, rows, trace):
+    """(threshold [L, S, A], above [L*S*A], candidates [L*S*A], winners [L*S], the row fleets): ref_price_fleet on
+    at_row(fleet, rows, l) per level, or with `trace` on ref_trace's fleet of tick t, whose current allocation is
+    c_t (apply_winners of the ticks before)."""
+    out, fleets, cur = [], [], fleet
+    for l in range(n_rows(rows)):
+        f = at_row(cur, rows, l)
+        r = ref_price_fleet(oracle_mod, f)
+        out.append(r)
+        fleets.append(f)
+        if trace:
+            cur = cur.apply_winners(r[3])
+    S, A = fleet.n_servers, fleet.n_acc
+    if not out:
+        empty = np.zeros(0, oracle_mod.ALLOC_DTYPE)
+        return np.zeros((0, S, A), F32), empty, empty, empty, fleets
+    return (np.stack([r[0] for r in out]),) + tuple(np.concatenate([r[k] for r in out]) for k in (1, 2, 3)) + (fleets,)
+
+
+def edge_fleet(seed, keep=False, factor=0.1, n=10, n_acc=4):
+    """mixed_fleet with one type per accelerator, accelerators 1 and 2 identical (ties on value), and current costs
+    0, 1e38 and -MaxFloat32."""
+    f = mixed_fleet(n, n_acc, seed, keep)
+    f.accel_penalty_factor = factor
+    for k in ("perf_alpha", "perf_beta", "perf_gamma", "perf_delta", "perf_acc_count", "perf_max_batch",
+              "perf_at_tokens", "perf_present"):
+        getattr(f, k)[:, 2] = getattr(f, k)[:, 1]
+    f.acc_cost[2] = f.acc_cost[1]
+    f.acc_type[:] = np.arange(n_acc)
+    f.type_capacity = np.full(n_acc, 1000, np.int32)
+    f.acc_multiplicity[:] = np.arange(n_acc) % 3 + 1
+    f.srv_cur_cost[5::5] = 0.0
+    f.srv_cur_cost[6::5] = F32(1e38)
+    f.srv_cur_cost[7::5] = -F32_MAX
+    return f
+
+
+def moving_fleet(seed):
+    """Penalty factor 0 and min_replicas 1: the cheapest accelerator wins, so c_t changes accelerator on the trace."""
+    f = edge_fleet(seed, factor=0.0)
+    f.srv_min_replicas[:] = 1
+    return f
+
+
+PRICE_CALLS = {False: "price_threshold_grid", True: "price_threshold_trace"}
+
+
+def check_price_rows(engine, oracle_mod, fleet, rows, trace, what, ref=None):
+    """Engine.price_threshold_grid / price_threshold_trace against ref_price_rows (or `ref`, its result), bit for
+    bit: (threshold, candidates, winners) of the reference."""
+    th_o, above_o, cand_o, win_o, _ = ref if ref is not None else ref_price_rows(oracle_mod, fleet, rows, trace)
+    th_g, above_g, cand_g, win_g = getattr(engine, PRICE_CALLS[trace])(fleet, **rows, want_candidates=True)
+    assert_f32_bits_equal(th_g.reshape(-1), th_o.reshape(-1), f"{what}: threshold")
+    assert_allocs_equal(above_g, above_o, f"{what}: above")
+    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
+    assert_allocs_equal(win_g, win_o, f"{what}: winners")
+    return th_o, cand_o, win_o
+
+
+# ---- long horizons: nil runs and periodic days ---------------------------------------------------------------
+
+def gap_mask(n_servers, L, gaps, start):
+    """[L, S] bool: server s is in its nil run on ticks [start[s], start[s] + gaps[s]) (gaps[s] 0: none)."""
+    gaps = np.broadcast_to(np.asarray(gaps), (n_servers,))
+    start = np.broadcast_to(np.asarray(start), (n_servers,))
+    t = np.arange(L)[:, None]
+    return (t >= start[None, :]) & (t < (start + gaps)[None, :])
+
+
+def gap_rows(fleet, L, gaps, start, seed):
+    """{"arrival_rpm": [L, S]}: each server's own load (at least 200 req/min) times a seeded log-uniform factor in
+    [0.1, 50] per (tick, server), which spans many replica counts, so that a 32-tick window holds several feasible winners that differ;
+    positive and finite everywhere except that server s is nil (rate -1) on ticks [start[s], start[s] + gaps[s])."""
+    rng = np.random.default_rng(seed)
+    S = fleet.n_servers
+    base = np.maximum(fleet.srv_arrival_rpm, 200.0)
+    rpm = (base[None, :] * np.exp(rng.uniform(np.log(0.1), np.log(50.0), (L, S)))).astype(F32)
+    rpm[gap_mask(S, L, gaps, start)] = -1.0
+    return {"arrival_rpm": rpm}
+
+
+def _tile(x, L):
+    """Rows t = x[t % period] for t < L."""
+    return np.ascontiguousarray(x[np.arange(L) % x.shape[0]])
+
+
+def day_rows(fleet, L, period, seed, special=True):
+    """{"arrival_rpm", "in_tokens", "out_tokens"}, each [L, S], repeating every `period` ticks: a diurnal rate (the
+    server's own load, at least 100 req/min, times a smooth daily factor from e^-2 to e^2 with a per-server phase,
+    times per-server noise) and tokens from
+    a small per-period set of the server's own.  With `special`, a few ticks of the day carry the edge values of
+    load_levels and workload_levels (rates 0, -1, +Inf, tiny and huge; in -1 / 0 / large, out -1 / 0 / 1 / large),
+    so they too repeat daily."""
+    rng = np.random.default_rng(seed)
+    S = fleet.n_servers
+    base = np.maximum(fleet.srv_arrival_rpm, 100.0)
+    t = np.arange(period)[:, None]
+    phase = rng.uniform(0, 2 * np.pi, S)
+    daily = np.exp(2.0 * np.sin(2 * np.pi * t / period + phase[None, :]))
+    rpm = (base[None, :] * daily * rng.lognormal(0.0, 0.15, (period, S))).astype(F32)
+    in_tok = (fleet.srv_in_tokens[None, :] * rng.choice([0.5, 1.0, 1.0, 2.0], (period, S))).astype(np.int32)
+    out_tok = np.maximum(fleet.srv_out_tokens[None, :] * rng.choice([0.75, 1.0, 1.0, 1.5], (period, S)),
+                         1).astype(np.int32)
+    if special:
+        for k, v in enumerate((0.0, -1.0, np.inf, 1e-3, 1e6)):
+            rpm[(7 * k + 3) % period, k::5 + k] = v
+        for k, (col, v) in enumerate((("in", -1), ("out", -1), ("out", 0), ("in", 0), ("in", 100000), ("out", 1),
+                                      ("out", 20000))):
+            (in_tok if col == "in" else out_tok)[(11 * k + 5) % period, k % 3::4 + k] = v
+    return {"arrival_rpm": _tile(rpm, L), "in_tokens": _tile(in_tok, L), "out_tokens": _tile(out_tok, L)}
+
+
+def day_profile_rows(fleet, L, period, seed):
+    """Profile rows over a day that repeats every `period` ticks: acc_cost an hourly price curve per accelerator
+    (own phase and depth), beta x 1.1 on every entry from tick L // 2 on, and the last accelerator withdrawn
+    (perf_present 0) on ticks [period // 4, period // 2) of every day."""
+    rng = np.random.default_rng(seed)
+    A = fleet.n_acc
+    t = np.arange(period)[:, None]
+    phase, depth = rng.uniform(0, 2 * np.pi, A), rng.uniform(0.2, 0.8, A)
+    curve = 1.0 + depth * np.sin(2 * np.pi * t / period + phase) + rng.normal(0, 0.03, (period, A))
+    acc = (fleet.acc_cost[None] * np.maximum(curve, 0.05)).astype(F32)
+    present = np.repeat(fleet.perf_present[None], period, axis=0)
+    present[period // 4:period // 2, :, A - 1] = 0
+    beta = np.repeat(fleet.perf_beta[None], L, axis=0).astype(F32)
+    beta[L // 2:] *= F32(1.1)
+    return {"acc_cost": _tile(acc, L), "perf_present": _tile(present, L), "perf_beta": beta}
+
+
+def day_slo_rows(fleet, L, period):
+    """SLO rows over a day that repeats every `period` ticks: the ITL target x 0.75 in the middle third of the day,
+    the TTFT target x 1.5 in its first quarter, the fleet's own TPS target."""
+    own = {k: np.repeat(getattr(fleet, ROW_COLUMN[k])[None], period, axis=0).astype(F32) for k in SLO}
+    own["slo_itl"][period // 3:2 * period // 3] *= F32(0.75)
+    own["slo_ttft"][:max(period // 4, 1)] *= F32(1.5)
+    return {k: _tile(v, L) for k, v in own.items()}
+
+
+def last_feasible(win, S):
+    """[L, S]: the tick of each server's last feasible winner before tick t, -1 for none (c_t is then the fleet's
+    own current allocation)."""
+    feas = win.reshape(-1, S)["feasible"] != 0
+    out = np.full(feas.shape, -1, np.int64)
+    for t in range(1, feas.shape[0]):
+        out[t] = np.where(feas[t - 1], t - 1, out[t - 1])
+    return out
 
 
 ACC_CM = {  # CreateAcceleratorUnitCostConfigMap, JSON-decoded as readAccFunc does (optimizer_test.go:72-86)

@@ -1,7 +1,7 @@
 """wva_price_threshold_grid / wva_price_threshold_trace: wva_price_thresholds at every level of a grid or tick of a
 trace, in one call.
 
-The expected result is ref_price_rows below: per level the fleet at_row(fleet, rows, l), per tick the fleet of
+The expected result is tests.levels.ref_price_rows: per level the fleet at_row(fleet, rows, l), per tick the fleet of
 ref_trace's chain (current allocation c_t), each through the single-fleet composition of wva_price_thresholds
 (Server.Calculate, a's record re-priced, the one-server Solver.Solve and a bisection over the float32 bit patterns).
 The CPU tests pin that composition to a full Server.Calculate + Solver.Solve at the price, and demand_by_level to
@@ -12,141 +12,14 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.levels import (at_row, from_bits, load_levels, mixed_fleet, n_rows, overflow_fleet, rates_at_rate_star,
-                          transition_penalty, u32_bits, workload_levels)
-from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED,
-                        assert_allocs_equal, assert_f32_bits_equal, error_code, same_bytes)
+from tests.levels import (PRICE_CALLS, PRICE_MAX_BITS, at_price, at_row, check_price_rows, edge_fleet, from_bits,
+                          load_levels, mixed_fleet, moving_fleet, overflow_fleet, pred, rates_at_rate_star,
+                          ref_price_rows, u32_bits, workload_levels)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, error_code,
+                        same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, demand_by_level, synth_fleet
 
 F32 = np.float32
-CALLS = {False: "price_threshold_grid", True: "price_threshold_trace"}
-
-
-# ---- the reference: wva_price_thresholds' composition at each level's or tick's fleet ---------------------------
-
-PRICE_MAX_BITS = 0x7F7FFFFF
-
-
-def pred(x):
-    """The largest float32 below x (x > 0)."""
-    return from_bits(u32_bits(x) - 1)
-
-
-def at_price(fleet, a, p):
-    """A copy of the fleet with acc_cost[a] = p, unlimited."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    f.acc_cost[a] = p
-    f.unlimited = True
-    return f
-
-
-def priced(fleet, s, a, rec, p):
-    """a's record of server s at price p: cost = p * f32(NumInstances * replicas), value = TransitionPenalty against
-    the fleet's current allocation (allocation.go:144-145, :274-275, :291-300); a nil record is unchanged."""
-    r = rec.copy()
-    if not r["feasible"]:
-        return r
-    inst = int(fleet.perf_acc_count[int(fleet.srv_model[s]), a])
-    inst = 1 if inst <= 0 else inst
-    with np.errstate(all="ignore"):
-        r["cost"] = F32(p) * F32(inst * int(r["replicas"]))
-    r["value"] = transition_penalty(F32(fleet.accel_penalty_factor), int(fleet.srv_cur_acc[s]),
-                                    int(fleet.srv_cur_replicas[s]), fleet.srv_cur_cost[s], int(r["acc"]),
-                                    int(r["replicas"]), r["cost"])
-    return r
-
-
-class PriceServer:
-    """One server's winner as a's price moves: Server.Calculate's row with a's record re-priced, decided by the
-    oracle's Solver.Solve on the one-server fleet.  SolveUnlimited reads only feasible and value, so the solve sees
-    each record with its column id in the batch field, which names the winning column."""
-
-    def __init__(self, oracle_mod, fleet, cand, s):
-        self.o, self.fleet, self.row, self.s = oracle_mod, fleet, cand[s], s
-        self.f1 = fleet.take_servers(np.array([s]))
-        self.f1.unlimited = True
-
-    def winner(self, a, p):
-        """(winning column or -1, winner record) with a's record at price p."""
-        row = self.row.copy()
-        row[a] = priced(self.fleet, self.s, a, row[a], p)
-        tagged = row.copy()
-        tagged["batch"] = np.arange(row.size)
-        w = self.o.solve(self.f1, tagged[None])[1][0]
-        if not w["feasible"]:
-            return -1, w
-        return int(w["batch"]), row[int(w["batch"])]
-
-    def wins(self, a, p):
-        return self.winner(a, p)[0] == a
-
-    def threshold(self, a):
-        """The first float32 price in [+0, MaxFloat32] at which a stops winning, by bisecting the bit patterns."""
-        if self.wins(a, from_bits(PRICE_MAX_BITS)):
-            return F32(np.inf)
-        if not self.wins(a, F32(0.0)):
-            return F32(0.0)
-        lo, hi = 0, PRICE_MAX_BITS
-        while hi - lo > 1:
-            mid = (lo + hi) // 2
-            if self.wins(a, from_bits(mid)):
-                lo = mid
-            else:
-                hi = mid
-        return from_bits(hi)
-
-
-def ref_price_fleet(oracle_mod, fleet):
-    """(threshold [S, A], above [S*A], candidates [S*A], winners [S]) of one fleet: wva_price_thresholds' contract
-    composed from the oracle."""
-    cand = oracle_mod.calculate(fleet)
-    S, A = fleet.n_servers, fleet.n_acc
-    th = np.zeros((S, A), F32)
-    above = np.zeros(S * A, oracle_mod.ALLOC_DTYPE)
-    for s in range(S):
-        sp = PriceServer(oracle_mod, fleet, cand, s)
-        for a in range(A):
-            th[s, a] = sp.threshold(a)
-            if np.isfinite(th[s, a]):
-                above[s * A + a] = sp.winner(a, th[s, a])[1]
-    return th, above, cand.reshape(-1), oracle_mod.solve(fleet, cand)[1]
-
-
-def ref_price_rows(oracle_mod, fleet, rows, trace):
-    """(threshold [L, S, A], above [L*S*A], candidates [L*S*A], winners [L*S], the row fleets): ref_price_fleet on
-    at_row(fleet, rows, l) per level, or with `trace` on ref_trace's fleet of tick t, whose current allocation is
-    c_t (apply_winners of the ticks before)."""
-    out, fleets, cur = [], [], fleet
-    for l in range(n_rows(rows)):
-        f = at_row(cur, rows, l)
-        r = ref_price_fleet(oracle_mod, f)
-        out.append(r)
-        fleets.append(f)
-        if trace:
-            cur = cur.apply_winners(r[3])
-    S, A = fleet.n_servers, fleet.n_acc
-    if not out:
-        empty = np.zeros(0, oracle_mod.ALLOC_DTYPE)
-        return np.zeros((0, S, A), F32), empty, empty, empty, fleets
-    return (np.stack([r[0] for r in out]),) + tuple(np.concatenate([r[k] for r in out]) for k in (1, 2, 3)) + (fleets,)
-
-
-def edge_fleet(seed, keep=False, factor=0.1, n=10, n_acc=4):
-    """mixed_fleet with one type per accelerator, accelerators 1 and 2 identical (ties on value), and current costs
-    0, 1e38 and -MaxFloat32."""
-    f = mixed_fleet(n, n_acc, seed, keep)
-    f.accel_penalty_factor = factor
-    for k in ("perf_alpha", "perf_beta", "perf_gamma", "perf_delta", "perf_acc_count", "perf_max_batch",
-              "perf_at_tokens", "perf_present"):
-        getattr(f, k)[:, 2] = getattr(f, k)[:, 1]
-    f.acc_cost[2] = f.acc_cost[1]
-    f.acc_type[:] = np.arange(n_acc)
-    f.type_capacity = np.full(n_acc, 1000, np.int32)
-    f.acc_multiplicity[:] = np.arange(n_acc) % 3 + 1
-    f.srv_cur_cost[5::5] = 0.0
-    f.srv_cur_cost[6::5] = F32(1e38)
-    f.srv_cur_cost[7::5] = -F32_MAX
-    return f
 
 
 def load_rows(fleet, L, seed):
@@ -157,28 +30,11 @@ def token_rows(fleet, L, seed):
     return dict(zip(("arrival_rpm", "in_tokens", "out_tokens"), workload_levels(fleet, L, seed)))
 
 
-def moving_fleet(seed):
-    """Penalty factor 0 and min_replicas 1: the cheapest accelerator wins, so c_t changes accelerator on the trace."""
-    f = edge_fleet(seed, factor=0.0)
-    f.srv_min_replicas[:] = 1
-    return f
-
-
 def _to_allocs(rec):
     out = Allocs(rec.size)
     for k in ALLOC_FIELDS:
         getattr(out, k)[:] = rec[k]
     return out
-
-
-def _check(engine, oracle_mod, fleet, rows, trace, what, ref=None):
-    th_o, above_o, cand_o, win_o, _ = ref if ref is not None else ref_price_rows(oracle_mod, fleet, rows, trace)
-    th_g, above_g, cand_g, win_g = getattr(engine, CALLS[trace])(fleet, **rows, want_candidates=True)
-    assert_f32_bits_equal(th_g.reshape(-1), th_o.reshape(-1), f"{what}: threshold")
-    assert_allocs_equal(above_g, above_o, f"{what}: above")
-    assert_allocs_equal(cand_g, cand_o, f"{what}: candidates")
-    assert_allocs_equal(win_g, win_o, f"{what}: winners")
-    return th_o, cand_o, win_o
 
 
 # ---- CPU: the composition ---------------------------------------------------------------------
@@ -274,14 +130,14 @@ def test_demand_by_level_is_allocate_by_type(oracle_mod, trace):
 def test_mixed_fleet_rows(engine, oracle_mod, rows_of, keep, trace):
     """mixed_fleet with load_levels rows (0, negative, +Inf, tiny and huge rates) or workload_levels rows."""
     fleet = edge_fleet(41 + keep, keep)
-    th, _, _ = _check(engine, oracle_mod, fleet, rows_of(fleet, 5, 17), trace,
+    th, _, _ = check_price_rows(engine, oracle_mod, fleet, rows_of(fleet, 5, 17), trace,
                       f"{rows_of.__name__}, keep = {keep}, trace = {trace}")
     assert ((th > 0) & np.isfinite(th)).sum() >= 3
 
 
 @pytest.mark.gpu
 def test_trace_with_a_moving_current_allocation(engine, oracle_mod):
-    _check(engine, oracle_mod, moving_fleet(43), load_rows(moving_fleet(43), 6, 3), True, "moving c_t")
+    check_price_rows(engine, oracle_mod, moving_fleet(43), load_rows(moving_fleet(43), 6, 3), True, "moving c_t")
 
 
 @pytest.fixture(scope="module")
@@ -299,7 +155,7 @@ def test_rounds_every_tree_depth(engine, oracle_mod, rounds_case, monkeypatch, d
     monkeypatch.setenv("WVA_SIZE_DEPTH", depth)
     fleet, rows, ref = rounds_case
     for trace in (False, True):
-        _check(engine, oracle_mod, fleet, rows, trace, f"rounds, D = {depth}, trace = {trace}", ref[trace])
+        check_price_rows(engine, oracle_mod, fleet, rows, trace, f"rounds, D = {depth}, trace = {trace}", ref[trace])
 
 
 @pytest.mark.gpu
@@ -314,7 +170,7 @@ def test_many_accelerators(engine, oracle_mod, n_acc):
         getattr(fleet, k)[:, n_acc - 1] = getattr(fleet, k)[:, 0]
     rows = load_rows(fleet, 2, 7)
     for trace in (False, True):
-        _check(engine, oracle_mod, fleet, rows, trace, f"A = {n_acc}, trace = {trace}")
+        check_price_rows(engine, oracle_mod, fleet, rows, trace, f"A = {n_acc}, trace = {trace}")
 
 
 @pytest.mark.gpu
@@ -324,7 +180,7 @@ def test_stored_vector_fallback(engine, oracle_mod):
     rates = [rates_at_rate_star(oracle_mod, fleet, s, 0) for s in range(fleet.n_servers)]
     rows = {"arrival_rpm": np.array([[r[k % len(r)] for r in rates] for k in range(3)], F32)}
     for trace in (False, True):
-        _, cand, _ = _check(engine, oracle_mod, fleet, rows, trace, f"stored-vector fallback, trace = {trace}")
+        _, cand, _ = check_price_rows(engine, oracle_mod, fleet, rows, trace, f"stored-vector fallback, trace = {trace}")
         assert cand["feasible"].sum() >= 1
 
 
@@ -336,7 +192,7 @@ def test_nan_and_huge_values_and_ties(engine, oracle_mod):
     fleet.acc_cost[3] = F32_MAX
     fleet.srv_cur_cost[fleet.srv_cur_cost > F32(1e37)] = 0.0  # keep the trace's carried costs finite
     for trace in (False, True):
-        _check(engine, oracle_mod, fleet, load_rows(fleet, 3, 2), trace, f"NaN / huge values, trace = {trace}")
+        check_price_rows(engine, oracle_mod, fleet, load_rows(fleet, 3, 2), trace, f"NaN / huge values, trace = {trace}")
 
 
 @pytest.mark.gpu
@@ -356,9 +212,9 @@ def test_current_allocation_equal_to_a_candidate(engine, oracle_mod, keep):
             fleet.srv_cur_cost[s] = cand[s, a]["cost"]
             same.append((s, a))
     assert len(same) >= 2
-    th, _, _ = _check(engine, oracle_mod, fleet, rows, False, f"same replica count, keep = {keep}")
+    th, _, _ = check_price_rows(engine, oracle_mod, fleet, rows, False, f"same replica count, keep = {keep}")
     assert all(th[0, s, a] == 0 or np.isinf(th[0, s, a]) for s, a in same)
-    _check(engine, oracle_mod, fleet, rows, True, f"same replica count, trace, keep = {keep}")
+    check_price_rows(engine, oracle_mod, fleet, rows, True, f"same replica count, trace, keep = {keep}")
 
 
 @pytest.mark.gpu
@@ -369,7 +225,7 @@ def test_zero_load_min_replicas_zero(engine, oracle_mod):
     rows = load_rows(fleet, 3, 11)
     rows["arrival_rpm"][:, ::2] = 0.0
     for trace in (False, True):
-        _, cand, _ = _check(engine, oracle_mod, fleet, rows, trace, f"zero load, trace = {trace}")
+        _, cand, _ = check_price_rows(engine, oracle_mod, fleet, rows, trace, f"zero load, trace = {trace}")
         assert ((cand["acc"] == -1) & (cand["feasible"] == 1)).sum() >= 2
 
 
@@ -400,7 +256,7 @@ def test_every_block_is_the_single_call(engine, big_case, trace):
     the winners equal wva_workload_grid's (wva_workload_trace's)."""
     fleet, rows = big_case
     S, A = fleet.n_servers, fleet.n_acc
-    th, above, cand, win = getattr(engine, CALLS[trace])(fleet, **rows, want_candidates=True)
+    th, above, cand, win = getattr(engine, PRICE_CALLS[trace])(fleet, **rows, want_candidates=True)
     _, w_ref = (engine.workload_trace if trace else engine.workload_grid)(fleet, **rows)
     for k in ALLOC_FIELDS:
         assert same_bytes(getattr(win, k), getattr(w_ref, k)), k
@@ -424,7 +280,7 @@ def test_profile_grid_at_each_threshold(engine, big_case, trace):
     the threshold, and above is the winner there."""
     fleet, rows = big_case
     S, A = fleet.n_servers, fleet.n_acc
-    th, above, _, win = getattr(engine, CALLS[trace])(fleet, **rows)
+    th, above, _, win = getattr(engine, PRICE_CALLS[trace])(fleet, **rows)
     cur, pairs = fleet, 0
     for l in range(th.shape[0]):
         f = at_row(cur, rows, l)
@@ -458,7 +314,7 @@ def test_profile_grid_at_each_threshold(engine, big_case, trace):
 # ---- GPU: refusals and bookkeeping ----------------------------------------------------------------
 
 def _call(engine, trace, fleet, rows):
-    return error_code(lambda: getattr(engine, CALLS[trace])(fleet, **rows))
+    return error_code(lambda: getattr(engine, PRICE_CALLS[trace])(fleet, **rows))
 
 
 @pytest.mark.gpu
@@ -523,7 +379,7 @@ def test_trace_refuses_a_carried_infinite_cost(engine):
 def test_argument_errors_and_empty_calls(engine, trace):
     fleet = mixed_fleet(6, 2, 79, False)
     S, A, L = fleet.n_servers, fleet.n_acc, 2
-    fn = getattr(engine._L, "wva_" + CALLS[trace])
+    fn = getattr(engine._L, "wva_" + PRICE_CALLS[trace])
     h, fc = engine._h, fleet.as_c()
     rpm = np.repeat(fleet.srv_arrival_rpm[None], L, axis=0).astype(F32)
     th = np.zeros(L * S * A, F32)
@@ -538,18 +394,18 @@ def test_argument_errors_and_empty_calls(engine, trace):
     assert fn(h, None, L, p(rpm), None, None, p(th), None, None, C.byref(win.as_c())) == WVA_ERR_BAD_ARG
     # NULL token lists, above and candidates: the thresholds alone, the fleet's own tokens
     assert fn(h, *args(L, p(rpm), p(th), C.byref(win.as_c()))) == 0
-    ref = getattr(engine, CALLS[trace])(fleet, rpm, fleet.srv_in_tokens[None].repeat(L, 0),
+    ref = getattr(engine, PRICE_CALLS[trace])(fleet, rpm, fleet.srv_in_tokens[None].repeat(L, 0),
                                         fleet.srv_out_tokens[None].repeat(L, 0))
     assert same_bytes(th, ref[0].reshape(-1))
     for k in ALLOC_FIELDS:
         assert same_bytes(getattr(win, k), getattr(ref[3], k)), k
-    th0, above0, cand0, win0 = getattr(engine, CALLS[trace])(fleet, rpm[:0], want_candidates=True)
+    th0, above0, cand0, win0 = getattr(engine, PRICE_CALLS[trace])(fleet, rpm[:0], want_candidates=True)
     assert th0.shape == (0, S, A) and above0.n == cand0.n == win0.n == 0
     empty = fleet.take_servers(np.arange(0))
-    th0, above0, _, win0 = getattr(engine, CALLS[trace])(empty, np.zeros((3, 0), F32))
+    th0, above0, _, win0 = getattr(engine, PRICE_CALLS[trace])(empty, np.zeros((3, 0), F32))
     assert th0.shape == (3, 0, A) and above0.n == win0.n == 0
     with pytest.raises(ValueError):
-        getattr(engine, CALLS[trace])(fleet, None)
+        getattr(engine, PRICE_CALLS[trace])(fleet, None)
 
 
 @pytest.mark.gpu
@@ -564,10 +420,10 @@ def test_launch_count_does_not_depend_on_the_rows(engine, trace):
         call()
         return engine.launch_count - n0
     extra = set()
-    for L in (1, 4, 16):
+    for L in (1, 4, 16, 65, 1440):
         rows = load_rows(fleet, L, 3)
         rows["arrival_rpm"] = np.abs(rows["arrival_rpm"]).clip(1, 1e4)
-        extra.add(launches(lambda: getattr(engine, CALLS[trace])(fleet, **rows)) -
+        extra.add(launches(lambda: getattr(engine, PRICE_CALLS[trace])(fleet, **rows)) -
                   launches(lambda: workload(fleet, **rows)))
     assert extra == {1}
 

@@ -12,124 +12,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.levels import _adversarial_fleet, mixed_fleet, overflow_fleet, rates_at_rate_star, transition_penalty
-from tests.util import ALLOC_FIELDS, assert_allocs_equal, assert_f32_bits_equal, error_code, same_bytes
+from tests.levels import (PRICE_MAX_BITS, PriceServer, _adversarial_fleet, at_price, edge_fleet, from_bits, mixed_fleet,
+                          overflow_fleet, pred, priced, rates_at_rate_star, ref_price_fleet, u32_bits)
+from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
+                        assert_f32_bits_equal, error_code, same_bytes)
 from workload_variant_autoscaler_b200 import Allocs, Engine, WvaError, accelerator_demand, synth_fleet
 
 F32 = np.float32
-F32_MAX = F32(np.finfo(np.float32).max)
-MAX_BITS = 0x7F7FFFFF
-WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED = -1, -5, -6
-
-
-def _f(bits):
-    return np.array([bits], np.uint32).view(F32)[0]
-
-
-def _bits(x):
-    return int(np.array([x], F32).view(np.uint32)[0])
-
-
-def pred(x):
-    """The largest float32 below x (x > 0)."""
-    return _f(_bits(x) - 1)
-
-
-def at_price(fleet, a, p):
-    """f(p): a copy of the fleet with acc_cost[a] = p, unlimited."""
-    f = fleet.take_servers(np.arange(fleet.n_servers))
-    f.acc_cost[a] = p
-    f.unlimited = True
-    return f
-
-
-def priced(fleet, s, a, rec, p):
-    """a's record of server s at price p: cost = p * f32(NumInstances * replicas), value = TransitionPenalty
-    (allocation.go:144-145, :274-275, :291-300); every other field and a nil record are unchanged."""
-    r = rec.copy()
-    if not r["feasible"]:
-        return r
-    inst = int(fleet.perf_acc_count[int(fleet.srv_model[s]), a])
-    inst = 1 if inst <= 0 else inst
-    with np.errstate(all="ignore"):
-        r["cost"] = F32(p) * F32(inst * int(r["replicas"]))
-    r["value"] = transition_penalty(F32(fleet.accel_penalty_factor), int(fleet.srv_cur_acc[s]),
-                                    int(fleet.srv_cur_replicas[s]), fleet.srv_cur_cost[s], int(r["acc"]),
-                                    int(r["replicas"]), r["cost"])
-    return r
-
-
-class ServerPrices:
-    """The winner of one server as a's price moves, from the oracle's Solver.Solve on the one-server fleet.
-    SolveUnlimited reads only feasible and value, so the solve sees each record with its column id in the batch
-    field, which names the winning column."""
-
-    def __init__(self, oracle_mod, fleet, cand, s):
-        self.o, self.fleet, self.row, self.s = oracle_mod, fleet, cand[s], s
-        self.f1 = fleet.take_servers(np.array([s]))
-        self.f1.unlimited = True
-
-    def winner(self, a, p):
-        """(winning column or -1, winner record) with a's record at price p."""
-        row = self.row.copy()
-        row[a] = priced(self.fleet, self.s, a, row[a], p)
-        tagged = row.copy()
-        tagged["batch"] = np.arange(row.size)
-        w = self.o.solve(self.f1, tagged[None])[1][0]
-        if not w["feasible"]:
-            return -1, w
-        return int(w["batch"]), row[int(w["batch"])]
-
-    def wins(self, a, p):
-        return self.winner(a, p)[0] == a
-
-    def threshold(self, a):
-        if self.wins(a, _f(MAX_BITS)):
-            return F32(np.inf)
-        if not self.wins(a, F32(0.0)):
-            return F32(0.0)
-        lo, hi = 0, MAX_BITS
-        while hi - lo > 1:
-            mid = (lo + hi) // 2
-            if self.wins(a, _f(mid)):
-                lo = mid
-            else:
-                hi = mid
-        return _f(hi)
-
-
-def ref_price_thresholds(oracle_mod, fleet):
-    """(threshold [S, A], above [S*A], candidates [S*A]) composed from the oracle."""
-    cand = oracle_mod.calculate(fleet)
-    S, A = fleet.n_servers, fleet.n_acc
-    th = np.zeros((S, A), F32)
-    above = np.zeros(S * A, oracle_mod.ALLOC_DTYPE)
-    for s in range(S):
-        sp = ServerPrices(oracle_mod, fleet, cand, s)
-        for a in range(A):
-            th[s, a] = sp.threshold(a)
-            if np.isfinite(th[s, a]):
-                above[s * A + a] = sp.winner(a, th[s, a])[1]
-    return th, above, cand.reshape(-1)
-
-
-def edge_fleet(seed, keep=False, factor=0.1):
-    """mixed_fleet with per-accelerator types and multiplicities, accelerators 1 and 2 identical (ties on value),
-    current costs 0, huge and -MaxFloat32 (values that round to MaxFloat32 or overflow), and an unknown current
-    accelerator."""
-    f = mixed_fleet(14, 4, seed, keep)
-    f.accel_penalty_factor = factor
-    for k in ("perf_alpha", "perf_beta", "perf_gamma", "perf_delta", "perf_acc_count", "perf_max_batch",
-              "perf_at_tokens", "perf_present"):
-        getattr(f, k)[:, 2] = getattr(f, k)[:, 1]
-    f.acc_cost[2] = f.acc_cost[1]
-    f.acc_type[:] = np.arange(4)
-    f.type_capacity = np.full(4, 1000, np.int32)
-    f.acc_multiplicity[:] = [1, 2, 1, 3]
-    f.srv_cur_cost[5::5] = 0.0
-    f.srv_cur_cost[6::5] = F32(1e38)
-    f.srv_cur_cost[7::5] = -F32_MAX
-    return f
 
 
 # ---- CPU: the composition ---------------------------------------------------------------------
@@ -137,8 +26,8 @@ def edge_fleet(seed, keep=False, factor=0.1):
 def _prices(th, rng, n):
     """Each finite positive threshold and the float below it, 0, MaxFloat32 and n random bit patterns."""
     t = th[np.isfinite(th) & (th > 0)]
-    ps = [F32(0.0), _f(MAX_BITS)] + [x for v in np.unique(t) for x in (v, pred(v))]
-    ps += [_f(int(b)) for b in rng.integers(0, MAX_BITS + 1, n)]
+    ps = [F32(0.0), from_bits(PRICE_MAX_BITS)] + [x for v in np.unique(t) for x in (v, pred(v))]
+    ps += [from_bits(int(b)) for b in rng.integers(0, PRICE_MAX_BITS + 1, n)]
     return ps
 
 
@@ -146,8 +35,8 @@ def _prices(th, rng, n):
 def test_repriced_table_is_calculate_at_the_price(oracle_mod, seed, factor):
     """CreateAllocation reads acc_cost[a] only in the cost of a's records: at each threshold, the float below it and
     random prices, re-pricing column a of the fleet's table gives Server.Calculate on f(p) bit for bit."""
-    fleet = edge_fleet(seed, factor=factor)
-    th, _, cand = ref_price_thresholds(oracle_mod, fleet)
+    fleet = edge_fleet(seed, factor=factor, n=14)
+    th, _, cand = ref_price_fleet(oracle_mod, fleet)[:3]
     cand = cand.reshape(fleet.n_servers, fleet.n_acc)
     rng = np.random.default_rng(seed)
     checked = 0
@@ -167,13 +56,13 @@ def test_a_wins_exactly_below_the_threshold(oracle_mod, keep, factor):
     """The monotonicity claim, checked on the predicate itself: at dense prices (every threshold and the float
     below it, random bit patterns, 0 and MaxFloat32) a wins iff p < threshold, with ties between accelerators,
     penalty factor 0, NaN and MaxFloat32 values, and current costs 0 and huge."""
-    fleet = edge_fleet(11, keep, factor)
-    th, _, cand = ref_price_thresholds(oracle_mod, fleet)
+    fleet = edge_fleet(11, keep, factor, n=14)
+    th, _, cand = ref_price_fleet(oracle_mod, fleet)[:3]
     cand = cand.reshape(fleet.n_servers, fleet.n_acc)
     rng = np.random.default_rng(7)
     kinds = set()
     for s in range(fleet.n_servers):
-        sp = ServerPrices(oracle_mod, fleet, cand, s)
+        sp = PriceServer(oracle_mod, fleet, cand, s)
         for a in range(fleet.n_acc):
             t = th[s, a]
             kinds.add("0" if t == 0 else "inf" if np.isinf(t) else "finite")
@@ -186,8 +75,8 @@ def test_a_wins_exactly_below_the_threshold(oracle_mod, keep, factor):
 def test_accelerator_demand_is_allocate_by_type(oracle_mod):
     """accelerator_demand equals AllocateByType's count of a's type (one accelerator per type) over the oracle's
     winners on f(p), at each stretch's start and one ulp below each breakpoint."""
-    fleet = edge_fleet(5)
-    th, _, cand_o = ref_price_thresholds(oracle_mod, fleet)
+    fleet = edge_fleet(5, n=14)
+    th, _, cand_o = ref_price_fleet(oracle_mod, fleet)[:3]
     cand = Allocs(cand_o.size)
     for k in ALLOC_FIELDS:
         getattr(cand, k)[:] = cand_o[k]
@@ -211,7 +100,7 @@ def test_accelerator_demand_is_allocate_by_type(oracle_mod):
 # ---- GPU: bit for bit against the composition ---------------------------------------------------
 
 def _check(engine, oracle_mod, fleet, what):
-    th_o, above_o, cand_o = ref_price_thresholds(oracle_mod, fleet)
+    th_o, above_o, cand_o = ref_price_fleet(oracle_mod, fleet)[:3]
     th_g, above_g, cand_g = engine.price_thresholds(fleet, want_candidates=True)
     assert_f32_bits_equal(th_g.reshape(-1), th_o.reshape(-1), f"{what}: threshold")
     assert_allocs_equal(above_g, above_o, f"{what}: above")
@@ -222,7 +111,7 @@ def _check(engine, oracle_mod, fleet, what):
 @pytest.mark.gpu
 @pytest.mark.parametrize("keep", [False, True])
 def test_small_fleet_warp_path(engine, oracle_mod, keep):
-    th, _, _ = _check(engine, oracle_mod, edge_fleet(31, keep), f"warp path, keep = {keep}")
+    th, _, _ = _check(engine, oracle_mod, edge_fleet(31, keep, n=14), f"warp path, keep = {keep}")
     assert ((th > 0) & np.isfinite(th)).sum() >= 3
 
 
@@ -230,7 +119,7 @@ def test_small_fleet_warp_path(engine, oracle_mod, keep):
 def rounds_case(oracle_mod):
     fleet = mixed_fleet(60, 4, 37, False)
     fleet.srv_keep_acc[::2] = 1
-    return fleet, ref_price_thresholds(oracle_mod, fleet)
+    return fleet, ref_price_fleet(oracle_mod, fleet)[:3]
 
 
 @pytest.mark.gpu
@@ -250,7 +139,7 @@ def test_rounds_every_tree_depth(engine, rounds_case, monkeypatch, depth):
 def test_current_allocation_with_the_same_replica_count(engine, oracle_mod, keep):
     """Servers whose current allocation is a's candidate itself (same accelerator and replica count): the value
     is 0 at every price, so the threshold is 0 or +Inf."""
-    fleet = edge_fleet(13, keep)
+    fleet = edge_fleet(13, keep, n=14)
     cand = oracle_mod.calculate(fleet)
     same = []
     for s in range(fleet.n_servers):
@@ -268,7 +157,7 @@ def test_current_allocation_with_the_same_replica_count(engine, oracle_mod, keep
 @pytest.mark.gpu
 def test_zero_load_min_replicas_zero(engine, oracle_mod):
     """Zero-load servers with min_replicas 0 (the accelerator-"" record, cost 0 at every price) and 1."""
-    fleet = edge_fleet(17)
+    fleet = edge_fleet(17, n=14)
     fleet.srv_arrival_rpm[::2] = 0.0
     fleet.srv_min_replicas[::4] = 0
     fleet.srv_min_replicas[2::4] = 1
@@ -301,7 +190,7 @@ def test_stored_vector_fallback(engine, oracle_mod):
 @pytest.mark.gpu
 def test_nan_and_huge_values_and_ties(engine, oracle_mod):
     """Values that are NaN (an overflowed cost under factor 0) or MaxFloat32, huge prices, and ties on value."""
-    fleet = edge_fleet(19, factor=0.0)
+    fleet = edge_fleet(19, factor=0.0, n=14)
     fleet.acc_cost[0] = F32(1e38)
     fleet.acc_cost[3] = F32_MAX
     th, _, cand = _check(engine, oracle_mod, fleet, "NaN / huge values and ties")
@@ -350,7 +239,7 @@ def test_profile_grid_at_every_threshold(engine):
     for a in range(A):
         for t in np.unique(th[:, a][(th[:, a] > 0) & np.isfinite(th[:, a])]):
             for p in (t, pred(t)):
-                index[(a, _bits(p))] = len(rows)
+                index[(a, u32_bits(p))] = len(rows)
                 r = fleet.acc_cost.copy()
                 r[a] = p
                 rows.append(r)
@@ -362,7 +251,7 @@ def test_profile_grid_at_every_threshold(engine):
             t = th[s, a]
             if not (t > 0 and np.isfinite(t)):
                 continue
-            at, below = index[(a, _bits(t))] * S + s, index[(a, _bits(pred(t)))] * S + s
+            at, below = index[(a, u32_bits(t))] * S + s, index[(a, u32_bits(pred(t)))] * S + s
             assert win.feasible[below] == 1 and win.acc[below] == a, (s, a)
             assert not (win.feasible[at] == 1 and win.acc[at] == a), (s, a)
             for k in ALLOC_FIELDS:

@@ -307,12 +307,15 @@ def test_one_tick_is_the_slo_grid(engine, monkeypatch, rounds):
         _same_allocs(got[1], want[1], f"tick {t}: winners")
 
 
+CONTINUATION_L = {1: 7, 3: 7, 5: 7, 32: 70, 33: 70, 65: 100}  # the trace length per split tick k
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("k", [1, 3, 5])
+@pytest.mark.parametrize("k", [1, 3, 5, 32, 33, 65])
 def test_continuation(engine, k):
     fleet = low_penalty_fleet(30, 3, 103, True)
     fleet.srv_min_replicas[::2] = 0
-    L, S = 7, fleet.n_servers
+    L, S = CONTINUATION_L[k], fleet.n_servers
     rows = [np.array(r) for r in slo_trace_rows(fleet, L, 37)]
     rows[0][2, ::3] = 0.0
     cand, win = _call(engine, fleet, rows, want_candidates=True)

@@ -291,13 +291,16 @@ def test_each_tick_is_solve_on_the_advanced_fleet(engine):
             assert same_bytes(getattr(got, k), getattr(want, k)), k
 
 
+CONTINUATION_L = {1: 7, 3: 7, 5: 7, 32: 70, 33: 70, 65: 100}  # the trace length per split tick k
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("k", [1, 3, 5])
+@pytest.mark.parametrize("k", [1, 3, 5, 32, 33, 65])
 def test_continuation(engine, k):
     """The trace over [0, L) is the trace over [0, k) followed by the trace over [k, L) from c_k."""
     fleet = low_penalty_fleet(30, 3, 103, True)
     fleet.srv_min_replicas[::2] = 0
-    L = 7
+    L = CONTINUATION_L[k]
     rows = workload_levels(fleet, L, 37)
     rows[0][2, ::3] = 0.0
     S = fleet.n_servers
