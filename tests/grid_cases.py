@@ -867,3 +867,158 @@ def bounds_cases():
                 en.append(N)
     edge = _fleet(ea, 0.0, np.full(len(ea), 600.0), en, ratio=SIZE_RATIO)
     return [main, edge]
+
+
+# the solves a level call's tail runs, with their profiles (test_gpu_tail_windows, test_gpu_margin_edges)
+class _Solves:
+    """(rates, K, lambda, candidate) of every streaming solve a tail runs, profiled in one vectorised pass."""
+
+    def __init__(self):
+        self.sr, self.K, self.lam, self.cand = [], [], [], []
+
+    def add(self, qa, lam, cand):
+        self.sr.append(qa.serv_rate())
+        self.K.append(qa.K)
+        self.lam.append(f32(lam))
+        self.cand.append(cand)
+
+    def profile(self):
+        P = chain_profile(self.sr, np.array(self.K), np.array(self.lam, np.float32))
+        P["lam"] = np.array(self.lam, np.float32)
+        P["sr0"] = np.array([r[0] for r in self.sr], np.float32)
+        P["srN"] = np.array([r[-1] for r in self.sr], np.float32)
+        P["K"] = np.array(self.K)
+        P["cand"] = list(self.cand)
+        return P
+
+
+def _final_lam(rpm, tps, out_tok, replicas):
+    """The final Analyze's lambda: totalRate / replicas in req/s, over 1000 (allocation.go:134-153)."""
+    total = f32(f32(tps) / f32(out_tok)) if tps > 0 else f32(f32(rpm) / f32(60))
+    return _lam_of_rate(f32(total / f32(replicas)))
+
+
+def _bails(P):
+    """The solves that leave the streaming windows: a rate or lambda outside [2^-60, 2^60), p at 2^880 or above, the
+    sum at 2^900 or above, or a float64 overflow."""
+    def inside(v):
+        return (v >= f32(2.0 ** -60)) & (v < f32(P60))
+    return P["over"] | (P["emax"] >= 880) | (P["esum"] >= 900) | ~inside(P["lam"]) | ~inside(P["sr0"]) | \
+        ~inside(P["srN"])
+
+
+def tail_bands(P):
+    b = wide_bands(P, steep=False)
+    for k, v in _rate_bands(P).items():
+        b[k] = (int(v),) * 2
+    return b
+
+
+# ---- the load margins' records at the exponent windows (test_gpu_margin_edges) -------------------------------------
+BELOW_NS = list(range(465, 482)) + list(range(608, 633)) + list(range(700, 741, 2))  # lambda ~ rateStar
+ABOVE_NS = list(range(934, 966)) + list(range(1208, 1290)) + list(range(1380, 1481, 5))  # ~ rateStar / 2
+MARGIN_DELTAS = (1e-5, 3e-5, 5e-5)
+ABOVE_DELTAS = (1e-5, 2e-5, 3e-5, 4e-5, 5e-5, 6e-5)  # E(sum) 900 is narrow at rateStar / 2
+
+
+def _rate_star(fleet, s):
+    """rateStar (req/s) of server s's only pair: Size's throughput without a target."""
+    err, _, met, _ = _qa(*_model(fleet, s)).size(0.0, 0.0, 0.0)
+    assert err == 0
+    return f32(met["throughput"])
+
+
+def _step_rows(fleet, rows):
+    """(rate, lo, hi) [L, S] from rows of (r, lo, hi) multiples of each server's first replica step 60 rateStar."""
+    step = np.array([60.0 * float(_rate_star(fleet, s)) for s in range(fleet.n_servers)])
+    m = np.asarray(rows, np.float64)
+    return tuple((m[:, k:k + 1] * step[None, :]).astype(np.float32) for k in range(3))
+
+
+def _grid_fleet(ns, deltas=MARGIN_DELTAS):
+    rows = [(N, d) for N in ns for d in deltas]
+    return _fleet(1.0, 0.0, np.ones(len(rows)), [r[0] for r in rows], delta=[r[1] for r in rows], ratio=SIZE_RATIO)
+
+
+def margin_cases():
+    """(name, fleet, rate, lo, hi) of wva_load_margins whose records' solves sit at the exponent windows.
+
+    at: the load grid's main rows (load_cases), every other level with a one-point window and the others with a
+        window of +-1 % holding no step; the edge fleet's rows with +-0.1 % windows.
+    below: BELOW_NS x MARGIN_DELTAS at 1.5 steps (window [0.5, 1.5] steps: below is one replica at the float under
+        the step, lambda just under rateStar) and at 99.5 steps (window [98.5, 100.5]: all three records within 1 %
+        of rateStar).
+    above: ABOVE_NS x ABOVE_DELTAS at half a step (window [0.5, 1.5] steps: above is two replicas at the step,
+        lambda just over rateStar / 2).
+    edge steps: the edge fleet at 1.5, 2.5 and 3.5 steps with windows down to the step below, and at 0.5, 1.5 and
+        2.5 steps with windows up to the step above."""
+    (main, rpm), _, (edge, erpm) = load_cases()
+    lo, hi = rpm.copy(), rpm.copy()
+    lo[1::2] = (rpm[1::2] * f32(0.99)).astype(np.float32)
+    hi[1::2] = (rpm[1::2] * f32(1.01)).astype(np.float32)
+    out = [("at main", main, rpm, lo, hi),
+           ("at edge", edge, erpm, (erpm * f32(0.999)).astype(np.float32), (erpm * f32(1.001)).astype(np.float32))]
+    fb = _grid_fleet(BELOW_NS)
+    out.append(("below", fb) + _step_rows(fb, [(1.5, 0.5, 1.5), (99.5, 98.5, 100.5)]))
+    fa = _grid_fleet(ABOVE_NS, ABOVE_DELTAS)
+    out.append(("above", fa) + _step_rows(fa, [(0.5, 0.5, 1.5)]))
+    out.append(("edge steps", edge) + _step_rows(edge, [(k + 1.5, k + 0.5, k + 1.5) for k in range(3)] +
+                                                  [(k + 0.5, k + 0.5, k + 1.5) for k in range(3)]))
+    return out
+
+
+# ---- the bisection brackets of iv_advance and mg_start (test_gpu_margin_edges) -------------------------------------
+BRACKET_RATIO = 1000  # K = 16000 at N = 16: the blocking at lambda_max is below float32's ulp, so rateStar = RateRange.Max
+F32_MAX_BITS = 0x7F7FFFFF
+
+
+def _alpha_for_rate_max(rmax):
+    """A float32 alpha (N = 16, delta 0) whose RateRange.Max is near rmax (req/s)."""
+    return float(f32(16 * 0.999 * 1000 / rmax))
+
+
+def bracket_fleet():
+    """N = 16, queue ratio 1000, one server per model: 0 and 2 with alpha 1 (rateStar = RateRange.Max ~ 16,000
+    req/s), 1 with RateRange.Max ~ 3.2e29 req/s, so that counts past 2^24 lie just below float32's maximum and the
+    bisections' estimates reach 3e38.  Server 2 has min_replicas 3."""
+    f = _fleet([1.0, _alpha_for_rate_max(3.2e29), 1.0], 0.0, np.ones(3), 16, ratio=BRACKET_RATIO)
+    f.srv_min_replicas[2] = 3
+    return f
+
+
+def _gate_points(fleet, s, start, gate, k):
+    """The first k float32 rates at or above start whose pair state has the given gate (levels.pair_state)."""
+    from tests.levels import from_bits, pair_state, u32_bits
+    rs = _rate_star(fleet, s)
+    rmax = f32(_qa(*_model(fleet, s)).rate_range()[1])
+    out, b = [], u32_bits(f32(start))
+    while len(out) < k and b <= F32_MAX_BITS:
+        if pair_state(fleet, s, rs, rmax, from_bits(b))[1] == gate:
+            out.append(b)
+        b += 1
+    assert len(out) == k, (s, gate)
+    return out
+
+
+def bracket_cases():
+    """(fleet, rate, lo, hi) [4, 3] on bracket_fleet.  Servers 0 and 1: two rates of the gate-2 states past 2^24
+    replicas (float32(total / float32(nrep)) rounds above RateRange.Max), a gate-1 rate among them, each with a
+    window of +-100 floats, and one replica at half a step.  Server 2 (min_replicas 3): windows from the smallest
+    positive rate, at 1.5 and 2.5 steps, and one from a quarter step."""
+    from tests.levels import TINY, from_bits
+    fleet = bracket_fleet()
+    L, S = 4, fleet.n_servers
+    rate, lo, hi = (np.zeros((L, S), np.float32) for _ in range(3))
+    for s in (0, 1):
+        step = 60.0 * float(_rate_star(fleet, s))
+        first = step * (2 ** 24 + 1)
+        g2 = _gate_points(fleet, s, first, 2, 2)
+        g1 = [b + 10 for b in _gate_points(fleet, s, first, 1, 1)]
+        for l, b in enumerate(g2 + g1):
+            rate[l, s], lo[l, s], hi[l, s] = from_bits(b), from_bits(b - 100), from_bits(b + 100)
+        rate[3, s], lo[3, s], hi[3, s] = f32(0.5 * step), f32(0.25 * step), f32(0.75 * step)
+    step = 60.0 * float(_rate_star(fleet, 2))
+    for l, (r, b, t) in enumerate(((1.5, None, 1.5), (2.5, None, 3.5), (0.5, 0.25, 0.5), (0.5, 0.25, 0.5))):
+        rate[l, 2], hi[l, 2] = f32(r * step), f32(t * step)
+        lo[l, 2] = TINY if b is None else f32(b * step)
+    return fleet, rate, lo, hi

@@ -13,7 +13,7 @@ import pytest
 
 from tests.util import (ACC_NONE, ACC_UNKNOWN, ALLOC_FIELDS, F32_MAX, assert_allocs_equal, assert_f32_bits_equal,
                         same_bytes)
-from workload_variant_autoscaler_b200 import synth_fleet
+from workload_variant_autoscaler_b200 import MARGIN_HI_OPEN, MARGIN_LO_OPEN, MARGIN_TRUNCATED, synth_fleet
 from workload_variant_autoscaler_b200._abi import SAT_NONE
 
 F32 = np.float32
@@ -466,6 +466,60 @@ def next_step(fleet, s, rate_star, rmax, x, hi):
     return from_bits(hi_b)
 
 
+def _est_bits(est):
+    """__double2float_rn(est) as float32 bits (+Inf above the range)."""
+    with np.errstate(over="ignore"):
+        return u32_bits(F32(est))
+
+
+def iv_branch(fleet, s, rate_star, rmax, x, hi):
+    """Which search iv_advance runs for a load pair at x in a window topped by hi (wva_size.cuh): None when it does
+    not search (over, or hi <= x), "bracket" when the +-64-ulp bracket around its estimate holds the step, "whole"
+    when it falls back to (x, hi] and a step lies there, "none" when it falls back and finds none.  Returns
+    (gate at x, branch)."""
+    at = pair_state(fleet, s, rate_star, rmax, x)
+    nrep, gate, over = at
+    lo_b, hi_b = u32_bits(x), u32_bits(hi)
+    if over or hi_b <= lo_b:
+        return gate, None
+
+    def differs(b):
+        return pair_state(fleet, s, rate_star, rmax, from_bits(b)) != at
+    if nrep >= 1:
+        est = 60.0 * float(nrep) * float(rate_star)
+        if gate == 1:
+            est = min(est, 60.0 * float(nrep) * float(rmax))
+        e = _est_bits(est)
+        bl = e - 64 if e > lo_b and e - lo_b > 64 else lo_b
+        bh = e + 64 if e < hi_b and hi_b - e > 64 else hi_b
+        if gate != 0 and est < 3.0e38 and bl < bh and (bl == lo_b or not differs(bl)) and differs(bh):
+            return gate, "bracket"
+    return gate, ("whole" if differs(hi_b) else "none")
+
+
+def mg_branch(fleet, s, rate_star, rmax, x, bottom):
+    """Which search mg_start runs for a load pair at x above the window's smallest positive rate bottom: None when
+    the state at x holds down to bottom, else "bracket" or "whole" as iv_branch.  Returns (gate at x, branch)."""
+    at = pair_state(fleet, s, rate_star, rmax, x)
+    nrep, gate, _ = at
+    lo_b, hi_b = u32_bits(bottom), u32_bits(x)
+
+    def same(b):
+        return pair_state(fleet, s, rate_star, rmax, from_bits(b)) == at
+    if hi_b <= lo_b or same(lo_b):
+        return gate, None
+    if nrep >= 1 and gate != 0:
+        est = 60.0 * float(nrep - 1) * float(rate_star)
+        if gate == 2:
+            est = max(est, 60.0 * float(nrep) * float(rmax))
+        e = _est_bits(est)
+        bl = e - 64 if e > lo_b and e - lo_b > 64 else lo_b
+        bh = e + 64 if e < hi_b and hi_b - e > 64 else hi_b
+        if est < 3.0e38 and bl < bh and (bl == lo_b or not same(bl)) and (bh == hi_b or same(bh)):
+            return gate, "bracket"
+    return gate, "whole"
+
+
 def server_steps(oracle_mod, fleet, s, lo, hi):
     """(the points to evaluate in [lo, hi], the first rate at which a pair overflows or None)."""
     pts = {F32(lo)}
@@ -544,6 +598,86 @@ def check_intervals(engine, oracle_mod, fleet, lo, hi, M, what):
     assert same_bytes(start, start_o), f"{what}: start_rpm"
     assert_allocs_equal(rec, rec_o, f"{what}: records")
     return count_o, trunc_o
+
+
+# ---- the load margins' composition ---------------------------------------------------------------
+
+M_ALL = 4096  # intervals per server in the margins' composition: more than any window of the tests holds
+
+
+def below(x):
+    """nextafter(x, 0) in float32."""
+    return np.nextafter(F32(x), F32(0))
+
+
+def ref_margins(oracle_mod, fleet, rate, lo, hi):
+    """(lo (L, S), hi (L, S), flags (L, S), at, below, above as structured arrays of L * S records).
+
+    ref_intervals over each level's window (with M large enough never to truncate at M) lists the intervals; the
+    margin is the one that holds the level's rate r, the next start is hi, and the records are the oracle's winners
+    (winners_at) at r, one float32 below lo and at hi.  A replica overflow (server_steps) ends the stretch as it ends
+    the interval list."""
+    L, S = rate.shape
+    lo_e, hi_e = np.zeros((L, S), np.float32), np.zeros((L, S), np.float32)
+    flags = np.zeros((L, S), np.uint8)
+    recs = {k: np.zeros(L * S, oracle_mod.ALLOC_DTYPE) for k in ("at", "below", "above")}
+    points = [[] for _ in range(S)]  # (record kind, index, rate) per server, over all levels
+    for l in range(L):
+        count, trunc, start, rec, _ = ref_intervals(oracle_mod, fleet, lo[l], hi[l], M_ALL)
+        assert not (count == M_ALL).any()
+        for s in range(S):
+            i, r = l * S + s, F32(rate[l, s])
+            over_at = server_steps(oracle_mod, fleet, s, lo[l, s], hi[l, s])[1] if trunc[s] else None
+            points[s].append(("at", i, r))
+            if over_at is not None and over_at <= r:
+                flags[l, s] = MARGIN_TRUNCATED
+                lo_e[l, s] = hi_e[l, s] = r
+                continue
+            n = int(count[s])
+            j = max(k for k in range(n) if start[s, k] <= r)
+            lo_e[l, s] = start[s, j]
+            if j == 0:
+                flags[l, s] |= MARGIN_LO_OPEN
+            else:
+                points[s].append(("below", i, below(start[s, j])))
+            if j + 1 < n:
+                hi_e[l, s] = start[s, j + 1]
+                recs["above"][i] = rec[s * M_ALL + j + 1]
+            elif over_at is not None:
+                flags[l, s] |= MARGIN_TRUNCATED
+                hi_e[l, s] = over_at
+            else:
+                flags[l, s] |= MARGIN_HI_OPEN
+                hi_e[l, s] = F32(np.inf)
+    wins = winners_at(oracle_mod, fleet, [[x for _, _, x in p] for p in points])
+    for s in range(S):
+        for (kind, i, _), w in zip(points[s], wins[s]):
+            recs[kind][i] = w
+    return lo_e, hi_e, flags, recs["at"], recs["below"], recs["above"]
+
+
+def margin_record_rates(rate, lo_e, hi_e, flags):
+    """The rate margin_tail solves each record at, from ref_margins' lo, hi and flags [L, S]: {"at", "below",
+    "above"} -> [L * S], NaN where the record is not written."""
+    r = rate.reshape(-1)
+    f = flags.reshape(-1)
+    nan = np.full(r.shape, np.nan, np.float32)
+    down = np.where((f & (MARGIN_LO_OPEN | MARGIN_TRUNCATED)) == 0, below(lo_e.reshape(-1)), nan)
+    up = np.where((f & (MARGIN_HI_OPEN | MARGIN_TRUNCATED)) == 0, hi_e.reshape(-1), nan)
+    return {"at": r, "below": down.astype(np.float32), "above": up.astype(np.float32)}
+
+
+def check_margins(engine, oracle_mod, fleet, rate, lo, hi, what, own_rate=False, ref=None):
+    """Engine.load_margins against ref_margins (or `ref`, its result), bit for bit; own_rate passes arrival_rpm=None
+    (one level at the fleet's own load)."""
+    want = ref_margins(oracle_mod, fleet, rate, lo, hi) if ref is None else ref
+    got = engine.load_margins(fleet, None if own_rate else rate, lo, hi)
+    for name, g, w in zip(("lo", "hi"), got[:2], want[:2]):
+        assert same_bytes(g, w), f"{what}: {name}: got {g[g.view(np.uint32) != w.view(np.uint32)]}"
+    assert np.array_equal(got[2], want[2]), f"{what}: flags {got[2]} vs {want[2]}"
+    for name, g, w in zip(("at", "below", "above"), got[3:], want[3:]):
+        assert_allocs_equal(g, w, f"{what}: {name}")
+    return want
 
 
 INF_BITS, PAST = 0x7F800000, 0x7F800001

@@ -1,7 +1,7 @@
 """wva_load_margins: the stretch of float32 arrival rates around each level's rate on which the load-grid winner keeps
 its decision.
 
-The expected margins come from ref_margins, a composition over the CPU oracle: levels.ref_intervals over each level's
+The expected margins come from levels.ref_margins, a composition over the CPU oracle: levels.ref_intervals over each level's
 window (with M large enough never to truncate at M) lists the intervals; the margin is the one that holds the level's
 rate r, the next start is hi, and the records are the oracle's winners (levels.winners_at) at r, one float32 below lo
 and at hi.  A replica overflow (levels.server_steps) ends the stretch as it ends the interval list.  The GPU tests
@@ -14,8 +14,8 @@ import tempfile
 import numpy as np
 import pytest
 
-from tests.levels import (F32, KEY_FIELDS, TINY, from_bits, load_levels, load_pair, mixed_fleet, overflow_fleet,
-                          pair_state, rates_at_rate_star, rec_key, ref_intervals, server_steps, u32_bits, winners_at)
+from tests.levels import (F32, KEY_FIELDS, TINY, below, check_margins, from_bits, load_levels, load_pair, mixed_fleet,
+                          overflow_fleet, pair_state, rates_at_rate_star, rec_key, ref_margins, u32_bits, winners_at)
 from tests.util import (ALLOC_FIELDS, F32_MAX, WVA_ERR_BAD_ARG, WVA_ERR_STATE, WVA_ERR_UNSUPPORTED, assert_allocs_equal,
                         same_bytes)
 from workload_variant_autoscaler_b200 import (MARGIN_HI_OPEN, MARGIN_LO_OPEN, MARGIN_TRUNCATED, Allocs, Engine,
@@ -23,67 +23,6 @@ from workload_variant_autoscaler_b200 import (MARGIN_HI_OPEN, MARGIN_LO_OPEN, MA
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INF = F32(np.inf)
-M_ALL = 4096  # intervals per server in the composition: more than any window here holds
-
-
-# ---- the oracle composition ---------------------------------------------------------------------
-
-def below(x):
-    return np.nextafter(F32(x), F32(0))
-
-
-def ref_margins(oracle_mod, fleet, rate, lo, hi):
-    """(lo (L, S), hi (L, S), flags (L, S), at, below, above as structured arrays of L * S records)."""
-    L, S = rate.shape
-    lo_e, hi_e = np.zeros((L, S), np.float32), np.zeros((L, S), np.float32)
-    flags = np.zeros((L, S), np.uint8)
-    recs = {k: np.zeros(L * S, oracle_mod.ALLOC_DTYPE) for k in ("at", "below", "above")}
-    points = [[] for _ in range(S)]  # (record kind, index, rate) per server, over all levels
-    for l in range(L):
-        count, trunc, start, rec, _ = ref_intervals(oracle_mod, fleet, lo[l], hi[l], M_ALL)
-        assert not (count == M_ALL).any()
-        for s in range(S):
-            i, r = l * S + s, F32(rate[l, s])
-            over_at = server_steps(oracle_mod, fleet, s, lo[l, s], hi[l, s])[1] if trunc[s] else None
-            points[s].append(("at", i, r))
-            if over_at is not None and over_at <= r:
-                flags[l, s] = MARGIN_TRUNCATED
-                lo_e[l, s] = hi_e[l, s] = r
-                continue
-            n = int(count[s])
-            j = max(k for k in range(n) if start[s, k] <= r)
-            lo_e[l, s] = start[s, j]
-            if j == 0:
-                flags[l, s] |= MARGIN_LO_OPEN
-            else:
-                points[s].append(("below", i, below(start[s, j])))
-            if j + 1 < n:
-                hi_e[l, s] = start[s, j + 1]
-                recs["above"][i] = rec[s * M_ALL + j + 1]
-            elif over_at is not None:
-                flags[l, s] |= MARGIN_TRUNCATED
-                hi_e[l, s] = over_at
-            else:
-                flags[l, s] |= MARGIN_HI_OPEN
-                hi_e[l, s] = INF
-    wins = winners_at(oracle_mod, fleet, [[x for _, _, x in p] for p in points])
-    for s in range(S):
-        for (kind, i, _), w in zip(points[s], wins[s]):
-            recs[kind][i] = w
-    return lo_e, hi_e, flags, recs["at"], recs["below"], recs["above"]
-
-
-def check_margins(engine, oracle_mod, fleet, rate, lo, hi, what, own_rate=False):
-    """Engine.load_margins against ref_margins, bit for bit; own_rate passes arrival_rpm=None (one level at the
-    fleet's own load)."""
-    want = ref_margins(oracle_mod, fleet, rate, lo, hi)
-    got = engine.load_margins(fleet, None if own_rate else rate, lo, hi)
-    for name, g, w in zip(("lo", "hi"), got[:2], want[:2]):
-        assert same_bytes(g, w), f"{what}: {name}: got {g[g.view(np.uint32) != w.view(np.uint32)]}"
-    assert np.array_equal(got[2], want[2]), f"{what}: flags {got[2]} vs {want[2]}"
-    for name, g, w in zip(("at", "below", "above"), got[3:], want[3:]):
-        assert_allocs_equal(g, w, f"{what}: {name}")
-    return want
 
 
 def windows(fleet, rate, seed):

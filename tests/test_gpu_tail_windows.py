@@ -63,9 +63,9 @@ from __future__ import annotations
 
 import numpy as np
 import pytest
-from tests.grid_cases import (DELTA, MAIN_N, P60, SIZE_RATIO, XS, _concat, _edge_fleet, _edge_rpm, _fleet, _lam_of_rate,
-                              _lam_star, _model, _qa, _rate_bands, _x_rpm, bounds_cases, chain_profile, f32, load_cases,
-                              profile_cases, slo_cases, wide_bands)
+from tests.grid_cases import (DELTA, MAIN_N, P60, SIZE_RATIO, XS, _bails, _concat, _edge_fleet, _edge_rpm, _final_lam,
+                              _fleet, _lam_of_rate, _lam_star, _model, _qa, _Solves, _x_rpm, bounds_cases, f32,
+                              load_cases, profile_cases, slo_cases, tail_bands)
 from tests.levels import (LOAD, SLO, check_intervals, check_level_call, check_slo_bounds, lam_range, ref_grid,
                           ref_intervals, ref_slo_bounds, ref_trace)
 from tests.util import assert_allocs_equal
@@ -75,36 +75,8 @@ FB_SLOTS = 128  # kFbBlocks * kFbThreads: the threads of every re-run kernel
 # x = lambda * alpha of the levels: E(sum) 679 / 680 near x = 472; E(max p) 879 / 880, the pass-2 IEEE band and
 # E(sum) 899 / 900 between 604 and 632; float64 overflow above ~705
 # ---------------------------------------------------------------------------------------------------------------
-# the solves a tail runs, with their profiles
+# the solves a tail runs
 # ---------------------------------------------------------------------------------------------------------------
-class _Solves:
-    """(rates, K, lambda, candidate) of every streaming solve a tail runs, profiled in one vectorised pass."""
-
-    def __init__(self):
-        self.sr, self.K, self.lam, self.cand = [], [], [], []
-
-    def add(self, qa, lam, cand):
-        self.sr.append(qa.serv_rate())
-        self.K.append(qa.K)
-        self.lam.append(f32(lam))
-        self.cand.append(cand)
-
-    def profile(self):
-        P = chain_profile(self.sr, np.array(self.K), np.array(self.lam, np.float32))
-        P["lam"] = np.array(self.lam, np.float32)
-        P["sr0"] = np.array([r[0] for r in self.sr], np.float32)
-        P["srN"] = np.array([r[-1] for r in self.sr], np.float32)
-        P["K"] = np.array(self.K)
-        P["cand"] = list(self.cand)
-        return P
-
-
-def _final_lam(rpm, tps, out_tok, replicas):
-    """The final Analyze's lambda: totalRate / replicas in req/s, over 1000 (allocation.go:134-153)."""
-    total = f32(f32(tps) / f32(out_tok)) if tps > 0 else f32(f32(rpm) / f32(60))
-    return _lam_of_rate(f32(total / f32(replicas)))
-
-
 def _add_finals(S, cand, fleet, rpm, tps, tokens, what):
     """The final solve of every feasible record of an [L, S] candidate block (A = 1)."""
     L = rpm.shape[0]
@@ -328,15 +300,6 @@ def tail_solves(oracle_mod):
 # ---------------------------------------------------------------------------------------------------------------
 # CPU: every tail reaches its bands, bails on both sides of an edge, and on more than 128 items of different K
 # ---------------------------------------------------------------------------------------------------------------
-def _bails(P):
-    """The solves that leave the streaming windows: a rate or lambda outside [2^-60, 2^60), p at 2^880 or above, the
-    sum at 2^900 or above, or a float64 overflow."""
-    def inside(v):
-        return (v >= f32(2.0 ** -60)) & (v < f32(P60))
-    return P["over"] | (P["emax"] >= 880) | (P["esum"] >= 900) | ~inside(P["lam"]) | ~inside(P["sr0"]) | \
-        ~inside(P["srN"])
-
-
 def _items(P):
     """Each solve's item: (call, server, level / tick / start / end).  An SLO item holds two solves."""
     return [c[:3] for c in P["cand"]]
@@ -355,13 +318,6 @@ def _streamed(P):
 
 def _take(P, m):
     return {k: (v[m] if isinstance(v, np.ndarray) else [x for x, t in zip(v, m) if t]) for k, v in P.items()}
-
-
-def tail_bands(P):
-    b = wide_bands(P, steep=False)
-    for k, v in _rate_bands(P).items():
-        b[k] = (int(v),) * 2
-    return b
 
 
 @pytest.mark.parametrize("tail", list(TAILS))

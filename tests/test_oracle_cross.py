@@ -457,3 +457,32 @@ def test_tail_windows_cross(oracle_mod, case):
         main = grid_cases.bounds_cases()[0]
         cross_fleet(oracle_mod, main, t, "bounds", pairs=[(int(s), 0) for s in sample(main.n_servers, 24)])
         t.report(case, min_feasible=20, min_infeasible=0)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the load margins' records at the exponent windows and the bracket cases (test_gpu_margin_edges)
+# ---------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("case", ["at main", "at edge", "below", "above", "edge steps", "brackets"])
+def test_margin_edges_cross(oracle_mod, case):
+    """The records test_gpu_margin_edges judges wva_load_margins on (their bands are asserted there): each record's
+    rate (r, the float under lo, hi, from the oracle composition) applied to a copy of the fleet, on an even sample of
+    the levels and servers of each record kind; every level and server of the bracket cases."""
+    t = Tally()
+    sample = lambda n, k: np.unique(np.linspace(0, n - 1, k).round().astype(int))  # noqa: E731
+    if case == "brackets":
+        fleet, rate, lo, hi = grid_cases.bracket_cases()
+        levels_, servers = range(rate.shape[0]), range(fleet.n_servers)
+    else:
+        _, fleet, rate, lo, hi = next(c for c in grid_cases.margin_cases() if c[0] == case)
+        levels_, servers = sample(rate.shape[0], 6), sample(fleet.n_servers, 12)
+    L, S = rate.shape
+    xs = levels.margin_record_rates(rate, *levels.ref_margins(oracle_mod, fleet, rate, lo, hi)[:3])
+    for kind, x in xs.items():
+        x = x.reshape(L, S)
+        for l in levels_:
+            pairs = [(int(s), 0) for s in servers if not np.isnan(x[l, s])]
+            if pairs:
+                row = np.where(np.isnan(x[l]), rate[l], x[l]).astype(np.float32)
+                cross_fleet(oracle_mod, at_row(fleet, {"arrival_rpm": row[None, :]}, 0), t, f"{kind} level {l}",
+                            pairs=pairs)
+    t.report(case, min_feasible=8, min_infeasible=4 if case == "brackets" else 0)

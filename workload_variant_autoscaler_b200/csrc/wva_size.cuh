@@ -1321,6 +1321,9 @@ struct IvAcc {
     int tail;       // 1: a load pair, whose record needs the tail (the latency columns) at an interval start
     bool over;
 };
+// The host sizes interval_kernel's and margin_kernel's warps per block from this (64 A and 68 A bytes per warp), and
+// the tests place their accelerator counts on those layout thresholds.
+static_assert(sizeof(IvAcc) == 64, "IvAcc layout");
 
 __device__ __forceinline__ IvState iv_state(const DevFleet& f, int s, int a, const IvAcc& p, float rpm, Cand* key) {
     const float total = total_rate_of(f, s, rpm);
