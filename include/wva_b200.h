@@ -638,6 +638,45 @@ int wva_load_margins(wva_handle *h, const wva_fleet *fleet, int32_t n_levels,
                      const float *rpm_lo, const float *rpm_hi /* [L*S] search window, req/min */, wva_margins *out);
 
 /*
+ * Load margin trace: wva_load_margins along a replayed reconcile.  Every level of wva_load_margins is solved against
+ * the fleet's own current allocation c_0, but a controller that follows a forecast holds, at tick t, the current
+ * allocation c_t that wva_workload_trace carries into tick t: the last feasible winner of ticks 0..t-1, or c_0 when
+ * there is none.  TransitionPenalty and keepAccelerator read it, so the margins around tick t's load depend on the
+ * chain.  This call gives them in one call, without one upload and one sizing per tick.
+ *
+ * Rows are laid out as in wva_load_margins (index t*S + s, n_ticks*S entries per column of out), over load only:
+ * the tokens are the fleet's own columns.  Let f_t be the fleet with srv_arrival_rpm = row t of arrival_rpm and
+ * its current-allocation columns (srv_cur_acc, srv_cur_replicas, srv_cur_cost) = c_t, where c_{t+1} is winner t's
+ * (acc, replicas, cost) when that winner is feasible and c_t otherwise.  A zero-load winner with min_replicas 0 has
+ * accelerator WVA_ACC_NONE, 0 replicas and cost 0, and becomes exactly that.
+ *   - Block t of lo_rpm, hi_rpm, flags, at, below and above is byte for byte wva_load_margins(f_t) with one level:
+ *     rate row t, window row t (rpm_lo, rpm_hi).  The load moves at tick t only; the ticks before t do not read it,
+ *     so c_t does not move with it.
+ *   - Together, the `at` blocks are byte for byte wva_workload_trace's winners on the same rate rows with token rows
+ *     equal to the fleet's own columns.  That is a check of the chain that needs no oracle.
+ * A trace can be continued as wva_workload_trace's can: ticks 0..L-1 equal ticks 0..k-1 followed by ticks k..L-1 on
+ * the fleet whose srv_cur_* columns hold c_k (Fleet.apply_winners over the `at` blocks in Python).
+ *
+ * Sizing (DESIGN.md §3.21): phase 1 is wva_load_margins', with keepAccelerator honoured on the pinned servers only
+ * (wva_workload_trace's rule: keepAccelerator set, a current accelerator other than WVA_ACC_NONE, and either
+ * WVA_ACC_UNKNOWN or min_replicas != 0), since any other server's current accelerator can change along the chain.
+ * One kernel then walks each server's ticks for c_t, and the margin walk and the records read c_t.
+ *
+ * Only unlimited mode is covered; fleet->unlimited and the capacities are not read.  The fleet becomes resident,
+ * and wva_summarize returns WVA_ERR_STATE afterwards.  Columns of at, below and above may be NULL (not written).
+ * n_ticks == 0 and S == 0 are valid (nothing is written).  WVA_ERR_BAD_ARG: n_ticks < 0, out NULL, arrival_rpm,
+ * rpm_lo, rpm_hi, lo_rpm, hi_rpm or flags NULL with S*n_ticks > 0, or a row that wva_load_margins(f_t) refuses
+ * (NaN, infinite or negative, or the rate outside its window).  WVA_ERR_UNSUPPORTED: 3*S*n_ticks >= 2^31 (refused
+ * before the fleet is read), or where wva_load_margins(f_t) refuses at some tick t.  This set of refusals can be
+ * larger than the union over t of what wva_load_margins(f_t) refuses, but only through the pairs of a server that
+ * is not pinned yet has keepAccelerator set, at ticks where the chain keeps them masked.  The call never returns a
+ * result that differs from the per-tick composition.
+ */
+int wva_load_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks,
+                          const float *arrival_rpm /* [L*S], required */,
+                          const float *rpm_lo, const float *rpm_hi /* [L*S] windows, req/min */, wva_margins *out);
+
+/*
  * Price thresholds: for each server s and accelerator a, the exact accelerator price at which s's unlimited
  * winner leaves a.  Let f(p) be the fleet with acc_cost[a] = p, solved in unlimited mode.
  *

@@ -943,7 +943,8 @@ int enqueue_size_grid(wva_handle* h, int B, const int32_t* batch, const AllocCol
 // call).  Each passes the fleet it sizes: the resident one, or the workload grid's key fleet.
 //
 // prepare_load_star uploads the candidate lists of fleet hf with the caller's columns (laid out in c, written by
-// fill; `pairs` holds the candidates' pair ids by the time fill runs).  enqueue_load_star then builds the tables
+// fill; `pairs` holds the candidates' pair ids by the time fill runs).  pin, when given (a trace's trace_pinned
+// flags), keeps keepAccelerator on the pinned servers only.  enqueue_load_star then builds the tables
 // for the device image f of the same fleet and sizes fallback list 1 for the caller's tail (prepare_tail, which the
 // SLO grid shares), and enqueues phase 1.
 struct LoadStar {
@@ -953,10 +954,12 @@ struct LoadStar {
 };
 template <class Fill>
 int prepare_load_star(wva_handle* h, const HostFleet& hf, const std::vector<char>& loaded, std::vector<int>& pairs,
-                      Cols& c, Fill&& fill) {
+                      Cols& c, Fill&& fill, const uint8_t* pin = nullptr) {
     std::vector<int> Ns;
     int rc = sorted_pairs(
-        h, hf, [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, true, 1.0f) == PAIR_LOAD; }, pairs, Ns);
+        h, hf,
+        [&](int s, int a) { return loaded[s] && hf.pair_class(s, a, !pin || pin[s], 1.0f) == PAIR_LOAD; }, pairs,
+        Ns);
     if (rc) return rc;
     return upload_tables(h, h->lg_tabs, pairs, Ns, true, c, fill);
 }
@@ -1164,36 +1167,91 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int 
     return WVA_OK;
 }
 
+// The servers whose accelerator no tick of a trace can change (DESIGN.md §3.13), as flags [S]: with keepAccelerator
+// and a current accelerator other than "" only that accelerator is a candidate, and its load and zero-load
+// candidates carry it unless min_replicas is 0 (a zero-load candidate is then ""); an unknown one has no candidate at
+// all.  A nil winner keeps the current allocation, so neither ever moves.  A trace's records carry keepAccelerator on
+// these servers only: trace_kernel applies the rest of the mask tick by tick.
+std::vector<uint8_t> trace_pinned(const HostFleet& hf) {
+    std::vector<uint8_t> pin(hf.S);
+    for (int s = 0; s < hf.S; ++s) {
+        const int cur = hf.srv_cur_acc[s];
+        pin[s] = hf.srv_keep_acc[s] && cur != WVA_ACC_NONE && (cur == WVA_ACC_UNKNOWN || hf.srv_min_replicas[s] != 0);
+    }
+    return pin;
+}
+
 // ---- load margins: the stretch around each level's rate on which the load-grid winner keeps its decision -------
 static_assert(MG_LO_OPEN == WVA_MARGIN_LO_OPEN && MG_HI_OPEN == WVA_MARGIN_HI_OPEN &&
               MG_TRUNCATED == WVA_MARGIN_TRUNCATED, "margin flags");
 
 // The device columns of one call: lo_out, hi_out and flags [n] come back to the caller, the work list [3n] stays
-// on the device.
+// on the device, and so do a trace's c_t columns [n] (acc, replicas, cost), which margin_chain writes.
 struct MarginCols {
     Cols cols{16};
-    size_t o_lo = 0, o_hi = 0, o_flags = 0, o_items = 0;
+    size_t o_lo = 0, o_hi = 0, o_flags = 0, o_items = 0, o_cur_acc = 0, o_cur_rep = 0, o_cur_cost = 0;
 };
+
+// Warps per block (up to 4) of a kernel that runs one warp per item with per_warp bytes of dynamic shared memory per
+// warp, the block's bytes, and the kernel's opt-in to more than 48 KiB where it needs that.
+template <class Kernel>
+int warp_layout(wva_handle* h, Kernel kernel, size_t per_warp, const char* what, int& wpb, size_t& smem) {
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    if (per_warp > (size_t)optin) return h->fail(WVA_ERR_UNSUPPORTED, what);
+    wpb = (int)std::max<size_t>(1, std::min<size_t>(4, (48u << 10) / std::max<size_t>(per_warp, 1)));
+    smem = per_warp * wpb;
+    if (smem > (48u << 10)) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return WVA_OK;
+}
+
+// margin_kernel, margin_tail and margin_fallback of g (the Trace instantiations on a trace).
+template <bool Trace>
+int launch_margins(wva_handle* h, const MarginArgs& g, const LoadStar& ls) {
+    // one warp per (level, server), A accelerator states and stretch starts per warp in shared memory
+    int wpb = 0;
+    size_t smem = 0;
+    const int rc = warp_layout(h, margin_kernel<Trace>, (sizeof(IvAcc) + sizeof(float)) * (size_t)h->hf.A,
+                               "too many accelerators for the margin kernel's shared memory", wpb, smem);
+    if (rc) return rc;
+    const int n = g.n;
+    margin_kernel<Trace><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, (3ll * n + 255) / 256);
+    margin_tail<Trace><<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
+    h->launches += 2;
+    CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1, the chain and the margin kernels
+    launch_fallback(h, margin_fallback<Trace>, g, ls.fb2);
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
 
 // Phase 1 over the servers with some window top > 0, margin_kernel, margin_tail and margin_fallback.  rate / lo /
 // hi [L*S] are the caller's rows (rate NULL: the fleet's own column); rec ([3*L*S]) is a device block; the other
 // columns are in h->d_iv at mc's offsets.
+//
+// With `trace` (wva_load_margin_trace, DESIGN.md §3.21) row t is tick t against c_t.  Phase 1 then honours
+// keepAccelerator on the pinned servers only (trace_pinned): an unpinned server's chain can lift the mask at a later
+// tick.  margin_chain writes c_t into mc's columns before the margin kernels read them through at_tick.
 int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* lo, const float* hi,
-                         const MarginCols& mc, const AllocCols& rec, size_t rec_bytes) {
+                         const MarginCols& mc, const AllocCols& rec, size_t rec_bytes, bool trace) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A, n = S * L;
     std::vector<char> loaded(S, 0);
     for (int i = 0; i < n; ++i) loaded[i % S] |= hi[i] > 0.0f;
+    const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
     std::vector<int> pairs;
     Cols c(16);
     RowLists lists{hf, L, c};
     lists.put_rpm(rate);
     const size_t o_lo = c.put(lo, 4 * (size_t)n), o_hi = c.put(hi, 4 * (size_t)n), o_cop = c.take(4 * (size_t)S * A);
-    int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
-        int* cop = (int*)(p + o_cop);
-        std::fill(cop, cop + (size_t)S * A, -1);
-        for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
-    });
+    int rc = prepare_load_star(
+        h, hf, loaded, pairs, c,
+        [&](char* p) {
+            int* cop = (int*)(p + o_cop);
+            std::fill(cop, cop + (size_t)S * A, -1);
+            for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
+        },
+        trace ? pin.data() : nullptr);
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
@@ -1218,22 +1276,65 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* l
     g.rec = rec;
     g.items = FbList{(int*)h->d_ctrl.p + CTRL_COUNTER, (unsigned long long*)(d + mc.o_items), 3 * n};
     g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
-    // one warp per (level, server), A accelerator states and stretch starts per warp in shared memory
-    const size_t per_warp = (sizeof(IvAcc) + sizeof(float)) * (size_t)A;
-    int optin = 0;
-    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-    if (per_warp > (size_t)optin)
-        return h->fail(WVA_ERR_UNSUPPORTED, "too many accelerators for the margin kernel's shared memory");
-    const int wpb = (int)std::max<size_t>(1, std::min<size_t>(4, (48u << 10) / std::max<size_t>(per_warp, 1)));
-    const size_t smem = per_warp * wpb;
-    if (smem > (48u << 10)) CK(cudaFuncSetAttribute(margin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    margin_kernel<<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
-    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, (3ll * n + 255) / 256);
-    margin_tail<<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
-    h->launches += 2;
-    CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1 and the margin kernels
-    launch_fallback(h, margin_fallback, g, ls.fb2);
-    CK(cudaGetLastError());
+    if (!trace) return launch_margins<false>(h, g, ls);
+    g.cur_acc = (int*)(d + mc.o_cur_acc);
+    g.cur_replicas = (int*)(d + mc.o_cur_rep);
+    g.cur_cost = (float*)(d + mc.o_cur_cost);
+    // one warp per server, A accelerator states per warp in shared memory
+    int wpb = 0;
+    size_t smem = 0;
+    rc = warp_layout(h, margin_chain, sizeof(IvAcc) * (size_t)A,
+                     "too many accelerators for the margin chain's shared memory", wpb, smem);
+    if (rc) return rc;
+    margin_chain<<<(unsigned)((S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    h->launches++;
+    return launch_margins<true>(h, g, ls);
+}
+
+// wva_load_margins, or with `trace` wva_load_margin_trace (which requires the rate rows)
+int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                      const float* rpm_lo, const float* rpm_hi, wva_margins* out, bool trace) {
+    if (!h) return WVA_ERR_BAD_ARG;
+    if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
+    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, trace ? "negative tick count" : "negative level count");
+    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
+    const int S = fleet->n_servers, L = n_levels;
+    // three records per (level, server), each indexed in int32
+    if (3ll * S * L >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "load margins too large for one call (>= 2^31 records)");
+    const int n = S * L;
+    if (n > 0 && (!rpm_lo || !rpm_hi || !out->lo_rpm || !out->hi_rpm || !out->flags))
+        return h->fail(WVA_ERR_BAD_ARG, "NULL window or output column");
+    if (n > 0 && trace && !arrival_rpm) return h->fail(WVA_ERR_BAD_ARG, "NULL arrival rate rows");
+    for (int i = 0; i < n; ++i) {
+        const float r = arrival_rpm ? arrival_rpm[i] : fleet->srv_arrival_rpm[i % S], lo = rpm_lo[i], hi = rpm_hi[i];
+        if (!std::isfinite(r) || !std::isfinite(lo) || !std::isfinite(hi) || r < 0.0f || lo < 0.0f || hi < 0.0f ||
+            lo > r || r > hi)
+            return h->fail(WVA_ERR_BAD_ARG, "rate or window NaN, infinite or negative, or the rate outside its window");
+    }
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    MarginCols mc;
+    mc.o_lo = mc.cols.take(4 * (size_t)n, out->lo_rpm);
+    mc.o_hi = mc.cols.take(4 * (size_t)n, out->hi_rpm);
+    mc.o_flags = mc.cols.take((size_t)n, out->flags);
+    mc.o_items = mc.cols.take(8 * 3 * (size_t)n);
+    if (trace) {
+        mc.o_cur_acc = mc.cols.take(4 * (size_t)n);
+        mc.o_cur_rep = mc.cols.take(4 * (size_t)n);
+        mc.o_cur_cost = mc.cols.take(4 * (size_t)n);
+    }
+    CK(h->d_iv.ensure(mc.cols.bytes));
+    HostCall c{3 * (size_t)n, n > 0, false, &mc.cols, h->d_iv.p};
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
+        return enqueue_load_margins(h, L, arrival_rpm, rpm_lo, rpm_hi, mc, dc, c.bc.bytes, trace);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    const wva_allocs* recs[3] = {&out->at, &out->below, &out->above};
+    if (n > 0)
+        for (int k = 0; k < 3; ++k) scatter_block(c.cand_host, sub_block(c.bc, k, n), recs[k]);
     return WVA_OK;
 }
 
@@ -1489,20 +1590,6 @@ struct KeyFleet {
         return f;
     }
 };
-
-// The servers whose accelerator no tick of a trace can change (DESIGN.md §3.13), as flags [S]: with keepAccelerator
-// and a current accelerator other than "" only that accelerator is a candidate, and its load and zero-load
-// candidates carry it unless min_replicas is 0 (a zero-load candidate is then ""); an unknown one has no candidate at
-// all.  A nil winner keeps the current allocation, so neither ever moves.  A trace's records carry keepAccelerator on
-// these servers only: trace_kernel applies the rest of the mask tick by tick.
-std::vector<uint8_t> trace_pinned(const HostFleet& hf) {
-    std::vector<uint8_t> pin(hf.S);
-    for (int s = 0; s < hf.S; ++s) {
-        const int cur = hf.srv_cur_acc[s];
-        pin[s] = hf.srv_keep_acc[s] && cur != WVA_ACC_NONE && (cur == WVA_ACC_UNKNOWN || hf.srv_min_replicas[s] != 0);
-    }
-    return pin;
-}
 
 // The workload grid's tail (workload_kernel, then workload_fallback) after phase 1 (ls): g's key and level lists and
 // g.n_items items, at the rates level_rpm [L * g.S], into cand.  ev_k1 is recorded after workload_kernel: the
@@ -3229,42 +3316,12 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
 
 int wva_load_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                      const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    if (!h) return WVA_ERR_BAD_ARG;
-    if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
-    if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, "negative level count");
-    if (const char* what = fleet_problem(fleet)) return h->fail(WVA_ERR_BAD_ARG, what);
-    const int S = fleet->n_servers, L = n_levels;
-    // three records per (level, server), each indexed in int32
-    if (3ll * S * L >= (1ll << 31))
-        return h->fail(WVA_ERR_UNSUPPORTED, "load margins too large for one call (>= 2^31 records)");
-    const int n = S * L;
-    if (n > 0 && (!rpm_lo || !rpm_hi || !out->lo_rpm || !out->hi_rpm || !out->flags))
-        return h->fail(WVA_ERR_BAD_ARG, "NULL window or output column");
-    for (int i = 0; i < n; ++i) {
-        const float r = arrival_rpm ? arrival_rpm[i] : fleet->srv_arrival_rpm[i % S], lo = rpm_lo[i], hi = rpm_hi[i];
-        if (!std::isfinite(r) || !std::isfinite(lo) || !std::isfinite(hi) || r < 0.0f || lo < 0.0f || hi < 0.0f ||
-            lo > r || r > hi)
-            return h->fail(WVA_ERR_BAD_ARG, "rate or window NaN, infinite or negative, or the rate outside its window");
-    }
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    MarginCols mc;
-    mc.o_lo = mc.cols.take(4 * (size_t)n, out->lo_rpm);
-    mc.o_hi = mc.cols.take(4 * (size_t)n, out->hi_rpm);
-    mc.o_flags = mc.cols.take((size_t)n, out->flags);
-    mc.o_items = mc.cols.take(8 * 3 * (size_t)n);
-    CK(h->d_iv.ensure(mc.cols.bytes));
-    HostCall c{3 * (size_t)n, n > 0, false, &mc.cols, h->d_iv.p};
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
-        return enqueue_load_margins(h, L, arrival_rpm, rpm_lo, rpm_hi, mc, dc, c.bc.bytes);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    const wva_allocs* recs[3] = {&out->at, &out->below, &out->above};
-    if (n > 0)
-        for (int k = 0; k < 3; ++k) scatter_block(c.cand_host, sub_block(c.bc, k, n), recs[k]);
-    return WVA_OK;
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, rpm_lo, rpm_hi, out, false);
+}
+
+int wva_load_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                          const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, rpm_lo, rpm_hi, out, true);
 }
 
 int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold, wva_allocs* above,

@@ -1346,10 +1346,11 @@ __device__ __forceinline__ IvState iv_state(const DevFleet& f, int s, int a, con
 
 // Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.  g is the call's
 // IntervalArgs or MarginArgs; the window of x is row `row` of its bound lists g.lo / g.hi (the load intervals have
-// one row).
+// one row).  f is the fleet the key is taken on: g.ld.f, or on a margin trace the row's view at_tick.  With hi = x it
+// returns right after the key.
 template <class Args>
-__device__ __forceinline__ void iv_advance(const Args& g, int row, int s, int a, float x, float hi, IvAcc& p) {
-    const DevFleet& f = g.ld.f;
+__device__ __forceinline__ void iv_advance(const Args& g, const DevFleet& f, int row, int s, int a, float x, float hi,
+                                           IvAcc& p) {
     const float inf = __int_as_float(0x7f800000);
     // the class at x: pair_class reads only whether the rate is negative or zero, and lo is 0 when x = 0
     const int cls = pair_class(at_level(f, x == 0.0f ? g.lo : g.hi, row), s, a, true);
@@ -1407,6 +1408,10 @@ __device__ __forceinline__ void iv_advance(const Args& g, int row, int s, int a,
         else l = m;
     }
     p.next = __uint_as_float(h);
+}
+template <class Args>
+__device__ __forceinline__ void iv_advance(const Args& g, int row, int s, int a, float x, float hi, IvAcc& p) {
+    iv_advance(g, g.ld.f, row, s, a, x, hi, p);
 }
 
 // SolveUnlimited over the warp's accelerators: strict '<' from MaxFloat32, ties to the lower accelerator id.
@@ -1529,6 +1534,10 @@ __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec
 // changes, and the walk stops at the first such y whose float below changes the key.  margin_tail then runs the load
 // grid's tail at the records (at r, below lo, at hi) whose winner is a load pair, and margin_fallback re-runs the
 // items it bailed on.
+//
+// On a trace (DESIGN.md §3.21, the kernels' Trace instantiations) level t is tick t, solved against the current
+// allocation c_t that the workload trace carries into it.  margin_chain writes c_t of every (tick, server) first, and
+// every read of the current allocation then goes through at_tick's view of the fleet.
 // ---------------------------------------------------------------------------
 enum { MG_LO_OPEN = 1, MG_HI_OPEN = 2, MG_TRUNCATED = 4 };  // the header's WVA_MARGIN_*
 
@@ -1545,7 +1554,57 @@ struct MarginArgs {
     AllocCols rec;             // [3 * n]: at (k = 0), below (1), above (2), record k * n + i
     FbList items;              // margin_tail's work list: fb_pack(accelerator, record)
     int* status;               // set when a window holds a rate at which a pair has 0 replicas (see iv_advance)
+    int* cur_acc;              // [n] on a trace: c_t of item t * S + s, written by margin_chain (unused otherwise)
+    int* cur_replicas;
+    float* cur_cost;
 };
+
+// The fleet of a trace's tick t: the resident fleet with the current allocation c_t.
+__device__ __forceinline__ DevFleet at_tick(const MarginArgs& g, int t) {
+    DevFleet ft = g.ld.f;
+    const size_t o = (size_t)t * g.ld.f.S;
+    ft.srv_cur_acc = g.cur_acc + o;
+    ft.srv_cur_replicas = g.cur_replicas + o;
+    ft.srv_cur_cost = g.cur_cost + o;
+    return ft;
+}
+
+// The trace's chain: one warp per server walks the ticks with c_t in registers (c_0 from the fleet), lanes over the
+// accelerators as in margin_kernel.  At tick t it stores c_t, takes every pair's key at the tick's rate against c_t
+// (iv_advance with hi = the rate, which returns after the key) and the winner (iv_winner: strict '<' from MaxFloat32,
+// ties to the lower accelerator id); c_{t+1} is the winner's (acc, replicas, cost) when there is one, c_t otherwise
+// (Server.ApplyDesiredAlloc).  Those key columns are the ones margin_tail writes into `at`, so the chain needs no
+// latency solve.  Launched with up to 128 threads; A IvAcc states per warp in dynamic shared memory.
+__global__ void __launch_bounds__(128) margin_chain(MarginArgs g) {
+    extern __shared__ IvAcc iv_acc[];
+    const DevFleet& f = g.ld.f;
+    const int A = f.A, S = f.S, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int s = blockIdx.x * (blockDim.x >> 5) + wid;
+    if (s >= S) return;
+    IvAcc* acc = iv_acc + (size_t)wid * A;
+    int cur_acc = f.srv_cur_acc[s], cur_replicas = f.srv_cur_replicas[s];
+    float cur_cost = f.srv_cur_cost[s];
+    const int L = g.n / S;
+    for (int t = 0; t < L; ++t) {
+        const int i = t * S + s;
+        if (lane == 0) {
+            g.cur_acc[i] = cur_acc;
+            g.cur_replicas[i] = cur_replicas;
+            g.cur_cost[i] = cur_cost;
+        }
+        __syncwarp();  // c_t is visible to the warp, and the previous tick's reads of acc are done
+        const DevFleet ft = at_tick(g, t);
+        const float r = g.rate[i];
+        for (int a = lane; a < A; a += 32) iv_advance(g, ft, t, s, a, r, r, acc[a]);
+        __syncwarp();
+        const int w = iv_winner(acc, A, lane);
+        if (w >= 0) {
+            cur_acc = acc[w].key.acc;
+            cur_replicas = acc[w].key.replicas;
+            cur_cost = acc[w].key.cost;
+        }
+    }
+}
 
 // nextafterf(x, 0) for x > 0
 __device__ __forceinline__ float mg_below(float x) { return __uint_as_float(__float_as_uint(x) - 1u); }
@@ -1605,18 +1664,22 @@ __device__ __forceinline__ void mg_emit(const MarginArgs& g, int k, int i, int w
 // One warp per (level, server) item i = l * S + s; the accelerators' IvAcc states, then their stretch starts, live
 // in dynamic shared memory (A entries of each per warp).  Launched with up to 128 threads; with
 // __launch_bounds__(128) ptxas keeps it at 72 registers and spills, with room for 96 it uses 80 and does not.
+// Trace: level l is tick l, on the fleet at_tick(g, l).
+template <bool Trace>
 __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
     extern __shared__ IvAcc iv_acc[];
-    const DevFleet& f = g.ld.f;
-    const int A = f.A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+    const int A = g.ld.f.A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
     const int i = blockIdx.x * wpb + wid;
     if (i >= g.n) return;
-    const int l = i / f.S, s = i - l * f.S;
+    const int l = i / g.ld.f.S, s = i - l * g.ld.f.S;
+    DevFleet ft;
+    if constexpr (Trace) ft = at_tick(g, l);
+    const DevFleet& f = Trace ? ft : g.ld.f;
     IvAcc* acc = iv_acc + (size_t)wid * A;
     float* start = (float*)(iv_acc + (size_t)wpb * A) + (size_t)wid * A;
     const float r = g.rate[i], lo = g.lo[i], hi = g.hi[i];
     const float inf = __int_as_float(0x7f800000);
-    auto advance = [&](int a, float x) { iv_advance(g, l, s, a, x, hi, acc[a]); };
+    auto advance = [&](int a, float x) { iv_advance(g, f, l, s, a, x, hi, acc[a]); };
     bool over = false;
     for (int a = lane; a < A; a += 32) {
         advance(a, r);
@@ -1714,7 +1777,8 @@ __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
 }
 
 // The item fb_pack(a, k * n + i): record k of item i, whose winner is the load pair of accelerator a, the load
-// grid's tail at the record's rate (r, the float below lo_out, or hi_out), then the value.
+// grid's tail at the record's rate (r, the float below lo_out, or hi_out), then the value (on a trace against c_t).
+template <bool Trace>
 struct MgTail {
     const MarginArgs& g;
     template <class Solve>
@@ -1724,19 +1788,24 @@ struct MgTail {
         const float x = k == 0 ? g.rate[i] : (k == 1 ? mg_below(g.lo_out[i]) : g.hi_out[i]);
         const int e = g.cand_of_pair[s * f.A + a];
         if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, x); }, solve, out)) return false;
-        if (out.feasible) out.value = penalty_of(f, s, out);
+        if (out.feasible) {
+            if constexpr (Trace) out.value = penalty_of(at_tick(g, i / f.S), s, out);
+            else out.value = penalty_of(f, s, out);
+        }
         return true;
     }
     __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
 };
 
+template <bool Trace>
 __global__ void __launch_bounds__(256) margin_tail(MarginArgs g) {
     const int n = min(*g.items.count, g.items.cap);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-        tail_item(g.ld.fb, g.rec, g.items.item[i], MgTail{g});
+        tail_item(g.ld.fb, g.rec, g.items.item[i], MgTail<Trace>{g});
 }
 
 // Stored-vector re-run of the records margin_tail bailed on.
-__global__ void margin_fallback(MarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail{g}); }
+template <bool Trace>
+__global__ void margin_fallback(MarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace>{g}); }
 
 }  // namespace wva

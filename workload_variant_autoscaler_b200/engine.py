@@ -182,7 +182,10 @@ def within_margins(lo, hi, flags, new_rpm, rpm_hi):
     The stretch is ``[lo, hi)``.  An open end is the window's edge, not a change: below ``rpm_lo`` (= ``lo`` with
     ``MARGIN_LO_OPEN``) and above ``rpm_hi`` (the window tops the margins were computed over, needed because ``hi``
     is +Inf with ``MARGIN_HI_OPEN``) nothing is known, so a rate there is outside.  A stretch truncated at the rate
-    itself (``lo == hi``) holds nothing; NaN is never inside."""
+    itself (``lo == hi``) holds nothing; NaN is never inside.
+
+    It works unchanged on ``Engine.load_margin_trace``'s result: there the servers inside their stretch at tick t
+    keep the decision the replayed reconcile makes at tick t."""
     lo, hi, top, x = (np.asarray(v, np.float32) for v in (lo, hi, rpm_hi, new_rpm))
     flags = np.asarray(flags, np.uint8)
     if not lo.shape == hi.shape == flags.shape == top.shape == x.shape:
@@ -502,6 +505,23 @@ class Engine:
         rate, one float32 below ``lo`` and at ``hi``.  ``flags`` holds ``MARGIN_LO_OPEN`` (no change down to
         ``rpm_lo``), ``MARGIN_HI_OPEN`` (none up to ``rpm_hi``, ``hi`` = +Inf) and ``MARGIN_TRUNCATED`` (see
         ``wva_load_margins`` in include/wva_b200.h).  ``within_margins`` tests new rates against the result."""
+        return self._margins(self._L.wva_load_margins, fleet, arrival_rpm, rpm_lo, rpm_hi)
+
+    def load_margin_trace(self, fleet: Fleet, arrival_rpm, rpm_lo=None, rpm_hi=None):
+        """``load_margins`` at every tick of ``workload_trace`` over the rates ``arrival_rpm`` (shape (L, S),
+        req/min, required; the tokens are the fleet's own) -> the same tuple as ``load_margins``.
+
+        Block ``t`` is ``load_margins`` with one level (row ``t`` of the rates and of the windows, by default
+        ``[0, 2 * rate]``) on the fleet whose current allocation is the one the trace carries into tick ``t``
+        (``fleet.apply_winners`` of every earlier tick's ``at`` in turn): the load moves at tick ``t`` only.  The
+        ``at`` records are ``workload_trace``'s winners (see ``wva_load_margin_trace`` in include/wva_b200.h).
+        ``within_margins`` tests new rates against the result as it does for ``load_margins``."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        return self._margins(self._L.wva_load_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi)
+
+    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi):
+        """wva_load_margins / wva_load_margin_trace over (L, S) rows and windows; the output arrays."""
         S = fleet.n_servers
         rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "rpm_lo": rpm_lo, "rpm_hi": rpm_hi})
         L = 1 if L is None else L
@@ -515,8 +535,8 @@ class Engine:
                            at.as_c(), below.as_c(), above.as_c())
         fc = fleet.as_c()
         self._resident(fleet)
-        self._check(self._L.wva_load_margins(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)),
-                                             _abi.ptr(lo.reshape(-1)), _abi.ptr(hi.reshape(-1)), C.byref(oc)))
+        self._check(call(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)), _abi.ptr(lo.reshape(-1)),
+                         _abi.ptr(hi.reshape(-1)), C.byref(oc)))
         return lo_out, hi_out, flags, at, below, above
 
     def price_thresholds(self, fleet: Fleet, want_candidates: bool = False):
