@@ -1100,73 +1100,7 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     return WVA_OK;
 }
 
-// ---- load intervals: where each server's load-grid winner changes in [lo, hi] ---------------------------------
-// The device columns of one call: count [S], truncated [S] and start [S*M] come back to the caller, the work list
-// [S*M] stays on the device.
-struct IntervalCols {
-    Cols cols{16};
-    size_t o_count = 0, o_trunc = 0, o_start = 0, o_items = 0;
-};
-
-// Phase 1 over the servers with hi > 0, interval_kernel, interval_tail and interval_fallback.  lo / hi [S] are
-// the caller's bounds; rec ([S*M]) is a device block; the other columns are in h->d_iv at iv's offsets.
-int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, int M, const IntervalCols& iv,
-                           const AllocCols& rec, size_t rec_bytes) {
-    const HostFleet& hf = h->hf;
-    const int S = hf.S, A = hf.A;
-    std::vector<char> loaded(S, 0);
-    for (int s = 0; s < S; ++s) loaded[s] = hi[s] > 0.0f;
-    std::vector<int> pairs;
-    Cols c(16);
-    const size_t o_lo = c.put(lo, 4 * (size_t)S), o_hi = c.put(hi, 4 * (size_t)S), o_cop = c.take(4 * (size_t)S * A);
-    int rc = prepare_load_star(h, hf, loaded, pairs, c, [&](char* p) {
-        int* cop = (int*)(p + o_cop);
-        std::fill(cop, cop + (size_t)S * A, -1);
-        for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
-    });
-    if (rc) return rc;
-    rc = ensure_ctrl(h);
-    if (rc) return rc;
-    // records and starts past a server's count read back as zero
-    char* d = (char*)h->d_iv.p;
-    CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
-    CK(cudaMemsetAsync(d + iv.o_start, 0, 4 * (size_t)S * M, h->stream));
-    LoadStar ls;
-    rc = enqueue_load_star(h, hf, h->df, (long long)S * M, ls);
-    if (rc) return rc;
-    if (S == 0) return WVA_OK;
-    const char* dl = (const char*)h->lg_tabs.lists.p;
-    IntervalArgs g{};
-    g.ld = load_args(h, ls);
-    g.cand_of_pair = (const int*)(dl + o_cop);
-    g.lo = (const float*)(dl + o_lo);
-    g.hi = (const float*)(dl + o_hi);
-    g.M = M;
-    g.count = (int*)(d + iv.o_count);
-    g.truncated = (uint8_t*)(d + iv.o_trunc);
-    g.start = (float*)(d + iv.o_start);
-    g.rec = rec;
-    g.items = FbList{(int*)h->d_ctrl.p + CTRL_COUNTER, (unsigned long long*)(d + iv.o_items), S * M};
-    g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
-    // one warp per server, A accelerator states per warp in shared memory
-    const size_t per_warp = sizeof(IvAcc) * (size_t)A;
-    int optin = 0;
-    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-    if (per_warp > (size_t)optin)
-        return h->fail(WVA_ERR_UNSUPPORTED, "too many accelerators for the interval kernel's shared memory");
-    const int wpb = (int)std::max<size_t>(1, std::min<size_t>(4, (48u << 10) / std::max<size_t>(per_warp, 1)));
-    const size_t smem = per_warp * wpb;
-    if (smem > (48u << 10)) CK(cudaFuncSetAttribute(interval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    interval_kernel<<<(unsigned)((S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
-    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, ((long long)S * M + 255) / 256);
-    interval_tail<<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
-    h->launches += 2;
-    CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1 and the interval kernels
-    launch_fallback(h, interval_fallback, g, ls.fb2);
-    CK(cudaGetLastError());
-    return WVA_OK;
-}
-
+// ---- walks: the load intervals and the load margins -----------------------------------------------------------
 // The servers whose accelerator no tick of a trace can change (DESIGN.md §3.13), as flags [S]: with keepAccelerator
 // and a current accelerator other than "" only that accelerator is a candidate, and its load and zero-load
 // candidates carry it unless min_replicas is 0 (a zero-load candidate is then ""); an unknown one has no candidate at
@@ -1181,17 +1115,6 @@ std::vector<uint8_t> trace_pinned(const HostFleet& hf) {
     return pin;
 }
 
-// ---- load margins: the stretch around each level's rate on which the load-grid winner keeps its decision -------
-static_assert(MG_LO_OPEN == WVA_MARGIN_LO_OPEN && MG_HI_OPEN == WVA_MARGIN_HI_OPEN &&
-              MG_TRUNCATED == WVA_MARGIN_TRUNCATED, "margin flags");
-
-// The device columns of one call: lo_out, hi_out and flags [n] come back to the caller, the work list [3n] stays
-// on the device, and so do a trace's c_t columns [n] (acc, replicas, cost), which margin_chain writes.
-struct MarginCols {
-    Cols cols{16};
-    size_t o_lo = 0, o_hi = 0, o_flags = 0, o_items = 0, o_cur_acc = 0, o_cur_rep = 0, o_cur_cost = 0;
-};
-
 // Warps per block (up to 4) of a kernel that runs one warp per item with per_warp bytes of dynamic shared memory per
 // warp, the block's bytes, and the kernel's opt-in to more than 48 KiB where it needs that.
 template <class Kernel>
@@ -1205,44 +1128,18 @@ int warp_layout(wva_handle* h, Kernel kernel, size_t per_warp, const char* what,
     return WVA_OK;
 }
 
-// margin_kernel, margin_tail and margin_fallback of g (the Trace instantiations on a trace).
-template <bool Trace>
-int launch_margins(wva_handle* h, const MarginArgs& g, const LoadStar& ls) {
-    // one warp per (level, server), A accelerator states and stretch starts per warp in shared memory
-    int wpb = 0;
-    size_t smem = 0;
-    const int rc = warp_layout(h, margin_kernel<Trace>, (sizeof(IvAcc) + sizeof(float)) * (size_t)h->hf.A,
-                               "too many accelerators for the margin kernel's shared memory", wpb, smem);
-    if (rc) return rc;
-    const int n = g.n;
-    margin_kernel<Trace><<<(unsigned)((n + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
-    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, (3ll * n + 255) / 256);
-    margin_tail<Trace><<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
-    h->launches += 2;
-    CK(cudaEventRecord(h->ev_k1, h->stream));  // the call's kernel time: phase 1, the chain and the margin kernels
-    launch_fallback(h, margin_fallback<Trace>, g, ls.fb2);
-    CK(cudaGetLastError());
-    return WVA_OK;
-}
-
-// Phase 1 over the servers with some window top > 0, margin_kernel, margin_tail and margin_fallback.  rate / lo /
-// hi [L*S] are the caller's rows (rate NULL: the fleet's own column); rec ([3*L*S]) is a device block; the other
-// columns are in h->d_iv at mc's offsets.
-//
-// With `trace` (wva_load_margin_trace, DESIGN.md §3.21) row t is tick t against c_t.  Phase 1 then honours
-// keepAccelerator on the pinned servers only (trace_pinned): an unpinned server's chain can lift the mask at a later
-// tick.  margin_chain writes c_t into mc's columns before the margin kernels read them through at_tick.
-int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* lo, const float* hi,
-                         const MarginCols& mc, const AllocCols& rec, size_t rec_bytes, bool trace) {
+// The first half of a walk call over n = L * S windows lo / hi [n] (rows of S), whose device lists the caller has
+// begun to place in c: phase 1 over the servers with some window top > 0, on a trace honouring keepAccelerator on
+// the pinned servers only (trace_pinned); the record block g.rec (rec_bytes) zeroed, so that a record the walk does
+// not write reads back as zero bytes; and the rest of g, whose records and work list (item, cap) the caller has set.
+int enqueue_walk_star(wva_handle* h, Cols& c, int L, const float* lo, const float* hi, bool trace, size_t rec_bytes,
+                      WalkArgs& g, LoadStar& ls) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A, n = S * L;
     std::vector<char> loaded(S, 0);
     for (int i = 0; i < n; ++i) loaded[i % S] |= hi[i] > 0.0f;
     const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
     std::vector<int> pairs;
-    Cols c(16);
-    RowLists lists{hf, L, c};
-    lists.put_rpm(rate);
     const size_t o_lo = c.put(lo, 4 * (size_t)n), o_hi = c.put(hi, 4 * (size_t)n), o_cop = c.take(4 * (size_t)S * A);
     int rc = prepare_load_star(
         h, hf, loaded, pairs, c,
@@ -1255,40 +1152,124 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* l
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
-    // below and above are zero bytes where the walk writes none
-    if (n > 0) CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
-    LoadStar ls;
-    rc = enqueue_load_star(h, hf, h->df, 3ll * n, ls);
+    if (g.items.cap > 0) CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
+    rc = enqueue_load_star(h, hf, h->df, g.items.cap, ls);
     if (rc) return rc;
-    if (n == 0) return WVA_OK;
     const char* dl = (const char*)h->lg_tabs.lists.p;
-    char* d = (char*)h->d_iv.p;
-    MarginArgs g{};
     g.ld = load_args(h, ls);
     g.cand_of_pair = (const int*)(dl + o_cop);
-    g.rate = lists.rpm.dev(dl);
     g.lo = (const float*)(dl + o_lo);
     g.hi = (const float*)(dl + o_hi);
-    g.n = n;
-    g.lo_out = (float*)(d + mc.o_lo);
-    g.hi_out = (float*)(d + mc.o_hi);
-    g.flags = (uint8_t*)(d + mc.o_flags);
-    g.rec = rec;
-    g.items = FbList{(int*)h->d_ctrl.p + CTRL_COUNTER, (unsigned long long*)(d + mc.o_items), 3 * n};
+    g.items.count = (int*)h->d_ctrl.p + CTRL_COUNTER;
     g.status = (int*)h->d_ctrl.p + CTRL_FB_STATUS;
-    if (!trace) return launch_margins<false>(h, g, ls);
-    g.cur_acc = (int*)(d + mc.o_cur_acc);
-    g.cur_replicas = (int*)(d + mc.o_cur_rep);
-    g.cur_cost = (float*)(d + mc.o_cur_cost);
+    return WVA_OK;
+}
+
+// The walk kernel over `warps` items, one warp each with per_warp bytes of dynamic shared memory (refused with
+// `what` where that does not fit a block), its tail over g's work list, ev_k1 (the call's kernel time: phase 1, a
+// trace's chain and the walk kernels) and the re-run of the tail's bails (fallback over fb).
+template <class Args>
+int launch_walk(wva_handle* h, void (*walk)(Args), void (*tail)(Args), void (*fallback)(Args, FbRun), const Args& g,
+                int warps, size_t per_warp, const char* what, const FbRun& fb) {
+    int wpb = 0;
+    size_t smem = 0;
+    const int rc = warp_layout(h, walk, per_warp, what, wpb, smem);
+    if (rc) return rc;
+    walk<<<(unsigned)((warps + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    const long long tail_blocks = std::min<long long>((long long)h->sm_count * 8, ((long long)g.items.cap + 255) / 256);
+    tail<<<(unsigned)tail_blocks, 256, 0, h->stream>>>(g);
+    h->launches += 2;
+    CK(cudaEventRecord(h->ev_k1, h->stream));
+    launch_fallback(h, fallback, g, fb);
+    CK(cudaGetLastError());
+    return WVA_OK;
+}
+
+// The end of a walk call from the upload on.  The call's device columns `cols` and then the work list [n_rec] live
+// in h->d_iv, and the columns taken with a host destination come back to it; the n_rec records form one candidate
+// block, copied back with `copy`.  enqueue(w, d, rec_bytes) runs under run_host, with d = h->d_iv.p and w the walk
+// arguments' records and work list.  The block then goes back as recs.size() lists of equal length, one per entry.
+template <class Enqueue>
+int run_walk(wva_handle* h, const wva_fleet* fleet, Cols& cols, size_t n_rec, bool copy,
+             std::initializer_list<const wva_allocs*> recs, Enqueue&& enqueue) {
+    CK(cudaSetDevice(h->device));
+    int rc = upload_fleet(h, fleet);
+    if (rc) return rc;
+    const size_t o_items = cols.take(8 * n_rec);
+    CK(h->d_iv.ensure(cols.bytes));
+    char* d = (char*)h->d_iv.p;
+    HostCall c{n_rec, copy, false, &cols, d};
+    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
+        WalkArgs w{};
+        w.rec = dc;
+        w.items = FbList{nullptr, (unsigned long long*)(d + o_items), (int)n_rec};
+        return enqueue(w, d, c.bc.bytes);
+    });
+    // no single solution to summarise (upload_fleet cleared last_kind)
+    if (rc) return rc;
+    size_t k = 0;
+    if (copy)
+        for (const wva_allocs* r : recs) scatter_block(c.cand_host, sub_block(c.bc, k++, n_rec / recs.size()), r);
+    return WVA_OK;
+}
+
+// ---- load intervals: where each server's load-grid winner changes in [lo, hi] ---------------------------------
+// Phase 1 over the servers with hi > 0, interval_kernel, interval_tail and interval_fallback.  lo / hi [S] are the
+// caller's bounds; g holds the call's device output columns, records and work list.
+int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, IntervalArgs& g, size_t rec_bytes) {
+    const int S = h->hf.S;
+    Cols c(16);
+    LoadStar ls;
+    int rc = enqueue_walk_star(h, c, 1, lo, hi, false, rec_bytes, g, ls);
+    if (rc) return rc;
+    // starts past a server's count read back as zero
+    CK(cudaMemsetAsync(g.start, 0, 4 * (size_t)S * g.M, h->stream));
+    if (S == 0) return WVA_OK;
+    // one warp per server, A accelerator states per warp in shared memory
+    return launch_walk(h, interval_kernel, interval_tail, interval_fallback, g, S, sizeof(IvAcc) * (size_t)h->hf.A,
+                       "too many accelerators for the interval kernel's shared memory", ls.fb2);
+}
+
+// ---- load margins: the stretch around each level's rate on which the load-grid winner keeps its decision -------
+static_assert(MG_LO_OPEN == WVA_MARGIN_LO_OPEN && MG_HI_OPEN == WVA_MARGIN_HI_OPEN &&
+              MG_TRUNCATED == WVA_MARGIN_TRUNCATED, "margin flags");
+
+// margin_kernel, margin_tail and margin_fallback of g (the Trace instantiations on a trace): one warp per (level,
+// server), A accelerator states and stretch starts per warp in shared memory.
+template <bool Trace>
+int launch_margins(wva_handle* h, const MarginArgs& g, const FbRun& fb) {
+    return launch_walk(h, margin_kernel<Trace>, margin_tail<Trace>, margin_fallback<Trace>, g, g.n,
+                       (sizeof(IvAcc) + sizeof(float)) * (size_t)h->hf.A,
+                       "too many accelerators for the margin kernel's shared memory", fb);
+}
+
+// Phase 1 over the servers with some window top > 0, then the margin kernels.  rate / lo / hi [L*S] are the caller's
+// rows (rate NULL: the fleet's own column); g holds the call's device output columns, records and work list.
+//
+// With `trace` (wva_load_margin_trace, DESIGN.md §3.21) row t is tick t against c_t.  Phase 1 then honours
+// keepAccelerator on the pinned servers only (trace_pinned): an unpinned server's chain can lift the mask at a later
+// tick.  margin_chain writes c_t into g's c_t columns before the margin kernels read them through at_tick.
+int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* lo, const float* hi, MarginArgs& g,
+                         size_t rec_bytes, bool trace) {
+    const HostFleet& hf = h->hf;
+    Cols c(16);
+    RowLists lists{hf, L, c};
+    lists.put_rpm(rate);
+    LoadStar ls;
+    int rc = enqueue_walk_star(h, c, L, lo, hi, trace, rec_bytes, g, ls);
+    if (rc) return rc;
+    if (g.n == 0) return WVA_OK;
+    g.rate = lists.rpm.dev((const char*)h->lg_tabs.lists.p);
+    if (!trace) return launch_margins<false>(h, g, ls.fb2);
     // one warp per server, A accelerator states per warp in shared memory
     int wpb = 0;
     size_t smem = 0;
-    rc = warp_layout(h, margin_chain, sizeof(IvAcc) * (size_t)A,
+    rc = warp_layout(h, margin_chain, sizeof(IvAcc) * (size_t)hf.A,
                      "too many accelerators for the margin chain's shared memory", wpb, smem);
     if (rc) return rc;
-    margin_chain<<<(unsigned)((S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    margin_chain<<<(unsigned)((hf.S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
     h->launches++;
-    return launch_margins<true>(h, g, ls);
+    return launch_margins<true>(h, g, ls.fb2);
 }
 
 // wva_load_margins, or with `trace` wva_load_margin_trace (which requires the rate rows)
@@ -1312,30 +1293,24 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
             lo > r || r > hi)
             return h->fail(WVA_ERR_BAD_ARG, "rate or window NaN, infinite or negative, or the rate outside its window");
     }
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    MarginCols mc;
-    mc.o_lo = mc.cols.take(4 * (size_t)n, out->lo_rpm);
-    mc.o_hi = mc.cols.take(4 * (size_t)n, out->hi_rpm);
-    mc.o_flags = mc.cols.take((size_t)n, out->flags);
-    mc.o_items = mc.cols.take(8 * 3 * (size_t)n);
-    if (trace) {
-        mc.o_cur_acc = mc.cols.take(4 * (size_t)n);
-        mc.o_cur_rep = mc.cols.take(4 * (size_t)n);
-        mc.o_cur_cost = mc.cols.take(4 * (size_t)n);
-    }
-    CK(h->d_iv.ensure(mc.cols.bytes));
-    HostCall c{3 * (size_t)n, n > 0, false, &mc.cols, h->d_iv.p};
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
-        return enqueue_load_margins(h, L, arrival_rpm, rpm_lo, rpm_hi, mc, dc, c.bc.bytes, trace);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    const wva_allocs* recs[3] = {&out->at, &out->below, &out->above};
-    if (n > 0)
-        for (int k = 0; k < 3; ++k) scatter_block(c.cand_host, sub_block(c.bc, k, n), recs[k]);
-    return WVA_OK;
+    Cols cols(16);
+    const size_t o_lo = cols.take(4 * (size_t)n, out->lo_rpm), o_hi = cols.take(4 * (size_t)n, out->hi_rpm),
+                 o_flags = cols.take((size_t)n, out->flags);
+    const size_t o_cur = trace ? cols.take(12 * (size_t)n) : 0;  // a trace's c_t: acc, replicas, cost [n] each
+    return run_walk(h, fleet, cols, 3 * (size_t)n, n > 0, {&out->at, &out->below, &out->above},
+                    [&](const WalkArgs& w, char* d, size_t rec_bytes) {
+                        MarginArgs g{w};
+                        g.n = n;
+                        g.lo_out = (float*)(d + o_lo);
+                        g.hi_out = (float*)(d + o_hi);
+                        g.flags = (uint8_t*)(d + o_flags);
+                        if (trace) {
+                            g.cur_acc = (int*)(d + o_cur);
+                            g.cur_replicas = (int*)(d + o_cur) + n;
+                            g.cur_cost = (float*)(d + o_cur) + 2 * (size_t)n;
+                        }
+                        return enqueue_load_margins(h, L, arrival_rpm, rpm_lo, rpm_hi, g, rec_bytes, trace);
+                    });
 }
 
 // ---- SLO grid: CreateAllocation and the unlimited winner at every listed (ITL, TTFT, TPS) target row -----------
@@ -3295,23 +3270,18 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
     for (int s = 0; s < S; ++s)
         if (!std::isfinite(rpm_lo[s]) || !std::isfinite(rpm_hi[s]) || rpm_lo[s] < 0.0f || !(rpm_lo[s] <= rpm_hi[s]))
             return h->fail(WVA_ERR_BAD_ARG, "bound NaN, infinite or negative, or rpm_lo above rpm_hi");
-    CK(cudaSetDevice(h->device));
-    int rc = upload_fleet(h, fleet);
-    if (rc) return rc;
-    IntervalCols iv;
-    iv.o_count = iv.cols.take(4 * (size_t)S, out->count);
-    iv.o_trunc = iv.cols.take((size_t)S, out->truncated);
-    iv.o_start = iv.cols.take(4 * (size_t)S * M, out->start_rpm);
-    iv.o_items = iv.cols.take(8 * (size_t)S * M);
-    CK(h->d_iv.ensure(iv.cols.bytes));
-    HostCall c{(size_t)S * M, true, false, &iv.cols, h->d_iv.p};
-    rc = run_host(h, c, [&](const AllocCols& dc, const AllocCols&) {
-        return enqueue_load_intervals(h, rpm_lo, rpm_hi, M, iv, dc, c.bc.bytes);
-    });
-    // no single solution to summarise (upload_fleet cleared last_kind)
-    if (rc) return rc;
-    scatter_block(c.cand_host, c.bc, &out->rec);
-    return WVA_OK;
+    Cols cols(16);
+    const size_t o_count = cols.take(4 * (size_t)S, out->count), o_trunc = cols.take((size_t)S, out->truncated),
+                 o_start = cols.take(4 * (size_t)S * M, out->start_rpm);
+    return run_walk(h, fleet, cols, (size_t)S * M, true, {&out->rec},
+                    [&](const WalkArgs& w, char* d, size_t rec_bytes) {
+                        IntervalArgs g{w};
+                        g.M = M;
+                        g.count = (int*)(d + o_count);
+                        g.truncated = (uint8_t*)(d + o_trunc);
+                        g.start = (float*)(d + o_start);
+                        return enqueue_load_intervals(h, rpm_lo, rpm_hi, g, rec_bytes);
+                    });
 }
 
 int wva_load_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,

@@ -1038,4 +1038,16 @@ __device__ __forceinline__ float transition_penalty(float factor, int cur_acc, i
     return __fadd_rn(__fmul_rn(factor, __fadd_rn(cur_cost, new_cost)), __fsub_rn(new_cost, cur_cost));
 }
 
+// The first bit pattern in (l, h] at which pred holds, given that it fails at l, holds at h and never fails again
+// once it holds: a bisection over float32 bit patterns, which are ordered like the values of one sign.
+template <class Pred>
+__device__ __forceinline__ unsigned bits_first(unsigned l, unsigned h, Pred&& pred) {
+    while (h - l > 1u) {
+        const unsigned m = l + (h - l) / 2u;
+        if (pred(m)) h = m;
+        else l = m;
+    }
+    return h;
+}
+
 }  // namespace wva

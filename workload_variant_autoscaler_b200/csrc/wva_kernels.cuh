@@ -1998,14 +1998,8 @@ __global__ void __launch_bounds__(128) price_kernel(PriceArgs g) {
             };
             if (wins(max_bits)) {
                 t = __int_as_float(0x7f800000);
-            } else if (wins(0u)) {
-                unsigned lo = 0u, hi = max_bits;  // a wins at lo, not at hi
-                while (hi - lo > 1u) {
-                    const unsigned mid = lo + (hi - lo) / 2u;
-                    if (wins(mid)) lo = mid;
-                    else hi = mid;
-                }
-                t = __uint_as_float(hi);
+            } else if (wins(0u)) {  // a wins at 0, not at max_bits: the first price at which it stops winning
+                t = __uint_as_float(bits_first(0u, max_bits, [&](unsigned bits) { return !wins(bits); }));
             }
         }
         threshold[i] = t;

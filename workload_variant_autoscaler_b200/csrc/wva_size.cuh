@@ -1237,18 +1237,13 @@ __device__ __forceinline__ int bounds_rank(float y0, float y1, bool rising, floa
     return rising ? cls : 2 - cls;
 }
 // The smallest positive float32 target (bits 1 .. 0x7f800000 = +Inf) of rank >= k, or NaN when +Inf's rank is
-// below k: a bisection over the bit patterns, which are ordered like the values.
+// below k: a bisection over the bit patterns.
 __device__ __forceinline__ float bounds_first(float y0, float y1, bool rising, int k) {
     const unsigned inf = 0x7f800000u;
-    if (bounds_rank(y0, y1, rising, __uint_as_float(inf)) < k) return __uint_as_float(0x7fc00000u);
-    if (bounds_rank(y0, y1, rising, __uint_as_float(1u)) >= k) return __uint_as_float(1u);
-    unsigned lo = 1u, hi = inf;  // rank(lo) < k <= rank(hi)
-    while (hi - lo > 1u) {
-        const unsigned mid = lo + (hi - lo) / 2u;
-        if (bounds_rank(y0, y1, rising, __uint_as_float(mid)) >= k) hi = mid;
-        else lo = mid;
-    }
-    return __uint_as_float(hi);
+    const auto reaches = [&](unsigned bits) { return bounds_rank(y0, y1, rising, __uint_as_float(bits)) >= k; };
+    if (!reaches(inf)) return __uint_as_float(0x7fc00000u);
+    if (reaches(1u)) return __uint_as_float(1u);
+    return __uint_as_float(bits_first(1u, inf, reaches));
 }
 
 // One thread per (pair, search) entry (s * A + a) * 2 + which.
@@ -1288,18 +1283,22 @@ __global__ void __launch_bounds__(256) bounds_kernel(BoundsArgs g) {
 // winner's key changes; interval_tail then runs the load grid's tail (load_tail) at every interval start whose
 // winner is a load pair, and interval_fallback re-runs the items it bailed on.
 // ---------------------------------------------------------------------------
-struct IntervalArgs {
+// What the walks (the load intervals and the load margins) and their tails share.
+struct WalkArgs {
     LoadArgs ld;               // phase 1's candidates and rateStar records (level_rpm, L and cand unused)
     const int* cand_of_pair;   // [S * A] the pair's index in ld's candidate list, -1: not a load candidate
-    const float* lo;           // [S] range bounds (req/min)
+    const float* lo;           // the windows (req/min), one row of S per level
     const float* hi;
+    AllocCols rec;             // the records
+    FbList items;              // the tail's work list: fb_pack(accelerator, record)
+    int* status;               // set when a window holds a rate at which a pair has 0 replicas (see iv_advance)
+};
+
+struct IntervalArgs : WalkArgs {  // one row of windows; rec [S * M]
     int M;                     // intervals per server
     int* count;                // [S]
     uint8_t* truncated;        // [S]
     float* start;              // [S * M]
-    AllocCols rec;             // [S * M]
-    FbList items;              // interval_tail's work list: fb_pack(accelerator, record)
-    int* status;               // set when a pair has 0 replicas at a positive rate (see iv_advance)
 };
 
 // A pair's state at one rate: the key is a function of (nrep, gate), and over marks a replica count beyond
@@ -1344,13 +1343,26 @@ __device__ __forceinline__ IvState iv_state(const DevFleet& f, int s, int a, con
     return st;
 }
 
-// Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.  g is the call's
-// IntervalArgs or MarginArgs; the window of x is row `row` of its bound lists g.lo / g.hi (the load intervals have
-// one row).  f is the fleet the key is taken on: g.ld.f, or on a margin trace the row's view at_tick.  With hi = x it
-// returns right after the key.
-template <class Args>
-__device__ __forceinline__ void iv_advance(const Args& g, const DevFleet& f, int row, int s, int a, float x, float hi,
-                                           IvAcc& p) {
+// Narrows a bisection for pred's first hold in (l, h] to the +-64-ulp bracket around est's float32 when pred fails at
+// the bracket's bottom (or that is l) and holds at its top (or that is h, where top_known says it holds).  Returns
+// whether it did; a bracket that does not check out leaves (l, h] alone, so the bisection finds the same point.
+template <class Pred>
+__device__ __forceinline__ bool ulp_bracket(double est, bool top_known, unsigned& l, unsigned& h, Pred&& pred) {
+    const unsigned e = __float_as_uint(__double2float_rn(est));
+    const unsigned bl = e > l && e - l > 64 ? e - 64 : l, bh = e < h && h - e > 64 ? e + 64 : h;
+    if (est < 3.0e38 && bl < bh && (bl == l || !pred(bl)) && ((top_known && bh == h) || pred(bh))) {
+        l = bl;
+        h = bh;
+        return true;
+    }
+    return false;
+}
+
+// Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.  The window of x is row
+// `row` of the bound lists g.lo / g.hi (the load intervals have one row).  f is the fleet the key is taken on: g.ld.f,
+// or on a margin trace the row's view at_tick.  With hi = x it returns right after the key.
+__device__ __forceinline__ void iv_advance(const WalkArgs& g, const DevFleet& f, int row, int s, int a, float x,
+                                           float hi, IvAcc& p) {
     const float inf = __int_as_float(0x7f800000);
     // the class at x: pair_class reads only whether the rate is negative or zero, and lo is 0 when x = 0
     const int cls = pair_class(at_level(f, x == 0.0f ? g.lo : g.hi, row), s, a, true);
@@ -1386,32 +1398,16 @@ __device__ __forceinline__ void iv_advance(const Args& g, const DevFleet& f, int
     unsigned l = __float_as_uint(x), h = __float_as_uint(hi);
     if (h <= l) return;
     // The step is within a few ulps of 60 * nrep * rateStar (the count grows) or 60 * nrep * RateRange.Max (the
-    // rate check starts rejecting): when a bracket of +-64 ulps around the nearer estimate holds it, bisect there;
-    // otherwise over the whole range.  Either way the result is the predicate's first flip.
-    if (at.nrep >= 1) {
+    // rate check starts rejecting): bisect in the bracket around the nearer estimate when it holds the step;
+    // otherwise over the whole range, when that holds one.
+    bool bracketed = false;
+    if (at.nrep >= 1 && at.gate != 0) {
         double est = 60.0 * (double)at.nrep * (double)p.rate_star;
         if (at.gate == 1) est = fmin(est, 60.0 * (double)at.nrep * (double)p.rmax);
-        const unsigned e = __float_as_uint(__double2float_rn(est));
-        const unsigned bl = e > l && e - l > 64 ? e - 64 : l, bh = e < h && h - e > 64 ? e + 64 : h;
-        if (at.gate != 0 && est < 3.0e38 && bl < bh && (bl == l || !differs(bl)) && differs(bh)) {
-            l = bl;
-            h = bh;
-        } else if (!differs(h)) {
-            return;
-        }
-    } else if (!differs(h)) {
-        return;
+        bracketed = ulp_bracket(est, false, l, h, differs);
     }
-    while (h - l > 1) {
-        const unsigned m = l + (h - l) / 2;
-        if (differs(m)) h = m;
-        else l = m;
-    }
-    p.next = __uint_as_float(h);
-}
-template <class Args>
-__device__ __forceinline__ void iv_advance(const Args& g, int row, int s, int a, float x, float hi, IvAcc& p) {
-    iv_advance(g, g.ld.f, row, s, a, x, hi, p);
+    if (!bracketed && !differs(h)) return;
+    p.next = __uint_as_float(bits_first(l, h, differs));
 }
 
 // SolveUnlimited over the warp's accelerators: strict '<' from MaxFloat32, ties to the lower accelerator id.
@@ -1443,6 +1439,38 @@ __device__ __forceinline__ bool iv_same_key(const Cand& x, const Cand& y) {
            __float_as_uint(x.max_rate) == __float_as_uint(y.max_rate);
 }
 
+// The warp's least and greatest v.
+__device__ __forceinline__ float warp_fmin(float v) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, d));
+    return v;
+}
+__device__ __forceinline__ float warp_fmax(float v) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, d));
+    return v;
+}
+
+// One step up the union of the warp's pair steps: nx, the least next step of the warp's accelerators, and where
+// nx <= hi the pairs that step there advanced to it (advance(a, nx)), after which `over` is set on every lane when
+// some pair of the warp is over.  Returns nx.
+template <class Advance>
+__device__ __forceinline__ float iv_step(const IvAcc* acc, int A, int lane, float hi, bool& over, Advance&& advance) {
+    float nx = __int_as_float(0x7f800000);
+    for (int a = lane; a < A; a += 32) nx = fminf(nx, acc[a].next);
+    nx = warp_fmin(nx);
+    if (!(nx <= hi)) return nx;
+    __syncwarp();
+    for (int a = lane; a < A; a += 32)
+        if (acc[a].next == nx) {
+            advance(a, nx);
+            over |= acc[a].over;
+        }
+    __syncwarp();
+    over = __any_sync(0xffffffffu, over);
+    return nx;
+}
+
 // One warp per server; the accelerators' state lives in dynamic shared memory (A entries per warp).
 __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     extern __shared__ IvAcc iv_acc[];
@@ -1453,14 +1481,15 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     IvAcc* acc = iv_acc + (size_t)wid * A;
     const float hi = g.hi[s];
     float x = g.lo[s];
-    bool over = false;
+    auto advance = [&](int a, float y) { iv_advance(g, f, 0, s, a, y, hi, acc[a]); };
+    bool truncated = false;
     for (int a = lane; a < A; a += 32) {
-        iv_advance(g, 0, s, a, x, hi, acc[a]);
-        over |= acc[a].over;
+        advance(a, x);
+        truncated |= acc[a].over;
     }
     __syncwarp();
     int n = 0;
-    bool truncated = __any_sync(0xffffffffu, over);  // a pair needs more than INT32_MAX replicas at lo
+    truncated = __any_sync(0xffffffffu, truncated);  // a pair needs more than INT32_MAX replicas at lo
     Cand prev = cand_nil();
     while (!truncated) {
         const int w = iv_winner(acc, A, lane);
@@ -1479,19 +1508,9 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
             prev = key;
             ++n;
         }
-        float nx = __int_as_float(0x7f800000);
-        for (int a = lane; a < A; a += 32) nx = fminf(nx, acc[a].next);
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) nx = fminf(nx, __shfl_xor_sync(0xffffffffu, nx, d));
+        // the list ends below the first rate that overflows
+        const float nx = iv_step(acc, A, lane, hi, truncated, advance);
         if (!(nx <= hi)) break;
-        __syncwarp();
-        for (int a = lane; a < A; a += 32)
-            if (acc[a].next == nx) {
-                iv_advance(g, 0, s, a, nx, hi, acc[a]);
-                over |= acc[a].over;
-            }
-        __syncwarp();
-        truncated = __any_sync(0xffffffffu, over);  // the list ends below the first rate that overflows
         x = nx;
     }
     if (lane == 0) {
@@ -1500,27 +1519,38 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     }
 }
 
-// The item fb_pack(a, r): the record r at an interval start whose winner is the load pair of accelerator a, the load
-// grid's tail at that rate, then the value.
+// Item fb_pack(a, r) of a walk's work list: record r, whose winner is the load pair of accelerator a of server s, is
+// the load grid's tail at rate x, then the value against the fleet fleet() returns.
+template <class Fleet, class Solve>
+__device__ __forceinline__ bool walk_load_tail(const WalkArgs& g, unsigned long long item, int s, float x,
+                                               Fleet&& fleet, Solve&& solve, Cand& out) {
+    const DevFleet& f = g.ld.f;
+    const int e = g.cand_of_pair[s * f.A + (int)(item >> 32)];
+    if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, x); }, solve, out)) return false;
+    if (out.feasible) out.value = penalty_of(fleet(), s, out);
+    return true;
+}
+
+// A walk's tail kernel: eval over the work list, grid-stride.
+template <class Eval>
+__device__ __forceinline__ void walk_tail(const WalkArgs& g, const Eval& eval) {
+    const int n = min(*g.items.count, g.items.cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        tail_item(g.ld.fb, g.rec, g.items.item[i], eval);
+}
+
+// The record r at an interval start.
 struct IvTail {
     const IntervalArgs& g;
     template <class Solve>
     __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
-        const DevFleet& f = g.ld.f;
-        const int r = (int)(unsigned)item, a = (int)(item >> 32), s = r / g.M;
-        const int e = g.cand_of_pair[s * f.A + a];
-        if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, g.start[r]); }, solve, out)) return false;
-        if (out.feasible) out.value = penalty_of(f, s, out);
-        return true;
+        const int r = (int)(unsigned)item;
+        return walk_load_tail(g, item, r / g.M, g.start[r], [&]() -> const DevFleet& { return g.ld.f; }, solve, out);
     }
     __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
 };
 
-__global__ void __launch_bounds__(256) interval_tail(IntervalArgs g) {
-    const int n = min(*g.items.count, g.items.cap);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-        tail_item(g.ld.fb, g.rec, g.items.item[i], IvTail{g});
-}
+__global__ void __launch_bounds__(256) interval_tail(IntervalArgs g) { walk_tail(g, IvTail{g}); }
 
 // Stored-vector re-run of the interval starts interval_tail bailed on.
 __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec, IvTail{g}); }
@@ -1541,19 +1571,12 @@ __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec
 // ---------------------------------------------------------------------------
 enum { MG_LO_OPEN = 1, MG_HI_OPEN = 2, MG_TRUNCATED = 4 };  // the header's WVA_MARGIN_*
 
-struct MarginArgs {
-    LoadArgs ld;               // phase 1's candidates and rateStar records (level_rpm, L and cand unused)
-    const int* cand_of_pair;   // [S * A] the pair's index in ld's candidate list, -1: not a load candidate
+struct MarginArgs : WalkArgs {  // windows [n]; rec [3 * n]: at (k = 0), below (1), above (2), record k * n + i
     const float* rate;         // [n] the levels' rates, index l * S + s (req/min)
-    const float* lo;           // [n] the windows
-    const float* hi;
     int n;                     // L * S, with 3 * n < 2^31
     float* lo_out;             // [n]
     float* hi_out;             // [n]
     uint8_t* flags;            // [n]
-    AllocCols rec;             // [3 * n]: at (k = 0), below (1), above (2), record k * n + i
-    FbList items;              // margin_tail's work list: fb_pack(accelerator, record)
-    int* status;               // set when a window holds a rate at which a pair has 0 replicas (see iv_advance)
     int* cur_acc;              // [n] on a trace: c_t of item t * S + s, written by margin_chain (unused otherwise)
     int* cur_replicas;
     float* cur_cost;
@@ -1621,24 +1644,14 @@ __device__ __forceinline__ float mg_start(const DevFleet& f, int s, int a, IvAcc
     unsigned l = __float_as_uint(bottom), h = __float_as_uint(x);
     if (h <= l || same(l)) return bottom;
     // !same(l), same(h).  The start is within a few ulps of 60 * (nrep - 1) * rateStar (the count reached nrep) or,
-    // at a rate the check rejects, 60 * nrep * RateRange.Max (the rejection started): when a bracket of +-64 ulps
-    // around that estimate holds it, bisect there; otherwise over the whole range.
+    // at a rate the check rejects, 60 * nrep * RateRange.Max (the rejection started): bisect in the bracket around
+    // that estimate when it holds the start, otherwise over the whole range.
     if (at.nrep >= 1 && at.gate != 0) {
         double est = 60.0 * (double)(at.nrep - 1) * (double)p.rate_star;
         if (at.gate == 2) est = fmax(est, 60.0 * (double)at.nrep * (double)p.rmax);
-        const unsigned e = __float_as_uint(__double2float_rn(est));
-        const unsigned bl = e > l && e - l > 64 ? e - 64 : l, bh = e < h && h - e > 64 ? e + 64 : h;
-        if (est < 3.0e38 && bl < bh && (bl == l || !same(bl)) && (bh == h || same(bh))) {
-            l = bl;
-            h = bh;
-        }
+        ulp_bracket(est, true, l, h, same);
     }
-    while (h - l > 1) {
-        const unsigned m = l + (h - l) / 2;
-        if (same(m)) h = m;
-        else l = m;
-    }
-    return __uint_as_float(h);
+    return __uint_as_float(bits_first(l, h, same));
 }
 
 // Accelerator a of server s at rate 0 of row `row` (the window's bottom lo = 0): its zero-load record or nil, as
@@ -1702,24 +1715,14 @@ __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
     } else {
         // up: the union of the pairs' steps above r, as interval_kernel walks it
         for (;;) {
-            float nx = inf;
-            for (int a = lane; a < A; a += 32) nx = fminf(nx, acc[a].next);
-#pragma unroll
-            for (int d = 16; d > 0; d >>= 1) nx = fminf(nx, __shfl_xor_sync(0xffffffffu, nx, d));
+            const float nx = iv_step(acc, A, lane, hi, over, advance);
             if (!(nx <= hi)) {
                 flags |= MG_HI_OPEN;
                 hi_out = inf;
                 break;
             }
-            __syncwarp();
-            for (int a = lane; a < A; a += 32)
-                if (acc[a].next == nx) {
-                    advance(a, nx);
-                    over |= acc[a].over;
-                }
-            __syncwarp();
             hi_out = nx;
-            if (__any_sync(0xffffffffu, over)) {  // the stretch ends below the first rate that overflows
+            if (over) {  // the stretch ends below the first rate that overflows
                 flags |= MG_TRUNCATED;
                 break;
             }
@@ -1757,8 +1760,7 @@ __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
                 }
                 y = bottom;
                 for (int a = lane; a < A; a += 32) y = fmaxf(y, start[a]);
-#pragma unroll
-                for (int d = 16; d > 0; d >>= 1) y = fmaxf(y, __shfl_xor_sync(0xffffffffu, y, d));
+                y = warp_fmax(y);
                 // no pair changes its state in [bottom, x]: the stretch reaches the window's bottom
                 if (at_zero || (y == bottom && lo > 0.0f)) {
                     flags |= MG_LO_OPEN;
@@ -1776,33 +1778,23 @@ __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
     }
 }
 
-// The item fb_pack(a, k * n + i): record k of item i, whose winner is the load pair of accelerator a, the load
-// grid's tail at the record's rate (r, the float below lo_out, or hi_out), then the value (on a trace against c_t).
+// The record r = k * n + i: record k of item i, at the record's rate (r, the float below lo_out, or hi_out), its
+// value on a trace against c_t.
 template <bool Trace>
 struct MgTail {
     const MarginArgs& g;
     template <class Solve>
     __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
-        const DevFleet& f = g.ld.f;
-        const int r = (int)(unsigned)item, a = (int)(item >> 32), k = r / g.n, i = r - k * g.n, s = i % f.S;
+        const int r = (int)(unsigned)item, k = r / g.n, i = r - k * g.n, S = g.ld.f.S;
         const float x = k == 0 ? g.rate[i] : (k == 1 ? mg_below(g.lo_out[i]) : g.hi_out[i]);
-        const int e = g.cand_of_pair[s * f.A + a];
-        if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, x); }, solve, out)) return false;
-        if (out.feasible) {
-            if constexpr (Trace) out.value = penalty_of(at_tick(g, i / f.S), s, out);
-            else out.value = penalty_of(f, s, out);
-        }
-        return true;
+        if constexpr (Trace) return walk_load_tail(g, item, i % S, x, [&] { return at_tick(g, i / S); }, solve, out);
+        else return walk_load_tail(g, item, i % S, x, [&]() -> const DevFleet& { return g.ld.f; }, solve, out);
     }
     __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
 };
 
 template <bool Trace>
-__global__ void __launch_bounds__(256) margin_tail(MarginArgs g) {
-    const int n = min(*g.items.count, g.items.cap);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-        tail_item(g.ld.fb, g.rec, g.items.item[i], MgTail<Trace>{g});
-}
+__global__ void __launch_bounds__(256) margin_tail(MarginArgs g) { walk_tail(g, MgTail<Trace>{g}); }
 
 // Stored-vector re-run of the records margin_tail bailed on.
 template <bool Trace>
