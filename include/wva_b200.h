@@ -677,6 +677,55 @@ int wva_load_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks
                           const float *rpm_lo, const float *rpm_hi /* [L*S] windows, req/min */, wva_margins *out);
 
 /*
+ * Workload margins: wva_load_margins and wva_load_margin_trace at rows that carry their own token lengths, as the
+ * collector reports them on every tick (arrival rate, AvgInTokens, AvgOutTokens).  A reconcile loop can skip its
+ * re-solve while the load stays inside a row's stretch and the tokens stay the row's, and a planner sees how far the
+ * load of each row of a (rate, in, out) forecast may stray.  Without this call that takes one wva_load_margins per
+ * row, each re-uploading and re-sizing the fleet with its token columns rewritten.
+ *
+ * Rows are laid out as in wva_workload_grid: arrival_rpm, in_tokens, out_tokens, rpm_lo and rpm_hi are [L*S], index
+ * l*S + s, with L = n_levels or n_ticks, and so is every column of out.  arrival_rpm is required; a NULL token list
+ * is the fleet's own column at every row.
+ *   - Grid, level l.  Let f_l be the fleet with srv_arrival_rpm, srv_in_tokens and srv_out_tokens replaced by row
+ *     l.  Block l of lo_rpm, hi_rpm, flags, at, below and above is byte for byte wva_load_margins(f_l) with one
+ *     level: rate row l, window row l.  Together, the `at` blocks are wva_workload_grid's winners on the same rows.
+ *   - Trace, tick t.  Let f_t be that fleet with row t and srv_cur_* = c_t, the allocation wva_workload_trace
+ *     carries into tick t on the same (rate, in, out) rows.  Block t is byte for byte wva_load_margins(f_t) with one
+ *     level, and the `at` blocks are wva_workload_trace's winners.  A trace continues as wva_workload_trace's does:
+ *     ticks 0..L-1 equal ticks 0..k-1 followed by ticks k..L-1 on the fleet whose srv_cur_* hold c_k
+ *     (Fleet.apply_winners over the `at` blocks in Python).
+ *   - With both token lists NULL the result is byte for byte wva_load_margins (grid) or wva_load_margin_trace
+ *     (trace) on the same rate rows and windows.
+ * A new rate inside [lo_rpm, hi_rpm) keeps the row's decision when the new tokens equal the row's; the stretch says
+ * nothing about other tokens.
+ *
+ * Sizing (DESIGN.md §3.22): QueueAnalyzer.Size, lambda* and rateStar read the tokens but not the rate, so phase 1
+ * runs once per distinct (server, accelerator, in_tokens, out_tokens) over the rows whose window top rpm_hi is above
+ * 0 and whose tokens class a pair as a load (in_tokens >= 0, out_tokens >= 1); on a trace with keepAccelerator
+ * honoured on the pinned servers only, as wva_workload_trace does.  The walk then reads each row's tokens.
+ *
+ * Only unlimited mode is covered; fleet->unlimited and the capacities are not read, nor are srv_arrival_rpm and, where
+ * a token list is given, its column.  The fleet becomes resident, and wva_summarize returns WVA_ERR_STATE afterwards.
+ * Columns of at, below and above may be NULL (not written).  L == 0 and S == 0 are valid (nothing is written).
+ * WVA_ERR_BAD_ARG: L < 0, out NULL, arrival_rpm, rpm_lo, rpm_hi, lo_rpm, hi_rpm or flags NULL with S*L > 0, or a row
+ * that wva_load_margins refuses (NaN, infinite or negative, or the rate outside its window).  WVA_ERR_UNSUPPORTED:
+ * 3*S*L >= 2^31 (refused before the fleet is read); distinct keys x A >= 2^31; or, for the grid, exactly where
+ * wva_load_margins(f_l) refuses at some level l: a pair outside the queue-size rule at row l's out_tokens, a rescale
+ * loop that would not terminate, too many stored-vector fallbacks, or a window holding a positive rate below
+ * 60 * 2^-150 req/min on a server with a min_replicas-0 load pair.  A token pair used only at rows whose window is
+ * [0, 0] is never sized and does not fail the call.  The trace's refusals can be larger than the union over t of what
+ * wva_load_margins(f_t) refuses, but only through the pairs of a server that is not pinned yet has keepAccelerator
+ * set, at ticks where the chain keeps them masked.  The call never returns a result that differs from the per-row
+ * composition.
+ */
+int wva_workload_margins(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
+                         const int32_t *in_tokens, const int32_t *out_tokens,
+                         const float *rpm_lo, const float *rpm_hi, wva_margins *out);
+int wva_workload_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                              const int32_t *in_tokens, const int32_t *out_tokens,
+                              const float *rpm_lo, const float *rpm_hi, wva_margins *out);
+
+/*
  * Price thresholds: for each server s and accelerator a, the exact accelerator price at which s's unlimited
  * winner leaves a.  Let f(p) be the fleet with acc_cost[a] = p, solved in unlimited mode.
  *

@@ -17,7 +17,9 @@
 #include <cstring>
 #include <functional>
 #include <numeric>
+#include <optional>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/wva_b200.h"
@@ -1100,6 +1102,147 @@ int enqueue_load_grid(wva_handle* h, int L, const float* rpm, const AllocCols& c
     return WVA_OK;
 }
 
+// ---- token keys: the workload calls' distinct (server, in_tokens, out_tokens) rows (DESIGN.md §3.12) -----------
+// Which lengths of WVA_FLEET_COLUMNS are per server.
+#define WVA_PER_SERVER_A 0
+#define WVA_PER_SERVER_T 0
+#define WVA_PER_SERVER_MA 0
+#define WVA_PER_SERVER_S 1
+// ... per (model, accelerator): a key fleet of the profile grid has its own (own_ma).
+#define WVA_PER_MODEL_A 0
+#define WVA_PER_MODEL_T 0
+#define WVA_PER_MODEL_MA 1
+#define WVA_PER_MODEL_S 0
+
+// The fleet the workload grid sizes (DESIGN.md §3.12): row k is server srv[k] of the resident fleet at the key's
+// tokens, with a positive rate (phase 1 reads no rate; the tail reads the level's).  The A, T and M columns are the
+// resident fleet's.  On the device the server columns lie in an upload image of the caller's (place), and
+// view() points a copy of the resident DevFleet at them, so the resident arena is never written.  The profile grid
+// also gives the key fleet its own models (own_ma): M and the perf_* columns are then the key fleet's.
+struct KeyFleet {
+    HostFleet hf;
+    bool own_ma = false;
+    struct {
+#define KEY_OFFSET(abi, name, type, len) size_t name = 0;
+        WVA_FLEET_COLUMNS(KEY_OFFSET)
+#undef KEY_OFFSET
+    } off;
+    KeyFleet(const HostFleet& fleet, const std::vector<int>& srv, const std::vector<int>& in,
+             const std::vector<int>& out)
+        : hf(fleet) {
+        const size_t K = srv.size();
+        hf.S = (int)K;
+#define KEY_GATHER(abi, name, type, len)                                     \
+    if (WVA_PER_SERVER_##len) {                                              \
+        hf.name.resize(K);                                                   \
+        for (size_t k = 0; k < K; ++k) hf.name[k] = fleet.name[srv[k]];      \
+    }
+        WVA_FLEET_COLUMNS(KEY_GATHER)
+#undef KEY_GATHER
+        std::fill(hf.srv_arrival_rpm.begin(), hf.srv_arrival_rpm.end(), 1.0f);
+        hf.srv_in_tokens = in;
+        hf.srv_out_tokens = out;
+    }
+    void place(Cols& c) {
+#define KEY_PLACE(abi, name, type, len)                            \
+    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) \
+        off.name = c.put(hf.name.data(), sizeof(type) * hf.name.size());
+        WVA_FLEET_COLUMNS(KEY_PLACE)
+#undef KEY_PLACE
+    }
+    DevFleet view(DevFleet f, const char* d) const {
+        f.S = hf.S;
+        if (own_ma) f.M = hf.M;
+#define KEY_VIEW(abi, name, type, len) \
+    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) f.name = (const type*)(d + off.name);
+        WVA_FLEET_COLUMNS(KEY_VIEW)
+#undef KEY_VIEW
+        return f;
+    }
+};
+
+// The levels at which server s is a load under the rows rpm / in / out [L*S] (rate not negative and not 0, NaN and
+// +Inf included; in_tokens >= 0; out_tokens >= 1), as ((in << 32) | out, level) in `uses`, sorted; then
+// group(in, out, u0, u1) for each (in, out) in ascending order, whose levels are uses[u0 .. u1), ascending.
+template <class Group>
+void load_groups(int L, int S, int s, const float* rpm, const int32_t* in, const int32_t* out,
+                 std::vector<std::pair<uint64_t, int>>& uses, Group&& group) {
+    uses.clear();
+    for (int l = 0; l < L; ++l) {
+        const size_t i = (size_t)l * S + s;
+        if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1)
+            uses.emplace_back((uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], l);
+    }
+    std::sort(uses.begin(), uses.end());
+    for (size_t u0 = 0, u1; u0 < uses.size(); u0 = u1) {
+        for (u1 = u0; u1 < uses.size() && uses[u1].first == uses[u0].first;) ++u1;
+        group((int)(uses[u0].first >> 32), (int)(uint32_t)uses[u0].first, u0, u1);
+    }
+}
+
+// Key rows (server, in_tokens, out_tokens) with their levels: row k's are lev[lev_off[k] .. lev_off[k + 1]).  On
+// the device the workload grid's tail reads the servers, the level lists and each candidate's first item, which
+// lie in the call's upload image (place, write) and which args() hands to a WorkloadArgs.
+struct TokenKeys {
+    std::vector<int> srv, in, out, lev_off{0}, lev;
+    size_t o_srv = 0, o_loff = 0, o_lev = 0, o_item = 0;
+    int n_items = 0;  // set by write
+    void add(int s, int ki, int ko) {
+        srv.push_back(s);
+        in.push_back(ki);
+        out.push_back(ko);
+        lev_off.push_back(lev_off.back());
+    }
+    void add_level(int l) {
+        lev.push_back(l);
+        lev_off.back()++;
+    }
+    // the key rows, and room for the item offsets of up to n_cand candidates
+    void place(Cols& c, size_t n_cand) {
+        o_srv = c.put(srv.data(), 4 * srv.size());
+        o_loff = c.put(lev_off.data(), 4 * lev_off.size());
+        o_lev = c.put(lev.data(), 4 * lev.size());
+        o_item = c.take(4 * (n_cand + 1));
+    }
+    // candidate j's items: one per level of its key row pairs[j] / A
+    void write(char* p, const std::vector<int>& pairs, int A) {
+        int* item = (int*)(p + o_item);
+        item[0] = 0;
+        for (size_t j = 0; j < pairs.size(); ++j) {
+            const int k = pairs[j] / A;
+            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
+        }
+        n_items = item[pairs.size()];
+    }
+    // the tail's lists uploaded at d, for levels of S servers
+    WorkloadArgs args(const char* d, int S) const {
+        WorkloadArgs g{};
+        g.key_srv = (const int*)(d + o_srv);
+        g.lev_off = (const int*)(d + o_loff);
+        g.lev = (const int*)(d + o_lev);
+        g.item_off = (const int*)(d + o_item);
+        g.S = S;
+        g.n_items = n_items;
+        return g;
+    }
+};
+// The workload grid's keys (DESIGN.md §3.12) of the rows rpm / in / out into tk: per server, its distinct (in, out)
+// under load, ascending.  Returns their key fleet, which with pin (a trace's trace_pinned flags) keeps
+// keepAccelerator on the pinned servers only, so that phase 1 sizes their current accelerator alone.
+KeyFleet workload_keys(const HostFleet& hf, int L, const float* rpm, const int32_t* in, const int32_t* out,
+                       const uint8_t* pin, TokenKeys& tk) {
+    std::vector<std::pair<uint64_t, int>> uses;
+    for (int s = 0; s < hf.S; ++s)
+        load_groups(L, hf.S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
+            tk.add(s, ki, ko);
+            for (size_t u = u0; u < u1; ++u) tk.add_level(uses[u].second);
+        });
+    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
+    if (pin)
+        for (size_t k = 0; k < tk.srv.size(); ++k) kf.hf.srv_keep_acc[k] = pin[tk.srv[k]];
+    return kf;
+}
+
 // ---- walks: the load intervals and the load margins -----------------------------------------------------------
 // The servers whose accelerator no tick of a trace can change (DESIGN.md §3.13), as flags [S]: with keepAccelerator
 // and a current accelerator other than "" only that accelerator is a candidate, and its load and zero-load
@@ -1132,13 +1275,16 @@ int warp_layout(wva_handle* h, Kernel kernel, size_t per_warp, const char* what,
 // begun to place in c: phase 1 over the servers with some window top > 0, on a trace honouring keepAccelerator on
 // the pinned servers only (trace_pinned); the record block g.rec (rec_bytes) zeroed, so that a record the walk does
 // not write reads back as zero bytes; and the rest of g, whose records and work list (item, cap) the caller has set.
+// With kf (the workload margins), phase 1 runs on every row of that key fleet instead, whose keepAccelerator column
+// the caller has set, and whose columns it has placed in c; g.cand_of_pair then has K * A entries.
 int enqueue_walk_star(wva_handle* h, Cols& c, int L, const float* lo, const float* hi, bool trace, size_t rec_bytes,
-                      WalkArgs& g, LoadStar& ls) {
-    const HostFleet& hf = h->hf;
-    const int S = hf.S, A = hf.A, n = S * L;
-    std::vector<char> loaded(S, 0);
-    for (int i = 0; i < n; ++i) loaded[i % S] |= hi[i] > 0.0f;
-    const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
+                      WalkArgs& g, LoadStar& ls, const KeyFleet* kf = nullptr) {
+    const HostFleet& hf = kf ? kf->hf : h->hf;
+    const int S = hf.S, A = hf.A, n = h->hf.S * L;
+    std::vector<char> loaded(S, kf != nullptr);
+    if (!kf)
+        for (int i = 0; i < n; ++i) loaded[i % S] |= hi[i] > 0.0f;
+    const std::vector<uint8_t> pin = trace && !kf ? trace_pinned(hf) : std::vector<uint8_t>();
     std::vector<int> pairs;
     const size_t o_lo = c.put(lo, 4 * (size_t)n), o_hi = c.put(hi, 4 * (size_t)n), o_cop = c.take(4 * (size_t)S * A);
     int rc = prepare_load_star(
@@ -1148,14 +1294,14 @@ int enqueue_walk_star(wva_handle* h, Cols& c, int L, const float* lo, const floa
             std::fill(cop, cop + (size_t)S * A, -1);
             for (size_t j = 0; j < pairs.size(); ++j) cop[pairs[j]] = (int)j;
         },
-        trace ? pin.data() : nullptr);
+        pin.empty() ? nullptr : pin.data());
     if (rc) return rc;
     rc = ensure_ctrl(h);
     if (rc) return rc;
     if (g.items.cap > 0) CK(cudaMemsetAsync(h->d_cand_block.p, 0, rec_bytes, h->stream));
-    rc = enqueue_load_star(h, hf, h->df, g.items.cap, ls);
-    if (rc) return rc;
     const char* dl = (const char*)h->lg_tabs.lists.p;
+    rc = enqueue_load_star(h, hf, kf ? kf->view(h->df, dl) : h->df, g.items.cap, ls);
+    if (rc) return rc;
     g.ld = load_args(h, ls);
     g.cand_of_pair = (const int*)(dl + o_cop);
     g.lo = (const float*)(dl + o_lo);
@@ -1234,13 +1380,26 @@ int enqueue_load_intervals(wva_handle* h, const float* lo, const float* hi, Inte
 static_assert(MG_LO_OPEN == WVA_MARGIN_LO_OPEN && MG_HI_OPEN == WVA_MARGIN_HI_OPEN &&
               MG_TRUNCATED == WVA_MARGIN_TRUNCATED, "margin flags");
 
-// margin_kernel, margin_tail and margin_fallback of g (the Trace instantiations on a trace): one warp per (level,
-// server), A accelerator states and stretch starts per warp in shared memory.
-template <bool Trace>
-int launch_margins(wva_handle* h, const MarginArgs& g, const FbRun& fb) {
-    return launch_walk(h, margin_kernel<Trace>, margin_tail<Trace>, margin_fallback<Trace>, g, g.n,
-                       (sizeof(IvAcc) + sizeof(float)) * (size_t)h->hf.A,
-                       "too many accelerators for the margin kernel's shared memory", fb);
+// margin_kernel, margin_tail and margin_fallback of g (the Trace instantiations on a trace, after margin_chain): one
+// warp per (level, server), A accelerator states and stretch starts per warp in shared memory.  Args is MarginArgs,
+// or TokenMarginArgs for the workload margins.
+template <class Args>
+int launch_margins(wva_handle* h, const Args& g, bool trace, const FbRun& fb) {
+    const size_t per_warp = (sizeof(IvAcc) + sizeof(float)) * (size_t)h->hf.A;
+    const char* what = "too many accelerators for the margin kernel's shared memory";
+    if (!trace)
+        return launch_walk(h, margin_kernel<false>, margin_tail<false>, margin_fallback<false>, g, g.n, per_warp, what,
+                           fb);
+    // one warp per server, A accelerator states per warp in shared memory
+    void (*chain)(Args) = margin_chain;
+    int wpb = 0;
+    size_t smem = 0;
+    const int rc = warp_layout(h, chain, sizeof(IvAcc) * (size_t)h->hf.A,
+                               "too many accelerators for the margin chain's shared memory", wpb, smem);
+    if (rc) return rc;
+    chain<<<(unsigned)((h->hf.S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
+    h->launches++;
+    return launch_walk(h, margin_kernel<true>, margin_tail<true>, margin_fallback<true>, g, g.n, per_warp, what, fb);
 }
 
 // Phase 1 over the servers with some window top > 0, then the margin kernels.  rate / lo / hi [L*S] are the caller's
@@ -1248,33 +1407,58 @@ int launch_margins(wva_handle* h, const MarginArgs& g, const FbRun& fb) {
 //
 // With `trace` (wva_load_margin_trace, DESIGN.md §3.21) row t is tick t against c_t.  Phase 1 then honours
 // keepAccelerator on the pinned servers only (trace_pinned): an unpinned server's chain can lift the mask at a later
-// tick.  margin_chain writes c_t into g's c_t columns before the margin kernels read them through at_tick.
-int enqueue_load_margins(wva_handle* h, int L, const float* rate, const float* lo, const float* hi, MarginArgs& g,
-                         size_t rec_bytes, bool trace) {
+// tick.  margin_chain writes c_t into g's c_t columns before the margin kernels read them through mg_view.
+//
+// With `tokens` (the workload margins, DESIGN.md §3.22) row l also has its own tokens, in / out [L*S] (NULL: the
+// fleet's own column).  Size, lambda* and rateStar read the tokens but not the rate (§3.12), so phase 1 runs on the
+// workload calls' key fleet: one row per distinct (server, in, out) over the rows whose window top is above 0 and
+// whose tokens class a pair as a load (workload_keys with the window tops as its rates; on a trace with
+// keepAccelerator on the pinned servers only).  The key column [L*S] names each row's key (-1: none), and the
+// kernels read the rows' tokens through the row's view of the resident fleet.
+int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t* in, const int32_t* out, bool tokens,
+                         const float* lo, const float* hi, TokenMarginArgs& g, size_t rec_bytes, bool trace) {
     const HostFleet& hf = h->hf;
+    const int S = hf.S;
     Cols c(16);
     RowLists lists{hf, L, c};
     lists.put_rpm(rate);
+    TokenKeys tk;
+    std::optional<KeyFleet> kf;
+    std::vector<int> key;
+    size_t o_key = 0;
+    if (tokens) {
+        lists.put_tokens(in, out);
+        const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
+        kf.emplace(workload_keys(hf, L, hi, lists.in.host, lists.out.host, trace ? pin.data() : nullptr, tk));
+        // the keys' pairs are indexed in int32 on the device
+        if ((long long)tk.srv.size() * hf.A >= (1ll << 31))
+            return h->fail(WVA_ERR_UNSUPPORTED, "workload margins: too many token keys for one call (K*A >= 2^31)");
+        key.assign((size_t)L * S, -1);
+        for (size_t k = 0; k < tk.srv.size(); ++k)
+            for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j) key[(size_t)tk.lev[j] * S + tk.srv[k]] = (int)k;
+        o_key = c.put(key.data(), 4 * key.size());
+        kf->place(c);
+    }
     LoadStar ls;
-    int rc = enqueue_walk_star(h, c, L, lo, hi, trace, rec_bytes, g, ls);
+    int rc = enqueue_walk_star(h, c, L, lo, hi, trace, rec_bytes, g, ls, kf ? &*kf : nullptr);
     if (rc) return rc;
     if (g.n == 0) return WVA_OK;
-    g.rate = lists.rpm.dev((const char*)h->lg_tabs.lists.p);
-    if (!trace) return launch_margins<false>(h, g, ls.fb2);
-    // one warp per server, A accelerator states per warp in shared memory
-    int wpb = 0;
-    size_t smem = 0;
-    rc = warp_layout(h, margin_chain, sizeof(IvAcc) * (size_t)hf.A,
-                     "too many accelerators for the margin chain's shared memory", wpb, smem);
-    if (rc) return rc;
-    margin_chain<<<(unsigned)((hf.S + wpb - 1) / wpb), 32 * wpb, smem, h->stream>>>(g);
-    h->launches++;
-    return launch_margins<true>(h, g, ls.fb2);
+    const char* d = (const char*)h->lg_tabs.lists.p;
+    g.rate = lists.rpm.dev(d);
+    if (!tokens) return launch_margins(h, static_cast<const MarginArgs&>(g), trace, ls.fb2);
+    g.f = h->df;
+    g.key = (const int*)(d + o_key);
+    g.in_tokens = lists.in.dev(d);
+    g.out_tokens = lists.out.dev(d);
+    return launch_margins(h, g, trace, ls.fb2);
 }
 
-// wva_load_margins, or with `trace` wva_load_margin_trace (which requires the rate rows)
+// wva_load_margins, or with `trace` wva_load_margin_trace; with `tokens` wva_workload_margins or
+// wva_workload_margin_trace (in / out: NULL is the fleet's own column).  All but wva_load_margins require the rate
+// rows.
 int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
-                      const float* rpm_lo, const float* rpm_hi, wva_margins* out, bool trace) {
+                      const int32_t* in_tokens, const int32_t* out_tokens, bool tokens, const float* rpm_lo,
+                      const float* rpm_hi, wva_margins* out, bool trace) {
     if (!h) return WVA_ERR_BAD_ARG;
     if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
     if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, trace ? "negative tick count" : "negative level count");
@@ -1286,7 +1470,7 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
     const int n = S * L;
     if (n > 0 && (!rpm_lo || !rpm_hi || !out->lo_rpm || !out->hi_rpm || !out->flags))
         return h->fail(WVA_ERR_BAD_ARG, "NULL window or output column");
-    if (n > 0 && trace && !arrival_rpm) return h->fail(WVA_ERR_BAD_ARG, "NULL arrival rate rows");
+    if (n > 0 && (trace || tokens) && !arrival_rpm) return h->fail(WVA_ERR_BAD_ARG, "NULL arrival rate rows");
     for (int i = 0; i < n; ++i) {
         const float r = arrival_rpm ? arrival_rpm[i] : fleet->srv_arrival_rpm[i % S], lo = rpm_lo[i], hi = rpm_hi[i];
         if (!std::isfinite(r) || !std::isfinite(lo) || !std::isfinite(hi) || r < 0.0f || lo < 0.0f || hi < 0.0f ||
@@ -1299,7 +1483,7 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
     const size_t o_cur = trace ? cols.take(12 * (size_t)n) : 0;  // a trace's c_t: acc, replicas, cost [n] each
     return run_walk(h, fleet, cols, 3 * (size_t)n, n > 0, {&out->at, &out->below, &out->above},
                     [&](const WalkArgs& w, char* d, size_t rec_bytes) {
-                        MarginArgs g{w};
+                        TokenMarginArgs g{MarginArgs{w}};
                         g.n = n;
                         g.lo_out = (float*)(d + o_lo);
                         g.hi_out = (float*)(d + o_hi);
@@ -1309,7 +1493,8 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
                             g.cur_replicas = (int*)(d + o_cur) + n;
                             g.cur_cost = (float*)(d + o_cur) + 2 * (size_t)n;
                         }
-                        return enqueue_load_margins(h, L, arrival_rpm, rpm_lo, rpm_hi, g, rec_bytes, trace);
+                        return enqueue_load_margins(h, L, arrival_rpm, in_tokens, out_tokens, tokens, rpm_lo, rpm_hi,
+                                                    g, rec_bytes, trace);
                     });
 }
 
@@ -1508,64 +1693,6 @@ int enqueue_slo_grid(wva_handle* h, int L, const float* itl, const float* ttft, 
 }
 
 // ---- workload grid: CreateAllocation and the unlimited winner at every listed (rate, in, out) row --------------
-// Which lengths of WVA_FLEET_COLUMNS are per server.
-#define WVA_PER_SERVER_A 0
-#define WVA_PER_SERVER_T 0
-#define WVA_PER_SERVER_MA 0
-#define WVA_PER_SERVER_S 1
-// ... per (model, accelerator): a key fleet of the profile grid has its own (own_ma).
-#define WVA_PER_MODEL_A 0
-#define WVA_PER_MODEL_T 0
-#define WVA_PER_MODEL_MA 1
-#define WVA_PER_MODEL_S 0
-
-// The fleet the workload grid sizes (DESIGN.md §3.12): row k is server srv[k] of the resident fleet at the key's
-// tokens, with a positive rate (phase 1 reads no rate; the tail reads the level's).  The A, T and M columns are the
-// resident fleet's.  On the device the server columns lie in an upload image of the caller's (place), and
-// view() points a copy of the resident DevFleet at them, so the resident arena is never written.  The profile grid
-// also gives the key fleet its own models (own_ma): M and the perf_* columns are then the key fleet's.
-struct KeyFleet {
-    HostFleet hf;
-    bool own_ma = false;
-    struct {
-#define KEY_OFFSET(abi, name, type, len) size_t name = 0;
-        WVA_FLEET_COLUMNS(KEY_OFFSET)
-#undef KEY_OFFSET
-    } off;
-    KeyFleet(const HostFleet& fleet, const std::vector<int>& srv, const std::vector<int>& in,
-             const std::vector<int>& out)
-        : hf(fleet) {
-        const size_t K = srv.size();
-        hf.S = (int)K;
-#define KEY_GATHER(abi, name, type, len)                                     \
-    if (WVA_PER_SERVER_##len) {                                              \
-        hf.name.resize(K);                                                   \
-        for (size_t k = 0; k < K; ++k) hf.name[k] = fleet.name[srv[k]];      \
-    }
-        WVA_FLEET_COLUMNS(KEY_GATHER)
-#undef KEY_GATHER
-        std::fill(hf.srv_arrival_rpm.begin(), hf.srv_arrival_rpm.end(), 1.0f);
-        hf.srv_in_tokens = in;
-        hf.srv_out_tokens = out;
-    }
-    void place(Cols& c) {
-#define KEY_PLACE(abi, name, type, len)                            \
-    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) \
-        off.name = c.put(hf.name.data(), sizeof(type) * hf.name.size());
-        WVA_FLEET_COLUMNS(KEY_PLACE)
-#undef KEY_PLACE
-    }
-    DevFleet view(DevFleet f, const char* d) const {
-        f.S = hf.S;
-        if (own_ma) f.M = hf.M;
-#define KEY_VIEW(abi, name, type, len) \
-    if (WVA_PER_SERVER_##len || (own_ma && WVA_PER_MODEL_##len)) f.name = (const type*)(d + off.name);
-        WVA_FLEET_COLUMNS(KEY_VIEW)
-#undef KEY_VIEW
-        return f;
-    }
-};
-
 // The workload grid's tail (workload_kernel, then workload_fallback) after phase 1 (ls): g's key and level lists and
 // g.n_items items, at the rates level_rpm [L * g.S], into cand.  ev_k1 is recorded after workload_kernel: the
 // call's kernel time covers both phases.
@@ -1578,88 +1705,6 @@ int enqueue_workload_tail(wva_handle* h, const LoadStar& ls, WorkloadArgs& g, co
     g.ld.counter = (unsigned*)h->d_ctrl.p + CTRL_COUNTER;
     g.ld.cand = cand;
     return launch_tail(h, workload_kernel, workload_fallback, g, ((long long)g.n_items + 31) / 32, ls.fb2);
-}
-
-// The levels at which server s is a load under the rows rpm / in / out [L*S] (rate not negative and not 0, NaN and
-// +Inf included; in_tokens >= 0; out_tokens >= 1), as ((in << 32) | out, level) in `uses`, sorted; then
-// group(in, out, u0, u1) for each (in, out) in ascending order, whose levels are uses[u0 .. u1), ascending.
-template <class Group>
-void load_groups(int L, int S, int s, const float* rpm, const int32_t* in, const int32_t* out,
-                 std::vector<std::pair<uint64_t, int>>& uses, Group&& group) {
-    uses.clear();
-    for (int l = 0; l < L; ++l) {
-        const size_t i = (size_t)l * S + s;
-        if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1)
-            uses.emplace_back((uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], l);
-    }
-    std::sort(uses.begin(), uses.end());
-    for (size_t u0 = 0, u1; u0 < uses.size(); u0 = u1) {
-        for (u1 = u0; u1 < uses.size() && uses[u1].first == uses[u0].first;) ++u1;
-        group((int)(uses[u0].first >> 32), (int)(uint32_t)uses[u0].first, u0, u1);
-    }
-}
-
-// Key rows (server, in_tokens, out_tokens) with their levels: row k's are lev[lev_off[k] .. lev_off[k + 1]).  On
-// the device the workload grid's tail reads the servers, the level lists and each candidate's first item, which
-// lie in the call's upload image (place, write) and which args() hands to a WorkloadArgs.
-struct TokenKeys {
-    std::vector<int> srv, in, out, lev_off{0}, lev;
-    size_t o_srv = 0, o_loff = 0, o_lev = 0, o_item = 0;
-    int n_items = 0;  // set by write
-    void add(int s, int ki, int ko) {
-        srv.push_back(s);
-        in.push_back(ki);
-        out.push_back(ko);
-        lev_off.push_back(lev_off.back());
-    }
-    void add_level(int l) {
-        lev.push_back(l);
-        lev_off.back()++;
-    }
-    // the key rows, and room for the item offsets of up to n_cand candidates
-    void place(Cols& c, size_t n_cand) {
-        o_srv = c.put(srv.data(), 4 * srv.size());
-        o_loff = c.put(lev_off.data(), 4 * lev_off.size());
-        o_lev = c.put(lev.data(), 4 * lev.size());
-        o_item = c.take(4 * (n_cand + 1));
-    }
-    // candidate j's items: one per level of its key row pairs[j] / A
-    void write(char* p, const std::vector<int>& pairs, int A) {
-        int* item = (int*)(p + o_item);
-        item[0] = 0;
-        for (size_t j = 0; j < pairs.size(); ++j) {
-            const int k = pairs[j] / A;
-            item[j + 1] = item[j] + lev_off[k + 1] - lev_off[k];
-        }
-        n_items = item[pairs.size()];
-    }
-    // the tail's lists uploaded at d, for levels of S servers
-    WorkloadArgs args(const char* d, int S) const {
-        WorkloadArgs g{};
-        g.key_srv = (const int*)(d + o_srv);
-        g.lev_off = (const int*)(d + o_loff);
-        g.lev = (const int*)(d + o_lev);
-        g.item_off = (const int*)(d + o_item);
-        g.S = S;
-        g.n_items = n_items;
-        return g;
-    }
-};
-// The workload grid's keys (DESIGN.md §3.12) of the rows rpm / in / out into tk: per server, its distinct (in, out)
-// under load, ascending.  Returns their key fleet, which with pin (a trace's trace_pinned flags) keeps
-// keepAccelerator on the pinned servers only, so that phase 1 sizes their current accelerator alone.
-KeyFleet workload_keys(const HostFleet& hf, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                       const uint8_t* pin, TokenKeys& tk) {
-    std::vector<std::pair<uint64_t, int>> uses;
-    for (int s = 0; s < hf.S; ++s)
-        load_groups(L, hf.S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
-            tk.add(s, ki, ko);
-            for (size_t u = u0; u < u1; ++u) tk.add_level(uses[u].second);
-        });
-    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
-    if (pin)
-        for (size_t k = 0; k < tk.srv.size(); ++k) kf.hf.srv_keep_acc[k] = pin[tk.srv[k]];
-    return kf;
 }
 
 // QueueAnalyzer.Size, lambda* and rateStar read a server's tokens but not its rate (DESIGN.md §3.12), so phase 1
@@ -3286,12 +3331,24 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
 
 int wva_load_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                      const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_levels, arrival_rpm, rpm_lo, rpm_hi, out, false);
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, nullptr, nullptr, false, rpm_lo, rpm_hi, out, false);
 }
 
 int wva_load_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                           const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_ticks, arrival_rpm, rpm_lo, rpm_hi, out, true);
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, nullptr, nullptr, false, rpm_lo, rpm_hi, out, true);
+}
+
+int wva_workload_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                         const int32_t* in_tokens, const int32_t* out_tokens, const float* rpm_lo, const float* rpm_hi,
+                         wva_margins* out) {
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, rpm_lo, rpm_hi, out, false);
+}
+
+int wva_workload_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                              const int32_t* in_tokens, const int32_t* out_tokens, const float* rpm_lo,
+                              const float* rpm_hi, wva_margins* out) {
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, rpm_lo, rpm_hi, out, true);
 }
 
 int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold, wva_allocs* above,

@@ -1360,9 +1360,10 @@ __device__ __forceinline__ bool ulp_bracket(double est, bool top_known, unsigned
 
 // Accelerator a of server s at rate x (x = 0 or in (0, hi]): its key and its next step.  The window of x is row
 // `row` of the bound lists g.lo / g.hi (the load intervals have one row).  f is the fleet the key is taken on: g.ld.f,
-// or on a margin trace the row's view at_tick.  With hi = x it returns right after the key.
-__device__ __forceinline__ void iv_advance(const WalkArgs& g, const DevFleet& f, int row, int s, int a, float x,
-                                           float hi, IvAcc& p) {
+// or on a margin call the row's view (mg_view).  k is the row of g.ld that phase 1 sized the pair on: s, or on a
+// workload margin call the row's token key.  With hi = x it returns right after the key.
+__device__ __forceinline__ void iv_advance(const WalkArgs& g, const DevFleet& f, int row, int s, int k, int a,
+                                           float x, float hi, IvAcc& p) {
     const float inf = __int_as_float(0x7f800000);
     // the class at x: pair_class reads only whether the rate is negative or zero, and lo is 0 when x = 0
     const int cls = pair_class(at_level(f, x == 0.0f ? g.lo : g.hi, row), s, a, true);
@@ -1377,14 +1378,14 @@ __device__ __forceinline__ void iv_advance(const WalkArgs& g, const DevFleet& f,
         }
         return;
     }
-    const int e = g.cand_of_pair[s * f.A + a];
-    if (!g.ld.star_ok[s * f.A + a]) {  // nil at every load
+    const int e = g.cand_of_pair[k * f.A + a];
+    if (!g.ld.star_ok[k * f.A + a]) {  // nil at every load
         p.key = cand_nil();
         return;
     }
     p.tail = 1;
     p.N = g.ld.cand_N[e];
-    p.rate_star = g.ld.rate_star[s * f.A + a];
+    p.rate_star = g.ld.rate_star[k * f.A + a];
     p.rmax = rate_max_of((float)g.ld.tab[4 * (g.ld.tab_off[e] + p.N - 1)]);
     const IvState at = iv_state(f, s, a, p, x, &p.key);
     p.over = at.over;
@@ -1481,7 +1482,7 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     IvAcc* acc = iv_acc + (size_t)wid * A;
     const float hi = g.hi[s];
     float x = g.lo[s];
-    auto advance = [&](int a, float y) { iv_advance(g, f, 0, s, a, y, hi, acc[a]); };
+    auto advance = [&](int a, float y) { iv_advance(g, f, 0, s, s, a, y, hi, acc[a]); };
     bool truncated = false;
     for (int a = lane; a < A; a += 32) {
         advance(a, x);
@@ -1519,14 +1520,15 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
     }
 }
 
-// Item fb_pack(a, r) of a walk's work list: record r, whose winner is the load pair of accelerator a of server s, is
-// the load grid's tail at rate x, then the value against the fleet fleet() returns.
+// Item fb_pack(a, r) of a walk's work list: record r, whose winner is the load pair of accelerator a of server s,
+// sized on row k of g.ld (see iv_advance), is the load grid's tail at rate x, then the value against the fleet
+// fleet() returns.
 template <class Fleet, class Solve>
-__device__ __forceinline__ bool walk_load_tail(const WalkArgs& g, unsigned long long item, int s, float x,
+__device__ __forceinline__ bool walk_load_tail(const WalkArgs& g, unsigned long long item, int s, int k, float x,
                                                Fleet&& fleet, Solve&& solve, Cand& out) {
     const DevFleet& f = g.ld.f;
-    const int e = g.cand_of_pair[s * f.A + (int)(item >> 32)];
-    if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, s, x); }, solve, out)) return false;
+    const int e = g.cand_of_pair[k * f.A + (int)(item >> 32)];
+    if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, k, x); }, solve, out)) return false;
     if (out.feasible) out.value = penalty_of(fleet(), s, out);
     return true;
 }
@@ -1544,8 +1546,8 @@ struct IvTail {
     const IntervalArgs& g;
     template <class Solve>
     __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
-        const int r = (int)(unsigned)item;
-        return walk_load_tail(g, item, r / g.M, g.start[r], [&]() -> const DevFleet& { return g.ld.f; }, solve, out);
+        const int r = (int)(unsigned)item, s = r / g.M;
+        return walk_load_tail(g, item, s, s, g.start[r], [&]() -> const DevFleet& { return g.ld.f; }, solve, out);
     }
     __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
 };
@@ -1567,7 +1569,13 @@ __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec
 //
 // On a trace (DESIGN.md §3.21, the kernels' Trace instantiations) level t is tick t, solved against the current
 // allocation c_t that the workload trace carries into it.  margin_chain writes c_t of every (tick, server) first, and
-// every read of the current allocation then goes through at_tick's view of the fleet.
+// every read of the current allocation then goes through the row's view of the fleet (mg_view).
+//
+// The workload margins (DESIGN.md §3.22) give each row its own tokens.  The kernels then take a TokenMarginArgs:
+// phase 1 sized the rows' token keys, so ld.f is the key fleet and item i's pairs are those of its key row key[i];
+// the resident fleet is f, and every read of a server's rate, tokens or current allocation goes through the row's
+// view, which carries the row's tokens.  The kernels exist once per Trace, overloaded on the argument type, so the
+// load-only calls' kernels keep their names and code.
 // ---------------------------------------------------------------------------
 enum { MG_LO_OPEN = 1, MG_HI_OPEN = 2, MG_TRUNCATED = 4 };  // the header's WVA_MARGIN_*
 
@@ -1582,13 +1590,33 @@ struct MarginArgs : WalkArgs {  // windows [n]; rec [3 * n]: at (k = 0), below (
     float* cur_cost;
 };
 
-// The fleet of a trace's tick t: the resident fleet with the current allocation c_t.
-__device__ __forceinline__ DevFleet at_tick(const MarginArgs& g, int t) {
-    DevFleet ft = g.ld.f;
-    const size_t o = (size_t)t * g.ld.f.S;
-    ft.srv_cur_acc = g.cur_acc + o;
-    ft.srv_cur_replicas = g.cur_replicas + o;
-    ft.srv_cur_cost = g.cur_cost + o;
+struct TokenMarginArgs : MarginArgs {  // ld: phase 1 on the key fleet, one row per (server, in, out) key
+    DevFleet f;                // the resident fleet
+    const int* key;            // [n] item i's key row in ld, -1: none (window top 0, or tokens that are no load)
+    const int* in_tokens;      // [n] the rows' tokens, index l * S + s
+    const int* out_tokens;
+};
+
+// The resident fleet; item i's row in ld (phase 1's records), for server s; and row l's fleet without c_t.
+__device__ __forceinline__ const DevFleet& mg_fleet(const MarginArgs& g) { return g.ld.f; }
+__device__ __forceinline__ const DevFleet& mg_fleet(const TokenMarginArgs& g) { return g.f; }
+__device__ __forceinline__ int mg_key(const MarginArgs&, int, int s) { return s; }
+__device__ __forceinline__ int mg_key(const TokenMarginArgs& g, int i, int) { return g.key[i]; }
+__device__ __forceinline__ const DevFleet& mg_row(const MarginArgs& g, int) { return g.ld.f; }
+__device__ __forceinline__ DevFleet mg_row(const TokenMarginArgs& g, int l) {
+    return at_rows(g.f, LoadRows{nullptr, g.in_tokens, g.out_tokens}, l);
+}
+
+// The fleet of row l: on a trace with the current allocation c_t of tick t = l.
+template <bool Trace, class Args>
+__device__ __forceinline__ DevFleet mg_view(const Args& g, int l) {
+    DevFleet ft = mg_row(g, l);
+    if constexpr (Trace) {
+        const size_t o = (size_t)l * mg_fleet(g).S;
+        ft.srv_cur_acc = g.cur_acc + o;
+        ft.srv_cur_replicas = g.cur_replicas + o;
+        ft.srv_cur_cost = g.cur_cost + o;
+    }
     return ft;
 }
 
@@ -1598,9 +1626,10 @@ __device__ __forceinline__ DevFleet at_tick(const MarginArgs& g, int t) {
 // ties to the lower accelerator id); c_{t+1} is the winner's (acc, replicas, cost) when there is one, c_t otherwise
 // (Server.ApplyDesiredAlloc).  Those key columns are the ones margin_tail writes into `at`, so the chain needs no
 // latency solve.  Launched with up to 128 threads; A IvAcc states per warp in dynamic shared memory.
-__global__ void __launch_bounds__(128) margin_chain(MarginArgs g) {
+template <class Args>
+__device__ __forceinline__ void mg_chain(const Args& g) {
     extern __shared__ IvAcc iv_acc[];
-    const DevFleet& f = g.ld.f;
+    const DevFleet& f = mg_fleet(g);
     const int A = f.A, S = f.S, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int s = blockIdx.x * (blockDim.x >> 5) + wid;
     if (s >= S) return;
@@ -1616,9 +1645,10 @@ __global__ void __launch_bounds__(128) margin_chain(MarginArgs g) {
             g.cur_cost[i] = cur_cost;
         }
         __syncwarp();  // c_t is visible to the warp, and the previous tick's reads of acc are done
-        const DevFleet ft = at_tick(g, t);
+        const DevFleet ft = mg_view<true>(g, t);
+        const int k = mg_key(g, i, s);
         const float r = g.rate[i];
-        for (int a = lane; a < A; a += 32) iv_advance(g, ft, t, s, a, r, r, acc[a]);
+        for (int a = lane; a < A; a += 32) iv_advance(g, ft, t, s, k, a, r, r, acc[a]);
         __syncwarp();
         const int w = iv_winner(acc, A, lane);
         if (w >= 0) {
@@ -1628,6 +1658,8 @@ __global__ void __launch_bounds__(128) margin_chain(MarginArgs g) {
         }
     }
 }
+__global__ void __launch_bounds__(128) margin_chain(MarginArgs g) { mg_chain(g); }
+__global__ void __launch_bounds__(128) margin_chain(TokenMarginArgs g) { mg_chain(g); }
 
 // nextafterf(x, 0) for x > 0
 __device__ __forceinline__ float mg_below(float x) { return __uint_as_float(__float_as_uint(x) - 1u); }
@@ -1677,22 +1709,23 @@ __device__ __forceinline__ void mg_emit(const MarginArgs& g, int k, int i, int w
 // One warp per (level, server) item i = l * S + s; the accelerators' IvAcc states, then their stretch starts, live
 // in dynamic shared memory (A entries of each per warp).  Launched with up to 128 threads; with
 // __launch_bounds__(128) ptxas keeps it at 72 registers and spills, with room for 96 it uses 80 and does not.
-// Trace: level l is tick l, on the fleet at_tick(g, l).
-template <bool Trace>
-__global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
+// Trace: level l is tick l, on the fleet mg_view(g, l).
+template <bool Trace, class Args>
+__device__ __forceinline__ void mg_walk(const Args& g) {
+    constexpr bool Rows = Trace || !std::is_same<Args, MarginArgs>::value;  // f is a row view, not g.ld.f
     extern __shared__ IvAcc iv_acc[];
-    const int A = g.ld.f.A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+    const int A = mg_fleet(g).A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
     const int i = blockIdx.x * wpb + wid;
     if (i >= g.n) return;
-    const int l = i / g.ld.f.S, s = i - l * g.ld.f.S;
+    const int l = i / mg_fleet(g).S, s = i - l * mg_fleet(g).S, k = mg_key(g, i, s);
     DevFleet ft;
-    if constexpr (Trace) ft = at_tick(g, l);
-    const DevFleet& f = Trace ? ft : g.ld.f;
+    if constexpr (Rows) ft = mg_view<Trace>(g, l);
+    const DevFleet& f = Rows ? ft : g.ld.f;
     IvAcc* acc = iv_acc + (size_t)wid * A;
     float* start = (float*)(iv_acc + (size_t)wpb * A) + (size_t)wid * A;
     const float r = g.rate[i], lo = g.lo[i], hi = g.hi[i];
     const float inf = __int_as_float(0x7f800000);
-    auto advance = [&](int a, float x) { iv_advance(g, f, l, s, a, x, hi, acc[a]); };
+    auto advance = [&](int a, float x) { iv_advance(g, f, l, s, k, a, x, hi, acc[a]); };
     bool over = false;
     for (int a = lane; a < A; a += 32) {
         advance(a, r);
@@ -1777,27 +1810,38 @@ __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) {
         g.flags[i] = (uint8_t)flags;
     }
 }
+template <bool Trace>
+__global__ void __maxnreg__(96) margin_kernel(MarginArgs g) { mg_walk<Trace>(g); }
+template <bool Trace>
+__global__ void __maxnreg__(96) margin_kernel(TokenMarginArgs g) { mg_walk<Trace>(g); }
 
 // The record r = k * n + i: record k of item i, at the record's rate (r, the float below lo_out, or hi_out), its
 // value on a trace against c_t.
-template <bool Trace>
+template <bool Trace, class Args>
 struct MgTail {
-    const MarginArgs& g;
+    const Args& g;
     template <class Solve>
     __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
-        const int r = (int)(unsigned)item, k = r / g.n, i = r - k * g.n, S = g.ld.f.S;
+        const int r = (int)(unsigned)item, k = r / g.n, i = r - k * g.n, S = mg_fleet(g).S;
         const float x = k == 0 ? g.rate[i] : (k == 1 ? mg_below(g.lo_out[i]) : g.hi_out[i]);
-        if constexpr (Trace) return walk_load_tail(g, item, i % S, x, [&] { return at_tick(g, i / S); }, solve, out);
-        else return walk_load_tail(g, item, i % S, x, [&]() -> const DevFleet& { return g.ld.f; }, solve, out);
+        const int s = i % S, key = mg_key(g, i, s);
+        if constexpr (Trace) return walk_load_tail(g, item, s, key, x, [&] { return mg_view<true>(g, i / S); }, solve, out);
+        else return walk_load_tail(g, item, s, key, x, [&]() -> const DevFleet& { return mg_fleet(g); }, solve, out);
     }
     __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
 };
 
 template <bool Trace>
-__global__ void __launch_bounds__(256) margin_tail(MarginArgs g) { walk_tail(g, MgTail<Trace>{g}); }
+__global__ void __launch_bounds__(256) margin_tail(MarginArgs g) { walk_tail(g, MgTail<Trace, MarginArgs>{g}); }
+template <bool Trace>
+__global__ void __launch_bounds__(256) margin_tail(TokenMarginArgs g) {
+    walk_tail(g, MgTail<Trace, TokenMarginArgs>{g});
+}
 
 // Stored-vector re-run of the records margin_tail bailed on.
 template <bool Trace>
-__global__ void margin_fallback(MarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace>{g}); }
+__global__ void margin_fallback(MarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace, MarginArgs>{g}); }
+template <bool Trace>
+__global__ void margin_fallback(TokenMarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace, TokenMarginArgs>{g}); }
 
 }  // namespace wva

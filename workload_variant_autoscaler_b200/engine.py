@@ -185,7 +185,9 @@ def within_margins(lo, hi, flags, new_rpm, rpm_hi):
     itself (``lo == hi``) holds nothing; NaN is never inside.
 
     It works unchanged on ``Engine.load_margin_trace``'s result: there the servers inside their stretch at tick t
-    keep the decision the replayed reconcile makes at tick t."""
+    keep the decision the replayed reconcile makes at tick t.  On ``Engine.workload_margins`` and
+    ``Engine.workload_margin_trace`` a new rate inside the stretch keeps the row's decision when the new tokens equal
+    the row's; the mask does not look at tokens."""
     lo, hi, top, x = (np.asarray(v, np.float32) for v in (lo, hi, rpm_hi, new_rpm))
     flags = np.asarray(flags, np.uint8)
     if not lo.shape == hi.shape == flags.shape == top.shape == x.shape:
@@ -520,10 +522,41 @@ class Engine:
             raise ValueError("arrival_rpm is required")
         return self._margins(self._L.wva_load_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi)
 
-    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi):
-        """wva_load_margins / wva_load_margin_trace over (L, S) rows and windows; the output arrays."""
+    def workload_margins(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, rpm_lo=None,
+                         rpm_hi=None):
+        """``load_margins`` at rows that carry their own tokens: level ``l`` is ``workload_grid``'s row ``l`` of
+        (``arrival_rpm`` req/min, required; ``in_tokens``, ``out_tokens``), each of shape (L, S) -> the same tuple as
+        ``load_margins``.  A token list of ``None`` is the fleet's own column at every level.
+
+        Block ``l`` is ``load_margins`` with one level (row ``l`` of the rates and of the windows, by default
+        ``[0, 2 * rate]``) on the fleet with ``srv_in_tokens`` and ``srv_out_tokens`` = row ``l``, and the ``at``
+        records are ``workload_grid``'s winners; each distinct (server, in, out) under a window top above 0 is sized
+        once (see ``wva_workload_margins`` in include/wva_b200.h).  A new rate inside ``[lo, hi)`` keeps the row's
+        decision when the new tokens equal the row's: ``within_margins`` tests the rate only."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        return self._margins(self._L.wva_workload_margins, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens, out_tokens)
+
+    def workload_margin_trace(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, rpm_lo=None,
+                              rpm_hi=None):
+        """``workload_margins`` at every tick of ``workload_trace`` over the same (rate, in, out) rows -> the same
+        tuple as ``load_margins``.
+
+        Block ``t`` is ``workload_margins`` with one level on the fleet whose current allocation is the one the trace
+        carries into tick ``t`` (``fleet.apply_winners`` of every earlier tick's ``at`` in turn), and the ``at``
+        records are ``workload_trace``'s winners (see ``wva_workload_margin_trace`` in include/wva_b200.h).  A new
+        rate inside ``[lo, hi)`` keeps tick ``t``'s decision when the new tokens equal the row's."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        return self._margins(self._L.wva_workload_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens,
+                             out_tokens)
+
+    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi, *tokens):
+        """wva_load_margins / wva_load_margin_trace over (L, S) rows and windows, or with `tokens` (in_tokens,
+        out_tokens; None: the fleet's own) wva_workload_margins / wva_workload_margin_trace; the output arrays."""
         S = fleet.n_servers
-        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "rpm_lo": rpm_lo, "rpm_hi": rpm_hi})
+        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "rpm_lo": rpm_lo, "rpm_hi": rpm_hi,
+                                     **dict(zip(("in_tokens", "out_tokens"), tokens))})
         L = 1 if L is None else L
         rate = rows.get("arrival_rpm", np.ascontiguousarray(np.broadcast_to(fleet.srv_arrival_rpm, (L, S)), np.float32))
         lo = rows.get("rpm_lo", np.zeros((L, S), np.float32))
@@ -535,7 +568,9 @@ class Engine:
                            at.as_c(), below.as_c(), above.as_c())
         fc = fleet.as_c()
         self._resident(fleet)
-        self._check(call(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)), _abi.ptr(lo.reshape(-1)),
+        token_rows = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None
+                      for k in ("in_tokens", "out_tokens")[:len(tokens)]]
+        self._check(call(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)), *token_rows, _abi.ptr(lo.reshape(-1)),
                          _abi.ptr(hi.reshape(-1)), C.byref(oc)))
         return lo_out, hi_out, flags, at, below, above
 
