@@ -726,6 +726,58 @@ int wva_workload_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_t
                               const float *rpm_lo, const float *rpm_hi, wva_margins *out);
 
 /*
+ * Profile margins: wva_workload_margins and wva_workload_margin_trace at rows that also carry their own accelerator
+ * costs and performance profiles, as wva_profile_grid and wva_profile_trace take them: hourly spot or time-of-use
+ * prices, an accelerator brought online or withdrawn, a beta change.  A planner replaying a day of prices sees how
+ * far the load of each row may stray at that row's prices.  Without this call that takes one wva_load_margins per
+ * row, each re-uploading and re-sizing the fleet with its acc_cost and perf_* columns rewritten.
+ *
+ * Rows: arrival_rpm, in_tokens, out_tokens, rpm_lo and rpm_hi are [L*S], index l*S + s, with L = n_levels or n_ticks;
+ * `rows` has wva_profile_rows' layout (acc_cost [L*A], each perf_* [L*M*A]); every column of out is [L*S].
+ * arrival_rpm is required; a NULL token list, a NULL profile column, or rows NULL, is the fleet's own column at every
+ * row.
+ *   - Grid, level l.  Let f_l be the fleet with srv_arrival_rpm, srv_in_tokens, srv_out_tokens, acc_cost and the
+ *     nine perf_* columns replaced by row l.  Block l of lo_rpm, hi_rpm, flags, at, below and above is byte for byte
+ *     wva_load_margins(f_l) with one level: rate row l, window row l.  The `at` blocks are wva_profile_trace's winner
+ *     for each row alone (one tick on f_l); with arrival_rpm the fleet's own column at every row and NULL token lists
+ *     they are wva_profile_grid's winners.
+ *   - Trace, tick t.  Let f_t be that fleet with row t and srv_cur_* = c_t, the allocation wva_profile_trace carries
+ *     into tick t on the same rows: the cost it carries is the winner's at its own tick's prices, and c_0's
+ *     srv_cur_cost is not re-priced.  Block t is byte for byte wva_load_margins(f_t) with one level, and the `at`
+ *     blocks are wva_profile_trace's winners.  The trace continues as wva_profile_trace's does: ticks 0..L-1 equal
+ *     ticks 0..k-1 followed by ticks k..L-1 on the fleet whose srv_cur_* hold c_k.
+ *   - With every profile column NULL the result is byte for byte wva_workload_margins (grid) or
+ *     wva_workload_margin_trace (trace) on the same load rows and windows.
+ * A new rate inside [lo_rpm, hi_rpm) keeps the row's decision when the tokens, prices and profiles stay the row's.
+ *
+ * Sizing (DESIGN.md §3.23): price and AccCount enter only the cost, price x NumInstances x replicas, and alpha .. delta
+ * and N fix a pair's sizing without reading the rate.  So a pair's phase-1 record at row l is fixed by its key (s, a,
+ * in_l, out_l, bits of alpha, beta, gamma, delta at row l, N at row l), N being srv_max_batch or else
+ * max(perf_max_batch * perf_at_tokens / out_tokens, 1) in 64 bits.  Each distinct key is sized once over the rows
+ * whose window top rpm_hi is above 0 and at which the pair is a load pair (perf_present at the row, in_tokens >= 0,
+ * out_tokens >= 1); on a trace keepAccelerator is honoured on the pinned servers only.  Without a perf column the keys
+ * are wva_workload_margins' (server, in, out) rows, and the call sizes the same pairs in the same order.
+ *
+ * Only unlimited mode is covered; fleet->unlimited, the capacities, acc_type and acc_multiplicity are not read, nor
+ * are srv_arrival_rpm and the columns whose row lists are given.  The fleet becomes resident, and wva_summarize
+ * returns WVA_ERR_STATE afterwards.  Columns of at, below and above may be NULL (not written).  L == 0 and S == 0 are
+ * valid (nothing is written).  WVA_ERR_BAD_ARG: L < 0, out NULL, arrival_rpm, rpm_lo, rpm_hi, lo_rpm, hi_rpm or flags
+ * NULL with S*L > 0, or a row that wva_load_margins refuses.  WVA_ERR_UNSUPPORTED: 3*S*L >= 2^31 or L*M*A >= 2^31
+ * (both refused before the fleet is read); distinct key pairs x A >= 2^31; or, for the grid, exactly where
+ * wva_load_margins(f_l) refuses at some level l (a row's perf_max_batch, perf_at_tokens or out_tokens can push N
+ * above 2^20).  A key used only at rows whose window is [0, 0] is never sized and does not fail the call.  The trace's
+ * refusals can be larger than the union over t of what wva_load_margins(f_t) refuses, but only through the pairs of a
+ * server that is not pinned yet has keepAccelerator set.  The call never returns a result that differs from the
+ * per-row composition.
+ */
+int wva_profile_margins(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
+                        const int32_t *in_tokens, const int32_t *out_tokens, const wva_profile_rows *rows,
+                        const float *rpm_lo, const float *rpm_hi, wva_margins *out);
+int wva_profile_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                             const int32_t *in_tokens, const int32_t *out_tokens, const wva_profile_rows *rows,
+                             const float *rpm_lo, const float *rpm_hi, wva_margins *out);
+
+/*
  * Price thresholds: for each server s and accelerator a, the exact accelerator price at which s's unlimited
  * winner leaves a.  Let f(p) be the fleet with acc_cost[a] = p, solved in unlimited mode.
  *

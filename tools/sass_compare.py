@@ -3,7 +3,9 @@
     python tools/sass_compare.py OLD.so NEW.so
 
 Runs ``cuobjdump -sass`` on both libraries, splits each listing at its ``Function :`` headers and reports every
-kernel as identical, different or missing (present in one library only).  Exits 1 unless every kernel is identical.
+kernel as identical, different or missing (present in one library only).  Runs of blanks are compared as one: the
+listing pads its columns to the widest instruction of the whole library, so a new kernel can re-pad unchanged ones.
+Exits 1 unless every kernel is identical.
 """
 from __future__ import annotations
 
@@ -20,7 +22,7 @@ def kernels(so: str) -> dict[str, str]:
     out = {}
     parts = re.split(r"^\s*Function : (\S+)\s*$", text, flags=re.M)
     for name, body in zip(parts[1::2], parts[2::2]):
-        out[name] = body
+        out[name] = re.sub(r"[ \t]+", " ", body)
     return out
 
 

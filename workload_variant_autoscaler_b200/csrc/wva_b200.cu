@@ -1243,6 +1243,187 @@ KeyFleet workload_keys(const HostFleet& hf, int L, const float* rpm, const int32
     return kf;
 }
 
+// The rows of a wva_profile_rows list as the profile grid and the profile trace size them.  Per (m, a) the host ranks
+// the distinct present rows that the levels use (elsewhere no pair of m is a load); key-model (m, j) = moff[m] + j
+// holds the j-th distinct row of (m, a) at every accelerator a that has one, so a key fleet's tables stay within
+// L * M * A entries.  The caller's row lists travel in the call's upload image (place), and set_rows points a
+// ProfileArgs at them.
+struct ProfileRanks {
+    using Row = std::array<uint32_t, 6>;  // bits of alpha, beta, gamma, delta; max_batch, at_tokens
+    const void* lists[9];                 // column c: the caller's row list (bit c of per_level) or NULL
+    unsigned per_level = 0;
+    bool perf_rows = false;               // some perf column is a row list
+    int L, A;
+    size_t MA;
+    // the distinct present rows of (m, a) = k: row_v[row_off[k] .. row_off[k + 1]), ascending; rank [L*M*A] is row
+    // (l, k)'s index among them (-1: absent), built only when perf_rows
+    std::vector<Row> row_v;
+    std::vector<int> row_off, rank;
+    std::vector<int> moff;  // [M + 1]: key-model (m, j) = moff[m] + j, j < the most distinct rows of m at any a
+    size_t o_list[9] = {};
+
+    ProfileRanks(const HostFleet& hf, int L_, const wva_profile_rows& rows)
+        : lists{rows.acc_cost,  rows.perf_present,   rows.perf_alpha,     rows.perf_beta,     rows.perf_gamma,
+                rows.perf_delta, rows.perf_acc_count, rows.perf_max_batch, rows.perf_at_tokens},
+          L(L_), A(hf.A), MA((size_t)hf.M * hf.A), row_off(MA + 1, 0), moff(hf.M + 1, 0) {
+        for (int c = 0; c < 9; ++c) per_level |= lists[c] ? 1u << c : 0u;
+        perf_rows = (per_level >> 1) != 0;
+        // column c of row l at entry k
+        auto at = [&](const auto* list, const auto& own, int l, size_t k) { return list ? list[l * MA + k] : own[k]; };
+        auto bits = [](float x) {
+            uint32_t u;
+            memcpy(&u, &x, 4);
+            return u;
+        };
+        auto row_of = [&](int l, size_t k) {
+            return Row{bits(at(rows.perf_alpha, hf.perf_alpha, l, k)), bits(at(rows.perf_beta, hf.perf_beta, l, k)),
+                       bits(at(rows.perf_gamma, hf.perf_gamma, l, k)), bits(at(rows.perf_delta, hf.perf_delta, l, k)),
+                       (uint32_t)at(rows.perf_max_batch, hf.perf_max_batch, l, k),
+                       (uint32_t)at(rows.perf_at_tokens, hf.perf_at_tokens, l, k)};
+        };
+        if (perf_rows) {
+            rank.assign((size_t)L * MA, -1);
+            std::vector<std::pair<Row, int>> uses;
+            for (size_t k = 0; k < MA; ++k) {
+                uses.clear();
+                for (int l = 0; l < L; ++l)
+                    if (at(rows.perf_present, hf.perf_present, l, k)) uses.emplace_back(row_of(l, k), l);
+                std::sort(uses.begin(), uses.end());
+                for (size_t u = 0; u < uses.size(); ++u) {
+                    if (u == 0 || uses[u].first != uses[u - 1].first) row_v.push_back(uses[u].first);
+                    rank[(size_t)uses[u].second * MA + k] = (int)row_v.size() - 1 - row_off[k];
+                }
+                row_off[k + 1] = (int)row_v.size();
+            }
+        } else {
+            for (size_t k = 0; k < MA; ++k) {
+                if (L > 0 && hf.perf_present[k]) row_v.push_back(row_of(0, k));
+                row_off[k + 1] = (int)row_v.size();
+            }
+        }
+        for (int m = 0; m < hf.M; ++m) {
+            int J = 0;
+            for (int a = 0; a < A; ++a) J = std::max(J, row_off[(size_t)m * A + a + 1] - row_off[(size_t)m * A + a]);
+            moff[m + 1] = moff[m] + J;
+        }
+    }
+    // row (l, k)'s index among the distinct rows of k, -1 where (m, a) is absent at row l
+    int rank_at(int l, size_t k) const {
+        if (perf_rows) return rank[(size_t)l * MA + k];
+        return row_off[k + 1] > row_off[k] ? 0 : -1;
+    }
+    // What a load pair's sizing reads of row j of k = (m, a): ((alpha, beta), (gamma, delta), N), N being the
+    // server's batch size max_batch when positive and the row's AtTokens rule at out_tokens out otherwise.
+    std::array<uint64_t, 3> sizing_key(size_t k, int j, int max_batch, int out) const {
+        const Row& r = row_v[row_off[k] + j];
+        const long long t = (long long)(int32_t)r[4] * (int32_t)r[5] / out;
+        const long long N = max_batch > 0 ? max_batch : std::max<long long>(t, 1);
+        return {(uint64_t)r[0] << 32 | r[1], (uint64_t)r[2] << 32 | r[3], (uint64_t)N};
+    }
+    // the key fleet's models: M and the perf columns of the key-models (kh starts as a copy of the fleet)
+    void fill(HostFleet& kh) const {
+        kh.M = moff.back();
+        const size_t KMA = (size_t)kh.M * A;
+        kh.perf_present.assign(KMA, 0);
+        kh.perf_acc_count.assign(KMA, 1);
+        for (auto* col : {&kh.perf_alpha, &kh.perf_beta, &kh.perf_gamma, &kh.perf_delta}) col->assign(KMA, 0.0f);
+        kh.perf_max_batch.assign(KMA, 0);
+        kh.perf_at_tokens.assign(KMA, 0);
+        for (size_t m = 0; m + 1 < moff.size(); ++m)
+            for (int a = 0; a < A; ++a) {
+                const size_t k = m * A + a;
+                for (int j = 0; j < row_off[k + 1] - row_off[k]; ++j) {
+                    const Row& r = row_v[row_off[k] + j];
+                    const size_t q = (size_t)(moff[m] + j) * A + a;
+                    kh.perf_present[q] = 1;
+                    memcpy(&kh.perf_alpha[q], &r[0], 4);
+                    memcpy(&kh.perf_beta[q], &r[1], 4);
+                    memcpy(&kh.perf_gamma[q], &r[2], 4);
+                    memcpy(&kh.perf_delta[q], &r[3], 4);
+                    kh.perf_max_batch[q] = (int32_t)r[4];
+                    kh.perf_at_tokens[q] = (int32_t)r[5];
+                }
+            }
+    }
+    size_t list_bytes(int c) const {
+        static const size_t elem[9] = {4, 1, 4, 4, 4, 4, 4, 4, 4};
+        return elem[c] * (size_t)L * (c == 0 ? (size_t)A : MA);
+    }
+    void place(Cols& c) {
+        for (int b = 0; b < 9; ++b)
+            if (lists[b]) o_list[b] = c.put(lists[b], list_bytes(b));
+    }
+    // g.rows: g.f with the row lists uploaded at d, and per_level (g: a ProfileArgs or a ProfileMarginArgs)
+    template <class Args>
+    void set_rows(Args& g, const char* d) const {
+        g.rows = g.f;
+        const auto row = [&](int b) { return (const void*)(d + o_list[b]); };
+        if (lists[0]) g.rows.acc_cost = (const float*)row(0);
+        if (lists[1]) g.rows.perf_present = (const uint8_t*)row(1);
+        if (lists[2]) g.rows.perf_alpha = (const float*)row(2);
+        if (lists[3]) g.rows.perf_beta = (const float*)row(3);
+        if (lists[4]) g.rows.perf_gamma = (const float*)row(4);
+        if (lists[5]) g.rows.perf_delta = (const float*)row(5);
+        if (lists[6]) g.rows.perf_acc_count = (const int32_t*)row(6);
+        if (lists[7]) g.rows.perf_max_batch = (const int32_t*)row(7);
+        if (lists[8]) g.rows.perf_at_tokens = (const int32_t*)row(8);
+        g.per_level = per_level;
+    }
+};
+
+
+// The profile calls' keys with a perf column (DESIGN.md §3.15) of the rows rpm / in / out [L*S] into tk: per server
+// the rows at which s is a load, grouped by (in, out) as in the workload calls; per group and accelerator a the rows
+// at which (m, a) is present, grouped by the row's sizing key, one key row per key pair, whose accelerator and
+// key-model go to key_acc and key_model.  skip(s, a) holds for a pair that keepAccelerator masks at every row.
+template <class Skip>
+void profile_keys(const HostFleet& hf, const ProfileRanks& pr, int L, const float* rpm, const int32_t* in,
+                  const int32_t* out, Skip&& skip, TokenKeys& tk, std::vector<int>& key_acc,
+                  std::vector<int>& key_model) {
+    const int S = hf.S, A = hf.A, M = hf.M;
+    std::vector<std::pair<uint64_t, int>> uses;                 // ((in << 32) | out, row)
+    std::vector<std::pair<std::array<uint64_t, 3>, int>> prof;  // (sizing key, row)
+    for (int s = 0; s < S; ++s) {
+        const int m = hf.srv_model[s];
+        if (m < 0 || m >= M || !hf.srv_has_target[s]) continue;
+        load_groups(L, S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
+            for (int a = 0; a < A; ++a) {
+                if (skip(s, a)) continue;
+                const size_t k = (size_t)m * A + a;
+                prof.clear();
+                for (size_t u = u0; u < u1; ++u) {
+                    const int t = uses[u].second, j = pr.rank_at(t, k);
+                    if (j >= 0) prof.emplace_back(pr.sizing_key(k, j, hf.srv_max_batch[s], ko), t);
+                }
+                std::sort(prof.begin(), prof.end());
+                for (size_t v = 0; v < prof.size(); ++v) {
+                    if (v == 0 || prof[v].first != prof[v - 1].first) {
+                        tk.add(s, ki, ko);
+                        key_acc.push_back(a);
+                        key_model.push_back(pr.moff[m] + pr.rank_at(prof[v].second, k));
+                    }
+                    tk.add_level(prof[v].second);
+                }
+            }
+        });
+    }
+}
+// Their key fleet: key row k is server tk.srv[k] at the key's tokens on key-model key_model[k], with
+// keepAccelerator and current accelerator key_acc[k], so that phase 1 sizes that pair alone.
+KeyFleet profile_key_fleet(const HostFleet& hf, const ProfileRanks& pr, const TokenKeys& tk,
+                           const std::vector<int>& key_acc, const std::vector<int>& key_model) {
+    KeyFleet kf(hf, tk.srv, tk.in, tk.out);
+    HostFleet& kh = kf.hf;
+    kf.own_ma = true;
+    for (size_t k = 0; k < tk.srv.size(); ++k) {
+        kh.srv_model[k] = key_model[k];
+        kh.srv_keep_acc[k] = 1;
+        kh.srv_cur_acc[k] = key_acc[k];
+    }
+    pr.fill(kh);
+    return kf;
+}
+
 // ---- walks: the load intervals and the load margins -----------------------------------------------------------
 // The servers whose accelerator no tick of a trace can change (DESIGN.md §3.13), as flags [S]: with keepAccelerator
 // and a current accelerator other than "" only that accelerator is a candidate, and its load and zero-load
@@ -1415,29 +1596,59 @@ int launch_margins(wva_handle* h, const Args& g, bool trace, const FbRun& fb) {
 // whose tokens class a pair as a load (workload_keys with the window tops as its rates; on a trace with
 // keepAccelerator on the pinned servers only).  The key column [L*S] names each row's key (-1: none), and the
 // kernels read the rows' tokens through the row's view of the resident fleet.
+//
+// With `prof` (the profile margins, DESIGN.md §3.23) row l also has its own acc_cost and perf_* columns (ProfileRanks'
+// layout; a NULL column is the fleet's own).  Price and AccCount enter only the cost, so without a perf column the
+// keys are the workload margins' and the kernels price every record at its row.  With one, a load pair's record at
+// row l is fixed by (s, a, in, out, the row's alpha .. delta and N), and the keys are the profile trace's
+// (profile_keys, with the window tops as rates): one key row per key pair, so the key column [L*S*A] names each
+// (row, server, accelerator)'s key row (-1: none).  keepAccelerator masks a pair at every row on the grid, and on a
+// trace only on the pinned servers.
 int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t* in, const int32_t* out, bool tokens,
-                         const float* lo, const float* hi, TokenMarginArgs& g, size_t rec_bytes, bool trace) {
+                         const wva_profile_rows* prof, const float* lo, const float* hi, ProfileMarginArgs& g,
+                         size_t rec_bytes, bool trace) {
     const HostFleet& hf = h->hf;
-    const int S = hf.S;
+    const int S = hf.S, A = hf.A;
     Cols c(16);
     RowLists lists{hf, L, c};
     lists.put_rpm(rate);
     TokenKeys tk;
     std::optional<KeyFleet> kf;
+    std::optional<ProfileRanks> pr;
     std::vector<int> key;
     size_t o_key = 0;
     if (tokens) {
         lists.put_tokens(in, out);
         const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
-        kf.emplace(workload_keys(hf, L, hi, lists.in.host, lists.out.host, trace ? pin.data() : nullptr, tk));
-        // the keys' pairs are indexed in int32 on the device
-        if ((long long)tk.srv.size() * hf.A >= (1ll << 31))
-            return h->fail(WVA_ERR_UNSUPPORTED, "workload margins: too many token keys for one call (K*A >= 2^31)");
-        key.assign((size_t)L * S, -1);
-        for (size_t k = 0; k < tk.srv.size(); ++k)
-            for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j) key[(size_t)tk.lev[j] * S + tk.srv[k]] = (int)k;
+        if (prof) pr.emplace(hf, L, *prof);
+        if (pr && pr->perf_rows) {
+            std::vector<int> key_acc, key_model;
+            profile_keys(hf, *pr, L, hi, lists.in.host, lists.out.host,
+                         [&](int s, int a) {
+                             const int cur = hf.srv_cur_acc[s];
+                             return (trace ? pin[s] : hf.srv_keep_acc[s] && cur != WVA_ACC_NONE) && cur != a;
+                         },
+                         tk, key_acc, key_model);
+            // the keys' pairs are indexed in int32 on the device
+            if ((long long)tk.srv.size() * A >= (1ll << 31))
+                return h->fail(WVA_ERR_UNSUPPORTED, "profile margins: too many key pairs for one call (K*A >= 2^31)");
+            kf.emplace(profile_key_fleet(hf, *pr, tk, key_acc, key_model));
+            key.assign((size_t)L * S * A, -1);
+            for (size_t k = 0; k < tk.srv.size(); ++k)
+                for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j)
+                    key[((size_t)tk.lev[j] * S + tk.srv[k]) * A + key_acc[k]] = (int)k;
+        } else {
+            kf.emplace(workload_keys(hf, L, hi, lists.in.host, lists.out.host, trace ? pin.data() : nullptr, tk));
+            // the keys' pairs are indexed in int32 on the device
+            if ((long long)tk.srv.size() * A >= (1ll << 31))
+                return h->fail(WVA_ERR_UNSUPPORTED, "workload margins: too many token keys for one call (K*A >= 2^31)");
+            key.assign((size_t)L * S, -1);
+            for (size_t k = 0; k < tk.srv.size(); ++k)
+                for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j) key[(size_t)tk.lev[j] * S + tk.srv[k]] = (int)k;
+        }
         o_key = c.put(key.data(), 4 * key.size());
         kf->place(c);
+        if (pr) pr->place(c);
     }
     LoadStar ls;
     int rc = enqueue_walk_star(h, c, L, lo, hi, trace, rec_bytes, g, ls, kf ? &*kf : nullptr);
@@ -1450,15 +1661,18 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t*
     g.key = (const int*)(d + o_key);
     g.in_tokens = lists.in.dev(d);
     g.out_tokens = lists.out.dev(d);
+    if (!pr) return launch_margins(h, static_cast<const TokenMarginArgs&>(g), trace, ls.fb2);
+    pr->set_rows(g, d);
+    g.pair_key = pr->perf_rows ? g.key : nullptr;
     return launch_margins(h, g, trace, ls.fb2);
 }
 
 // wva_load_margins, or with `trace` wva_load_margin_trace; with `tokens` wva_workload_margins or
-// wva_workload_margin_trace (in / out: NULL is the fleet's own column).  All but wva_load_margins require the rate
-// rows.
+// wva_workload_margin_trace (in / out: NULL is the fleet's own column), and with `prof` as well
+// wva_profile_margins or wva_profile_margin_trace.  All but wva_load_margins require the rate rows.
 int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
-                      const int32_t* in_tokens, const int32_t* out_tokens, bool tokens, const float* rpm_lo,
-                      const float* rpm_hi, wva_margins* out, bool trace) {
+                      const int32_t* in_tokens, const int32_t* out_tokens, bool tokens, const wva_profile_rows* prof,
+                      const float* rpm_lo, const float* rpm_hi, wva_margins* out, bool trace) {
     if (!h) return WVA_ERR_BAD_ARG;
     if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
     if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, trace ? "negative tick count" : "negative level count");
@@ -1467,6 +1681,8 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
     // three records per (level, server), each indexed in int32
     if (3ll * S * L >= (1ll << 31))
         return h->fail(WVA_ERR_UNSUPPORTED, "load margins too large for one call (>= 2^31 records)");
+    if (prof && (long long)L * fleet->n_models * fleet->n_acc >= (1ll << 31))
+        return h->fail(WVA_ERR_UNSUPPORTED, "profile margins too large for one call (>= 2^31 row entries)");
     const int n = S * L;
     if (n > 0 && (!rpm_lo || !rpm_hi || !out->lo_rpm || !out->hi_rpm || !out->flags))
         return h->fail(WVA_ERR_BAD_ARG, "NULL window or output column");
@@ -1483,7 +1699,7 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
     const size_t o_cur = trace ? cols.take(12 * (size_t)n) : 0;  // a trace's c_t: acc, replicas, cost [n] each
     return run_walk(h, fleet, cols, 3 * (size_t)n, n > 0, {&out->at, &out->below, &out->above},
                     [&](const WalkArgs& w, char* d, size_t rec_bytes) {
-                        TokenMarginArgs g{MarginArgs{w}};
+                        ProfileMarginArgs g{TokenMarginArgs{MarginArgs{w}}};
                         g.n = n;
                         g.lo_out = (float*)(d + o_lo);
                         g.hi_out = (float*)(d + o_hi);
@@ -1493,8 +1709,8 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
                             g.cur_replicas = (int*)(d + o_cur) + n;
                             g.cur_cost = (float*)(d + o_cur) + 2 * (size_t)n;
                         }
-                        return enqueue_load_margins(h, L, arrival_rpm, in_tokens, out_tokens, tokens, rpm_lo, rpm_hi,
-                                                    g, rec_bytes, trace);
+                        return enqueue_load_margins(h, L, arrival_rpm, in_tokens, out_tokens, tokens, prof, rpm_lo,
+                                                    rpm_hi, g, rec_bytes, trace);
                     });
 }
 
@@ -1853,133 +2069,6 @@ int enqueue_slo_trace(wva_handle* h, int L, const float* rpm, const int32_t* in,
 // run on the key fleet with one "level" (its own rates), writing one record per key pair; profile_kernel then writes
 // every level's records and the existing L-block unlimited_kernel the winners.  The lists, the row lists and the key
 // fleet's columns go into lg_tabs, rebuilt on every call.  cand ([L*S*A]) and winners ([L*S]) are device columns.
-// The rows of a wva_profile_rows list as the profile grid and the profile trace size them.  Per (m, a) the host ranks
-// the distinct present rows that the levels use (elsewhere no pair of m is a load); key-model (m, j) = moff[m] + j
-// holds the j-th distinct row of (m, a) at every accelerator a that has one, so a key fleet's tables stay within
-// L * M * A entries.  The caller's row lists travel in the call's upload image (place), and set_rows points a
-// ProfileArgs at them.
-struct ProfileRanks {
-    using Row = std::array<uint32_t, 6>;  // bits of alpha, beta, gamma, delta; max_batch, at_tokens
-    const void* lists[9];                 // column c: the caller's row list (bit c of per_level) or NULL
-    unsigned per_level = 0;
-    bool perf_rows = false;               // some perf column is a row list
-    int L, A;
-    size_t MA;
-    // the distinct present rows of (m, a) = k: row_v[row_off[k] .. row_off[k + 1]), ascending; rank [L*M*A] is row
-    // (l, k)'s index among them (-1: absent), built only when perf_rows
-    std::vector<Row> row_v;
-    std::vector<int> row_off, rank;
-    std::vector<int> moff;  // [M + 1]: key-model (m, j) = moff[m] + j, j < the most distinct rows of m at any a
-    size_t o_list[9] = {};
-
-    ProfileRanks(const HostFleet& hf, int L_, const wva_profile_rows& rows)
-        : lists{rows.acc_cost,  rows.perf_present,   rows.perf_alpha,     rows.perf_beta,     rows.perf_gamma,
-                rows.perf_delta, rows.perf_acc_count, rows.perf_max_batch, rows.perf_at_tokens},
-          L(L_), A(hf.A), MA((size_t)hf.M * hf.A), row_off(MA + 1, 0), moff(hf.M + 1, 0) {
-        for (int c = 0; c < 9; ++c) per_level |= lists[c] ? 1u << c : 0u;
-        perf_rows = (per_level >> 1) != 0;
-        // column c of row l at entry k
-        auto at = [&](const auto* list, const auto& own, int l, size_t k) { return list ? list[l * MA + k] : own[k]; };
-        auto bits = [](float x) {
-            uint32_t u;
-            memcpy(&u, &x, 4);
-            return u;
-        };
-        auto row_of = [&](int l, size_t k) {
-            return Row{bits(at(rows.perf_alpha, hf.perf_alpha, l, k)), bits(at(rows.perf_beta, hf.perf_beta, l, k)),
-                       bits(at(rows.perf_gamma, hf.perf_gamma, l, k)), bits(at(rows.perf_delta, hf.perf_delta, l, k)),
-                       (uint32_t)at(rows.perf_max_batch, hf.perf_max_batch, l, k),
-                       (uint32_t)at(rows.perf_at_tokens, hf.perf_at_tokens, l, k)};
-        };
-        if (perf_rows) {
-            rank.assign((size_t)L * MA, -1);
-            std::vector<std::pair<Row, int>> uses;
-            for (size_t k = 0; k < MA; ++k) {
-                uses.clear();
-                for (int l = 0; l < L; ++l)
-                    if (at(rows.perf_present, hf.perf_present, l, k)) uses.emplace_back(row_of(l, k), l);
-                std::sort(uses.begin(), uses.end());
-                for (size_t u = 0; u < uses.size(); ++u) {
-                    if (u == 0 || uses[u].first != uses[u - 1].first) row_v.push_back(uses[u].first);
-                    rank[(size_t)uses[u].second * MA + k] = (int)row_v.size() - 1 - row_off[k];
-                }
-                row_off[k + 1] = (int)row_v.size();
-            }
-        } else {
-            for (size_t k = 0; k < MA; ++k) {
-                if (L > 0 && hf.perf_present[k]) row_v.push_back(row_of(0, k));
-                row_off[k + 1] = (int)row_v.size();
-            }
-        }
-        for (int m = 0; m < hf.M; ++m) {
-            int J = 0;
-            for (int a = 0; a < A; ++a) J = std::max(J, row_off[(size_t)m * A + a + 1] - row_off[(size_t)m * A + a]);
-            moff[m + 1] = moff[m] + J;
-        }
-    }
-    // row (l, k)'s index among the distinct rows of k, -1 where (m, a) is absent at row l
-    int rank_at(int l, size_t k) const {
-        if (perf_rows) return rank[(size_t)l * MA + k];
-        return row_off[k + 1] > row_off[k] ? 0 : -1;
-    }
-    // What a load pair's sizing reads of row j of k = (m, a): ((alpha, beta), (gamma, delta), N), N being the
-    // server's batch size max_batch when positive and the row's AtTokens rule at out_tokens out otherwise.
-    std::array<uint64_t, 3> sizing_key(size_t k, int j, int max_batch, int out) const {
-        const Row& r = row_v[row_off[k] + j];
-        const long long t = (long long)(int32_t)r[4] * (int32_t)r[5] / out;
-        const long long N = max_batch > 0 ? max_batch : std::max<long long>(t, 1);
-        return {(uint64_t)r[0] << 32 | r[1], (uint64_t)r[2] << 32 | r[3], (uint64_t)N};
-    }
-    // the key fleet's models: M and the perf columns of the key-models (kh starts as a copy of the fleet)
-    void fill(HostFleet& kh) const {
-        kh.M = moff.back();
-        const size_t KMA = (size_t)kh.M * A;
-        kh.perf_present.assign(KMA, 0);
-        kh.perf_acc_count.assign(KMA, 1);
-        for (auto* col : {&kh.perf_alpha, &kh.perf_beta, &kh.perf_gamma, &kh.perf_delta}) col->assign(KMA, 0.0f);
-        kh.perf_max_batch.assign(KMA, 0);
-        kh.perf_at_tokens.assign(KMA, 0);
-        for (size_t m = 0; m + 1 < moff.size(); ++m)
-            for (int a = 0; a < A; ++a) {
-                const size_t k = m * A + a;
-                for (int j = 0; j < row_off[k + 1] - row_off[k]; ++j) {
-                    const Row& r = row_v[row_off[k] + j];
-                    const size_t q = (size_t)(moff[m] + j) * A + a;
-                    kh.perf_present[q] = 1;
-                    memcpy(&kh.perf_alpha[q], &r[0], 4);
-                    memcpy(&kh.perf_beta[q], &r[1], 4);
-                    memcpy(&kh.perf_gamma[q], &r[2], 4);
-                    memcpy(&kh.perf_delta[q], &r[3], 4);
-                    kh.perf_max_batch[q] = (int32_t)r[4];
-                    kh.perf_at_tokens[q] = (int32_t)r[5];
-                }
-            }
-    }
-    size_t list_bytes(int c) const {
-        static const size_t elem[9] = {4, 1, 4, 4, 4, 4, 4, 4, 4};
-        return elem[c] * (size_t)L * (c == 0 ? (size_t)A : MA);
-    }
-    void place(Cols& c) {
-        for (int b = 0; b < 9; ++b)
-            if (lists[b]) o_list[b] = c.put(lists[b], list_bytes(b));
-    }
-    // g.rows: g.f with the row lists uploaded at d, and per_level
-    void set_rows(ProfileArgs& g, const char* d) const {
-        g.rows = g.f;
-        const auto row = [&](int b) { return (const void*)(d + o_list[b]); };
-        if (lists[0]) g.rows.acc_cost = (const float*)row(0);
-        if (lists[1]) g.rows.perf_present = (const uint8_t*)row(1);
-        if (lists[2]) g.rows.perf_alpha = (const float*)row(2);
-        if (lists[3]) g.rows.perf_beta = (const float*)row(3);
-        if (lists[4]) g.rows.perf_gamma = (const float*)row(4);
-        if (lists[5]) g.rows.perf_delta = (const float*)row(5);
-        if (lists[6]) g.rows.perf_acc_count = (const int32_t*)row(6);
-        if (lists[7]) g.rows.perf_max_batch = (const int32_t*)row(7);
-        if (lists[8]) g.rows.perf_at_tokens = (const int32_t*)row(8);
-        g.per_level = per_level;
-    }
-};
-
 int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, const AllocCols& cand,
                          const AllocCols& winners) {
     const HostFleet& hf = h->hf;
@@ -2128,7 +2217,7 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
 int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
                           const wva_profile_rows& rows, const AllocCols& cand, const AllocCols& winners) {
     const HostFleet& hf = h->hf;
-    const int S = hf.S, A = hf.A, M = hf.M;
+    const int S = hf.S, A = hf.A;
     Cols c(16);
     RowLists lists{hf, L, c};
     lists.put_rpm(rpm);
@@ -2139,56 +2228,22 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
     ProfileRanks pr(hf, L, rows);
     const std::vector<uint8_t> pin = trace_pinned(hf);
     const size_t o_pin = c.put(pin.data(), S);
-    // The keys.  Without a perf column: the workload trace's (s, in, out) rows.  With one: per server the ticks at
-    // which s is a load, grouped by (in, out) as in the workload trace; per group and accelerator the ticks at which
-    // (m, a) is present, grouped by the row's sizing key, one row per key pair.  A pinned server sizes its current
-    // pair alone.
+    // The keys.  Without a perf column: the workload trace's (s, in, out) rows.  With one: profile_keys, a pinned
+    // server sizing its current pair alone.
     TokenKeys tk;
     std::vector<int> key_acc, key_model;  // with a perf column: key row k's accelerator and key-model
     if (pr.perf_rows) {
-        std::vector<std::pair<uint64_t, int>> uses;                 // ((in << 32) | out, tick)
-        std::vector<std::pair<std::array<uint64_t, 3>, int>> prof;  // (sizing key, tick)
-        for (int s = 0; s < S; ++s) {
-            const int m = hf.srv_model[s];
-            if (m < 0 || m >= M || !hf.srv_has_target[s]) continue;
-            load_groups(L, S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
-                for (int a = 0; a < A; ++a) {
-                    if (pin[s] && hf.srv_cur_acc[s] != a) continue;
-                    const size_t k = (size_t)m * A + a;
-                    prof.clear();
-                    for (size_t u = u0; u < u1; ++u) {
-                        const int t = uses[u].second, j = pr.rank_at(t, k);
-                        if (j >= 0) prof.emplace_back(pr.sizing_key(k, j, hf.srv_max_batch[s], ko), t);
-                    }
-                    std::sort(prof.begin(), prof.end());
-                    for (size_t v = 0; v < prof.size(); ++v) {
-                        if (v == 0 || prof[v].first != prof[v - 1].first) {
-                            tk.add(s, ki, ko);
-                            key_acc.push_back(a);
-                            key_model.push_back(pr.moff[m] + pr.rank_at(prof[v].second, k));
-                        }
-                        tk.add_level(prof[v].second);
-                    }
-                }
-            });
-        }
+        profile_keys(hf, pr, L, rpm, in, out, [&](int s, int a) { return pin[s] && hf.srv_cur_acc[s] != a; }, tk,
+                     key_acc, key_model);
         // at most L * S * A key rows; the key fleet's pair ids k * A + a are int
         if ((long long)tk.srv.size() * A >= (1ll << 31))
             return h->fail(WVA_ERR_UNSUPPORTED,
                            "profile trace too large for one call (>= 2^31 key pairs x accelerators)");
     }
-    KeyFleet kf = pr.perf_rows ? KeyFleet(hf, tk.srv, tk.in, tk.out) : workload_keys(hf, L, rpm, in, out, pin.data(), tk);
+    KeyFleet kf = pr.perf_rows ? profile_key_fleet(hf, pr, tk, key_acc, key_model)
+                               : workload_keys(hf, L, rpm, in, out, pin.data(), tk);
     const int K = (int)tk.srv.size();
     HostFleet& kh = kf.hf;
-    if (pr.perf_rows) {
-        kf.own_ma = true;
-        for (int k = 0; k < K; ++k) {
-            kh.srv_model[k] = key_model[k];
-            kh.srv_keep_acc[k] = 1;
-            kh.srv_cur_acc[k] = key_acc[k];
-        }
-        pr.fill(kh);
-    }
     kf.place(c);
     pr.place(c);
     // the tail's candidates: one per key row with a perf column, up to A without
@@ -3331,24 +3386,44 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
 
 int wva_load_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                      const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_levels, arrival_rpm, nullptr, nullptr, false, rpm_lo, rpm_hi, out, false);
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, nullptr, nullptr, false, nullptr, rpm_lo, rpm_hi, out,
+                             false);
 }
 
 int wva_load_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                           const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_ticks, arrival_rpm, nullptr, nullptr, false, rpm_lo, rpm_hi, out, true);
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, nullptr, nullptr, false, nullptr, rpm_lo, rpm_hi, out,
+                             true);
 }
 
 int wva_workload_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                          const int32_t* in_tokens, const int32_t* out_tokens, const float* rpm_lo, const float* rpm_hi,
                          wva_margins* out) {
-    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, rpm_lo, rpm_hi, out, false);
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, nullptr, rpm_lo, rpm_hi, out,
+                             false);
 }
 
 int wva_workload_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                               const int32_t* in_tokens, const int32_t* out_tokens, const float* rpm_lo,
                               const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, rpm_lo, rpm_hi, out, true);
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, nullptr, rpm_lo, rpm_hi, out,
+                             true);
+}
+
+int wva_profile_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                        const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
+                        const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
+    const wva_profile_rows own{};
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, rows ? rows : &own, rpm_lo,
+                             rpm_hi, out, false);
+}
+
+int wva_profile_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                             const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
+                             const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
+    const wva_profile_rows own{};
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, rows ? rows : &own, rpm_lo,
+                             rpm_hi, out, true);
 }
 
 int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold, wva_allocs* above,

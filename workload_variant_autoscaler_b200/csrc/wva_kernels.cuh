@@ -1828,7 +1828,9 @@ struct ProfileArgs {
     AllocCols cand;       // [L * S * A]
     int L;
 };
-__device__ __forceinline__ DevFleet profile_at(const ProfileArgs& g, int l) {
+// Args: ProfileArgs, or any argument type with its f, rows and per_level (the profile margins' ProfileMarginArgs)
+template <class Args>
+__device__ __forceinline__ DevFleet profile_at(const Args& g, int l) {
     DevFleet fl = g.f;
     const size_t ra = (size_t)l * g.f.A, rma = (size_t)l * g.f.M * g.f.A;
     fl.acc_cost = g.rows.acc_cost + (g.per_level & 1u ? ra : 0);

@@ -1523,13 +1523,21 @@ __global__ void __launch_bounds__(128) interval_kernel(IntervalArgs g) {
 // Item fb_pack(a, r) of a walk's work list: record r, whose winner is the load pair of accelerator a of server s,
 // sized on row k of g.ld (see iv_advance), is the load grid's tail at rate x, then the value against the fleet
 // fleet() returns.
-template <class Fleet, class Solve>
+// Priced: phase 1 sized the pair at another price or AccCount (the profile margins' key fleet), so the record is
+// first priced at fleet()'s (priced_at).
+template <bool Priced = false, class Fleet, class Solve>
 __device__ __forceinline__ bool walk_load_tail(const WalkArgs& g, unsigned long long item, int s, int k, float x,
                                                Fleet&& fleet, Solve&& solve, Cand& out) {
     const DevFleet& f = g.ld.f;
-    const int e = g.cand_of_pair[k * f.A + (int)(item >> 32)];
+    const int a = (int)(item >> 32), e = g.cand_of_pair[k * f.A + a];
     if (!load_tail(g.ld, e, [&](int) { return total_rate_of(f, k, x); }, solve, out)) return false;
-    if (out.feasible) out.value = penalty_of(fleet(), s, out);
+    if constexpr (Priced) {
+        const DevFleet& fl = fleet();
+        out = priced_at(fl, fl.srv_model[s], a, out);
+        if (out.feasible) out.value = penalty_of(fl, s, out);
+    } else {
+        if (out.feasible) out.value = penalty_of(fleet(), s, out);
+    }
     return true;
 }
 
@@ -1576,6 +1584,10 @@ __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec
 // the resident fleet is f, and every read of a server's rate, tokens or current allocation goes through the row's
 // view, which carries the row's tokens.  The kernels exist once per Trace, overloaded on the argument type, so the
 // load-only calls' kernels keep their names and code.
+//
+// The profile margins (DESIGN.md §3.23) also give each row its own acc_cost and perf_* columns: a ProfileMarginArgs,
+// whose row view adds them (profile_at), whose keys are per (item, accelerator) with a perf column (mg_pair), and
+// whose tail records, sized on the key fleet, are priced at the row before their value.
 // ---------------------------------------------------------------------------
 enum { MG_LO_OPEN = 1, MG_HI_OPEN = 2, MG_TRUNCATED = 4 };  // the header's WVA_MARGIN_*
 
@@ -1597,14 +1609,37 @@ struct TokenMarginArgs : MarginArgs {  // ld: phase 1 on the key fleet, one row 
     const int* out_tokens;
 };
 
-// The resident fleet; item i's row in ld (phase 1's records), for server s; and row l's fleet without c_t.
+struct ProfileMarginArgs : TokenMarginArgs {  // ld: phase 1 on the profile calls' key fleet
+    DevFleet rows;             // acc_cost and perf_* at row 0: the caller's row lists, or f's own columns ...
+    unsigned per_level;        // ... bit c (0: acc_cost, 1 .. 8: perf_* in list order) set: column c is a row list
+    const int* pair_key;       // [n * A] item i's key row in ld for accelerator a, -1: none; NULL: key[i] for every a
+};
+
+// A key that names one row of ld for every accelerator of the item (the load and workload margins), or item i's row
+// per accelerator (the profile margins: pair_key, or key[i] for every accelerator without a perf column).  The
+// profile key holds the item, not a pointer, so that margin_kernel keeps to its registers.
+struct MgPairKey {
+    const ProfileMarginArgs& g;
+    int i;
+};
+__device__ __forceinline__ int mg_pair(int k, int) { return k; }
+__device__ __forceinline__ int mg_pair(const MgPairKey& k, int a) {
+    return k.g.pair_key ? k.g.pair_key[(size_t)k.i * k.g.f.A + a] : k.g.key[k.i];
+}
+
+// The resident fleet; item i's key in ld (phase 1's records), for server s; and row l's fleet without c_t.
 __device__ __forceinline__ const DevFleet& mg_fleet(const MarginArgs& g) { return g.ld.f; }
 __device__ __forceinline__ const DevFleet& mg_fleet(const TokenMarginArgs& g) { return g.f; }
 __device__ __forceinline__ int mg_key(const MarginArgs&, int, int s) { return s; }
 __device__ __forceinline__ int mg_key(const TokenMarginArgs& g, int i, int) { return g.key[i]; }
+__device__ __forceinline__ MgPairKey mg_key(const ProfileMarginArgs& g, int i, int) { return MgPairKey{g, i}; }
 __device__ __forceinline__ const DevFleet& mg_row(const MarginArgs& g, int) { return g.ld.f; }
 __device__ __forceinline__ DevFleet mg_row(const TokenMarginArgs& g, int l) {
     return at_rows(g.f, LoadRows{nullptr, g.in_tokens, g.out_tokens}, l);
+}
+// ... and with row l's acc_cost and perf_* columns (profile_at)
+__device__ __forceinline__ DevFleet mg_row(const ProfileMarginArgs& g, int l) {
+    return at_rows(profile_at(g, l), LoadRows{nullptr, g.in_tokens, g.out_tokens}, l);
 }
 
 // The fleet of row l: on a trace with the current allocation c_t of tick t = l.
@@ -1646,9 +1681,9 @@ __device__ __forceinline__ void mg_chain(const Args& g) {
         }
         __syncwarp();  // c_t is visible to the warp, and the previous tick's reads of acc are done
         const DevFleet ft = mg_view<true>(g, t);
-        const int k = mg_key(g, i, s);
+        const auto k = mg_key(g, i, s);
         const float r = g.rate[i];
-        for (int a = lane; a < A; a += 32) iv_advance(g, ft, t, s, k, a, r, r, acc[a]);
+        for (int a = lane; a < A; a += 32) iv_advance(g, ft, t, s, mg_pair(k, a), a, r, r, acc[a]);
         __syncwarp();
         const int w = iv_winner(acc, A, lane);
         if (w >= 0) {
@@ -1660,6 +1695,7 @@ __device__ __forceinline__ void mg_chain(const Args& g) {
 }
 __global__ void __launch_bounds__(128) margin_chain(MarginArgs g) { mg_chain(g); }
 __global__ void __launch_bounds__(128) margin_chain(TokenMarginArgs g) { mg_chain(g); }
+__global__ void __launch_bounds__(128) margin_chain(ProfileMarginArgs g) { mg_chain(g); }
 
 // nextafterf(x, 0) for x > 0
 __device__ __forceinline__ float mg_below(float x) { return __uint_as_float(__float_as_uint(x) - 1u); }
@@ -1717,7 +1753,8 @@ __device__ __forceinline__ void mg_walk(const Args& g) {
     const int A = mg_fleet(g).A, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
     const int i = blockIdx.x * wpb + wid;
     if (i >= g.n) return;
-    const int l = i / mg_fleet(g).S, s = i - l * mg_fleet(g).S, k = mg_key(g, i, s);
+    const int l = i / mg_fleet(g).S, s = i - l * mg_fleet(g).S;
+    const auto k = mg_key(g, i, s);
     DevFleet ft;
     if constexpr (Rows) ft = mg_view<Trace>(g, l);
     const DevFleet& f = Rows ? ft : g.ld.f;
@@ -1725,7 +1762,7 @@ __device__ __forceinline__ void mg_walk(const Args& g) {
     float* start = (float*)(iv_acc + (size_t)wpb * A) + (size_t)wid * A;
     const float r = g.rate[i], lo = g.lo[i], hi = g.hi[i];
     const float inf = __int_as_float(0x7f800000);
-    auto advance = [&](int a, float x) { iv_advance(g, f, l, s, k, a, x, hi, acc[a]); };
+    auto advance = [&](int a, float x) { iv_advance(g, f, l, s, mg_pair(k, a), a, x, hi, acc[a]); };
     bool over = false;
     for (int a = lane; a < A; a += 32) {
         advance(a, r);
@@ -1814,9 +1851,14 @@ template <bool Trace>
 __global__ void __maxnreg__(96) margin_kernel(MarginArgs g) { mg_walk<Trace>(g); }
 template <bool Trace>
 __global__ void __maxnreg__(96) margin_kernel(TokenMarginArgs g) { mg_walk<Trace>(g); }
+// The profile margins' row view holds eight more row pointers (acc_cost and the perf_* columns of row l) through the
+// walk: at 96 registers ptxas spills 116 bytes, with room for 120 it uses 118 and does not (4 blocks of 128 threads
+// per SM instead of 5).
+template <bool Trace>
+__global__ void __maxnreg__(120) margin_kernel(ProfileMarginArgs g) { mg_walk<Trace>(g); }
 
 // The record r = k * n + i: record k of item i, at the record's rate (r, the float below lo_out, or hi_out), its
-// value on a trace against c_t.
+// value on a trace against c_t.  The profile margins' records are priced at their row and valued on its view.
 template <bool Trace, class Args>
 struct MgTail {
     const Args& g;
@@ -1824,8 +1866,10 @@ struct MgTail {
     __device__ __forceinline__ bool operator()(unsigned long long item, Solve&& solve, Cand& out) const {
         const int r = (int)(unsigned)item, k = r / g.n, i = r - k * g.n, S = mg_fleet(g).S;
         const float x = k == 0 ? g.rate[i] : (k == 1 ? mg_below(g.lo_out[i]) : g.hi_out[i]);
-        const int s = i % S, key = mg_key(g, i, s);
-        if constexpr (Trace) return walk_load_tail(g, item, s, key, x, [&] { return mg_view<true>(g, i / S); }, solve, out);
+        const int s = i % S, key = mg_pair(mg_key(g, i, s), (int)(item >> 32));
+        if constexpr (std::is_same<Args, ProfileMarginArgs>::value)
+            return walk_load_tail<true>(g, item, s, key, x, [&] { return mg_view<Trace>(g, i / S); }, solve, out);
+        else if constexpr (Trace) return walk_load_tail(g, item, s, key, x, [&] { return mg_view<true>(g, i / S); }, solve, out);
         else return walk_load_tail(g, item, s, key, x, [&]() -> const DevFleet& { return mg_fleet(g); }, solve, out);
     }
     __device__ __forceinline__ size_t record(unsigned long long item) const { return (unsigned)item; }
@@ -1837,11 +1881,19 @@ template <bool Trace>
 __global__ void __launch_bounds__(256) margin_tail(TokenMarginArgs g) {
     walk_tail(g, MgTail<Trace, TokenMarginArgs>{g});
 }
+template <bool Trace>
+__global__ void __launch_bounds__(256) margin_tail(ProfileMarginArgs g) {
+    walk_tail(g, MgTail<Trace, ProfileMarginArgs>{g});
+}
 
 // Stored-vector re-run of the records margin_tail bailed on.
 template <bool Trace>
 __global__ void margin_fallback(MarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace, MarginArgs>{g}); }
 template <bool Trace>
 __global__ void margin_fallback(TokenMarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace, TokenMarginArgs>{g}); }
+template <bool Trace>
+__global__ void margin_fallback(ProfileMarginArgs g, FbRun r) {
+    tail_rerun(r, g.rec, MgTail<Trace, ProfileMarginArgs>{g});
+}
 
 }  // namespace wva

@@ -187,7 +187,8 @@ def within_margins(lo, hi, flags, new_rpm, rpm_hi):
     It works unchanged on ``Engine.load_margin_trace``'s result: there the servers inside their stretch at tick t
     keep the decision the replayed reconcile makes at tick t.  On ``Engine.workload_margins`` and
     ``Engine.workload_margin_trace`` a new rate inside the stretch keeps the row's decision when the new tokens equal
-    the row's; the mask does not look at tokens."""
+    the row's; the mask does not look at tokens.  On ``Engine.profile_margins`` and ``Engine.profile_margin_trace``
+    it holds when the tokens, prices and profiles also stay the row's."""
     lo, hi, top, x = (np.asarray(v, np.float32) for v in (lo, hi, rpm_hi, new_rpm))
     flags = np.asarray(flags, np.uint8)
     if not lo.shape == hi.shape == flags.shape == top.shape == x.shape:
@@ -551,12 +552,51 @@ class Engine:
         return self._margins(self._L.wva_workload_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens,
                              out_tokens)
 
-    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi, *tokens):
+    def profile_margins(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, rpm_lo=None, rpm_hi=None,
+                        *, acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None, perf_gamma=None,
+                        perf_delta=None, perf_acc_count=None, perf_max_batch=None, perf_at_tokens=None):
+        """``workload_margins`` at rows that also carry their own accelerator costs (``acc_cost``, shape (L, A)) and
+        performance profiles (``perf_*``, shape (L, M, A)), as ``profile_trace`` takes them -> the same tuple as
+        ``load_margins``.  A list of ``None`` is the fleet's own column at every level.
+
+        Block ``l`` is ``load_margins`` with one level (row ``l`` of the rates and of the windows, by default
+        ``[0, 2 * rate]``) on the fleet with every given column = row ``l``, and the ``at`` records are
+        ``profile_trace``'s winner for each row alone; each distinct (server, accelerator, in, out, alpha .. delta,
+        batch size) under a window top above 0 is sized once (see ``wva_profile_margins`` in include/wva_b200.h).
+        ``srv_cur_cost`` is not re-priced.  A new rate inside ``[lo, hi)`` keeps the row's decision when the tokens,
+        prices and profiles stay the row's."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        profile = dict(zip(_PROFILE_COLUMNS, (acc_cost, perf_present, perf_alpha, perf_beta, perf_gamma, perf_delta,
+                                              perf_acc_count, perf_max_batch, perf_at_tokens)))
+        return self._margins(self._L.wva_profile_margins, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens, out_tokens,
+                             profile=profile)
+
+    def profile_margin_trace(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, rpm_lo=None,
+                             rpm_hi=None, *, acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None,
+                             perf_gamma=None, perf_delta=None, perf_acc_count=None, perf_max_batch=None,
+                             perf_at_tokens=None):
+        """``profile_margins`` at every tick of ``profile_trace`` over the same rows -> the same tuple as
+        ``load_margins``.
+
+        Block ``t`` is ``profile_margins`` with one level on the fleet whose current allocation is the one the trace
+        carries into tick ``t`` (``fleet.apply_winners`` of every earlier tick's ``at`` in turn, each cost at its own
+        tick's prices), and the ``at`` records are ``profile_trace``'s winners (see ``wva_profile_margin_trace`` in
+        include/wva_b200.h)."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        profile = dict(zip(_PROFILE_COLUMNS, (acc_cost, perf_present, perf_alpha, perf_beta, perf_gamma, perf_delta,
+                                              perf_acc_count, perf_max_batch, perf_at_tokens)))
+        return self._margins(self._L.wva_profile_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens,
+                             out_tokens, profile=profile)
+
+    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi, *tokens, profile=None):
         """wva_load_margins / wva_load_margin_trace over (L, S) rows and windows, or with `tokens` (in_tokens,
-        out_tokens; None: the fleet's own) wva_workload_margins / wva_workload_margin_trace; the output arrays."""
+        out_tokens; None: the fleet's own) wva_workload_margins / wva_workload_margin_trace, and with `profile` as
+        well ({column: rows or None}) wva_profile_margins / wva_profile_margin_trace; the output arrays."""
         S = fleet.n_servers
         rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "rpm_lo": rpm_lo, "rpm_hi": rpm_hi,
-                                     **dict(zip(("in_tokens", "out_tokens"), tokens))})
+                                     **dict(zip(("in_tokens", "out_tokens"), tokens)), **(profile or {})})
         L = 1 if L is None else L
         rate = rows.get("arrival_rpm", np.ascontiguousarray(np.broadcast_to(fleet.srv_arrival_rpm, (L, S)), np.float32))
         lo = rows.get("rpm_lo", np.zeros((L, S), np.float32))
@@ -570,6 +610,9 @@ class Engine:
         self._resident(fleet)
         token_rows = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None
                       for k in ("in_tokens", "out_tokens")[:len(tokens)]]
+        if profile is not None:
+            rc_ = _profile_rows_c(rows)
+            token_rows.append(C.byref(rc_))
         self._check(call(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)), *token_rows, _abi.ptr(lo.reshape(-1)),
                          _abi.ptr(hi.reshape(-1)), C.byref(oc)))
         return lo_out, hi_out, flags, at, below, above
