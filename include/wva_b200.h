@@ -778,6 +778,58 @@ int wva_profile_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ti
                              const float *rpm_lo, const float *rpm_hi, wva_margins *out);
 
 /*
+ * SLO margins: wva_workload_margins and wva_workload_margin_trace at rows that also carry their own ITL, TTFT and
+ * TPS targets, as wva_slo_trace takes them: a premium class whose ITL is tightened during business hours, or a
+ * proposed target change replayed over recorded traffic.  A planner sees how far the load of each row may stray at
+ * that row's targets.  Without this call that takes one wva_load_margins per row, each re-uploading and re-sizing the
+ * fleet with its srv_slo_* columns rewritten.
+ *
+ * Rows: arrival_rpm, in_tokens, out_tokens, slo_itl, slo_ttft, slo_tps, rpm_lo and rpm_hi are [L*S], index l*S + s,
+ * with L = n_levels or n_ticks, as in wva_slo_trace; every column of out is [L*S].  arrival_rpm is required; a NULL
+ * token or target list is the fleet's own column at every row.
+ *   - Grid, level l.  Let f_l be the fleet with srv_arrival_rpm, srv_in_tokens, srv_out_tokens, srv_slo_itl,
+ *     srv_slo_ttft and srv_slo_tps replaced by row l.  Block l of lo_rpm, hi_rpm, flags, at, below and above is byte
+ *     for byte wva_load_margins(f_l) with one level: rate row l, window row l.  The `at` blocks are wva_slo_trace's
+ *     winner for each row alone (one tick on f_l); with arrival_rpm the fleet's own column at every row and NULL
+ *     token lists they are wva_slo_grid's winners.
+ *   - Trace, tick t.  Let f_t be that fleet with row t and srv_cur_* = c_t, the allocation wva_slo_trace carries into
+ *     tick t on the same rows.  Block t is byte for byte wva_load_margins(f_t) with one level, and the `at` blocks
+ *     are wva_slo_trace's winners.  The trace continues as wva_slo_trace's does: ticks 0..L-1 equal ticks 0..k-1
+ *     followed by ticks k..L-1 on the fleet whose srv_cur_* hold c_k.
+ *   - With all three target lists NULL the result is byte for byte wva_workload_margins (grid) or
+ *     wva_workload_margin_trace (trace) on the same load rows and windows, with the same launch count.
+ * A new rate inside [lo_rpm, hi_rpm) keeps the row's decision when the tokens and targets stay the row's.
+ *
+ * Sizing (DESIGN.md §3.24): QueueAnalyzer.Size reads the ITL and TTFT targets and whether the TPS target is positive,
+ * and the tail's totalRate reads the TPS target; none of them reads the rate.  So a pair's phase-1 record at row l is
+ * fixed by (s, a, in_l, out_l, bits of ITL_l, TTFT_l and TPS_l), and each distinct key is sized once over the rows
+ * whose window top rpm_hi is above 0 and whose tokens class a pair as a load (in_tokens >= 0, out_tokens >= 1); on a
+ * trace with keepAccelerator honoured on the pinned servers only.  With NULL target lists the keys are
+ * wva_workload_margins' (server, in, out) rows, and the call sizes the same pairs in the same order.  A key with a
+ * negative target is sized like any other (Size makes its pairs nil), as wva_load_margins(f_l) sizes it.
+ *
+ * Only unlimited mode is covered; fleet->unlimited and the capacities are not read, nor are srv_arrival_rpm and the
+ * columns whose row lists are given.  srv_has_target still gates a server's pairs.  The fleet becomes resident, and
+ * wva_summarize returns WVA_ERR_STATE afterwards.  Columns of at, below and above may be NULL (not written).  L == 0
+ * and S == 0 are valid (nothing is written).  WVA_ERR_BAD_ARG: L < 0, out NULL, arrival_rpm, rpm_lo, rpm_hi, lo_rpm,
+ * hi_rpm or flags NULL with S*L > 0, or a row that wva_load_margins refuses.  WVA_ERR_UNSUPPORTED: 3*S*L >= 2^31
+ * (refused before the fleet is read); distinct key pairs x A >= 2^31; or, for the grid, exactly where
+ * wva_load_margins(f_l) refuses at some level l, a NaN or tiny TPS target under a window top above 0 among them.  A
+ * key used only at rows whose window is [0, 0] is never sized and does not fail the call.  The trace's refusals can
+ * be larger than the union over t of what wva_load_margins(f_t) refuses, but only through the pairs of a server that
+ * is not pinned yet has keepAccelerator set.  The call never returns a result that differs from the per-row
+ * composition.
+ */
+int wva_slo_margins(wva_handle *h, const wva_fleet *fleet, int32_t n_levels, const float *arrival_rpm,
+                    const int32_t *in_tokens, const int32_t *out_tokens,
+                    const float *slo_itl, const float *slo_ttft, const float *slo_tps,
+                    const float *rpm_lo, const float *rpm_hi, wva_margins *out);
+int wva_slo_margin_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks, const float *arrival_rpm,
+                         const int32_t *in_tokens, const int32_t *out_tokens,
+                         const float *slo_itl, const float *slo_ttft, const float *slo_tps,
+                         const float *rpm_lo, const float *rpm_hi, wva_margins *out);
+
+/*
  * Price thresholds: for each server s and accelerator a, the exact accelerator price at which s's unlimited
  * winner leaves a.  Let f(p) be the fleet with acc_cost[a] = p, solved in unlimited mode.
  *

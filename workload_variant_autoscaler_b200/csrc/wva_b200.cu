@@ -1161,22 +1161,42 @@ struct KeyFleet {
     }
 };
 
+// [L*S] lists of the ITL, TTFT and TPS targets by row: the SLO margins' (DESIGN.md §3.24), all three given.
+struct TargetRows {
+    const float* itl;
+    const float* ttft;
+    const float* tps;
+};
+
+// A key of load_groups: (in << 32) | out, then the bits of (ITL << 32) | TTFT and of TPS (0 without target rows).
+using LoadKey = std::array<uint64_t, 3>;
+using LoadUses = std::vector<std::pair<LoadKey, int>>;
+
 // The levels at which server s is a load under the rows rpm / in / out [L*S] (rate not negative and not 0, NaN and
-// +Inf included; in_tokens >= 0; out_tokens >= 1), as ((in << 32) | out, level) in `uses`, sorted; then
-// group(in, out, u0, u1) for each (in, out) in ascending order, whose levels are uses[u0 .. u1), ascending.
+// +Inf included; in_tokens >= 0; out_tokens >= 1), as (key, level) in `uses`, sorted, the key being the level's
+// tokens and, with tg, its targets' bits; then group(in, out, u0, u1) for each key in ascending order, whose levels
+// are uses[u0 .. u1), ascending.  Without tg the keys are the (in, out) pairs.
 template <class Group>
-void load_groups(int L, int S, int s, const float* rpm, const int32_t* in, const int32_t* out,
-                 std::vector<std::pair<uint64_t, int>>& uses, Group&& group) {
+void load_groups(int L, int S, int s, const float* rpm, const int32_t* in, const int32_t* out, LoadUses& uses,
+                 Group&& group, const TargetRows* tg = nullptr) {
+    const auto bits = [](float x) {
+        uint32_t u;
+        memcpy(&u, &x, 4);
+        return (uint64_t)u;
+    };
     uses.clear();
     for (int l = 0; l < L; ++l) {
         const size_t i = (size_t)l * S + s;
-        if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1)
-            uses.emplace_back((uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], l);
+        if (!(rpm[i] < 0.0f) && rpm[i] != 0.0f && in[i] >= 0 && out[i] >= 1) {
+            LoadKey k{(uint64_t)(uint32_t)in[i] << 32 | (uint32_t)out[i], 0, 0};
+            if (tg) k = {k[0], bits(tg->itl[i]) << 32 | bits(tg->ttft[i]), bits(tg->tps[i])};
+            uses.emplace_back(k, l);
+        }
     }
     std::sort(uses.begin(), uses.end());
     for (size_t u0 = 0, u1; u0 < uses.size(); u0 = u1) {
         for (u1 = u0; u1 < uses.size() && uses[u1].first == uses[u0].first;) ++u1;
-        group((int)(uses[u0].first >> 32), (int)(uint32_t)uses[u0].first, u0, u1);
+        group((int)(uses[u0].first[0] >> 32), (int)(uint32_t)uses[u0].first[0], u0, u1);
     }
 }
 
@@ -1228,18 +1248,30 @@ struct TokenKeys {
 };
 // The workload grid's keys (DESIGN.md §3.12) of the rows rpm / in / out into tk: per server, its distinct (in, out)
 // under load, ascending.  Returns their key fleet, which with pin (a trace's trace_pinned flags) keeps
-// keepAccelerator on the pinned servers only, so that phase 1 sizes their current accelerator alone.
+// keepAccelerator on the pinned servers only, so that phase 1 sizes their current accelerator alone.  With tg (the SLO
+// margins, DESIGN.md §3.24) the keys are per server its distinct (in, out, target bits), and the key fleet's srv_slo_*
+// columns hold each key's targets.
 KeyFleet workload_keys(const HostFleet& hf, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                       const uint8_t* pin, TokenKeys& tk) {
-    std::vector<std::pair<uint64_t, int>> uses;
+                       const uint8_t* pin, TokenKeys& tk, const TargetRows* tg = nullptr) {
+    LoadUses uses;
     for (int s = 0; s < hf.S; ++s)
-        load_groups(L, hf.S, s, rpm, in, out, uses, [&](int ki, int ko, size_t u0, size_t u1) {
-            tk.add(s, ki, ko);
-            for (size_t u = u0; u < u1; ++u) tk.add_level(uses[u].second);
-        });
+        load_groups(
+            L, hf.S, s, rpm, in, out, uses,
+            [&](int ki, int ko, size_t u0, size_t u1) {
+                tk.add(s, ki, ko);
+                for (size_t u = u0; u < u1; ++u) tk.add_level(uses[u].second);
+            },
+            tg);
     KeyFleet kf(hf, tk.srv, tk.in, tk.out);
     if (pin)
         for (size_t k = 0; k < tk.srv.size(); ++k) kf.hf.srv_keep_acc[k] = pin[tk.srv[k]];
+    if (tg)
+        for (size_t k = 0; k < tk.srv.size(); ++k) {
+            const size_t i = (size_t)tk.lev[tk.lev_off[k]] * hf.S + tk.srv[k];  // the key's first row
+            kf.hf.srv_slo_itl[k] = tg->itl[i];
+            kf.hf.srv_slo_ttft[k] = tg->ttft[i];
+            kf.hf.srv_slo_tps[k] = tg->tps[i];
+        }
     return kf;
 }
 
@@ -1381,7 +1413,7 @@ void profile_keys(const HostFleet& hf, const ProfileRanks& pr, int L, const floa
                   const int32_t* out, Skip&& skip, TokenKeys& tk, std::vector<int>& key_acc,
                   std::vector<int>& key_model) {
     const int S = hf.S, A = hf.A, M = hf.M;
-    std::vector<std::pair<uint64_t, int>> uses;                 // ((in << 32) | out, row)
+    LoadUses uses;                                              // (tokens key, row)
     std::vector<std::pair<std::array<uint64_t, 3>, int>> prof;  // (sizing key, row)
     for (int s = 0; s < S; ++s) {
         const int m = hf.srv_model[s];
@@ -1563,7 +1595,7 @@ static_assert(MG_LO_OPEN == WVA_MARGIN_LO_OPEN && MG_HI_OPEN == WVA_MARGIN_HI_OP
 
 // margin_kernel, margin_tail and margin_fallback of g (the Trace instantiations on a trace, after margin_chain): one
 // warp per (level, server), A accelerator states and stretch starts per warp in shared memory.  Args is MarginArgs,
-// or TokenMarginArgs for the workload margins.
+// or TokenMarginArgs, ProfileMarginArgs or SloMarginArgs for the workload, profile and SLO margins.
 template <class Args>
 int launch_margins(wva_handle* h, const Args& g, bool trace, const FbRun& fb) {
     const size_t per_warp = (sizeof(IvAcc) + sizeof(float)) * (size_t)h->hf.A;
@@ -1604,9 +1636,15 @@ int launch_margins(wva_handle* h, const Args& g, bool trace, const FbRun& fb) {
 // (profile_keys, with the window tops as rates): one key row per key pair, so the key column [L*S*A] names each
 // (row, server, accelerator)'s key row (-1: none).  keepAccelerator masks a pair at every row on the grid, and on a
 // trace only on the pinned servers.
+//
+// With `slo` (the SLO margins, DESIGN.md §3.24) row l also has its own ITL, TTFT and TPS targets (NULL: the fleet's
+// own column).  Size reads the ITL and TTFT targets and whether TPS is positive, and the tail's totalRate reads the
+// TPS target, none of them the rate, so the keys are the workload margins' refined by the row's target bits
+// (workload_keys with the target rows), and the key fleet carries each key's targets.  The kernels read the rows'
+// targets through the row's view.
 int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t* in, const int32_t* out, bool tokens,
-                         const wva_profile_rows* prof, const float* lo, const float* hi, ProfileMarginArgs& g,
-                         size_t rec_bytes, bool trace) {
+                         const wva_profile_rows* prof, const TargetRows* slo, const float* lo, const float* hi,
+                         ProfileMarginArgs& g, size_t rec_bytes, bool trace) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     Cols c(16);
@@ -1619,6 +1657,8 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t*
     size_t o_key = 0;
     if (tokens) {
         lists.put_tokens(in, out);
+        if (slo) lists.put_targets(slo->itl, slo->ttft, slo->tps);
+        const TargetRows tg{lists.itl.host, lists.ttft.host, lists.tps.host};
         const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
         if (prof) pr.emplace(hf, L, *prof);
         if (pr && pr->perf_rows) {
@@ -1638,10 +1678,13 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t*
                 for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j)
                     key[((size_t)tk.lev[j] * S + tk.srv[k]) * A + key_acc[k]] = (int)k;
         } else {
-            kf.emplace(workload_keys(hf, L, hi, lists.in.host, lists.out.host, trace ? pin.data() : nullptr, tk));
+            kf.emplace(workload_keys(hf, L, hi, lists.in.host, lists.out.host, trace ? pin.data() : nullptr, tk,
+                                     slo ? &tg : nullptr));
             // the keys' pairs are indexed in int32 on the device
             if ((long long)tk.srv.size() * A >= (1ll << 31))
-                return h->fail(WVA_ERR_UNSUPPORTED, "workload margins: too many token keys for one call (K*A >= 2^31)");
+                return h->fail(WVA_ERR_UNSUPPORTED,
+                               slo ? "SLO margins: too many keys for one call (K*A >= 2^31)"
+                                   : "workload margins: too many token keys for one call (K*A >= 2^31)");
             key.assign((size_t)L * S, -1);
             for (size_t k = 0; k < tk.srv.size(); ++k)
                 for (int j = tk.lev_off[k]; j < tk.lev_off[k + 1]; ++j) key[(size_t)tk.lev[j] * S + tk.srv[k]] = (int)k;
@@ -1661,6 +1704,10 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t*
     g.key = (const int*)(d + o_key);
     g.in_tokens = lists.in.dev(d);
     g.out_tokens = lists.out.dev(d);
+    if (slo) {
+        const SloMarginArgs sg{g, lists.itl.dev(d), lists.ttft.dev(d), lists.tps.dev(d)};
+        return launch_margins(h, sg, trace, ls.fb2);
+    }
     if (!pr) return launch_margins(h, static_cast<const TokenMarginArgs&>(g), trace, ls.fb2);
     pr->set_rows(g, d);
     g.pair_key = pr->perf_rows ? g.key : nullptr;
@@ -1669,10 +1716,11 @@ int enqueue_load_margins(wva_handle* h, int L, const float* rate, const int32_t*
 
 // wva_load_margins, or with `trace` wva_load_margin_trace; with `tokens` wva_workload_margins or
 // wva_workload_margin_trace (in / out: NULL is the fleet's own column), and with `prof` as well
-// wva_profile_margins or wva_profile_margin_trace.  All but wva_load_margins require the rate rows.
+// wva_profile_margins or wva_profile_margin_trace, or with `slo` (its lists NULL: the fleet's own column)
+// wva_slo_margins or wva_slo_margin_trace.  All but wva_load_margins require the rate rows.
 int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                       const int32_t* in_tokens, const int32_t* out_tokens, bool tokens, const wva_profile_rows* prof,
-                      const float* rpm_lo, const float* rpm_hi, wva_margins* out, bool trace) {
+                      const TargetRows* slo, const float* rpm_lo, const float* rpm_hi, wva_margins* out, bool trace) {
     if (!h) return WVA_ERR_BAD_ARG;
     if (!out) return h->fail(WVA_ERR_BAD_ARG, "out is NULL");
     if (n_levels < 0) return h->fail(WVA_ERR_BAD_ARG, trace ? "negative tick count" : "negative level count");
@@ -1709,8 +1757,8 @@ int load_margins_call(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, c
                             g.cur_replicas = (int*)(d + o_cur) + n;
                             g.cur_cost = (float*)(d + o_cur) + 2 * (size_t)n;
                         }
-                        return enqueue_load_margins(h, L, arrival_rpm, in_tokens, out_tokens, tokens, prof, rpm_lo,
-                                                    rpm_hi, g, rec_bytes, trace);
+                        return enqueue_load_margins(h, L, arrival_rpm, in_tokens, out_tokens, tokens, prof, slo,
+                                                    rpm_lo, rpm_hi, g, rec_bytes, trace);
                     });
 }
 
@@ -3386,43 +3434,60 @@ int wva_load_intervals(wva_handle* h, const wva_fleet* fleet, const float* rpm_l
 
 int wva_load_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                      const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_levels, arrival_rpm, nullptr, nullptr, false, nullptr, rpm_lo, rpm_hi, out,
-                             false);
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, nullptr, nullptr, false, nullptr, nullptr, rpm_lo, rpm_hi,
+                             out, false);
 }
 
 int wva_load_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                           const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_ticks, arrival_rpm, nullptr, nullptr, false, nullptr, rpm_lo, rpm_hi, out,
-                             true);
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, nullptr, nullptr, false, nullptr, nullptr, rpm_lo, rpm_hi,
+                             out, true);
 }
 
 int wva_workload_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                          const int32_t* in_tokens, const int32_t* out_tokens, const float* rpm_lo, const float* rpm_hi,
                          wva_margins* out) {
-    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, nullptr, rpm_lo, rpm_hi, out,
-                             false);
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, nullptr, nullptr, rpm_lo,
+                             rpm_hi, out, false);
 }
 
 int wva_workload_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                               const int32_t* in_tokens, const int32_t* out_tokens, const float* rpm_lo,
                               const float* rpm_hi, wva_margins* out) {
-    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, nullptr, rpm_lo, rpm_hi, out,
-                             true);
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, nullptr, nullptr, rpm_lo,
+                             rpm_hi, out, true);
 }
 
 int wva_profile_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                         const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
                         const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
     const wva_profile_rows own{};
-    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, rows ? rows : &own, rpm_lo,
-                             rpm_hi, out, false);
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, rows ? rows : &own, nullptr,
+                             rpm_lo, rpm_hi, out, false);
 }
 
 int wva_profile_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                              const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
                              const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
     const wva_profile_rows own{};
-    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, rows ? rows : &own, rpm_lo,
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, rows ? rows : &own, nullptr,
+                             rpm_lo, rpm_hi, out, true);
+}
+
+int wva_slo_margins(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                    const int32_t* in_tokens, const int32_t* out_tokens, const float* slo_itl, const float* slo_ttft,
+                    const float* slo_tps, const float* rpm_lo, const float* rpm_hi, wva_margins* out) {
+    const TargetRows slo{slo_itl, slo_ttft, slo_tps};
+    return load_margins_call(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, true, nullptr, &slo, rpm_lo,
+                             rpm_hi, out, false);
+}
+
+int wva_slo_margin_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
+                         const int32_t* in_tokens, const int32_t* out_tokens, const float* slo_itl,
+                         const float* slo_ttft, const float* slo_tps, const float* rpm_lo, const float* rpm_hi,
+                         wva_margins* out) {
+    const TargetRows slo{slo_itl, slo_ttft, slo_tps};
+    return load_margins_call(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, true, nullptr, &slo, rpm_lo,
                              rpm_hi, out, true);
 }
 

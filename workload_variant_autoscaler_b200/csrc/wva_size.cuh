@@ -1588,6 +1588,10 @@ __global__ void interval_fallback(IntervalArgs g, FbRun r) { tail_rerun(r, g.rec
 // The profile margins (DESIGN.md §3.23) also give each row its own acc_cost and perf_* columns: a ProfileMarginArgs,
 // whose row view adds them (profile_at), whose keys are per (item, accelerator) with a perf column (mg_pair), and
 // whose tail records, sized on the key fleet, are priced at the row before their value.
+//
+// The SLO margins (DESIGN.md §3.24) give each row its own ITL, TTFT and TPS targets: an SloMarginArgs, whose row view
+// adds them, so that pair_class, iv_state's totalRate and mg_start's TPS test read row l's.  Its keys are the
+// workload margins' refined by the targets' bits, one per item, and the key fleet carries each key's targets.
 // ---------------------------------------------------------------------------
 enum { MG_LO_OPEN = 1, MG_HI_OPEN = 2, MG_TRUNCATED = 4 };  // the header's WVA_MARGIN_*
 
@@ -1615,6 +1619,12 @@ struct ProfileMarginArgs : TokenMarginArgs {  // ld: phase 1 on the profile call
     const int* pair_key;       // [n * A] item i's key row in ld for accelerator a, -1: none; NULL: key[i] for every a
 };
 
+struct SloMarginArgs : TokenMarginArgs {  // ld: phase 1 on the key fleet, one row per (server, tokens, targets) key
+    const float* slo_itl;      // [n] the rows' targets, index l * S + s
+    const float* slo_ttft;
+    const float* slo_tps;
+};
+
 // A key that names one row of ld for every accelerator of the item (the load and workload margins), or item i's row
 // per accelerator (the profile margins: pair_key, or key[i] for every accelerator without a perf column).  The
 // profile key holds the item, not a pointer, so that margin_kernel keeps to its registers.
@@ -1640,6 +1650,15 @@ __device__ __forceinline__ DevFleet mg_row(const TokenMarginArgs& g, int l) {
 // ... and with row l's acc_cost and perf_* columns (profile_at)
 __device__ __forceinline__ DevFleet mg_row(const ProfileMarginArgs& g, int l) {
     return at_rows(profile_at(g, l), LoadRows{nullptr, g.in_tokens, g.out_tokens}, l);
+}
+// ... and with row l's ITL, TTFT and TPS targets
+__device__ __forceinline__ DevFleet mg_row(const SloMarginArgs& g, int l) {
+    DevFleet fl = at_rows(g.f, LoadRows{nullptr, g.in_tokens, g.out_tokens}, l);
+    const size_t o = (size_t)l * g.f.S;
+    fl.srv_slo_itl = g.slo_itl + o;
+    fl.srv_slo_ttft = g.slo_ttft + o;
+    fl.srv_slo_tps = g.slo_tps + o;
+    return fl;
 }
 
 // The fleet of row l: on a trace with the current allocation c_t of tick t = l.
@@ -1696,6 +1715,7 @@ __device__ __forceinline__ void mg_chain(const Args& g) {
 __global__ void __launch_bounds__(128) margin_chain(MarginArgs g) { mg_chain(g); }
 __global__ void __launch_bounds__(128) margin_chain(TokenMarginArgs g) { mg_chain(g); }
 __global__ void __launch_bounds__(128) margin_chain(ProfileMarginArgs g) { mg_chain(g); }
+__global__ void __launch_bounds__(128) margin_chain(SloMarginArgs g) { mg_chain(g); }
 
 // nextafterf(x, 0) for x > 0
 __device__ __forceinline__ float mg_below(float x) { return __uint_as_float(__float_as_uint(x) - 1u); }
@@ -1856,6 +1876,11 @@ __global__ void __maxnreg__(96) margin_kernel(TokenMarginArgs g) { mg_walk<Trace
 // per SM instead of 5).
 template <bool Trace>
 __global__ void __maxnreg__(120) margin_kernel(ProfileMarginArgs g) { mg_walk<Trace>(g); }
+// The SLO margins' row view holds three more row pointers (the targets of row l) through the walk: at 96 registers
+// ptxas spills 4 bytes in the grid's instantiation, with room for 104 it uses 100 and does not (4 blocks of 128
+// threads per SM instead of 5); the trace's uses 96 either way.
+template <bool Trace>
+__global__ void __maxnreg__(104) margin_kernel(SloMarginArgs g) { mg_walk<Trace>(g); }
 
 // The record r = k * n + i: record k of item i, at the record's rate (r, the float below lo_out, or hi_out), its
 // value on a trace against c_t.  The profile margins' records are priced at their row and valued on its view.
@@ -1885,6 +1910,8 @@ template <bool Trace>
 __global__ void __launch_bounds__(256) margin_tail(ProfileMarginArgs g) {
     walk_tail(g, MgTail<Trace, ProfileMarginArgs>{g});
 }
+template <bool Trace>
+__global__ void __launch_bounds__(256) margin_tail(SloMarginArgs g) { walk_tail(g, MgTail<Trace, SloMarginArgs>{g}); }
 
 // Stored-vector re-run of the records margin_tail bailed on.
 template <bool Trace>
@@ -1895,5 +1922,7 @@ template <bool Trace>
 __global__ void margin_fallback(ProfileMarginArgs g, FbRun r) {
     tail_rerun(r, g.rec, MgTail<Trace, ProfileMarginArgs>{g});
 }
+template <bool Trace>
+__global__ void margin_fallback(SloMarginArgs g, FbRun r) { tail_rerun(r, g.rec, MgTail<Trace, SloMarginArgs>{g}); }
 
 }  // namespace wva

@@ -188,7 +188,8 @@ def within_margins(lo, hi, flags, new_rpm, rpm_hi):
     keep the decision the replayed reconcile makes at tick t.  On ``Engine.workload_margins`` and
     ``Engine.workload_margin_trace`` a new rate inside the stretch keeps the row's decision when the new tokens equal
     the row's; the mask does not look at tokens.  On ``Engine.profile_margins`` and ``Engine.profile_margin_trace``
-    it holds when the tokens, prices and profiles also stay the row's."""
+    it holds when the tokens, prices and profiles also stay the row's, and on ``Engine.slo_margins`` and
+    ``Engine.slo_margin_trace`` when the tokens and targets do."""
     lo, hi, top, x = (np.asarray(v, np.float32) for v in (lo, hi, rpm_hi, new_rpm))
     flags = np.asarray(flags, np.uint8)
     if not lo.shape == hi.shape == flags.shape == top.shape == x.shape:
@@ -590,13 +591,43 @@ class Engine:
         return self._margins(self._L.wva_profile_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens,
                              out_tokens, profile=profile)
 
-    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi, *tokens, profile=None):
+    def slo_margins(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, rpm_lo=None, rpm_hi=None, *,
+                    slo_itl=None, slo_ttft=None, slo_tps=None):
+        """``workload_margins`` at rows that also carry their own service-class targets (``slo_itl``, ``slo_ttft``,
+        ``slo_tps``, shape (L, S), in the fleet columns' units), as ``slo_trace`` takes them -> the same tuple as
+        ``load_margins``.  A list of ``None`` is the fleet's own column at every level.
+
+        Block ``l`` is ``load_margins`` with one level (row ``l`` of the rates and of the windows, by default
+        ``[0, 2 * rate]``) on the fleet with every given column = row ``l``, and the ``at`` records are
+        ``slo_trace``'s winner for each row alone; each distinct (server, in, out, ITL, TTFT, TPS) under a window top
+        above 0 is sized once (see ``wva_slo_margins`` in include/wva_b200.h).  A new rate inside ``[lo, hi)`` keeps
+        the row's decision when the tokens and targets stay the row's."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        return self._margins(self._L.wva_slo_margins, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens, out_tokens,
+                             slo={"slo_itl": slo_itl, "slo_ttft": slo_ttft, "slo_tps": slo_tps})
+
+    def slo_margin_trace(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, rpm_lo=None, rpm_hi=None,
+                         *, slo_itl=None, slo_ttft=None, slo_tps=None):
+        """``slo_margins`` at every tick of ``slo_trace`` over the same rows -> the same tuple as ``load_margins``.
+
+        Block ``t`` is ``slo_margins`` with one level on the fleet whose current allocation is the one the trace
+        carries into tick ``t`` (``fleet.apply_winners`` of every earlier tick's ``at`` in turn), and the ``at``
+        records are ``slo_trace``'s winners (see ``wva_slo_margin_trace`` in include/wva_b200.h)."""
+        if arrival_rpm is None:
+            raise ValueError("arrival_rpm is required")
+        return self._margins(self._L.wva_slo_margin_trace, fleet, arrival_rpm, rpm_lo, rpm_hi, in_tokens, out_tokens,
+                             slo={"slo_itl": slo_itl, "slo_ttft": slo_ttft, "slo_tps": slo_tps})
+
+    def _margins(self, call, fleet, arrival_rpm, rpm_lo, rpm_hi, *tokens, profile=None, slo=None):
         """wva_load_margins / wva_load_margin_trace over (L, S) rows and windows, or with `tokens` (in_tokens,
         out_tokens; None: the fleet's own) wva_workload_margins / wva_workload_margin_trace, and with `profile` as
-        well ({column: rows or None}) wva_profile_margins / wva_profile_margin_trace; the output arrays."""
+        well ({column: rows or None}) wva_profile_margins / wva_profile_margin_trace, or with `slo` ({target: rows
+        or None}) wva_slo_margins / wva_slo_margin_trace; the output arrays."""
         S = fleet.n_servers
         rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "rpm_lo": rpm_lo, "rpm_hi": rpm_hi,
-                                     **dict(zip(("in_tokens", "out_tokens"), tokens)), **(profile or {})})
+                                     **dict(zip(("in_tokens", "out_tokens"), tokens)), **(profile or {}),
+                                     **(slo or {})})
         L = 1 if L is None else L
         rate = rows.get("arrival_rpm", np.ascontiguousarray(np.broadcast_to(fleet.srv_arrival_rpm, (L, S)), np.float32))
         lo = rows.get("rpm_lo", np.zeros((L, S), np.float32))
@@ -613,6 +644,8 @@ class Engine:
         if profile is not None:
             rc_ = _profile_rows_c(rows)
             token_rows.append(C.byref(rc_))
+        if slo is not None:
+            token_rows += [_abi.ptr(rows[k].reshape(-1)) if k in rows else None for k in slo]
         self._check(call(self._h, C.byref(fc), L, _abi.ptr(rate.reshape(-1)), *token_rows, _abi.ptr(lo.reshape(-1)),
                          _abi.ptr(hi.reshape(-1)), C.byref(oc)))
         return lo_out, hi_out, flags, at, below, above
