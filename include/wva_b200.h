@@ -901,6 +901,53 @@ int wva_price_threshold_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_t
                               wva_allocs *candidates /* [L*S*A], may be NULL */, wva_allocs *winners /* [L*S] */);
 
 /*
+ * Profile price thresholds: the price threshold grid and trace at rows that also carry their own accelerator costs
+ * and performance profiles, e.g. a day of hourly prices on every accelerator, an AccCount or beta change after an
+ * upgrade, or an accelerator that comes online at some hour.  The load rows are laid out as in
+ * wva_price_threshold_grid, the profile rows as in wva_profile_trace (acc_cost [L*A], each perf_* [L*M*A]).
+ * arrival_rpm is required; a NULL token list, a NULL profile column or rows == NULL is the fleet's own column at every
+ * row.  The output layout is wva_price_threshold_grid's.
+ *
+ *   - Grid, level l.  Let f_l be the fleet with row l of the three load lists, of acc_cost and of the nine perf_*
+ *     columns.  Block l of threshold, above and candidates is byte for byte what wva_price_thresholds(f_l) returns,
+ *     and winner block l is wva_solve(f_l)'s with unlimited = 1.  With arrival_rpm the fleet's own column at every
+ *     row and NULL token lists, candidates and winners are wva_profile_grid's.
+ *   - Trace, tick t.  Let f_t be that fleet with srv_cur_* = c_t, the allocation wva_profile_trace carries into tick
+ *     t, whose cost is at its own tick's prices.  Block t is byte for byte wva_price_thresholds(f_t), and candidates
+ *     and winners are wva_profile_trace's.  The trace continues as wva_profile_trace's does: ticks 0..L-1 equal
+ *     ticks 0..k-1 of one call followed by ticks k..L-1 of a call on the fleet with c_k in its srv_cur_* columns.
+ *
+ * Column a of threshold and of above, in block l, does not read row l's acc_cost[a]: a's price moves at row l
+ * alone, and every other record of the row keeps the row's prices.  srv_cur_cost is not re-priced.  With every
+ * profile column NULL the result is byte for byte wva_price_threshold_grid's or wva_price_threshold_trace's on the
+ * same load rows, with the same kernel launches.
+ *
+ * Only unlimited mode is covered.  The fleet becomes resident, and wva_summarize returns WVA_ERR_STATE afterwards.
+ * above and candidates may be NULL, and so may any of their columns; winners may not.  L == 0 is valid.
+ * WVA_ERR_BAD_ARG: L < 0, winners NULL, arrival_rpm NULL with L*S > 0, threshold NULL with L*S*A > 0.
+ * WVA_ERR_UNSUPPORTED, with wva_last_error naming the rule and, for a current cost, the server and the level or tick:
+ *   - whatever wva_profile_trace (trace) or its grid mode (grid) refuses on the same rows: L*S*A >= 2^31,
+ *     L*M*A >= 2^31, 2^31 or more key pairs x accelerators, and the sizing's own refusals;
+ *   - wva_price_threshold_grid's and _trace's price rules, at f_l or f_t: a penalty factor that is NaN, negative or
+ *     infinite, and a current cost that is NaN or infinite on a server with a pair not classed nil at that row,
+ *     under the row's perf_present, rate and tokens.  The grid checks before any launch, the trace after the
+ *     winners are known.  A carried cost can be +Inf or NaN at a row with an infinite or NaN price: a winner with
+ *     c_t's accelerator and replica count has value 0 whatever its cost.
+ */
+int wva_profile_price_threshold_grid(wva_handle *h, const wva_fleet *fleet, int32_t n_levels,
+                                     const float *arrival_rpm, const int32_t *in_tokens, const int32_t *out_tokens,
+                                     const wva_profile_rows *rows, float *threshold /* [L*S*A] */,
+                                     wva_allocs *above /* [L*S*A], may be NULL */,
+                                     wva_allocs *candidates /* [L*S*A], may be NULL */,
+                                     wva_allocs *winners /* [L*S] */);
+int wva_profile_price_threshold_trace(wva_handle *h, const wva_fleet *fleet, int32_t n_ticks,
+                                      const float *arrival_rpm, const int32_t *in_tokens, const int32_t *out_tokens,
+                                      const wva_profile_rows *rows, float *threshold /* [L*S*A] */,
+                                      wva_allocs *above /* [L*S*A], may be NULL */,
+                                      wva_allocs *candidates /* [L*S*A], may be NULL */,
+                                      wva_allocs *winners /* [L*S] */);
+
+/*
  * SLO bounds: for each (server s, accelerator a) and search w (0: TTFT, 1: ITL), the exact targets at which the
  * reference's candidate turns nil and at which its target stops binding.  Entry (s*A + a)*2 + w of each column.
  *

@@ -44,7 +44,8 @@ EXPORTS = (
     "wva_workload_trace", "wva_profile_grid", "wva_profile_trace", "wva_price_thresholds", "wva_slo_bounds",
     "wva_slo_trace", "wva_price_threshold_grid", "wva_price_threshold_trace", "wva_load_margin_trace",
     "wva_workload_margins", "wva_workload_margin_trace", "wva_profile_margins", "wva_profile_margin_trace",
-    "wva_slo_margins", "wva_slo_margin_trace",
+    "wva_slo_margins", "wva_slo_margin_trace", "wva_profile_price_threshold_grid",
+    "wva_profile_price_threshold_trace",
 )
 
 _lib = None
@@ -107,6 +108,12 @@ def lib():
                                       C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
         ("wva_price_threshold_trace", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p, f32p, C.POINTER(_abi.AllocsC),
                                        C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
+        ("wva_profile_price_threshold_grid", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p,
+                                              C.POINTER(_abi.ProfileRowsC), f32p, C.POINTER(_abi.AllocsC),
+                                              C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
+        ("wva_profile_price_threshold_trace", [vp, C.POINTER(_abi.FleetC), i32, f32p, i32p, i32p,
+                                               C.POINTER(_abi.ProfileRowsC), f32p, C.POINTER(_abi.AllocsC),
+                                               C.POINTER(_abi.AllocsC), C.POINTER(_abi.AllocsC)]),
         ("wva_slo_bounds", [vp, C.POINTER(_abi.FleetC), C.POINTER(_abi.SloBoundsC)]),
         ("wva_sweep", [vp, C.POINTER(_abi.FleetC), i32, C.POINTER(_abi.SweepOutC)]),
         ("wva_upload", [vp, C.POINTER(_abi.FleetC)]),

@@ -2262,8 +2262,16 @@ int enqueue_profile_grid(wva_handle* h, int L, const wva_profile_rows& rows, con
 // profile_trace_kernel then writes the nil and zero-load records and prices the tail's at row t, and the workload
 // trace's trace_kernel runs the chain.  rpm / in / out [L*S] are the caller's rows (NULL: the fleet's own column at
 // every tick); cand ([L*S*A]) and winners ([L*S]) are device columns.
+//
+// Without `trace` (the grid mode of the profile price thresholds, DESIGN.md §3.25) every row is a level against the
+// fleet's own current allocation.  keepAccelerator then masks a pair at every row, as on the profile margins' grid:
+// the keys skip it (profile_keys) or carry the fleet's own keepAccelerator (workload_keys without pins),
+// profile_trace_kernel classes the records with the resident keepAccelerator, and unlimited_kernel picks each
+// level's winners.  acc_count, when given, receives the device copy of the perf_acc_count row list (NULL without
+// one), which stays in place until the next call.
 int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                          const wva_profile_rows& rows, const AllocCols& cand, const AllocCols& winners) {
+                          const wva_profile_rows& rows, const AllocCols& cand, const AllocCols& winners,
+                          bool trace = true, const int32_t** acc_count = nullptr) {
     const HostFleet& hf = h->hf;
     const int S = hf.S, A = hf.A;
     Cols c(16);
@@ -2274,22 +2282,27 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
     in = lists.in.host;
     out = lists.out.host;
     ProfileRanks pr(hf, L, rows);
-    const std::vector<uint8_t> pin = trace_pinned(hf);
-    const size_t o_pin = c.put(pin.data(), S);
-    // The keys.  Without a perf column: the workload trace's (s, in, out) rows.  With one: profile_keys, a pinned
-    // server sizing its current pair alone.
+    const std::vector<uint8_t> pin = trace ? trace_pinned(hf) : std::vector<uint8_t>();
+    const size_t o_pin = trace ? c.put(pin.data(), S) : 0;
+    // The keys.  Without a perf column: the workload trace's (s, in, out) rows (the workload grid's without
+    // `trace`).  With one: profile_keys, a pinned server sizing its current pair alone.
     TokenKeys tk;
     std::vector<int> key_acc, key_model;  // with a perf column: key row k's accelerator and key-model
     if (pr.perf_rows) {
-        profile_keys(hf, pr, L, rpm, in, out, [&](int s, int a) { return pin[s] && hf.srv_cur_acc[s] != a; }, tk,
-                     key_acc, key_model);
+        profile_keys(hf, pr, L, rpm, in, out,
+                     [&](int s, int a) {
+                         const int cur = hf.srv_cur_acc[s];
+                         return (trace ? pin[s] : hf.srv_keep_acc[s] && cur != WVA_ACC_NONE) && cur != a;
+                     },
+                     tk, key_acc, key_model);
         // at most L * S * A key rows; the key fleet's pair ids k * A + a are int
         if ((long long)tk.srv.size() * A >= (1ll << 31))
-            return h->fail(WVA_ERR_UNSUPPORTED,
-                           "profile trace too large for one call (>= 2^31 key pairs x accelerators)");
+            return h->fail(WVA_ERR_UNSUPPORTED, trace
+                               ? "profile trace too large for one call (>= 2^31 key pairs x accelerators)"
+                               : "profile rows too large for one call (>= 2^31 key pairs x accelerators)");
     }
     KeyFleet kf = pr.perf_rows ? profile_key_fleet(hf, pr, tk, key_acc, key_model)
-                               : workload_keys(hf, L, rpm, in, out, pin.data(), tk);
+                               : workload_keys(hf, L, rpm, in, out, trace ? pin.data() : nullptr, tk);
     const int K = (int)tk.srv.size();
     HostFleet& kh = kf.hf;
     kf.place(c);
@@ -2310,13 +2323,14 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
     if (rc) return rc;
     ProfileTraceArgs r{};
     r.p.f = h->df;
-    r.p.f.srv_keep_acc = (const uint8_t*)(d + o_pin);
+    if (trace) r.p.f.srv_keep_acc = (const uint8_t*)(d + o_pin);
     pr.set_rows(r.p, d);
     r.p.cand = cand;
     r.p.L = L;
     r.rows = lists.load(d);
     launch_records(h, (long long)S * A * L, profile_trace_kernel, r);
-    enqueue_level_winners(h, cand, winners, L, true);
+    enqueue_level_winners(h, cand, winners, L, trace);
+    if (acc_count) *acc_count = rows.perf_acc_count ? r.p.rows.perf_acc_count : nullptr;
     CK(cudaGetLastError());
     return WVA_OK;
 }
@@ -2326,15 +2340,16 @@ int enqueue_profile_trace(wva_handle* h, int L, const float* rpm, const int32_t*
 // interval from 0: a penalty factor that is NaN, negative or infinite, or a non-finite current cost on a server
 // that has a candidate (a pair wva_analyze does not class nil).  The first rule is the fleet's; the second is
 // checked per row of L rows (the single call's one row is the fleet itself): at row l server s has the arrival rate
-// rpm[l*S + s], the tokens in / out[l*S + s] (NULL: the fleet's own column) and the current allocation cur(l, s) ->
-// (accelerator, cost).  Each returns its refusal, empty when there is none.
+// rpm[l*S + s], the tokens in / out[l*S + s] (NULL: the fleet's own column), the models' perf_present
+// present[(l*M + m)*A + a] (NULL: the fleet's own column) and the current allocation cur(l, s) -> (accelerator,
+// cost).  Each returns its refusal, empty when there is none.
 std::string price_factor_refusal(const HostFleet& hf) {
     const float f = hf.tun.accel_penalty_factor;
     return !(f >= 0.0f) || std::isinf(f) ? "penalty factor NaN, negative or infinite" : "";
 }
 template <class Cur>
 std::string price_cost_refusal(const HostFleet& hf, int L, const float* rpm, const int32_t* in, const int32_t* out,
-                               const char* row, Cur&& cur) {
+                               const uint8_t* present, const char* row, Cur&& cur) {
     const int S = hf.S;
     for (int l = 0; l < L; ++l)
         for (int s = 0; s < S; ++s) {
@@ -2342,8 +2357,12 @@ std::string price_cost_refusal(const HostFleet& hf, int L, const float* rpm, con
             if (std::isfinite(c.second)) continue;
             const size_t i = (size_t)l * S + s;
             const int ki = in ? in[i] : hf.srv_in_tokens[s], ko = out ? out[i] : hf.srv_out_tokens[s];
+            const int m = hf.srv_model[s];
+            const bool known = m >= 0 && m < hf.M;
             for (int a = 0; a < hf.A; ++a)
-                if (hf.pair_class(s, a, true, rpm[i], ki, ko, c.first)) {
+                if (present ? hf.pair_class(s, a, true, rpm[i], ki, ko, c.first,
+                                            known && present[((size_t)l * hf.M + m) * hf.A + a])
+                            : hf.pair_class(s, a, true, rpm[i], ki, ko, c.first)) {
                     std::string what = "current cost NaN or infinite on a server with a candidate (server " +
                                        std::to_string(s);
                     return row ? what + ", " + row + " " + std::to_string(l) + ")" : what + ")";
@@ -2354,20 +2373,24 @@ std::string price_cost_refusal(const HostFleet& hf, int L, const float* rpm, con
 std::string price_refusal(const HostFleet& hf) {
     const std::string what = price_factor_refusal(hf);
     if (!what.empty()) return what;
-    return price_cost_refusal(hf, 1, hf.srv_arrival_rpm.data(), nullptr, nullptr, nullptr,
+    return price_cost_refusal(hf, 1, hf.srv_arrival_rpm.data(), nullptr, nullptr, nullptr, nullptr,
                               [&](int, int s) { return std::make_pair(hf.srv_cur_acc[s], hf.srv_cur_cost[s]); });
 }
 
 // price_kernel over L candidate blocks whose values are set (DESIGN.md §3.16, §3.20): threshold and above
 // ([L*S*A], device; a NULL above column is not written), the current allocation the fleet's, or with `chain` the
-// trace's c_l from its winner blocks ([L*S]).
+// trace's c_l from its winner blocks ([L*S]).  With acc_count ([L*M*A], device; DESIGN.md §3.25) block l prices at
+// row l's AccCount.
 void enqueue_price(wva_handle* h, int L, const AllocCols& cand, float* threshold, const AllocCols& above,
-                   const AllocCols* chain) {
+                   const AllocCols* chain, const int32_t* acc_count = nullptr) {
     const HostFleet& hf = h->hf;
     const long long warps = (long long)L * hf.S;
     if (warps * hf.A <= 0) return;
-    price_kernel<<<(unsigned)((warps + 3) / 4), 128, 0, h->stream>>>(
-        PriceArgs{h->df, cand, threshold, above, chain ? *chain : AllocCols{}, L});
+    const PriceArgs g{h->df, cand, threshold, above, chain ? *chain : AllocCols{}, L};
+    if (acc_count)
+        price_kernel<<<(unsigned)((warps + 3) / 4), 128, 0, h->stream>>>(ProfilePriceArgs{g, acc_count});
+    else
+        price_kernel<<<(unsigned)((warps + 3) / 4), 128, 0, h->stream>>>(g);
     h->launches++;
 }
 
@@ -2385,12 +2408,22 @@ int enqueue_price_thresholds(wva_handle* h, float* threshold, const AllocCols& c
 // price_kernel after the winners.  threshold and above's columns are the call's further device columns in d_price,
 // copied straight to the caller.  The cost rule is checked per level before any launch; for a trace c_t is known only
 // from the winners, so it is checked per tick after the sync, on the winner block's host copy.
+//
+// With `prof` (the profile price thresholds, DESIGN.md §3.25) the rows also carry acc_cost and perf_* (a NULL
+// column: the fleet's own).  The call is then the profile path's (enqueue_profile_trace, in grid mode on a grid),
+// price_kernel prices at the rows' AccCount when that column is given, and the cost rule reads the rows'
+// perf_present.  With every column NULL it is the workload call's, byte and launch for launch.
 int run_price_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const float* rpm, const int32_t* in,
-                     const int32_t* out, float* threshold, wva_allocs* above, wva_allocs* candidates,
-                     wva_allocs* winners, bool trace) {
+                     const int32_t* out, const wva_profile_rows* prof, float* threshold, wva_allocs* above,
+                     wva_allocs* candidates, wva_allocs* winners, bool trace) {
     if (h && winners && fleet && L > 0 && (long long)fleet->n_servers * fleet->n_acc > 0 && !threshold)
         return h->fail(WVA_ERR_BAD_ARG, "threshold is NULL");
-    const char* name = trace ? "price threshold trace" : "price threshold grid";
+    const char* name = prof ? (trace ? "profile price threshold trace" : "profile price threshold grid")
+                            : (trace ? "price threshold trace" : "price threshold grid");
+    const uint8_t* present = prof ? prof->perf_present : nullptr;
+    const bool rows = prof && (prof->acc_cost || prof->perf_present || prof->perf_alpha || prof->perf_beta ||
+                               prof->perf_gamma || prof->perf_delta || prof->perf_acc_count || prof->perf_max_batch ||
+                               prof->perf_at_tokens);
     Cols cols(16);
     AllocCols dab{};  // above's device columns, set by place
     LevelMore more;
@@ -2398,7 +2431,7 @@ int run_price_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const flo
         const HostFleet& hf = h->hf;
         std::string what = price_factor_refusal(hf);
         if (what.empty() && !trace)
-            what = price_cost_refusal(hf, L, rpm, in, out, "level", [&](int, int s) {
+            what = price_cost_refusal(hf, L, rpm, in, out, present, "level", [&](int, int s) {
                 return std::make_pair(hf.srv_cur_acc[s], hf.srv_cur_cost[s]);
             });
         if (!what.empty()) return h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
@@ -2428,7 +2461,7 @@ int run_price_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const flo
             // c_t per server, advanced tick by tick as price_cost_refusal walks the rows in order
             std::vector<std::pair<int, float>> cur(hf.S);
             for (int s = 0; s < hf.S; ++s) cur[s] = {hf.srv_cur_acc[s], hf.srv_cur_cost[s]};
-            const std::string what = price_cost_refusal(hf, L, rpm, in, out, "tick", [&](int t, int s) {
+            const std::string what = price_cost_refusal(hf, L, rpm, in, out, present, "tick", [&](int t, int s) {
                 const std::pair<int, float> ct = cur[s];
                 const size_t j = (size_t)t * hf.S + s;
                 if (feasible[j]) cur[s] = {acc[j], cost[j]};
@@ -2437,11 +2470,13 @@ int run_price_levels(wva_handle* h, const wva_fleet* fleet, int32_t L, const flo
             return what.empty() ? WVA_OK : h->fail(WVA_ERR_UNSUPPORTED, what.c_str());
         };
     return run_levels(
-        h, fleet, L, name, rpm ? nullptr : "NULL arrival rate list", false, candidates, winners,
+        h, fleet, L, name, rpm ? nullptr : "NULL arrival rate list", prof != nullptr, candidates, winners,
         [&](const AllocCols& dc, const AllocCols& dw) {
-            const int rc = enqueue_workload(h, L, rpm, in, out, dc, dw, trace);
+            const int32_t* acc_count = nullptr;  // row l's AccCount, on the device
+            const int rc = rows ? enqueue_profile_trace(h, L, rpm, in, out, *prof, dc, dw, trace, &acc_count)
+                                : enqueue_workload(h, L, rpm, in, out, dc, dw, trace);
             if (rc) return rc;
-            enqueue_price(h, L, dc, (float*)h->d_price.p, dab, trace ? &dw : nullptr);
+            enqueue_price(h, L, dc, (float*)h->d_price.p, dab, trace ? &dw : nullptr, acc_count);
             CK(cudaGetLastError());
             return WVA_OK;
         },
@@ -3520,15 +3555,33 @@ int wva_price_thresholds(wva_handle* h, const wva_fleet* fleet, float* threshold
 int wva_price_threshold_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
                              const int32_t* in_tokens, const int32_t* out_tokens, float* threshold, wva_allocs* above,
                              wva_allocs* candidates, wva_allocs* winners) {
-    return run_price_levels(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, threshold, above, candidates,
-                            winners, false);
+    return run_price_levels(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, nullptr, threshold, above,
+                            candidates, winners, false);
 }
 
 int wva_price_threshold_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks, const float* arrival_rpm,
                               const int32_t* in_tokens, const int32_t* out_tokens, float* threshold, wva_allocs* above,
                               wva_allocs* candidates, wva_allocs* winners) {
-    return run_price_levels(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, threshold, above, candidates,
-                            winners, true);
+    return run_price_levels(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, nullptr, threshold, above,
+                            candidates, winners, true);
+}
+
+int wva_profile_price_threshold_grid(wva_handle* h, const wva_fleet* fleet, int32_t n_levels, const float* arrival_rpm,
+                                     const int32_t* in_tokens, const int32_t* out_tokens, const wva_profile_rows* rows,
+                                     float* threshold, wva_allocs* above, wva_allocs* candidates,
+                                     wva_allocs* winners) {
+    const wva_profile_rows own{};
+    return run_price_levels(h, fleet, n_levels, arrival_rpm, in_tokens, out_tokens, rows ? rows : &own, threshold,
+                            above, candidates, winners, false);
+}
+
+int wva_profile_price_threshold_trace(wva_handle* h, const wva_fleet* fleet, int32_t n_ticks,
+                                      const float* arrival_rpm, const int32_t* in_tokens, const int32_t* out_tokens,
+                                      const wva_profile_rows* rows, float* threshold, wva_allocs* above,
+                                      wva_allocs* candidates, wva_allocs* winners) {
+    const wva_profile_rows own{};
+    return run_price_levels(h, fleet, n_ticks, arrival_rpm, in_tokens, out_tokens, rows ? rows : &own, threshold,
+                            above, candidates, winners, true);
 }
 
 int wva_slo_bounds(wva_handle* h, const wva_fleet* fleet, wva_slo_bounds_out* out) {

@@ -1934,7 +1934,20 @@ struct PriceArgs {
     AllocCols chain;    // a trace's winners [L * S], tick-major; chain.feasible NULL: the fleet's current allocation
     int L;
 };
-__global__ void __launch_bounds__(128) price_kernel(PriceArgs g) {
+// The profile price thresholds (DESIGN.md §3.25): block l's records already carry row l's prices and profiles, and
+// the bisection prices a's record at row l's AccCount, entry (l * M + m) * A + a of the row list.
+struct ProfilePriceArgs : PriceArgs {
+    const int32_t* acc_count;  // [L * M * A] perf_acc_count by row
+};
+// The fleet cost_at reads at block l: the fleet itself, or with ProfilePriceArgs the fleet with row l's AccCount.
+__device__ __forceinline__ const DevFleet& price_fleet(const PriceArgs& g, int) { return g.f; }
+__device__ __forceinline__ DevFleet price_fleet(const ProfilePriceArgs& g, int l) {
+    DevFleet fl = g.f;
+    fl.perf_acc_count = g.acc_count + (size_t)l * g.f.M * g.f.A;
+    return fl;
+}
+template <class Args>
+__device__ __forceinline__ void price_levels(const Args& g) {
     const DevFleet& f = g.f;
     const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -1987,6 +2000,7 @@ __global__ void __launch_bounds__(128) price_kernel(PriceArgs g) {
             }
         }
     }
+    const DevFleet& fp = price_fleet(g, l);
     for (int a = lane; a < f.A; a += 32) {
         const size_t i = (size_t)s * f.A + a;
         const PriceBest w = b1.a == a ? b2 : b1;
@@ -1995,7 +2009,7 @@ __global__ void __launch_bounds__(128) price_kernel(PriceArgs g) {
             const int acc = cand.acc[i], replicas = cand.replicas[i];
             const auto wins = [&](unsigned bits) {
                 const float v = transition_penalty(f.penalty, cur_acc, cur_replicas, cur_cost, acc, replicas,
-                                                   cost_at(f, m, a, replicas, __uint_as_float(bits)));
+                                                   cost_at(fp, m, a, replicas, __uint_as_float(bits)));
                 return v < max_f32 && price_before(v, a, w);
             };
             if (wins(max_bits)) {
@@ -2010,6 +2024,8 @@ __global__ void __launch_bounds__(128) price_kernel(PriceArgs g) {
         store_cand(above, i, r);
     }
 }
+__global__ void __launch_bounds__(128) price_kernel(PriceArgs g) { price_levels(g); }
+__global__ void __launch_bounds__(128) price_kernel(ProfilePriceArgs g) { price_levels(g); }
 
 // wva_size_grid's value + per-server minimum: one warp per server over its A * B candidates (record
 // (s * A + a) * B + bi), strided, so any A * B fits.  Every feasible candidate gets value = TransitionPenalty as in

@@ -50,6 +50,11 @@ def accelerator_demand(fleet: Fleet, threshold, candidates: Allocs, a: int):
     counted as ``System.AllocateByType`` counts them (pkg/core/system.go:271-300): replicas * NumInstances *
     multiplicity over the servers whose winner is ``a``'s candidate, i.e. whose threshold lies above the price.  A
     zero-replica candidate (accelerator "") uses no units."""
+    return _demand(fleet, threshold, candidates, a, fleet.perf_acc_count)
+
+
+def _demand(fleet: Fleet, threshold, candidates: Allocs, a: int, acc_count):
+    """accelerator_demand with NumInstances read from acc_count (M, A) in place of the fleet's perf_acc_count."""
     S, A = fleet.n_servers, fleet.n_acc
     if not 0 <= a < A:
         raise ValueError(f"accelerator {a} out of range [0, {A})")
@@ -60,7 +65,7 @@ def accelerator_demand(fleet: Fleet, threshold, candidates: Allocs, a: int):
     idx = np.arange(S) * A + a
     m = fleet.srv_model
     on_a = candidates.acc[idx] == a  # a feasible record in column a is on a, or on "" with 0 replicas
-    inst = np.maximum(fleet.perf_acc_count[np.where(on_a, m, 0), a].astype(np.int64), 1)
+    inst = np.maximum(acc_count[np.where(on_a, m, 0), a].astype(np.int64), 1)
     units = np.where(on_a, candidates.replicas[idx].astype(np.int64) * inst, 0) * int(fleet.acc_multiplicity[a])
     breakpoints = np.unique(col[(col > 0) & np.isfinite(col)])
     starts = np.concatenate([[np.float32(0.0)], breakpoints]).astype(np.float32)
@@ -71,26 +76,35 @@ def accelerator_demand(fleet: Fleet, threshold, candidates: Allocs, a: int):
     return breakpoints, np.cumsum(per_k[::-1])[::-1][1:]
 
 
-def demand_by_level(fleet: Fleet, threshold, candidates: Allocs, a: int):
-    """The demand curve for accelerator ``a`` at every row of ``Engine.price_threshold_grid`` or
-    ``price_threshold_trace`` (host only, no GPU) -> (breakpoints, units (L, len(breakpoints) + 1) int64).
+def demand_by_level(fleet: Fleet, threshold, candidates: Allocs, a: int, *, perf_acc_count=None):
+    """The demand curve for accelerator ``a`` at every row of ``Engine.price_threshold_grid``,
+    ``price_threshold_trace``, ``profile_price_threshold_grid`` or ``profile_price_threshold_trace`` (host only, no
+    GPU) -> (breakpoints, units (L, len(breakpoints) + 1) int64).
 
     ``breakpoints`` is the ascending union over the rows of column ``a``'s distinct thresholds in (0, MaxFloat32];
     it cuts the prices [+0, MaxFloat32] into stretches as ``accelerator_demand`` does.  ``units[l, j]`` is
     ``accelerator_demand``'s count for row ``l`` (threshold block ``l`` and candidate block ``l``, which for a trace
-    is tick ``l``'s block, masked against its current allocation) on stretch ``j`` of the union."""
+    is tick ``l``'s block, masked against its current allocation) on stretch ``j`` of the union.
+    ``perf_acc_count`` (shape (L, M, A), the profile calls' AccCount rows; None: the fleet's own at every row) makes
+    row ``l`` count NumInstances at that row's AccCount."""
     S, A = fleet.n_servers, fleet.n_acc
     th = np.ascontiguousarray(threshold, np.float32)
     if th.ndim != 3 or th.shape[1:] != (S, A) or candidates.n != th.shape[0] * S * A:
         raise ValueError("threshold must have shape (L, n_servers, n_acc) and candidates L * n_servers * n_acc "
                          "records")
+    if perf_acc_count is not None:
+        perf_acc_count = np.asarray(perf_acc_count)
+        if perf_acc_count.shape != (th.shape[0], fleet.n_models, A):
+            raise ValueError(f"perf_acc_count must have shape ({th.shape[0]}, {fleet.n_models}, {A}), got "
+                             f"{perf_acc_count.shape}")
     n = S * A
     per_level = []
     for l in range(th.shape[0]):
         block = Allocs(n)
         for k in block.columns():
             getattr(block, k)[:] = getattr(candidates, k)[l * n:(l + 1) * n]
-        per_level.append(accelerator_demand(fleet, th[l], block, a))
+        per_level.append(_demand(fleet, th[l], block, a,
+                                 fleet.perf_acc_count if perf_acc_count is None else perf_acc_count[l]))
     breakpoints = np.unique(np.concatenate([bp for bp, _ in per_level] + [np.zeros(0, np.float32)]))
     starts = np.concatenate([[np.float32(0.0)], breakpoints]).astype(np.float32)
     units = np.zeros((th.shape[0], starts.size), np.int64)
@@ -695,9 +709,46 @@ class Engine:
         return self._price_rows(self._L.wva_price_threshold_trace, fleet, arrival_rpm, in_tokens, out_tokens,
                                 want_candidates)
 
-    def _price_rows(self, call, fleet, arrival_rpm, in_tokens, out_tokens, want_candidates):
+    def profile_price_threshold_grid(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, *,
+                                     acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None,
+                                     perf_gamma=None, perf_delta=None, perf_acc_count=None, perf_max_batch=None,
+                                     perf_at_tokens=None, want_candidates: bool = False):
+        """``price_threshold_grid`` at rows that also carry their own accelerator costs (``acc_cost``, shape (L, A))
+        and performance profiles (``perf_*``, shape (L, M, A)), as ``profile_trace`` takes them -> (threshold (L, S,
+        A) float32, above: ``Allocs`` of L * S * A, candidates [L*S*A] | None, winners [L*S]).
+
+        Block ``l`` of threshold, above and candidates is ``price_thresholds`` on the fleet with every given column
+        = row ``l``, and winner block ``l`` is ``solve``'s in unlimited mode on that fleet.  Column ``a`` of block
+        ``l`` does not read row ``l``'s ``acc_cost[a]``.  A list of ``None`` is the fleet's own column at every
+        level; ``srv_cur_cost`` is not re-priced (see ``wva_profile_price_threshold_grid`` in include/wva_b200.h).
+        ``demand_by_level`` with ``perf_acc_count`` turns a column into demand curves."""
+        profile = dict(zip(_PROFILE_COLUMNS, (acc_cost, perf_present, perf_alpha, perf_beta, perf_gamma, perf_delta,
+                                              perf_acc_count, perf_max_batch, perf_at_tokens)))
+        return self._price_rows(self._L.wva_profile_price_threshold_grid, fleet, arrival_rpm, in_tokens, out_tokens,
+                                want_candidates, profile)
+
+    def profile_price_threshold_trace(self, fleet: Fleet, arrival_rpm, in_tokens=None, out_tokens=None, *,
+                                      acc_cost=None, perf_present=None, perf_alpha=None, perf_beta=None,
+                                      perf_gamma=None, perf_delta=None, perf_acc_count=None, perf_max_batch=None,
+                                      perf_at_tokens=None, want_candidates: bool = False):
+        """``price_thresholds`` at every tick of ``profile_trace`` over the same rows -> the same tuple as
+        ``profile_price_threshold_grid``.
+
+        Block ``t`` is ``price_thresholds`` on the fleet with every given column = row ``t`` and the current
+        allocation the trace carries into tick ``t`` (``fleet.apply_winners`` of every earlier tick in turn, each
+        cost at its own tick's prices), and winners and candidates are ``profile_trace``'s (see
+        ``wva_profile_price_threshold_trace`` in include/wva_b200.h)."""
+        profile = dict(zip(_PROFILE_COLUMNS, (acc_cost, perf_present, perf_alpha, perf_beta, perf_gamma, perf_delta,
+                                              perf_acc_count, perf_max_batch, perf_at_tokens)))
+        return self._price_rows(self._L.wva_profile_price_threshold_trace, fleet, arrival_rpm, in_tokens, out_tokens,
+                                want_candidates, profile)
+
+    def _price_rows(self, call, fleet, arrival_rpm, in_tokens, out_tokens, want_candidates, profile=None):
+        """wva_price_threshold_grid / _trace over (L, S) rows, or with `profile` ({column: rows or None})
+        wva_profile_price_threshold_grid / _trace; the output arrays."""
         S, A = fleet.n_servers, fleet.n_acc
-        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "in_tokens": in_tokens, "out_tokens": out_tokens})
+        rows, L = _row_lists(fleet, {"arrival_rpm": arrival_rpm, "in_tokens": in_tokens, "out_tokens": out_tokens,
+                                     **(profile or {})})
         if "arrival_rpm" not in rows:
             raise ValueError("arrival_rpm is required")
         threshold = np.zeros((L, S, A), np.float32)
@@ -707,6 +758,9 @@ class Engine:
         cc = cand.as_c() if cand is not None else None
         ptrs = [_abi.ptr(rows[k].reshape(-1)) if k in rows else None
                 for k in ("arrival_rpm", "in_tokens", "out_tokens")]
+        if profile is not None:
+            rc_ = _profile_rows_c(rows)
+            ptrs.append(C.byref(rc_))
         self._resident(fleet)
         self._check(call(self._h, C.byref(fc), L, *ptrs, _abi.ptr(threshold.reshape(-1)), C.byref(ac),
                          C.byref(cc) if cc is not None else None, C.byref(wc)))
