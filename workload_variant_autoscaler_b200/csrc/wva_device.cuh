@@ -275,10 +275,6 @@ __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefe
 // Fast-window test on the high word: lo <= hi(p) < lo + span.
 #define WVA_FASTWIN(p, lo, span) ((((unsigned)__double2hiint(p)) - (lo)) < (span))
 
-// STASH > 0: the first STASH states of pass 1 are kept in shared memory (stash[(j-1)*32] for
-// state j, one 8-byte column per lane) and pass 2 reads them back instead of re-running the
-// recurrence for those states — most grid chains are shorter than that.
-//
 // STAGED (grid_kernel): when the 32 lanes of a full warp read the SAME pair table (they usually do: an
 // item is cut from one pair's cells) the head of both passes runs from a 32-entry window of the table
 // that the warp stages in shared memory (`tbuf`, 1 KB per warp) with one coalesced load per 32 steps,
@@ -293,18 +289,50 @@ __device__ __forceinline__ void dev_cp_async16(void* smem_dst, const void* gmem_
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
 }
+// The float32 tail of mm1modelstatedependent.go:56-66 from avgNumInSystem (acc), avgNumInServers (in_serv) and
+// p[K] / sum (pnK, 0 when the chain ended early).
+__device__ __forceinline__ void stats_epilogue(double acc, double in_serv, double pnK, float lambda, ModelStats& st) {
+    st.avg_num_in_servers = (float)in_serv;
+    const float avg_num_in_system = (float)acc;
+    st.throughput = __fmul_rn(lambda, __fsub_rn(1.0f, (float)pnK));
+    st.avg_resp_time = __fdiv_rn(avg_num_in_system, st.throughput);
+    st.avg_serv_time = __fdiv_rn(st.avg_num_in_servers, st.throughput);
+    float w = __fsub_rn(st.avg_resp_time, st.avg_serv_time);
+    if (w < 0.0f) w = 0.0f;
+    st.avg_wait_time = w;
+}
+// True when every real y with |y - x| <= E rounds to the same float32 as x: (float)x is a normal float32 below
+// FLT_MAX and [x - E, x + E] lies strictly between the two rounding midpoints next to it (exact doubles: the mean of
+// two neighbouring float32 values; below a power of two the lower one is half as far away).  The ends of the
+// interval are rounded outwards.
+__device__ __forceinline__ bool f32_decided(double x, double E) {
+    const double ax = fabs(x);
+    const float f = __double2float_rn(ax);
+    const unsigned fb = __float_as_uint(f);
+    if (!(fb >= 0x00800000u && fb < 0x7f7fffffu)) return false;  // 0, subnormal, FLT_MAX, inf, NaN
+    const double fd = (double)f;
+    const double m_hi = __dmul_rn(__dadd_rn(fd, (double)__uint_as_float(fb + 1u)), 0.5);
+    const double m_lo = __dmul_rn(__dadd_rn(fd, (double)__uint_as_float(fb - 1u)), 0.5);
+    return __dsub_rd(ax, E) > m_lo && __dadd_ru(ax, E) < m_hi;
+}
+// One-pass bounds (DESIGN.md §3.2b): c·u with u = 2^-53 and c = 1 + 2^-16 absorbing the second-order terms, and an
+// absolute slack for the states whose quotient p[i]/sum or i·q[i] is subnormal.
+constexpr double kOnePassCu = 0x1p-53 * (1.0 + 0x1p-16);
+constexpr double kOnePassAbs = 0x1p-1000;
+
 constexpr int kStagedFirst = 64;   // entries in the first staged window
 constexpr int kStagedSlots = 96;   // window slots of tbuf: pass 2 may index up to (hmax - 1) + 31 <= 94 when it re-uses the window
 constexpr int kStagedTbufD = kStagedSlots * 4 + 128;  // doubles per warp: the window, then one 32-byte tail entry per lane
 // WIDE: the windows of the comment above kHiPLo.  grid_kernel's instantiation (STAGED) keeps the round-1 windows
 // (2^600 / 2^620, fixed pass-2 bound): its batch sizes stay below what needs more, and the extra pass-2 set-up
 // perturbs its register allocation; everything else (size path, sweep, row solve callers) is WIDE.
-template <int STASH, int PF = 10, bool STAGED = false, bool WIDE = !STAGED>
+template <int PF = 10, bool STAGED = false, bool WIDE = !STAGED>
 __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N, int K, float lambda, ModelStats& st,
-                                           double* __restrict__ stash, double* __restrict__ tbuf = nullptr) {
+                                           double* __restrict__ tbuf = nullptr) {
     constexpr unsigned kHiPHi = WIDE ? wva::kHiPHi : kHiPHiNarrow;   // shadow the namespace constants
     constexpr unsigned kHiSumHi = WIDE ? wva::kHiSumHi : kHiSumHiNarrow;
     constexpr int kPHiExp = WIDE ? wva::kPHiExp : kPHiExpNarrow;
+    constexpr bool ONEPASS = STAGED;  // pass 1 also accumulates sum(i*p[i]) and decides the float32 outputs (§3.2b)
     const unsigned warp_mask = __activemask();
     const double lam = (double)lambda;
     const int nh = N - 1;
@@ -404,8 +432,10 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
 
     // ---- pass 1 -----------------------------------------------------------------
     double sum = __dadd_rn(1.0, p);
+    // ONEPASS: mom = sum(i*p[i]) (one FMA per state, dw = i), with sum and mom kept at state min(N, last state) in
+    // sum_N / mom_N
+    double mom = p, dw = 2.0, sum_N = sum, mom_N = p;
     int j_end = K + 1;
-    if (STASH > 0) stash[0] = p;
     {
         int n = 1;  // p holds p[n]
         const int n_stop = bail ? 0 : K;
@@ -413,12 +443,12 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             // steps n < nh read entry n from the window, later steps the lane's own tail entry; all lanes
             // hold the same n (they advance together or leave together).  A window in which every lane
             // is still in its head (the usual case: grid_sort_cands keeps cells of one pair and similar
-            // length together) needs no per-lane select; only the first window feeds the stash.
+            // length together) needs no per-lane select.
             const double4* tab4 = reinterpret_cast<const double4*>(tab);
             double4* tb = reinterpret_cast<double4*>(tbuf);
             const int lane = threadIdx.x & 31;
             bool ok = true;
-#define WVA_SP1_GROUP(SEL, ST)                                                                                    \
+#define WVA_SP1_GROUP(SEL)                                                                                        \
     _Pragma("unroll") for (int u = 0; u < 4; ++u) {                                                               \
         const double4 e = *((SEL) && !(n < nh) ? (const double4*)tsave4 : (const double4*)(tb + (k + u)));       \
         RateRecip R;                                                                                              \
@@ -427,27 +457,31 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
         R.yl = e.z;                                                                                               \
         p = div_rate(__dmul_rn(p, lam), R);                                                                       \
         sum = __dadd_rn(sum, p);                                                                                  \
-        if (ST && n < STASH) stash[n * 32] = p;                                                                   \
+        if constexpr (ONEPASS) {                                                                                  \
+            mom = __fma_rn(dw, p, mom);                                                                           \
+            dw = __dadd_rn(dw, 1.0);                                                                              \
+        }                                                                                                         \
         ++n;                                                                                                      \
+        if constexpr (ONEPASS) { if (n <= N) { sum_N = sum; mom_N = mom; } }                                      \
     }
-#define WVA_SP1(ST, W)                                                                                            \
+#define WVA_SP1(W)                                                                                                \
     _Pragma("unroll 1") for (int k = 0; k < (W); k += 4) {                                                        \
         if (n >= hmax) break; /* every lane is past its head: the pure-tail loops below take over */             \
         if (!__all_sync(0xffffffffu, n + 4 <= n_stop && WVA_FASTWIN(p, blk_lo, blk_span))) { ok = false; break; } \
-        if (n + 4 <= hmin) { WVA_SP1_GROUP(false, ST) } else { WVA_SP1_GROUP(true, ST) }                          \
+        if (n + 4 <= hmin) { WVA_SP1_GROUP(false) } else { WVA_SP1_GROUP(true) }                                  \
     }
             // first window: entries 1..64 in slots 0..63 (slot k holds the entry of step 1 + k)
             asm volatile("cp.async.wait_group 0;" ::: "memory");
             __syncwarp();
             double4 nxt;  // later windows travel in registers
             if (kStagedFirst + 1 < hmax) nxt = tab4[min(kStagedFirst + 1 + lane, hmax)];
-            if (STASH > 0) { WVA_SP1(true, kStagedFirst) } else { WVA_SP1(false, kStagedFirst) }
+            WVA_SP1(kStagedFirst)
             for (int n0 = kStagedFirst + 1; ok && n0 < hmax; n0 += 32) {
                 __syncwarp();
                 tb[lane] = nxt;
                 __syncwarp();
                 if (n0 + 32 < hmax) nxt = tab4[min(n0 + 32 + lane, hmax)];
-                WVA_SP1(false, 32)
+                WVA_SP1(32)
             }
 #undef WVA_SP1_GROUP
 #undef WVA_SP1
@@ -463,21 +497,29 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     p = div_rate(__dmul_rn(p, lam), R);                                     \
     if (n < nh) load_recip(tab, n + 2 < nh ? n + 2 : nh, R);                \
     sum = __dadd_rn(sum, p);                                                \
-    if (STASH > 0 && n < STASH) stash[n * 32] = p;                          \
-    ++n;
+    if constexpr (ONEPASS) {                                                \
+        mom = __fma_rn(dw, p, mom);                                         \
+        dw = __dadd_rn(dw, 1.0);                                            \
+    }                                                                       \
+    ++n;                                                                    \
+    if constexpr (ONEPASS) { if (n <= N) { sum_N = sum; mom_N = mom; } }
             // Block phase.  All lanes that are still in this loop take a block path together or not at all
             // (a lane on the per-step path next to lanes on a block path would serialise the warp).
-            //  * pure-tail 16-step blocks: every lane is past its table head (and past the stash), so a step
+            //  * pure-tail 16-step blocks: every lane is past its table head, so a step
             //    is just the recurrence and the running sum — no loads, no selects; this is where the long
             //    chains spend 10/11 of their steps;
             //  * generic 4-step blocks otherwise.
             for (;;) {
-                if (__all_sync(__activemask(), n > nh + 1 && n >= STASH && n + 16 <= n_stop && WVA_FASTWIN(p, blk16_lo, blk16_span))) {
+                if (__all_sync(__activemask(), n > nh + 1 && n + 16 <= n_stop && WVA_FASTWIN(p, blk16_lo, blk16_span))) {
                     const double cA = __dmul_rn(lam, A.yl);
 #pragma unroll
                     for (int u = 0; u < 16; ++u) {
                         p = step_rate(p, lam, cA, A);
                         sum = __dadd_rn(sum, p);
+                        if constexpr (ONEPASS) {  // n > N: past sum_N / mom_N
+                            mom = __fma_rn(dw, p, mom);
+                            dw = __dadd_rn(dw, 1.0);
+                        }
                     }
                     n += 16;
                     continue;
@@ -517,8 +559,12 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
             if (n < nh) load_recip(tab, n, A);
             p = hp >= kHiPLo ? div_rate(__dmul_rn(p, lam), A) : __ddiv_rn(__dmul_rn(p, lam), A.b);
             sum = __dadd_rn(sum, p);
-            if (STASH > 0 && n < STASH) stash[n * 32] = p;
+            if constexpr (ONEPASS) {
+                mom = __fma_rn(dw, p, mom);
+                dw = __dadd_rn(dw, 1.0);
+            }
             ++n;
+            if constexpr (ONEPASS) { if (n <= N) { sum_N = sum; mom_N = mom; } }
             WVA_LOAD_TAIL(A)
             B = A;
             if (n < nh) load_recip(tab, n, A);
@@ -536,6 +582,28 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     z.b = sum;
     z.yh = __ddiv_rn(1.0, sum);
     z.yl = __dmul_rn(__fma_rn(-sum, z.yh, 1.0), z.yh);
+    if constexpr (ONEPASS) {
+        // Pass 1's sums with zh = RN(1/sum) in place of pass 2's exact quotients: A1 ~ acc, I1 ~ in_serv, each
+        // within its bound E of pass 2's value (§3.2b).  When that decides both float32 roundings on every lane (a
+        // lane that bailed has nothing to decide) the warp skips pass 2; p[K]/sum is exact either way.
+        const int m1 = min(N, j_end - 1);  // the last state in sumP and acc_at_N
+        const double A1 = __dmul_rn(mom, z.yh), AN = __dmul_rn(mom_N, z.yh), s1 = __dmul_rn(sum_N, z.yh);
+        const double d1 = __dsub_rn(1.0, s1), dN = (double)N;
+        const double I1 = __dadd_rn(AN, __dmul_rn(d1, dN));
+        const double E_acc = __dadd_ru(__dmul_ru(__dmul_ru(2.0 * (double)j_end, kOnePassCu), A1), kOnePassAbs);
+        double t = __dmul_ru(2.0 * (double)(m1 + 1), AN);
+        t = __dadd_ru(t, __dmul_ru(__dmul_ru(dN, (double)(2 * m1 + 3)), s1));
+        t = __dadd_ru(t, __dmul_ru(4.0 * dN, fabs(d1)));
+        t = __dadd_ru(t, 2.0 * fabs(I1));
+        const double E_in = __dadd_ru(__dmul_ru(t, kOnePassCu), kOnePassAbs);
+        const bool decided = bail || (f32_decided(A1, E_acc) && f32_decided(I1, E_in));
+        if (__all_sync(warp_mask, decided)) {
+            double pnK = 0.0;
+            if (j_end == K + 1) pnK = WVA_FASTWIN(p, kHiPLo, kHiPHi - kHiPLo) ? div_recip(p, z) : __ddiv_rn(p, sum);
+            stats_epilogue(A1, I1, pnK, lambda, st);
+            return bail ? kSolveBail : kSolveOk;
+        }
+    }
     double acc = 0.0, sum_p = z.yh, pn = 0.0, di = 1.0, acc_at_N = 0.0;
     p = p1;
     // pass 2 uses the same windows unless the sum is above 2^680: then the division by the sum needs
@@ -562,62 +630,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     __syncwarp(warp_mask);
     {
         int i = 1;  // p holds p[i]
-        if (STASH > 0) {
-            // states 1..min(STASH, j_end-1) come back from shared memory: no recurrence, no table loads
-            const int i_st = (j_end - 1 < STASH) ? j_end - 1 : STASH;
-            // four states at a time while all four are inside the window and below N: the four
-            // normalisations are independent, only the accumulations are serial
-            {
-                const int i4 = i_st < N ? i_st : N;
-                while (i + 3 <= i4) {
-                    const double q0 = stash[(i - 1) * 32], q1 = stash[i * 32], q2 = stash[(i + 1) * 32], q3 = stash[(i + 2) * 32];
-                    if (!(WVA_FASTWIN(q0, lo2, span2) && WVA_FASTWIN(q1, lo2, span2) &&
-                          WVA_FASTWIN(q2, lo2, span2) && WVA_FASTWIN(q3, lo2, span2)))
-                        break;
-                    const double n0 = div_recip(q0, z), n1 = div_recip(q1, z), n2 = div_recip(q2, z), n3 = div_recip(q3, z);
-                    acc = __dadd_rn(acc, __dmul_rn(di, n0));
-                    di = __dadd_rn(di, 1.0);
-                    sum_p = __dadd_rn(sum_p, n0);
-                    acc = __dadd_rn(acc, __dmul_rn(di, n1));
-                    di = __dadd_rn(di, 1.0);
-                    sum_p = __dadd_rn(sum_p, n1);
-                    acc = __dadd_rn(acc, __dmul_rn(di, n2));
-                    di = __dadd_rn(di, 1.0);
-                    sum_p = __dadd_rn(sum_p, n2);
-                    acc = __dadd_rn(acc, __dmul_rn(di, n3));
-                    di = __dadd_rn(di, 1.0);
-                    sum_p = __dadd_rn(sum_p, n3);
-                    pn = n3;
-                    p = q3;
-                    acc_at_N = acc;
-                    i += 4;
-                }
-            }
-#pragma unroll 2
-            for (; i <= i_st; ++i) {
-                p = stash[(i - 1) * 32];
-                if (!WVA_FASTWIN(p, lo2, span2)) break;
-                pn = div_recip(p, z);
-                acc = __dadd_rn(acc, __dmul_rn(di, pn));
-                di = __dadd_rn(di, 1.0);
-                if (i <= N) {
-                    sum_p = __dadd_rn(sum_p, pn);
-                    acc_at_N = acc;
-                }
-            }
-            // i = first state not yet accumulated; p must hold p[i] for the generic loop below
-            if (i <= i_st) {
-                // left early: p = p[i] is outside the fast window (tiny or zero): generic loop handles it
-            } else if (i < j_end) {
-                // continue the recurrence from the last stashed state: p[i] = step(p[i-1])
-                WVA_LOAD_TAIL(A)
-                if (i - 1 < nh) load_recip(tab, i - 1, A);
-                const double pprev = stash[(i - 2) * 32];
-                p = WVA_FASTWIN(pprev, lo2, span2) ? div_rate(__dmul_rn(pprev, lam), A)
-                                                                 : __ddiv_rn(__dmul_rn(pprev, lam), A.b);
-            }
-        }
-        if (STAGED && staged && __all_sync(0xffffffffu, i == __shfl_sync(0xffffffffu, i, 0))) {
+        if (STAGED && staged) {
             // staged head of pass 2 (see pass 1): states i < nh take their step's entry from the window
             const double4* tab4 = reinterpret_cast<const double4*>(tab);
             double4* tb = reinterpret_cast<double4*>(tbuf);
@@ -747,15 +760,7 @@ __device__ __noinline__ int solve_shared_t(const double* __restrict__ tab, int N
     // acc_at_N tracked acc while i <= N: it holds acc at state min(N, last state)
     const double in_serv = __dadd_rn(acc_at_N, __dmul_rn(__dsub_rn(1.0, sum_p), (double)N));
     const double pnK = (j_end == K + 1) ? pn : 0.0;
-
-    st.avg_num_in_servers = (float)in_serv;
-    const float avg_num_in_system = (float)acc;
-    st.throughput = __fmul_rn(lambda, __fsub_rn(1.0f, (float)pnK));
-    st.avg_resp_time = __fdiv_rn(avg_num_in_system, st.throughput);
-    st.avg_serv_time = __fdiv_rn(st.avg_num_in_servers, st.throughput);
-    float w = __fsub_rn(st.avg_resp_time, st.avg_serv_time);
-    if (w < 0.0f) w = 0.0f;
-    st.avg_wait_time = w;
+    stats_epilogue(acc, in_serv, pnK, lambda, st);
 #undef WVA_LOAD_TAIL
     return bail ? kSolveBail : kSolveOk;
 }
@@ -886,11 +891,11 @@ __device__ __forceinline__ void stats_from_row(double acc, double sum_p, int N, 
 }
 
 __device__ __forceinline__ int solve_shared(const double* __restrict__ tab, int N, int K, float lambda, ModelStats& st) {
-    return solve_shared_t<0>(tab, N, K, lambda, st, nullptr);
+    return solve_shared_t<>(tab, N, K, lambda, st);
 }
 // Per-lane private tables (size path): every lane streams its own table, so prefetch much further ahead.
 __device__ __forceinline__ int solve_private(const double* __restrict__ tab, int N, int K, float lambda, ModelStats& st) {
-    return solve_shared_t<0, 48>(tab, N, K, lambda, st, nullptr);
+    return solve_shared_t<48>(tab, N, K, lambda, st);
 }
 
 // Stored-vector fallback: a literal restatement of computeProbabilities /

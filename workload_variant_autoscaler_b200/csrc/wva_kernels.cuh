@@ -394,7 +394,6 @@ struct CellCols {
 };
 constexpr int kSortChunk = 8192;   // cells per CTA in the local counting sort
 constexpr int kSortThreads = 512;
-constexpr int kGridStash = 24;     // chain states kept in shared memory between the two passes (per lane)
 constexpr int kClasses = 256;      // 8-bit length classes; class 255 = not analysable
 struct GridArgs {
     DevFleet f;
@@ -1331,12 +1330,11 @@ __global__ void __launch_bounds__(256) grid_items_scatter(GridArgs g) {
 // ---------------------------------------------------------------------------
 constexpr int kQLongN = 2 * kClasses + 1, kQLongCtr = kQLongN + 1, kQShortCtr = kQLongN + 2;  // in item_count[]
 
-// Per-warp shared memory of grid_kernel (doubles): the pass-1 stash, the staged table window (+ the lanes' tail
-// entries) and the pair record of the current item.
-constexpr int kGkStashD = kGridStash * 32;              // [state][lane]
+// Per-warp shared memory of grid_kernel (doubles): the staged table window (+ the lanes' tail entries) and the pair
+// record of the current item.
 constexpr int kGkTbufD = kStagedTbufD;                  // staged table window + the lanes' tail entries
 constexpr int kGkPairD = 8;                             // 48-byte pair record (padded to 64)
-constexpr int kGkWarpD = kGkStashD + kGkTbufD + kGkPairD;
+constexpr int kGkWarpD = kGkTbufD + kGkPairD;
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
@@ -1352,9 +1350,8 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 // across the solver call and none is fetched by a dependent load afterwards.
 __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const uint4 rec, unsigned lane, double* warp_smem) {
     const DevFleet& f = g.f;
-    double* stash_warp = warp_smem;
-    double* tbuf_warp = warp_smem + kGkStashD;
-    float4* pair_buf = reinterpret_cast<float4*>(warp_smem + kGkStashD + kGkTbufD);
+    double* tbuf_warp = warp_smem;
+    float4* pair_buf = reinterpret_cast<float4*>(warp_smem + kGkTbufD);
     const unsigned idx = w * 32 + lane;
     const long long t_start = g.dbg_cycles ? clock64() : 0;
     unsigned long long t_start_ns = 0;
@@ -1381,7 +1378,7 @@ __device__ __forceinline__ void item_run(const GridArgs& g, unsigned w, const ui
     if (lane < 3) cp_async16(pair_buf + lane, g.pair_rec + 3 * (size_t)pair + lane);
     cp_async_commit();
     ModelStats st;
-    const int rc = solve_shared_t<kGridStash, 10, true>(tab, N, K, lambda, st, stash_warp + lane, tbuf_warp);
+    const int rc = solve_shared_t<10, true>(tab, N, K, lambda, st, tbuf_warp);
     cp_async_wait<0>();
     __syncwarp();
     if (valid) {
